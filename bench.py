@@ -1,18 +1,19 @@
 #!/usr/bin/env python
 """Benchmark of the hot path: images/sec @1024x512 (det+seg forward + NMS + seg argmax == reference detect.py:144-148,191-193).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--cfg s_psp|m_lab] [--batch B]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--cfg s_psp|m_lab] [--batch B] [--dump-outputs DIR]
 
 N=1 workload = BASELINE.json configs[1]: yolov5s_city_seg.yaml (PSP head), batch 16 x 3 x 512 x 1024 synthetic, fp16 storage /
 fp32 accumulate.  N>1 (torchrun): one replica per GPU, no collective on the data path (inference shards by image) -> "weak".
 Prints ONE JSON line on rank 0.  See DESIGN.md (Measurement) for the roofline arithmetic.
+--dump-outputs DIR writes what the last timed step returned (detections, their count, the class map) as float32 .npy files, so that
+two builds can be compared output for output: inputs and weights are seeded, identical from run to run for the same arguments.
 """
 import argparse
 import json
 import os
 import subprocess
 import sys
-import threading
 import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
@@ -25,6 +26,8 @@ CFGS = {"s_psp": ("yolov5s_city_seg.yaml", 29.70e9), "m_lab": ("yolov5m_city_seg
         "m_psp": ("yolov5m_city_seg.yaml", None), "s_bise": ("yolov5s_city_seg_bise.yaml", 32.91e9),
         "s_base": ("yolov5s_city_seg_base.yaml", 30.87e9)}
 H, W = 512, 1024
+# NVIDIA H100 SXM data sheet (700 W card): dense FP16 tensor rate and HBM3 bandwidth, the ceilings of the roofline figures
+H100_FP16_TFLOPS, H100_HBM_GBS = 989.0, 3350.0
 # synthetic Detect objectness-bias shifts (per level) calibrated so that ~1% of the 32256 anchors pass obj>0.25
 # (a realistic O(300) candidates/img NMS load instead of the ~10k the near-critical synthetic weights would give)
 OBJ_BIAS_SHIFT = {"s_psp": (-17.5, -10.5, -18.2), "m_lab": (-5.9, -4.6, -5.2)}
@@ -42,38 +45,29 @@ def make_weights(tag):
     return yml, cfg, sd
 
 
-class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md 'clocks line')."""
+def gpu_state(gpu_index):
+    """name, power limit and clocks of the card, read once next to the measurement (a number is only worth something with them)"""
+    q = "name,power.limit,clocks.sm,clocks.max.sm"
+    try:
+        out = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits", "-i", str(gpu_index)],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        name, power_w, sm, sm_max = [v.strip() for v in out.split(",")]
+        return {"name": name, "power_limit_w": float(power_w), "sm_mhz": float(sm), "sm_max_mhz": float(sm_max)}
+    except Exception as e:
+        return {"name": torch.cuda.get_device_name(gpu_index), "unavailable": f"{type(e).__name__}: {e}"[:200]}
 
-    def __init__(self, gpu_index):
-        super().__init__(daemon=True)
-        self.gpu, self.stop_flag, self.samples = gpu_index, False, []
 
-    def run(self):
-        q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-             "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
-        try:
-            p = subprocess.Popen(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits", "-i", str(self.gpu), "-lms", "20"],
-                                 stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
-        except Exception:
-            return
-        while not self.stop_flag:
-            line = p.stdout.readline()
-            if not line:
-                break
-            self.samples.append([s.strip() for s in line.split(",")])
-        p.terminate()
-
-    def summary(self):
-        sm = [float(s[0]) for s in self.samples if s and s[0].replace(".", "").isdigit()]
-        mx = [float(s[1]) for s in self.samples if len(s) > 1 and s[1].replace(".", "").isdigit()]
-        reasons = set()
-        for s in self.samples:
-            for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), s[3:7]):
-                if v.lower().startswith("active"):
-                    reasons.add(name)
-        return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": sorted(reasons),
-                "samples": len(sm)}
+def dump_outputs(out_dir, det, cnt, cls):
+    """the arrays the caller of the timed step receives, as float32 .npy (class map 16 x 512 x 1024: 32 MB; padded detection rows past
+    each image's count are zeroed so that stale buffer contents never enter a comparison)"""
+    os.makedirs(out_dir, exist_ok=True)
+    det = det.float().cpu().clone()
+    cnt = cnt.cpu()
+    for b in range(det.shape[0]):
+        det[b, int(cnt[b]):] = 0
+    np.save(os.path.join(out_dir, "detections.npy"), det.numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "detection_counts.npy"), cnt.numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "seg_classes.npy"), cls.cpu().numpy().astype(np.float32))
 
 
 def cpu_reference_line(args, tag, steps, warmup, as_main):
@@ -153,7 +147,7 @@ def reference_gpu_infer(tag, B, steps, warmup):
         return {"unavailable": f"{type(e).__name__}: {e}"[:300]}
 
 
-def infer_record(tag, B, steps, warmup, world, min_seconds=1.0):
+def infer_record(tag, B, steps, warmup, world):
     """sub-record for another inference config (BASELINE.json configs[2]: yolov5m + Lab head, batch 8): same step as the headline"""
     import torch.distributed as dist
     from multiyolov5_b200.models.yolo import Model
@@ -189,11 +183,8 @@ def infer_record(tag, B, steps, warmup, world, min_seconds=1.0):
     for i in range(max(3, warmup)):
         step(i)
     ms = run(steps)
-    n_long = max(steps, int(min_seconds * 1e3 / (ms / steps)) + 1)
-    ms_long = run(n_long)
     rec = {"workload": f"{yml} inference, batch {B}x3x{H}x{W} per GPU, half mode: Model.forward + NMS(0.25,0.45) + seg argmax", "n_gpus": world, "steps": steps,
            "ms_per_step": ms / steps, "images_per_s": B * world * steps / (ms * 1e-3),
-           "sustained": {"steps": n_long, "seconds": ms_long * 1e-3, "images_per_s": B * world * n_long / (ms_long * 1e-3)},
            "gflop_per_image": (CFGS[tag][1] or 0) / 1e9}
     del model, xs
     torch.cuda.empty_cache()
@@ -212,6 +203,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--fp32-logits", action="store_true", help="keep fp32 I/O (fp32 seg logits) instead of the reference's half() mode")
     ap.add_argument("--profile-ops", action="store_true", help="print the per-op device-time table to stderr")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs (detections, counts, class map) to DIR/<name>.npy as float32")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -223,7 +216,7 @@ def main():
             print(json.dumps(cpu_reference_line(args, args.cfg, max(3, min(args.steps, 30)), min(warmup, 3), True)), flush=True)
         return
     if args.impl == "reference-gpu":
-        # the reference's own GPU configuration (torch fp16 + cuDNN, cudnn.benchmark; detect.py:96-103,124) on ONE B200: a baseline arm
+        # the reference's own GPU configuration (torch fp16 + cuDNN, cudnn.benchmark; detect.py:96-103,124) on one GPU: a baseline arm
         if rank == 0:
             torch.cuda.set_device(local)
             B = args.batch or (16 if args.cfg.startswith("s_") else 8)
@@ -323,10 +316,8 @@ def main():
             ev_out[k].record(s_out)
         return det, cnt, cls
 
-    def timed(fn, steps, sampler=None, finalize=None):
-        if sampler:
-            sampler.start()     # samples cover warm-up + timed region (identical load)
-        for i in range(warmup + (40 if sampler else 0)):
+    def timed(fn, steps, finalize=None, last=None):
+        for i in range(warmup):
             fn(i)
         torch.cuda.synchronize()
         if world > 1:
@@ -336,13 +327,13 @@ def main():
         launches0 = None
         e0.record()
         for i in range(steps):
-            fn(i)
+            out = fn(i)
+        if last is not None:
+            last.append(out)
         if finalize:
             finalize()       # e.g. make the timed stream wait for the last device->host copies
         e1.record()
         torch.cuda.synchronize()
-        if sampler:
-            sampler.stop_flag = True
         if world > 1:
             dist.barrier()
         ms = e0.elapsed_time(e1)
@@ -351,19 +342,14 @@ def main():
             dist.all_reduce(t, op=dist.ReduceOp.MAX)
         return float(t.item())
 
-    sampler = ClockSampler(local) if rank == 0 else None
-    ms_total = timed(step_resident, args.steps, sampler)
-    # the same step for >= 1 s (the driver's `steps` make a ~50 ms region: a burst figure; this one runs at sustained clocks / power)
-    n_long = max(args.steps, int(1000.0 / (ms_total / args.steps)) + 1)
-    sampler_long = ClockSampler(local) if rank == 0 else None
-    if sampler_long:
-        sampler_long.start()
-    ms_long = timed(step_resident, n_long)
-    if sampler_long:
-        sampler_long.stop_flag = True
-    det, cnt, cls = step_resident(0)
-    torch.cuda.synchronize()
+    last = []
+    ms_total = timed(step_resident, args.steps, last=last)
+    gpu = gpu_state(local) if rank == 0 else None
+    det, cnt, cls = last[0]
     n_cand = float(cnt.float().mean().item())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, det, cnt, cls)
+    del last, det, cnt, cls
     launches_per_step = eng.launches() + 2 + 1          # forward ops + (nms filter, nms) + seg argmax
     def e2e_tail():
         for k in range(2):
@@ -413,7 +399,7 @@ def main():
         non_max_suppression(out[0][0], 0.25, 0.45, return_padded=True)
     ms_fused = timed(step_fused, args.steps)
 
-    # per-op device time (CUDA events around every op on the launching stream) -> roofline of the tcgen05 conv kernel
+    # per-op device time (CUDA events around every op on the launching stream) -> roofline of the wgmma conv kernel
     roof = None
     if rank == 0:
         reps = 5
@@ -438,7 +424,7 @@ def main():
                 s = pb.slots[o.slot].conv
                 f = conv_algorithmic_flops(s, B, o.out)      # the reference layer's 2 x MACs (restated layer-0 conv included)
                 _lib.check(_lib.lib().myolo_plan_conv_info(eng.last_plan.handle, i, info))
-                if info[0]:      # tcgen05 kernel
+                if info[0]:      # tensor-core (wgmma) kernel
                     conv_ms += per_op[i]; n_conv += 1; flops += f
                     # algorithmic bytes of the launch: input + output (+ residual) activations once, weights once, fp16 (fp32 head outputs: 4 B)
                     nbytes = (B * o.in_.h * o.in_.w * o.in_.c * 2 + B * o.out.h * o.out.w * s.out_channels * (2 if o.out.buf.dtype == _lib.F16 else 4)
@@ -449,34 +435,22 @@ def main():
                     simt_ms += per_op[i]; n_simt += 1; simt_flops += f
                 conv_table.append((i, o.tag, f"{s.in_channels}->{s.out_channels} k{s.kernel_size[0]}s{s.stride[0]}d{s.dilation[0]} @{o.out.h}x{o.out.w}",
                                    list(info), per_op[i] * 1e3, f))
-        peaks = {}
-        try:
-            peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        except Exception:
-            pass
-        peak = peaks.get("bf16_tflops_sustained", 1400.0)
+        peak = H100_FP16_TFLOPS
         ach = flops / (conv_ms * 1e-3) / 1e12
-        traffic = None
-        try:   # dram__bytes_read+write per conv_tc launch from the committed `ncu --set full` capture of the same step (profiles/)
-            tj = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-            if tj.get("cfg") == tag and tj.get("batch") == B:
-                traffic = tj["dram_bytes_per_launch"]
-        except Exception:
-            pass
-        roof = {"bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": traffic,
-                "kernel": "conv_tc_kernel (the tcgen05 Conv+BN+SiLU launches of one forward; CUDA-core conv launches are listed separately)",
+        roof = {"bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak,
+                "kernel": "conv_tc_kernel (the wgmma Conv+BN+SiLU launches of one forward; CUDA-core conv launches are listed separately)",
                 "launches": n_conv, "avg_launch_ms": conv_ms / n_conv, "simt_conv_launches": n_simt, "simt_conv_ms": simt_ms,
                 "simt_conv_flops_per_step": simt_flops,
-                "algorithmic_flops_per_step": flops, "peak_source": "MEASURED_PEAKS.json bf16_tflops_sustained" if peaks else "fallback 1.4 PF sustained",
+                "algorithmic_flops_per_step": flops, "peak_source": "H100 SXM data sheet, dense FP16 (700 W card; see `gpu` for this card's power limit)",
                 "conv_share_of_forward": conv_ms / float(per_op.sum())}
         # the same launches against their OWN roofline min(tensor, AI x HBM): most layers of this network are activation-bandwidth bound
         # (1x1 convs, 16-64 channel layers), so the aggregate tensor fraction above cannot approach 1 whatever the kernel does
-        hbm_peak = peaks.get("hbm_gbs", 6500.0) * 1e9
+        hbm_peak = H100_HBM_GBS * 1e9
         t_bound = [max(f / (peak * 1e12), nb / hbm_peak) * 1e3 for f, nb, _ in layer_rows]
         roof["per_layer"] = {"bound_ms": float(sum(t_bound)), "measured_ms": float(conv_ms), "frac": float(sum(t_bound) / conv_ms),
                              "hbm_bound_launches": int(sum(1 for (f, nb, _) in layer_rows if nb / hbm_peak > f / (peak * 1e12))),
                              "tensor_bound_launches": int(sum(1 for (f, nb, _) in layer_rows if nb / hbm_peak <= f / (peak * 1e12))),
-                             "note": "sum over the tcgen05 conv launches of max(FLOP / tensor peak, algorithmic bytes / HBM peak) / measured device time"}
+                             "note": "sum over the wgmma conv launches of max(FLOP / tensor peak, algorithmic bytes / HBM peak) / measured device time"}
         if args.profile_ops:
             for i, o in enumerate(pb.ops):
                 print(f"{i:3d} kind={o.kind:2d} {o.tag:24s} {per_op[i] * 1e3:9.1f} us", file=sys.stderr)
@@ -491,7 +465,7 @@ def main():
                 "vs_baseline": None, "dtype": "f16 storage / f32 accumulate", "data": "synthetic",
                 "config": {"workload": f"{yml} inference, batch {B}x3x{H}x{W} per GPU: Model.forward (z, raw, {'fp32' if args.fp32_logits else 'fp16'} seg logits) + NMS(0.25,0.45) + "
                                        "seg upsample/argmax", "global_batch": B * world, "parallelism": f"replicas x{world} (no collective)",
-                           "l2": f"inputs rotate over {NROT} batches ({NROT * B * 3 * H * W * 4 / 1e6:.0f} MB > 126 MB L2); activations are rewritten every step",
+                           "l2": f"inputs rotate over {NROT} batches ({NROT * B * 3 * H * W * 4 / 1e6:.0f} MB > 50 MB L2); activations are rewritten every step",
                            "nms_candidates_kept_per_img": n_cand},
                 "e2e": {"value": imgs / (ms_e2e * 1e-3), "unit": "images/s", "h2d_bytes_per_step": B * 3 * H * W,
                         "d2h_bytes_per_step": B * H * W * 1 + B * 300 * 6 * 4 + B * 4,
@@ -500,10 +474,7 @@ def main():
                 "e2e_from_raw_frames": {"value": imgs / (ms_raw * 1e-3), "unit": "images/s", "h2d_bytes_per_step": B * 4 * H * W * 3,
                                         "note": "2048x1024 BGR uint8 frames -> device letterbox/pre-process kernel (bit exact with cv2) -> forward -> post-process"},
                 "model_only_images_per_s": imgs / (ms_model * 1e-3), "fused_argmax_images_per_s": imgs / (ms_fused * 1e-3),
-                "clocks": sampler.summary() if sampler else None, "roofline": roof,
-                "sustained": {"steps": n_long, "seconds": ms_long * 1e-3, "ms_per_step": ms_long / n_long,
-                              "value": B * world * n_long / (ms_long * 1e-3), "clocks": sampler_long.summary() if sampler_long else None,
-                              "note": "same resident step as `value`, timed for >= 1 s"}}
+                "gpu": gpu, "roofline": roof}
         line["e2e"]["d2h_note"] = "class map returned as uint8 (19 classes); the reference's .cpu() moves the same map as int64, 8x the bytes"
     # ---- sub-records for the other BASELINE.json configs (every rank takes part: the train step contains the path's one collective)
     extras = {}
@@ -512,7 +483,7 @@ def main():
         model = eng = None
         torch.cuda.empty_cache()
         from tools.bench_train import train_record
-        extras["train"] = train_record(world, rank, steps=max(6, args.steps // 2), warmup=warmup, B=4, with_reference_gpu=(world == 1))
+        extras["train"] = train_record(world, rank, steps=args.steps, warmup=warmup, B=4, min_seconds=0.0, with_reference_gpu=(world == 1))
         extras["m_lab"] = infer_record("m_lab", 8, args.steps, warmup, world)
         if rank == 0 and world == 1:
             extras["reference_gpu"] = reference_gpu_infer(tag, B, 10, warmup)

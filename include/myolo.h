@@ -1,5 +1,5 @@
 /*
- * libmyolo_sm100a — C ABI of the B200-native joint detection+segmentation hot path.
+ * libmyolo_sm90a — C ABI of the H100-native (sm_90a) joint detection+segmentation hot path.
  *
  * The reference (TomMao23/multiyolov5) is pure Python: the interfaces this library sits behind are
  *   - models.yolo.Model.forward / forward_once          (reference models/yolo.py:273-316)
@@ -14,7 +14,7 @@
  *   - all data pointers are DEVICE pointers unless the name says `host_`; the library never frees caller memory.
  *   - `stream` is a cudaStream_t passed as void* (torch.cuda.current_stream().cuda_stream); the library never
  *     synchronises the device on its own.
- *   - there is NO CPU fallback: every function needs an sm_100 device and fails loudly otherwise.
+ *   - there is NO CPU fallback: every function needs an sm_90 (H100) device and fails loudly otherwise.
  */
 #ifndef MYOLO_H_
 #define MYOLO_H_
@@ -32,7 +32,7 @@ extern "C" {
 #define MYOLO_OK 0
 #define MYOLO_E_INVALID (-1)  /* bad argument / unsupported shape           */
 #define MYOLO_E_CUDA (-2)     /* CUDA runtime / driver error                */
-#define MYOLO_E_NODEVICE (-3) /* no sm_100 device                           */
+#define MYOLO_E_NODEVICE (-3) /* no sm_90 device                            */
 #define MYOLO_E_STATE (-4)    /* call order (e.g. forward before weights)   */
 
 /* dtypes */
@@ -128,8 +128,8 @@ int myolo_plan_forward(myolo_plan* plan, const void* x, int x_dtype, float* z, f
 int myolo_plan_read_view(myolo_plan* plan, myolo_view view, float* dst_nchw, void* stream);
 /* number of kernels the last myolo_plan_forward launched (bench.py's gpu_launches) */
 int64_t myolo_plan_last_launch_count(const myolo_plan* plan);
-/* which kernel conv op `op_index` takes and its tiling: info[12] = {1 tcgen05 / 0 CUDA-core, grid, smem bytes, BN, stages, mode (0 taps /
- * 1 strip / 2 vertical rounds), weights-stationary, G, tiles, N tiles, kc, CTAs per SM}.  Feeds bench.py's roofline record and profiles/. */
+/* which kernel conv op `op_index` takes and its tiling: info[12] = {1 wgmma / 0 CUDA-core, grid, smem bytes, BN, stages, mode (always 0:
+ * one TMA box per tap), weights-stationary (0), tiles per round (1), tiles, N tiles, kc, CTAs per SM (1)}.  Feeds bench.py's roofline record. */
 int myolo_plan_conv_info(myolo_plan* plan, int op_index, int32_t* info);
 /* per-op device time of the next forward (CUDA events around every op; host array of n_ops floats, ms) */
 int myolo_plan_profile(myolo_plan* plan, const void* x, int x_dtype, float* z, float* const* raw, void* seg, int seg_dtype,
@@ -173,7 +173,7 @@ int myolo_plan_read_grad_view(myolo_plan* plan, myolo_view view, float* dst_nchw
  * nullable = 1); when *found_inf != 0 the update is skipped (amp.GradScaler.step, train.py:396); zero_grad clears the gradients in the
  * same pass (optimizer.zero_grad, train.py:398).  lr / weight_decay are HOST arrays of n_groups (<= 4) floats. */
 /* standalone weight gradient of one conv (per-op parity tests / ncu): x (B,H,W,ci) and dy (B,Ho,Wo,co) NHWC fp16, "same" padding
- * dil*(k/2); dW fp32 [co][ci][k][k] is ACCUMULATED into.  path 0: mma.sync kernel, 1: tcgen05 kernel (needs ci % 64 == 0, Wo % 16 == 0) */
+ * dil*(k/2); dW fp32 [co][ci][k][k] is ACCUMULATED into.  path 0: mma.sync kernel, 1: wgmma kernel (needs ci % 64 == 0, Wo % 16 == 0) */
 int myolo_conv_wgrad(const void* x, const void* dy, int B, int H, int W, int ci, int co, int k, int stride, int dil, float* dW, int path,
                      void* stream);
 int myolo_grads_check_finite(const float* grad, int64_t n, int32_t* found_inf /* device */, void* stream);
@@ -234,7 +234,7 @@ int myolo_seg_upsample_argmax(const void* logits, int dtype, int B, int C, int h
 int myolo_bilinear_nchw(const float* src, int B, int C, int h, int w, int H, int W, float* dst, void* stream);
 
 /* ---- standalone kernels for per-op parity tests and ncu captures ---- */
-/* SiLU(conv(x)*bnscale+bnshift) on NHWC fp16: x (B,H,W,Ci) -> y (B,Ho,Wo,Co); w fp32 [Co][Ci][k][k]; path: 0 auto, 1 tcgen05, 2 simt, 3 tcgen05 with pair mode (two M tiles per weight fetch) wherever legal */
+/* SiLU(conv(x)*bnscale+bnshift) on NHWC fp16: x (B,H,W,Ci) -> y (B,Ho,Wo,Co); w fp32 [Co][Ci][k][k]; path: 0 auto, 1 wgmma, 2 simt, 3 wgmma (same kernel as 1) */
 int myolo_conv_bn_silu(const void* x_nhwc_f16, int B, int H, int W, int ci, const float* w, int co, int k, int stride,
                        int dil, const float* gamma, const float* beta, const float* mean, const float* var, float eps,
                        const float* bias, int act, const void* residual_nhwc_f16, void* y_nhwc_f16, int path, void* stream);

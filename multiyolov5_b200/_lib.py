@@ -1,13 +1,13 @@
-"""ctypes binding of libmyolo_sm100a.so (C ABI: include/myolo.h).
+"""ctypes binding of libmyolo_sm90a.so (C ABI: include/myolo.h).
 
-There is no CPU / PyTorch fallback: if the shared library is missing or no sm_100 device is present every entry
+There is no CPU / PyTorch fallback: if the shared library is missing or no sm_90 (H100) device is present every entry
 point raises.  Build with `python -c "import __graft_entry__ as g; g.build()"` or `make -C multiyolov5_b200/csrc`.
 """
 import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("MYOLO_LIB") or os.path.join(_HERE, "libmyolo_sm100a.so")   # MYOLO_LIB: developer builds (e.g. the clock64 timeline variant)
+LIB_PATH = os.environ.get("MYOLO_LIB") or os.path.join(_HERE, "libmyolo_sm90a.so")   # MYOLO_LIB: developer builds (e.g. the clock64 timeline variant)
 
 F16, F32, U8, I64 = 0, 1, 2, 3
 ACT_NONE, ACT_SILU, ACT_SIGMOID = 0, 1, 2
@@ -102,14 +102,14 @@ def lib():
     for name in EXPORTS:
         getattr(L, name)  # AttributeError here == header / library mismatch
     if L.myolo_abi_version() != 1:
-        raise MyoloError("libmyolo_sm100a ABI version mismatch")
+        raise MyoloError("libmyolo_sm90a ABI version mismatch")
     _lib = L
     return L
 
 
 def check(rc: int):
     if rc != 0:
-        raise MyoloError(f"libmyolo_sm100a error {rc}: {lib().myolo_last_error().decode(errors='replace')}")
+        raise MyoloError(f"libmyolo_sm90a error {rc}: {lib().myolo_last_error().decode(errors='replace')}")
 
 
 def stream_ptr():

@@ -35,7 +35,7 @@ int launch_lut_blend(const void* idx, int idx_dtype, long n, const unsigned char
   MYOLO_REQUIRE(idx && lut && n > 0 && n_entries > 0 && ch > 0 && n_entries * ch <= 4096 && (out || blend) && (!blend || im),
                 "lut_blend: bad arguments");
   MYOLO_REQUIRE(idx_dtype == MYOLO_U8 || idx_dtype == MYOLO_I64, "lut_blend: class map must be uint8 or int64");
-  lut_blend_kernel<<<(int)std::min<long>(148L * 8, (n + 255) / 256), 256, n_entries * ch, s>>>(idx, idx_dtype, n, lut, n_entries, ch, reverse, out,
+  lut_blend_kernel<<<(int)std::min<long>(132L * 8, (n + 255) / 256), 256, n_entries * ch, s>>>(idx, idx_dtype, n, lut, n_entries, ch, reverse, out,
                                                                                               im, alpha, beta, blend);
   MYOLO_LAUNCH_CHECK();
   return 0;
@@ -70,7 +70,7 @@ int launch_seg_hist(const void* pred, int pred_dtype, const long long* target, l
   MYOLO_REQUIRE(pred && target && counters && n > 0 && n_cls > 0 && n_cls <= 1024, "seg_hist: bad arguments");
   MYOLO_REQUIRE(pred_dtype == MYOLO_U8 || pred_dtype == MYOLO_I64, "seg_hist: prediction must be uint8 or int64");
   // one block sees at most 2^32 - 1 pixels per counter: blocks of <= 2^24 pixels each
-  const int blocks = (int)std::max<long>(std::min<long>(148L * 8, (n + 255) / 256), (n + (1L << 24) - 1) >> 24);
+  const int blocks = (int)std::max<long>(std::min<long>(132L * 8, (n + 255) / 256), (n + (1L << 24) - 1) >> 24);
   seg_hist_kernel<<<blocks, 256, (2 + 3 * n_cls) * sizeof(unsigned int), s>>>(pred, pred_dtype, target, n, n_cls, counters);
   MYOLO_LAUNCH_CHECK();
   return 0;

@@ -20,12 +20,11 @@ static inline FastDiv make_fastdiv(unsigned d) {     // exact for 0 <= n < 2^31,
 
 struct ConvTcParams {
   int B, Ho, Wo;
-  int tw, th;            // output tile = tw x th pixels, tw*th == 128 (UMMA M)
+  int tw, th;            // output tile = tw x th pixels, tw*th == 128 (two wgmma M = 64 halves)
+  int log2_tw;
   int tiles_x, tiles_y;  // per image
   int n_tiles_n, total_tiles;
-  int G;                 // M tiles per accumulator round (G*BN <= 128 TMEM columns); G > 1 only when n_tiles_n == 1
-  int total_rounds;
-  int BN;                // UMMA N (multiple of 16, <= 128)
+  int BN;                // wgmma N (multiple of 16, <= 128)
   int Co;                // real output channels
   int kc;                // channels per K chunk: 16 / 32 / 64  (swizzle 32B / 64B / 128B)
   int cblocks;           // Ci_pad / kc
@@ -35,33 +34,14 @@ struct ConvTcParams {
   int act;
   int num_stages;
   int a_stage_bytes, b_stage_bytes;
-  int out_mode;          // 0: fp16 NHWC slice via per-warp TMA stores, 1: fp32 NHWC direct stores
-  int log2_tw;
-  int ws_mode;           // weights-stationary: the whole [BN x K] weight tile stays resident in shared memory
-  int b_res_bytes;       // bytes of the resident weight region (ws_mode)
-  // epilogue: 8 warps = 4 TMEM lane quarters x 2 "halves"; a half takes every other tile (G >= 2) or half of the columns (G == 1)
-  int ep_cols;           // columns handled by one warp per tile
-  int ep_split_cols;     // 1: halves split the columns, 0: halves split the tiles (or half 1 idles when the chunk count is odd)
-  int ow, log2_ow;       // per-warp TMA-store sub-box width in channels (16/32/64)
-  int n_sub;             // sub-boxes per warp per tile
-  int n_stg;             // staging buffers per warp (1 or 2)
-  int rows_w, rows_h;    // the 32 tile rows of a warp as an rows_w x rows_h pixel rectangle (store box)
-  // strip mode (3x3 stride 1, th == 1): one TMA strip of tw + 2*dil pixels per (ky, channel block) serves the three kx taps
-  int strip;             // 0 off; 1: shifted descriptors with base_offset 0; 2: base_offset = (addr >> 7) & 7
-  int vround;            // strip + weights-stationary + dil 1: the G tiles of a round are vertically adjacent rows sharing G+2 strips
-  int rounds_per_img;
-  int dil;
+  int out_mode;          // 0: fp16 NHWC slice, 1: fp32 NHWC
+  int out_c, out_ctot;   // channels of the output slice / channel pitch of its buffer
   const float* bias;
   const __half* residual;  // nullable; base of the residual slice (image 0, pixel 0, channel 0 of the slice)
   int res_ctot;
+  __half* out_f16;
   float* out_f32;
-  int out_f32_ctot;
-  long long* dbg;        // optional clock64 timeline buffer (MYOLO_CONV_TIMELINE=1), else null
-  // pair mode: a round is TWO M tiles (same N tile) that share every weight load - 256 x BN outputs per B fetch (L2->SM-bound layers)
-  int pair, m_tiles, n_pair_rounds, m_done;   // rounds [0, n_pair_rounds) are pairs, later rounds single tiles from M tile m_done on
-  int acc_stride, tmem_cols;                  // TMEM columns per accumulator stage / allocated (256 / 512 when a pair needs 2 x 128)
-  unsigned spin_ns;      // back-off of the roles that wait for the epilogue (0 = plain polling)
-  FastDiv fd_ntn, fd_tpi, fd_tx, fd_rpi;   // n_tiles_n, tiles_x * tiles_y, tiles_x, rounds_per_img
+  FastDiv fd_ntn, fd_tpi, fd_tx;   // n_tiles_n, tiles_x * tiles_y, tiles_x
 };
 
 struct ConvOp {
@@ -72,17 +52,16 @@ struct ConvOp {
   const float* bias = nullptr;
   int Ci_pad = 0, Co_pad = 0, Co = 0;
   bool use_tc = false;
-  // tcgen05 path state (built once at plan creation)
-  CUtensorMap tmA[4], tmB, tmO;
+  // tensor-core path state (built once at plan creation)
+  CUtensorMap tmA[4], tmB;
   ConvTcParams p;
   int grid = 0, smem = 0;
 };
 
-// decides whether the tcgen05 path can run this op; fills tile geometry (no device pointers needed)
+// decides whether the tensor-core (wgmma) path can run this op; fills tile geometry (no device pointers needed)
 bool conv_tc_eligible(const ConvOp& op);
 // builds tensor maps / params; requires op.in/out/res/w/bias device pointers to be final
 int conv_tc_prepare(ConvOp& op, int num_sms);
-extern int g_conv_tc_force_pair;   // tests: take pair mode wherever it is legal, not only where the cost rule picks it (myolo_conv_bn_silu path 3)
 int conv_tc_launch(const ConvOp& op, cudaStream_t stream);
 int conv_simt_launch(const ConvOp& op, cudaStream_t stream);
 int conv_simt_launch_group(const ConvOp* const* ops, int n, cudaStream_t stream);   // <= 4 small convs of one input type in one launch

@@ -1,4 +1,4 @@
-// Generic CUDA-core conv (+bias+act+residual) on NHWC views.  Used for shapes the tcgen05 kernel does not take
+// Generic CUDA-core conv (+bias+act+residual) on NHWC views.  Used for shapes the wgmma kernel does not take
 // (maps smaller than one 128-pixel tile: PPM 1x1..6x6 bins, FFM attention FCs, P5 at tiny test resolutions) and,
 // with MYOLO_FORCE_SIMT=1, as an independent on-device cross-check of the tensor-core path.
 // One warp computes one output pixel x 32 consecutive output channels; lanes split K (coalesced 16-byte loads of both
@@ -131,7 +131,7 @@ int conv_simt_launch_group(const ConvOp* const* ops, int n, cudaStream_t stream)
     if (rc) return rc;
     most = std::max(most, ((long)g.p[i].B * g.p[i].Ho * g.p[i].Wo * ((g.p[i].Co + 7) / 8) + 7) / 8);
   }
-  if (most > 148 * 16) most = 148 * 16;
+  if (most > 132 * 16) most = 132 * 16;
   if (ops[0]->in.dtype == MYOLO_F16) MYOLO_CHECK_CUDA(launch_pdl(conv_simt_group_kernel<__half>, dim3((int)most, n), dim3(256), 0, stream, g));
   else MYOLO_CHECK_CUDA(launch_pdl(conv_simt_group_kernel<float>, dim3((int)most, n), dim3(256), 0, stream, g));
   MYOLO_LAUNCH_CHECK();
@@ -150,7 +150,7 @@ int conv_simt_launch(const ConvOp& op, cudaStream_t stream) {
   MYOLO_REQUIRE(op.in.C >= op.Ci_pad, "conv_simt: input view has %d channels, packed weights expect %d", op.in.C, op.Ci_pad);
   const long warps = (long)p.B * p.Ho * p.Wo * ((p.Co + 7) / 8);
   long blocks = (warps + 7) / 8;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   if (blocks < 1) blocks = 1;
   if (op.in.dtype == MYOLO_F16) MYOLO_CHECK_CUDA(launch_pdl(conv_simt_kernel<__half>, dim3((int)blocks), dim3(256), 0, stream, p));
   else MYOLO_CHECK_CUDA(launch_pdl(conv_simt_kernel<float>, dim3((int)blocks), dim3(256), 0, stream, p));

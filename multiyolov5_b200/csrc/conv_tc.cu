@@ -1,79 +1,48 @@
-// Fused Conv(+folded BN)+bias+SiLU(+residual) as an implicit GEMM on the 5th-gen tensor cores (tcgen05), sm_100a only.
+// Fused Conv(+folded BN)+bias+SiLU(+residual) as an implicit GEMM on the Hopper tensor cores (wgmma), sm_90a.
 //
-//   D[128 pixels x BN channels] (fp32, TMEM)  +=  A[128 x kc] (NHWC activations, fp16)  *  B[BN x kc]^T (packed weights, fp16)
+//   D[128 pixels x BN channels] (fp32, registers)  +=  A[128 x kc] (NHWC activations, fp16)  *  B[BN x kc]^T (packed weights, fp16)
 //
 // * M tile  = a tw x th rectangle of output pixels of ONE image (tw*th = 128).  For every filter tap the A operand is the
 //   same rectangle shifted by (dx,dy): one 4-D TMA box load {kc channels, tw, th, 1} with hardware zero fill at the
 //   image border (that is the conv padding).  Stride-2 convs use four "parity" tensor maps (even/odd rows x cols)
 //   so that the stride-2 gather is again a dense box.  No im2col buffer ever exists in HBM.
-// * strip mode (3x3, stride 1, full-row tiles): ONE strip of tw+2*dil pixels per (filter row, channel block) feeds the
-//   three kx taps through row-shifted UMMA descriptors -> 3x less L2->SM traffic than nine tap boxes.
 // * K loop  = taps x (Ci/kc) chunks, 64 K-elements per pipeline stage; operands are K-major with the 32/64/128-byte
-//   TMA swizzle named in the UMMA shared-memory descriptor.  Small weight tiles stay resident in smem (weights-stationary).
-// * warp roles (320 threads): warp0 = TMA producer (1 thread), warp1 = MMA issuer (1 thread; the warp owns TMEM
-//   alloc/dealloc), warps 2..9 = epilogue.  An accumulator "round" holds G M-tiles (G*BN <= 128 TMEM columns, two rounds
-//   double-buffered).  Every epilogue warp is autonomous: it owns 32 TMEM lanes (= 32 pixels), converts its share of the
-//   round (TMEM -> regs -> bias/SiLU/residual -> fp16 -> its private swizzled staging) and issues its OWN TMA store into the
-//   channel slice of the consumer's concat buffer - no CTA-wide barrier anywhere in the steady state.
-// * persistent grid, two CTAs per SM, programmatic dependent launch (prologue overlaps the previous kernel's tail).
+//   TMA swizzle named in the wgmma shared-memory descriptor.
+// * warp roles (384 threads = 3 warpgroups): warp 0 = TMA producer (one elected lane issues), warps 1-3 idle, warpgroups 1 and 2 =
+//   consumers.  Consumer warpgroup w issues m64nBNk16 wgmma for pixel rows [64w, 64w+64) of the tile into its register accumulators,
+//   releases each operand stage as soon as the MMAs that read it have retired, and runs the epilogue (bias, activation, residual,
+//   fp16 / fp32 stores) straight from the accumulator fragment while the producer already fetches the next tile.
+// * persistent grid (one CTA per SM, deep operand ring), programmatic dependent launch (prologue overlaps the previous kernel's tail).
 //
 // Reference semantics: Conv.fuseforward (reference models/common.py:45-46) with BN folded as in
 // utils/torch_utils.py:182-202; Bottleneck shortcut add (models/common.py:105).
 #include "conv.h"
+#include "wgmma.cuh"
 
 #ifndef MYOLO_SILU_SFU_EVERY
-#define MYOLO_SILU_SFU_EVERY 2   // every n-th element of an epilogue chunk takes the two-MUFU SiLU: measured on B200 (tools/ab_lib.sh) 4 -> 3 -> 2: 9429 -> 9453 -> 9518 img/s
+#define MYOLO_SILU_SFU_EVERY 2   // every n-th output channel of a 16-channel group takes the two-MUFU SiLU (balances the FMA pipe and the SFU)
 #endif
 
 namespace myolo {
 
 static constexpr int kTileM = 128;
 static constexpr int kKStage = 64;        // K elements per pipeline stage
-static constexpr int kEpiWarps = 8;
-static constexpr int kNumThreads = 64 + kEpiWarps * 32;
-static constexpr int kTmemCols = 256;     // 2 accumulator rounds x 128 columns
-static constexpr int kAccStride = 128;
-static constexpr int kMaxWsBytes = 40 * 1024;
-static constexpr int kMaxWsBytesBig = 40 * 1024;    // = kMaxWsBytes: resident tiles that force one CTA per SM (MYOLO_WS_BIG_KB=100: 3x3 64->64,
-                                                     // 1x1 256->128 ...) measured 29 us SLOWER per forward on B200 (no co-resident CTA to overlap with)
-static constexpr int kSmemPerCta = 112 * 1024;   // two CTAs per SM: their epilogues / TMA latencies overlap
-static constexpr int kBiasBytes = 8192;         // bias vector of the layer in shared memory (<= 1920 output channels: the data gradient
-                                                // of SPP.cv2 has 1024)
+static constexpr int kNumThreads = 384;   // producer warpgroup + two consumer warpgroups
+static constexpr int kMaxStages = 8;
+static constexpr int kSmemBudget = 227 * 1024;
+static constexpr int kBiasBytes = 8192;   // bias vector of the layer in shared memory (<= 1920 output channels: the data gradient
+                                          // of SPP.cv2 has 1024)
 
-#ifdef MYOLO_TIMELINE
-#define DBG_STAMP(slot) do { if (p.dbg && blockIdx.x == 0 && it < 64) p.dbg[it * 16 + (slot)] = clock64(); } while (0)
-#define DBG_STAMP0(slot) do { if (p.dbg && blockIdx.x == 0 && threadIdx.x == 0) p.dbg[(slot)] = clock64(); } while (0)
-#else
-#define DBG_STAMP(slot) do { } while (0)
-#define DBG_STAMP0(slot) do { } while (0)
-#endif
-
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, int kc, uint32_t base_offset) {
-  // K-major canonical layout, rows of kc*2 bytes, 8-row groups (PTX ISA "matrix descriptor", sm_100 version=1)
-  const uint32_t sw_bytes = kc * 2;
-  const uint64_t layout = sw_bytes == 128 ? 2ull : (sw_bytes == 64 ? 4ull : 6ull);
-  const uint64_t sbo = (8u * sw_bytes) >> 4;
+// K-major swizzled operand (rows of kc*2 bytes = the swizzle width, 8-row swizzle atoms), PTX ISA "matrix descriptor" of wgmma
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, int row_bytes) {
+  const uint64_t layout = row_bytes == 128 ? 1ull : (row_bytes == 64 ? 2ull : 3ull);
   uint64_t d = 0;
-  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);   // start address, bits [0,14)
-  d |= (uint64_t)1 << 16;                    // leading byte offset (ignored for swizzled K-major), bits [16,30)
-  d |= sbo << 32;                            // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                    // descriptor version (Blackwell)
-  d |= (uint64_t)(base_offset & 7) << 49;    // matrix base offset (start not aligned to the swizzle repeat)
-  d |= layout << 61;                         // swizzle mode
+  d |= (uint64_t)((saddr & 0x3FFFF) >> 4);             // start address
+  d |= (uint64_t)1 << 16;                              // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)((8u * row_bytes) >> 4) << 32;        // stride byte offset: next group of 8 rows
+  d |= layout << 62;                                   // swizzle mode
   return d;
 }
-
-// The MMA issuer is ONE thread: every instruction it executes sits on the critical path of the tensor pipe.  Descriptors are
-// therefore split into a kernel-constant high word and a low word that is a plain 32-bit add away from a per-stage base.
-__device__ __forceinline__ uint32_t desc_hi(int kc) { return (uint32_t)(make_smem_desc(0u, kc, 0u) >> 32); }
-__device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr & 0x3FFFFu) >> 4) | (1u << 16); }
-__device__ __forceinline__ uint64_t desc_join(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
-
-__device__ __forceinline__ void sts128(uint32_t addr, const uint4& v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-template <int N>
-__device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
 
 struct TileCoord { int b, y0, x0, n0; };
 __device__ __forceinline__ int fdiv(int n, const FastDiv& f) { return (int)((__umulhi((unsigned)n, f.mul) + (unsigned)n) >> f.shr); }
@@ -89,598 +58,149 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvTcParams& p, int tile
   t.n0 = n_tile * p.BN;
   return t;
 }
-// tile g of a vertical round (MODE 2): G consecutive output rows of one full-row column block
-__device__ __forceinline__ TileCoord decode_vround(const ConvTcParams& p, int round, int g) {
-  TileCoord t;
-  t.b = fdiv(round, p.fd_rpi);
-  const int r = round - t.b * p.rounds_per_img;
-  const int tyg = fdiv(r, p.fd_tx);
-  t.x0 = (r - tyg * p.tiles_x) * p.tw;
-  t.y0 = tyg * p.G + g;
-  t.n0 = 0;
-  return t;
+
+__device__ __forceinline__ float act_out(float v, int act, int ch) {
+  if (act == MYOLO_ACT_SILU) return (ch & 15) % MYOLO_SILU_SFU_EVERY == MYOLO_SILU_SFU_EVERY - 1 ? silu_f_sfu(v) : silu_f(v);
+  if (act == MYOLO_ACT_SIGMOID) return sigmoid_f(v);
+  return v;
 }
 
-// tile g of a round: pair mode maps rounds to (M-tile pair, N tile) and, past n_pair_rounds, to single tiles; otherwise tile = round*G + g
-__device__ __forceinline__ TileCoord decode_rg(const ConvTcParams& p, int round, int g, int tiles_per_img) {
-  if (!p.pair) return decode_tile(p, round * p.G + g, tiles_per_img);
-  int m, nt;
-  if (round < p.n_pair_rounds) {
-    const int pm = fdiv(round, p.fd_ntn);
-    nt = round - pm * p.n_tiles_n;
-    m = 2 * pm + g;
-  } else {
-    const int s = round - p.n_pair_rounds;
-    const int ms = fdiv(s, p.fd_ntn);
-    nt = s - ms * p.n_tiles_n;
-    m = p.m_done + ms;
-  }
-  TileCoord t;
-  t.b = fdiv(m, p.fd_tpi);
-  const int r = m - t.b * tiles_per_img;
-  const int ty = fdiv(r, p.fd_tx);
-  t.y0 = ty * p.th;
-  t.x0 = (r - ty * p.tiles_x) * p.tw;
-  t.n0 = nt * p.BN;
-  return t;
-}
-__device__ __forceinline__ int round_tiles(const ConvTcParams& p, int round) {
-  return p.pair ? (round < p.n_pair_rounds ? 2 : 1) : min(p.G, p.total_tiles - round * p.G);
-}
-
-// the kc/16 MMAs of one K chunk (16 K-elements = 32 bytes inside the swizzle atom: +2 in the (addr >> 4) descriptor field), fully unrolled
-// for every chunk width so that the issuing lane runs straight-line code.  `acc0`: accumulate flag of the first MMA (the rest accumulate).
-template <int KM>
-__device__ __forceinline__ void mma_chunk_k(uint32_t tmem_d, uint32_t la, uint32_t lb, uint32_t dhi, uint32_t idesc, uint32_t acc0) {
+// epilogue of one consumer warpgroup: the m64nBN accumulator fragment holds, for j < BN/8 and h < 2, output channels 8j + 2(lane%4) + {0,1}
+// of tile row 16*(warp%4) + lane/4 + 8h, in acc[4j + 2h + {0,1}]
+template <int BN, bool RES>
+__device__ __forceinline__ void epilogue(const ConvTcParams& p, const float (&acc)[BN / 2], const float* bias_s, const TileCoord& tc, int row0) {
+  const int lane = threadIdx.x & 31;
 #pragma unroll
-  for (int k = 0; k < KM; ++k) umma_f16_ss(tmem_d, desc_join(la + 2 * k, dhi), desc_join(lb + 2 * k, dhi), idesc, k == 0 ? acc0 : 1u);
-}
-__device__ __forceinline__ void mma_chunk(int kmma, uint32_t tmem_d, uint32_t la, uint32_t lb, uint32_t dhi, uint32_t idesc, uint32_t acc0) {
-  if (kmma == 4) mma_chunk_k<4>(tmem_d, la, lb, dhi, idesc, acc0);
-  else if (kmma == 2) mma_chunk_k<2>(tmem_d, la, lb, dhi, idesc, acc0);
-  else mma_chunk_k<1>(tmem_d, la, lb, dhi, idesc, acc0);
-}
-
-__device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
-  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-// one 16-column chunk of the epilogue: accumulators + bias -> activation (+ residual) -> fp16 staging / fp32 global
-__device__ __forceinline__ void epilogue_chunk(const ConvTcParams& p, const uint32_t* v, const float* bias_s, int nb, const uint4& rr0,
-                                               const uint4& rr1, bool has_res, int ci, uint32_t stg, int sub_bytes, int sw, bool pix_ok,
-                                               size_t pix) {
-  const float4* bp = reinterpret_cast<const float4*>(bias_s + nb);       // shared memory, same address for the whole warp: broadcast
-  const float4 b0 = bp[0], b1 = bp[1], b2 = bp[2], b3 = bp[3];
-  float f[16];
-  f[0] = __uint_as_float(v[0]) + b0.x;   f[1] = __uint_as_float(v[1]) + b0.y;
-  f[2] = __uint_as_float(v[2]) + b0.z;   f[3] = __uint_as_float(v[3]) + b0.w;
-  f[4] = __uint_as_float(v[4]) + b1.x;   f[5] = __uint_as_float(v[5]) + b1.y;
-  f[6] = __uint_as_float(v[6]) + b1.z;   f[7] = __uint_as_float(v[7]) + b1.w;
-  f[8] = __uint_as_float(v[8]) + b2.x;   f[9] = __uint_as_float(v[9]) + b2.y;
-  f[10] = __uint_as_float(v[10]) + b2.z; f[11] = __uint_as_float(v[11]) + b2.w;
-  f[12] = __uint_as_float(v[12]) + b3.x; f[13] = __uint_as_float(v[13]) + b3.y;
-  f[14] = __uint_as_float(v[14]) + b3.z; f[15] = __uint_as_float(v[15]) + b3.w;
-  if (p.act == MYOLO_ACT_SILU) {
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + (lane >> 2) + 8 * h;
+    const int py = tc.y0 + (row >> p.log2_tw), px = tc.x0 + (row & (p.tw - 1));
+    if (py >= p.Ho || px >= p.Wo) continue;
+    const size_t pix = ((size_t)tc.b * p.Ho + py) * p.Wo + px;
 #pragma unroll
-    for (int e = 0; e < 16; ++e) f[e] = (e % MYOLO_SILU_SFU_EVERY) == MYOLO_SILU_SFU_EVERY - 1 ? silu_f_sfu(f[e]) : silu_f(f[e]);
-  } else if (p.act == MYOLO_ACT_SIGMOID) {
-#pragma unroll
-    for (int e = 0; e < 16; ++e) f[e] = sigmoid_f(f[e]);
-  }
-  if (has_res) {
-    const __half2* r0 = reinterpret_cast<const __half2*>(&rr0);
-    const __half2* r1 = reinterpret_cast<const __half2*>(&rr1);
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const float2 fa = __half22float2(r0[e]), fb = __half22float2(r1[e]);
-      f[2 * e] += fa.x;     f[2 * e + 1] += fa.y;
-      f[8 + 2 * e] += fb.x; f[8 + 2 * e + 1] += fb.y;
-    }
-  }
-  if (p.out_mode == 0) {
-    const int ch = ci << 4;
-    const int sub = ch >> p.log2_ow;
-    const int u0 = (ch & (p.ow - 1)) >> 3;
-    const uint32_t srow = stg + sub * sub_bytes;
-#pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      uint4 o;
-      __half2* o2 = reinterpret_cast<__half2*>(&o);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) o2[e] = __floats2half2_rn(f[h * 8 + 2 * e], f[h * 8 + 2 * e + 1]);
-      sts128(srow + (((u0 + h) ^ sw) << 4), o);
-    }
-  } else if (pix_ok) {
-    float* op = p.out_f32 + pix * p.out_f32_ctot + nb;
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      if (nb + 4 * e < p.out_f32_ctot)
-        *reinterpret_cast<float4*>(op + 4 * e) = make_float4(f[4 * e], f[4 * e + 1], f[4 * e + 2], f[4 * e + 3]);
+    for (int j = 0; j < BN / 8; ++j) {
+      const int c = 8 * j + 2 * (lane & 3);
+      const int n = tc.n0 + c;
+      float v0 = act_out(acc[4 * j + 2 * h] + bias_s[n], p.act, c);
+      float v1 = act_out(acc[4 * j + 2 * h + 1] + bias_s[n + 1], p.act, c + 1);
+      if (p.out_mode == 0) {
+        if (n >= p.out_c) continue;
+        if (RES && n < p.Co) {
+          const float2 r = __half22float2(*reinterpret_cast<const __half2*>(p.residual + pix * p.res_ctot + n));
+          v0 += r.x;
+          v1 += r.y;
+        }
+        *reinterpret_cast<__half2*>(p.out_f16 + pix * p.out_ctot + n) = __floats2half2_rn(v0, v1);
+      } else if (n < p.out_ctot) {
+        *reinterpret_cast<float2*>(p.out_f32 + pix * p.out_ctot + n) = make_float2(v0, v1);
+      }
     }
   }
 }
 
-// MODE 0: one TMA box per filter tap (1x1, stride 2, partial-row tiles, very wide dilations)
-// MODE 1: strip mode (3x3 stride 1, full-row tiles): one strip per (filter row, channel block) feeds the three kx taps
-// MODE 2: strip mode + vertical rounds (weights resident): the G tiles of a round are G consecutive rows sharing G+2 strips
-template <int MODE, bool RES>
-__global__ void __launch_bounds__(kNumThreads, 2)
+template <int BN, bool RES>
+__global__ void __launch_bounds__(kNumThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmA3,
-               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmO,
-               const __grid_constant__ ConvTcParams p) {
+               const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ConvTcParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int S = p.num_stages;
   uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem_a + S * p.a_stage_bytes;                 // per-stage B ring, or the resident weight tile (ws_mode)
-  uint8_t* smem_o = smem_b + (p.ws_mode ? p.b_res_bytes : S * p.b_stage_bytes);
-  const int sub_bytes = 32 * p.ow * 2;                            // one warp sub-box: 32 rows x ow channels
-  const int stg_warp_bytes = p.n_sub * sub_bytes;
-  float* bias_s = reinterpret_cast<float*>(smem_o + kEpiWarps * p.n_stg * stg_warp_bytes);   // [n_tiles_n * BN] fp32
-  uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(bias_s) + kBiasBytes);
-  uint64_t* full_bar = bars;
-  uint64_t* empty_bar = bars + S;
-  uint64_t* tfull_bar = bars + 2 * S;
-  uint64_t* tempty_bar = bars + 2 * S + 2;
-  uint64_t* bres_bar = bars + 2 * S + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * S + 5);
+  uint8_t* smem_b = smem_a + S * p.a_stage_bytes;
+  float* bias_s = reinterpret_cast<float*>(smem_b + S * p.b_stage_bytes);   // [n_tiles_n * BN] fp32
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(bias_s) + kBiasBytes);
+  uint64_t* empty_bar = full_bar + S;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int b_sub_bytes = p.BN * p.kc * 2;
-  DBG_STAMP0(11);
-
-  // ---- set-up.  Warp 0 (the TMA producer) only ARRIVES at the set-up barrier: it initialises the mbarriers and then starts fetching
-  // while warp 1 allocates TMEM and the epilogue warps copy the bias vector (a weight constant) into shared memory. ----
-  // Programmatic dependent launch: let the next kernel of the stream start its own prologue as early as possible.
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
-  if (warp == 0) {
-    if (lane == 0) {
-      tma_prefetch_desc(&tmA0);
-      tma_prefetch_desc(&tmB);
-      if (p.out_mode == 0) tma_prefetch_desc(&tmO);
-      for (int i = 0; i < S; ++i) {
-        mbar_init(&full_bar[i], 1);
-        mbar_init(&empty_bar[i], 1);
-      }
-      for (int i = 0; i < 2; ++i) {
-        mbar_init(&tfull_bar[i], 1);
-        mbar_init(&tempty_bar[i], kEpiWarps);
-      }
-      mbar_init(bres_bar, 1);
-      fence_mbar_init();
-      __threadfence_block();
-    }
-    __syncwarp();
-    named_bar_arrive(1, kNumThreads);
-  } else {
-    if (warp == 1) {
-      tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-    } else {
-      const int nb_tot = p.n_tiles_n * p.BN;
-      for (int i = threadIdx.x - 64; i < nb_tot; i += kEpiWarps * 32) bias_s[i] = __ldg(p.bias + i);
-    }
-    tcgen05_fence_before();
-    named_bar_sync(1, kNumThreads);
-    tcgen05_fence_after();
-  }
-  DBG_STAMP0(12);
-
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);   // warp-uniform for the compiler: wgmma is issued under role branches
   const int a_sub_bytes = kTileM * p.kc * 2;
-  const int row_bytes = p.kc * 2;
+  const int b_sub_bytes = BN * p.kc * 2;
   const int tiles_per_img = p.tiles_x * p.tiles_y;
 
-  // Producer and MMA roles run WARP-CONVERGED: every lane executes the (warp-uniform) address / descriptor arithmetic so that ptxas keeps it
-  // in uniform registers, and only the issuing instructions are predicated on one elected lane.  (Run inside an `if (lane == 0)` branch the
-  // same code needs ~7 R2UR moves per tcgen05.mma / TMA instruction: ~125 clk per MMA where an N = 64 MMA occupies the tensor pipe for 32.)
-  if (warp == 0) {
-    // ===================== TMA producer =====================
-    const bool leader = elect_one();
-    if (p.ws_mode && leader) {
-      // weights are constants (never written by a predecessor kernel): fetch the resident weight tile before the dependency wait
-      mbar_arrive_expect_tx(bres_bar, p.n_chunks * b_sub_bytes);
-      for (int q = 0; q < p.n_chunks; ++q) tma_load_2d(smem_b + q * b_sub_bytes, &tmB, bres_bar, q * p.kc, 0);
+  // programmatic dependent launch: let the next kernel of the stream start its own prologue as early as possible
+  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA0);
+    tma_prefetch_desc(&tmB);
+    for (int i = 0; i < S; ++i) {
+      mbar_init(&full_bar[i], 1);
+      mbar_init(&empty_bar[i], 2);          // one arrive per consumer warpgroup
     }
-    // ... wait here until every predecessor grid has completed and flushed (activations / residual come from them)
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    DBG_STAMP0(13);
-    int stage = 0;
-    uint32_t phase = 0;
-    int it = 0;
-    for (int round = blockIdx.x; round < p.total_rounds; round += gridDim.x) {
-      if (MODE == 2) {
-        // G vertically adjacent full-row tiles: rows y0 .. y0+n_valid-1 need input rows y0-1 .. y0+n_valid -> n_valid+2 strips
-        const TileCoord t = decode_vround(p, round, 0);
-        const int n_valid = min(p.G, p.Ho - t.y0);
-        if (leader) DBG_STAMP(0);
-        for (int cb = 0; cb < p.cblocks; ++cb)
-          for (int s = 0; s < n_valid + 2; ++s) {
-            mbar_wait_relaxed(&empty_bar[stage], phase ^ 1, p.spin_ns);
-            __syncwarp();
-            if (leader) {
-              mbar_arrive_expect_tx(&full_bar[stage], (p.tw + 2) * row_bytes);
-              tma_load_4d(smem_a + stage * p.a_stage_bytes, &tmA0, &full_bar[stage], cb * p.kc, t.x0 - 1, t.y0 - 1 + s, t.b);
-            }
-            if (++stage == S) { stage = 0; phase ^= 1; }
-          }
-        if (leader) DBG_STAMP(1);
-        it += n_valid;
-        continue;
-      }
-      if (MODE != 2 && p.pair) {
-        // two M tiles, one weight fetch: every stage holds [A of tile 0 | A of tile 1 | B]
-        const int nv = round < p.n_pair_rounds ? 2 : 1;
-        const TileCoord t0 = decode_rg(p, round, 0, tiles_per_img);
-        const TileCoord t1 = decode_rg(p, round, nv - 1, tiles_per_img);
-        const int a_half = p.a_stage_bytes >> 1;
-        if (leader) DBG_STAMP(0);
-        if (MODE == 1) {
-          for (int ky = 0; ky < 3; ++ky)
-            for (int cb = 0; cb < p.cblocks; ++cb) {
-              mbar_wait_relaxed(&empty_bar[stage], phase ^ 1, p.spin_ns);
-              __syncwarp();
-              if (leader) {
-                uint8_t* sa = smem_a + stage * p.a_stage_bytes;
-                mbar_arrive_expect_tx(&full_bar[stage], nv * (p.tw + 2 * p.dil) * row_bytes + 3 * b_sub_bytes);
-                tma_load_4d(sa, &tmA0, &full_bar[stage], cb * p.kc, t0.x0 - p.dil, t0.y0 + (ky - 1) * p.dil, t0.b);
-                if (nv == 2) tma_load_4d(sa + a_half, &tmA0, &full_bar[stage], cb * p.kc, t1.x0 - p.dil, t1.y0 + (ky - 1) * p.dil, t1.b);
-                for (int kx = 0; kx < 3; ++kx)
-                  tma_load_2d(smem_b + stage * p.b_stage_bytes + kx * b_sub_bytes, &tmB, &full_bar[stage],
-                              ((ky * 3 + kx) * p.cblocks + cb) * p.kc, t0.n0);
-              }
-              if (++stage == S) { stage = 0; phase ^= 1; }
-            }
-        } else {
-          int tap = 0, cb = 0, q = 0;
-          for (int ks = 0; ks < p.n_kstages; ++ks) {
-            mbar_wait_relaxed(&empty_bar[stage], phase ^ 1, p.spin_ns);
-            __syncwarp();
-            const int nch = min(p.chunks_per_stage, p.n_chunks - q);
-            if (leader) mbar_arrive_expect_tx(&full_bar[stage], nch * (nv * a_sub_bytes + b_sub_bytes));
-            uint8_t* sa = smem_a + stage * p.a_stage_bytes;
-            uint8_t* sb = smem_b + stage * p.b_stage_bytes;
-            for (int j = 0; j < nch; ++j, ++q) {
-              const int mi = p.tap_map[tap];
-              const CUtensorMap* tm = mi == 0 ? &tmA0 : (mi == 1 ? &tmA1 : (mi == 2 ? &tmA2 : &tmA3));
-              if (leader) {
-                tma_load_4d(sa + j * a_sub_bytes, tm, &full_bar[stage], cb * p.kc, t0.x0 + p.tap_dx[tap], t0.y0 + p.tap_dy[tap], t0.b);
-                if (nv == 2)
-                  tma_load_4d(sa + a_half + j * a_sub_bytes, tm, &full_bar[stage], cb * p.kc, t1.x0 + p.tap_dx[tap], t1.y0 + p.tap_dy[tap], t1.b);
-                tma_load_2d(sb + j * b_sub_bytes, &tmB, &full_bar[stage], q * p.kc, t0.n0);
-              }
-              if (++cb == p.cblocks) { cb = 0; ++tap; }
-            }
-            if (++stage == S) { stage = 0; phase ^= 1; }
-          }
-        }
-        if (leader) DBG_STAMP(1);
-        ++it;
-        continue;
-      }
-      for (int g = 0; g < p.G; ++g) {
-        const int tile = round * p.G + g;
-        if (tile >= p.total_tiles) break;
-        const TileCoord t = decode_tile(p, tile, tiles_per_img);
-        if (leader) DBG_STAMP(0);
-        if (MODE == 1) {
-          for (int ky = 0; ky < 3; ++ky)
-            for (int cb = 0; cb < p.cblocks; ++cb) {
-              mbar_wait_relaxed(&empty_bar[stage], phase ^ 1, p.spin_ns);
-              __syncwarp();
-              if (leader) {
-                mbar_arrive_expect_tx(&full_bar[stage], (p.tw + 2 * p.dil) * row_bytes + (p.ws_mode ? 0 : 3 * b_sub_bytes));
-                tma_load_4d(smem_a + stage * p.a_stage_bytes, &tmA0, &full_bar[stage], cb * p.kc, t.x0 - p.dil, t.y0 + (ky - 1) * p.dil, t.b);
-                if (!p.ws_mode)
-                  for (int kx = 0; kx < 3; ++kx)
-                    tma_load_2d(smem_b + stage * p.b_stage_bytes + kx * b_sub_bytes, &tmB, &full_bar[stage],
-                                ((ky * 3 + kx) * p.cblocks + cb) * p.kc, t.n0);
-              }
-              if (++stage == S) { stage = 0; phase ^= 1; }
-            }
-        } else {
-          int tap = 0, cb = 0, q = 0;
-          const int stage_tx = a_sub_bytes + (p.ws_mode ? 0 : b_sub_bytes);
-          for (int ks = 0; ks < p.n_kstages; ++ks) {
-            mbar_wait_relaxed(&empty_bar[stage], phase ^ 1, p.spin_ns);
-            __syncwarp();
-            const int nch = min(p.chunks_per_stage, p.n_chunks - q);
-            if (leader) mbar_arrive_expect_tx(&full_bar[stage], nch * stage_tx);
-            uint8_t* sa = smem_a + stage * p.a_stage_bytes;
-            uint8_t* sb = smem_b + stage * p.b_stage_bytes;
-            for (int j = 0; j < nch; ++j, ++q) {
-              const int mi = p.tap_map[tap];
-              const CUtensorMap* tm = mi == 0 ? &tmA0 : (mi == 1 ? &tmA1 : (mi == 2 ? &tmA2 : &tmA3));
-              if (leader) {
-                tma_load_4d(sa + j * a_sub_bytes, tm, &full_bar[stage], cb * p.kc, t.x0 + p.tap_dx[tap], t.y0 + p.tap_dy[tap], t.b);
-                if (!p.ws_mode) tma_load_2d(sb + j * b_sub_bytes, &tmB, &full_bar[stage], q * p.kc, t.n0);
-              }
-              if (++cb == p.cblocks) { cb = 0; ++tap; }
-            }
-            if (++stage == S) { stage = 0; phase ^= 1; }
-          }
-        }
-        if (leader) DBG_STAMP(1);
-        ++it;
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer (one elected lane issues; the warp computes the descriptors) =====================
-    const bool leader = elect_one();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t idesc = (1u << 4)                       // D format: fp32
-                           | (0u << 7) | (0u << 10)        // A, B format: fp16
-                           | (0u << 15) | (0u << 16)       // A, B K-major
-                           | ((uint32_t)(p.BN >> 3) << 17) // N
-                           | ((uint32_t)(kTileM >> 4) << 24);  // M
-    int stage = 0;
-    uint32_t phase = 0;
-    int as = 0;
-    uint32_t aphase = 0;
-    const int kmma = p.kc / 16;
-    const uint32_t dhi = desc_hi(p.kc);
-    const uint32_t lb_res = desc_lo(smem_u32(smem_b));
-    const uint32_t la_base = desc_lo(smem_u32(smem_a));
-    const uint32_t lb_base = desc_lo(smem_u32(smem_b));
-    const uint32_t a_stage16 = (uint32_t)(p.a_stage_bytes >> 4), b_stage16 = (uint32_t)(p.b_stage_bytes >> 4);
-    const int bsub16 = b_sub_bytes >> 4, asub16 = a_sub_bytes >> 4, row16 = row_bytes >> 4;
-    if (p.ws_mode) { mbar_wait(bres_bar, 0); __syncwarp(); }
-    int it = 0;
-    for (int round = blockIdx.x; round < p.total_rounds; round += gridDim.x) {
-      if (leader) DBG_STAMP(2);
-      mbar_wait_relaxed(&tempty_bar[as], aphase ^ 1, p.spin_ns);
-      __syncwarp();
-      tcgen05_fence_after();
-      if (leader) DBG_STAMP(3);
-      if (MODE == 2) {
-        const int r = round - fdiv(round, p.fd_rpi) * p.rounds_per_img;
-        const int n_valid = min(p.G, p.Ho - fdiv(r, p.fd_tx) * p.G);
-        for (int cb = 0; cb < p.cblocks; ++cb)
-          for (int s = 0; s < n_valid + 2; ++s) {
-            mbar_wait(&full_bar[stage], phase);
-            __syncwarp();
-            tcgen05_fence_after();
-            const uint32_t la = la_base + (uint32_t)stage * a_stage16;
-            // strip s (input row y0-1+s) is filter row ky = s-g of output row g
-            for (int g = max(0, s - 2); g <= min(n_valid - 1, s); ++g) {
-              const int ky = s - g;
-              const uint32_t tmem_d = tmem_base + as * kAccStride + g * p.BN;
-              uint32_t lb = lb_res + (uint32_t)((ky * 3 * p.cblocks + cb) * bsub16);
-#pragma unroll
-              for (int kx = 0; kx < 3; ++kx) {
-                const uint32_t lak = la + kx * row16;
-                if (leader) mma_chunk(kmma, tmem_d, lak, lb, dhi, idesc, (uint32_t)((cb | ky | kx) != 0));
-                lb += (uint32_t)(p.cblocks * bsub16);
-              }
-            }
-            if (leader) umma_commit(&empty_bar[stage]);
-            if (++stage == S) { stage = 0; phase ^= 1; }
-          }
-      } else if (p.pair) {
-        const int nv = round < p.n_pair_rounds ? 2 : 1;
-        const uint32_t a_half16 = (uint32_t)(p.a_stage_bytes >> 5);
-        const uint32_t tmem_r = tmem_base + as * p.acc_stride;
-        if (MODE == 1) {
-          uint32_t first = 0;
-          for (int ky = 0; ky < 3; ++ky)
-            for (int cb = 0; cb < p.cblocks; ++cb) {
-              mbar_wait(&full_bar[stage], phase);
-              __syncwarp();
-              tcgen05_fence_after();
-              const uint32_t la = la_base + (uint32_t)stage * a_stage16;
-              const uint32_t lb0 = lb_base + (uint32_t)stage * b_stage16;
-              for (int g = 0; g < nv; ++g) {
-                uint32_t lb = lb0;
-#pragma unroll
-                for (int kx = 0; kx < 3; ++kx) {
-                  if (leader) mma_chunk(kmma, tmem_r + g * p.BN, la + g * a_half16 + kx * p.dil * row16, lb, dhi, idesc, kx == 0 ? first : 1u);
-                  lb += (uint32_t)bsub16;
-                }
-              }
-              first = 1;
-              if (leader) umma_commit(&empty_bar[stage]);
-              if (++stage == S) { stage = 0; phase ^= 1; }
-            }
-        } else {
-          int q = 0;
-          for (int ks = 0; ks < p.n_kstages; ++ks) {
-            mbar_wait(&full_bar[stage], phase);
-            __syncwarp();
-            tcgen05_fence_after();
-            if (ks == 0 && leader) DBG_STAMP(4);
-            const int nch = min(p.chunks_per_stage, p.n_chunks - q);
-            for (int g = 0; g < nv; ++g) {
-              uint32_t la = la_base + (uint32_t)stage * a_stage16 + g * a_half16;
-              uint32_t lb = lb_base + (uint32_t)stage * b_stage16;
-              for (int j = 0; j < nch; ++j) {
-                if (leader) mma_chunk(kmma, tmem_r + g * p.BN, la, lb, dhi, idesc, (uint32_t)((ks | j) != 0));
-                la += asub16;
-                lb += bsub16;
-              }
-            }
-            q += nch;
-            if (leader) umma_commit(&empty_bar[stage]);
-            if (++stage == S) { stage = 0; phase ^= 1; }
-          }
-        }
-      } else {
-        for (int g = 0; g < p.G; ++g) {
-          if (round * p.G + g >= p.total_tiles) break;
-          const uint32_t tmem_d = tmem_base + as * kAccStride + g * p.BN;
-          if (MODE == 1) {
-            uint32_t first = 0;
-            for (int ky = 0; ky < 3; ++ky)
-              for (int cb = 0; cb < p.cblocks; ++cb) {
-                mbar_wait(&full_bar[stage], phase);
-                __syncwarp();
-                tcgen05_fence_after();
-                const uint32_t la = la_base + (uint32_t)stage * a_stage16;
-                uint32_t lb = p.ws_mode ? lb_res + (uint32_t)((ky * 3 * p.cblocks + cb) * bsub16) : lb_base + (uint32_t)stage * b_stage16;
-                const uint32_t lb_step = p.ws_mode ? (uint32_t)(p.cblocks * bsub16) : (uint32_t)bsub16;
-#pragma unroll
-                for (int kx = 0; kx < 3; ++kx) {
-                  const uint32_t lak = la + kx * p.dil * row16;          // same strip, shifted by kx*dil pixels
-                  if (leader) mma_chunk(kmma, tmem_d, lak, lb, dhi, idesc, first);
-                  first = 1;
-                  lb += lb_step;
-                }
-                if (leader) umma_commit(&empty_bar[stage]);
-                if (++stage == S) { stage = 0; phase ^= 1; }
-              }
-          } else {
-            int q = 0;
-            for (int ks = 0; ks < p.n_kstages; ++ks) {
-              mbar_wait(&full_bar[stage], phase);
-              __syncwarp();
-              tcgen05_fence_after();
-              if (ks == 0 && leader) DBG_STAMP(4);
-              const int nch = min(p.chunks_per_stage, p.n_chunks - q);
-              uint32_t la = la_base + (uint32_t)stage * a_stage16;
-              uint32_t lb = p.ws_mode ? lb_res + (uint32_t)(q * bsub16) : lb_base + (uint32_t)stage * b_stage16;
-              for (int j = 0; j < nch; ++j, ++q) {
-                if (leader) mma_chunk(kmma, tmem_d, la, lb, dhi, idesc, (uint32_t)((ks | j) != 0));
-                la += asub16;
-                lb += bsub16;
-              }
-              if (leader) umma_commit(&empty_bar[stage]);  // smem slot reusable once these MMAs have read it
-              if (++stage == S) { stage = 0; phase ^= 1; }
-            }
-          }
-        }
-      }
-      if (leader) umma_commit(&tfull_bar[as]);       // all accumulators of the round complete -> epilogue
-      if (leader) DBG_STAMP(5);
-      if (++as == 2) { as = 0; aphase ^= 1; }
-      ++it;
-    }
-  } else if (warp >= 2) {
-    // ===================== epilogue: 8 autonomous warps =====================
-    const uint32_t tmem_base = *tmem_slot;
-    const int quarter = warp & 3;                  // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;
-    const int row = quarter * 32 + lane;           // tile row == pixel index inside the tw x th rectangle
-    const int ry = row >> p.log2_tw, rx = row & (p.tw - 1);
-    const int wy = (quarter * 32) >> p.log2_tw, wx = (quarter * 32) & (p.tw - 1);   // origin of this warp's 32-row rectangle
-    const int units_log2 = p.log2_ow - 3;          // 16-byte units per staging row: 8 / 4 / 2
-    const int sw = units_log2 == 3 ? (lane & 7) : (units_log2 == 2 ? ((lane >> 1) & 3) : ((lane >> 2) & 1));
-    const uint32_t stg0 = smem_u32(smem_o) + (warp - 2) * p.n_stg * stg_warp_bytes + lane * (p.ow * 2);
-    const int nchunks_w = p.ep_cols >> 4;
-    const int c_lo = p.ep_split_cols ? half * nchunks_w : 0;
-    const int g_first = p.ep_split_cols ? 0 : half;
-    const int g_step = p.ep_split_cols ? 1 : 2;
-    const bool idle_half = (!p.ep_split_cols && p.G == 1 && !p.pair && half == 1);
-    constexpr bool has_res = RES;
-    int as = 0;
-    uint32_t aphase = 0;
-    int sbuf = 0;
-    int it = 0;
-    // the predecessor's output (the residual) is only read after the dependency wait
-    if (has_res) asm volatile("griddepcontrol.wait;" ::: "memory");
-    for (int round = blockIdx.x; round < p.total_rounds; round += gridDim.x) {
-      int n_valid;
-      if (MODE == 2) {
-        const int r = round - fdiv(round, p.fd_rpi) * p.rounds_per_img;
-        n_valid = min(p.G, p.Ho - fdiv(r, p.fd_tx) * p.G);
-      } else {
-        n_valid = round_tiles(p, round);
-      }
-      if (warp == 2 && lane == 0) DBG_STAMP(6);
-      bool waited = false;
-      if (!idle_half) {
-        for (int g = g_first; g < n_valid; g += g_step) {
-          const TileCoord tc = MODE == 2 ? decode_vround(p, round, g) : decode_rg(p, round, g, tiles_per_img);
-          const int py = tc.y0 + ry, px = tc.x0 + rx;
-          const bool pix_ok = (py < p.Ho) && (px < p.Wo);
-          const size_t pix = ((size_t)tc.b * p.Ho + py) * p.Wo + px;
-          // residual of the first column pair: issued before the accumulator wait so that its latency hides behind the MMAs
-          uint4 rr[4];
-          rr[0] = rr[1] = rr[2] = rr[3] = make_uint4(0, 0, 0, 0);
-          const __half* rp = has_res ? p.residual + pix * p.res_ctot + tc.n0 + c_lo * 16 : nullptr;
-          if (has_res && pix_ok) {
-            const int nb = tc.n0 + c_lo * 16;
-            if (nb < p.Co) rr[0] = __ldg(reinterpret_cast<const uint4*>(rp));
-            if (nb + 8 < p.Co) rr[1] = __ldg(reinterpret_cast<const uint4*>(rp + 8));
-            if (nchunks_w > 1) {
-              if (nb + 16 < p.Co) rr[2] = __ldg(reinterpret_cast<const uint4*>(rp + 16));
-              if (nb + 24 < p.Co) rr[3] = __ldg(reinterpret_cast<const uint4*>(rp + 24));
-            }
-          }
-          if (p.out_mode == 0) {
-            // my staging buffer was handed to the TMA engine n_stg stores ago: it must have been read by now
-            if (lane == 0) {
-              if (p.n_stg == 2) tma_store_wait_read<1>();
-              else tma_store_wait_read<0>();
-            }
-            __syncwarp();
-            if (warp == 2 && lane == 0 && g == g_first) DBG_STAMP(8);
-          }
-          if (!waited) {
-            mbar_wait(&tfull_bar[as], aphase);
-            tcgen05_fence_after();
-            waited = true;
-            if (warp == 2 && lane == 0) DBG_STAMP(7);
-          }
-          const uint32_t taddr = tmem_base + ((uint32_t)(quarter * 32) << 16) + as * p.acc_stride + g * p.BN;
-          const uint32_t stg = stg0 + sbuf * stg_warp_bytes;
-          for (int cp = 0; cp < nchunks_w; cp += 2) {
-            const bool two = cp + 1 < nchunks_w;
-            const int c = c_lo + cp;
-            const int nb = tc.n0 + c * 16;
-            uint32_t v[32];
-            tmem_ld_32x32b_x16(taddr + c * 16, *reinterpret_cast<uint32_t(*)[16]>(&v[0]));
-            if (two) tmem_ld_32x32b_x16(taddr + c * 16 + 16, *reinterpret_cast<uint32_t(*)[16]>(&v[16]));
-            if (cp > 0 && has_res && pix_ok) {
-              const __half* rq = rp + cp * 16;
-              rr[0] = rr[1] = rr[2] = rr[3] = make_uint4(0, 0, 0, 0);
-              if (nb < p.Co) rr[0] = __ldg(reinterpret_cast<const uint4*>(rq));
-              if (nb + 8 < p.Co) rr[1] = __ldg(reinterpret_cast<const uint4*>(rq + 8));
-              if (two) {
-                if (nb + 16 < p.Co) rr[2] = __ldg(reinterpret_cast<const uint4*>(rq + 16));
-                if (nb + 24 < p.Co) rr[3] = __ldg(reinterpret_cast<const uint4*>(rq + 24));
-              }
-            }
-            tmem_ld_wait();
-            epilogue_chunk(p, &v[0], bias_s, nb, rr[0], rr[1], has_res, cp, stg, sub_bytes, sw, pix_ok, pix);
-            if (two) epilogue_chunk(p, &v[16], bias_s, nb + 16, rr[2], rr[3], has_res, cp + 1, stg, sub_bytes, sw, pix_ok, pix);
-          }
-          if (p.out_mode == 0) {
-            fence_proxy_async_smem();
-            __syncwarp();
-            if (lane == 0) {
-              const int nbase = tc.n0 + c_lo * 16;
-              for (int s = 0; s < p.n_sub; ++s) {
-                if (nbase + s * p.ow < p.Co)
-                  tma_store_4d(&tmO, smem_o + (warp - 2) * p.n_stg * stg_warp_bytes + sbuf * stg_warp_bytes + s * sub_bytes,
-                               nbase + s * p.ow, tc.x0 + wx, tc.y0 + wy, tc.b);
-              }
-              tma_store_commit();
-            }
-            if (p.n_stg == 2) sbuf ^= 1;
-          }
-        }
-      }
-      if (!waited) {   // idle half / no tile for this warp in a partial round: still take part in the accumulator hand-shake
-        mbar_wait(&tfull_bar[as], aphase);
-        tcgen05_fence_after();
-      }
-      // all TMEM reads of this warp for the round are complete (every tcgen05.ld was waited on): release the accumulators
-      tcgen05_fence_before();
-      __syncwarp();
-      if (warp == 2 && lane == 0) DBG_STAMP(9);
-      if (lane == 0) mbar_arrive(&tempty_bar[as]);
-      if (++as == 2) { as = 0; aphase ^= 1; }
-      ++it;
-    }
-    // shared memory must stay valid until the bulk stores have READ it; global visibility is given at grid completion
-    if (p.out_mode == 0 && lane == 0) tma_store_wait_read<0>();
+    fence_mbar_init();
   }
-
-  tcgen05_fence_before();
+  if (threadIdx.x >= 128) {                 // the bias vector is a weight constant: copied before the dependency wait
+    const int nb_tot = p.n_tiles_n * BN;
+    for (int i = threadIdx.x - 128; i < nb_tot; i += kNumThreads - 128) bias_s[i] = __ldg(p.bias + i);
+  }
   __syncthreads();
-  DBG_STAMP0(14);
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(*tmem_slot, (uint32_t)p.tmem_cols);
+
+  if (warp == 0) {
+    // ===================== TMA producer (warp-converged; one elected lane issues) =====================
+    const bool leader = elect_one();
+    asm volatile("griddepcontrol.wait;" ::: "memory");   // activations come from predecessor kernels
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      const TileCoord t = decode_tile(p, tile, tiles_per_img);
+      int tap = 0, cb = 0, q = 0;
+      for (int ks = 0; ks < p.n_kstages; ++ks) {
+        mbar_wait(&empty_bar[stage], phase ^ 1);
+        __syncwarp();
+        const int nch = min(p.chunks_per_stage, p.n_chunks - q);
+        if (leader) mbar_arrive_expect_tx(&full_bar[stage], nch * (a_sub_bytes + b_sub_bytes));
+        uint8_t* sa = smem_a + stage * p.a_stage_bytes;
+        uint8_t* sb = smem_b + stage * p.b_stage_bytes;
+        for (int j = 0; j < nch; ++j, ++q) {
+          const int mi = p.tap_map[tap];
+          const CUtensorMap* tm = mi == 0 ? &tmA0 : (mi == 1 ? &tmA1 : (mi == 2 ? &tmA2 : &tmA3));
+          if (leader) {
+            tma_load_4d(sa + j * a_sub_bytes, tm, &full_bar[stage], cb * p.kc, t.x0 + p.tap_dx[tap], t.y0 + p.tap_dy[tap], t.b);
+            tma_load_2d(sb + j * b_sub_bytes, &tmB, &full_bar[stage], q * p.kc, t.n0);
+          }
+          if (++cb == p.cblocks) { cb = 0; ++tap; }
+        }
+        if (++stage == S) { stage = 0; phase ^= 1; }
+      }
+    }
+  } else if (warp >= 4) {
+    // ===================== consumers: two warpgroups, 64 pixel rows each =====================
+    const int cw = (warp >> 2) - 1;
+    const bool signaller = (threadIdx.x & 127) == 0;
+    const int row_bytes = p.kc * 2;
+    const int kmma = p.kc / 16;
+    if (RES) asm volatile("griddepcontrol.wait;" ::: "memory");   // the residual is a predecessor's output
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    const uint32_t a_base = smem_u32(smem_a) + (uint32_t)(cw * 64 * row_bytes);
+    const uint32_t b_base = smem_u32(smem_b);
+    for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
+      const TileCoord t = decode_tile(p, tile, tiles_per_img);
+      int q = 0, prev = -1;
+      for (int ks = 0; ks < p.n_kstages; ++ks) {
+        mbar_wait(&full_bar[stage], phase);
+        const int nch = min(p.chunks_per_stage, p.n_chunks - q);
+        const uint32_t sa = a_base + (uint32_t)(stage * p.a_stage_bytes);
+        const uint32_t sb = b_base + (uint32_t)(stage * p.b_stage_bytes);
+        wgmma_fence();
+        wgmma_fence_regs(acc);
+        for (int j = 0; j < nch; ++j)
+          for (int k = 0; k < kmma; ++k)      // 16 K-elements = 32 bytes further inside the swizzle atom
+            wgmma_f16<BN, 0, 0>(acc, make_smem_desc(sa + j * a_sub_bytes + 32 * k, row_bytes),
+                                make_smem_desc(sb + j * b_sub_bytes + 32 * k, row_bytes), (uint32_t)((ks | j | k) != 0));
+        wgmma_commit();
+        wgmma_wait<1>();                        // the previous stage's MMAs have retired: its operands may be overwritten
+        if (prev >= 0 && signaller) mbar_arrive(&empty_bar[prev]);
+        prev = stage;
+        q += nch;
+        if (++stage == S) { stage = 0; phase ^= 1; }
+      }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0 && signaller) mbar_arrive(&empty_bar[prev]);
+      epilogue<BN, RES>(p, acc, bias_s, t, cw * 64 + (warp & 3) * 16);
+    }
   }
 }
 
@@ -772,8 +292,6 @@ bool conv_tc_eligible(const ConvOp& op) {
   return true;
 }
 
-int g_conv_tc_force_pair = 0;
-
 int conv_tc_prepare(ConvOp& op, int num_sms) {
   ConvTcParams& p = op.p;
   memset(&p, 0, sizeof(p));
@@ -794,16 +312,6 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
     for (int bn = 128; bn >= 16; bn -= 16)
       if (co16 % bn == 0) { p.BN = bn; break; }
   }
-  // small grids (P4/P5 layers): trade N-tile width for CTA count until every SM has work (A is re-read from L2, which is cheap here)
-  static int split_env = -1;
-  if (split_env < 0) {
-    const char* e = getenv("MYOLO_NSPLIT");
-    split_env = e ? atoi(e) : 0;   // measured on B200: narrower tiles lose (more weight re-reads, same latency chain) - off by default
-  }
-  if (split_env) {
-    const int m_tiles = p.B * p.tiles_x * p.tiles_y;
-    while (p.BN >= 64 && p.BN % 32 == 0 && m_tiles * ceil_div(co16, p.BN) < 2 * num_sms) p.BN /= 2;
-  }
   p.n_tiles_n = ceil_div(co16, p.BN);
   MYOLO_REQUIRE(op.Co_pad >= p.n_tiles_n * p.BN, "conv_tc: Co_pad %d < %d", op.Co_pad, p.n_tiles_n * p.BN);
   p.total_tiles = p.B * p.tiles_x * p.tiles_y * p.n_tiles_n;
@@ -814,14 +322,14 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
   p.chunks_per_stage = kKStage / p.kc;
   p.n_kstages = ceil_div(p.n_chunks, p.chunks_per_stage);
   p.act = op.act;
-  p.dil = op.dil;
   p.bias = op.bias;
   p.residual = op.has_res ? reinterpret_cast<const __half*>(op.res.base) : nullptr;
   p.res_ctot = op.has_res ? op.res.ctot : 0;
   p.out_mode = op.out.dtype == MYOLO_F16 ? 0 : 1;
+  p.out_f16 = p.out_mode ? nullptr : reinterpret_cast<__half*>(op.out.base);
   p.out_f32 = p.out_mode ? reinterpret_cast<float*>(op.out.base) : nullptr;
-  p.out_f32_ctot = p.out_mode ? op.out.ctot : 0;
-  p.dbg = nullptr;
+  p.out_c = op.out.C;
+  p.out_ctot = op.out.ctot;
   for (int t = 0; t < p.taps; ++t) {
     const int ky = op.k == 3 ? t / 3 : 1, kx = op.k == 3 ? t % 3 : 1;
     if (op.stride == 1) {
@@ -835,159 +343,21 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
       p.tap_dx[t] = (kx == 0) ? -1 : 0;
     }
   }
-  const int max_ctas = 2 * num_sms;
-  // strip mode: 3x3 stride-1 conv on full-row tiles (any swizzle width: rows are shifted by whole pixels)
-  static int strip_env = -1;
-  if (strip_env < 0) {
-    const char* e = getenv("MYOLO_STRIP");
-    strip_env = e ? atoi(e) : 1;   // 1: shifted start addresses (the UMMA swizzle is a function of the absolute smem address - verified on B200)
-  }
-  p.strip = (strip_env > 0 && op.k == 3 && op.stride == 1 && p.th == 1 && p.tw + 2 * op.dil <= 256) ? strip_env : 0;
-  // weights-stationary mode: one N tile and the whole [BN x K] weight tile stays resident in shared memory.  Up to kMaxWsBytes two CTAs
-  // share an SM; larger tiles (up to kMaxWsBytesBig: 3x3 64->64, 1x1 256->128, 384->64 ...) take the SM alone - shared-memory fill
-  // bandwidth (measured: 40 B/clk per SM) is what bounds these layers, so not re-fetching the weights per M tile is worth the lost co-residency
-  static int ws_kb = -1, ws_big_kb = -1;
-  if (ws_kb < 0) {
-    const char* e = getenv("MYOLO_WS_KB");
-    ws_kb = e ? atoi(e) : kMaxWsBytes / 1024;
-    const char* e2 = getenv("MYOLO_WS_BIG_KB");
-    ws_big_kb = e2 ? atoi(e2) : kMaxWsBytesBig / 1024;
-  }
-  const int w_bytes = p.n_chunks * p.BN * p.kc * 2;
-  p.ws_mode = (p.n_tiles_n == 1 && w_bytes <= (ws_big_kb > ws_kb ? ws_big_kb : ws_kb) * 1024) ? 1 : 0;
-  const bool ws_big = p.ws_mode && w_bytes > ws_kb * 1024;       // forces one CTA per SM
-  p.b_res_bytes = p.ws_mode ? (int)align_up(w_bytes, 1024) : 0;
-  // accumulator rounds: G tiles share one TMEM stage when the layer is big enough to keep every CTA busy
-  const int cta_budget = ws_big ? num_sms : max_ctas;
-  // (rounds >= g_rounds_x100 / 100 per CTA: with fewer, a CTA's tiles no longer overlap each other's load / MMA / epilogue phases)
-  static int g_rounds_x100 = -1;
-  if (g_rounds_x100 < 0) {
-    const char* e = getenv("MYOLO_G_ROUNDS_X100");
-    g_rounds_x100 = e ? atoi(e) : 200;
-  }
-  p.G = 1;
-  if (p.n_tiles_n == 1) {
-    for (int g = 4; g >= 2; g >>= 1)
-      if (g * p.BN <= kAccStride && (long)(p.total_tiles / g) * 100 >= (long)g_rounds_x100 * cta_budget) { p.G = g; break; }
-  }
-  p.total_rounds = ceil_div(p.total_tiles, p.G);
-  // vertical rounds: the G tiles of a round are G consecutive image rows, so G+2 strips feed 3*G (row, filter-row) pairs
-  static int vr_env = -1;
-  if (vr_env < 0) {
-    const char* e = getenv("MYOLO_VROUND");
-    vr_env = e ? atoi(e) : 1;
-  }
-  p.vround = (vr_env && p.strip && p.ws_mode && op.dil == 1 && p.G >= 2) ? 1 : 0;
-  if (p.vround) {
-    p.rounds_per_img = p.tiles_x * ceil_div(Ho, p.G);
-    p.total_rounds = p.B * p.rounds_per_img;
-  }
-  // pair mode (see ConvTcParams): for layers whose shared-memory fill is dominated by weight re-loads (one [BN x K] fetch per 128-pixel
-  // tile: FFM 3x3, the stride-2 3x3 convs, the P4 bottleneck 3x3s).  One CTA per SM; full waves of pair rounds, the remainder as single
-  // tiles so that the makespan in tile-times never grows
-  static int pair_env = -1;
-  if (pair_env < 0) {
-    const char* e = getenv("MYOLO_PAIR");
-    pair_env = e ? atoi(e) : 1;
-  }
-  p.m_tiles = p.B * p.tiles_x * p.tiles_y;
-  p.pair = 0;
-  p.n_pair_rounds = 0;
-  p.m_done = 0;
-  p.acc_stride = kAccStride;
-  p.tmem_cols = kTmemCols;
-  {
-    const long a_tile = p.strip ? 3L * p.cblocks * (p.tw + 2 * op.dil) * p.kc * 2 : (long)p.n_chunks * kTileM * p.kc * 2;
-    const long b_tile = (long)p.n_chunks * p.BN * p.kc * 2;
-    const int pairs_total = (p.m_tiles / 2) * p.n_tiles_n;
-    // measured per layer on B200 (bench.py --profile-ops, MYOLO_PAIR=0/1): wins where the weight tile is big - N tile 128 and K >= 1024 or
-    // stride 2 (L3/L5/L7/L18 -2..-4 us each, FFM 3x3 -8 us, SPP.cv2 -1.6 us); loses 1-3 us on 64-channel 3x3 strips and K <= 512 1x1 convs,
-    // whose two co-resident CTAs hide each other's epilogue better than one CTA with a pair does
-    const long k_total = (long)p.n_chunks * p.kc;
-    const bool legal = !p.ws_mode && p.G == 1 && !p.vround && p.out_mode == 0 && p.m_tiles % 2 == 0 && pairs_total >= 2;
-    const bool wins = p.BN == 128 && (k_total >= 1024 || op.stride == 2) && 2 * b_tile >= a_tile && pairs_total * 100 >= 80 * num_sms;
-    if (legal && ((pair_env && wins) || pair_env == 2 || g_conv_tc_force_pair)) {
-      p.pair = 1;
-      const int grid = std::min(pairs_total, num_sms);
-      const int tail_pairs = pairs_total % grid;
-      int npr = pairs_total;                                     // all pairs ...
-      if (tail_pairs > 0 && 2 * tail_pairs <= grid)              // ... unless the last partial wave is cheaper as single tiles (one wave)
-        npr = ((pairs_total - tail_pairs) / p.n_tiles_n) * p.n_tiles_n;
-      p.n_pair_rounds = npr;
-      p.m_done = 2 * (npr / p.n_tiles_n);
-      p.total_rounds = npr + (p.m_tiles - p.m_done) * p.n_tiles_n;
-      if (2 * p.BN > kAccStride) { p.acc_stride = 256; p.tmem_cols = 512; }
-    }
-  }
-  static int spin_ns = -1;
-  if (spin_ns < 0) {
-    const char* e = getenv("MYOLO_SPIN_NS");
-    spin_ns = e ? atoi(e) : 0;
-  }
-  p.spin_ns = spin_ns;
   p.fd_ntn = make_fastdiv((unsigned)p.n_tiles_n);
   p.fd_tpi = make_fastdiv((unsigned)(p.tiles_x * p.tiles_y));
   p.fd_tx = make_fastdiv((unsigned)p.tiles_x);
-  p.fd_rpi = make_fastdiv((unsigned)std::max(1, p.rounds_per_img));
-  // epilogue work split between the two warps of a TMEM lane quarter
-  const int nchunk16 = p.BN / 16;
-  if (p.G >= 2 || (p.pair && nchunk16 % 2 != 0)) { p.ep_split_cols = 0; p.ep_cols = p.BN; }
-  else if (nchunk16 % 2 == 0) { p.ep_split_cols = 1; p.ep_cols = p.BN / 2; }
-  else { p.ep_split_cols = 0; p.ep_cols = p.BN; }
-  p.ow = p.ep_cols % 64 == 0 ? 64 : (p.ep_cols % 32 == 0 ? 32 : 16);
-  p.log2_ow = ilog2(p.ow);
-  p.n_sub = p.out_mode == 0 ? p.ep_cols / p.ow : 0;
-  p.rows_w = p.tw < 32 ? p.tw : 32;
-  p.rows_h = 32 / p.rows_w;
-  // stage geometry
-  if (p.strip) {
-    p.a_stage_bytes = (int)align_up((p.tw + 2 * op.dil) * p.kc * 2, 1024);
-    p.b_stage_bytes = p.ws_mode ? 0 : (int)align_up(3 * p.BN * p.kc * 2, 1024);
-    p.n_kstages = 3 * p.cblocks;
-  } else {
-    p.a_stage_bytes = kTileM * kKStage * 2;
-    p.b_stage_bytes = p.ws_mode ? 0 : (int)align_up(p.BN * kKStage * 2, 1024);
-  }
-  if (p.pair) p.a_stage_bytes *= 2;        // [tile 0 | tile 1] halves, one weight block
-  // shared memory budget: two co-resident CTAs per SM (<= 112 KB each, their epilogues / TMA latencies overlap) for multi-wave layers;
-  // ONE CTA per SM with a deep operand ring when the layer has at most `one_cta_x100`/100 rounds per SM (P4/P5 maps: the pipeline depth,
-  // i.e. bytes in flight per SM, is what bounds those launches) or when two CTAs would leave fewer than 2 stages
+  // stage geometry: one CTA per SM with as deep an operand ring as shared memory allows
+  p.a_stage_bytes = kTileM * kKStage * 2;
+  p.b_stage_bytes = (int)align_up(p.BN * kKStage * 2, 1024);
   const int stage_bytes = p.a_stage_bytes + p.b_stage_bytes;
-  const int stg1 = kEpiWarps * p.n_sub * 32 * p.ow * 2;     // one staging buffer for each of the 8 warps
   const int misc = 1024 /*barriers*/ + kBiasBytes + 1024 /*alignment slack*/;
-  static int one_cta_x100 = -1;
-  if (one_cta_x100 < 0) {
-    const char* e = getenv("MYOLO_ONE_CTA_X100");
-    one_cta_x100 = e ? atoi(e) : 100;
-  }
-  int ctas_per_sm = (ws_big || p.pair || (long)p.total_rounds * 100 <= (long)one_cta_x100 * num_sms) ? 1 : 2;
-  int S = 0;
-  if (ctas_per_sm == 2) {
-    p.n_stg = p.out_mode == 0 ? 2 : 0;
-    S = (kSmemPerCta - p.b_res_bytes - p.n_stg * stg1 - misc) / stage_bytes;
-    if (S < 3 && p.n_stg == 2) {
-      p.n_stg = 1;
-      S = (kSmemPerCta - p.b_res_bytes - p.n_stg * stg1 - misc) / stage_bytes;
-    }
-    if (S < 2) ctas_per_sm = 1;
-  }
-  if (ctas_per_sm == 1) {
-    // a CTA that runs a single round in which every epilogue warp stores at most one tile never reuses its staging buffer
-    const bool single_use = !p.pair && p.total_rounds <= num_sms && (p.G == 1 || (p.G == 2 && !p.ep_split_cols));
-    p.n_stg = p.out_mode == 0 ? (single_use ? 1 : 2) : 0;
-    S = (220 * 1024 - p.b_res_bytes - p.n_stg * stg1 - misc) / stage_bytes;
-    if (p.pair && S < 3 && p.n_stg == 2) {          // operand stages before a second staging buffer
-      p.n_stg = 1;
-      S = (220 * 1024 - p.b_res_bytes - p.n_stg * stg1 - misc) / stage_bytes;
-    }
-  }
-  if (S > 8) S = 8;
+  int S = (kSmemBudget - misc) / stage_bytes;
+  if (S > kMaxStages) S = kMaxStages;
   MYOLO_REQUIRE(S >= 2, "conv_tc: not enough shared memory for 2 stages");
   MYOLO_REQUIRE(p.n_tiles_n * p.BN * 4 <= kBiasBytes, "conv_tc: %d output channels exceed the shared-memory bias buffer", p.n_tiles_n * p.BN);
   p.num_stages = S;
-  op.smem = S * stage_bytes + p.b_res_bytes + p.n_stg * stg1 + misc;
-  const int cta_cap = num_sms * ctas_per_sm;
-  op.grid = p.total_rounds < cta_cap ? p.total_rounds : cta_cap;
+  op.smem = S * stage_bytes + misc;
+  op.grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
 
   // ---- tensor maps ----
   const int esz = 2;
@@ -996,7 +366,7 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
   if (op.stride == 1) {
     uint64_t dims[4] = {(uint64_t)in.C, (uint64_t)in.W, (uint64_t)in.H, (uint64_t)in.B};
     uint64_t str[3] = {(uint64_t)in.ctot * esz, (uint64_t)in.W * in.ctot * esz, (uint64_t)in.H * in.W * in.ctot * esz};
-    uint32_t box[4] = {(uint32_t)p.kc, (uint32_t)(p.strip ? p.tw + 2 * op.dil : p.tw), (uint32_t)p.th, 1};
+    uint32_t box[4] = {(uint32_t)p.kc, (uint32_t)p.tw, (uint32_t)p.th, 1};
     int rc = encode_map(&op.tmA[0], 4, in.base, dims, str, box, sw);
     if (rc) return rc;
     op.tmA[1] = op.tmA[2] = op.tmA[3] = op.tmA[0];
@@ -1020,41 +390,37 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
     int rc = encode_map(&op.tmB, 2, const_cast<__half*>(op.w), dims, str, box, sw);
     if (rc) return rc;
   }
-  if (p.out_mode == 0) {
-    const TensorView& o = op.out;
-    uint64_t dims[4] = {(uint64_t)o.C, (uint64_t)o.W, (uint64_t)o.H, (uint64_t)o.B};
-    uint64_t str[3] = {(uint64_t)o.ctot * esz, (uint64_t)o.W * o.ctot * esz, (uint64_t)o.H * o.W * o.ctot * esz};
-    uint32_t box[4] = {(uint32_t)p.ow, (uint32_t)p.rows_w, (uint32_t)p.rows_h, 1};
-    int rc = encode_map(&op.tmO, 4, o.base, dims, str, box, p.ow * 2);
-    if (rc) return rc;
-  } else {
-    op.tmO = op.tmB;
-  }
-  static int null_env = -1;
-  if (null_env < 0) {
-    const char* e = getenv("MYOLO_CONV_NULL");       // measurement aid: every conv launch runs prologue + teardown only (launch floor)
-    null_env = (e && e[0] == '1') ? 1 : 0;
-  }
-  if (null_env) { p.total_rounds = 0; p.ws_mode = 0; }
-  static bool attr_set = false;
-  if (!attr_set) {
-    MYOLO_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    MYOLO_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    MYOLO_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<1, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    MYOLO_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<1, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    MYOLO_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<2, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    MYOLO_CHECK_CUDA(cudaFuncSetAttribute(conv_tc_kernel<2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
   return 0;
 }
 
-int conv_tc_launch(const ConvOp& op, cudaStream_t stream) {
-  static int use_pdl = -1;
-  if (use_pdl < 0) {
-    const char* e = getenv("MYOLO_NO_PDL");
-    use_pdl = (e && e[0] == '1') ? 0 : 1;
+template <int BN, bool RES>
+static cudaError_t launch_bn(const ConvOp& op, const cudaLaunchConfig_t& cfg) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
+    if (e != cudaSuccess) return e;
+    attr_set = true;
   }
+  return cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, RES>, op.tmA[0], op.tmA[1], op.tmA[2], op.tmA[3], op.tmB, op.p);
+}
+
+template <bool RES>
+static cudaError_t launch_res(const ConvOp& op, const cudaLaunchConfig_t& cfg) {
+  switch (op.p.BN) {
+    case 16: return launch_bn<16, RES>(op, cfg);
+    case 32: return launch_bn<32, RES>(op, cfg);
+    case 48: return launch_bn<48, RES>(op, cfg);
+    case 64: return launch_bn<64, RES>(op, cfg);
+    case 80: return launch_bn<80, RES>(op, cfg);
+    case 96: return launch_bn<96, RES>(op, cfg);
+    case 112: return launch_bn<112, RES>(op, cfg);
+    case 128: return launch_bn<128, RES>(op, cfg);
+  }
+  return cudaErrorInvalidValue;
+}
+
+int conv_tc_launch(const ConvOp& op, cudaStream_t stream) {
+  MYOLO_REQUIRE(op.p.BN % 16 == 0 && op.p.BN >= 16 && op.p.BN <= 128, "conv_tc: unsupported N tile %d", op.p.BN);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(op.grid);
   cfg.blockDim = dim3(kNumThreads);
@@ -1064,12 +430,8 @@ int conv_tc_launch(const ConvOp& op, cudaStream_t stream) {
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = use_pdl ? 1 : 0;
-  const bool res = op.p.residual != nullptr;
-  auto kern = op.p.vround ? (res ? conv_tc_kernel<2, true> : conv_tc_kernel<2, false>)
-              : op.p.strip ? (res ? conv_tc_kernel<1, true> : conv_tc_kernel<1, false>)
-                           : (res ? conv_tc_kernel<0, true> : conv_tc_kernel<0, false>);
-  MYOLO_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, op.tmA[0], op.tmA[1], op.tmA[2], op.tmA[3], op.tmB, op.tmO, op.p));
+  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  MYOLO_CHECK_CUDA(op.p.residual != nullptr ? launch_res<true>(op, cfg) : launch_res<false>(op, cfg));
   g_launch_count++;
   return 0;
 }

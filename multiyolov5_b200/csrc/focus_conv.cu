@@ -1,7 +1,7 @@
 // Layer 0 of the network in ONE kernel: Focus space-to-depth (reference models/common.py:549-550) + 3x3 Conv(12 -> Co) with folded BN +
 // SiLU, straight from the caller's NCHW image (fp32 / fp16 / uint8 scaled by 1/255 like detect.py:137) to the NHWC fp16 activation.
 //
-// Why not the tcgen05 kernel: with only 12 input channels an implicit-GEMM row is 32 bytes, and TMA issues one request per row -
+// Why not the wgmma kernel: with only 12 input channels an implicit-GEMM row is 32 bytes, and TMA issues one request per row -
 // the layer ends up bound by the TMA row rate, 4x above its HBM roofline (profiles/README.md).  Here a CTA converts the raw halo
 // (20 x 132 x 3 pixels for an 8 x 64 output tile) ONCE into a space-to-depth fp16 tile in shared memory and feeds legacy
 // mma.sync.m16n8k16 (K = 9 taps x 16 padded channels) from it with ldmatrix; the layer is memory bound (14.5 GFLOP vs 201 MB per

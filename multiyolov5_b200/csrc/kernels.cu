@@ -5,7 +5,7 @@
 
 namespace myolo {
 
-static inline int grid_for(long items, int block, int max_blocks = 148 * 32) {
+static inline int grid_for(long items, int block, int max_blocks = 132 * 32) {
   long b = (items + block - 1) / block;
   if (b > max_blocks) b = max_blocks;
   if (b < 1) b = 1;
@@ -832,9 +832,9 @@ extern "C" int myolo_seg_upsample_argmax(const void* logits, int dtype, int B, i
   MYOLO_REQUIRE((dtype == MYOLO_F32 || dtype == MYOLO_F16) && (out_dtype == MYOLO_I64 || out_dtype == MYOLO_U8),
                 "seg_upsample_argmax: unsupported dtype");
   cudaStream_t s = (cudaStream_t)stream;
-  const int g = grid_for((long)B * H * W, 256, 148 * 64);
+  const int g = grid_for((long)B * H * W, 256, 132 * 64);
   if (dtype == MYOLO_F32 && H == h && W == w && ((long)H * W) % 4 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0) {
-    const int g4 = grid_for((long)B * H * W / 4, 256, 148 * 32);
+    const int g4 = grid_for((long)B * H * W / 4, 256, 132 * 32);
     if (out_dtype == MYOLO_I64) argmax_nchw_f32x4_kernel<int64_t><<<g4, 256, 0, s>>>((const float*)logits, B, C, (long)H * W, (int64_t*)out);
     else argmax_nchw_f32x4_kernel<uint8_t><<<g4, 256, 0, s>>>((const float*)logits, B, C, (long)H * W, (uint8_t*)out);
     MYOLO_LAUNCH_CHECK();
@@ -842,14 +842,14 @@ extern "C" int myolo_seg_upsample_argmax(const void* logits, int dtype, int B, i
   }
   if (dtype == MYOLO_F16 && H == h && W == w && ((long)H * W) % 16 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0 &&
       (reinterpret_cast<uintptr_t>(out) & 15) == 0 && C <= 255) {
-    const int g16 = grid_for((long)B * H * W / 16, 256, 148 * 32);
+    const int g16 = grid_for((long)B * H * W / 16, 256, 132 * 32);
     if (out_dtype == MYOLO_I64) argmax_nchw_f16x16_kernel<int64_t><<<g16, 256, 0, s>>>((const __half*)logits, B, C, (long)H * W, (int64_t*)out);
     else argmax_nchw_f16x16_kernel<uint8_t><<<g16, 256, 0, s>>>((const __half*)logits, B, C, (long)H * W, (uint8_t*)out);
     MYOLO_LAUNCH_CHECK();
     return 0;
   }
   if (dtype == MYOLO_F16 && H == h && W == w && ((long)H * W) % 8 == 0 && (reinterpret_cast<uintptr_t>(logits) & 15) == 0) {
-    const int g8 = grid_for((long)B * H * W / 8, 256, 148 * 32);
+    const int g8 = grid_for((long)B * H * W / 8, 256, 132 * 32);
     if (out_dtype == MYOLO_I64) argmax_nchw_f16x8_kernel<int64_t><<<g8, 256, 0, s>>>((const __half*)logits, B, C, (long)H * W, (int64_t*)out);
     else argmax_nchw_f16x8_kernel<uint8_t><<<g8, 256, 0, s>>>((const __half*)logits, B, C, (long)H * W, (uint8_t*)out);
     MYOLO_LAUNCH_CHECK();
@@ -868,7 +868,7 @@ extern "C" int myolo_seg_upsample_argmax(const void* logits, int dtype, int B, i
 
 extern "C" int myolo_bilinear_nchw(const float* src, int B, int C, int h, int w, int H, int W, float* dst, void* stream) {
   MYOLO_REQUIRE(src && dst && B > 0 && C > 0, "bilinear_nchw: bad arguments");
-  bilinear_nchw_kernel<<<grid_for((long)B * C * H * W, 256, 148 * 64), 256, 0, (cudaStream_t)stream>>>(src, B, C, h, w, H, W, dst);
+  bilinear_nchw_kernel<<<grid_for((long)B * C * H * W, 256, 132 * 64), 256, 0, (cudaStream_t)stream>>>(src, B, C, h, w, H, W, dst);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }

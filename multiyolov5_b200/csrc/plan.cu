@@ -48,8 +48,8 @@ static int check_device(int* sms) {
     set_error("cudaGetDeviceProperties: %s", cudaGetErrorString(e));
     return MYOLO_E_NODEVICE;
   }
-  if (prop.major != 10) {
-    set_error("libmyolo_sm100a needs an sm_100 (Blackwell B200) device, found sm_%d%d (%s); there is no fallback path", prop.major,
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("libmyolo_sm90a needs an sm_90 (Hopper H100) device, found sm_%d%d (%s); there is no fallback path", prop.major,
               prop.minor, prop.name);
     return MYOLO_E_NODEVICE;
   }
@@ -71,7 +71,7 @@ struct WeightSlot {
   float* d_bias = nullptr;
   __half* w_dgrad = nullptr;         // flipped / transposed fp16 pack for the data gradient
   float* zero_bias = nullptr;
-  float* dw_packed = nullptr;        // fp32 [co][k*k][ci] accumulation buffer of the tcgen05 weight-gradient kernel
+  float* dw_packed = nullptr;        // fp32 [co][k*k][ci] accumulation buffer of the wgmma weight-gradient kernel
   bool dgrad_valid = false;          // w_dgrad matches the current master weights
   int dgrad_n_pad = 0, dgrad_cpad = 0;
 };
@@ -81,7 +81,7 @@ struct WeightSlot {
 using namespace myolo;
 
 struct myolo_plan {
-  int B = 0, H = 0, W = 0, num_sms = 148;
+  int B = 0, H = 0, W = 0, num_sms = 132;
   std::vector<myolo_op> ops;
   std::vector<myolo_buf_desc> bufs;
   std::vector<int32_t> extra;
@@ -257,7 +257,7 @@ extern "C" void myolo_plan_destroy(myolo_plan* pl) {
 }
 
 static int conv_n_pad(int co) {
-  // Co_pad must cover n_tiles_n * BN of the tcgen05 kernel (see conv_tc_prepare) and stay a multiple of 16 for the simt kernel
+  // Co_pad must cover n_tiles_n * BN of the wgmma kernel (see conv_tc_prepare) and stay a multiple of 16 for the simt kernel
   const int co16 = (int)align_up(co, 16);
   if (co16 <= 128) return co16;
   for (int bn = 128; bn >= 16; bn -= 16)
@@ -567,10 +567,9 @@ static int build_graph(myolo_plan* pl) {
     const char* e = getenv("MYOLO_LANES");
     nl_env = e ? std::max(4, std::min(16, atoi(e))) : 4;      // >= 4: the captured backward uses lanes 0-3
   }
-  // forward graphs: ONE lane by default.  Measured on B200 (CUPTI, tools/kernel_trace.py): every conv launch fills the machine, so branch
-  // concurrency buys nothing, while a multi-lane capture makes the graph runtime spread the nodes over ~70 internal streams - every edge
-  // becomes a cross-stream dependency (~5.5 us node to node instead of ~3.5 us), the programmatic-dependent-launch edges between
-  // consecutive convs are lost and the graph launch itself takes ~100 us instead of ~10.  MYOLO_FWD_LANES > 1 restores the branch lanes.
+  // forward graphs: ONE lane by default.  Every conv launch fills the machine, so branch concurrency buys little, while a multi-lane
+  // capture makes the graph runtime spread the nodes over many internal streams - every edge becomes a cross-stream dependency and the
+  // programmatic-dependent-launch edges between consecutive convs are lost.  MYOLO_FWD_LANES > 1 restores the branch lanes.
   static int fwd_lanes = -1;
   if (fwd_lanes < 0) {
     const char* e = getenv("MYOLO_FWD_LANES");
@@ -746,8 +745,8 @@ extern "C" int myolo_plan_profile(myolo_plan* pl, const void* x, int x_dtype, fl
 extern "C" int64_t myolo_plan_last_launch_count(const myolo_plan* pl) { return pl ? pl->last_launches : 0; }
 
 // which kernel a conv op of the plan takes and how it is tiled (valid after the first forward): info[0..11] =
-// {1 tcgen05 / 0 CUDA-core, grid, dynamic smem bytes, BN, pipeline stages, mode (0 taps, 1 strip, 2 vertical rounds), weights-stationary,
-//  G, total tiles, n tiles in N, kc, CTAs per SM}
+// {1 wgmma / 0 CUDA-core, grid, dynamic smem bytes, BN, pipeline stages, mode (always 0: one TMA box per tap), weights-stationary (always 0),
+//  tiles per accumulator round (always 1), total tiles, n tiles in N, kc, CTAs per SM (always 1)}
 extern "C" int myolo_plan_conv_info(myolo_plan* pl, int op_index, int32_t* info) {
   MYOLO_REQUIRE(pl && info && op_index >= 0 && op_index < (int)pl->ops.size(), "conv_info: bad arguments");
   MYOLO_REQUIRE(pl->ops[op_index].kind == MYOLO_OP_CONV, "conv_info: op %d is not a conv", op_index);
@@ -757,9 +756,9 @@ extern "C" int myolo_plan_conv_info(myolo_plan* pl, int op_index, int32_t* info)
   for (int i = 0; i < 12; ++i) info[i] = 0;
   info[0] = c.use_tc ? 1 : 0;
   if (c.use_tc) {
-    info[1] = c.grid; info[2] = c.smem; info[3] = c.p.BN; info[4] = c.p.num_stages; info[5] = c.p.vround ? 2 : (c.p.strip ? 1 : 0);
-    info[6] = c.p.ws_mode; info[7] = c.p.G; info[8] = c.p.total_tiles; info[9] = c.p.n_tiles_n; info[10] = c.p.kc;
-    info[11] = c.smem > 113 * 1024 ? 1 : 2;
+    info[1] = c.grid; info[2] = c.smem; info[3] = c.p.BN; info[4] = c.p.num_stages; info[5] = 0;
+    info[6] = 0; info[7] = 1; info[8] = c.p.total_tiles; info[9] = c.p.n_tiles_n; info[10] = c.p.kc;
+    info[11] = 1;
   }
   return 0;
 }
@@ -1173,8 +1172,8 @@ static int backward_walk(myolo_plan* pl, std::vector<char>& live, cudaStream_t s
   static int ml_env = -1;
   if (ml_env < 0) {
     const char* e = getenv("MYOLO_BWD_LANES");
-    ml_env = e ? atoi(e) : 0;     // measured on B200: the three-lane chain costs 2.7 ms per step (14.6 -> 11.9 ms): like the forward graph, a
-                                  // multi-lane capture is spread over dozens of internal streams and every edge becomes a cross-stream wait
+    ml_env = e ? atoi(e) : 0;     // like the forward graph, a multi-lane capture is spread over dozens of internal streams and every edge
+                                  // becomes a cross-stream wait
   }
   cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
   cudaStreamIsCapturing(s, &cap);
@@ -1364,7 +1363,7 @@ extern "C" int myolo_conv_wgrad(const void* x, const void* dy, int B, int H, int
   TensorView dv{const_cast<void*>(dy), B, Ho, Wo, co, co, MYOLO_F16};
   cudaStream_t s = (cudaStream_t)stream;
   if (path == 0) return launch_conv_wgrad(xv, dv, k, stride, dil, dW, co, ci, nullptr, s);
-  MYOLO_REQUIRE(conv_wgrad_tc_eligible(xv, dv, k, stride, dil, co, ci), "conv_wgrad: geometry not supported by the tcgen05 kernel");
+  MYOLO_REQUIRE(conv_wgrad_tc_eligible(xv, dv, k, stride, dil, co, ci), "conv_wgrad: geometry not supported by the wgmma kernel");
   float* packed = nullptr;
   const size_t nb = conv_wgrad_packed_bytes(dW, co, ci, k);
   if (nb) {
@@ -1455,41 +1454,13 @@ extern "C" int myolo_conv_bn_silu(const void* x, int B, int H, int W, int ci, co
   if (!rc) {
     const bool elig = conv_tc_eligible(c);
     if ((path == 1 || path == 3) && !elig) {
-      set_error("conv_bn_silu: shape not eligible for the tcgen05 path");
+      set_error("conv_bn_silu: shape not eligible for the tensor-core path");
       rc = MYOLO_E_INVALID;
     } else if (path == 2 || (path == 0 && !elig)) {
       rc = conv_simt_launch(c, s);
     } else {
-      g_conv_tc_force_pair = path == 3;
       rc = conv_tc_prepare(c, sms);
-      g_conv_tc_force_pair = 0;
-      const char* tl = getenv("MYOLO_CONV_TIMELINE");
-      long long* dbg = nullptr;
-      if (!rc && tl && tl[0] == '1') {
-        cudaMalloc(&dbg, 64 * 16 * sizeof(long long));
-        cudaMemset(dbg, 0, 64 * 16 * sizeof(long long));
-        c.p.dbg = dbg;
-        conv_tc_launch(c, s);   // warm (tensor maps, L2)
-        cudaStreamSynchronize(s);
-        cudaMemset(dbg, 0, 64 * 16 * sizeof(long long));
-      }
       if (!rc) rc = conv_tc_launch(c, s);
-      if (dbg) {
-        cudaStreamSynchronize(s);
-        std::vector<long long> h(64 * 16);
-        cudaMemcpy(h.data(), dbg, h.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-        const long long t0 = h[11] ? h[11] : h[0];
-        printf("# prologue: entry 0 | setup done %lld | dependency wait done %lld | teardown %lld   (cycles since kernel entry of CTA0)\n", h[12] - t0, h[13] - t0, h[14] - t0);
-        printf("# conv timeline CTA0: grid %d tiles %d BN %d kc %d kstages %d S %d ws %d n_stg %d smem %d\n", c.grid, c.p.total_tiles, c.p.BN, c.p.kc,
-               c.p.n_kstages, c.p.num_stages, c.p.ws_mode, c.p.n_stg, c.smem);
-        printf("# it: P_begin P_issued | M_begin M_tempty M_full0 M_commit | E_begin E_tfull E_stgready E_done E_store   (cycles since first stamp)\n");
-        for (int it = 0; it < 64 && h[it * 16] != 0; ++it) {
-          printf("%2d:", it);
-          for (int k = 0; k <= 10; ++k) printf(" %7lld", h[it * 16 + k] ? h[it * 16 + k] - t0 : -1);
-          printf("\n");
-        }
-        cudaFree(dbg);
-      }
     }
   }
   cudaError_t e = cudaStreamSynchronize(s);

@@ -102,7 +102,7 @@ int launch_letterbox(const unsigned char* src, int B, int H0, int W0, int rw, in
   p.out_dtype = out_dtype; p.chw = chw; p.swap_rb = swap_rb;
   for (int c = 0; c < 3; ++c) p.pad[c] = pad3 ? pad3[c] : 114;
   const long total = (long)B * H * W;
-  letterbox_kernel<<<(int)std::min<long>(148L * 16, (total + 255) / 256), 256, 0, s>>>(p);
+  letterbox_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(p);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }

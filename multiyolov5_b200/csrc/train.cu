@@ -1,4 +1,4 @@
-// Training-mode kernels (see train.h).  Correct-first implementations: the data gradients of all convolutions reuse the tcgen05
+// Training-mode kernels (see train.h).  Correct-first implementations: the data gradients of all convolutions reuse the wgmma
 // implicit-GEMM kernel (a conv of dY with flipped/transposed weights); weight gradients run on legacy mma.sync with split-K
 // atomics; everything else is plain coalesced CUDA.  Reference semantics: torch.autograd through models/common.py / models/yolo.py
 // in train mode (BatchNorm with batch statistics, eps 1e-3, momentum 0.03: reference utils/torch_utils.py:150-152).
@@ -8,7 +8,7 @@
 
 namespace myolo {
 
-static inline int grid_for_t(long items, int block, int max_blocks = 148 * 32) {
+static inline int grid_for_t(long items, int block, int max_blocks = 132 * 32) {
   long b = (items + block - 1) / block;
   if (b > max_blocks) b = max_blocks;
   if (b < 1) b = 1;
@@ -172,7 +172,7 @@ __global__ void __launch_bounds__(256) chan_reduce_v_kernel(TensorView a, Tensor
 }
 static inline int reduce_v_grid(long npix, int C) {
   const int lanes = 256 / (C / 8);
-  return (int)std::max<long>(1, std::min<long>(148 * 2, npix / ((long)lanes * 4)));
+  return (int)std::max<long>(1, std::min<long>(132 * 2, npix / ((long)lanes * 4)));
 }
 
 __global__ void bn_finalize_kernel(float* sums, float* stats, BnParams bn, long npix) {
@@ -864,7 +864,7 @@ int launch_seg_ce_fused(const TensorView& lo, int n_cls, const long long* labels
   float* loss_sum = reinterpret_cast<float*>(n_valid + 1);
   MYOLO_CHECK_CUDA(cudaMemsetAsync(scratch16, 0, 16, s));
   const long n = (long)lo.B * H * W;
-  count_valid_kernel<<<grid_for_t(n, 256, 148 * 8), 256, 0, s>>>(labels, n, ignore_index, n_cls, n_valid);
+  count_valid_kernel<<<grid_for_t(n, 256, 132 * 8), 256, 0, s>>>(labels, n, ignore_index, n_cls, n_valid);
   MYOLO_LAUNCH_CHECK();
   const int rsplit = 4;
   const int g1 = grid_for_t(n, 128), g2 = grid_for_t((long)lo.B * lo.H * lo.W * rsplit, 128);
@@ -1074,7 +1074,7 @@ int launch_conv_wgrad(const TensorView& x, const TensorView& dy, int k, int stri
   const long npix = (long)dy.B * dy.H * dy.W;
   const int tiles = ceil_div(co, 64) * ceil_div(ci, 64) * k * k;
   long chunks = (npix + 31) / 32;
-  int splits = (int)std::min<long>(chunks, std::max<long>(1, (148L * 8) / tiles));
+  int splits = (int)std::min<long>(chunks, std::max<long>(1, (132L * 8) / tiles));
   dim3 grid(ceil_div(co, 64), ceil_div(ci, 64) * k * k, splits);
   conv_wgrad_kernel<<<grid, 128, 0, s>>>(x, dy, k, stride, dil, dW, co, ci, splits);
   MYOLO_LAUNCH_CHECK();
@@ -1183,7 +1183,7 @@ __global__ void grads_check_finite_kernel(const float* __restrict__ g, long n, i
 int launch_grads_check_finite(const float* g, long n, int* found_inf, cudaStream_t s) {
   MYOLO_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "grads_check_finite: gradient buffer must be 16-byte aligned");
   MYOLO_CHECK_CUDA(cudaMemsetAsync(found_inf, 0, sizeof(int), s));
-  grads_check_finite_kernel<<<grid_for_t(std::max<long>(1, n / 4), 256, 148 * 8), 256, 0, s>>>(g, n, found_inf);
+  grads_check_finite_kernel<<<grid_for_t(std::max<long>(1, n / 4), 256, 132 * 8), 256, 0, s>>>(g, n, found_inf);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }
@@ -1211,7 +1211,7 @@ int launch_sgd_step(float* p, float* g, float* buf, const unsigned char* group, 
   MYOLO_REQUIRE(p && g && buf && group && n > 0 && n_groups >= 1 && n_groups <= 4, "sgd_step: bad arguments");
   SgdGroups gr{};
   for (int i = 0; i < n_groups; ++i) { gr.lr[i] = lr[i]; gr.wd[i] = wd[i]; }
-  sgd_step_kernel<<<grid_for_t(n, 256, 148 * 8), 256, 0, s>>>(p, g, buf, group, n, gr, momentum, nesterov, inv_scale, found_inf, zero_grad);
+  sgd_step_kernel<<<grid_for_t(n, 256, 132 * 8), 256, 0, s>>>(p, g, buf, group, n, gr, momentum, nesterov, inv_scale, found_inf, zero_grad);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }

@@ -81,7 +81,7 @@ int launch_bias_grad(const TensorView& dy, float* dbias, int co, cudaStream_t s)
 int launch_grads_check_finite(const float* g, long n, int* found_inf, cudaStream_t s);
 int launch_sgd_step(float* p, float* g, float* buf, const unsigned char* group, long n, const float* lr, const float* wd, int n_groups,
                     float momentum, int nesterov, const float* inv_scale, const int* found_inf, int zero_grad, cudaStream_t s);
-// tcgen05 weight gradient (wgrad_tc.cu): dw_packed is a zeroed fp32 [co][k*k][ci] accumulation buffer owned by the caller
+// wgmma weight gradient (wgrad_tc.cu): dw_packed is a zeroed fp32 [co][k*k][ci] accumulation buffer owned by the caller
 bool conv_wgrad_tc_eligible(const TensorView& x, const TensorView& dy, int k, int stride, int dil, int co, int ci);
 size_t conv_wgrad_packed_bytes(const float* dW, int co, int ci, int k);   // 0: accumulates straight into dW
 int launch_conv_wgrad_tc(const TensorView& x, const TensorView& dy, int k, int stride, int dil, float* dW, float* dw_packed, int co, int ci,

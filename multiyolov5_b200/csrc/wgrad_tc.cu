@@ -1,22 +1,23 @@
-// Convolution weight gradient on tcgen05 (sm_100a), training row a13 of SURVEY.md section 8:
+// Convolution weight gradient on the Hopper tensor cores (wgmma, sm_90a), training row a13 of SURVEY.md section 8:
 //
 //     dW[co][ky][kx][ci] += sum over output pixels p of dY[p][co] * X[in(p, ky, kx)][ci]
 //
 // As a GEMM: D (M = co, N = ci) accumulates over K = output pixels.  Both operands live in HBM as NHWC fp16, i.e. with the GEMM's
 // M / N dimension contiguous and K (pixels) strided: "MN-major" operands.  TMA loads [Kc pixels] x [64 channels] boxes (128-byte
-// rows, SWIZZLE_128B); the UMMA shared-memory descriptors describe exactly that layout (8-row x 128-byte swizzle atoms, SBO = 1024
-// bytes between 8-pixel groups, LBO = one box between 64-channel chunks) and the instruction descriptor marks A and B as MN-major.
+// rows, SWIZZLE_128B); the wgmma shared-memory descriptors describe exactly that layout (8-row x 128-byte swizzle atoms, SBO = 1024
+// bytes between 8-pixel groups, LBO = one box between 64-channel chunks) and the instruction marks A and B as transposed (MN-major).
 //
-// One CTA = (128 output channels) x (64 or 128 input channels) x (one filter row ky: k taps) x (a slab of output rows):
-//   warp 0      TMA producer: per pipeline stage one dY box set and k shifted X box sets (image border = TMA zero fill = padding;
-//               stride 2 through the four parity tensor maps, as in the forward kernel)
-//   warp 1      one thread issues k * Kc/16 tcgen05.mma per stage into k TMEM accumulators (k*N <= 384 columns)
-//   warps 2-5   epilogue: tcgen05.ld -> vector red.global.add into a [Co][k*k][Ci] fp32 buffer (coalesced along ci);
-//               `unpack` then adds that buffer into the caller's PyTorch-layout [Co][Ci][k][k] gradient and clears it.
+// One CTA = (128 output channels) x (N input channels) x (one filter row ky: k taps) x (a slab of output rows):
+//   warp 0             TMA producer: per pipeline stage one dY box set and k shifted X box sets (image border = TMA zero fill =
+//                      padding; stride 2 through the four parity tensor maps, as in the forward kernel)
+//   warpgroups 1 and 2 output channels [0, 64) and [64, 128) of the tile: k register accumulators of m64nNk16 wgmma (N <= 64 for 3x3
+//                      so that 3 x N/2 accumulator registers per thread fit), then vector red.global.add into a [Co][k*k][Ci] fp32
+//                      buffer; `unpack` adds that buffer into the caller's PyTorch-layout [Co][Ci][k][k] gradient and clears it.
 // Split-K over row slabs gives every SM work; partial sums meet in the fp32 reductions.
 #include <cuda.h>
 
 #include "train.h"
+#include "wgmma.cuh"
 
 namespace myolo {
 
@@ -29,28 +30,27 @@ struct WgradTcParams {
   int m_tiles, n_tiles, N, n_boxes;
   int bc, ci_pad, a_boxes;            // channels per X box (64 / 32 / 16 -> 128 / 64 / 32-byte swizzle); padded Ci of the packed buffer
   int num_stages, stage_bytes, a_bytes, b_bytes;
-  int tmem_cols;
   float* dw_packed;
 };
 
-static constexpr int kWgThreads = 192;
+static constexpr int kWgThreads = 384;
 
 // MN-major canonical layout: rows of `row_bytes` (128 / 64 / 32 = the swizzle width) per pixel, 8-pixel swizzle atoms
 __device__ __forceinline__ uint64_t mn_major_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t row_bytes) {
-  const uint64_t layout = row_bytes == 128 ? 2ull : (row_bytes == 64 ? 4ull : 6ull);
+  const uint64_t layout = row_bytes == 128 ? 1ull : (row_bytes == 64 ? 2ull : 3ull);
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);          // start address
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;  // leading byte offset: next channel chunk (one box)
   d |= (uint64_t)((8 * row_bytes) >> 4) << 32;       // stride byte offset: next group of 8 pixels
-  d |= (uint64_t)1 << 46;                            // descriptor version (Blackwell)
-  d |= layout << 61;                                 // swizzle mode
+  d |= layout << 62;                                 // swizzle mode
   return d;
 }
 
-__device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
-  asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b) {
+  asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
 }
 
+template <int N, int K>
 __global__ void __launch_bounds__(kWgThreads, 1)
 conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_constant__ CUtensorMap tmX0,
                      const __grid_constant__ CUtensorMap tmX1, const __grid_constant__ CUtensorMap tmX2,
@@ -60,42 +60,34 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)p.num_stages * p.stage_bytes);
   uint64_t* full = bars;
   uint64_t* empty = bars + p.num_stages;
-  uint64_t* acc_full = bars + 2 * p.num_stages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * p.num_stages + 1);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;   // warp-uniform for the compiler
   // work item
   int t = blockIdx.x;
-  const int ky = t % p.k; t /= p.k;
+  const int ky = t % K; t /= K;
   const int n_tile = t % p.n_tiles; t /= p.n_tiles;
   const int m_tile = t;
-  const int co0 = m_tile * 128, ci0 = n_tile * p.N;
+  const int co0 = m_tile * 128, ci0 = n_tile * N;
   const int row0 = blockIdx.y * p.rows_per_cta;
   const int row1 = min(p.rows_total, row0 + p.rows_per_cta);
   const int n_steps = (row1 - row0) * p.steps_per_row;
 
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");      // programmatic dependent launch: see common.cuh launch_pdl
   if (threadIdx.x == 0) {
-    for (int s = 0; s < p.num_stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(acc_full, 1);
+    for (int s = 0; s < p.num_stages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 2); }
     fence_mbar_init();
     tma_prefetch_desc(&tmDy);
     tma_prefetch_desc(&tmX0);
   }
-  if (warp == 1) tmem_alloc(tmem_slot, (uint32_t)p.tmem_cols);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   // dY, X and the packed accumulation buffer come from predecessor kernels: every thread waits (the epilogue's red.global.add must not
   // race a predecessor's unpack of the same buffer)
   asm volatile("griddepcontrol.wait;" ::: "memory");
 
-  // producer / MMA roles run warp-converged with one elected issuing lane (descriptor arithmetic stays in uniform registers; see conv_tc.cu)
   if (warp == 0) {
-    // ===================== TMA producer =====================
+    // ===================== TMA producer (warp-converged; one elected lane issues) =====================
     const bool leader = elect_one();
-    const int half = p.k / 2;
+    const int half = K / 2;
     int stage = 0;
     uint32_t phase = 0;
     for (int r = row0; r < row1; ++r) {
@@ -109,11 +101,11 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
         __syncwarp();
         uint8_t* sa = smem + (size_t)stage * p.stage_bytes;
         if (leader) {
-          mbar_arrive_expect_tx(&full[stage], (uint32_t)(p.a_boxes * p.Kc * 128 + p.k * p.b_bytes));
+          mbar_arrive_expect_tx(&full[stage], (uint32_t)(p.a_boxes * p.Kc * 128 + K * p.b_bytes));
           tma_load_4d(sa, &tmDy, &full[stage], co0, ox0, oy, b);
           if (p.a_boxes == 2) tma_load_4d(sa + p.Kc * 128, &tmDy, &full[stage], co0 + 64, ox0, oy, b);
         }
-        for (int kx = 0; kx < p.k; ++kx) {
+        for (int kx = 0; kx < K; ++kx) {
           uint8_t* sb = sa + p.a_bytes + kx * p.b_bytes;
           int ix0, px = 0;
           if (p.stride == 1) ix0 = ox0 + (kx - half) * p.dil;
@@ -126,64 +118,57 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
         if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    const bool leader = elect_one();
-    const uint32_t idesc = (1u << 4)                            // D: fp32
-                           | (0u << 7) | (0u << 10)             // A, B: fp16
-                           | (1u << 15) | (1u << 16)            // A, B MN-major (channels contiguous, pixels strided)
-                           | ((uint32_t)(p.N >> 3) << 17)       // N
-                           | ((uint32_t)(128 >> 4) << 24);      // M
-    int stage = 0;
-    uint32_t phase = 0;
-    const uint32_t lbo = (uint32_t)p.Kc * 128;
-    const uint32_t rb = (uint32_t)p.bc * 2, lbo_b = (uint32_t)p.Kc * rb;
-    const uint32_t jb = (16 * rb) >> 4;   // descriptor start-address step of B per 16 pixels
+  } else if (warp >= 4) {
+    // ===================== consumers: output channels [64 cw, 64 cw + 64) of the tile =====================
+    const int cw = (warp >> 2) - 1;
+    const bool active = cw < p.a_boxes;      // the second warpgroup has no rows when Co <= 64
+    const bool signaller = (threadIdx.x & 127) == 0;
+    float acc[K][N / 2];
+#pragma unroll
+    for (int kx = 0; kx < K; ++kx)
+#pragma unroll
+      for (int i = 0; i < N / 2; ++i) acc[kx][i] = 0.f;
+    const uint32_t lbo_b = (uint32_t)p.Kc * p.bc * 2, rb = (uint32_t)p.bc * 2;
     const int jn = p.Kc / 16;
+    int stage = 0, prev = -1;
+    uint32_t phase = 0;
     for (int s = 0; s < n_steps; ++s) {
       mbar_wait(&full[stage], phase);
-      __syncwarp();
-      tcgen05_fence_after();
-      const uint32_t sa = smem_u32(smem + (size_t)stage * p.stage_bytes);
-      const uint64_t da = mn_major_desc(sa, lbo, 128);
-      for (int kx = 0; kx < p.k; ++kx) {
-        const uint64_t db = mn_major_desc(sa + p.a_bytes + kx * p.b_bytes, lbo_b, rb);
-#pragma unroll 4
-        for (int j = 0; j < jn; ++j)   // 16 pixels per instruction = two 8-pixel groups = 2048 bytes
-          if (leader) umma_f16_ss(tmem_base + kx * p.N, da + (uint64_t)(j * 128), db + (uint64_t)(j * jb), idesc, (uint32_t)((s | j) != 0));
+      if (active) {
+        const uint32_t sa = smem_u32(smem + (size_t)stage * p.stage_bytes);
+        wgmma_fence();
+#pragma unroll
+        for (int kx = 0; kx < K; ++kx) {
+          wgmma_fence_regs(acc[kx]);
+          for (int j = 0; j < jn; ++j)      // 16 pixels per instruction = two 8-pixel groups
+            wgmma_f16<N, 1, 1>(acc[kx], mn_major_desc(sa + cw * p.Kc * 128 + j * 2048, (uint32_t)p.Kc * 128, 128),
+                               mn_major_desc(sa + p.a_bytes + kx * p.b_bytes + j * 16 * rb, lbo_b, rb), (uint32_t)((s | j) != 0));
+        }
+        wgmma_commit();
+        wgmma_wait<1>();                    // the previous stage's MMAs have retired
       }
-      if (leader) umma_commit(&empty[stage]);
+      if (prev >= 0 && signaller) mbar_arrive(&empty[prev]);
+      prev = stage;
       if (++stage == p.num_stages) { stage = 0; phase ^= 1; }
     }
-    if (leader) umma_commit(acc_full);
-  } else if (warp >= 2) {
-    // ===================== epilogue: TMEM -> fp32 reductions =====================
-    if (n_steps > 0) {
-      mbar_wait(acc_full, 0);
-      tcgen05_fence_after();
-      const int q = warp & 3;
-      const int co = co0 + q * 32 + lane;
-      const int taps = p.k * p.k;
-      for (int kx = 0; kx < p.k; ++kx) {
-        float* dst = p.dw_packed + ((size_t)co * taps + ky * p.k + kx) * p.ci_pad + ci0;
-        for (int c = 0; c < p.N; c += 16) {
-          uint32_t v[16];
-          tmem_ld_32x32b_x16(tmem_base + ((uint32_t)(q * 32) << 16) + kx * p.N + c, v);
-          tmem_ld_wait();
-          if (co < p.Co) {
+    wgmma_wait<0>();
+    if (prev >= 0 && signaller) mbar_arrive(&empty[prev]);
+    if (active && n_steps > 0) {
+      // fragment: row (co) 16*(warp%4) + lane/4 + 8h, columns (ci) 8j + 2*(lane%4) + {0,1} in acc[kx][4j + 2h + {0,1}]
+      const int taps = K * K;
 #pragma unroll
-            for (int i = 0; i < 16; i += 4)
-              red_add_v4(dst + c + i, __uint_as_float(v[i]), __uint_as_float(v[i + 1]), __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
-          }
+      for (int kx = 0; kx < K; ++kx) {
+        wgmma_fence_regs(acc[kx]);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int co = co0 + cw * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * h;
+          if (co >= p.Co) continue;
+          float* dst = p.dw_packed + ((size_t)co * taps + ky * K + kx) * p.ci_pad + ci0 + 2 * (lane & 3);
+#pragma unroll
+          for (int j = 0; j < N / 8; ++j) red_add_v2(dst + 8 * j, acc[kx][4 * j + 2 * h], acc[kx][4 * j + 2 * h + 1]);
         }
       }
     }
-  }
-  tcgen05_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, (uint32_t)p.tmem_cols);
   }
 }
 
@@ -199,6 +184,35 @@ __global__ void wgrad_unpack_kernel(float* __restrict__ packed, float* __restric
     packed[i] = 0.f;
     if (c < ci && v != 0.f) atomicAdd(dW + ((size_t)o * ci + c) * taps + t, v);   // both passes of a step may unpack concurrently
   }
+}
+
+template <int N, int K>
+static cudaError_t launch_nk(const WgradTcParams& p, dim3 grid, size_t smem, cudaStream_t s, const CUtensorMap& tmDy, const CUtensorMap* tmX) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_tc_kernel<N, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    attr_set = true;
+  }
+  return launch_pdl(conv_wgrad_tc_kernel<N, K>, grid, dim3(kWgThreads), smem, s, tmDy, tmX[0], tmX[1], tmX[2], tmX[3], p);
+}
+
+static cudaError_t launch_wgrad(const WgradTcParams& p, dim3 grid, size_t smem, cudaStream_t s, const CUtensorMap& tmDy, const CUtensorMap* tmX) {
+  if (p.k == 1) {
+    switch (p.N) {
+      case 16: return launch_nk<16, 1>(p, grid, smem, s, tmDy, tmX);
+      case 32: return launch_nk<32, 1>(p, grid, smem, s, tmDy, tmX);
+      case 64: return launch_nk<64, 1>(p, grid, smem, s, tmDy, tmX);
+      case 128: return launch_nk<128, 1>(p, grid, smem, s, tmDy, tmX);
+    }
+  } else {
+    switch (p.N) {
+      case 16: return launch_nk<16, 3>(p, grid, smem, s, tmDy, tmX);
+      case 32: return launch_nk<32, 3>(p, grid, smem, s, tmDy, tmX);
+      case 64: return launch_nk<64, 3>(p, grid, smem, s, tmDy, tmX);
+    }
+  }
+  return cudaErrorInvalidValue;
 }
 
 bool conv_wgrad_tc_eligible(const TensorView& x, const TensorView& dy, int k, int stride, int dil, int co, int ci) {
@@ -237,12 +251,12 @@ int launch_conv_wgrad_tc(const TensorView& x, const TensorView& dy, int k, int s
   p.B = dy.B; p.Ho = dy.H; p.Wo = dy.W; p.Co = co; p.Ci = ci; p.k = k; p.stride = stride; p.dil = dil;
   p.Kc = dy.W % 64 == 0 ? 64 : (dy.W % 32 == 0 ? 32 : 16);
   p.ci_pad = cp;
-  p.N = cp % 128 == 0 ? 128 : (cp % 64 == 0 ? 64 : cp);
+  p.N = cp % 128 == 0 && k == 1 ? 128 : (cp % 64 == 0 ? 64 : cp);   // 3x3: three register accumulators of N/2 floats per thread
   p.bc = p.N >= 64 ? 64 : p.N;
   p.n_boxes = p.N / p.bc;
   p.a_boxes = co > 64 ? 2 : 1;                          // the second 64-channel dY box is skipped when it would be all padding
   auto geom = [&]() {
-    p.a_bytes = 2 * p.Kc * 128;                         // (the MMA still addresses 128 rows; rows 64.. feed unused TMEM lanes)
+    p.a_bytes = 2 * p.Kc * 128;                         // room for both 64-channel dY boxes (the second is not loaded when Co <= 64)
     p.b_bytes = (int)align_up(p.n_boxes * p.Kc * p.bc * 2, 1024);
     p.stage_bytes = p.a_bytes + k * p.b_bytes;
   };
@@ -262,8 +276,6 @@ int launch_conv_wgrad_tc(const TensorView& x, const TensorView& dy, int k, int s
   slabs = std::min(slabs, std::max(1, p.rows_total / min_rows));
   p.rows_per_cta = ceil_div(p.rows_total, slabs);
   slabs = ceil_div(p.rows_total, p.rows_per_cta);
-  const int cols = k * p.N;
-  p.tmem_cols = cols <= 32 ? 32 : (cols <= 64 ? 64 : (cols <= 128 ? 128 : (cols <= 256 ? 256 : 512)));
   p.dw_packed = direct ? dW : dw_packed;
 
   CUtensorMap tmDy, tmX[4];
@@ -294,15 +306,10 @@ int launch_conv_wgrad_tc(const TensorView& x, const TensorView& dy, int k, int s
       }
   }
   const int smem = p.num_stages * p.stage_bytes + 1024 /*alignment*/ + 256 /*barriers*/;
-  static bool attr_set = false;
-  if (!attr_set) {
-    MYOLO_CHECK_CUDA(cudaFuncSetAttribute(conv_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    attr_set = true;
-  }
-  MYOLO_CHECK_CUDA(launch_pdl(conv_wgrad_tc_kernel, dim3(items, slabs), dim3(kWgThreads), (size_t)smem, s, tmDy, tmX[0], tmX[1], tmX[2], tmX[3], p));
+  MYOLO_CHECK_CUDA(launch_wgrad(p, dim3(items, slabs), (size_t)smem, s, tmDy, tmX));
   MYOLO_LAUNCH_CHECK();
   if (!direct) {
-    MYOLO_CHECK_CUDA(launch_pdl(wgrad_unpack_kernel, dim3(std::min(148 * 8, ceil_div(co * cp * k * k, 256))), dim3(256), 0, s, dw_packed, dW, co, ci,
+    MYOLO_CHECK_CUDA(launch_pdl(wgrad_unpack_kernel, dim3(std::min(num_sms * 8, ceil_div(co * cp * k * k, 256))), dim3(256), 0, s, dw_packed, dW, co, ci,
                                 cp, k * k));
     MYOLO_LAUNCH_CHECK();
   }

@@ -1,4 +1,4 @@
-"""Runtime glue between the nn.Module shells and libmyolo_sm100a.so: compiles one plan per input shape, uploads
+"""Runtime glue between the nn.Module shells and libmyolo_sm90a.so: compiles one plan per input shape, uploads
 (BN-folded, fp16-packed) weights, allocates caller-owned output tensors and launches the plan on the current stream."""
 import os
 import ctypes as C

@@ -2,7 +2,7 @@
 
 The classes keep the reference's constructor signatures and sub-module names so that `state_dict()` keys are
 identical (tests/golden/manifest_*.json) and reference checkpoints' tensors load unchanged.  They contain NO arithmetic:
-compute happens in the compiled layer plan (multiyolov5_b200/plan.py -> libmyolo_sm100a.so) driven by Model.forward.
+compute happens in the compiled layer plan (multiyolov5_b200/plan.py -> libmyolo_sm90a.so) driven by Model.forward.
 Calling a block's forward() directly raises - there is deliberately no eager PyTorch path.
 """
 import torch.nn as nn
@@ -11,7 +11,7 @@ import torch.nn as nn
 class _PlanOnly(nn.Module):
     def forward(self, *a, **k):
         raise RuntimeError(f"{type(self).__name__} holds parameters only; run it through models.yolo.Model.forward "
-                           "(compiled sm_100a plan). There is no eager PyTorch fallback.")
+                           "(compiled sm_90a plan). There is no eager PyTorch fallback.")
 
 
 def autopad(k, p=None):  # reference models/common.py:22-26

@@ -1,9 +1,9 @@
-"""`Model(cfg).forward` of the reference (reference models/yolo.py:233-370) on a compiled sm_100a layer plan.
+"""`Model(cfg).forward` of the reference (reference models/yolo.py:233-370) on a compiled sm_90a layer plan.
 
 Surface kept from the reference: Model(cfg='*.yaml' | dict, ch=3, nc=None, anchors=None), .forward(x) ->
 eval `[(z, [x0,x1,x2]), seg]`, .fuse(), .stride, .names, .yaml, .save, .model[-1] (Detect with nl/na/nc/no/anchors/
 anchor_grid/stride), state_dict() keys (tests/golden/manifest_*.json).  The seg heads and Detect are parameter shells like
-models/common.py; all arithmetic runs in libmyolo_sm100a.so.
+models/common.py; all arithmetic runs in libmyolo_sm90a.so.
 """
 import math
 import os

@@ -53,7 +53,7 @@ def allreduce_flat_grads(flat_grad: torch.Tensor, group=None, stream=None) -> in
             from . import _lib
             sp = stream.cuda_stream if stream is not None else _lib.stream_ptr()
             _lib.check(_lib.lib().myolo_allreduce_grads(_lib.ptr(flat_grad), flat_grad.numel(), comm, sp))
-            LAST_ALLREDUCE_PATH = "myolo_allreduce_grads (ncclAllReduce on torch's communicator, issued by libmyolo_sm100a)"
+            LAST_ALLREDUCE_PATH = "myolo_allreduce_grads (ncclAllReduce on torch's communicator, issued by libmyolo_sm90a)"
         else:
             dist.all_reduce(flat_grad, op=dist.ReduceOp.SUM, group=group)
             LAST_ALLREDUCE_PATH = f"torch.distributed.all_reduce ({dist.get_backend(group)})"

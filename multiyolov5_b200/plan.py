@@ -1,5 +1,5 @@
 """Host-side planner: lowers the module tree built by models.yolo.parse_model to the flat op list that
-libmyolo_sm100a.so replays (include/myolo.h `myolo_op`), i.e. the compiled form of Model.forward_once
+libmyolo_sm90a.so replays (include/myolo.h `myolo_op`), i.e. the compiled form of Model.forward_once
 (reference models/yolo.py:293-316).
 
 Design points
@@ -106,7 +106,7 @@ class _PairedConv:
     pairs j-1, j, j+1, so the restated conv is again 3x3 / stride 1 / pad 1 with
         W'[p_out*Co + co, p_in*16 + ci, ky, pt] = W[co, ci, ky, kx],  kx = 2*(pt-1) + p_in - p_out + 1  (zero where kx is outside 0..2).
     Same arithmetic (the extra products are exact zeros), but the implicit-GEMM kernel sees 64-byte instead of 32-byte pixel rows, half as
-    many of them, and N = 2 Co: the first layer is bound by the TMA's per-row cost (~4.4 clk per 32-byte row measured on B200)."""
+    many of them, and N = 2 Co: the first layer is bound by the TMA's per-row cost (one request per 32-byte row)."""
 
     def __init__(self, conv: nn.Conv2d):
         assert conv.kernel_size == (3, 3) and conv.stride == (1, 1) and conv.dilation == (1, 1) and conv.padding == (1, 1)
@@ -161,7 +161,7 @@ class PlanBuilder:
     def __init__(self, B: int, H: int, W: int, train: bool = False):
         self.B, self.H, self.W = B, H, W
         self.train = train                      # train mode: raw conv -> batch-stat BN + act ops, nothing in place, no aliasing
-        # cv1 and cv2 of a C3 read the same input: ONE launch with concatenated output channels (measured on B200: -70 us per forward)
+        # cv1 and cv2 of a C3 read the same input: ONE launch with concatenated output channels (one read of the input)
         self.fuse_c3 = os.environ.get("MYOLO_FUSE_C3", "1") == "1"
         self.bn_slots: List[nn.BatchNorm2d] = []
         self.bufs: List[Buf] = []
@@ -342,8 +342,8 @@ class PlanBuilder:
         import os
         if (conv.kernel_size == (3, 3) and conv.out_channels in (32, 48) and isinstance(m.conv.act, nn.SiLU)
                 and os.environ.get("MYOLO_FOCUS_FUSION") == "1" and not self.train):
-            # opt-in: whole layer in one kernel straight from the NCHW image (csrc/focus_conv.cu).  Measured on B200 it is still
-            # slower (190 us) than space-to-depth kernel + tcgen05 conv (26 + 108 us), so the two-kernel path stays the default.
+            # opt-in: whole layer in one kernel straight from the NCHW image (csrc/focus_conv.cu).  It has not been measured on
+            # H100 against the space-to-depth kernel + wgmma conv, so the two-kernel path stays the default.
             dst = dst or self.new_buf(self.H // 2, self.W // 2, conv.out_channels)
             slot = len(self.slots)
             self.slots.append(WeightSlot(conv, m.conv.bn, "focus"))

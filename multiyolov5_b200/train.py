@@ -5,7 +5,7 @@
     every `accumulate` iterations: ONE all-reduce of the flat gradient buffer (the reference's DDP reducer, train.py:243-245),
     GradScaler-style finite check, SGD(momentum, nesterov) with the three parameter groups of train.py:108-126, zero_grad.
 
-What is B200-native here: forward/backward are the hand-written kernels behind `Model.forward` (engine._TrainFunction); all
+What is GPU-native here: forward/backward are the hand-written kernels behind `Model.forward` (engine._TrainFunction); all
 parameters, gradients and momentum buffers live in three FLAT fp32 buffers, so the collective is a single NCCL call over one
 contiguous 31 MB region and the optimiser is a single HBM-bound launch (`myolo_sgd_step`) that also unscales, skips on overflow and
 clears the gradients.  `torch.distributed` is plumbing only (process group + all_reduce on the flat buffer).
@@ -118,7 +118,7 @@ class Trainer:
         # overlap_passes: the seg pass runs on its own train plan and stream.  Its forward starts when the det FORWARD has finished (BatchNorm
         # running statistics are then updated in the reference's order, det batch first: train.py:364,381), so the seg forward/backward
         # overlaps the det loss + backward; parameter gradients of both passes add up atomically in the one flat buffer.  At 4 images per
-        # pass the kernels are launch/latency bound and each pass alone leaves most of the 148 SMs idle.
+        # pass the kernels are launch/latency bound and each pass alone leaves most of the 132 SMs idle.
         self.overlap_passes = bool(overlap_passes) and (graph_loss or fused_det_loss)
         self._s_seg = torch.cuda.Stream() if self.overlap_passes else None
         if concurrent_forwards is None:

@@ -5,7 +5,7 @@
 
 `img` is a uint8 HWC BGR frame (numpy array or torch tensor; a CPU input is uploaded as uint8 - 4x less than the fp32 the reference
 ships to the GPU); the resize (OpenCV's 8-bit INTER_LINEAR arithmetic, bit exact), the 114 border, the channel swap, the transpose and
-the /255 run in ONE kernel of libmyolo_sm100a.  The host only does the reference's shape arithmetic.
+the /255 run in ONE kernel of libmyolo_sm90a.  The host only does the reference's shape arithmetic.
 """
 import ctypes as C
 

@@ -169,7 +169,7 @@ class ComputeLoss:
 
 
 class FusedComputeLoss:
-    """`ComputeLoss` forward + backward in four launches of libmyolo_sm100a (`myolo_det_loss`, csrc/detloss.cu): same arithmetic as the class
+    """`ComputeLoss` forward + backward in four launches of libmyolo_sm90a (`myolo_det_loss`, csrc/detloss.cu): same arithmetic as the class
     above (which is the yardstick of tests/test_gpu_train.py::test_fused_det_loss_matches_torch_formulation and the fallback for focal loss /
     positive weights / autobalance).  `__call__(p, targets, mult, scale)` returns (grads [d loss / d p_i], loss_items); the gradient is that of
     `ComputeLoss(...)(p, targets)[0] * mult / batch * scale` with the batch factor already inside, i.e. of `loss * mult_after_bs * scale`."""

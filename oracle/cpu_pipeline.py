@@ -65,9 +65,9 @@ class CpuPipeline:
 
 
 class ReferencePipeline:
-    """The UNMODIFIED reference tree (MYOLO_REFERENCE_ROOT, `baseline/_ref`, or /root/reference - whichever exists) imported through
+    """The UNMODIFIED reference tree (MYOLO_REFERENCE_ROOT or `baseline/_ref`, whichever exists) imported through
     oracle/ref_shims.py and driven exactly like detect.py:144-148,191-193.  The tree cannot travel to the GPU box (it is not an installable
-    package: `pip install /root/reference` fails with "Neither 'setup.py' nor 'pyproject.toml' found", DESIGN.md), so this class is what
+    package: `pip install <reference checkout>` fails with "Neither 'setup.py' nor 'pyproject.toml' found", DESIGN.md), so this class is what
     bench.py uses in the build container and CpuPipeline (the port) is what it uses where the tree is absent."""
 
     def __init__(self, cfg, sd, threads=None):
@@ -101,7 +101,7 @@ def reference_root():
     """first existing location of the unmodified reference tree, or None"""
     import os
     here = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    for cand in (os.environ.get("MYOLO_REFERENCE_ROOT"), os.path.join(here, "baseline", "_ref"), "/root/reference"):
+    for cand in (os.environ.get("MYOLO_REFERENCE_ROOT"), os.path.join(here, "baseline", "_ref")):
         if cand and os.path.isfile(os.path.join(cand, "models", "yolo.py")):
             return cand
     return None

@@ -1,4 +1,4 @@
-"""BENCH INFRASTRUCTURE - the reference's OWN GPU path as a baseline on the same B200 (BASELINE.md section 3 "secondary, honest comparison"):
+"""BENCH INFRASTRUCTURE - the reference's OWN GPU path as a baseline on the same GPU (BASELINE.md section 3 "secondary, honest comparison"):
 PyTorch fp16 + cuDNN with `cudnn.benchmark = True` (reference detect.py:96-103,115-124,144-148,191-193) for the detect.py job, and an
 `amp.autocast` step (reference train.py:363-401) for training.  The graph is the oracle restatement run on CUDA tensors (the reference tree
 itself cannot travel to the GPU box); when the unmodified tree is present (build container) the module builds the real reference `Model`.

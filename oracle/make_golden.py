@@ -1,8 +1,8 @@
-"""TEST INFRASTRUCTURE — generates tests/golden/* by running the UNMODIFIED reference (imported from
-/root/reference through oracle/ref_shims.py) in the build container.  The reference ships no golden
+"""TEST INFRASTRUCTURE — generates tests/golden/* by running the UNMODIFIED reference (a checkout of
+TomMao23/multiyolov5 named by MYOLO_REFERENCE_ROOT, imported through oracle/ref_shims.py) on a CPU machine.  The reference ships no golden
 vectors (SURVEY.md §4), so these fixtures are what pins the oracle restatement and the CUDA path.
 
-    python oracle/make_golden.py            # regenerate everything (needs /root/reference)
+    python oracle/make_golden.py            # regenerate everything (needs MYOLO_REFERENCE_ROOT)
 
 Fixtures (all small; weights are NOT stored — they are re-synthesised from the manifest + seed):
   manifest_<tag>.json      reference state_dict keys / shapes / dtypes for each model config
@@ -239,7 +239,7 @@ def gen_consumers():
     print("consumers", int(correct), int(labeled), inter[:4], union[:4])
 
 
-# tcgen05-sized inference fixtures: every backbone / neck / head conv of these inputs runs on conv_tc_kernel (the 64x96 fixtures above
+# tensor-core-sized inference fixtures: every backbone / neck / head conv of these inputs runs on conv_tc_kernel (the 64x96 fixtures above
 # put every map below P2 on the CUDA-core kernel).  Stored compactly: z fp32, raw x_i fp16, low-resolution seg logits fp32, two taps.
 BIG_CASES = {
     "s_psp_256x512": ("s_psp", "yolov5s_city_seg.yaml", 1, 256, 512, 3),

@@ -1,5 +1,5 @@
-"""TEST INFRASTRUCTURE — import-only shims so the UNMODIFIED reference at /root/reference can be
-imported in the build container (it cannot travel to the GPU box).
+"""TEST INFRASTRUCTURE — import-only shims so the UNMODIFIED reference (a checkout named by
+MYOLO_REFERENCE_ROOT) can be imported on a CPU machine to generate fixtures (it is not an installable package).
 
 Only oracle/make_golden.py and oracle/check_restatement.py use this module.  Nothing in the product
 (multiyolov5_b200/), bench.py's default arm, or the `-m gpu` tests may import it.
@@ -13,7 +13,7 @@ import os
 import sys
 import types
 
-REF_ROOT = os.environ.get("MYOLO_REFERENCE_ROOT", "/root/reference")
+REF_ROOT = os.environ.get("MYOLO_REFERENCE_ROOT", "")
 
 
 def reference_available() -> bool:

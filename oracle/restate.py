@@ -665,7 +665,7 @@ def seg_ce_loss(seg: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
 
 # ------------------------------------------------------------------------------------------------
 # pre-process (SURVEY.md section 8f rank 1): letterbox + BGR->RGB + HWC->CHW  (reference utils/datasets.py:818-848, :185-189)
-# The arithmetic lives in a third-party dependency that is not under /root/reference: OpenCV `cv2.resize(..., INTER_LINEAR)` and
+# The arithmetic lives in a third-party dependency that is not part of the reference tree: OpenCV `cv2.resize(..., INTER_LINEAR)` and
 # `cv2.copyMakeBorder` (requirements.txt: opencv-python>=4.1.2; 4.13.0 installed).  Its published 8-bit algorithm (imgproc/resize.cpp)
 # is restated here and pinned against cv2 itself through the fixtures (tests/golden/letterbox_cases.npz, generated by running the
 # reference's own `letterbox`).

@@ -1,4 +1,4 @@
-"""GPU: the fused Conv+BN+SiLU(+residual) kernels (tcgen05 path and CUDA-core path) against a torch fp32 restatement of
+"""GPU: the fused Conv+BN+SiLU(+residual) kernels (wgmma path and CUDA-core path) against a torch fp32 restatement of
 Conv.fuseforward (reference models/common.py:45-46, BN fold utils/torch_utils.py:182-202) on identical fp16-rounded inputs.
 Tolerance: |err| <= 2e-3 * max|ref| + fp16 output rounding (the kernels accumulate in fp32; only the sum order differs)."""
 import numpy as np
@@ -28,24 +28,24 @@ SHAPES = [
     (1, 32, 32, 48, 96, 3, 1, 1, False),      # kc=16 with Ci=48, Co=96
     (1, 16, 32, 192, 192, 1, 1, 1, False),    # Co=192 -> BN=96 x 2
     (3, 8, 16, 64, 64, 1, 1, 1, False),       # exactly one tile per image
-    (2, 16, 128, 64, 64, 3, 1, 1, False),     # full-row tiles (tw=128): strip mode when MYOLO_STRIP is set
-    (1, 12, 128, 64, 64, 3, 1, 2, True),      # strip + dilation 2 + residual
-    (1, 8, 128, 64, 64, 3, 1, 3, False),      # strip + dilation 3
-    (1, 8, 256, 256, 128, 3, 1, 1, False),    # strip, 4 channel blocks, W=256 (2 tiles per row), streamed weights
-    (2, 16, 256, 32, 32, 3, 1, 1, True),      # strip with 64-byte rows (kc=32) + residual (L2 bottleneck class)
-    (2, 16, 512, 16, 32, 3, 1, 1, False),     # strip with 32-byte rows (kc=16): Focus conv class
-    (1, 8, 128, 48, 96, 3, 1, 2, False),      # strip, kc=16 x 3 channel blocks, dilation 2
-    (16, 64, 256, 32, 32, 3, 1, 1, True),     # vertical rounds: 2 rows share 4 strips (weights-stationary) + residual
-    (16, 128, 256, 16, 32, 3, 1, 1, False),   # vertical rounds: 4 rows share 6 strips, 32-byte rows (Focus conv at scale)
-    (8, 37, 512, 32, 32, 3, 1, 1, False),     # vertical rounds with a ragged last row group (Ho = 37)
-    (16, 64, 256, 32, 32, 1, 1, 1, False),    # many tiles, BN=32 -> 4 tiles per accumulator round
-    (8, 64, 128, 64, 64, 1, 1, 1, True),      # 2 tiles per round + residual
-    # pair mode (two M tiles per weight fetch; needs >= ~120 pair rounds: layers at bench scale)
-    (16, 32, 64, 128, 128, 3, 1, 1, True),    # P4 bottleneck 3x3: 128 pair rounds, taps, 2 x 128 TMEM columns per stage, residual
-    (16, 64, 128, 64, 64, 3, 1, 2, False),    # strip + dilation 2: 444 pair rounds + 136 single-tile tail rounds
-    (16, 64, 128, 128, 256, 3, 2, 1, False),  # stride 2, two N tiles: pairs share the N tile
-    (16, 32, 64, 128, 80, 3, 1, 1, False),    # five 16-column chunks: the epilogue halves split the pair's tiles instead of columns
-    (6, 64, 128, 256, 128, 3, 1, 1, False),   # FFM class: strip, 4 channel blocks, 384 tiles -> 148 pair rounds + 88 singles
+    (2, 16, 128, 64, 64, 3, 1, 1, False),     # full-row tiles (tw=128)
+    (1, 12, 128, 64, 64, 3, 1, 2, True),      # full-row tiles + dilation 2 + residual
+    (1, 8, 128, 64, 64, 3, 1, 3, False),      # full-row tiles + dilation 3
+    (1, 8, 256, 256, 128, 3, 1, 1, False),    # 4 channel blocks, W=256 (2 tiles per row)
+    (2, 16, 256, 32, 32, 3, 1, 1, True),      # 64-byte rows (kc=32) + residual (L2 bottleneck class)
+    (2, 16, 512, 16, 32, 3, 1, 1, False),     # 32-byte rows (kc=16): Focus conv class
+    (1, 8, 128, 48, 96, 3, 1, 2, False),      # kc=16 x 3 channel blocks, dilation 2
+    (16, 64, 256, 32, 32, 3, 1, 1, True),     # many full-row tiles + residual
+    (16, 128, 256, 16, 32, 3, 1, 1, False),   # many full-row tiles, 32-byte rows (Focus conv at scale)
+    (8, 37, 512, 32, 32, 3, 1, 1, False),     # ragged image height (Ho = 37)
+    (16, 64, 256, 32, 32, 1, 1, 1, False),    # many tiles, BN=32
+    (8, 64, 128, 64, 64, 1, 1, 1, True),      # many tiles + residual
+    # layers at bench scale (more tiles than SMs: the persistent CTAs take several tiles each)
+    (16, 32, 64, 128, 128, 3, 1, 1, True),    # P4 bottleneck 3x3, residual
+    (16, 64, 128, 64, 64, 3, 1, 2, False),    # dilation 2, 1024 tiles
+    (16, 64, 128, 128, 256, 3, 2, 1, False),  # stride 2, two N tiles
+    (16, 32, 64, 128, 80, 3, 1, 1, False),    # N tile of 80 channels
+    (6, 64, 128, 256, 128, 3, 1, 1, False),   # FFM class: 4 channel blocks, 384 tiles
 ]
 
 
@@ -62,7 +62,7 @@ def torch_ref(x_nhwc, w, bn, stride, dil, residual, eps=1e-3):
     return y.permute(0, 2, 3, 1).contiguous()
 
 
-# path 2: CUDA-core kernel, 1: tcgen05 kernel with the planner's tiling rules, 3: tcgen05 with pair mode wherever it is legal
+# path 2: CUDA-core kernel, 1: wgmma kernel with the planner's tiling rules, 3: the same wgmma kernel through the standalone path-3 entry
 PAIR_SHAPES = [s for s in SHAPES if s[0] >= 6 and s[5] == 3][-5:] + [(16, 32, 64, 256, 128, 1, 1, 1, False), (2, 32, 64, 64, 64, 1, 1, 1, False)]
 
 

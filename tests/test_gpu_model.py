@@ -1,4 +1,4 @@
-"""GPU: Model(cfg).forward on the compiled sm_100a plan vs (a) the fp16-storage emulation of the oracle (tight: only fp32
+"""GPU: Model(cfg).forward on the compiled sm_90a plan vs (a) the fp16-storage emulation of the oracle (tight: only fp32
 accumulation order differs) and (b) the fixtures produced by the unmodified fp32 reference (north_star budget; measured
 deviations are recorded in DESIGN.md)."""
 import os
@@ -70,7 +70,7 @@ def test_forward_matches_reference_fixture(tag):
 
 @pytest.mark.parametrize("tag,hw", [("s_psp", (256, 512)), ("m_lab", (256, 256))])
 def test_forward_tensor_core_sizes(tag, hw):
-    """resolution where every backbone/neck/head conv takes the tcgen05 path (P5 = 8x16 >= one 128-pixel tile)."""
+    """resolution where every backbone/neck/head conv takes the wgmma path (P5 = 8x16 >= one 128-pixel tile)."""
     model, cfg, sd = build(tag)
     x = synth.synth_image(2, hw[0], hw[1], seed=3).cuda()
     (z, raw), seg = model(x)
@@ -92,7 +92,7 @@ def test_forward_tensor_core_sizes(tag, hw):
 
 @pytest.mark.parametrize("tag", list(NETS))
 def test_forward_full_resolution_all_heads(tag):
-    """BASELINE.json resolution (512x1024): every head / model size on the tensor-core path incl. strip mode, vertical rounds,
+    """BASELINE.json resolution (512x1024): every head / model size on the tensor-core path incl. full-row tiles,
     dilation 6/9 (Lab ASPP), the BiSe global branch and C3SPP (Base)."""
     model, cfg, sd = build(tag)
     x = synth.synth_image(1, 512, 1024, seed=7).cuda()
@@ -111,7 +111,7 @@ def test_forward_full_resolution_all_heads(tag):
 
 @pytest.mark.parametrize("tag,dtype", [("s_psp", torch.float32), ("s_psp", torch.uint8), ("m_psp", torch.float16)])
 def test_fused_layer0_matches_unfused_path(tag, dtype, monkeypatch):
-    """csrc/focus_conv.cu (Focus + conv in one kernel from the NCHW image) vs the space-to-depth kernel + tcgen05 conv."""
+    """csrc/focus_conv.cu (Focus + conv in one kernel from the NCHW image) vs the space-to-depth kernel + wgmma conv."""
     model, cfg, sd = build(tag)
     x8 = torch.randint(0, 256, (2, 3, 128, 256), dtype=torch.uint8, generator=torch.Generator().manual_seed(3)).cuda()
     x = x8 if dtype == torch.uint8 else (x8.float() / 255.0).to(dtype)

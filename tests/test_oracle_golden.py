@@ -217,7 +217,7 @@ BIG = {"s_psp_256x512": ("s_psp", "yolov5s_city_seg.yaml"), "m_lab_256x512": ("m
 
 @pytest.mark.parametrize("name", list(BIG))
 def test_forward_restatement_matches_reference_at_tensor_core_sizes(name):
-    """the tcgen05-sized reference fixtures (netbig_*.npz) also pin the restatement (fp32 CPU both sides)"""
+    """the tensor-core-sized reference fixtures (netbig_*.npz) also pin the restatement (fp32 CPU both sides)"""
     tag, yml = BIG[name]
     cfg = synth.load_cfg(yml)
     sd = synth.synth_state_dict(synth.load_manifest(tag), cfg, seed=1)

@@ -1,5 +1,5 @@
 """Three warm-up steps then exactly ONE step of the bench workload (yolov5s_city_seg, batch 16 x 512 x 1024, half mode: forward + NMS + seg
-argmax) for ncu captures (tools/capture_profiles.sh).  Prints, last line, the number of kernels of that one step.
+argmax) for Nsight Compute captures.  Prints, last line, the number of kernels of that one step.
     --skip-count: only print how many conv_tc launches precede the measured step (for `ncu -s`)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

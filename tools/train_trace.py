@@ -1,5 +1,6 @@
 """CUPTI timeline of ONE training step (tools/bench_train.make_workload): wall, busy time per stream, union coverage, kernels ranked by total
-device time.  Usage: python tools/train_trace.py [--no-overlap]"""
+device time.  Usage: python tools/train_trace.py [--no-overlap] [--out DIR]   (full per-kernel listing: DIR/train_trace_full.txt,
+default a temporary directory)"""
 import collections, json, os, sys, tempfile
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -76,9 +77,11 @@ for e in st:
     if any(k in e["name"] for k in ("conv_simt", "spp_bwd", "seg_ce", "zero_stuff")):
         print(f"{e['ts'] - t0:9.0f} {e['dur']:7.1f} grid{e['args'].get('grid')} {e['name'].replace('myolo::', '')[:60]}")
 
-# the whole step, one line per kernel (start us, duration us, stream, name): gpurun_out/train_trace_full.txt
-os.makedirs("gpurun_out", exist_ok=True)
-with open("gpurun_out/train_trace_full.txt", "w") as fh:
+# the whole step, one line per kernel (start us, duration us, stream, name): <out>/train_trace_full.txt
+out_dir = sys.argv[sys.argv.index("--out") + 1] if "--out" in sys.argv else tempfile.mkdtemp(prefix="train_trace_")
+os.makedirs(out_dir, exist_ok=True)
+print(f"# full listing: {os.path.join(out_dir, 'train_trace_full.txt')}")
+with open(os.path.join(out_dir, "train_trace_full.txt"), "w") as fh:
     for e in st:
         fh.write(f"{e['ts'] - t0:9.1f} {e['dur']:7.1f} s{e['args'].get('stream')} grid{e['args'].get('grid')} "
                  f"{e['name'].replace('myolo::', '').replace('void ', '')[:90]}\n")
