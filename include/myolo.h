@@ -207,6 +207,36 @@ int myolo_allreduce_grads(float* flat_grad, int64_t n, void* nccl_comm, void* st
 int myolo_letterbox(const uint8_t* src, int B, int H0, int W0, int resized_w, int resized_h, int top, int left, int H, int W,
                     const int32_t* pad_bgr, void* out, int out_dtype, int chw, int swap_rb, void* stream);
 
+/* ---- detection training batches (reference utils/datasets.py:518-593 LoadImagesAndLabels.__getitem__, augment=True) ----
+ * myolo_resize_u8: cv2.resize(src, (W, H), INTER_LINEAR) of one uint8 HWC image (H0,W0,3) into dst (H,W,3), bit exact with OpenCV's
+ * 8-bit path (exact 2x down-scaling takes its area path): `load_image`'s resize to long side img_size (:629-643) for the device cache.
+ * myolo_augment_det: one batch of B augmented S x S images.  items: DEVICE array of B myolo_aug_item, built on the host from the
+ * reference's random draws (multiyolov5_b200/utils/datasets.py DetAugmenter).  Per output pixel: cv2.warpAffine (INTER_LINEAR, border 114)
+ * of the virtual canvas of warp[0] (mosaic tiles or a letterboxed image, 114 elsewhere), optionally mixed with warp[1]
+ * (trunc(a*mix_r + b*mix_q) in double), augment_hsv through the three LUTs, flipud / fliplr, BGR->RGB.
+ * out: (B,3,S,S) of out_dtype MYOLO_U8 / MYOLO_F16 / MYOLO_F32 (float = value / 255, as imgs.float() / 255 on the GPU). */
+typedef struct {
+  const uint8_t* src[4];  /* tile images: HWC BGR uint8, device */
+  int32_t rect[4][4];     /* canvas rectangle [x1, x2) x [y1, y2) covered by tile t: x1, y1, x2, y2 */
+  int32_t off[4][2];      /* source pixel of canvas pixel (x, y): (x - off[t][0], y - off[t][1]) */
+  int32_t src_w[4];       /* source row length in pixels */
+  int32_t n_tiles;        /* 1..4 */
+  int32_t reserved;
+  double minv[6];         /* the affine M inverted the way cv2.warpAffine inverts it: canvas = minv * (x, y, 1) */
+} myolo_aug_warp;
+
+typedef struct {
+  myolo_aug_warp warp[2];
+  double mix_r, mix_q;    /* mixup ratio r and 1 - r (computed by the caller) */
+  int32_t n_warps;        /* 1, or 2 with mixup */
+  int32_t flipud, fliplr;
+  int32_t reserved;
+  uint8_t lut[3][256];    /* augment_hsv LUTs: hue, saturation, value */
+} myolo_aug_item;
+
+int myolo_resize_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream);
+int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, void* stream);
+
 /* ---- consumers of the seg output (SURVEY.md section 8f rank 2) ----
  * myolo_seg_lut_blend: out[i][c] = lut[class_map[i]][c] (label2image / trainid2id, reference detect.py:69-77; reverse_channels gives the
  * BGR order of detect.py:193) and, if `blend` is given, blend[i][c] = cv2.addWeighted(out, alpha, image, beta, 0) (detect.py:194).

@@ -22,6 +22,7 @@ EXPORTS = [
     "myolo_plan_profile", "myolo_nms_workspace_bytes", "myolo_nms", "myolo_seg_upsample_argmax", "myolo_bilinear_nchw",
     "myolo_conv_bn_silu", "myolo_plan_set_bn", "myolo_plan_set_conv_grad", "myolo_plan_train_forward", "myolo_plan_backward",
     "myolo_grads_check_finite", "myolo_sgd_step", "myolo_conv_wgrad", "myolo_letterbox", "myolo_seg_lut_blend", "myolo_seg_metrics", "myolo_plan_backward_seg_ce", "myolo_plan_read_grad_view", "myolo_plan_set_seed", "myolo_plan_train_forward_multi", "myolo_plan_backward_multi", "myolo_plan_conv_info", "myolo_allreduce_grads", "myolo_det_loss", "myolo_det_loss_workspace_bytes", "myolo_plan_set_defer_running", "myolo_plan_apply_running",
+    "myolo_resize_u8", "myolo_augment_det",
 ]
 
 
@@ -37,6 +38,16 @@ class Op(C.Structure):
     _fields_ = [("kind", C.c_int32), ("in_", View), ("in2", View), ("out", View), ("k", C.c_int32), ("stride", C.c_int32),
                 ("dil", C.c_int32), ("act", C.c_int32), ("flags", C.c_int32), ("weight_slot", C.c_int32),
                 ("aux", C.c_int32 * 8), ("faux", C.c_float * 4)]
+
+
+class AugWarp(C.Structure):
+    _fields_ = [("src", C.c_void_p * 4), ("rect", (C.c_int32 * 4) * 4), ("off", (C.c_int32 * 2) * 4), ("src_w", C.c_int32 * 4),
+                ("n_tiles", C.c_int32), ("reserved", C.c_int32), ("minv", C.c_double * 6)]
+
+
+class AugItem(C.Structure):
+    _fields_ = [("warp", AugWarp * 2), ("mix_r", C.c_double), ("mix_q", C.c_double), ("n_warps", C.c_int32), ("flipud", C.c_int32),
+                ("fliplr", C.c_int32), ("reserved", C.c_int32), ("lut", (C.c_uint8 * 256) * 3)]
 
 
 class MyoloError(RuntimeError):
@@ -75,6 +86,8 @@ def lib():
     L.myolo_plan_train_forward.argtypes = [vp, vp, i32, C.POINTER(vp), vp, vp]
     L.myolo_plan_backward.argtypes = [vp, C.POINTER(vp), vp, vp]
     L.myolo_letterbox.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp, vp, i32, i32, i32, vp]
+    L.myolo_resize_u8.argtypes = [vp, i32, i32, vp, i32, i32, vp]
+    L.myolo_augment_det.argtypes = [vp, i32, i32, vp, i32, vp]
     L.myolo_seg_lut_blend.argtypes = [vp, i32, i64, vp, i32, i32, i32, vp, vp, f32, f32, vp, vp]
     L.myolo_seg_metrics.argtypes = [vp, i32, vp, i64, i32, vp, vp]
     L.myolo_plan_backward_seg_ce.argtypes = [vp, vp, i32, f32, vp, vp, vp]

@@ -1,0 +1,143 @@
+// Detection training batches on the device (reference utils/datasets.py:518-593 `LoadImagesAndLabels.__getitem__` with augment=True):
+// the image cache resize of `load_image` (:629-643), and ONE fused kernel per batch for the 4-image mosaic (:671-724), the affine
+// `random_perspective` warp (:851-893), mixup (:529-532), `augment_hsv` (:646-657), the flips (:571-582) and BGR->RGB / HWC->CHW (:589).
+// The host draws the random parameters and transforms the labels (multiyolov5_b200/utils/datasets.py DetAugmenter); this file only moves
+// pixels.  Every step is bit exact with OpenCV 8-bit arithmetic:
+//   * cv2.warpAffine INTER_LINEAR / BORDER_CONSTANT 114: 10-bit fixed-point source addresses, 5-bit fractions, 15-bit weights;
+//   * the 2s x 2s mosaic canvas is never built: a canvas pixel is the tile covering it, else 114 (also outside the canvas);
+//   * cv2.COLOR_BGR2HSV: integer (hsv_shift 12) with rounded division tables;
+//   * cv2.COLOR_HSV2BGR: float32 with the (1 - s*h) terms as fused multiply-adds and the result *255 truncated, which is what OpenCV's
+//     8-bit path computes (proven over all 180x256x256 inputs by tests/test_augment_host.py against cv2 itself).
+// Double precision is written with __dmul_rn / __dadd_rn so that nvcc cannot contract it into fused multiply-adds.
+// Parity: tests/test_gpu_augment.py.
+#include "kernels.h"
+#include "resize.cuh"
+
+namespace myolo {
+
+static_assert(sizeof(myolo_aug_warp) == 200 && sizeof(myolo_aug_item) == 1200, "layout shared with multiyolov5_b200/_lib.py");
+
+__global__ void resize_u8_kernel(const unsigned char* src, ResizeGeom g, unsigned char* dst, int H, int W) {
+  const long total = (long)H * W;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    int v[3];
+    resize_pixel_u8(src, g, (int)(i % W), (int)(i / W), v);
+    dst[i * 3 + 0] = (unsigned char)v[0];
+    dst[i * 3 + 1] = (unsigned char)v[1];
+    dst[i * 3 + 2] = (unsigned char)v[2];
+  }
+}
+
+int launch_resize_u8(const unsigned char* src, int H0, int W0, unsigned char* dst, int H, int W, cudaStream_t s) {
+  MYOLO_REQUIRE(src && dst && H0 > 0 && W0 > 0 && H > 0 && W > 0, "resize_u8: bad geometry (src %dx%d dst %dx%d)", W0, H0, W, H);
+  const long total = (long)H * W;
+  resize_u8_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(src, resize_geom(H0, W0, H, W), dst, H, W);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+// one of the (up to) four tiles of a warp's virtual canvas
+__device__ __forceinline__ void canvas_px(const myolo_aug_warp& w, int cx, int cy, int v[3]) {
+  v[0] = v[1] = v[2] = 114;
+  for (int t = 0; t < w.n_tiles; ++t) {       // mosaic tiles are disjoint; a later tile would win like the later img4 assignment
+    if (cx >= w.rect[t][0] && cy >= w.rect[t][1] && cx < w.rect[t][2] && cy < w.rect[t][3]) {
+      const unsigned char* q = w.src[t] + ((size_t)(cy - w.off[t][1]) * w.src_w[t] + (cx - w.off[t][0])) * 3;
+      v[0] = __ldg(q); v[1] = __ldg(q + 1); v[2] = __ldg(q + 2);
+    }
+  }
+}
+
+// cv2.warpAffine(canvas, M, (S, S), INTER_LINEAR, BORDER_CONSTANT, 114) at destination pixel (x, y); minv is M inverted as cv2 inverts it
+__device__ __forceinline__ void warp_px(const myolo_aug_warp& w, int x, int y, int v[3]) {
+  const double* m = w.minv;
+  const int adelta = __double2int_rn(__dmul_rn(__dmul_rn(m[0], (double)x), 1024.0));
+  const int bdelta = __double2int_rn(__dmul_rn(__dmul_rn(m[3], (double)x), 1024.0));
+  const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[1], (double)y), m[2]), 1024.0)) + 16;
+  const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(m[4], (double)y), m[5]), 1024.0)) + 16;
+  const int X = (X0 + adelta) >> 5, Y = (Y0 + bdelta) >> 5;
+  const int sx = X >> 5, sy = Y >> 5, fx = X & 31, fy = Y & 31;
+  // initInterTab2D's 15-bit weights: float products of multiples of 1/32 are exact, so they round to these integers and their sum is
+  // always 2^15 (the table's rounding-error correction never fires)
+  const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
+  int p00[3], p01[3], p10[3], p11[3];
+  canvas_px(w, sx, sy, p00);
+  canvas_px(w, sx + 1, sy, p01);
+  canvas_px(w, sx, sy + 1, p10);
+  canvas_px(w, sx + 1, sy + 1, p11);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) v[c] = min(255, max(0, (p00[c] * w00 + p01[c] * w01 + p10[c] * w10 + p11[c] * w11 + (1 << 14)) >> 15));
+}
+
+__global__ void __launch_bounds__(256) augment_det_kernel(const myolo_aug_item* __restrict__ items, int B, int S, void* out, int out_dtype) {
+  __shared__ int sdiv[256], hdiv[256];          // cv2 RGB2HSV_b tables: round((255 << 12) / v), round((180 << 12) / (6 * diff))
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) {
+    sdiv[i] = i ? __double2int_rn(__ddiv_rn(255.0 * 4096.0, (double)i)) : 0;
+    hdiv[i] = i ? __double2int_rn(__ddiv_rn(180.0 * 4096.0, __dmul_rn(6.0, (double)i))) : 0;
+  }
+  __syncthreads();
+  const long plane = (long)S * S, total = (long)B * plane;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int b = (int)(i / plane);
+    const int y = (int)((i % plane) / S), x = (int)(i % S);
+    const myolo_aug_item& it = items[b];
+    const int ys = it.flipud ? S - 1 - y : y, xs = it.fliplr ? S - 1 - x : x;    // np.flipud / np.fliplr of the augmented image
+    int px[3];
+    warp_px(it.warp[0], xs, ys, px);
+    if (it.n_warps == 2) {                       // mixup: (img * r + img2 * (1 - r)).astype(np.uint8) in float64
+      int px2[3];
+      warp_px(it.warp[1], xs, ys, px2);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) px[c] = (int)__dadd_rn(__dmul_rn((double)px[c], it.mix_r), __dmul_rn((double)px2[c], it.mix_q));
+    }
+    // ---- augment_hsv: BGR -> HSV (integer), LUTs, HSV -> BGR
+    const int bb = px[0], gg = px[1], rr = px[2];
+    const int vmax = max(bb, max(gg, rr)), vmin = min(bb, min(gg, rr)), diff = vmax - vmin;
+    const int vr = vmax == rr ? -1 : 0, vg = vmax == gg ? -1 : 0;
+    const int sat = (diff * sdiv[vmax] + (1 << 11)) >> 12;
+    int hue = (vr & (gg - bb)) + (~vr & ((vg & (bb - rr + 2 * diff)) + ((~vg) & (rr - gg + 4 * diff))));
+    hue = (hue * hdiv[diff] + (1 << 11)) >> 12;
+    hue += hue < 0 ? 180 : 0;
+    const float hf = (float)it.lut[0][hue];
+    const float sf = __fmul_rn((float)it.lut[1][sat], 1.0f / 255.0f);
+    const float vf = __fmul_rn((float)it.lut[2][vmax], 1.0f / 255.0f);
+    const float hx = __fmul_rn(hf, 6.0f / 180.0f);
+    const float sector_f = floorf(hx);
+    const float fr = __fsub_rn(hx, sector_f);
+    const float tab1 = __fmul_rn(vf, __fsub_rn(1.0f, sf));
+    const float tab2 = __fmul_rn(vf, __fmaf_rn(-sf, fr, 1.0f));
+    const float tab3 = __fmul_rn(vf, __fmaf_rn(-sf, __fsub_rn(1.0f, fr), 1.0f));
+    int sector = (int)sector_f;
+    sector = sector < 0 || sector > 5 ? 0 : sector;
+    // sector -> (b, g, r) entries of the table (v, tab1, tab2, tab3): {1,3,0} {1,0,2} {3,0,1} {0,2,1} {0,1,3} {2,1,0}, 2 bits each, 6 bits per sector
+    const unsigned long long code = 0x0Dull | (0x21ull << 6) | (0x13ull << 12) | (0x18ull << 18) | (0x34ull << 24) | (0x06ull << 30);
+    const unsigned sel = (unsigned)(code >> (6 * sector)) & 63u;
+    int bgr[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {                // selects instead of an indexed array: keeps the table in registers
+      const unsigned k = (sel >> (2 * c)) & 3u;
+      const float t = k == 0 ? vf : k == 1 ? tab1 : k == 2 ? tab2 : tab3;
+      bgr[c] = (int)__fmul_rn(t, 255.0f);      // truncation, as cv2's 8-bit path
+    }
+    // ---- BGR -> RGB, HWC -> CHW
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const int val = bgr[2 - c];
+      const size_t o = ((size_t)b * 3 + c) * plane + (size_t)y * S + x;
+      if (out_dtype == MYOLO_U8) reinterpret_cast<unsigned char*>(out)[o] = (unsigned char)val;
+      // imgs.float() / 255 on a CUDA tensor (reference train.py:342): ATen multiplies by the fp32 reciprocal of a scalar divisor
+      else if (out_dtype == MYOLO_F16) reinterpret_cast<__half*>(out)[o] = __float2half_rn(__fmul_rn((float)val, 1.0f / 255.0f));
+      else reinterpret_cast<float*>(out)[o] = __fmul_rn((float)val, 1.0f / 255.0f);
+    }
+  }
+}
+
+int launch_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, cudaStream_t s) {
+  MYOLO_REQUIRE(items && out && B > 0 && S > 0, "augment_det: bad arguments (B %d S %d)", B, S);
+  MYOLO_REQUIRE(out_dtype == MYOLO_U8 || out_dtype == MYOLO_F16 || out_dtype == MYOLO_F32, "augment_det: output dtype");
+  const long total = (long)B * S * S;
+  augment_det_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(items, B, S, out, out_dtype);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace myolo

@@ -35,6 +35,10 @@ int launch_read_view(const TensorView& v, float* dst_nchw, cudaStream_t s);
 int launch_letterbox(const unsigned char* src, int B, int H0, int W0, int rw, int rh, int top, int left, int H, int W, const int* pad3,
                      void* dst, int out_dtype, int chw, int swap_rb, cudaStream_t s);
 
+// detection training batches (augment.cu): image cache resize and the fused mosaic / warp / mixup / HSV / flip kernel
+int launch_resize_u8(const unsigned char* src, int H0, int W0, unsigned char* dst, int H, int W, cudaStream_t s);
+int launch_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, cudaStream_t s);
+
 // seg output consumers (consumers.cu)
 int launch_lut_blend(const void* idx, int idx_dtype, long n, const unsigned char* lut, int n_entries, int ch, int reverse, unsigned char* out,
                      const unsigned char* im, float alpha, float beta, unsigned char* blend, cudaStream_t s);

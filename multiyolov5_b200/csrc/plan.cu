@@ -1334,6 +1334,18 @@ extern "C" int myolo_letterbox(const uint8_t* src, int B, int H0, int W0, int re
   return launch_letterbox(src, B, H0, W0, resized_w, resized_h, top, left, H, W, pad_bgr, out, out_dtype, chw, swap_rb, (cudaStream_t)stream);
 }
 
+extern "C" int myolo_resize_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_resize_u8(src, H0, W0, dst, H, W, (cudaStream_t)stream);
+}
+
+extern "C" int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_augment_det(items, B, S, out, out_dtype, (cudaStream_t)stream);
+}
+
 extern "C" int myolo_seg_lut_blend(const void* class_map, int map_dtype, int64_t n_pixels, const uint8_t* lut, int n_entries, int channels,
                                    int reverse_channels, uint8_t* out, const uint8_t* image, float alpha, float beta, uint8_t* blend,
                                    void* stream) {
