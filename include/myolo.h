@@ -6,6 +6,8 @@
  *   - models.yolo.Model.fuse  (BN folding)              (reference models/yolo.py:339-347, utils/torch_utils.py:182-202)
  *   - utils.general.non_max_suppression                 (reference utils/general.py:421-509)
  *   - detect.py's seg upsample + argmax                 (reference detect.py:191-193)
+ *   - the training batch loaders: LoadImagesAndLabels.__getitem__ (utils/datasets.py:518-593) and the segmentation
+ *     datasets' `_sync_transform` + ColorJitter + ToTensor (SegmentationDataset.py:118-151, :458-531)
  * so the "FFI binding" a maintainer adds on the reference side is a ctypes stub (INTEGRATION.md).
  *
  * Conventions
@@ -236,6 +238,34 @@ typedef struct {
 
 int myolo_resize_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream);
 int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, void* stream);
+
+/* ---- segmentation training batches (reference SegmentationDataset.py:118-151 `_sync_transform` + ColorJitter + ToTensor, and the
+ * testval items of :81-94) ----
+ * myolo_augment_seg: B items in two launches on `stream`.  Per item: Pillow's bilinear Image.resize of the source (mirrored when `flip`)
+ * evaluated over the h x w crop window only, right/bottom pad 0, the ColorJitter ops in `order`, ToTensor; the mask through Pillow's
+ * NEAREST resize (pad 255) and `lut` into out_mask (B,mh,mw) int64.  items: DEVICE array, built on the host
+ * (multiyolov5_b200/utils/datasets.py SegAugmenter); lsum must be 0 on entry (the kernel accumulates into it).  tables: DEVICE int32
+ * array the items' offsets index.  scratch: B*h*w*3 bytes.  out_img: (B,3,h,w) of out_dtype MYOLO_U8 / MYOLO_F16 / MYOLO_F32
+ * (float = v / 255 as ToTensor divides, fp16 that value rounded).  All arithmetic is bit exact with Pillow's. */
+typedef struct {
+  const uint8_t* img;     /* source (H0, W0, 3) RGB uint8, device */
+  const uint8_t* mask;    /* source (H0, W0) uint8, device */
+  int32_t H0, W0;
+  int32_t flip;           /* mirror: source column x is read as W0-1-x */
+  int32_t kx, ky;         /* coefficients per column / row entry */
+  int32_t col, row;       /* offsets in `tables` of w column / h row entries {first source index, taps (0 = pad), kx|ky int32
+                             coefficients with 22 fraction bits} */
+  int32_t mcol, mrow;     /* offsets in `tables` of mw / mh mask source indices (-1 = pad) */
+  int32_t order[4];       /* jitter ops in application order, -1 = none: 0 brightness, 1 contrast, 2 saturation, 3 hue */
+  float factor[3];        /* brightness, contrast, saturation factors (C float, as Image.blend narrows them) */
+  int32_t hue_shift;      /* added to H modulo 256 */
+  int32_t reserved;
+  uint64_t lsum;          /* sum of convert("L") of the image entering contrast: 0 on entry */
+  int32_t lut[256];       /* mask value -> label */
+} myolo_seg_item;
+
+int myolo_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int mw, const int32_t* tables, uint8_t* scratch, void* out_img,
+                      int out_dtype, int64_t* out_mask, void* stream);
 
 /* ---- consumers of the seg output (SURVEY.md section 8f rank 2) ----
  * myolo_seg_lut_blend: out[i][c] = lut[class_map[i]][c] (label2image / trainid2id, reference detect.py:69-77; reverse_channels gives the

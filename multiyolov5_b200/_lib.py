@@ -22,7 +22,7 @@ EXPORTS = [
     "myolo_plan_profile", "myolo_nms_workspace_bytes", "myolo_nms", "myolo_seg_upsample_argmax", "myolo_bilinear_nchw",
     "myolo_conv_bn_silu", "myolo_plan_set_bn", "myolo_plan_set_conv_grad", "myolo_plan_train_forward", "myolo_plan_backward",
     "myolo_grads_check_finite", "myolo_sgd_step", "myolo_conv_wgrad", "myolo_letterbox", "myolo_seg_lut_blend", "myolo_seg_metrics", "myolo_plan_backward_seg_ce", "myolo_plan_read_grad_view", "myolo_plan_set_seed", "myolo_plan_train_forward_multi", "myolo_plan_backward_multi", "myolo_plan_conv_info", "myolo_allreduce_grads", "myolo_det_loss", "myolo_det_loss_workspace_bytes", "myolo_plan_set_defer_running", "myolo_plan_apply_running",
-    "myolo_resize_u8", "myolo_augment_det",
+    "myolo_resize_u8", "myolo_augment_det", "myolo_augment_seg",
 ]
 
 
@@ -48,6 +48,13 @@ class AugWarp(C.Structure):
 class AugItem(C.Structure):
     _fields_ = [("warp", AugWarp * 2), ("mix_r", C.c_double), ("mix_q", C.c_double), ("n_warps", C.c_int32), ("flipud", C.c_int32),
                 ("fliplr", C.c_int32), ("reserved", C.c_int32), ("lut", (C.c_uint8 * 256) * 3)]
+
+
+class SegItem(C.Structure):
+    _fields_ = [("img", C.c_void_p), ("mask", C.c_void_p), ("H0", C.c_int32), ("W0", C.c_int32), ("flip", C.c_int32), ("kx", C.c_int32),
+                ("ky", C.c_int32), ("col", C.c_int32), ("row", C.c_int32), ("mcol", C.c_int32), ("mrow", C.c_int32),
+                ("order", C.c_int32 * 4), ("factor", C.c_float * 3), ("hue_shift", C.c_int32), ("reserved", C.c_int32),
+                ("lsum", C.c_uint64), ("lut", C.c_int32 * 256)]
 
 
 class MyoloError(RuntimeError):
@@ -88,6 +95,7 @@ def lib():
     L.myolo_letterbox.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp, vp, i32, i32, i32, vp]
     L.myolo_resize_u8.argtypes = [vp, i32, i32, vp, i32, i32, vp]
     L.myolo_augment_det.argtypes = [vp, i32, i32, vp, i32, vp]
+    L.myolo_augment_seg.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp]
     L.myolo_seg_lut_blend.argtypes = [vp, i32, i64, vp, i32, i32, i32, vp, vp, f32, f32, vp, vp]
     L.myolo_seg_metrics.argtypes = [vp, i32, vp, i64, i32, vp, vp]
     L.myolo_plan_backward_seg_ce.argtypes = [vp, vp, i32, f32, vp, vp, vp]

@@ -39,6 +39,10 @@ int launch_letterbox(const unsigned char* src, int B, int H0, int W0, int rw, in
 int launch_resize_u8(const unsigned char* src, int H0, int W0, unsigned char* dst, int H, int W, cudaStream_t s);
 int launch_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, cudaStream_t s);
 
+// segmentation training batches (augment_seg.cu): crop-window resample + pad + mask LUT, then the ColorJitter / ToTensor kernel
+int launch_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int mw, const int* tables, unsigned char* scratch, void* out,
+                       int out_dtype, long long* out_mask, cudaStream_t s);
+
 // seg output consumers (consumers.cu)
 int launch_lut_blend(const void* idx, int idx_dtype, long n, const unsigned char* lut, int n_entries, int ch, int reverse, unsigned char* out,
                      const unsigned char* im, float alpha, float beta, unsigned char* blend, cudaStream_t s);

@@ -1346,6 +1346,13 @@ extern "C" int myolo_augment_det(const myolo_aug_item* items, int B, int S, void
   return launch_augment_det(items, B, S, out, out_dtype, (cudaStream_t)stream);
 }
 
+extern "C" int myolo_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int mw, const int32_t* tables, uint8_t* scratch,
+                                 void* out_img, int out_dtype, int64_t* out_mask, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_augment_seg(items, B, h, w, mh, mw, tables, scratch, out_img, out_dtype, (long long*)out_mask, (cudaStream_t)stream);
+}
+
 extern "C" int myolo_seg_lut_blend(const void* class_map, int map_dtype, int64_t n_pixels, const uint8_t* lut, int n_entries, int channels,
                                    int reverse_channels, uint8_t* out, const uint8_t* image, float alpha, float beta, uint8_t* blend,
                                    void* stream) {

@@ -3,12 +3,15 @@
     letterbox(img, new_shape, color, auto, scaleFill, scaleup, stride) -> (img, ratio, (dw, dh))     reference utils/datasets.py:818-848
     preprocess(img0, img_size, stride, half)  -> (1|B,3,H,W) float tensor in [0,1]                     :185-189 + detect.py:135-137
     DeviceImageCache(images, img_size, labels) / DetAugmenter(cache, hyp)(indices) -> (imgs, targets)   :518-599 (augment=True)
+    DeviceSegCache(images, masks, mask_map) / SegAugmenter(cache, base_size, crop_size, preset)(indices) -> (segimgs, segtargets)
+                                                                             SegmentationDataset.py:118-151 + ColorJitter + ToTensor
 
 `img` is a uint8 HWC BGR frame (numpy array or torch tensor; a CPU input is uploaded as uint8 - 4x less than the fp32 the reference
 ships to the GPU); the resize (OpenCV's 8-bit INTER_LINEAR arithmetic, bit exact), the 114 border, the channel swap, the transpose and
 the /255 run in ONE kernel of libmyolo_sm90a.  The host only does the reference's shape arithmetic.
 """
 import ctypes as C
+import functools
 import math
 import random
 
@@ -330,3 +333,300 @@ class DetAugmenter:
         targets = torch.cat(targets, 0).pin_memory().cuda(non_blocking=True)
         self._keep = [dev_items] + self._keep
         return imgs, targets
+
+
+# ------------------------------------------------------------------------------------------------
+# segmentation training batches (reference SegmentationDataset.py:118-151 _sync_transform, :182-189 / :219-222 _mask_transform,
+# :81-94 _testval_img_transform, and the loader functions' ColorJitter + ToTensor, :458-531)
+# ------------------------------------------------------------------------------------------------
+# Cityscapes label id -> train id (the reference's `_key` at np.digitize(id, range(-1, 34), right=True) = id + 1)
+_CITYSCAPES_KEY = np.array([-1, -1, -1, -1, -1, -1, -1, -1, 0, 1, -1, -1, 2, 3, 4, -1, -1, -1, 5, -1, 6, 7, 8, 9, 10, 11, 12, 13, 14,
+                            15, -1, -1, 16, 17, 18])
+_INVALID = -2
+
+# the reference's get_citys_loader / get_citysbdd_loader / get_custom_loader: ColorJitter(b, c, s, h), get_long_size(low, high, std), crop
+SEG_PRESETS = {
+    "citys": dict(brightness=0.45, contrast=0.45, saturation=0.45, hue=0.15, low=0.65, high=3.0, std=25, crop_size=(1024, 512)),
+    "citysbdd": dict(brightness=0.4, contrast=0.4, saturation=0.4, hue=0.05, low=0.65, high=2.0, std=40, crop_size=(1024, 512)),
+    "custom": dict(brightness=0.4, contrast=0.4, saturation=0.4, hue=0.0, low=0.75, high=1.5, std=35, crop_size=None),   # (base, base)
+}
+
+
+def seg_mask_lut(kind):
+    """256-entry int64 label map of a uint8 mask: 'cityscapes' is `_class_to_index` (255 -> 0, then id -> trainId; ids 34..254 are not
+    in the reference's mapping and are marked -2), 'trainid' maps 255 -> -1 and keeps every other value"""
+    lut = np.full(256, _INVALID, np.int64)
+    if kind == "cityscapes":
+        lut[:34] = _CITYSCAPES_KEY[1:]
+        lut[255] = _CITYSCAPES_KEY[1]
+    elif kind == "trainid":
+        lut[:] = np.arange(256)
+        lut[255] = -1
+    else:
+        raise ValueError(f"mask_map: expected 'cityscapes' or 'trainid', got {kind!r}")
+    return lut
+
+
+def _norm_pdf(x, mean, std):
+    """scipy.stats.norm.pdf(x, mean, std), computed as scipy computes it (tests/test_seg_augment_host.py pins it ==)"""
+    y = (np.asarray(x, np.float64) - mean) / std
+    return np.exp(-y ** 2 / 2.0) / np.sqrt(2 * np.pi) / std
+
+
+@functools.lru_cache(128)
+def range_and_prob(base_size, low=0.5, high=3.0, std=25):
+    """the reference's range_and_prob (SegmentationDataset.py:25-35): long-side candidates / 32 and their cumulative probabilities"""
+    lo = math.ceil((base_size * low) / 32)
+    hi = math.ceil((base_size * high) / 32)
+    mean = math.ceil(base_size / 32) - 4
+    x = np.array(list(range(lo, hi + 1)))
+    p = _norm_pdf(x, mean, std)
+    p = p / p.sum()
+    return x, np.cumsum(p)
+
+
+@functools.lru_cache(256)
+def _bilinear_table(in_size, out_size):
+    """Pillow's bilinear precompute_coeffs + normalize_coeffs_8bpc for an axis in_size -> out_size, as int32 rows {xmin, taps, k[0..K)}
+    (22 fraction bits).  An unchanged axis is a one-tap identity, which equals Pillow's skipped pass."""
+    if in_size == out_size:
+        t = np.zeros((out_size, 3), np.int32)
+        t[:, 0], t[:, 1], t[:, 2] = np.arange(out_size), 1, 1 << 22
+        return t
+    scale = float(in_size) / out_size
+    filterscale = max(scale, 1.0)
+    support = filterscale
+    ksize = int(math.ceil(support)) * 2 + 1
+    center = (np.arange(out_size) + 0.5) * scale
+    xmin = np.maximum((center - support + 0.5).astype(np.int64), 0)
+    xmax = np.minimum((center + support + 0.5).astype(np.int64), in_size) - xmin
+    w = np.zeros((out_size, ksize))
+    ww = np.zeros(out_size)
+    for x in range(ksize):                                   # Pillow's loop order: ww accumulates tap by tap
+        t = np.abs((x + xmin - center + 0.5) * (1.0 / filterscale))
+        w[:, x] = np.where(x < xmax, np.where(t < 1.0, 1.0 - t, 0.0), 0.0)
+        ww = ww + w[:, x]
+    k = np.where(ww[:, None] != 0.0, w / np.where(ww == 0.0, 1.0, ww)[:, None], w)
+    kk = np.where(k < 0, (-0.5 + k * (1 << 22)).astype(np.int64), (0.5 + k * (1 << 22)).astype(np.int64))
+    t = np.zeros((out_size, ksize + 2), np.int32)
+    t[:, 0], t[:, 1], t[:, 2:] = xmin, xmax, np.where(np.arange(ksize) < xmax[:, None], kk, 0)
+    return t
+
+
+@functools.lru_cache(256)
+def _nearest_index(in_size, out_size):
+    """source index per output position of Pillow's NEAREST resize (ImagingScaleAffine: xo = a/2, then xo += a, in double)"""
+    a = float(in_size) / out_size
+    idx = np.empty(out_size, np.int32)
+    xo = a * 0.5
+    for x in range(out_size):
+        idx[x] = -1 if xo < 0.0 else int(xo)
+        xo += a
+    return idx
+
+
+def _crop_rows(table, start, n, pad):
+    """rows start..start+n of an axis table, `pad` (taps 0 / index -1) beyond its end"""
+    out = np.empty((n,) + table.shape[1:], np.int32)
+    m = max(0, min(n, len(table) - start))
+    out[:m] = table[start:start + m]
+    out[m:] = pad
+    return out
+
+
+class DeviceSegCache:
+    """Decoded segmentation sources on the device: uint8 (H, W, 3) RGB frames as PIL's `convert('RGB')` decodes them and uint8 (H, W)
+    masks as `np.array(Image.open(mask))` reads them, kept at native resolution (no resize at cache time) in ONE device arena.  Decoding
+    stays with the caller.  The arena holds 4 bytes per source pixel: Cityscapes train (2975 frames of 2048x1024) is about 25 GB.
+
+    `mask_map` is 'cityscapes' (the reference's `_class_to_index`: 255 -> 0, then label id -> train id), 'trainid' (255 -> -1, every other
+    value kept: BDD100k and custom data), or a list with one of those per item (City+BDD, whose .png items are Cityscapes ids and .jpg
+    items train ids).  Masks are validated on the host before upload: a 'cityscapes' mask holding a value outside the reference's mapping
+    (34..254) raises ValueError, as the reference's assert fails on it."""
+
+    def __init__(self, images, masks, mask_map="cityscapes"):
+        if len(images) != len(masks):
+            raise ValueError(f"DeviceSegCache: {len(images)} images but {len(masks)} masks")
+        self.n = len(images)
+        kinds = [mask_map] * self.n if isinstance(mask_map, str) else list(mask_map)
+        if len(kinds) != self.n:
+            raise ValueError(f"DeviceSegCache: mask_map has {len(kinds)} entries for {self.n} items")
+        self.luts = [seg_mask_lut(k) for k in kinds]
+        self.shapes, self.img_off, self.mask_off = [], [], []
+        total = 0
+        host = []
+        for i, (im, m) in enumerate(zip(images, masks)):
+            im = im.cpu().numpy() if isinstance(im, torch.Tensor) else np.asarray(im)
+            m = m.cpu().numpy() if isinstance(m, torch.Tensor) else np.asarray(m)
+            if im.dtype != np.uint8 or im.ndim != 3 or im.shape[2] != 3:
+                raise ValueError(f"DeviceSegCache: image {i} must be uint8 (H, W, 3) RGB, got {im.dtype} {im.shape}")
+            if m.dtype != np.uint8 or m.shape != im.shape[:2]:
+                raise ValueError(f"DeviceSegCache: mask {i} must be uint8 {im.shape[:2]}, got {m.dtype} {m.shape}")
+            bad = np.flatnonzero((self.luts[i][np.flatnonzero(np.bincount(m.ravel(), minlength=256))] == _INVALID))
+            if bad.size:
+                vals = np.flatnonzero(np.bincount(m.ravel(), minlength=256))[bad]
+                raise ValueError(f"DeviceSegCache: mask {i} holds values {vals.tolist()} outside the {kinds[i]} mapping")
+            h, w = im.shape[:2]
+            self.shapes.append((h, w))
+            self.img_off.append(total)
+            self.mask_off.append(total + h * w * 3)
+            total += h * w * 4
+            host.append((im, m))
+        if not torch.cuda.is_available():
+            raise _lib.MyoloError("DeviceSegCache needs a CUDA device: multiyolov5_b200 has no CPU path")
+        self.arena = torch.empty(max(total, 1), dtype=torch.uint8, device="cuda")
+        for (im, m), io, mo in zip(host, self.img_off, self.mask_off):
+            self.arena[io:mo].copy_(torch.from_numpy(np.ascontiguousarray(im)).view(-1))
+            self.arena[mo:mo + m.size].copy_(torch.from_numpy(np.ascontiguousarray(m)).view(-1))
+
+    def image(self, i):
+        h, w = self.shapes[i]
+        return self.arena[self.img_off[i]:self.img_off[i] + h * w * 3].view(h, w, 3)
+
+    def mask(self, i):
+        h, w = self.shapes[i]
+        return self.arena[self.mask_off[i]:self.mask_off[i] + h * w].view(h, w)
+
+
+class SegAugmenter:
+    """Segmentation training batches on the device: `SegAugmenter(cache, base_size, crop_size, preset)(indices)` returns what
+    `default_collate([dataset[i] for i in indices])` returns for the reference's mode='train' datasets (CitySegmentation,
+    CityBddSegmentation, CustomSegmentation with the transforms of their loader functions): float32 (B, 3, h, w) images = uint8 / 255 as
+    ToTensor divides (or uint8 / float16 = that float32 rounded) and int64 (B, h, w) labels with -1 = ignore, both on the GPU; (w, h) is
+    `crop_size`.
+
+    `preset` is 'citys', 'citysbdd' or 'custom' (SEG_PRESETS: jitter factors, long-side sampling low / high / std, crop); explicit
+    arguments override it.  The random parameters are drawn on the host in exactly the reference's order and number: `random.random()`
+    (mirror), `random.choices` (long side), `random.randint` (x1, then y1), then ColorJitter.get_params on torch's CPU generator
+    (`torch.randperm(4)` and one `uniform_` per enabled factor).  Under the same seeds, with items taken in sequence (num_workers=0), the
+    batch equals the reference's bit for bit.  The pixels are two kernel launches per batch on the current stream, after one pinned
+    host-to-device copy of the parameters, without a device synchronisation.
+
+    `testval(indices)` gives the reference's mode='testval' items.  Not built: mode='val' (`_val_sync_transform`), which raises in every
+    reference loader because crop_size is a tuple there."""
+
+    def __init__(self, cache, base_size=1024, crop_size=None, preset="citys", brightness=None, contrast=None, saturation=None, hue=None,
+                 low=None, high=None, std=None):
+        if preset not in SEG_PRESETS:
+            raise ValueError(f"SegAugmenter: preset must be one of {sorted(SEG_PRESETS)}, got {preset!r}")
+        p = dict(SEG_PRESETS[preset])
+        for k, v in dict(brightness=brightness, contrast=contrast, saturation=saturation, hue=hue, low=low, high=high, std=std).items():
+            if v is not None:
+                p[k] = v
+        self.cache, self.base_size = cache, int(base_size)
+        crop = crop_size if crop_size is not None else p["crop_size"] or (self.base_size, self.base_size)
+        self.crop_size = (int(crop[0]), int(crop[1]))
+        self.low, self.high, self.std = p["low"], p["high"], p["std"]
+
+        def rng(v, center, clip):                        # ColorJitter._check_input for a number
+            lo, hi = center - float(v), center + float(v)
+            if clip:
+                lo = max(lo, 0.0)
+            return None if lo == hi == center else (float(lo), float(hi))
+        if not 0.0 <= float(p["hue"]) <= 0.5:
+            raise ValueError("SegAugmenter: hue must be in [0, 0.5]")
+        self.jitter_ranges = (rng(p["brightness"], 1, True), rng(p["contrast"], 1, True), rng(p["saturation"], 1, True),
+                              rng(p["hue"], 0, False))
+        self._keep = []
+
+    def draw(self, index):
+        """the random parameters of dataset[index] (mode='train'), consuming the reference's draws"""
+        h, w = self.cache.shapes[index]
+        flip = random.random() < 0.5
+        x, cum_p = range_and_prob(self.base_size, self.low, self.high, self.std)
+        long_size = random.choices(population=x, cum_weights=cum_p, k=1)[0] * 32
+        if h > w:
+            oh = long_size
+            ow = int(1.0 * w * long_size / h + 0.5)
+        else:
+            ow = long_size
+            oh = int(1.0 * h * long_size / w + 0.5)
+        cw, ch = self.crop_size
+        x1 = random.randint(0, max(ow, cw) - cw)
+        y1 = random.randint(0, max(oh, ch) - ch)
+        order = torch.randperm(4).tolist()
+        factors = [None if r is None else float(torch.empty(1).uniform_(r[0], r[1])) for r in self.jitter_ranges]
+        return dict(flip=flip, ow=int(ow), oh=int(oh), x1=x1, y1=y1, order=order, factors=factors)
+
+    @staticmethod
+    def _item(cache, index, flip, ow, oh, x1, y1, w, h, mw, mh, order, factors, tables, mask_size=None):
+        """one myolo_seg_item: the image resized to (ow, oh), the mask to `mask_size` (default (ow, oh)), both cropped at (x1, y1) to
+        (w, h) / (mw, mh); appends its tables (int32 arrays) to `tables` [(offset, array)]"""
+        H0, W0 = cache.shapes[index]
+        it = _lib.SegItem()
+        it.img, it.mask = cache.arena.data_ptr() + cache.img_off[index], cache.arena.data_ptr() + cache.mask_off[index]
+        it.H0, it.W0, it.flip = H0, W0, int(bool(flip))
+        tx, ty = _bilinear_table(W0, ow), _bilinear_table(H0, oh)
+        it.kx, it.ky = tx.shape[1] - 2, ty.shape[1] - 2
+        mow, moh = mask_size or (ow, oh)
+        parts = [_crop_rows(tx, x1, w, 0), _crop_rows(ty, y1, h, 0), _crop_rows(_nearest_index(W0, mow), x1, mw, -1),
+                 _crop_rows(_nearest_index(H0, moh), y1, mh, -1)]
+        off = tables[-1][0] + tables[-1][1].size if tables else 0
+        offs = []
+        for a in parts:
+            offs.append(off)
+            tables.append((off, a))
+            off += a.size
+        it.col, it.row, it.mcol, it.mrow = offs
+        ops = [k for k in order if factors[k] is not None]
+        it.order[:] = ops + [-1] * (4 - len(ops))
+        it.factor[:] = [0.0 if f is None else f for f in factors[:3]]
+        it.hue_shift = int(np.int32(factors[3] * 255).astype(np.uint8)) if factors[3] is not None else 0   # adjust_hue's uint8 shift
+        it.lut[:] = cache.luts[index].astype(np.int32).tolist()
+        return it
+
+    def _launch(self, items, tables, B, h, w, mh, mw, out_dtype):
+        isz = C.sizeof(_lib.SegItem)
+        n_tab = sum(a.size for _, a in tables)
+        host = torch.empty(B * isz + 4 * n_tab, dtype=torch.uint8).pin_memory()
+        C.memmove(host.data_ptr(), C.addressof(items), B * isz)
+        tab = host[B * isz:].view(torch.int32).numpy()
+        for off, a in tables:
+            tab[off:off + a.size] = a.ravel()
+        dev = host.cuda(non_blocking=True)
+        imgs = torch.empty((B, 3, h, w), dtype=out_dtype, device="cuda")
+        labels = torch.empty((B, mh, mw), dtype=torch.int64, device="cuda")
+        scratch = torch.empty(B * h * w * 3, dtype=torch.uint8, device="cuda")
+        _lib.check(_lib.lib().myolo_augment_seg(C.c_void_p(dev.data_ptr()), B, h, w, mh, mw, C.c_void_p(dev.data_ptr() + B * isz),
+                                                _lib.ptr(scratch), _lib.ptr(imgs), _lib.torch_dtype_code(out_dtype), _lib.ptr(labels),
+                                                _lib.stream_ptr()))
+        self._keep = [host, dev, scratch]
+        return imgs, labels
+
+    def build(self, indices, params, out_dtype=torch.float32):
+        """the batch of `indices` from drawn (or chosen) parameters, one dict per item as `draw` returns them"""
+        if out_dtype not in (torch.uint8, torch.float16, torch.float32):
+            raise ValueError(f"SegAugmenter: out_dtype must be uint8, float16 or float32, got {out_dtype}")
+        cw, ch = self.crop_size
+        B = len(indices)
+        items, tables = (_lib.SegItem * B)(), []
+        for b, (i, p) in enumerate(zip(indices, params)):
+            ow, oh, x1, y1 = int(p["ow"]), int(p["oh"]), int(p["x1"]), int(p["y1"])
+            if ow <= 0 or oh <= 0 or not 0 <= x1 <= max(ow, cw) - cw or not 0 <= y1 <= max(oh, ch) - ch:
+                raise ValueError(f"SegAugmenter: item {b}: crop ({x1}, {y1}) of {cw}x{ch} outside the padded {ow}x{oh} image")
+            items[b] = self._item(self.cache, i, p["flip"], ow, oh, x1, y1, cw, ch, cw, ch, p["order"], p["factors"], tables)
+        return self._launch(items, tables, B, ch, cw, ch, cw, out_dtype)
+
+    def __call__(self, indices, out_dtype=torch.float32):
+        """one mode='train' batch: (images (B, 3, h, w) of out_dtype, labels (B, h, w) int64) on the current CUDA device / stream"""
+        params = [self.draw(i) for i in indices]
+        return self.build(indices, params, out_dtype)
+
+    def testval(self, indices, out_dtype=torch.float32):
+        """mode='testval' items (`_testval_img_transform` + ToTensor, `_mask_transform` at native size): (images (B, 3, oh, ow), labels
+        (B, H, W) int64), the long side resized to make_divisible(base_size, 32) and the short side to a multiple of 32 by Pillow's
+        bilinear resize.  The items of one call must share their source size, as default_collate requires."""
+        shapes = {self.cache.shapes[i] for i in indices}
+        if len(shapes) != 1:
+            raise ValueError(f"SegAugmenter.testval: items of one batch must share a source size, got {sorted(shapes)}")
+        H0, W0 = shapes.pop()
+        outlong = math.ceil(self.base_size / 32) * 32
+        if W0 > H0:
+            ow, oh = outlong, math.ceil(int(1.0 * H0 * outlong / W0) / 32) * 32
+        else:
+            oh, ow = outlong, math.ceil(int(1.0 * W0 * outlong / H0) / 32) * 32
+        B = len(indices)
+        items, tables = (_lib.SegItem * B)(), []
+        for b, i in enumerate(indices):
+            items[b] = self._item(self.cache, i, False, ow, oh, 0, 0, ow, oh, W0, H0, [], [None] * 4, tables, mask_size=(W0, H0))
+        return self._launch(items, tables, B, oh, ow, H0, W0, out_dtype)
