@@ -278,6 +278,29 @@ int myolo_seg_lut_blend(const void* class_map, int map_dtype, int64_t n_pixels, 
 int myolo_seg_metrics(const void* pred, int pred_dtype, const int64_t* target, int64_t n_pixels, int n_classes, uint64_t* counters,
                       void* stream);
 
+/* ---- detection validation statistics (reference test.py:175,183-265 and utils/metrics.py:24-112; multiyolov5_b200/utils/metrics.py
+ * DetectionStats) ----
+ * The stats store holds one slot per (image, NMS row): correct (uint16, bit k = IoU > iouv[k]), conf (fp32) and class (uint8), plus the
+ * image's row count, and per-class target counts (uint64[256]).
+ * myolo_det_match: one launch for a batch of B images, written to images img_base .. img_base+B-1 of the store.  dets: (B,max_det,6)
+ * NMS rows, counts: (B) int32, targets: (n_targets,6) fp32 [image, class, x, y, w, h] normalised, all device.  geom: device (B,5) fp32
+ * (h0, w0, gain, padw, padh) of each image's loader shapes; iouv: device fp32[10].  Class ids outside [0,256) or not integral set bits of
+ * *err (MYOLO_DET_ERR_*), as do more than 1024 targets in one image; the kernel never indexes out of bounds.
+ * myolo_det_ap: ap_per_class over images 0 .. n_images-1 of the store, using the lowest `ncol` (<= 16) correct bits.  px: device
+ * float64[1000] and x101: float64[101], numpy's linspace(0, 1, 1000 | 101).  Outputs, one row per class with tcount > 0 in class order:
+ * out_ap (rows, ncol), out_p / out_r (rows, 1000) float64; out_info int32[2] = {any correct bit, number of predictions}.  Predictions of
+ * one class with equal conf keep their (image, row) order.  workspace: >= myolo_det_ap_workspace_bytes(n_images, max_det, ncol). */
+#define MYOLO_DET_ERR_TARGET_CLASS 1
+#define MYOLO_DET_ERR_PRED_CLASS 2
+#define MYOLO_DET_ERR_LABELS 4
+int myolo_det_match(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H, int W,
+                    const float* geom, const float* iouv, int img_base, uint16_t* st_correct, float* st_conf, uint8_t* st_cls,
+                    int32_t* st_rows, uint64_t* tcount, int32_t* err, void* stream);
+int64_t myolo_det_ap_workspace_bytes(int n_images, int max_det, int ncol);
+int myolo_det_ap(const uint16_t* correct, const float* conf, const uint8_t* cls, const int32_t* rows, int n_images, int max_det, int ncol,
+                 const uint64_t* tcount, const double* px, const double* x101, double* out_ap, double* out_p, double* out_r,
+                 int32_t* out_info, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- post-process ---- */
 /* utils.general.non_max_suppression (reference utils/general.py:421-509).  pred: (B,A,no) fp32.
  * out: (B,max_det,6) fp32 rows [x1,y1,x2,y2,conf,cls] in the reference's order; out_count: (B) int32.

@@ -43,6 +43,15 @@ int launch_augment_det(const myolo_aug_item* items, int B, int S, void* out, int
 int launch_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int mw, const int* tables, unsigned char* scratch, void* out,
                        int out_dtype, long long* out_mask, cudaStream_t s);
 
+// detection validation statistics (metrics.cu): per-batch matching into the stats store, ap_per_class over the whole store
+int launch_det_match(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H, int W,
+                     const float* geom, const float* iouv, int img_base, uint16_t* st_correct, float* st_conf, uint8_t* st_cls,
+                     int32_t* st_rows, unsigned long long* tcount, int32_t* err, cudaStream_t s);
+int64_t det_ap_workspace_bytes(int n_images, int max_det, int ncol);
+int launch_det_ap(const uint16_t* correct, const float* conf, const uint8_t* cls, const int32_t* rows, int n_images, int max_det, int ncol,
+                  const unsigned long long* tcount, const double* px, const double* x101, double* out_ap, double* out_p, double* out_r,
+                  int32_t* out_info, void* workspace, int64_t workspace_bytes, cudaStream_t s);
+
 // seg output consumers (consumers.cu)
 int launch_lut_blend(const void* idx, int idx_dtype, long n, const unsigned char* lut, int n_entries, int ch, int reverse, unsigned char* out,
                      const unsigned char* im, float alpha, float beta, unsigned char* blend, cudaStream_t s);

@@ -1370,6 +1370,28 @@ extern "C" int myolo_seg_metrics(const void* pred, int pred_dtype, const int64_t
                          reinterpret_cast<unsigned long long*>(counters), (cudaStream_t)stream);
 }
 
+extern "C" int myolo_det_match(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H, int W,
+                               const float* geom, const float* iouv, int img_base, uint16_t* st_correct, float* st_conf, uint8_t* st_cls,
+                               int32_t* st_rows, uint64_t* tcount, int32_t* err, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_det_match(dets, counts, B, max_det, targets, n_targets, H, W, geom, iouv, img_base, st_correct, st_conf, st_cls, st_rows,
+                          reinterpret_cast<unsigned long long*>(tcount), err, (cudaStream_t)stream);
+}
+
+extern "C" int64_t myolo_det_ap_workspace_bytes(int n_images, int max_det, int ncol) {
+  return det_ap_workspace_bytes(n_images, max_det, ncol);
+}
+
+extern "C" int myolo_det_ap(const uint16_t* correct, const float* conf, const uint8_t* cls, const int32_t* rows, int n_images, int max_det,
+                            int ncol, const uint64_t* tcount, const double* px, const double* x101, double* out_ap, double* out_p,
+                            double* out_r, int32_t* out_info, void* workspace, int64_t workspace_bytes, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_det_ap(correct, conf, cls, rows, n_images, max_det, ncol, reinterpret_cast<const unsigned long long*>(tcount), px, x101,
+                       out_ap, out_p, out_r, out_info, workspace, workspace_bytes, (cudaStream_t)stream);
+}
+
 extern "C" int myolo_conv_wgrad(const void* x, const void* dy, int B, int H, int W, int ci, int co, int k, int stride, int dil, float* dW,
                                 int path, void* stream) {
   MYOLO_REQUIRE(x && dy && dW && B > 0 && (k == 1 || k == 3) && (stride == 1 || stride == 2), "conv_wgrad: bad arguments");
