@@ -237,6 +237,12 @@ typedef struct {
 } myolo_aug_item;
 
 int myolo_resize_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream);
+
+/* myolo_resize_area_u8: cv2.resize(src, (W, H), INTER_AREA) of one uint8 HWC image (H0,W0,3) into dst (H,W,3), bit exact with OpenCV's
+ * 8-bit path: `load_image`'s augment=False cache resize when it shrinks (validation, :639).  Down-scaling only: H > H0 or W > W0 is
+ * MYOLO_E_INVALID.  cv2's choice of path: a copy at equal size, the 2x2 mean at exact 2x, the integer block sum times the float
+ * reciprocal of its area at other integral scales, else the general float32 area-weight arithmetic. */
+int myolo_resize_area_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream);
 int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, void* stream);
 
 /* ---- segmentation training batches (reference SegmentationDataset.py:118-151 `_sync_transform` + ColorJitter + ToTensor, and the

@@ -1,5 +1,5 @@
 // Detection training batches on the device (reference utils/datasets.py:518-593 `LoadImagesAndLabels.__getitem__` with augment=True):
-// the image cache resize of `load_image` (:629-643), and ONE fused kernel per batch for the 4-image mosaic (:671-724), the affine
+// the image cache resize of `load_image` (:629-643; INTER_LINEAR, and INTER_AREA for the augment=False cache), and ONE fused kernel per batch for the 4-image mosaic (:671-724), the affine
 // `random_perspective` warp (:851-893), mixup (:529-532), `augment_hsv` (:646-657), the flips (:571-582) and BGR->RGB / HWC->CHW (:589).
 // The host draws the random parameters and transforms the labels (multiyolov5_b200/utils/datasets.py DetAugmenter); this file only moves
 // pixels.  Every step is bit exact with OpenCV 8-bit arithmetic:
@@ -32,6 +32,27 @@ int launch_resize_u8(const unsigned char* src, int H0, int W0, unsigned char* ds
   MYOLO_REQUIRE(src && dst && H0 > 0 && W0 > 0 && H > 0 && W > 0, "resize_u8: bad geometry (src %dx%d dst %dx%d)", W0, H0, W, H);
   const long total = (long)H * W;
   resize_u8_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(src, resize_geom(H0, W0, H, W), dst, H, W);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+// load_image's augment=False cache resize: cv2.INTER_AREA whenever the image shrinks
+__global__ void resize_area_u8_kernel(const unsigned char* __restrict__ src, AreaGeom g, unsigned char* __restrict__ dst, int H, int W) {
+  const long total = (long)H * W;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    int v[3];
+    resize_area_pixel_u8(src, g, (int)(i % W), (int)(i / W), v);
+    dst[i * 3 + 0] = (unsigned char)v[0];
+    dst[i * 3 + 1] = (unsigned char)v[1];
+    dst[i * 3 + 2] = (unsigned char)v[2];
+  }
+}
+
+int launch_resize_area_u8(const unsigned char* src, int H0, int W0, unsigned char* dst, int H, int W, cudaStream_t s) {
+  MYOLO_REQUIRE(src && dst && H0 > 0 && W0 > 0 && H > 0 && W > 0, "resize_area_u8: bad geometry (src %dx%d dst %dx%d)", W0, H0, W, H);
+  MYOLO_REQUIRE(H <= H0 && W <= W0, "resize_area_u8: down-scaling only (src %dx%d dst %dx%d)", W0, H0, W, H);
+  const long total = (long)H * W;
+  resize_area_u8_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(src, area_geom(H0, W0, H, W), dst, H, W);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }

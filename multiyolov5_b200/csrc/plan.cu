@@ -1340,6 +1340,12 @@ extern "C" int myolo_resize_u8(const uint8_t* src, int H0, int W0, uint8_t* dst,
   return launch_resize_u8(src, H0, W0, dst, H, W, (cudaStream_t)stream);
 }
 
+extern "C" int myolo_resize_area_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_resize_area_u8(src, H0, W0, dst, H, W, (cudaStream_t)stream);
+}
+
 extern "C" int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, void* stream) {
   int rc = check_device(nullptr);
   if (rc) return rc;

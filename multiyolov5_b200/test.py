@@ -4,6 +4,10 @@ matching launch (utils.metrics.DetectionStats), with no host synchronisation; ap
 
 The reference validates in fp16 on CUDA (its z, NMS rows and box_iou are half tensors); this model keeps z in fp32, so the statistics
 equal the reference's fp32 statistics of the same predictions, which is what its test() computes on a CPU device.
+
+The batches can come from the device as well: `test(data, model=m, dataloader=DetValLoader(cache, 32), plots=False)` with
+`cache = utils.datasets.DeviceImageCache(frames, imgsz, labels, augment=False)` is the reference's rect validation loader of
+train.py:207-210 (`create_dataloader(..., rect=True, pad=0.5)`), bit exact with it.
 """
 from pathlib import Path
 

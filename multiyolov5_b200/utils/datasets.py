@@ -3,6 +3,8 @@
     letterbox(img, new_shape, color, auto, scaleFill, scaleup, stride) -> (img, ratio, (dw, dh))     reference utils/datasets.py:818-848
     preprocess(img0, img_size, stride, half)  -> (1|B,3,H,W) float tensor in [0,1]                     :185-189 + detect.py:135-137
     DeviceImageCache(images, img_size, labels) / DetAugmenter(cache, hyp)(indices) -> (imgs, targets)   :518-599 (augment=True)
+    DeviceImageCache(images, img_size, labels, augment=False) / DetValLoader(cache, batch_size) -> iterable of (imgs, targets, paths,
+        shapes) for test(data, model=m, dataloader=DetValLoader(cache, 32))                          :347-452 + :518-599 (rect=True)
     DeviceSegCache(images, masks, mask_map) / SegAugmenter(cache, base_size, crop_size, preset)(indices) -> (segimgs, segtargets)
                                                                              SegmentationDataset.py:118-151 + ColorJitter + ToTensor
 
@@ -107,16 +109,17 @@ def _xyxy2xywh(x):                      # reference utils/general.py:255-262 (nu
 
 class DeviceImageCache:
     """The reference's `cache_images` on the device: each decoded uint8 HWC BGR frame is resized so that its long side is `img_size`
-    (`load_image`, cv2.resize INTER_LINEAR as with augment=True; exact 2x down-scaling takes OpenCV's area path) by a bit-exact kernel and
-    kept in ONE device arena (`offsets` / `shapes` index it).  `labels[i]`: (n, 5) [class, x, y, w, h] normalised, stored as float32 like
-    the reference's label cache.  Decoding (cv2.imread) stays with the caller."""
+    (`load_image`) by a bit-exact kernel and kept in ONE device arena (`offsets` / `shapes` index it).  `augment` is the dataset's flag:
+    True (training) resizes with cv2.resize INTER_LINEAR (exact 2x down-scaling takes OpenCV's area path); False (validation) shrinks with
+    INTER_AREA and grows with INTER_LINEAR, as load_image does.  `labels[i]`: (n, 5) [class, x, y, w, h] normalised, stored as float32
+    like the reference's label cache.  Decoding (cv2.imread) stays with the caller."""
 
-    def __init__(self, images, img_size, labels=None, segments=None):
+    def __init__(self, images, img_size, labels=None, segments=None, augment=True):
         if segments is not None and any(len(s) for s in segments):
             raise NotImplementedError("DeviceImageCache: polygon label segments are not supported (boxes only)")
         if not torch.cuda.is_available():
             raise _lib.MyoloError("DeviceImageCache needs a CUDA device: multiyolov5_b200 has no CPU path")
-        self.img_size, self.n = int(img_size), len(images)
+        self.img_size, self.n, self.augment = int(img_size), len(images), bool(augment)
         self.shapes0, self.shapes, self.offsets = [], [], []
         total = 0
         for im in images:
@@ -130,7 +133,9 @@ class DeviceImageCache:
         L, sp = _lib.lib(), _lib.stream_ptr()
         for im, (h0, w0), (h, w), off in zip(images, self.shapes0, self.shapes, self.offsets):
             src = _as_device_frames(im)
-            _lib.check(L.myolo_resize_u8(_lib.ptr(src), h0, w0, C.c_void_p(self.arena.data_ptr() + off), h, w, sp))
+            shrink = not self.augment and self.img_size < max(h0, w0)         # load_image: INTER_AREA if r < 1 and not augment
+            resize = L.myolo_resize_area_u8 if shrink else L.myolo_resize_u8
+            _lib.check(resize(_lib.ptr(src), h0, w0, C.c_void_p(self.arena.data_ptr() + off), h, w, sp))
         self.labels = [np.array(l, dtype=np.float32).reshape(-1, 5) for l in labels] if labels is not None else \
             [np.zeros((0, 5), np.float32) for _ in range(self.n)]
         assert len(self.labels) == self.n
@@ -333,6 +338,106 @@ class DetAugmenter:
         targets = torch.cat(targets, 0).pin_memory().cuda(non_blocking=True)
         self._keep = [dev_items] + self._keep
         return imgs, targets
+
+
+# ------------------------------------------------------------------------------------------------
+# detection validation batches (reference utils/datasets.py:347-452 + :518-599 LoadImagesAndLabels(augment=False, rect=True) + collate_fn,
+# as create_dataloader builds it for test(): train.py:207-210)
+# ------------------------------------------------------------------------------------------------
+class ValBatch:
+    """one rect validation batch planned on the host: source indices, letterbox geometry per item ((new_w, new_h), ratio, (dw, dh),
+    (top, bottom, left, right)), the (n, 6) float32 targets and collate_fn's `shapes` tuple"""
+
+    def __init__(self, indices, geoms, targets, shapes):
+        self.indices, self.geoms, self.targets, self.shapes = indices, geoms, targets, shapes
+
+
+def det_val_plan(shapes0, shapes, labels, img_size, batch_size, stride=32, pad=0.5, single_cls=False):
+    """The host arithmetic of the reference's rect validation dataset over cached images, in its statements and dtypes: `shapes0` are the
+    original (h0, w0), `shapes` the cached (h, w), `labels` (n, 5) float32 normalised [class, x, y, w, h].  Returns (order, batch_shapes,
+    [ValBatch]): `order` is the aspect-ratio sort (numpy's default argsort kind, as the reference: not stable, so the order of equal
+    aspect ratios depends on the host CPU), `batch_shapes` the (nb, 2) [h, w] int letterbox shapes."""
+    n = len(shapes0)
+    if n == 0:
+        raise ValueError("det_val_plan: no images")
+    s = np.array([(w0, h0) for h0, w0 in shapes0], dtype=np.float64)         # the reference's self.shapes: wh
+    ar = s[:, 1] / s[:, 0]
+    order = ar.argsort()
+    ar = ar[order]
+    bi = np.floor(np.arange(n) / batch_size).astype(int)
+    nb = bi[-1] + 1
+    bshapes = [[1, 1]] * nb
+    for i in range(nb):
+        ari = ar[bi == i]
+        mini, maxi = ari.min(), ari.max()
+        if maxi < 1:
+            bshapes[i] = [maxi, 1]
+        elif mini > 1:
+            bshapes[i] = [1, 1 / mini]
+    batch_shapes = np.ceil(np.array(bshapes) * img_size / stride + pad).astype(int) * stride
+    batches = []
+    for b in range(nb):
+        shape = batch_shapes[b]                  # a numpy row, as the reference passes it: ratio and pad come out as numpy float64
+        indices, geoms, targets, shp = [], [], [], []
+        for pos, j in enumerate(np.flatnonzero(bi == b)):
+            index = int(order[j])
+            (h0, w0), (h, w) = shapes0[index], shapes[index]
+            geom = letterbox_geometry((h, w), shape, auto=False, scaleup=False)
+            ratio, pd = geom[1], geom[2]
+            lab = np.array(labels[index], dtype=np.float32).reshape(-1, 5)
+            if single_cls:
+                lab[:, 0] = 0
+            if lab.size:
+                lab[:, 1:] = _xywhn2xyxy(lab[:, 1:], ratio[0] * w, ratio[1] * h, pd[0], pd[1])
+            nL = len(lab)
+            if nL:
+                lab[:, 1:5] = _xyxy2xywh(lab[:, 1:5])
+                lab[:, [2, 4]] /= int(shape[0])
+                lab[:, [1, 3]] /= int(shape[1])
+            t = np.zeros((nL, 6), np.float32)
+            t[:, 0] = pos
+            t[:, 1:] = lab
+            indices.append(index)
+            geoms.append(geom)
+            targets.append(t)
+            shp.append(((h0, w0), ((h / h0, w / w0), pd)))
+        batches.append(ValBatch(tuple(indices), geoms, np.concatenate(targets, 0), tuple(shp)))
+    return order, batch_shapes, batches
+
+
+class DetValLoader:
+    """Detection validation batches on the device: the reference's `create_dataloader(path, imgsz, batch_size, gs, opt, rect=True,
+    pad=pad)` (a LoadImagesAndLabels with augment=False, rect=True, and collate_fn) over a DeviceImageCache built with augment=False.
+    Feeds `test.test(data, model=m, dataloader=DetValLoader(cache, 32))`; `batch_size` is the dataset's (train.py passes batch_size * 2).
+
+    Iterating yields one (img uint8 (B, 3, H, W) RGB, targets (n, 6) float32, paths, shapes) per batch in loader order, images and
+    targets on the device; `paths` are the source indices and `shapes` collate_fn's ((h0, w0), ((h / h0, w / w0), (dw, dh))) per item.
+    The order, batch shapes, letterbox geometry and labels are planned once at construction (det_val_plan) and every batch's targets
+    uploaded once: the batches are deterministic, so iterating does no label work and no host-to-device copy.  Each item is one
+    myolo_letterbox launch (114 border, BGR -> RGB, CHW) into its slice of the batch, on the current stream, without a synchronisation."""
+
+    def __init__(self, cache, batch_size, stride=32, pad=0.5, single_cls=False):
+        if cache.augment:
+            raise ValueError("DetValLoader: the cache must be built with augment=False (load_image's INTER_AREA validation resize)")
+        self.cache, self.batch_size, self.stride, self.pad = cache, int(batch_size), int(stride), pad
+        self.order, self.batch_shapes, self.batches = det_val_plan(cache.shapes0, cache.shapes, cache.labels, cache.img_size,
+                                                                   self.batch_size, self.stride, pad, single_cls)
+        self.targets = [torch.from_numpy(b.targets).cuda() for b in self.batches]
+
+    def __len__(self):
+        return len(self.batches)
+
+    def __iter__(self):
+        L, sp, cache = _lib.lib(), _lib.stream_ptr(), self.cache
+        color = (C.c_int32 * 3)(114, 114, 114)
+        for (H, W), batch, targets in zip(self.batch_shapes.tolist(), self.batches, self.targets):
+            imgs = torch.empty((len(batch.indices), 3, H, W), dtype=torch.uint8, device="cuda")
+            for k, (i, geom) in enumerate(zip(batch.indices, batch.geoms)):
+                (rw, rh), _, _, (top, _, left, _) = geom
+                h, w = cache.shapes[i]
+                _lib.check(L.myolo_letterbox(C.c_void_p(cache.ptr(i)), 1, h, w, rw, rh, top, left, H, W, color,
+                                             C.c_void_p(imgs.data_ptr() + k * 3 * H * W), _lib.U8, 1, 1, sp))
+            yield imgs, targets, batch.indices, batch.shapes
 
 
 # ------------------------------------------------------------------------------------------------
