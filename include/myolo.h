@@ -111,6 +111,19 @@ int myolo_device_info(char* name, int* sm_count, int* cc_major, int* cc_minor);
 int myolo_plan_create(const myolo_op* ops, int n_ops, const myolo_buf_desc* bufs, int n_bufs,
                       const int32_t* extra, int n_extra, /* variable-length tables referenced by aux[] */
                       int B, int H, int W, int64_t workspace_bytes, int n_weight_slots, myolo_plan** out);
+/* Like myolo_plan_create, but the plan binds to caller-owned activation / gradient workspaces `ws` / `gws` of `capacity` bytes each
+ * (256-byte aligned) instead of allocating private ones: train plans of several input shapes that run one after another on one stream
+ * (--multi-scale, reference train.py:354-359) share one pair sized for the largest.  MYOLO_E_INVALID when workspace_bytes > capacity.
+ * The addresses are baked into the plan's tensor maps and captured graphs: they must stay valid, at the same address, for the plan's life.
+ * The caller zeroes `ws` before the plan's first forward and again whenever another plan has written it since (the plan reads some
+ * never-written bytes, e.g. zero-padded channels, as zeros).  myolo_plan_destroy never frees them.
+ * The library does not track which plan wrote the shared workspaces last: a backward (myolo_plan_backward*, myolo_plan_backward_seg_ce)
+ * after ANOTHER plan's train forward on the same pair reads that plan's activations as its own and returns wrong gradients without an
+ * error.  The caller keeps one outstanding train forward per pair: forward, backward, then the next plan's forward (the Python engine
+ * refuses such a stale backward before it launches). */
+int myolo_plan_create_shared(const myolo_op* ops, int n_ops, const myolo_buf_desc* bufs, int n_bufs, const int32_t* extra, int n_extra,
+                             int B, int H, int W, int64_t workspace_bytes, int n_weight_slots, void* ws, void* gws, int64_t capacity,
+                             myolo_plan** out);
 void myolo_plan_destroy(myolo_plan* plan);
 /* folds BN (eval: w' = w*g/sqrt(var+eps), b' = beta - g*mean/sqrt(var+eps); reference utils/torch_utils.py:182-202),
  * converts to fp16 and packs [Co][Ci][k][k] fp32 -> [Co_pad][k*k][Ci_pad].  gamma..var / bias may be NULL. */
@@ -243,6 +256,12 @@ int myolo_resize_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int
  * MYOLO_E_INVALID.  cv2's choice of path: a copy at equal size, the 2x2 mean at exact 2x, the integer block sum times the float
  * reciprocal of its area at other integral scales, else the general float32 area-weight arithmetic. */
 int myolo_resize_area_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream);
+
+/* myolo_resize_bilinear: the det batch rescale of --multi-scale (reference train.py:354-359), F.interpolate(x, (Ho, Wo), mode='bilinear',
+ * align_corners=False) of NCHW src (B,C,H,W) into NCHW dst (B,C,Ho,Wo), bit exact with torch's CUDA kernel on fp32 input.  src_dtype
+ * MYOLO_U8 (each tap converted as imgs.float() / 255.0 converts it on the device: v * fp32(1/255)), MYOLO_F16 or MYOLO_F32; dst_dtype
+ * MYOLO_F16 (the fp32 result rounded to nearest) or MYOLO_F32.  Equal sizes convert only. */
+int myolo_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo, void* stream);
 int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, void* stream);
 
 /* ---- segmentation training batches (reference SegmentationDataset.py:118-151 `_sync_transform` + ColorJitter + ToTensor, and the

@@ -161,4 +161,86 @@ int launch_augment_det(const myolo_aug_item* items, int B, int S, void* out, int
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// --multi-scale (reference train.py:354-359): F.interpolate(imgs, size=ns, mode='bilinear', align_corners=False) of the det batch, bit
+// exact with ATen's CUDA kernel (UpSampleBilinear2d.cu upsample_bilinear2d_out_frame).  The host passes ATen's scales, float(in) / out.
+// ATen's expressions with nvcc's contractions as they appear in the sm_90 SASS of the kernel torch launches:
+//   src  = fma(dst + 0.5, scale, -0.5), clamped at 0 (area_pixel_compute_source_index);  i1 = trunc(src);  l1 = src - i1;  l0 = 1 - l1
+//   val  = fma(h0l, fma(w0l, a, w1l * b), h1l * fma(w0l, c, w1l * d))      a..d: taps (h1,w1) (h1,w1+w1p) (h1+h1p,w1) (h1+h1p,w1+w1p)
+// uint8 taps are first converted as `imgs.float() / 255.0` converts them on the device (train.py:342): v * fp32(1/255).
+// ------------------------------------------------------------------------------------------------
+template <typename T>
+__device__ __forceinline__ float bilinear_tap(const T* p);
+template <>
+__device__ __forceinline__ float bilinear_tap<unsigned char>(const unsigned char* p) { return __fmul_rn((float)__ldg(p), 1.0f / 255.0f); }
+template <>
+__device__ __forceinline__ float bilinear_tap<__half>(const __half* p) { return __half2float(__ldg(p)); }
+template <>
+__device__ __forceinline__ float bilinear_tap<float>(const float* p) { return __ldg(p); }
+
+__device__ __forceinline__ void bilinear_source(int d, int n_in, float scale, int* i0, int* i1, float* l0, float* l1) {
+  float src = __fmaf_rn(__fadd_rn((float)d, 0.5f), scale, -0.5f);
+  src = src < 0.f ? 0.f : src;
+  const int i = (int)src;
+  *i0 = i;
+  *i1 = i + (i < n_in - 1 ? 1 : 0);
+  *l1 = __fsub_rn(src, (float)i);
+  *l0 = __fsub_rn(1.0f, *l1);
+}
+
+// one thread per output pixel of one (image, channel) plane; grid (x tiles, rows, planes)
+template <typename Ts, typename Td>
+__global__ void __launch_bounds__(128) resize_bilinear_kernel(const Ts* __restrict__ src, int planes, int H, int W, Td* __restrict__ dst,
+                                                              int Ho, int Wo, float rh, float rw) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  if (x >= Wo) return;
+  const bool same = H == Ho && W == Wo;      // scale 1: the conversion alone
+  int h0 = y, h1 = y, w0 = x, w1 = x;
+  float h0l = 1.f, h1l = 0.f, w0l = 1.f, w1l = 0.f;
+  if (!same) {
+    bilinear_source(y, H, rh, &h0, &h1, &h0l, &h1l);
+    bilinear_source(x, W, rw, &w0, &w1, &w0l, &w1l);
+  }
+  for (int p = blockIdx.z; p < planes; p += gridDim.z) {
+    const Ts* s = src + (size_t)p * H * W;
+    float val;
+    if (same) {
+      val = bilinear_tap(s + (size_t)y * W + x);
+    } else {
+      const float a = bilinear_tap(s + (size_t)h0 * W + w0), b = bilinear_tap(s + (size_t)h0 * W + w1);
+      const float c = bilinear_tap(s + (size_t)h1 * W + w0), d = bilinear_tap(s + (size_t)h1 * W + w1);
+      const float top = __fmaf_rn(w0l, a, __fmul_rn(w1l, b));
+      const float bot = __fmaf_rn(w0l, c, __fmul_rn(w1l, d));
+      val = __fmaf_rn(h0l, top, __fmul_rn(h1l, bot));
+    }
+    const size_t o = ((size_t)p * Ho + y) * Wo + x;
+    if constexpr (sizeof(Td) == 2) dst[o] = __float2half_rn(val);
+    else dst[o] = val;
+  }
+}
+
+template <typename Ts>
+static void launch_resize_bilinear_from(const Ts* src, int planes, int H, int W, void* dst, int dst_dtype, int Ho, int Wo, float rh, float rw,
+                                        cudaStream_t s) {
+  const dim3 grid((Wo + 127) / 128, Ho, std::min(planes, 65535));
+  if (dst_dtype == MYOLO_F16) resize_bilinear_kernel<Ts, __half><<<grid, 128, 0, s>>>(src, planes, H, W, (__half*)dst, Ho, Wo, rh, rw);
+  else resize_bilinear_kernel<Ts, float><<<grid, 128, 0, s>>>(src, planes, H, W, (float*)dst, Ho, Wo, rh, rw);
+}
+
+int launch_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo, cudaStream_t s) {
+  MYOLO_REQUIRE(src && dst && B > 0 && C > 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0 && Ho <= 65535,
+                "resize_bilinear: bad geometry (B %d C %d src %dx%d dst %dx%d)", B, C, H, W, Ho, Wo);
+  MYOLO_REQUIRE(src_dtype == MYOLO_U8 || src_dtype == MYOLO_F16 || src_dtype == MYOLO_F32, "resize_bilinear: source dtype %d", src_dtype);
+  MYOLO_REQUIRE(dst_dtype == MYOLO_F16 || dst_dtype == MYOLO_F32, "resize_bilinear: output dtype %d", dst_dtype);
+  MYOLO_REQUIRE((long)B * C <= (1L << 31) - 1, "resize_bilinear: too many planes");
+  const int planes = B * C;
+  // area_pixel_compute_scale with no scale factor given: static_cast<float>(input_size) / output_size, in fp32 on the host
+  const float rh = (float)H / (float)Ho, rw = (float)W / (float)Wo;
+  if (src_dtype == MYOLO_U8) launch_resize_bilinear_from((const unsigned char*)src, planes, H, W, dst, dst_dtype, Ho, Wo, rh, rw, s);
+  else if (src_dtype == MYOLO_F16) launch_resize_bilinear_from((const __half*)src, planes, H, W, dst, dst_dtype, Ho, Wo, rh, rw, s);
+  else launch_resize_bilinear_from((const float*)src, planes, H, W, dst, dst_dtype, Ho, Wo, rh, rw, s);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace myolo

@@ -88,6 +88,7 @@ struct myolo_plan {
   int32_t* d_extra = nullptr;
   unsigned char* ws = nullptr;
   int64_t ws_bytes = 0;
+  bool owns_ws = true;            // false: ws / gws belong to the caller (myolo_plan_create_shared) and are never freed here
   std::vector<WeightSlot> slots;
   std::vector<ConvOp> convs;      // parallel to ops (valid for CONV ops)
   std::vector<int> conv_ready;    // tensor maps built
@@ -173,9 +174,22 @@ extern "C" int myolo_device_info(char* name, int* sm_count, int* cc_major, int* 
   return 0;
 }
 
-extern "C" int myolo_plan_create(const myolo_op* ops, int n_ops, const myolo_buf_desc* bufs, int n_bufs, const int32_t* extra,
-                                 int n_extra, int B, int H, int W, int64_t workspace_bytes, int n_weight_slots, myolo_plan** out) {
+// shared_ws / shared_gws: caller-owned activation / gradient workspaces of shared_capacity bytes each (myolo_plan_create_shared), or
+// null: the plan allocates (and frees) private ones
+static int plan_create(const myolo_op* ops, int n_ops, const myolo_buf_desc* bufs, int n_bufs, const int32_t* extra, int n_extra, int B,
+                       int H, int W, int64_t workspace_bytes, int n_weight_slots, void* shared_ws, void* shared_gws,
+                       int64_t shared_capacity, myolo_plan** out) {
   MYOLO_REQUIRE(ops && bufs && out && n_ops > 0 && n_bufs > 0 && B > 0 && H > 0 && W > 0, "plan_create: bad arguments");
+  const bool shared = shared_ws != nullptr;
+  if (shared) {
+    MYOLO_REQUIRE(shared_gws && shared_capacity > 0, "plan_create_shared: null gradient workspace / capacity %lld",
+                  (long long)shared_capacity);
+    MYOLO_REQUIRE(reinterpret_cast<uintptr_t>(shared_ws) % 256 == 0 && reinterpret_cast<uintptr_t>(shared_gws) % 256 == 0,
+                  "plan_create_shared: workspaces must be 256-byte aligned");
+    MYOLO_REQUIRE(workspace_bytes > 0 && workspace_bytes <= shared_capacity,
+                  "plan_create_shared: the plan needs %lld workspace bytes, the shared workspaces hold %lld", (long long)workspace_bytes,
+                  (long long)shared_capacity);
+  }
   int sms = 0;
   int rc = check_device(&sms);
   if (rc) return rc;
@@ -204,15 +218,22 @@ extern "C" int myolo_plan_create(const myolo_op* ops, int n_ops, const myolo_buf
       return MYOLO_E_INVALID;
     }
   }
-  cudaError_t e = cudaMalloc(&pl->ws, workspace_bytes);
-  if (e == cudaSuccess) e = cudaMemset(pl->ws, 0, workspace_bytes);
+  cudaError_t e = cudaSuccess;
+  if (shared) {              // the caller zeroes its workspaces (and re-zeroes them when another plan has written them)
+    pl->ws = static_cast<unsigned char*>(shared_ws);
+    pl->gws = static_cast<unsigned char*>(shared_gws);
+    pl->owns_ws = false;
+  } else {
+    e = cudaMalloc(&pl->ws, workspace_bytes);
+    if (e == cudaSuccess) e = cudaMemset(pl->ws, 0, workspace_bytes);
+  }
   if (e == cudaSuccess && n_extra > 0) {
     e = cudaMalloc(&pl->d_extra, (size_t)n_extra * 4);
     if (e == cudaSuccess) e = cudaMemcpy(pl->d_extra, extra, (size_t)n_extra * 4, cudaMemcpyHostToDevice);
   }
   if (e != cudaSuccess) {
     set_error("plan_create: device allocation failed: %s", cudaGetErrorString(e));
-    if (pl->ws) cudaFree(pl->ws);
+    if (pl->ws && pl->owns_ws) cudaFree(pl->ws);
     if (pl->d_extra) cudaFree(pl->d_extra);
     delete pl;
     return MYOLO_E_CUDA;
@@ -222,13 +243,25 @@ extern "C" int myolo_plan_create(const myolo_op* ops, int n_ops, const myolo_buf
   return 0;
 }
 
+extern "C" int myolo_plan_create(const myolo_op* ops, int n_ops, const myolo_buf_desc* bufs, int n_bufs, const int32_t* extra,
+                                 int n_extra, int B, int H, int W, int64_t workspace_bytes, int n_weight_slots, myolo_plan** out) {
+  return plan_create(ops, n_ops, bufs, n_bufs, extra, n_extra, B, H, W, workspace_bytes, n_weight_slots, nullptr, nullptr, 0, out);
+}
+
+extern "C" int myolo_plan_create_shared(const myolo_op* ops, int n_ops, const myolo_buf_desc* bufs, int n_bufs, const int32_t* extra,
+                                        int n_extra, int B, int H, int W, int64_t workspace_bytes, int n_weight_slots, void* ws, void* gws,
+                                        int64_t capacity, myolo_plan** out) {
+  MYOLO_REQUIRE(ws, "plan_create_shared: null activation workspace");
+  return plan_create(ops, n_ops, bufs, n_bufs, extra, n_extra, B, H, W, workspace_bytes, n_weight_slots, ws, gws, capacity, out);
+}
+
 extern "C" void myolo_plan_destroy(myolo_plan* pl) {
   if (!pl) return;
   for (auto& s : pl->slots) {
     if (s.w) cudaFree(s.w);
     if (s.bias) cudaFree(s.bias);
   }
-  if (pl->ws) cudaFree(pl->ws);
+  if (pl->ws && pl->owns_ws) cudaFree(pl->ws);
   if (pl->d_extra) cudaFree(pl->d_extra);
   if (pl->decode_stream) cudaStreamDestroy(pl->decode_stream);
   if (pl->d_pack_jobs) cudaFree(pl->d_pack_jobs);
@@ -245,7 +278,7 @@ extern "C" void myolo_plan_destroy(myolo_plan* pl) {
     if (sl.zero_bias) cudaFree(sl.zero_bias);
   }
   for (auto p : pl->bn_stats) if (p) cudaFree(p);
-  if (pl->gws) cudaFree(pl->gws);
+  if (pl->gws && pl->owns_ws) cudaFree(pl->gws);
   for (auto& sl : pl->slots) if (sl.dw_packed) cudaFree(sl.dw_packed);
   if (pl->tmp16) cudaFree(pl->tmp16);
   for (auto e : pl->bwd_ev) cudaEventDestroy(e);
@@ -1350,6 +1383,13 @@ extern "C" int myolo_augment_det(const myolo_aug_item* items, int B, int S, void
   int rc = check_device(nullptr);
   if (rc) return rc;
   return launch_augment_det(items, B, S, out, out_dtype, (cudaStream_t)stream);
+}
+
+extern "C" int myolo_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo,
+                                     void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_resize_bilinear(src, src_dtype, B, C, H, W, dst, dst_dtype, Ho, Wo, (cudaStream_t)stream);
 }
 
 extern "C" int myolo_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int mw, const int32_t* tables, uint8_t* scratch,

@@ -101,7 +101,9 @@ conv_wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmDy, const __grid_cons
         __syncwarp();
         uint8_t* sa = smem + (size_t)stage * p.stage_bytes;
         if (leader) {
-          mbar_arrive_expect_tx(&full[stage], (uint32_t)(p.a_boxes * p.Kc * 128 + K * p.b_bytes));
+          // the bytes the boxes deliver: b_bytes is rounded up to the 1024-byte swizzle alignment (16 pixels x 16 channels = 512 bytes
+          // per tap, layer 0 at input widths of 64 n + 32, would otherwise leave the barrier waiting for bytes that never come)
+          mbar_arrive_expect_tx(&full[stage], (uint32_t)(p.a_boxes * p.Kc * 128 + K * p.n_boxes * p.Kc * p.bc * 2));
           tma_load_4d(sa, &tmDy, &full[stage], co0, ox0, oy, b);
           if (p.a_boxes == 2) tma_load_4d(sa + p.Kc * 128, &tmDy, &full[stage], co0 + 64, ox0, oy, b);
         }

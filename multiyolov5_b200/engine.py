@@ -10,15 +10,53 @@ from . import _lib
 from .plan import build_plan, to_ctypes
 
 
+def shared_train_plans(model, B, shapes):
+    """host train plans for batches of B images at each (H, W) of `shapes`, and the workspace capacity they need when they share one
+    (the largest of their workspaces; every buffer of every plan lies inside its own plan's workspace_bytes)"""
+    pbs = {(int(h), int(w)): build_plan(model, B, int(h), int(w), train=True) for h, w in shapes}
+    return pbs, max([int(pb.workspace_bytes) for pb in pbs.values()], default=0)
+
+
+class TrainArena:
+    """One activation workspace and one gradient workspace shared by the train plans of one lane (Engine.reserve_train_shapes).
+
+    The plans bake the workspace address into their tensor maps and captured graphs, so the pair is allocated once, at its final size,
+    before the first plan binds to it, and never moves.  Plans of one lane run one after another on one stream; `owner` is the plan whose
+    forward wrote the activations last, `generation` counts the forwards (a backward is valid only for the arena's latest forward)."""
+
+    def __init__(self, capacity, device):
+        self.capacity = int(capacity)
+        self.ws = torch.zeros(self.capacity, dtype=torch.uint8, device=device)
+        self.gws = torch.zeros(self.capacity, dtype=torch.uint8, device=device)
+        self.owner = None
+        self.generation = 0
+
+    def claim(self, plan):
+        """called before `plan`'s forward, on the stream it runs on.  A plan reads some bytes of its workspace it never writes as zeros (the
+        zero-padded input channels and the padded fp32 head channels, plan.py); another shape's plan may have written anything there, so
+        the plan's whole workspace prefix is zeroed when the arena changes hands - the state a private workspace has after creation."""
+        if self.owner is not None and self.owner is not plan:
+            self.ws[:plan.pb.workspace_bytes].zero_()
+        self.owner = plan
+        self.generation += 1
+        return self.generation
+
+
 class CompiledPlan:
-    def __init__(self, model, B, H, W, noalias=False, train=False):
+    def __init__(self, model, B, H, W, noalias=False, train=False, arena=None, pb=None):
+        """arena: a TrainArena the (train) plan binds to instead of allocating private workspaces; pb: its already-built host plan"""
         self.train = train
-        self.pb = build_plan(model, B, H, W, noalias=noalias, train=train)
+        self.pb = pb if pb is not None else build_plan(model, B, H, W, noalias=noalias, train=train)
         self.ops, self.bufs, self.extra = to_ctypes(self.pb)
+        self.arena = arena                   # keeps the shared workspaces alive as long as the plan
         L = _lib.lib()
         h = C.c_void_p()
-        _lib.check(L.myolo_plan_create(self.ops, len(self.pb.ops), self.bufs, len(self.pb.bufs), self.extra, len(self.pb.extra),
-                                       B, H, W, int(self.pb.workspace_bytes), len(self.pb.slots), C.byref(h)))
+        args = (self.ops, len(self.pb.ops), self.bufs, len(self.pb.bufs), self.extra, len(self.pb.extra), B, H, W,
+                int(self.pb.workspace_bytes), len(self.pb.slots))
+        if arena is None:
+            _lib.check(L.myolo_plan_create(*args, C.byref(h)))
+        else:
+            _lib.check(L.myolo_plan_create_shared(*args, _lib.ptr(arena.ws), _lib.ptr(arena.gws), arena.capacity, C.byref(h)))
         self.handle = h
         self.B, self.H, self.W = B, H, W
         self.weights_uploaded = False
@@ -143,8 +181,35 @@ class Engine:
         can be in flight at the same time (train.Trainer overlap_passes)"""
         key = ("train", B, H, W) if lane == 0 else ("train", B, H, W, lane)
         if key not in self.plans:
-            self.plans[key] = CompiledPlan(self.model, B, H, W, train=True)
+            arena, pb = getattr(self, "_reserved", {}).get(key, (None, None))
+            self.plans[key] = CompiledPlan(self.model, B, H, W, train=True, arena=arena, pb=pb)
         return self.plans[key]
+
+    def reserve_train_shapes(self, B, shapes, lane=0):
+        """Train plans for batches of B images at each (H, W) of `shapes` on `lane` share ONE activation and ONE gradient workspace sized
+        for the largest of them (--multi-scale, reference train.py:354-359: 33 sizes at imgsz 1024 would need ~97 GB of private
+        workspaces; the shared pair needs 6.1 GB).  Builds the host plans now, allocates and zeroes the pair once; the device plans are
+        created on first use.  A lane keeps its pair for good: more shapes may be reserved later if they fit, a larger reservation raises
+        (the existing plans bake in the address).  Returns the TrainArena."""
+        shapes = sorted({(int(h), int(w)) for h, w in shapes})
+        if not shapes:
+            raise ValueError("reserve_train_shapes: no shapes")
+        self._reserved = getattr(self, "_reserved", {})
+        self._arenas = getattr(self, "_arenas", {})
+        keys = {hw: (("train", B) + hw if lane == 0 else ("train", B) + hw + (lane,)) for hw in shapes}
+        arena = self._arenas.get(lane)
+        pbs, need = shared_train_plans(self.model, B, [hw for hw in shapes
+                                                       if arena is None or self._reserved.get(keys[hw], (None,))[0] is not arena])
+        if arena is None:
+            arena = TrainArena(need, next(self.model.parameters()).device)
+            self._arenas[lane] = arena
+        elif need > arena.capacity:
+            raise _lib.MyoloError(f"lane {lane} already has a shared train workspace of {arena.capacity} bytes and the new shapes need {need}: "
+                                  "it cannot grow under the plans bound to it; reserve every shape (the largest first) before training")
+        for hw, pb in pbs.items():
+            self.plans.pop(keys[hw], None)           # a private plan of this shape is rebuilt on the shared workspaces
+            self._reserved[keys[hw]] = (arena, pb)
+        return arena
 
     def ensure_flat_grads(self):
         """every parameter's .grad is a view into ONE flat fp32 buffer (what the data-parallel all-reduce moves, reference
@@ -231,10 +296,12 @@ class Engine:
         segs = [torch.empty((B, seg_head.c_out, H, W), dtype=torch.float32, device=x.device) if want_seg else None for _ in range(n_seg)]
         raw_ptrs = (C.c_void_p * 3)(*[_lib.ptr(r) for r in raws])
         seg_ptrs = (C.c_void_p * 3)(*[_lib.ptr(segs[k]) if k < n_seg else None for k in range(3)])
+        gen = p.arena.claim(p) if p.arena is not None else None
         _lib.check(L.myolo_plan_train_forward_multi(p.handle, _lib.ptr(x), _lib.torch_dtype_code(x.dtype), raw_ptrs, seg_ptrs, sp))
         # activations / batch statistics / dropout step of THIS forward live in the plan's single workspace: a backward is only valid
-        # for the most recent train forward of the plan (the reference's order forward, backward, forward, backward - train.py:364-392)
-        p.fwd_generation = getattr(p, "fwd_generation", 0) + 1
+        # for the most recent train forward of the plan (the reference's order forward, backward, forward, backward - train.py:364-392);
+        # plans on a shared workspace: for the most recent train forward of ANY plan bound to it
+        p.fwd_generation = gen if gen is not None else getattr(p, "fwd_generation", 0) + 1
         # running_mean / running_var moved (raw pointers): every inference plan's BN-folded weights are stale now
         for q in self.plans.values():
             if not q.train:
@@ -254,6 +321,11 @@ class Engine:
         torch._foreach_add_(plan._nbt, 1)
 
     def _check_generation(self, plan, generation):
+        a = getattr(plan, "arena", None)
+        if a is not None and (a.owner is not plan or (generation is not None and generation != a.generation)):
+            raise _lib.MyoloError(f"backward of a stale train-mode forward: another train forward ran on the shared workspace of "
+                                  f"({plan.B},{plan.H},{plan.W}) after it and overwrote the saved activations (one outstanding forward per "
+                                  "lane; run forward, backward, forward, backward like reference train.py:364-392)")
         if generation is not None and generation != getattr(plan, "fwd_generation", 0):
             raise _lib.MyoloError("backward of a stale train-mode forward: another forward of the same (B,H,W) ran in between and overwrote the "
                                   "saved activations (one outstanding forward per shape; run forward, backward, forward, backward like "
@@ -273,6 +345,7 @@ class Engine:
         """fused seg loss + backward (SURVEY.md section 8f rank 3): mean CE(ignore_index) of the upsampled logits of the last train forward
         against `labels` (B,H,W) int64; gradients scaled by factor * scale (device scalar tensor).  Returns the mean CE (device scalar)."""
         assert labels.is_cuda and labels.dtype == torch.int64 and tuple(labels.shape) == (plan.B, plan.H, plan.W)
+        self._check_generation(plan, None)
         loss = torch.empty((), dtype=torch.float32, device=labels.device)
         _lib.check(_lib.lib().myolo_plan_backward_seg_ce(plan.handle, _lib.ptr(labels.contiguous()), int(ignore_index), float(factor),
                                                          _lib.ptr(scale), _lib.ptr(loss), _lib.stream_ptr()))

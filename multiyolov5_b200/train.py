@@ -13,7 +13,9 @@ clears the gradients.  `torch.distributed` is plumbing only (process group + all
 Out of scope (the reference's outer loop, not the hot path): data loading, LR schedule / warm-up (call `set_lr` / `set_momentum`),
 EMA, checkpointing, plotting, DDP buffer broadcast.
 """
+import math
 import os
+import random
 import ctypes as C
 
 import torch
@@ -81,12 +83,81 @@ class FlatState:
             raise RuntimeError("model parameters / gradients no longer alias the flat training buffers; rebuild the Trainer")
 
 
+class MultiScale:
+    """--multi-scale (reference train.py:354-359): each iteration rescales the det batch so that its long side is a random multiple of gs
+    in [imgsz/2, imgsz*3/2], with torch's bilinear (align_corners=False) interpolation, before the forward.
+
+        sz = random.randrange(imgsz * 0.5, imgsz * 1.5 + gs) // gs * gs
+        sf = sz / max(imgs.shape[2:])
+        if sf != 1: ns = [math.ceil(x * sf / gs) * gs for x in imgs.shape[2:]]; imgs = F.interpolate(imgs, size=ns, ...)
+
+    The reference passes float bounds to randrange, which Python 3.12 rejects; the draw here takes int() of the two bounds, which
+    consumes the `random` stream exactly as Python <= 3.11 did with integral floats (istart + _randbelow(width)).  Only the det batch is
+    rescaled: the seg batch, hyp['obj'] (scaled by imgsz) and the normalised targets stay as they are."""
+
+    def __init__(self, imgsz, gs=32):
+        self.imgsz, self.gs = int(imgsz), int(gs)
+        lo, hi = imgsz * 0.5, imgsz * 1.5 + gs
+        if lo != int(lo) or hi != int(hi):                   # what randrange of Python <= 3.11 raised for non-integral floats
+            raise ValueError(f"non-integer bounds {lo}, {hi} for randrange()")
+        self.lo, self.hi = int(lo), int(hi)
+
+    def _ns(self, sz, shape):
+        sf = sz / max(shape)
+        if sf == 1:
+            return None
+        return [math.ceil(x * sf / self.gs) * self.gs for x in shape]
+
+    def size(self, shape, rng=random):
+        """one draw: the new (H, W) as a list, or None when the batch keeps its size (sf == 1)"""
+        sz = rng.randrange(self.lo, self.hi) // self.gs * self.gs
+        return self._ns(sz, tuple(int(x) for x in shape))
+
+    def shapes(self, shape):
+        """every (H, W) a batch of `shape` can have after a draw, ascending: the rescaled sizes, and `shape` itself when a draw can keep it"""
+        shape = tuple(int(x) for x in shape)
+        out = set()
+        for sz in {v // self.gs * self.gs for v in range(self.lo, self.hi)}:
+            ns = self._ns(sz, shape)
+            out.add(shape if ns is None else tuple(ns))
+        return sorted(out)
+
+    def __call__(self, imgs, out_dtype=torch.float16, rng=random):
+        """draws once and rescales the (B, C, H, W) det batch on the device (uint8 / fp16 / fp32 in; uint8 is converted as
+        imgs.float() / 255.0 first).  fp16 out is the fp32 result rounded to nearest, which is what the train plan's input conversion does
+        to fp32 input.  When the draw keeps the size, a float batch of the requested dtype comes back as it is, without a launch."""
+        if out_dtype not in (torch.float16, torch.float32):
+            raise ValueError(f"MultiScale: out_dtype must be float16 or float32, got {out_dtype}")
+        if imgs.dtype not in (torch.uint8, torch.float16, torch.float32) or imgs.dim() != 4 or not imgs.is_cuda:
+            raise ValueError("MultiScale: expected a CUDA (B, C, H, W) uint8 / float16 / float32 tensor")
+        ns = self.size(imgs.shape[2:], rng)
+        if ns is None and imgs.dtype == out_dtype:
+            return imgs
+        return resize_bilinear(imgs, imgs.shape[2:] if ns is None else ns, out_dtype)
+
+
+def resize_bilinear(x, size, out_dtype=torch.float32):
+    """F.interpolate(x, size, mode='bilinear', align_corners=False) of a CUDA NCHW tensor on the library's kernel, bit exact with torch's
+    for fp32 input; uint8 input is converted as x.float() / 255.0 first; fp16 out = the fp32 result rounded to nearest"""
+    x = x.contiguous()
+    B, Cc, H, W = x.shape
+    Ho, Wo = int(size[0]), int(size[1])
+    out = torch.empty((B, Cc, Ho, Wo), dtype=out_dtype, device=x.device)
+    _lib.check(_lib.lib().myolo_resize_bilinear(_lib.ptr(x), _lib.torch_dtype_code(x.dtype), B, Cc, H, W, _lib.ptr(out),
+                                                _lib.torch_dtype_code(out_dtype), Ho, Wo, _lib.stream_ptr()))
+    return out
+
+
 class Trainer:
     """`Trainer(model, hyp, batch_size).step(imgs, targets, segimgs, segtargets)`; hyp already scaled (see scale_hyp)."""
 
     def __init__(self, model, hyp, batch_size, world_size=1, rank=-1, accumulate=1, detgain=0.6, seggain=0.35, init_scale=2.0 ** 16,
                  growth_interval=2000, process_group=None, graph_loss=True, fused_seg_loss=True, overlap_passes=True, fused_det_loss=True,
-                 concurrent_forwards=None):
+                 concurrent_forwards=None, multi_scale=None):
+        """multi_scale: a MultiScale.  The det lane's train plans for every size it can draw from an imgsz x imgsz batch are reserved on
+        one shared workspace (Engine.reserve_train_shapes); rescale each det batch with `multi_scale(imgs)` before `step`, as the reference
+        does before its forward (train.py:354-359).  A det batch of fewer images (the loader's partial last batch) reserves its sizes on
+        the same workspace the first time it comes; a batch of more images than batch_size does not fit it and raises MyoloError."""
         assert next(model.parameters()).is_cuda, "model.cuda() first"
         self.model, self.hyp, self.batch_size = model, hyp, batch_size
         self.world_size, self.rank, self.accumulate, self.pg = world_size, rank, accumulate, process_group
@@ -125,6 +196,15 @@ class Trainer:
             concurrent_forwards = os.environ.get("MYOLO_CONCURRENT_FWD", "1") != "0"
         self.concurrent_forwards = bool(concurrent_forwards) and self.overlap_passes
         self._ev_detfwd, self._ev_start, self._ev_seg = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
+        self.multi_scale = multi_scale
+        self._ms_batches = set()
+        if multi_scale is not None:
+            self._reserve_det(batch_size)
+
+    def _reserve_det(self, B):
+        ms = self.multi_scale
+        self.model.engine().reserve_train_shapes(B, ms.shapes((ms.imgsz, ms.imgsz)), lane=0)
+        self._ms_batches.add(B)
 
     def set_lr(self, lr_bn, lr_weight, lr_bias):
         self.lr = [float(lr_bn), float(lr_weight), float(lr_bias)]
@@ -244,6 +324,8 @@ class Trainer:
 
     def step(self, imgs, targets, segimgs, segtargets):
         """one iteration (train.py:363-401).  Returns (det loss items [lbox,lobj,lcls,loss], seg loss) as device tensors."""
+        if self.multi_scale is not None and imgs.shape[0] not in self._ms_batches:
+            self._reserve_det(int(imgs.shape[0]))               # host plans only: the shared workspace is already there
         fused_seg = self.fused_seg_loss and self.n_seg_outputs == 1 and self.model.model[-2].c_out in (19, 32)
         if self.overlap_passes and fused_seg:
             main = torch.cuda.current_stream()
