@@ -61,14 +61,12 @@ extern "C" {
 #define MYOLO_OP_DETECT_DECODE 10 /* Detect.forward view/permute/sigmoid/decode, models/yolo.py:211-225 */
 #define MYOLO_OP_SEG_UPSAMPLE 11 /* final x8 bilinear of the seg head -> NCHW logits, models/yolo.py:163 */
 #define MYOLO_OP_BROADCAST 12    /* F.interpolate(nearest) of a 1x1 map (RFB2 global branch), models/common.py:509 */
+/* 13 is retired (it was a fused Focus + conv layer 0) */
 #define MYOLO_OP_BN_ACT 14       /* train mode: batch-statistics BatchNorm + activation (+ residual) on a raw conv output; aux[0] = bn slot */
 #define MYOLO_OP_ACT 15          /* train mode: standalone activation (FFM attention SiLU / Sigmoid) so the pre-activation is kept */
 #define MYOLO_OP_DROPOUT 17      /* train mode: out = in * keep / (1-p), keep ~ Bernoulli(1-p) from a counter-based hash of (seed, forward step, op, element); faux[0] = p, aux[0] = op salt.  nn.Dropout(0.1) of the Base / BiSe heads (reference models/yolo.py:65,140) */
 #define MYOLO_OP_CHANNEL_SCALE_OOP 16 /* train mode: out = in * (1 + in2) out of place (in is needed by the backward pass) */
-#define MYOLO_OP_FOCUS_CONV 13   /* whole layer 0 fused: Focus slicing + Conv3x3+BN+SiLU from the NCHW image, models/common.py:542-551 */
 
-/* conv op flags */
-#define MYOLO_CONV_FORCE_SIMT 1 /* run on the generic CUDA-core kernel (tiny M / odd shapes / debugging) */
 /* op flags (any kind): a run of 2..4 CONSECUTIVE ops of one kind (REGION_COMBINE of one atom grid, small CONVs, BILINEARs with equal output
  * extents) may be executed as ONE launch: the first op carries GROUP_HEAD and the member count in aux[7], the others GROUP_MEMBER */
 #define MYOLO_OP_GROUP_HEAD 2

@@ -11,9 +11,22 @@ LIB_PATH = os.environ.get("MYOLO_LIB") or os.path.join(_HERE, "libmyolo_sm90a.so
 
 F16, F32, U8, I64 = 0, 1, 2, 3
 ACT_NONE, ACT_SILU, ACT_SIGMOID = 0, 1, 2
-(OP_INPUT_FOCUS, OP_CONV, OP_UPSAMPLE_NEAREST, OP_SPP_POOL, OP_BILINEAR, OP_REGION_SUM, OP_REGION_COMBINE, OP_CHANNEL_SCALE,
- OP_ADD, OP_DETECT_DECODE, OP_SEG_UPSAMPLE, OP_BROADCAST, OP_FOCUS_CONV, OP_BN_ACT, OP_ACT, OP_CHANNEL_SCALE_OOP, OP_DROPOUT) = range(1, 18)
-CONV_FORCE_SIMT = 1
+OP_INPUT_FOCUS = 1
+OP_CONV = 2
+OP_UPSAMPLE_NEAREST = 3
+OP_SPP_POOL = 4
+OP_BILINEAR = 5
+OP_REGION_SUM = 6
+OP_REGION_COMBINE = 7
+OP_CHANNEL_SCALE = 8
+OP_ADD = 9
+OP_DETECT_DECODE = 10
+OP_SEG_UPSAMPLE = 11
+OP_BROADCAST = 12
+OP_BN_ACT = 14      # 13 is retired
+OP_ACT = 15
+OP_CHANNEL_SCALE_OOP = 16
+OP_DROPOUT = 17
 OP_GROUP_HEAD, OP_GROUP_MEMBER = 2, 4      # include/myolo.h: consecutive ops of one kind executed as one launch
 
 EXPORTS = [

@@ -46,14 +46,6 @@ static inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 // Programmatic dependent launch for the small kernels of the training chains (~1350 launches per step, most of them 5-15 us): the kernel may be
 // scheduled while its stream predecessor is still running, which takes the ~2 us launch latency off the critical path.  A kernel launched
 // through launch_pdl() MUST call pdl_enter() before it touches memory (its predecessor's output is only visible after the wait).
-inline bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = getenv("MYOLO_NO_PDL");
-    v = (e && e[0] == '1') ? 0 : 1;
-  }
-  return v != 0;
-}
 template <typename... KArgs, typename... Args>
 static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t s, Args&&... args) {
   cudaLaunchConfig_t cfg = {};
@@ -65,7 +57,7 @@ static inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 blo
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kern, static_cast<KArgs>(args)...);
 }
 static inline int64_t align_up(int64_t a, int64_t b) { return (a + b - 1) / b * b; }

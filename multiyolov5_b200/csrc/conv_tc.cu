@@ -19,10 +19,6 @@
 #include "conv.h"
 #include "wgmma.cuh"
 
-#ifndef MYOLO_SILU_SFU_EVERY
-#define MYOLO_SILU_SFU_EVERY 2   // every n-th output channel of a 16-channel group takes the two-MUFU SiLU (balances the FMA pipe and the SFU)
-#endif
-
 namespace myolo {
 
 static constexpr int kTileM = 128;
@@ -32,6 +28,8 @@ static constexpr int kMaxStages = 8;
 static constexpr int kSmemBudget = 227 * 1024;
 static constexpr int kBiasBytes = 8192;   // bias vector of the layer in shared memory (<= 1920 output channels: the data gradient
                                           // of SPP.cv2 has 1024)
+static constexpr int kSiluSfuEvery = 2;   // every n-th output channel of a 16-channel group takes the two-MUFU SiLU (balances the FMA
+                                          // pipe and the SFU)
 
 // K-major swizzled operand (rows of kc*2 bytes = the swizzle width, 8-row swizzle atoms), PTX ISA "matrix descriptor" of wgmma
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, int row_bytes) {
@@ -60,7 +58,7 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvTcParams& p, int tile
 }
 
 __device__ __forceinline__ float act_out(float v, int act, int ch) {
-  if (act == MYOLO_ACT_SILU) return (ch & 15) % MYOLO_SILU_SFU_EVERY == MYOLO_SILU_SFU_EVERY - 1 ? silu_f_sfu(v) : silu_f(v);
+  if (act == MYOLO_ACT_SILU) return (ch & 15) % kSiluSfuEvery == kSiluSfuEvery - 1 ? silu_f_sfu(v) : silu_f(v);
   if (act == MYOLO_ACT_SIGMOID) return sigmoid_f(v);
   return v;
 }
@@ -430,7 +428,7 @@ int conv_tc_launch(const ConvOp& op, cudaStream_t stream) {
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = 1;
   MYOLO_CHECK_CUDA(op.p.residual != nullptr ? launch_res<true>(op, cfg) : launch_res<false>(op, cfg));
   g_launch_count++;
   return 0;

@@ -6,9 +6,6 @@ namespace myolo {
 
 // Focus.forward slicing + NCHW->NHWC + cast (reference models/common.py:549-550, detect.py:135-137)
 int launch_input_focus(const void* x, int x_dtype, int B, int H, int W, const TensorView& out, cudaStream_t s);
-// fused layer 0: Focus + Conv3x3(12->Co)+BN+SiLU from the NCHW image (packed weights [Co][9][16], fp32 bias)
-int launch_focus_conv(const void* x, int x_dtype, int B, int H, int W, const __half* wp, const float* bias, int co, const TensorView& out,
-                      cudaStream_t s);
 int launch_upsample_nearest2x(const TensorView& in, const TensorView& out, cudaStream_t s);
 // SPP: out slices 1..3 = maxpool 5/9/13 of slice 0 (views share one buffer); reference models/common.py:170-174
 int launch_spp_pool(const TensorView& in, const TensorView& out5, int n_cascade, cudaStream_t s);

@@ -94,13 +94,12 @@ struct myolo_plan {
   std::vector<int> conv_ready;    // tensor maps built
   int64_t last_launches = 0;
   bool force_simt = false;
-  // CUDA-graph replay of the internal ops (everything that does not touch caller-owned tensors), captured over several
-  // stream "lanes" so that independent branches (C3.cv1 || C3.cv2, seg head || detect head, PSP m8/m16/m32 ...) overlap
-  bool warmed = false, use_graph = true, graph_dirty = true;
-  std::vector<std::vector<int>> deps;
+  // CUDA-graph replay of the internal ops (everything that does not touch caller-owned tensors), captured in plan order as one chain.
+  // lanes[0] is the capture origin, lanes[1] the backward's weight-gradient side lane; op_ev holds the backward's per-conv fork events and,
+  // at n + 1, the join of the side lane.  Both are created by the first graph build.
+  bool warmed = false, graph_dirty = true;
   std::vector<cudaStream_t> lanes;
   std::vector<cudaEvent_t> op_ev;
-  cudaEvent_t ev_start = nullptr;
   cudaEvent_t ev_tail[3] = {nullptr, nullptr, nullptr};   // fork / join of the Detect decodes and the seg upsample behind the graph
   cudaGraph_t graph = nullptr;
   cudaGraphExec_t graph_exec = nullptr;
@@ -134,7 +133,6 @@ struct myolo_plan {
   int n_run_jobs = 0;
   unsigned long long seed = 0;       // dropout
   unsigned long long* d_step = nullptr;
-  std::vector<cudaEvent_t> bwd_ev;   // per-op completion events of the multi-lane captured backward (+4 join events)
   void* ce_scratch = nullptr;      // 16 bytes for the fused seg loss (valid-pixel count, loss sum)
   float* ce_gbuf = nullptr;        // per-pixel (softmax - onehot), NHWC fp32, of the fused seg loss
   size_t ce_gbuf_bytes = 0;
@@ -206,8 +204,6 @@ static int plan_create(const myolo_op* ops, int n_ops, const myolo_buf_desc* buf
   pl->conv_ready.assign(n_ops, 0);
   const char* fs = getenv("MYOLO_FORCE_SIMT");
   pl->force_simt = fs && fs[0] == '1';
-  const char* ng = getenv("MYOLO_NO_GRAPH");
-  pl->use_graph = !(ng && ng[0] == '1');
   for (int i = 0; i < n_bufs; ++i) {
     const myolo_buf_desc& bd = bufs[i];
     const int64_t bytes = (int64_t)B * bd.h * bd.w * bd.c * (bd.dtype == MYOLO_F16 ? 2 : 4);
@@ -270,7 +266,6 @@ extern "C" void myolo_plan_destroy(myolo_plan* pl) {
   for (auto& e : pl->bwd_exec) if (e) cudaGraphExecDestroy(e);
   if (pl->graph) cudaGraphDestroy(pl->graph);
   for (auto e : pl->op_ev) cudaEventDestroy(e);
-  if (pl->ev_start) cudaEventDestroy(pl->ev_start);
   for (auto& e : pl->ev_tail) if (e) cudaEventDestroy(e);
   for (auto st : pl->lanes) cudaStreamDestroy(st);
   for (auto& sl : pl->slots) {
@@ -281,7 +276,6 @@ extern "C" void myolo_plan_destroy(myolo_plan* pl) {
   if (pl->gws && pl->owns_ws) cudaFree(pl->gws);
   for (auto& sl : pl->slots) if (sl.dw_packed) cudaFree(sl.dw_packed);
   if (pl->tmp16) cudaFree(pl->tmp16);
-  for (auto e : pl->bwd_ev) cudaEventDestroy(e);
   if (pl->ce_scratch) cudaFree(pl->ce_scratch);
   if (pl->d_step) cudaFree(pl->d_step);
   if (pl->ce_gbuf) cudaFree(pl->ce_gbuf);
@@ -409,7 +403,7 @@ static int prepare_conv(myolo_plan* pl, int i) {
   const int ho = (c.in.H + 2 * pad - op.dil * (op.k - 1) - 1) / op.stride + 1;
   const int wo = (c.in.W + 2 * pad - op.dil * (op.k - 1) - 1) / op.stride + 1;
   MYOLO_REQUIRE(ho == c.out.H && wo == c.out.W, "op %d: conv output %dx%d does not match buffer %dx%d", i, ho, wo, c.out.H, c.out.W);
-  c.use_tc = !pl->force_simt && !(op.flags & MYOLO_CONV_FORCE_SIMT) && conv_tc_eligible(c);
+  c.use_tc = !pl->force_simt && conv_tc_eligible(c);
   if (c.use_tc && (rc = conv_tc_prepare(c, pl->num_sms))) return rc;
   pl->conv_ready[i] = 1;
   return 0;
@@ -463,14 +457,6 @@ static int run_op(myolo_plan* pl, int i, const void* x, int x_dtype, float* z, f
     case MYOLO_OP_INPUT_FOCUS:
       if ((rc = resolve_view(pl, op.out, &out))) return rc;
       return launch_input_focus(x, x_dtype, pl->B, pl->H, pl->W, out, s);
-    case MYOLO_OP_FOCUS_CONV: {
-      if ((rc = resolve_view(pl, op.out, &out))) return rc;
-      MYOLO_REQUIRE(op.weight_slot >= 0 && op.weight_slot < (int)pl->slots.size() && pl->slots[op.weight_slot].set,
-                    "op %d: focus_conv weights not set", i);
-      const WeightSlot& ws = pl->slots[op.weight_slot];
-      MYOLO_REQUIRE(ws.k == 3 && ws.ci == 12 && ws.ci_pad == 16, "op %d: focus_conv expects a 3x3 conv over 12 channels", i);
-      return launch_focus_conv(x, x_dtype, pl->B, pl->H, pl->W, ws.w, ws.bias, ws.co, out, s);
-    }
     case MYOLO_OP_CONV:
       if (!pl->conv_ready[i] && (rc = prepare_conv(pl, i))) return rc;
       return pl->convs[i].use_tc ? conv_tc_launch(pl->convs[i], s) : conv_simt_launch(pl->convs[i], s);
@@ -546,120 +532,32 @@ static int run_op(myolo_plan* pl, int i, const void* x, int x_dtype, float* z, f
 }
 
 // ------------------------------------------------------------------------------------------------
-// dependency analysis + multi-lane graph capture
+// graph capture of the internal ops
 // ------------------------------------------------------------------------------------------------
 static bool is_external_op(int kind) {
-  return kind == MYOLO_OP_INPUT_FOCUS || kind == MYOLO_OP_FOCUS_CONV || kind == MYOLO_OP_DETECT_DECODE || kind == MYOLO_OP_SEG_UPSAMPLE;
+  return kind == MYOLO_OP_INPUT_FOCUS || kind == MYOLO_OP_DETECT_DECODE || kind == MYOLO_OP_SEG_UPSAMPLE;
 }
 
-struct Access { int buf, c_lo, c_hi; int64_t lo, hi; bool write; };
-
-static void add_access(const myolo_plan* pl, const myolo_view& v, bool write, std::vector<Access>& out) {
-  if (v.buf < 0) return;
-  const myolo_buf_desc& bd = pl->bufs[v.buf];
-  const int64_t bytes = (int64_t)pl->B * bd.h * bd.w * bd.c * (bd.dtype == MYOLO_F16 ? 2 : 4);
-  out.push_back(Access{v.buf, v.c_off, v.c_off + v.c, bd.offset, bd.offset + bytes, write});
-}
-
-static void op_accesses(const myolo_plan* pl, const myolo_op& op, std::vector<Access>& acc) {
-  acc.clear();
-  add_access(pl, op.in, op.kind == MYOLO_OP_CHANNEL_SCALE, acc);   // channel_scale updates `in` in place
-  if (op.kind == MYOLO_OP_CHANNEL_SCALE) add_access(pl, op.in, false, acc);
-  add_access(pl, op.in2, false, acc);
-  add_access(pl, op.out, true, acc);
-}
-
-static bool conflicts(const Access& a, const Access& b) {
-  if (!(a.write || b.write)) return false;
-  if (a.hi <= b.lo || b.hi <= a.lo) return false;              // disjoint bytes
-  if (a.buf == b.buf) return a.c_lo < b.c_hi && b.c_lo < a.c_hi;  // same buffer: only overlapping channel slices collide
-  return true;                                                  // different buffers sharing workspace bytes (liveness packing)
-}
-
-static void compute_deps(myolo_plan* pl) {
-  const int n = (int)pl->ops.size();
-  pl->deps.assign(n, {});
-  std::vector<std::vector<Access>> acc(n);
-  for (int i = 0; i < n; ++i) op_accesses(pl, pl->ops[i], acc[i]);
-  for (int i = 0; i < n; ++i)
-    for (int j = 0; j < i; ++j) {
-      bool c = false;
-      for (const Access& a : acc[i]) {
-        for (const Access& b : acc[j])
-          if (conflicts(a, b)) { c = true; break; }
-        if (c) break;
-      }
-      if (c) pl->deps[i].push_back(j);
-    }
-}
-
+// The forward graph is ONE chain of the internal ops in plan order.  Every conv launch fills the machine, so branch concurrency buys
+// little, while a capture over several streams makes the graph runtime spread the nodes over many internal streams: every edge becomes a
+// cross-stream dependency and the programmatic-dependent-launch edges between consecutive convs are lost.
 static int build_graph(myolo_plan* pl) {
   const int n = (int)pl->ops.size();
-  static int nl_env = -1;
-  if (nl_env < 0) {
-    const char* e = getenv("MYOLO_LANES");
-    nl_env = e ? std::max(4, std::min(16, atoi(e))) : 4;      // >= 4: the captured backward uses lanes 0-3
-  }
-  // forward graphs: ONE lane by default.  Every conv launch fills the machine, so branch concurrency buys little, while a multi-lane
-  // capture makes the graph runtime spread the nodes over many internal streams - every edge becomes a cross-stream dependency and the
-  // programmatic-dependent-launch edges between consecutive convs are lost.  MYOLO_FWD_LANES > 1 restores the branch lanes.
-  static int fwd_lanes = -1;
-  if (fwd_lanes < 0) {
-    const char* e = getenv("MYOLO_FWD_LANES");
-    fwd_lanes = e ? std::max(1, std::min(nl_env, atoi(e))) : 1;
-  }
-  const int NL = nl_env;          // streams / events are sized for the backward's lanes
-  const int NLF = fwd_lanes;      // lanes this (forward) capture actually uses
-  if (pl->deps.empty()) compute_deps(pl);
   if (pl->lanes.empty()) {
-    pl->lanes.resize(NL);
+    pl->lanes.resize(2);
     for (auto& st : pl->lanes) MYOLO_CHECK_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
-    pl->op_ev.resize(n + NL);
+    pl->op_ev.resize(n + 2);
     for (auto& e : pl->op_ev) MYOLO_CHECK_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    MYOLO_CHECK_CUDA(cudaEventCreateWithFlags(&pl->ev_start, cudaEventDisableTiming));
   }
   if (pl->graph_exec) { cudaGraphExecDestroy(pl->graph_exec); pl->graph_exec = nullptr; }
   if (pl->graph) { cudaGraphDestroy(pl->graph); pl->graph = nullptr; }
-  std::vector<int> lane_of(n, -1), lane_last(NL, -1);
-  std::vector<char> lane_live(NL, 0);
   cudaStream_t origin = pl->lanes[0];
   MYOLO_CHECK_CUDA(cudaStreamBeginCapture(origin, cudaStreamCaptureModeThreadLocal));
-  MYOLO_CHECK_CUDA(cudaEventRecord(pl->ev_start, origin));
-  lane_live[0] = 1;
   int rc = 0, count = 0;
-  for (int i = 0; i < n && !rc; ++i) {
+  for (int i = 0; i < n; ++i) {
     if (is_external_op(pl->ops[i].kind)) continue;
-    // lane choice: continue on the lane of the most recent dependency if that lane has not moved on, else least recently used lane
-    int L = -1, latest = -1;
-    for (int d : pl->deps[i])
-      if (lane_of[d] >= 0 && d > latest) latest = d;
-    if (latest >= 0 && lane_last[lane_of[latest]] == latest) L = lane_of[latest];
-    if (L < 0) {
-      L = 0;
-      for (int k = 1; k < NLF; ++k)
-        if (lane_last[k] < lane_last[L]) L = k;
-    }
-    cudaStream_t st = pl->lanes[L];
-    if (!lane_live[L]) {
-      if (cudaStreamWaitEvent(st, pl->ev_start, 0) != cudaSuccess) { rc = MYOLO_E_CUDA; break; }
-      lane_live[L] = 1;
-    }
-    for (int d : pl->deps[i]) {
-      if (lane_of[d] < 0 || lane_of[d] == L) continue;   // external op (ordered by the stream) or same lane (stream order)
-      if (cudaStreamWaitEvent(st, pl->op_ev[d], 0) != cudaSuccess) { rc = MYOLO_E_CUDA; break; }
-    }
-    if (rc) break;
-    rc = run_op(pl, i, nullptr, 0, nullptr, nullptr, nullptr, 0, nullptr, st);
-    if (rc) break;
-    if (cudaEventRecord(pl->op_ev[i], st) != cudaSuccess) { rc = MYOLO_E_CUDA; break; }
-    lane_of[i] = L;
-    lane_last[L] = i;
+    if ((rc = run_op(pl, i, nullptr, 0, nullptr, nullptr, nullptr, 0, nullptr, origin))) break;
     ++count;
-  }
-  for (int k = 1; k < NL; ++k) {
-    if (!lane_live[k]) continue;
-    if (cudaEventRecord(pl->op_ev[n + k], pl->lanes[k]) != cudaSuccess || cudaStreamWaitEvent(origin, pl->op_ev[n + k], 0) != cudaSuccess)
-      rc = rc ? rc : MYOLO_E_CUDA;
   }
   cudaGraph_t g = nullptr;
   cudaError_t e = cudaStreamEndCapture(origin, &g);
@@ -682,8 +580,8 @@ extern "C" int myolo_plan_forward(myolo_plan* pl, const void* x, int x_dtype, fl
   MYOLO_REQUIRE(pl && x, "plan_forward: null plan / input");
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t l0 = g_launch_count;
-  if (!pl->warmed || !pl->use_graph) {
-    // first call (lazy tensor-map / attribute setup happens here) or graphs disabled: plain in-order replay
+  if (!pl->warmed) {
+    // first call (lazy tensor-map / attribute setup happens here): plain in-order replay
     for (size_t i = 0; i < pl->ops.size(); ++i) {
       int rc = run_op(pl, (int)i, x, x_dtype, z, raw, seg, seg_dtype, seg_argmax, s);
       if (rc) return rc;
@@ -703,7 +601,7 @@ extern "C" int myolo_plan_forward(myolo_plan* pl, const void* x, int x_dtype, fl
   }
   int n_ext = 0;
   for (size_t i = 0; i < pl->ops.size(); ++i)     // ops reading the caller's input: before the graph
-    if (pl->ops[i].kind == MYOLO_OP_INPUT_FOCUS || pl->ops[i].kind == MYOLO_OP_FOCUS_CONV) {
+    if (pl->ops[i].kind == MYOLO_OP_INPUT_FOCUS) {
       int rc = run_op(pl, (int)i, x, x_dtype, z, raw, seg, seg_dtype, seg_argmax, s);
       if (rc) return rc;
       ++n_ext;
@@ -902,7 +800,7 @@ extern "C" int myolo_plan_train_forward(myolo_plan* pl, const void* x, int x_dty
     int brc = launch_bump_step(pl->d_step, (cudaStream_t)stream);
     if (brc) return brc;
   }
-  // same executor as inference: first call in order (lazy allocations / tensor maps), then multi-lane CUDA-graph replay of the internal
+  // same executor as inference: first call in order (lazy allocations / tensor maps), then CUDA-graph replay of the internal
   // ops with the input conversion before and the caller-owned outputs (raw x_i, seg logits) after the graph
   int rc = myolo_plan_forward(pl, x, x_dtype, nullptr, raw, seg, MYOLO_F32, nullptr, stream);
   if (rc) return rc;
@@ -1088,7 +986,7 @@ static int backward_run(myolo_plan* pl, int mask, std::vector<char>& live, cudaS
     pl->bwd_dirty = false;
   }
   int n_ops = 0;
-  if (!pl->use_graph || !pl->bwd_warm[mask]) {
+  if (!pl->bwd_warm[mask]) {
     // first backward with this seed set: in order on the caller's stream (allocations, tensor maps, weight packs happen here)
     rc = backward_walk(pl, live, s, &n_ops);
     if (!rc && !pl->bwd_dirty) pl->bwd_warm[mask] = true;
@@ -1096,11 +994,6 @@ static int backward_run(myolo_plan* pl, int mask, std::vector<char>& live, cudaS
   }
   if (!pl->bwd_exec[mask]) {
     if (pl->lanes.empty()) { set_error("backward: forward graph state missing"); return MYOLO_E_INVALID; }
-    if (pl->bwd_ev.size() < pl->ops.size() + 4) {
-      const size_t old_n = pl->bwd_ev.size();
-      pl->bwd_ev.resize(pl->ops.size() + 4);
-      for (size_t k = old_n; k < pl->bwd_ev.size(); ++k) MYOLO_CHECK_CUDA(cudaEventCreateWithFlags(&pl->bwd_ev[k], cudaEventDisableTiming));
-    }
     cudaStream_t cs = pl->lanes[0];
     MYOLO_CHECK_CUDA(cudaStreamBeginCapture(cs, cudaStreamCaptureModeThreadLocal));
     rc = backward_walk(pl, live, cs, &n_ops);
@@ -1191,49 +1084,9 @@ static int backward_walk(myolo_plan* pl, std::vector<char>& live, cudaStream_t s
   int rc = 0;
   auto is_live = [&](const myolo_view& v) { return v.buf >= 0 && live[v.buf]; };
   auto mark = [&](const myolo_view& v) { if (v.buf >= 0) live[v.buf] = 1; };
-  static int side_env = -1;
-  if (side_env < 0) {
-    const char* e = getenv("MYOLO_WGRAD_LANE");
-    side_env = e ? atoi(e) : 1;
-  }
   // weight-gradient lane (exists once the forward graph has created the plan's streams / events)
-  cudaStream_t side = (side_env && pl->lanes.size() >= 2 && pl->lanes[1] != s && (int)pl->op_ev.size() >= n + 2) ? pl->lanes[1] : s;
+  cudaStream_t side = (pl->lanes.size() >= 2 && pl->lanes[1] != s && (int)pl->op_ev.size() >= n + 2) ? pl->lanes[1] : s;
   bool used_side = false;
-  // Under capture the chain itself is spread over three lanes: ops are ordered only by real dependencies on the GRADIENT buffers
-  // (reads of grad(out), read-modify-writes of grad(in) / grad(in2)) and on the two shared scratch areas, so the branches of C3 /
-  // SPP / PSP / the three detect levels overlap exactly as they do in the forward graph.
-  static int ml_env = -1;
-  if (ml_env < 0) {
-    const char* e = getenv("MYOLO_BWD_LANES");
-    ml_env = e ? atoi(e) : 0;     // like the forward graph, a multi-lane capture is spread over dozens of internal streams and every edge
-                                  // becomes a cross-stream wait
-  }
-  cudaStreamCaptureStatus cap = cudaStreamCaptureStatusNone;
-  cudaStreamIsCapturing(s, &cap);
-  const bool multi = ml_env && cap == cudaStreamCaptureStatusActive && pl->lanes.size() >= 4 && s == pl->lanes[0] &&
-                     (int)pl->bwd_ev.size() >= n + 4;
-  struct GAcc { int buf, c_lo, c_hi; bool write; };
-  auto acc_of = [&](int i, std::vector<GAcc>& out) {
-    const myolo_op& op = pl->ops[i];
-    out.clear();
-    auto add = [&](const myolo_view& v, bool w) { if (v.buf >= 0) out.push_back(GAcc{v.buf, v.c_off, v.c_off + v.c, w}); };
-    add(op.out, false);
-    add(op.in, true);
-    add(op.in2, true);
-    if (op.kind == MYOLO_OP_CONV && (op.stride == 2 || pl->bufs[op.out.buf].dtype == MYOLO_F32)) out.push_back(GAcc{-2, 0, 1, true});  // tmp16
-    if (op.kind == MYOLO_OP_BILINEAR || op.kind == MYOLO_OP_SPP_POOL) out.push_back(GAcc{-3, 0, 1, true});                          // fp32 scratch
-  };
-  std::vector<int> done;                       // executed ops, in execution order
-  std::vector<std::vector<GAcc>> done_acc;
-  std::vector<int> lane_of(n, -1);
-  const int NLc = 3;
-  cudaStream_t chain[NLc] = {s, multi ? pl->lanes[2] : s, multi ? pl->lanes[3] : s};
-  int lane_last[NLc] = {-1, -1, -1};           // position (in `done`) of the last op of each lane
-  bool lane_used[NLc] = {true, false, false};
-  if (multi) {
-    if (cudaEventRecord(pl->bwd_ev[n], s) != cudaSuccess) { set_error("backward: capture fork failed"); return MYOLO_E_CUDA; }
-  }
-  std::vector<GAcc> cur;
   for (int i = n - 1; i >= 0 && !rc; --i) {
     const myolo_op& op = pl->ops[i];
     TensorView a, b, c, d;
@@ -1242,39 +1095,6 @@ static int backward_walk(myolo_plan* pl, std::vector<char>& live, cudaStream_t s
     mark(op.in);
     mark(op.in2);
     ++*n_ops;
-    cudaStream_t s = chain[0];                 // (shadows the origin: the op's lane)
-    int L = 0;
-    if (multi) {
-      acc_of(i, cur);
-      std::vector<int> deps;                   // positions in `done`
-      for (int q = (int)done.size() - 1; q >= 0; --q) {
-        bool hit = false;
-        for (const GAcc& x : cur) {
-          for (const GAcc& y : done_acc[q])
-            if (x.buf == y.buf && (x.write || y.write) && x.c_lo < y.c_hi && y.c_lo < x.c_hi) { hit = true; break; }
-          if (hit) break;
-        }
-        if (hit) deps.push_back(q);
-      }
-      int latest = deps.empty() ? -1 : deps.front();         // deps are in decreasing position order
-      L = -1;
-      if (latest >= 0 && lane_last[lane_of[done[latest]]] == latest) L = lane_of[done[latest]];
-      if (L < 0) {
-        L = 0;
-        for (int k = 1; k < NLc; ++k)
-          if (lane_last[k] < lane_last[L]) L = k;
-      }
-      s = chain[L];
-      if (!lane_used[L]) {
-        if (cudaStreamWaitEvent(s, pl->bwd_ev[n], 0) != cudaSuccess) { rc = MYOLO_E_CUDA; break; }
-        lane_used[L] = true;
-      }
-      for (int q : deps) {
-        if (lane_of[done[q]] == L) continue;
-        if (cudaStreamWaitEvent(s, pl->bwd_ev[done[q]], 0) != cudaSuccess) { rc = MYOLO_E_CUDA; break; }
-      }
-      if (rc) break;
-    }
     switch (op.kind) {
       case MYOLO_OP_CONV:
         rc = conv_backward(pl, i, !is_input_buf[op.in.buf], s, side, &used_side);
@@ -1339,18 +1159,6 @@ static int backward_walk(myolo_plan* pl, std::vector<char>& live, cudaStream_t s
         set_error("backward: op %d of kind %d has no backward", i, op.kind);
         rc = MYOLO_E_INVALID;
     }
-    if (multi && !rc) {
-      if (cudaEventRecord(pl->bwd_ev[i], s) != cudaSuccess) { rc = MYOLO_E_CUDA; break; }
-      lane_of[i] = L;
-      done.push_back(i);
-      done_acc.push_back(cur);
-      lane_last[L] = (int)done.size() - 1;
-    }
-  }
-  if (multi) {   // join the chain lanes into the origin
-    for (int k = 1; k < NLc; ++k)
-      if (lane_used[k] && (cudaEventRecord(pl->bwd_ev[n + k], chain[k]) != cudaSuccess || cudaStreamWaitEvent(chain[0], pl->bwd_ev[n + k], 0) != cudaSuccess))
-        if (!rc) { set_error("backward: joining the capture lanes failed"); rc = MYOLO_E_CUDA; }
   }
   if (used_side) {   // join the weight-gradient lane (required to close a capture; in eager mode it orders the optimiser after it)
     if (cudaEventRecord(pl->op_ev[n + 1], side) != cudaSuccess || cudaStreamWaitEvent(s, pl->op_ev[n + 1], 0) != cudaSuccess) {

@@ -218,12 +218,6 @@ static cudaError_t launch_wgrad(const WgradTcParams& p, dim3 grid, size_t smem, 
 }
 
 bool conv_wgrad_tc_eligible(const TensorView& x, const TensorView& dy, int k, int stride, int dil, int co, int ci) {
-  static int env = -1;
-  if (env < 0) {
-    const char* e = getenv("MYOLO_WGRAD_TC");
-    env = e ? atoi(e) : 1;
-  }
-  if (!env) return false;
   if (x.dtype != MYOLO_F16 || dy.dtype != MYOLO_F16) return false;
   if (!(k == 1 || k == 3)) return false;
   if (!((stride == 1) || (stride == 2 && k == 3 && dil == 1 && !((x.H | x.W) & 1)))) return false;

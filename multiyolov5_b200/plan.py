@@ -20,7 +20,7 @@ import torch.nn as nn
 
 from . import _lib
 from ._lib import (ACT_NONE, ACT_SIGMOID, ACT_SILU, F16, F32, OP_ADD, OP_BILINEAR, OP_BROADCAST, OP_CHANNEL_SCALE, OP_CONV,
-                   OP_ACT, OP_BN_ACT, OP_CHANNEL_SCALE_OOP, OP_DROPOUT, OP_DETECT_DECODE, OP_FOCUS_CONV, OP_INPUT_FOCUS, OP_REGION_COMBINE, OP_REGION_SUM, OP_SEG_UPSAMPLE, OP_SPP_POOL,
+                   OP_ACT, OP_BN_ACT, OP_CHANNEL_SCALE_OOP, OP_DROPOUT, OP_DETECT_DECODE, OP_INPUT_FOCUS, OP_REGION_COMBINE, OP_REGION_SUM, OP_SEG_UPSAMPLE, OP_SPP_POOL,
                    OP_UPSAMPLE_NEAREST)
 from .models import common as cm
 
@@ -339,20 +339,10 @@ class PlanBuilder:
     def Focus(self, m: cm.Focus, dst=None) -> V:
         conv = m.conv.conv
         assert conv.in_channels == 12
-        import os
-        if (conv.kernel_size == (3, 3) and conv.out_channels in (32, 48) and isinstance(m.conv.act, nn.SiLU)
-                and os.environ.get("MYOLO_FOCUS_FUSION") == "1" and not self.train):
-            # opt-in: whole layer in one kernel straight from the NCHW image (csrc/focus_conv.cu).  It has not been measured on
-            # H100 against the space-to-depth kernel + wgmma conv, so the two-kernel path stays the default.
-            dst = dst or self.new_buf(self.H // 2, self.W // 2, conv.out_channels)
-            slot = len(self.slots)
-            self.slots.append(WeightSlot(conv, m.conv.bn, "focus"))
-            self.emit(OpRec(OP_FOCUS_CONV, None, None, dst, 3, 1, 1, ACT_SILU, 0, slot))
-            return dst
         s2d = self.new_buf(self.H // 2, self.W // 2, 16)
         self.emit(OpRec(OP_INPUT_FOCUS, None, None, s2d))
         if (not self.train and dst is None and conv.kernel_size == (3, 3) and conv.stride == (1, 1) and isinstance(m.conv.act, nn.SiLU)
-                and (self.W // 2) % 2 == 0 and os.environ.get("MYOLO_L0_PAIR", "1") == "1"):
+                and (self.W // 2) % 2 == 0):
             # layer 0 on pixel pairs (_PairedConv): same memory, 64-byte rows, N = 2 Co
             out = self.new_buf(self.H // 2, self.W // 2, conv.out_channels)
             x2 = self.alias_buf(s2d.buf, self.H // 2, self.W // 4, 32)
@@ -387,7 +377,7 @@ class PlanBuilder:
 
     def group(self, first: int, n: int):
         """ops[first : first+n] (same kind, emitted back to back) run as ONE launch (include/myolo.h MYOLO_OP_GROUP_*)"""
-        if n < 2 or n > 4 or self.train or os.environ.get("MYOLO_GROUP_OPS", "1") != "1":
+        if n < 2 or n > 4 or self.train:
             return
         kinds = {o.kind for o in self.ops[first:first + n]}
         assert len(kinds) == 1 and first + n <= len(self.ops)
@@ -585,7 +575,7 @@ def build_plan(model, B: int, H: int, W: int, noalias: bool = False, train: bool
     # other): the graph then ends with the seg classifier conv and the x8 seg upsample - the longest caller-output kernel, run after the
     # graph - no longer waits behind the three Detect convs
     order = list(range(n))
-    if not train and os.environ.get("MYOLO_DETECT_FIRST", "1") == "1":
+    if not train:
         for i in range(1, n):
             seg_types = (Y.SegMaskPSP, Y.SegMaskLab, Y.SegMaskBiSe, Y.SegMaskBase)
             if isinstance(layers[i], Y.Detect) and isinstance(layers[i - 1], seg_types) and \

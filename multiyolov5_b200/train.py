@@ -14,7 +14,6 @@ Out of scope (the reference's outer loop, not the hot path): data loading, LR sc
 EMA, checkpointing, plotting, DDP buffer broadcast.
 """
 import math
-import os
 import random
 import ctypes as C
 
@@ -192,9 +191,7 @@ class Trainer:
         # pass the kernels are launch/latency bound and each pass alone leaves most of the 132 SMs idle.
         self.overlap_passes = bool(overlap_passes) and (graph_loss or fused_det_loss)
         self._s_seg = torch.cuda.Stream() if self.overlap_passes else None
-        if concurrent_forwards is None:
-            concurrent_forwards = os.environ.get("MYOLO_CONCURRENT_FWD", "1") != "0"
-        self.concurrent_forwards = bool(concurrent_forwards) and self.overlap_passes
+        self.concurrent_forwards = (concurrent_forwards is None or bool(concurrent_forwards)) and self.overlap_passes
         self._ev_detfwd, self._ev_start, self._ev_seg = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
         self.multi_scale = multi_scale
         self._ms_batches = set()

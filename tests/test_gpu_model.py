@@ -109,28 +109,6 @@ def test_forward_full_resolution_all_heads(tag):
     assert torch.equal(z, z2) and torch.equal(seg, seg2)
 
 
-@pytest.mark.parametrize("tag,dtype", [("s_psp", torch.float32), ("s_psp", torch.uint8), ("m_psp", torch.float16)])
-def test_fused_layer0_matches_unfused_path(tag, dtype, monkeypatch):
-    """csrc/focus_conv.cu (Focus + conv in one kernel from the NCHW image) vs the space-to-depth kernel + wgmma conv."""
-    model, cfg, sd = build(tag)
-    x8 = torch.randint(0, 256, (2, 3, 128, 256), dtype=torch.uint8, generator=torch.Generator().manual_seed(3)).cuda()
-    x = x8 if dtype == torch.uint8 else (x8.float() / 255.0).to(dtype)
-    monkeypatch.setenv("MYOLO_FOCUS_FUSION", "1")
-    eng = model.engine()
-    eng.noalias = True          # keep layer 0's buffer readable after the forward
-    model(x)
-    y_fused = eng.read_view(eng.last_plan.pb.layer_views[0]).clone()
-    monkeypatch.setenv("MYOLO_FOCUS_FUSION", "0")
-    model2, _, _ = build(tag)
-    model2.engine().noalias = True
-    model2(x)
-    y_ref = model2.engine().read_view(model2.engine().last_plan.pb.layer_views[0])
-    from multiyolov5_b200 import _lib
-    assert any(o.kind == _lib.OP_FOCUS_CONV for o in eng.last_plan.pb.ops) and not any(o.kind == _lib.OP_FOCUS_CONV for o in model2.engine().last_plan.pb.ops)
-    o = restate.model_forward(cfg, sd, (x8.float() / 255.0).cpu(), quantised=True, keep=(0,))["layers"][0].numpy()
-    assert relmax(y_fused.cpu().numpy(), o) < 3e-3 and relmax(y_ref.cpu().numpy(), o) < 3e-3
-
-
 def test_half_mode_like_reference_cuda_path():
     """detect.py:96-103: model.half() + img.half() -> fp16 seg logits; class ids must agree with the fp32-IO run except at near-ties."""
     model, cfg, sd = build("s_psp")

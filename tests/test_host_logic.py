@@ -44,7 +44,7 @@ def test_model_surface():
 
 
 @pytest.mark.parametrize("tag,B,H,W", [("s_psp", 16, 512, 1024), ("m_lab", 8, 512, 1024), ("s_bise", 2, 256, 256), ("s_base", 1, 64, 96)])
-def test_planner_invariants(tag, B, H, W):
+def test_planner_op_and_buffer_invariants(tag, B, H, W):
     from multiyolov5_b200 import _lib
     from multiyolov5_b200.models.yolo import Model
     from multiyolov5_b200.plan import build_plan
@@ -63,7 +63,7 @@ def test_planner_invariants(tag, B, H, W):
     assert pb.workspace_bytes < sum(b.nbytes(B) for b in used)
     # every conv reads exactly the (16-padded) input channels it was packed for; outputs land in slices (no concat copies)
     kinds = [o.kind for o in pb.ops]
-    assert kinds.count(_lib.OP_INPUT_FOCUS) + kinds.count(_lib.OP_FOCUS_CONV) == 1   # layer 0: fused Focus+conv (or s2d + conv)
+    assert kinds.count(_lib.OP_INPUT_FOCUS) == 1   # layer 0: space-to-depth + conv
     assert kinds.count(_lib.OP_DETECT_DECODE) == 3 and kinds.count(_lib.OP_SEG_UPSAMPLE) == 1
     for o in pb.ops:
         if o.kind == _lib.OP_CONV:
@@ -201,9 +201,9 @@ def test_c3_pair_fusion_plan(monkeypatch):
     assert len(P.build_plan(model, 1, 64, 64, train=True).ops) > len(base.ops)          # train plans are never fused
 
 
-def test_inference_plan_lowers_detect_before_the_seg_head(monkeypatch):
+def test_inference_plan_always_lowers_detect_before_the_seg_head():
     """execution order is a planner decision: the Detect layer (yaml index 25) is lowered before the seg head (24) it follows - neither reads
-    the other - so that the captured graph ends with the seg classifier conv; train plans keep the yaml order; MYOLO_DETECT_FIRST=0 too"""
+    the other - so that the captured graph ends with the seg classifier conv; train plans keep the yaml order"""
     from multiyolov5_b200 import _lib, plan as P
     from multiyolov5_b200.models.yolo import Model
     model = Model("yolov5s_city_seg.yaml")
@@ -216,11 +216,7 @@ def test_inference_plan_lowers_detect_before_the_seg_head(monkeypatch):
     assert det and seg and max(det) < min(seg)
     det, seg = first_last(P.build_plan(model, 1, 64, 128, train=True))
     assert max(seg) < min(det)
-    monkeypatch.setenv("MYOLO_DETECT_FIRST", "0")
-    det, seg = first_last(P.build_plan(model, 1, 64, 128))
-    assert max(seg) < min(det)
-    # whatever the order, the ops reading caller-owned outputs keep their inputs alive to the end of the plan
-    monkeypatch.delenv("MYOLO_DETECT_FIRST")
+    # the ops reading caller-owned outputs keep their inputs alive to the end of the plan
     pb = P.build_plan(model, 1, 64, 128)
     for o in pb.ops:
         if o.kind in (_lib.OP_DETECT_DECODE, _lib.OP_SEG_UPSAMPLE):
