@@ -29,7 +29,7 @@ struct ConvTcParams {
   int kc;                // channels per K chunk: 16 / 32 / 64  (swizzle 32B / 64B / 128B)
   int cblocks;           // Ci_pad / kc
   int taps;              // k*k
-  int n_chunks, chunks_per_stage, n_kstages;
+  int n_chunks, n_kstages;
   int tap_map[9], tap_dx[9], tap_dy[9];
   int act;
   int num_stages;

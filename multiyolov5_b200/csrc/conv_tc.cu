@@ -7,7 +7,8 @@
 //   image border (that is the conv padding).  Stride-2 convs use four "parity" tensor maps (even/odd rows x cols)
 //   so that the stride-2 gather is again a dense box.  No im2col buffer ever exists in HBM.
 // * K loop  = taps x (Ci/kc) chunks, 64 K-elements per pipeline stage; operands are K-major with the 32/64/128-byte
-//   TMA swizzle named in the wgmma shared-memory descriptor.
+//   TMA swizzle named in the wgmma shared-memory descriptor.  kc is a template parameter, so the MMAs of a stage are one
+//   straight-line block and one wgmma group.
 // * warp roles (384 threads = 3 warpgroups): warp 0 = TMA producer (one elected lane issues), warps 1-3 idle, warpgroups 1 and 2 =
 //   consumers.  Consumer warpgroup w issues m64nBNk16 wgmma for pixel rows [64w, 64w+64) of the tile into its register accumulators,
 //   releases each operand stage as soon as the MMAs that read it have retired, and runs the epilogue (bias, activation, residual,
@@ -95,11 +96,29 @@ __device__ __forceinline__ void epilogue(const ConvTcParams& p, const float (&ac
   }
 }
 
-template <int BN, bool RES>
+// the MMAs of one operand stage that holds NCH K chunks of KC channels, committed as ONE wgmma group.  Fence, MMAs and commit sit in
+// one straight-line block: with a runtime trip count, or a commit behind a branch, ptxas closes a group after every loop body and
+// turns the commit into an empty group, so waiting for "all but the newest group" drains the tensor pipe once per stage.
+template <int KC, int BN, int NCH>
+__device__ __forceinline__ void mma_stage(float (&acc)[BN / 2], uint32_t sa, uint32_t sb, uint32_t scale_first) {
+  constexpr int kRowBytes = KC * 2;
+  wgmma_fence();
+  wgmma_fence_regs(acc);
+#pragma unroll
+  for (int j = 0; j < NCH; ++j)
+#pragma unroll
+    for (int k = 0; k < KC / 16; ++k)      // 16 K-elements = 32 bytes further inside the swizzle atom
+      wgmma_f16<BN, 0, 0>(acc, make_smem_desc(sa + j * (kTileM * KC * 2) + 32 * k, kRowBytes),
+                          make_smem_desc(sb + j * (BN * KC * 2) + 32 * k, kRowBytes), (j | k) != 0 ? 1u : scale_first);
+  wgmma_commit();
+}
+
+template <int KC, int BN, bool RES>
 __global__ void __launch_bounds__(kNumThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmA3,
                const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ConvTcParams p) {
+  constexpr int kChunksPerStage = kKStage / KC;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int S = p.num_stages;
@@ -110,8 +129,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
   uint64_t* empty_bar = full_bar + S;
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);   // warp-uniform for the compiler: wgmma is issued under role branches
-  const int a_sub_bytes = kTileM * p.kc * 2;
-  const int b_sub_bytes = BN * p.kc * 2;
+  constexpr int a_sub_bytes = kTileM * KC * 2;
+  constexpr int b_sub_bytes = BN * KC * 2;
   const int tiles_per_img = p.tiles_x * p.tiles_y;
 
   // programmatic dependent launch: let the next kernel of the stream start its own prologue as early as possible
@@ -143,7 +162,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
       for (int ks = 0; ks < p.n_kstages; ++ks) {
         mbar_wait(&empty_bar[stage], phase ^ 1);
         __syncwarp();
-        const int nch = min(p.chunks_per_stage, p.n_chunks - q);
+        const int nch = min(kChunksPerStage, p.n_chunks - q);
         if (leader) mbar_arrive_expect_tx(&full_bar[stage], nch * (a_sub_bytes + b_sub_bytes));
         uint8_t* sa = smem_a + stage * p.a_stage_bytes;
         uint8_t* sb = smem_b + stage * p.b_stage_bytes;
@@ -151,8 +170,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
           const int mi = p.tap_map[tap];
           const CUtensorMap* tm = mi == 0 ? &tmA0 : (mi == 1 ? &tmA1 : (mi == 2 ? &tmA2 : &tmA3));
           if (leader) {
-            tma_load_4d(sa + j * a_sub_bytes, tm, &full_bar[stage], cb * p.kc, t.x0 + p.tap_dx[tap], t.y0 + p.tap_dy[tap], t.b);
-            tma_load_2d(sb + j * b_sub_bytes, &tmB, &full_bar[stage], q * p.kc, t.n0);
+            tma_load_4d(sa + j * a_sub_bytes, tm, &full_bar[stage], cb * KC, t.x0 + p.tap_dx[tap], t.y0 + p.tap_dy[tap], t.b);
+            tma_load_2d(sb + j * b_sub_bytes, &tmB, &full_bar[stage], q * KC, t.n0);
           }
           if (++cb == p.cblocks) { cb = 0; ++tap; }
         }
@@ -163,35 +182,36 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
     // ===================== consumers: two warpgroups, 64 pixel rows each =====================
     const int cw = (warp >> 2) - 1;
     const bool signaller = (threadIdx.x & 127) == 0;
-    const int row_bytes = p.kc * 2;
-    const int kmma = p.kc / 16;
     if (RES) asm volatile("griddepcontrol.wait;" ::: "memory");   // the residual is a predecessor's output
     float acc[BN / 2];
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     int stage = 0;
     uint32_t phase = 0;
-    const uint32_t a_base = smem_u32(smem_a) + (uint32_t)(cw * 64 * row_bytes);
+    const uint32_t a_base = smem_u32(smem_a) + (uint32_t)(cw * 64 * KC * 2);
     const uint32_t b_base = smem_u32(smem_b);
+    const int n_full = p.n_chunks / kChunksPerStage;     // stages with kChunksPerStage chunks; a last one holds the remaining chunks
+    const int n_tail = p.n_chunks - n_full * kChunksPerStage;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const TileCoord t = decode_tile(p, tile, tiles_per_img);
-      int q = 0, prev = -1;
+      int prev = -1;
       for (int ks = 0; ks < p.n_kstages; ++ks) {
         mbar_wait(&full_bar[stage], phase);
-        const int nch = min(p.chunks_per_stage, p.n_chunks - q);
         const uint32_t sa = a_base + (uint32_t)(stage * p.a_stage_bytes);
         const uint32_t sb = b_base + (uint32_t)(stage * p.b_stage_bytes);
-        wgmma_fence();
-        wgmma_fence_regs(acc);
-        for (int j = 0; j < nch; ++j)
-          for (int k = 0; k < kmma; ++k)      // 16 K-elements = 32 bytes further inside the swizzle atom
-            wgmma_f16<BN, 0, 0>(acc, make_smem_desc(sa + j * a_sub_bytes + 32 * k, row_bytes),
-                                make_smem_desc(sb + j * b_sub_bytes + 32 * k, row_bytes), (uint32_t)((ks | j | k) != 0));
-        wgmma_commit();
+        const uint32_t scale_first = ks != 0;
+        if (kChunksPerStage == 1 || ks < n_full) {
+          mma_stage<KC, BN, kChunksPerStage>(acc, sa, sb, scale_first);
+        } else if constexpr (kChunksPerStage > 1) {
+          if (n_tail == 1) mma_stage<KC, BN, 1>(acc, sa, sb, scale_first);
+          if constexpr (kChunksPerStage > 2) {
+            if (n_tail == 2) mma_stage<KC, BN, 2>(acc, sa, sb, scale_first);
+            if (n_tail == 3) mma_stage<KC, BN, 3>(acc, sa, sb, scale_first);
+          }
+        }
         wgmma_wait<1>();                        // the previous stage's MMAs have retired: its operands may be overwritten
         if (prev >= 0 && signaller) mbar_arrive(&empty_bar[prev]);
         prev = stage;
-        q += nch;
         if (++stage == S) { stage = 0; phase ^= 1; }
       }
       wgmma_wait<0>();
@@ -317,8 +337,7 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
   p.cblocks = op.Ci_pad / p.kc;
   p.taps = op.k * op.k;
   p.n_chunks = p.taps * p.cblocks;
-  p.chunks_per_stage = kKStage / p.kc;
-  p.n_kstages = ceil_div(p.n_chunks, p.chunks_per_stage);
+  p.n_kstages = ceil_div(p.n_chunks, kKStage / p.kc);
   p.act = op.act;
   p.bias = op.bias;
   p.residual = op.has_res ? reinterpret_cast<const __half*>(op.res.base) : nullptr;
@@ -391,34 +410,45 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
   return 0;
 }
 
-template <int BN, bool RES>
+template <int KC, int BN, bool RES>
 static cudaError_t launch_bn(const ConvOp& op, const cudaLaunchConfig_t& cfg) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<BN, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<KC, BN, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  return cudaLaunchKernelEx(&cfg, conv_tc_kernel<BN, RES>, op.tmA[0], op.tmA[1], op.tmA[2], op.tmA[3], op.tmB, op.p);
+  return cudaLaunchKernelEx(&cfg, conv_tc_kernel<KC, BN, RES>, op.tmA[0], op.tmA[1], op.tmA[2], op.tmA[3], op.tmB, op.p);
+}
+
+template <int KC, bool RES>
+static cudaError_t launch_kc(const ConvOp& op, const cudaLaunchConfig_t& cfg) {
+  switch (op.p.BN) {
+    case 16: return launch_bn<KC, 16, RES>(op, cfg);
+    case 32: return launch_bn<KC, 32, RES>(op, cfg);
+    case 48: return launch_bn<KC, 48, RES>(op, cfg);
+    case 64: return launch_bn<KC, 64, RES>(op, cfg);
+    case 80: return launch_bn<KC, 80, RES>(op, cfg);
+    case 96: return launch_bn<KC, 96, RES>(op, cfg);
+    case 112: return launch_bn<KC, 112, RES>(op, cfg);
+    case 128: return launch_bn<KC, 128, RES>(op, cfg);
+  }
+  return cudaErrorInvalidValue;
 }
 
 template <bool RES>
 static cudaError_t launch_res(const ConvOp& op, const cudaLaunchConfig_t& cfg) {
-  switch (op.p.BN) {
-    case 16: return launch_bn<16, RES>(op, cfg);
-    case 32: return launch_bn<32, RES>(op, cfg);
-    case 48: return launch_bn<48, RES>(op, cfg);
-    case 64: return launch_bn<64, RES>(op, cfg);
-    case 80: return launch_bn<80, RES>(op, cfg);
-    case 96: return launch_bn<96, RES>(op, cfg);
-    case 112: return launch_bn<112, RES>(op, cfg);
-    case 128: return launch_bn<128, RES>(op, cfg);
+  switch (op.p.kc) {
+    case 16: return launch_kc<16, RES>(op, cfg);
+    case 32: return launch_kc<32, RES>(op, cfg);
+    case 64: return launch_kc<64, RES>(op, cfg);
   }
   return cudaErrorInvalidValue;
 }
 
 int conv_tc_launch(const ConvOp& op, cudaStream_t stream) {
   MYOLO_REQUIRE(op.p.BN % 16 == 0 && op.p.BN >= 16 && op.p.BN <= 128, "conv_tc: unsupported N tile %d", op.p.BN);
+  MYOLO_REQUIRE(op.p.kc == 16 || op.p.kc == 32 || op.p.kc == 64, "conv_tc: unsupported K chunk %d", op.p.kc);
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(op.grid);
   cfg.blockDim = dim3(kNumThreads);
