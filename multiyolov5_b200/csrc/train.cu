@@ -27,6 +27,11 @@ __device__ __forceinline__ void stv(const TensorView& v, int b, int y, int x, in
   if (v.dtype == MYOLO_F32) tvf(v, b, y, x)[c] = f;
   else tv(v, b, y, x)[c] = __float2half_rn(f);
 }
+// the per-channel shift of the BN statistics sums: the value at the centre pixel of image 0 (an interior pixel: a corner, the first
+// pixel, sees the zero padding of every 3x3 conv before it and on flat content lies farther from the mean than 0 does)
+__device__ __forceinline__ const __half* bn_shift_ptr(const TensorView& u) {
+  return reinterpret_cast<const __half*>(u.base) + ((size_t)(u.H / 2) * u.W + u.W / 2) * u.ctot;
+}
 __device__ __forceinline__ float act_fwd(float z, int act) {
   if (act == MYOLO_ACT_SILU) return z / (1.0f + __expf(-z));
   if (act == MYOLO_ACT_SIGMOID) return 1.0f / (1.0f + __expf(-z));
@@ -60,10 +65,11 @@ __global__ void chan_reduce_kernel(TensorView a, TensorView bview, const float* 
   if (c < C) {
     float mean = 0.f, istd = 0.f, g = 0.f, bt = 0.f;
     if (MODE == 1) { mean = stats[c]; istd = stats[C + c]; g = gamma[c]; bt = beta[c]; }
+    const float shift = MODE == 0 ? __half2float(bn_shift_ptr(a)[c]) : 0.f;     // MODE 0 sums u - shift (see chan_reduce_v_kernel)
     for (long p = p0 + lane_p; p < p1; p += 8) {
       const size_t off = (size_t)p * a.ctot + c;
       if (MODE == 0) {
-        const float u = __half2float(reinterpret_cast<const __half*>(a.base)[off]);
+        const float u = __half2float(reinterpret_cast<const __half*>(a.base)[off]) - shift;
         s0 += u; s1 += u * u;
       } else if (MODE == 1) {
         const float xh = (__half2float(reinterpret_cast<const __half*>(a.base)[off]) - mean) * istd;
@@ -89,6 +95,10 @@ __global__ void chan_reduce_kernel(TensorView a, TensorView bview, const float* 
 // per pixel), the block's threads tile (pixel lanes x channel vectors) so a pixel's channels are read as one contiguous run; per-block
 // partials are combined through shared memory and added atomically; the LAST block to finish (ticket) runs the per-channel epilogue:
 //   MODE 0: mean / inverse std -> stats, running-statistics update        MODE 1: dgamma += sum(dz*xhat), dbeta += sum(dz)
+// MODE 0 sums d = u - shift and d^2 with shift = one of the channel's own values (bn_shift_ptr): var = E[d^2] - E[d]^2 then cancels only
+// on the distance of the mean from that value.  Summing u itself loses the variance of a channel whose mean is large against its spread
+// (flat image content: letterbox padding, sky, road): at mean/std = 200 the fp32 E[u^2] - mean^2 is off by ~1e-2 of the normalised output.
+// final_out (MODE 0, deferred running statistics): batch mean and biased variance; (MODE 1): the two sums.
 template <int MODE>
 __global__ void __launch_bounds__(256) chan_reduce_v_kernel(TensorView a, TensorView bview, const float* __restrict__ stats,
                                                             const float* __restrict__ gamma, const float* __restrict__ beta, int act,
@@ -112,12 +122,18 @@ __global__ void __launch_bounds__(256) chan_reduce_v_kernel(TensorView a, Tensor
     }
     const __half* ab = reinterpret_cast<const __half*>(a.base);
     const __half* bb = reinterpret_cast<const __half*>(bview.base);
+    float shift[8];
+    if (MODE == 0) {
+      const uint4 q0 = *reinterpret_cast<const uint4*>(bn_shift_ptr(a) + cv * 8);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) shift[k] = __half2float(reinterpret_cast<const __half*>(&q0)[k]);
+    }
     for (long p = (long)blockIdx.x * lanes + lane; p < npix; p += (long)gridDim.x * lanes) {
       const uint4 q = *reinterpret_cast<const uint4*>(ab + (size_t)p * a.ctot + cv * 8);
       const __half* h = reinterpret_cast<const __half*>(&q);
       if (MODE == 0) {
 #pragma unroll
-        for (int k = 0; k < 8; ++k) { const float u = __half2float(h[k]); s0[k] += u; s1[k] += u * u; }
+        for (int k = 0; k < 8; ++k) { const float u = __half2float(h[k]) - shift[k]; s0[k] += u; s1[k] += u * u; }
       } else {
         const uint4 r = *reinterpret_cast<const uint4*>(bb + (size_t)p * bview.ctot + cv * 8);
         const __half* hr = reinterpret_cast<const __half*>(&r);
@@ -152,11 +168,12 @@ __global__ void __launch_bounds__(256) chan_reduce_v_kernel(TensorView a, Tensor
     const float x0 = __ldcg(out + c), x1 = __ldcg(out + C + c);
     out[c] = 0.f;
     out[C + c] = 0.f;
-    if (final_out) { final_out[c] = x0; final_out[C + c] = x1; }
     if (MODE == 0) {
       const float n = (float)npix;
-      const float mean = x0 / n;
-      const float var = fmaxf(x1 / n - mean * mean, 0.f);          // biased variance normalises (F.batch_norm, training=True)
+      const float d = x0 / n;
+      const float mean = __half2float(bn_shift_ptr(a)[c]) + d;
+      const float var = fmaxf(x1 / n - d * d, 0.f);                // biased variance normalises (F.batch_norm, training=True)
+      if (final_out) { final_out[c] = mean; final_out[C + c] = var; }
       stats_out[c] = mean;
       stats_out[C + c] = rsqrtf(var + bn.eps);
       if (bn.running_mean) {                                       // running stats: unbiased variance, momentum 0.03
@@ -164,6 +181,7 @@ __global__ void __launch_bounds__(256) chan_reduce_v_kernel(TensorView a, Tensor
         bn.running_var[c] = (1.f - bn.momentum) * bn.running_var[c] + bn.momentum * var * (n / fmaxf(n - 1.f, 1.f));
       }
     } else {
+      if (final_out) { final_out[c] = x0; final_out[C + c] = x1; }
       // parameter gradients are accumulated atomically everywhere: the det and the seg backward of one training step may run concurrently
       if (bn.d_beta) atomicAdd(bn.d_beta + c, x0);
       if (bn.d_gamma) atomicAdd(bn.d_gamma + c, x1);
@@ -175,12 +193,14 @@ static inline int reduce_v_grid(long npix, int C) {
   return (int)std::max<long>(1, std::min<long>(132 * 2, npix / ((long)lanes * 4)));
 }
 
-__global__ void bn_finalize_kernel(float* sums, float* stats, BnParams bn, long npix) {
+// sums of u - shift (chan_reduce_kernel<0>): the shift is read back from u
+__global__ void bn_finalize_kernel(TensorView u, float* sums, float* stats, BnParams bn, long npix) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= bn.C) return;
   const float n = (float)npix;
-  const float mean = sums[c] / n;
-  const float var = fmaxf(sums[bn.C + c] / n - mean * mean, 0.f);           // biased variance normalises (F.batch_norm, training=True)
+  const float d = sums[c] / n;
+  const float mean = __half2float(bn_shift_ptr(u)[c]) + d;
+  const float var = fmaxf(sums[bn.C + c] / n - d * d, 0.f);                 // biased variance normalises (F.batch_norm, training=True)
   stats[c] = mean;
   stats[bn.C + c] = rsqrtf(var + bn.eps);
   if (bn.running_mean) {                                                       // running stats: unbiased variance, momentum 0.03
@@ -189,13 +209,14 @@ __global__ void bn_finalize_kernel(float* sums, float* stats, BnParams bn, long 
   }
 }
 
-// deferred running statistics: one launch applies r <- (1-m) r + m * stat for every BN layer of a plan from the sums its last forward left
+// deferred running statistics: one launch applies r <- (1-m) r + m * stat for every BN layer of a plan from the batch mean and biased
+// variance its last forward left (computed from shifted sums by chan_reduce_v_kernel<0>)
 __global__ void __launch_bounds__(256) bn_apply_running_kernel(const RunningJob* __restrict__ jobs) {
   const RunningJob j = jobs[blockIdx.x];
   const float n = (float)j.npix;
   for (int c = threadIdx.x; c < j.C; c += 256) {
-    const float mean = j.sums[c] / n;
-    const float var = fmaxf(j.sums[j.C + c] / n - mean * mean, 0.f);
+    const float mean = j.batch_stats[c];
+    const float var = j.batch_stats[j.C + c];
     j.running_mean[c] = (1.f - j.momentum) * j.running_mean[c] + j.momentum * mean;
     j.running_var[c] = (1.f - j.momentum) * j.running_var[c] + j.momentum * var * (n / fmaxf(n - 1.f, 1.f));
   }
@@ -214,7 +235,8 @@ int launch_bn_stats(const TensorView& u, const BnParams& bn_in, float* stats, fl
   MYOLO_REQUIRE(!defer_running || (u.C % 8 == 0 && u.C <= 2048 && u.ctot % 8 == 0), "bn_stats: deferred running statistics need C %% 8 == 0");
   if (defer_running) bn.running_mean = bn.running_var = nullptr;     // the sums stay in scratch + 2C for myolo_plan_apply_running
   const long npix = (long)u.B * u.H * u.W;
-  // scratch (zero on entry, left zero by the kernel): 2*C sums, 2*C final sums (backward), the completion ticket
+  // scratch (zero on entry, left zero by the kernel): 2*C sums, 2*C final values (batch mean / variance of a deferring plan, the backward's
+  // sums), the completion ticket
   if (u.C % 8 == 0 && u.C <= 2048 && u.ctot % 8 == 0) {
     MYOLO_CHECK_CUDA(launch_pdl(chan_reduce_v_kernel<0>, dim3(reduce_v_grid(npix, u.C)), dim3(256), 0, s, u, u, (const float*)nullptr,
                                 (const float*)nullptr, (const float*)nullptr, 0, scratch, npix, u.C, bn, stats,
@@ -226,7 +248,7 @@ int launch_bn_stats(const TensorView& u, const BnParams& bn_in, float* stats, fl
   dim3 g(ceil_div(u.C, 32), (unsigned)std::min<long>(256, std::max<long>(1, npix / 256)));
   chan_reduce_kernel<0><<<g, 256, 0, s>>>(u, u, nullptr, nullptr, nullptr, 0, scratch, npix, u.C);
   MYOLO_LAUNCH_CHECK();
-  bn_finalize_kernel<<<ceil_div(u.C, 128), 128, 0, s>>>(scratch, stats, bn, npix);
+  bn_finalize_kernel<<<ceil_div(u.C, 128), 128, 0, s>>>(u, scratch, stats, bn, npix);
   MYOLO_LAUNCH_CHECK();
   MYOLO_CHECK_CUDA(cudaMemsetAsync(scratch, 0, (2 * (size_t)u.C) * sizeof(float), s));    // contract of the scratch: zero between launches
   return 0;

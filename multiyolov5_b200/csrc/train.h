@@ -22,10 +22,10 @@ struct BnParams {           // device pointers owned by the caller (nn.BatchNorm
 // ---- forward ----
 // per-channel mean / inverse std over (B,H,W) of u (fp16 NHWC view) -> stats[0..C) = mean, stats[C..2C) = invstd; updates running stats
 int launch_bn_stats(const TensorView& u, const BnParams& bn, float* stats, float* scratch, cudaStream_t s, bool defer_running = false);
-struct RunningJob {         // one BN layer of a deferred running-statistics update (sums = [sum | sum of squares] over npix values)
+struct RunningJob {         // one BN layer of a deferred running-statistics update (batch_stats = [mean | biased variance] of npix values)
   float* running_mean;
   float* running_var;
-  const float* sums;
+  const float* batch_stats;
   int C;
   long npix;
   float momentum;
