@@ -34,6 +34,12 @@ struct ConvTcParams {
   int act;
   int num_stages;
   int a_stage_bytes, b_stage_bytes;
+  int resident;          // 1: the CTA's whole weight slice stays in shared memory (one slot per K chunk), loaded by its first tile
+  int b_bytes;           // shared memory of the weight region: resident slots or num_stages ring stages
+  int strip;             // 1: 3x3 stride 1, one A box {kc, tw + 2 dil, th} per filter row and channel block feeds the row's three taps
+  int strip_w;           // tw + 2 dil: pixels per strip row
+  int strip_box_bytes, strip_sub_bytes;   // bytes of one strip box / its 1024-aligned slot in the stage
+  int dil;
   int out_mode;          // 0: fp16 NHWC slice, 1: fp32 NHWC
   int out_c, out_ctot;   // channels of the output slice / channel pitch of its buffer
   const float* bias;
@@ -52,6 +58,7 @@ struct ConvOp {
   const float* bias = nullptr;
   int Ci_pad = 0, Co_pad = 0, Co = 0;
   bool use_tc = false;
+  bool reuse = true;          // false: streamed weights, one ring stage per K step (the reference layout of the standalone entry's path 3)
   // tensor-core path state (built once at plan creation)
   CUtensorMap tmA[4], tmB;
   ConvTcParams p;

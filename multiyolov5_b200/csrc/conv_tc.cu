@@ -9,6 +9,8 @@
 // * K loop  = taps x (Ci/kc) chunks, 64 K-elements per pipeline stage; operands are K-major with the 32/64/128-byte
 //   TMA swizzle named in the wgmma shared-memory descriptor.  kc is a template parameter, so the MMAs of a stage are one
 //   straight-line block and one wgmma group.
+// * operand reuse: a weight slice that fits next to six A stages stays resident for the CTA's whole persistent loop, and 3x3 stride-1
+//   layers with resident weights load one strip {kc, tw + 2 dil, th, 1} per filter row that serves its three kx taps (conv_tc_prepare).
 // * warp roles (384 threads = 3 warpgroups): warp 0 = TMA producer (one elected lane issues), warps 1-3 idle, warpgroups 1 and 2 =
 //   consumers.  Consumer warpgroup w issues m64nBNk16 wgmma for pixel rows [64w, 64w+64) of the tile into its register accumulators,
 //   releases each operand stage as soon as the MMAs that read it have retired, and runs the epilogue (bias, activation, residual,
@@ -26,6 +28,9 @@ static constexpr int kTileM = 128;
 static constexpr int kKStage = 64;        // K elements per pipeline stage
 static constexpr int kNumThreads = 384;   // producer warpgroup + two consumer warpgroups
 static constexpr int kMaxStages = 8;
+static constexpr int kMinResidentStages = 6;   // A stages a layer keeps next to resident weights (with 4, the 144 KB pack of the
+                                               // 3x3 s2 64->128 layer left 4 stages and ran 5 us slower than streamed with 6)
+static constexpr int kMaxStripBlocks = 4;      // channel blocks of a strip-mode layer (mma_strip_row instantiations)
 static constexpr int kSmemBudget = 227 * 1024;
 static constexpr int kBiasBytes = 8192;   // bias vector of the layer in shared memory (<= 1920 output channels: the data gradient
                                           // of SPP.cv2 has 1024)
@@ -64,10 +69,32 @@ __device__ __forceinline__ float act_out(float v, int act, int ch) {
   return v;
 }
 
+// the residual values of the thread's epilogue fragment, all loads in flight at once.  Issued before the tile's last MMAs retire: loaded
+// one by one inside the store loop, each load waits behind the previous store (the output may alias the residual, as it does in the
+// data-gradient convs), and a tile's epilogue pays the global-load latency 2 * BN / 8 times.
+template <int BN>
+__device__ __forceinline__ void load_residual(const ConvTcParams& p, const TileCoord& tc, int row0, __half2 (&res)[2][BN / 8]) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int row = row0 + (lane >> 2) + 8 * h;
+    const int py = tc.y0 + (row >> p.log2_tw), px = tc.x0 + (row & (p.tw - 1));
+    const bool in_map = py < p.Ho && px < p.Wo;
+    const size_t pix = ((size_t)tc.b * p.Ho + py) * p.Wo + px;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int n = tc.n0 + 8 * j + 2 * (lane & 3);
+      res[h][j] = in_map && n < p.out_c && n < p.Co ? *reinterpret_cast<const __half2*>(p.residual + pix * p.res_ctot + n)
+                                                     : __floats2half2_rn(0.f, 0.f);
+    }
+  }
+}
+
 // epilogue of one consumer warpgroup: the m64nBN accumulator fragment holds, for j < BN/8 and h < 2, output channels 8j + 2(lane%4) + {0,1}
 // of tile row 16*(warp%4) + lane/4 + 8h, in acc[4j + 2h + {0,1}]
 template <int BN, bool RES>
-__device__ __forceinline__ void epilogue(const ConvTcParams& p, const float (&acc)[BN / 2], const float* bias_s, const TileCoord& tc, int row0) {
+__device__ __forceinline__ void epilogue(const ConvTcParams& p, const float (&acc)[BN / 2], const __half2 (&res)[2][BN / 8],
+                                         const float* bias_s, const TileCoord& tc, int row0) {
   const int lane = threadIdx.x & 31;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -84,7 +111,7 @@ __device__ __forceinline__ void epilogue(const ConvTcParams& p, const float (&ac
       if (p.out_mode == 0) {
         if (n >= p.out_c) continue;
         if (RES && n < p.Co) {
-          const float2 r = __half22float2(*reinterpret_cast<const __half2*>(p.residual + pix * p.res_ctot + n));
+          const float2 r = __half22float2(res[h][j]);
           v0 += r.x;
           v1 += r.y;
         }
@@ -113,6 +140,26 @@ __device__ __forceinline__ void mma_stage(float (&acc)[BN / 2], uint32_t sa, uin
   wgmma_commit();
 }
 
+// strip mode: the MMAs of one filter row ky, its three kx taps x CB channel blocks in the K order of the per-tap path (taps outer,
+// channel blocks inner), one wgmma group.  Tap kx reads the strip dx_bytes * kx further on: a start address off the 8-row swizzle
+// atom is fine, since wgmma applies the swizzle to absolute shared-memory address bits as TMA does (matrix base offset stays 0).
+template <int KC, int BN, int CB>
+__device__ __forceinline__ void mma_strip_row(float (&acc)[BN / 2], uint32_t sa, uint32_t sb, uint32_t strip_sub_bytes, uint32_t dx_bytes,
+                                              uint32_t scale_first) {
+  constexpr int kRowBytes = KC * 2;
+  wgmma_fence();
+  wgmma_fence_regs(acc);
+#pragma unroll
+  for (int kx = 0; kx < 3; ++kx)
+#pragma unroll
+    for (int c = 0; c < CB; ++c)
+#pragma unroll
+      for (int k = 0; k < KC / 16; ++k)
+        wgmma_f16<BN, 0, 0>(acc, make_smem_desc(sa + kx * dx_bytes + c * strip_sub_bytes + 32 * k, kRowBytes),
+                            make_smem_desc(sb + (kx * CB + c) * (BN * KC * 2) + 32 * k, kRowBytes), (kx | c | k) != 0 ? 1u : scale_first);
+  wgmma_commit();
+}
+
 template <int KC, int BN, bool RES>
 __global__ void __launch_bounds__(kNumThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
@@ -123,8 +170,8 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int S = p.num_stages;
   uint8_t* smem_a = smem;
-  uint8_t* smem_b = smem_a + S * p.a_stage_bytes;
-  float* bias_s = reinterpret_cast<float*>(smem_b + S * p.b_stage_bytes);   // [n_tiles_n * BN] fp32
+  uint8_t* smem_b = smem_a + S * p.a_stage_bytes;                         // resident: K chunk q in slot q; else one ring stage per A stage
+  float* bias_s = reinterpret_cast<float*>(smem_b + p.b_bytes);           // [n_tiles_n * BN] fp32
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(bias_s) + kBiasBytes);
   uint64_t* empty_bar = full_bar + S;
 
@@ -153,25 +200,44 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
   if (warp == 0) {
     // ===================== TMA producer (warp-converged; one elected lane issues) =====================
     const bool leader = elect_one();
-    asm volatile("griddepcontrol.wait;" ::: "memory");   // activations come from predecessor kernels
+    // Activations come from predecessor kernels.  The weights are loaded after this wait as well: the training step repacks them
+    // (myolo_plan_repack_weights) on the same stream before the forward, and only this wait orders that repack before the loads.
+    asm volatile("griddepcontrol.wait;" ::: "memory");
     int stage = 0;
     uint32_t phase = 0;
+    const int n_units = p.strip ? 3 : p.n_kstages;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const TileCoord t = decode_tile(p, tile, tiles_per_img);
+      // resident weights: the first tile fills the slots as its K loop reaches them (gridDim.x is a multiple of n_tiles_n, so every
+      // tile of this CTA has the same N tile); later tiles load A only
+      const bool load_b = !p.resident || tile == (int)blockIdx.x;
       int tap = 0, cb = 0, q = 0;
-      for (int ks = 0; ks < p.n_kstages; ++ks) {
+      for (int ks = 0; ks < n_units; ++ks) {
         mbar_wait(&empty_bar[stage], phase ^ 1);
         __syncwarp();
+        if (p.strip) {   // stage = filter row ks: one strip per channel block (x0 - dil .. x0 + tw + dil), weights of its 3 taps
+          const int nq = 3 * p.cblocks;
+          if (leader) {
+            mbar_arrive_expect_tx(&full_bar[stage], p.cblocks * p.strip_box_bytes + (load_b ? nq * b_sub_bytes : 0));
+            uint8_t* sa = smem_a + stage * p.a_stage_bytes;
+            for (int c = 0; c < p.cblocks; ++c)
+              tma_load_4d(sa + c * p.strip_sub_bytes, &tmA0, &full_bar[stage], c * KC, t.x0 - p.dil, t.y0 + (ks - 1) * p.dil, t.b);
+            if (load_b)
+              for (int j = ks * nq; j < (ks + 1) * nq; ++j) tma_load_2d(smem_b + j * b_sub_bytes, &tmB, &full_bar[stage], j * KC, t.n0);
+          }
+          if (++stage == S) { stage = 0; phase ^= 1; }
+          continue;
+        }
         const int nch = min(kChunksPerStage, p.n_chunks - q);
-        if (leader) mbar_arrive_expect_tx(&full_bar[stage], nch * (a_sub_bytes + b_sub_bytes));
+        if (leader) mbar_arrive_expect_tx(&full_bar[stage], nch * (a_sub_bytes + (load_b ? b_sub_bytes : 0)));
         uint8_t* sa = smem_a + stage * p.a_stage_bytes;
-        uint8_t* sb = smem_b + stage * p.b_stage_bytes;
+        uint8_t* sb = p.resident ? smem_b + q * b_sub_bytes : smem_b + stage * p.b_stage_bytes;
         for (int j = 0; j < nch; ++j, ++q) {
           const int mi = p.tap_map[tap];
           const CUtensorMap* tm = mi == 0 ? &tmA0 : (mi == 1 ? &tmA1 : (mi == 2 ? &tmA2 : &tmA3));
           if (leader) {
             tma_load_4d(sa + j * a_sub_bytes, tm, &full_bar[stage], cb * KC, t.x0 + p.tap_dx[tap], t.y0 + p.tap_dy[tap], t.b);
-            tma_load_2d(sb + j * b_sub_bytes, &tmB, &full_bar[stage], q * KC, t.n0);
+            if (load_b) tma_load_2d(sb + j * b_sub_bytes, &tmB, &full_bar[stage], q * KC, t.n0);
           }
           if (++cb == p.cblocks) { cb = 0; ++tap; }
         }
@@ -192,21 +258,36 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
     const uint32_t b_base = smem_u32(smem_b);
     const int n_full = p.n_chunks / kChunksPerStage;     // stages with kChunksPerStage chunks; a last one holds the remaining chunks
     const int n_tail = p.n_chunks - n_full * kChunksPerStage;
+    const int n_units = p.strip ? 3 : p.n_kstages;
+    // strip mode: this warpgroup's 64 output pixels start at strip row (64 cw) mod tw, in strip line (64 cw) / tw
+    const uint32_t strip_base = smem_u32(smem_a) + (uint32_t)((((cw * 64) & (p.tw - 1)) + ((cw * 64) >> p.log2_tw) * p.strip_w) * KC * 2);
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
       const TileCoord t = decode_tile(p, tile, tiles_per_img);
       int prev = -1;
-      for (int ks = 0; ks < p.n_kstages; ++ks) {
+      for (int ks = 0; ks < n_units; ++ks) {
         mbar_wait(&full_bar[stage], phase);
-        const uint32_t sa = a_base + (uint32_t)(stage * p.a_stage_bytes);
-        const uint32_t sb = b_base + (uint32_t)(stage * p.b_stage_bytes);
         const uint32_t scale_first = ks != 0;
-        if (kChunksPerStage == 1 || ks < n_full) {
-          mma_stage<KC, BN, kChunksPerStage>(acc, sa, sb, scale_first);
-        } else if constexpr (kChunksPerStage > 1) {
-          if (n_tail == 1) mma_stage<KC, BN, 1>(acc, sa, sb, scale_first);
-          if constexpr (kChunksPerStage > 2) {
-            if (n_tail == 2) mma_stage<KC, BN, 2>(acc, sa, sb, scale_first);
-            if (n_tail == 3) mma_stage<KC, BN, 3>(acc, sa, sb, scale_first);
+        if (p.strip) {
+          const uint32_t sa = strip_base + (uint32_t)(stage * p.a_stage_bytes);
+          const uint32_t sb = b_base + (uint32_t)(ks * 3 * p.cblocks * b_sub_bytes);
+          const uint32_t dx = (uint32_t)(p.dil * KC * 2), ss = (uint32_t)p.strip_sub_bytes;
+          switch (p.cblocks) {
+            case 1: mma_strip_row<KC, BN, 1>(acc, sa, sb, ss, dx, scale_first); break;
+            case 2: mma_strip_row<KC, BN, 2>(acc, sa, sb, ss, dx, scale_first); break;
+            case 3: mma_strip_row<KC, BN, 3>(acc, sa, sb, ss, dx, scale_first); break;
+            default: mma_strip_row<KC, BN, 4>(acc, sa, sb, ss, dx, scale_first); break;
+          }
+        } else {
+          const uint32_t sa = a_base + (uint32_t)(stage * p.a_stage_bytes);
+          const uint32_t sb = b_base + (uint32_t)(p.resident ? ks * (kChunksPerStage * b_sub_bytes) : stage * p.b_stage_bytes);
+          if (kChunksPerStage == 1 || ks < n_full) {
+            mma_stage<KC, BN, kChunksPerStage>(acc, sa, sb, scale_first);
+          } else if constexpr (kChunksPerStage > 1) {
+            if (n_tail == 1) mma_stage<KC, BN, 1>(acc, sa, sb, scale_first);
+            if constexpr (kChunksPerStage > 2) {
+              if (n_tail == 2) mma_stage<KC, BN, 2>(acc, sa, sb, scale_first);
+              if (n_tail == 3) mma_stage<KC, BN, 3>(acc, sa, sb, scale_first);
+            }
           }
         }
         wgmma_wait<1>();                        // the previous stage's MMAs have retired: its operands may be overwritten
@@ -214,10 +295,13 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
         prev = stage;
         if (++stage == S) { stage = 0; phase ^= 1; }
       }
+      const int row0 = cw * 64 + (warp & 3) * 16;
+      __half2 res[2][BN / 8];
+      if constexpr (RES) load_residual<BN>(p, t, row0, res);
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       if (prev >= 0 && signaller) mbar_arrive(&empty_bar[prev]);
-      epilogue<BN, RES>(p, acc, bias_s, t, cw * 64 + (warp & 3) * 16);
+      epilogue<BN, RES>(p, acc, res, bias_s, t, row0);
     }
   }
 }
@@ -363,18 +447,42 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
   p.fd_ntn = make_fastdiv((unsigned)p.n_tiles_n);
   p.fd_tpi = make_fastdiv((unsigned)(p.tiles_x * p.tiles_y));
   p.fd_tx = make_fastdiv((unsigned)p.tiles_x);
-  // stage geometry: one CTA per SM with as deep an operand ring as shared memory allows
+  // stage geometry: one CTA per SM with as deep an operand ring as shared memory allows.  The weight slice of one N tile stays resident
+  // when it fits next to kMinResidentStages A stages and every CTA of the persistent grid keeps one N tile (grid % n_tiles_n == 0):
+  // a CTA then reads its weights from L2 once instead of once per tile.
   p.a_stage_bytes = kTileM * kKStage * 2;
   p.b_stage_bytes = (int)align_up(p.BN * kKStage * 2, 1024);
-  const int stage_bytes = p.a_stage_bytes + p.b_stage_bytes;
   const int misc = 1024 /*barriers*/ + kBiasBytes + 1024 /*alignment slack*/;
-  int S = (kSmemBudget - misc) / stage_bytes;
+  const int b_resident_bytes = (int)align_up(p.n_chunks * p.BN * p.kc * 2, 1024);
+  int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
+  const int grid_resident = grid / p.n_tiles_n * p.n_tiles_n;
+  p.resident = op.reuse && grid_resident > 0 && b_resident_bytes + kMinResidentStages * p.a_stage_bytes + misc <= kSmemBudget;
+  // strip mode (3x3 stride 1 with resident weights, tw >= 64 so that each consumer's 64 pixels lie in one strip line): a stage holds
+  // one filter row's strips of all channel blocks; at least two such stages must fit
+  p.dil = op.dil;
+  if (p.resident && op.k == 3 && op.stride == 1 && p.tw >= 64 && p.cblocks <= kMaxStripBlocks && p.tw + 2 * op.dil <= 256) {
+    p.strip_w = p.tw + 2 * op.dil;
+    p.strip_box_bytes = p.strip_w * p.th * p.kc * 2;
+    p.strip_sub_bytes = (int)align_up(p.strip_box_bytes, 1024);
+    p.strip = (kSmemBudget - misc - b_resident_bytes) / (p.cblocks * p.strip_sub_bytes) >= 2;
+  }
+  int S;
+  if (p.resident) {
+    grid = grid_resident;
+    p.b_stage_bytes = 0;
+    if (p.strip) p.a_stage_bytes = p.cblocks * p.strip_sub_bytes;
+    S = (kSmemBudget - misc - b_resident_bytes) / p.a_stage_bytes;
+    p.b_bytes = b_resident_bytes;
+  } else {
+    S = (kSmemBudget - misc) / (p.a_stage_bytes + p.b_stage_bytes);
+  }
   if (S > kMaxStages) S = kMaxStages;
   MYOLO_REQUIRE(S >= 2, "conv_tc: not enough shared memory for 2 stages");
   MYOLO_REQUIRE(p.n_tiles_n * p.BN * 4 <= kBiasBytes, "conv_tc: %d output channels exceed the shared-memory bias buffer", p.n_tiles_n * p.BN);
   p.num_stages = S;
-  op.smem = S * stage_bytes + misc;
-  op.grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
+  if (!p.resident) p.b_bytes = S * p.b_stage_bytes;
+  op.smem = S * p.a_stage_bytes + p.b_bytes + misc;
+  op.grid = grid;
 
   // ---- tensor maps ----
   const int esz = 2;
@@ -383,7 +491,7 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
   if (op.stride == 1) {
     uint64_t dims[4] = {(uint64_t)in.C, (uint64_t)in.W, (uint64_t)in.H, (uint64_t)in.B};
     uint64_t str[3] = {(uint64_t)in.ctot * esz, (uint64_t)in.W * in.ctot * esz, (uint64_t)in.H * in.W * in.ctot * esz};
-    uint32_t box[4] = {(uint32_t)p.kc, (uint32_t)p.tw, (uint32_t)p.th, 1};
+    uint32_t box[4] = {(uint32_t)p.kc, (uint32_t)(p.strip ? p.strip_w : p.tw), (uint32_t)p.th, 1};
     int rc = encode_map(&op.tmA[0], 4, in.base, dims, str, box, sw);
     if (rc) return rc;
     op.tmA[1] = op.tmA[2] = op.tmA[3] = op.tmA[0];

@@ -676,7 +676,8 @@ extern "C" int myolo_plan_profile(myolo_plan* pl, const void* x, int x_dtype, fl
 extern "C" int64_t myolo_plan_last_launch_count(const myolo_plan* pl) { return pl ? pl->last_launches : 0; }
 
 // which kernel a conv op of the plan takes and how it is tiled (valid after the first forward): info[0..11] =
-// {1 wgmma / 0 CUDA-core, grid, dynamic smem bytes, BN, pipeline stages, mode (always 0: one TMA box per tap), weights-stationary (always 0),
+// {1 wgmma / 0 CUDA-core, grid, dynamic smem bytes, BN, pipeline stages, mode (0: one TMA box per tap, 1: one strip per filter row),
+//  weights-stationary (1: the CTA keeps its weight slice in shared memory),
 //  tiles per accumulator round (always 1), total tiles, n tiles in N, kc, CTAs per SM (always 1)}
 extern "C" int myolo_plan_conv_info(myolo_plan* pl, int op_index, int32_t* info) {
   MYOLO_REQUIRE(pl && info && op_index >= 0 && op_index < (int)pl->ops.size(), "conv_info: bad arguments");
@@ -687,8 +688,8 @@ extern "C" int myolo_plan_conv_info(myolo_plan* pl, int op_index, int32_t* info)
   for (int i = 0; i < 12; ++i) info[i] = 0;
   info[0] = c.use_tc ? 1 : 0;
   if (c.use_tc) {
-    info[1] = c.grid; info[2] = c.smem; info[3] = c.p.BN; info[4] = c.p.num_stages; info[5] = 0;
-    info[6] = 0; info[7] = 1; info[8] = c.p.total_tiles; info[9] = c.p.n_tiles_n; info[10] = c.p.kc;
+    info[1] = c.grid; info[2] = c.smem; info[3] = c.p.BN; info[4] = c.p.num_stages; info[5] = c.p.strip;
+    info[6] = c.p.resident; info[7] = 1; info[8] = c.p.total_tiles; info[9] = c.p.n_tiles_n; info[10] = c.p.kc;
     info[11] = 1;
   }
   return 0;
@@ -1354,6 +1355,7 @@ extern "C" int myolo_conv_bn_silu(const void* x, int B, int H, int W, int ci, co
     } else if (path == 2 || (path == 0 && !elig)) {
       rc = conv_simt_launch(c, s);
     } else {
+      c.reuse = path != 3;     // path 3: streamed weights, the layout the reuse paths are checked against
       rc = conv_tc_prepare(c, sms);
       if (!rc) rc = conv_tc_launch(c, s);
     }

@@ -7,7 +7,8 @@ from . import _lib
 def conv_bn_silu(x_nhwc: torch.Tensor, w: torch.Tensor, bn=None, bias=None, stride=1, dil=1, act=_lib.ACT_SILU, residual=None, path=0,
                  eps=1e-3):
     """x_nhwc: (B,H,W,Ci) fp16 CUDA; w: (Co,Ci,k,k) fp32 CUDA; bn: (gamma,beta,mean,var) fp32 or None.
-    path: 0 auto, 1 wgmma (tensor cores), 2 CUDA-core, 3 same as 1.  Returns (B,Ho,Wo,Co) fp16."""
+    path: 0 auto, 1 wgmma (tensor cores), 2 CUDA-core, 3 wgmma with streamed weights (the reference layout for path 1's weight
+    residency: same MMAs, same K order, bit-identical results).  Returns (B,Ho,Wo,Co) fp16."""
     assert x_nhwc.is_cuda and x_nhwc.dtype == torch.float16 and x_nhwc.is_contiguous()
     B, H, W, Ci = x_nhwc.shape
     Co, _, k, _ = w.shape
