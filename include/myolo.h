@@ -261,6 +261,9 @@ int myolo_resize_area_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H
  * MYOLO_F16 (the fp32 result rounded to nearest) or MYOLO_F32.  Equal sizes convert only. */
 int myolo_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo, void* stream);
 int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, void* stream);
+/* myolo_augment_det_hw: the same per-pixel work on B augmented H x W images (`LoadImagesAndLabels(augment=True, rect=True)`: a letterbox
+ * to the batch shape, random_perspective at (W, H), flips over H and W), out (B,3,H,W).  myolo_augment_det is its H = W = S case. */
+int myolo_augment_det_hw(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, void* stream);
 
 /* ---- segmentation training batches (reference SegmentationDataset.py:118-151 `_sync_transform` + ColorJitter + ToTensor, and the
  * testval items of :81-94) ----

@@ -2,7 +2,7 @@
 // the image cache resize of `load_image` (:629-643; INTER_LINEAR, and INTER_AREA for the augment=False cache), and ONE fused kernel per batch for the 4-image mosaic (:671-724), the affine
 // `random_perspective` warp (:851-893), mixup (:529-532), `augment_hsv` (:646-657), the flips (:571-582) and BGR->RGB / HWC->CHW (:589).
 // The host draws the random parameters and transforms the labels (multiyolov5_b200/utils/datasets.py DetAugmenter); this file only moves
-// pixels.  Every step is bit exact with OpenCV 8-bit arithmetic:
+// pixels.  The output is S x S (mosaic batches) or H x W (--rect batches, DetRectLoader).  Every step is bit exact with OpenCV 8-bit arithmetic:
 //   * cv2.warpAffine INTER_LINEAR / BORDER_CONSTANT 114: 10-bit fixed-point source addresses, 5-bit fractions, 15-bit weights;
 //   * the 2s x 2s mosaic canvas is never built: a canvas pixel is the tile covering it, else 114 (also outside the canvas);
 //   * cv2.COLOR_BGR2HSV: integer (hsv_shift 12) with rounded division tables;
@@ -68,7 +68,7 @@ __device__ __forceinline__ void canvas_px(const myolo_aug_warp& w, int cx, int c
   }
 }
 
-// cv2.warpAffine(canvas, M, (S, S), INTER_LINEAR, BORDER_CONSTANT, 114) at destination pixel (x, y); minv is M inverted as cv2 inverts it
+// cv2.warpAffine(canvas, M, (W, H), INTER_LINEAR, BORDER_CONSTANT, 114) at destination pixel (x, y); minv is M inverted as cv2 inverts it
 __device__ __forceinline__ void warp_px(const myolo_aug_warp& w, int x, int y, int v[3]) {
   const double* m = w.minv;
   const int adelta = __double2int_rn(__dmul_rn(__dmul_rn(m[0], (double)x), 1024.0));
@@ -89,19 +89,20 @@ __device__ __forceinline__ void warp_px(const myolo_aug_warp& w, int x, int y, i
   for (int c = 0; c < 3; ++c) v[c] = min(255, max(0, (p00[c] * w00 + p01[c] * w01 + p10[c] * w10 + p11[c] * w11 + (1 << 14)) >> 15));
 }
 
-__global__ void __launch_bounds__(256) augment_det_kernel(const myolo_aug_item* __restrict__ items, int B, int S, void* out, int out_dtype) {
+__global__ void __launch_bounds__(256) augment_det_kernel(const myolo_aug_item* __restrict__ items, int B, int H, int W, void* out,
+                                                         int out_dtype) {
   __shared__ int sdiv[256], hdiv[256];          // cv2 RGB2HSV_b tables: round((255 << 12) / v), round((180 << 12) / (6 * diff))
   for (int i = threadIdx.x; i < 256; i += blockDim.x) {
     sdiv[i] = i ? __double2int_rn(__ddiv_rn(255.0 * 4096.0, (double)i)) : 0;
     hdiv[i] = i ? __double2int_rn(__ddiv_rn(180.0 * 4096.0, __dmul_rn(6.0, (double)i))) : 0;
   }
   __syncthreads();
-  const long plane = (long)S * S, total = (long)B * plane;
+  const long plane = (long)H * W, total = (long)B * plane;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int b = (int)(i / plane);
-    const int y = (int)((i % plane) / S), x = (int)(i % S);
+    const int y = (int)((i % plane) / W), x = (int)(i % W);
     const myolo_aug_item& it = items[b];
-    const int ys = it.flipud ? S - 1 - y : y, xs = it.fliplr ? S - 1 - x : x;    // np.flipud / np.fliplr of the augmented image
+    const int ys = it.flipud ? H - 1 - y : y, xs = it.fliplr ? W - 1 - x : x;    // np.flipud / np.fliplr of the augmented image
     int px[3];
     warp_px(it.warp[0], xs, ys, px);
     if (it.n_warps == 2) {                       // mixup: (img * r + img2 * (1 - r)).astype(np.uint8) in float64
@@ -143,7 +144,7 @@ __global__ void __launch_bounds__(256) augment_det_kernel(const myolo_aug_item* 
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       const int val = bgr[2 - c];
-      const size_t o = ((size_t)b * 3 + c) * plane + (size_t)y * S + x;
+      const size_t o = ((size_t)b * 3 + c) * plane + (size_t)y * W + x;
       if (out_dtype == MYOLO_U8) reinterpret_cast<unsigned char*>(out)[o] = (unsigned char)val;
       // imgs.float() / 255 on a CUDA tensor (reference train.py:342): ATen multiplies by the fp32 reciprocal of a scalar divisor
       else if (out_dtype == MYOLO_F16) reinterpret_cast<__half*>(out)[o] = __float2half_rn(__fmul_rn((float)val, 1.0f / 255.0f));
@@ -152,11 +153,11 @@ __global__ void __launch_bounds__(256) augment_det_kernel(const myolo_aug_item* 
   }
 }
 
-int launch_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, cudaStream_t s) {
-  MYOLO_REQUIRE(items && out && B > 0 && S > 0, "augment_det: bad arguments (B %d S %d)", B, S);
+int launch_augment_det(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, cudaStream_t s) {
+  MYOLO_REQUIRE(items && out && B > 0 && H > 0 && W > 0, "augment_det: bad arguments (B %d H %d W %d)", B, H, W);
   MYOLO_REQUIRE(out_dtype == MYOLO_U8 || out_dtype == MYOLO_F16 || out_dtype == MYOLO_F32, "augment_det: output dtype");
-  const long total = (long)B * S * S;
-  augment_det_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(items, B, S, out, out_dtype);
+  const long total = (long)B * H * W;
+  augment_det_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(items, B, H, W, out, out_dtype);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }

@@ -35,7 +35,7 @@ int launch_letterbox(const unsigned char* src, int B, int H0, int W0, int rw, in
 // detection training batches (augment.cu): image cache resize and the fused mosaic / warp / mixup / HSV / flip kernel
 int launch_resize_u8(const unsigned char* src, int H0, int W0, unsigned char* dst, int H, int W, cudaStream_t s);
 int launch_resize_area_u8(const unsigned char* src, int H0, int W0, unsigned char* dst, int H, int W, cudaStream_t s);
-int launch_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, cudaStream_t s);
+int launch_augment_det(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, cudaStream_t s);
 int launch_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo, cudaStream_t s);
 
 // segmentation training batches (augment_seg.cu): crop-window resample + pad + mask LUT, then the ColorJitter / ToTensor kernel

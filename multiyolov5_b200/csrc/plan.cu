@@ -1191,7 +1191,13 @@ extern "C" int myolo_resize_area_u8(const uint8_t* src, int H0, int W0, uint8_t*
 extern "C" int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, void* stream) {
   int rc = check_device(nullptr);
   if (rc) return rc;
-  return launch_augment_det(items, B, S, out, out_dtype, (cudaStream_t)stream);
+  return launch_augment_det(items, B, S, S, out, out_dtype, (cudaStream_t)stream);
+}
+
+extern "C" int myolo_augment_det_hw(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_augment_det(items, B, H, W, out, out_dtype, (cudaStream_t)stream);
 }
 
 extern "C" int myolo_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo,

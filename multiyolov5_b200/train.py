@@ -152,11 +152,13 @@ class Trainer:
 
     def __init__(self, model, hyp, batch_size, world_size=1, rank=-1, accumulate=1, detgain=0.6, seggain=0.35, init_scale=2.0 ** 16,
                  growth_interval=2000, process_group=None, graph_loss=True, fused_seg_loss=True, overlap_passes=True, fused_det_loss=True,
-                 concurrent_forwards=None, multi_scale=None):
+                 concurrent_forwards=None, multi_scale=None, det_shapes=None):
         """multi_scale: a MultiScale.  The det lane's train plans for every size it can draw from an imgsz x imgsz batch are reserved on
         one shared workspace (Engine.reserve_train_shapes); rescale each det batch with `multi_scale(imgs)` before `step`, as the reference
         does before its forward (train.py:354-359).  A det batch of fewer images (the loader's partial last batch) reserves its sizes on
-        the same workspace the first time it comes; a batch of more images than batch_size does not fit it and raises MyoloError."""
+        the same workspace the first time it comes; a batch of more images than batch_size does not fit it and raises MyoloError.
+        det_shapes: the (H, W) shapes of the det batches (--rect: DetRectLoader.batch_shapes).  Their train plans are reserved on that one
+        shared workspace instead of a private pair per shape; with multi_scale, every size it can draw from each of them."""
         assert next(model.parameters()).is_cuda, "model.cuda() first"
         self.model, self.hyp, self.batch_size = model, hyp, batch_size
         self.world_size, self.rank, self.accumulate, self.pg = world_size, rank, accumulate, process_group
@@ -194,13 +196,19 @@ class Trainer:
         self.concurrent_forwards = (concurrent_forwards is None or bool(concurrent_forwards)) and self.overlap_passes
         self._ev_detfwd, self._ev_start, self._ev_seg = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
         self.multi_scale = multi_scale
+        self.det_shapes = None if det_shapes is None else sorted({(int(h), int(w)) for h, w in det_shapes})
         self._ms_batches = set()
-        if multi_scale is not None:
+        if multi_scale is not None or det_shapes is not None:
             self._reserve_det(batch_size)
 
-    def _reserve_det(self, B):
+    def det_train_shapes(self):
+        """every (H, W) the det lane's shared workspace holds plans for"""
         ms = self.multi_scale
-        self.model.engine().reserve_train_shapes(B, ms.shapes((ms.imgsz, ms.imgsz)), lane=0)
+        base = self.det_shapes if self.det_shapes is not None else [(ms.imgsz, ms.imgsz)]
+        return base if ms is None else sorted({hw for shape in base for hw in ms.shapes(shape)})
+
+    def _reserve_det(self, B):
+        self.model.engine().reserve_train_shapes(B, self.det_train_shapes(), lane=0)
         self._ms_batches.add(B)
 
     def set_lr(self, lr_bn, lr_weight, lr_bias):
@@ -321,7 +329,7 @@ class Trainer:
 
     def step(self, imgs, targets, segimgs, segtargets):
         """one iteration (train.py:363-401).  Returns (det loss items [lbox,lobj,lcls,loss], seg loss) as device tensors."""
-        if self.multi_scale is not None and imgs.shape[0] not in self._ms_batches:
+        if self._ms_batches and imgs.shape[0] not in self._ms_batches:
             self._reserve_det(int(imgs.shape[0]))               # host plans only: the shared workspace is already there
         fused_seg = self.fused_seg_loss and self.n_seg_outputs == 1 and self.model.model[-2].c_out in (19, 32)
         if self.overlap_passes and fused_seg:

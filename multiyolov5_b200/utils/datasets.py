@@ -3,6 +3,8 @@
     letterbox(img, new_shape, color, auto, scaleFill, scaleup, stride) -> (img, ratio, (dw, dh))     reference utils/datasets.py:818-848
     preprocess(img0, img_size, stride, half)  -> (1|B,3,H,W) float tensor in [0,1]                     :185-189 + detect.py:135-137
     DeviceImageCache(images, img_size, labels) / DetAugmenter(cache, hyp)(indices) -> (imgs, targets)   :518-599 (augment=True)
+    DeviceImageCache(images, img_size, labels) / DetRectLoader(cache, hyp, batch_size)(positions) -> (imgs, targets), iterable
+                                                                             :347-439 + :518-599 (augment=True, rect=True: --rect)
     DeviceImageCache(images, img_size, labels, augment=False) / DetValLoader(cache, batch_size) -> iterable of (imgs, targets, paths,
         shapes) for test(data, model=m, dataloader=DetValLoader(cache, 32))                          :347-452 + :518-599 (rect=True)
     DeviceSegCache(images, masks, mask_map) / SegAugmenter(cache, base_size, crop_size, preset)(indices) -> (segimgs, segtargets)
@@ -197,7 +199,6 @@ class DetAugmenter:
         T[0, 2] = random.uniform(0.5 - hyp["translate"], 0.5 + hyp["translate"]) * width
         T[1, 2] = random.uniform(0.5 - hyp["translate"], 0.5 + hyp["translate"]) * height
         M = T @ S @ R @ P @ C_
-        assert (height, width) == (self.img_size, self.img_size)
         n = len(targets)
         if n:
             xy = np.ones((n * 4, 3))
@@ -266,28 +267,37 @@ class DetAugmenter:
         return self._warp(tiles, M), labels4
 
     # ---- letterbox(auto=False, scaleup=True) + random_perspective(border=0) (reference :536-557)
-    def _single(self, index):
-        s, cache = self.img_size, self.cache
+    def _single(self, index, shape):
+        """`shape`: img_size (int), or a rect batch's [h, w] row of batch_shapes (numpy ints, as the reference passes it: ratio and pad
+        come out as numpy float64)"""
+        cache = self.cache
         h, w = cache.shapes[index]
-        (nw, nh), ratio, (dw, dh), (top, bottom, left, right) = letterbox_geometry((h, w), s, auto=False, scaleup=True)
-        if (w, h) != (nw, nh):
-            img = torch.empty((nh, nw, 3), dtype=torch.uint8, device="cuda")
-            _lib.check(_lib.lib().myolo_resize_u8(C.c_void_p(cache.ptr(index)), h, w, _lib.ptr(img), nh, nw, _lib.stream_ptr()))
-            self._keep.append(img)
-            p = img.data_ptr()
-        else:
-            p = cache.ptr(index)
+        (nw, nh), ratio, (dw, dh), (top, bottom, left, right) = letterbox_geometry((h, w), shape, auto=False, scaleup=True)
+        p = self._resized(index, nh, nw) if (w, h) != (nw, nh) else cache.ptr(index)
         labels = cache.labels[index].copy()
         if labels.size:
             labels[:, 1:] = _xywhn2xyxy(labels[:, 1:], ratio[0] * w, ratio[1] * h, dw, dh)
         M, labels = self._perspective(nh + top + bottom, nw + left + right, labels)
         return self._warp([(p, nw, left, top, left + nw, top + nh, left, top)], M), labels
 
-    def item(self, index):
-        """parameters (myolo_aug_item) and final labels (n, 5) of dataset[index]; consumes the random draws of one __getitem__"""
-        hyp, s = self.hyp, self.img_size
+    def _resized(self, index, nh, nw):
+        """device pointer of cached image `index` resized to nw x nh (letterbox's cv2.resize INTER_LINEAR), kept until the next batch"""
+        h, w = self.cache.shapes[index]
+        img = torch.empty((nh, nw, 3), dtype=torch.uint8, device="cuda")
+        _lib.check(_lib.lib().myolo_resize_u8(C.c_void_p(self.cache.ptr(index)), h, w, _lib.ptr(img), nh, nw, _lib.stream_ptr()))
+        self._keep.append(img)
+        return img.data_ptr()
+
+    def item(self, index, shape=None):
+        """parameters (myolo_aug_item) and final labels (n, 5) of dataset[index]; consumes the random draws of one __getitem__.  `shape`:
+        None for the square dataset (rect=False), or the item's rect batch shape [h, w] (rect=True: no mosaic draw, no mixup)"""
+        hyp = self.hyp
+        H, W = (self.img_size, self.img_size) if shape is None else (int(shape[0]), int(shape[1]))    # img.shape[:2] at :563-564
         it = _lib.AugItem()
-        if random.random() < hyp["mosaic"]:
+        if shape is not None:
+            it.warp[0], labels = self._single(index, shape)
+            it.n_warps = 1
+        elif random.random() < hyp["mosaic"]:
             it.warp[0], labels = self._mosaic(index)
             it.n_warps = 1
             if random.random() < hyp["mixup"]:
@@ -296,7 +306,7 @@ class DetAugmenter:
                 it.mix_r, it.mix_q, it.n_warps = float(r), float(1 - r), 2
                 labels = np.concatenate((labels, labels2), 0)
         else:
-            it.warp[0], labels = self._single(index)
+            it.warp[0], labels = self._single(index, self.img_size)
             it.n_warps = 1
         g = np.random.uniform(-1, 1, 3) * [hyp["hsv_h"], hyp["hsv_s"], hyp["hsv_v"]] + 1     # augment_hsv (reference :646-657)
         x = np.arange(0, 256, dtype=np.int16)
@@ -306,8 +316,8 @@ class DetAugmenter:
         nL = len(labels)
         if nL:
             labels[:, 1:5] = _xyxy2xywh(labels[:, 1:5])
-            labels[:, [2, 4]] /= s
-            labels[:, [1, 3]] /= s
+            labels[:, [2, 4]] /= H
+            labels[:, [1, 3]] /= W
         if random.random() < hyp["flipud"]:
             it.flipud = 1
             if nL:
@@ -321,11 +331,15 @@ class DetAugmenter:
     def __call__(self, indices, out_dtype=torch.uint8):
         """one batch: (imgs (B,3,s,s) of out_dtype, targets (n,6) float32), both on the current CUDA device / stream"""
         self._keep = []
-        B, s = len(indices), self.img_size
+        return self.launch([self.item(index) for index in indices], self.img_size, self.img_size, out_dtype)
+
+    def launch(self, items_labels, H, W, out_dtype=torch.uint8):
+        """the batch of drawn items [(myolo_aug_item, (n, 5) labels)] at H x W: one pinned copy of the items, one kernel, the targets"""
+        B = len(items_labels)
         items = (_lib.AugItem * B)()
         targets = []
-        for b, index in enumerate(indices):
-            items[b], labels = self.item(index)
+        for b, (it, labels) in enumerate(items_labels):
+            items[b] = it
             t = torch.zeros((len(labels), 6))
             t[:, 0] = b
             if len(labels):
@@ -333,8 +347,9 @@ class DetAugmenter:
             targets.append(t)
         host = torch.frombuffer(bytearray(items), dtype=torch.uint8).pin_memory()
         dev_items = host.cuda(non_blocking=True)
-        imgs = torch.empty((B, 3, s, s), dtype=out_dtype, device="cuda")
-        _lib.check(_lib.lib().myolo_augment_det(_lib.ptr(dev_items), B, s, _lib.ptr(imgs), _lib.torch_dtype_code(out_dtype), _lib.stream_ptr()))
+        imgs = torch.empty((B, 3, H, W), dtype=out_dtype, device="cuda")
+        _lib.check(_lib.lib().myolo_augment_det_hw(_lib.ptr(dev_items), B, H, W, _lib.ptr(imgs), _lib.torch_dtype_code(out_dtype),
+                                                   _lib.stream_ptr()))
         targets = torch.cat(targets, 0).pin_memory().cuda(non_blocking=True)
         self._keep = [dev_items] + self._keep
         return imgs, targets
@@ -352,14 +367,14 @@ class ValBatch:
         self.indices, self.geoms, self.targets, self.shapes = indices, geoms, targets, shapes
 
 
-def det_val_plan(shapes0, shapes, labels, img_size, batch_size, stride=32, pad=0.5, single_cls=False):
-    """The host arithmetic of the reference's rect validation dataset over cached images, in its statements and dtypes: `shapes0` are the
-    original (h0, w0), `shapes` the cached (h, w), `labels` (n, 5) float32 normalised [class, x, y, w, h].  Returns (order, batch_shapes,
-    [ValBatch]): `order` is the aspect-ratio sort (numpy's default argsort kind, as the reference: not stable, so the order of equal
-    aspect ratios depends on the host CPU), `batch_shapes` the (nb, 2) [h, w] int letterbox shapes."""
+def rect_plan(shapes0, img_size, batch_size, stride=32, pad=0.0):
+    """The rect arithmetic of the reference's LoadImagesAndLabels.__init__ (:410-439) over the original (h0, w0) `shapes0`: returns
+    (order, bi, batch_shapes).  `order` is the aspect-ratio sort (the reference's `irect`: numpy's default argsort kind, not stable, so
+    the order of equal aspect ratios depends on the host CPU), `bi` the batch index of each sorted position and `batch_shapes` the
+    (nb, 2) [h, w] int letterbox shapes."""
     n = len(shapes0)
     if n == 0:
-        raise ValueError("det_val_plan: no images")
+        raise ValueError("rect_plan: no images")
     s = np.array([(w0, h0) for h0, w0 in shapes0], dtype=np.float64)         # the reference's self.shapes: wh
     ar = s[:, 1] / s[:, 0]
     order = ar.argsort()
@@ -374,7 +389,15 @@ def det_val_plan(shapes0, shapes, labels, img_size, batch_size, stride=32, pad=0
             bshapes[i] = [maxi, 1]
         elif mini > 1:
             bshapes[i] = [1, 1 / mini]
-    batch_shapes = np.ceil(np.array(bshapes) * img_size / stride + pad).astype(int) * stride
+    return order, bi, np.ceil(np.array(bshapes) * img_size / stride + pad).astype(int) * stride
+
+
+def det_val_plan(shapes0, shapes, labels, img_size, batch_size, stride=32, pad=0.5, single_cls=False):
+    """The host arithmetic of the reference's rect validation dataset over cached images, in its statements and dtypes: `shapes0` are the
+    original (h0, w0), `shapes` the cached (h, w), `labels` (n, 5) float32 normalised [class, x, y, w, h].  Returns (order, batch_shapes,
+    [ValBatch]): `order` and `batch_shapes` as rect_plan gives them."""
+    order, bi, batch_shapes = rect_plan(shapes0, img_size, batch_size, stride, pad)
+    nb = len(batch_shapes)
     batches = []
     for b in range(nb):
         shape = batch_shapes[b]                  # a numpy row, as the reference passes it: ratio and pad come out as numpy float64
@@ -438,6 +461,83 @@ class DetValLoader:
                 _lib.check(L.myolo_letterbox(C.c_void_p(cache.ptr(i)), 1, h, w, rw, rh, top, left, H, W, color,
                                              C.c_void_p(imgs.data_ptr() + k * 3 * H * W), _lib.U8, 1, 1, sp))
             yield imgs, targets, batch.indices, batch.shapes
+
+
+# ------------------------------------------------------------------------------------------------
+# rect training batches (reference train.py:196-198 create_dataloader(..., augment=True, rect=opt.rect): LoadImagesAndLabels with
+# augment=True, rect=True (:347-439, __getitem__ :518-592 without mosaic) + collate_fn)
+# ------------------------------------------------------------------------------------------------
+class DetRectLoader:
+    """Detection training batches of `--rect` on the device, over a DeviceImageCache built with augment=True (INTER_LINEAR cache).
+
+    The dataset is sorted by aspect ratio and every run of `batch_size` sorted positions shares one letterbox shape, as the reference
+    plans it (rect_plan): `order` (position -> source index, the reference's `irect`), `batch` (position -> batch index) and
+    `batch_shapes` ((nb, 2) [h, w]).  `loader(positions)` builds the batch of those sorted positions: per item the reference's draws in
+    its order and number (random_perspective, augment_hsv, flipud, fliplr: no mosaic draw and no mixup under rect), the labels on the
+    host with its numpy formulas, the pixels (letterbox to the batch shape, affine warp at that size, HSV, flips, BGR->RGB, CHW) in one
+    myolo_augment_det_hw launch.  Positions whose batch shapes differ raise ValueError, as collate_fn's torch.stack does.
+
+    Iterating yields the batches of consecutive positions (no sampler: rank -1), the partial last batch included.  `epoch_positions`
+    gives one rank's positions under DDP (DistributedSampler(dataset) with shuffle, seed 0, set_epoch(epoch)); its batches are runs of
+    `batch_size` of them, and any run that mixes shapes raises, as it does in the reference."""
+
+    def __init__(self, cache, hyp, batch_size, stride=32, pad=0.0, single_cls=False):
+        if not cache.augment:
+            raise ValueError("DetRectLoader: the cache must be built with augment=True (load_image's INTER_LINEAR training resize)")
+        self.aug = DetAugmenter(cache, hyp, stride)
+        self.cache, self.batch_size, self.single_cls = cache, int(batch_size), bool(single_cls)
+        self.order, self.batch, self.batch_shapes = rect_plan(cache.shapes0, cache.img_size, self.batch_size, stride, pad)
+        self.n = cache.n
+
+    def __len__(self):
+        return len(self.batch_shapes)
+
+    def shape_of(self, positions):
+        """the batch shape [h, w] shared by `positions`; ValueError if they differ"""
+        shapes = {tuple(int(v) for v in self.batch_shapes[self.batch[p]]) for p in positions}
+        if len(shapes) != 1:
+            raise ValueError(f"DetRectLoader: positions {list(positions)} have different batch shapes {sorted(shapes)}: collate_fn's "
+                             "torch.stack cannot stack them")
+        return self.batch_shapes[self.batch[positions[0]]]
+
+    def item(self, position):
+        """(myolo_aug_item, (n, 5) float32 labels) of dataset[position]; consumes the reference's draws of one item"""
+        it, labels = self.aug.item(int(self.order[position]), self.batch_shapes[self.batch[position]])
+        if self.single_cls:
+            labels[:, 0] = 0
+        return it, labels
+
+    def __call__(self, positions, out_dtype=torch.uint8):
+        """the batch of sorted `positions`: (imgs (B, 3, h, w) of out_dtype, targets (n, 6) float32), both on the current CUDA device /
+        stream; float outputs are uint8 / 255 as the training loop's imgs.float() / 255"""
+        positions = [int(p) for p in positions]
+        if not positions or min(positions) < 0 or max(positions) >= self.n:
+            raise ValueError(f"DetRectLoader: positions must be in [0, {self.n}), got {positions}")
+        H, W = (int(v) for v in self.shape_of(positions))
+        self.aug._keep = []
+        return self.aug.launch([self.item(p) for p in positions], H, W, out_dtype)
+
+    def epoch_positions(self, epoch, rank, world_size, seed=0):
+        """rank's positions of one epoch under DistributedSampler(dataset, shuffle=True, seed=seed) after set_epoch(epoch): randperm from
+        a generator seeded with seed + epoch, padded with its own head to a multiple of world_size, then every world_size-th from rank"""
+        if not 0 <= rank < world_size:
+            raise ValueError(f"DetRectLoader: rank {rank} outside world size {world_size}")
+        g = torch.Generator()
+        g.manual_seed(seed + epoch)
+        idx = torch.randperm(self.n, generator=g).tolist()
+        total = math.ceil(self.n / world_size) * world_size
+        pad = total - len(idx)
+        idx += (idx * math.ceil(pad / len(idx)))[:pad] if pad else []
+        return idx[rank:total:world_size]
+
+    def batches(self, positions=None, out_dtype=torch.uint8):
+        """the batches of runs of batch_size `positions` (default: every position in order), the last one partial"""
+        positions = list(range(self.n)) if positions is None else list(positions)
+        for k in range(0, len(positions), self.batch_size):
+            yield self(positions[k:k + self.batch_size], out_dtype)
+
+    def __iter__(self):
+        return self.batches()
 
 
 # ------------------------------------------------------------------------------------------------
