@@ -193,6 +193,21 @@ int myolo_grads_check_finite(const float* grad, int64_t n, int32_t* found_inf /*
 int myolo_sgd_step(float* param, float* grad, float* momentum_buf, const uint8_t* group, int64_t n, const float* lr,
                    const float* weight_decay, int n_groups, float momentum, int nesterov, const float* inv_scale /* device */,
                    const int32_t* found_inf /* device, nullable */, int zero_grad, void* stream);
+/* torch.optim.Adam(betas=(beta1, beta2), eps) as reference train.py:128-137 builds it for --adam, behind amp.GradScaler, over the same
+ * flat buffers as myolo_sgd_step: bit-identical with GradScaler.unscale_ + torch's default CUDA Adam (foreach, capturable=False).
+ * exp_avg / exp_avg_sq: flat fp32 moments.  lr: HOST array of n_groups DOUBLES (torch divides the Python lr by the bias correction
+ * before rounding the step size to fp32); weight_decay: host floats, 0 = no decay term (torch's `if weight_decay != 0`).
+ * steps: device int32, the steps taken so far; the launch uses step *steps + 1 for the bias corrections and does NOT advance it: the caller
+ * adds (*found_inf == 0) after the launch.  When *found_inf != 0 nothing moves.  zero_grad clears the gradients in both cases.
+ * Every buffer 16-byte aligned, group 4-byte aligned; n need not be a multiple of 4. */
+int myolo_adam_step(float* param, float* grad, float* exp_avg, float* exp_avg_sq, const uint8_t* group, int64_t n, const double* lr,
+                    const float* weight_decay, int n_groups, double beta1, double beta2, double eps, const int32_t* steps /* device */,
+                    const float* inv_scale /* device */, const int32_t* found_inf /* device, nullable */, int zero_grad, void* stream);
+/* The scalars myolo_adam_step uses at step k = steps[i] (device int32, k >= 1), from the same device code: the double bias corrections
+ * bc1[i] = 1 - beta1^k and bc2[i] = 1 - beta2^k, and the fp32 scalars step_size[i] = (float)(-(lr / bc1[i])), bc2_sqrt[i] =
+ * (float)sqrt(bc2[i]). */
+int myolo_adam_scalars(const int32_t* steps, int64_t n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt,
+                       double* bc1, double* bc2, void* stream);
 
 /* Detection loss forward + backward in four launches (reference utils/loss.py:115-217 `ComputeLoss.__call__` / `build_targets` + autograd):
  * p[l] / dp[l]: the nl raw head outputs (B, na, ny[l], nx[l], no) fp32 and their gradients (overwritten); targets (nt, 6) [image, class,

@@ -36,7 +36,8 @@ EXPORTS = [
     "myolo_conv_bn_silu", "myolo_plan_set_bn", "myolo_plan_set_conv_grad", "myolo_plan_train_forward", "myolo_plan_backward",
     "myolo_grads_check_finite", "myolo_sgd_step", "myolo_conv_wgrad", "myolo_letterbox", "myolo_seg_lut_blend", "myolo_seg_metrics", "myolo_plan_backward_seg_ce", "myolo_plan_read_grad_view", "myolo_plan_set_seed", "myolo_plan_train_forward_multi", "myolo_plan_backward_multi", "myolo_plan_conv_info", "myolo_allreduce_grads", "myolo_det_loss", "myolo_det_loss_workspace_bytes", "myolo_plan_set_defer_running", "myolo_plan_apply_running",
     "myolo_resize_u8", "myolo_augment_det", "myolo_augment_seg", "myolo_det_match", "myolo_det_ap", "myolo_det_ap_workspace_bytes",
-    "myolo_resize_area_u8", "myolo_resize_bilinear", "myolo_plan_create_shared", "myolo_augment_det_hw",
+    "myolo_resize_area_u8", "myolo_resize_bilinear", "myolo_plan_create_shared", "myolo_augment_det_hw", "myolo_adam_step",
+    "myolo_adam_scalars",
 ]
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
 
@@ -132,6 +133,9 @@ def lib():
     L.myolo_conv_wgrad.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp]
     L.myolo_grads_check_finite.argtypes = [vp, i64, vp, vp]
     L.myolo_sgd_step.argtypes = [vp, vp, vp, vp, i64, C.POINTER(f32), C.POINTER(f32), i32, f32, i32, vp, vp, i32, vp]
+    L.myolo_adam_step.argtypes = [vp, vp, vp, vp, vp, i64, C.POINTER(C.c_double), C.POINTER(f32), i32, C.c_double, C.c_double, C.c_double,
+                                  vp, vp, vp, i32, vp]
+    L.myolo_adam_scalars.argtypes = [vp, i64, C.c_double, C.c_double, C.c_double, vp, vp, vp, vp, vp]
     L.myolo_allreduce_grads.argtypes = [vp, i64, vp, vp]
     L.myolo_det_loss_workspace_bytes.argtypes = [i32, i32, i32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     L.myolo_det_loss_workspace_bytes.restype = i64

@@ -1295,6 +1295,23 @@ extern "C" int myolo_sgd_step(float* param, float* grad, float* momentum_buf, co
                          zero_grad, (cudaStream_t)stream);
 }
 
+extern "C" int myolo_adam_step(float* param, float* grad, float* exp_avg, float* exp_avg_sq, const uint8_t* group, int64_t n, const double* lr,
+                               const float* weight_decay, int n_groups, double beta1, double beta2, double eps, const int32_t* steps,
+                               const float* inv_scale, const int32_t* found_inf, int zero_grad, void* stream) {
+  NvtxRange nvtx_("myolo_adam_step");
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_adam_step(param, grad, exp_avg, exp_avg_sq, group, (long)n, lr, weight_decay, n_groups, beta1, beta2, eps, steps, inv_scale,
+                          found_inf, zero_grad, (cudaStream_t)stream);
+}
+
+extern "C" int myolo_adam_scalars(const int32_t* steps, int64_t n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt,
+                                  double* bc1, double* bc2, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_adam_scalars(steps, (long)n, lr, beta1, beta2, step_size, bc2_sqrt, bc1, bc2, (cudaStream_t)stream);
+}
+
 // ------------------------------------------------------------------------------------------------
 // gradient exchange: NCCL all-reduce of the flat gradient buffer, bound at run time from the libnccl already in the process
 // ------------------------------------------------------------------------------------------------

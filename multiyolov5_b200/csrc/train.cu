@@ -1238,4 +1238,136 @@ int launch_sgd_step(float* p, float* g, float* buf, const unsigned char* group, 
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// torch.optim.Adam (reference train.py:128-129, --adam) behind amp.GradScaler, over the same flat buffers: 32 B of HBM traffic per
+// element (p, g, exp_avg, exp_avg_sq read and written) + 1 B of group.  Bit-identical with GradScaler.unscale_ + torch's default
+// CUDA implementation (_multi_tensor_adam, capturable=False), which runs one foreach kernel per line below, each rounding to fp32:
+//   g  = g * inv_scale                               _amp_foreach_non_finite_check_and_unscale_
+//   g  = fma(wd, p, g)          (wd != 0 only)       _foreach_add(g, p, alpha=wd)
+//   m  = fma(1-b1, g - m, m)                         _foreach_lerp_(m, g, 1-b1), at::native::lerp for a weight < 0.5
+//      (g - (g - m) * (1 - (1-b1)) for a weight >= 0.5)
+//   v  = v * b2;  v = fma(1-b2, g*g, v)              _foreach_mul_, _foreach_addcmul_(v, g, g, 1-b2)
+//   d  = sqrt(v) / bc2_sqrt + eps                    _foreach_sqrt, _foreach_div_(scalar list), _foreach_add_
+//   p  = fma(-lr/bc1, m / d, p)                      _foreach_addcdiv_(p, m, d, scalar list)
+// The explicit _rn intrinsics pin both the roundings and the contractions nvcc makes in torch's kernels.  The bias corrections are
+// Python double arithmetic in torch (1 - beta**step, (lr / bc1) * -1, bc2 ** 0.5), rounded to fp32 when the scalar lists reach the
+// kernels; they are computed here in double from the device step counter, so a skipped step (decided on the device) needs no host sync.
+// ------------------------------------------------------------------------------------------------
+struct AdamGroups { double lr[4]; float wd[4]; };
+struct AdamScalars { float step_size, bc2_sqrt; };
+
+// step k = 1, 2, ...: what torch hands its kernels for group lr (CUDA's double sqrt and division are correctly rounded, as glibc's are;
+// tests/test_gpu_optim.py compares the double bias corrections with Python's for every k up to 10^6).
+// beta^k rounded to double: CUDA's pow (2 ulp) differs from glibc's for some k (e.g. 0.937^3), so the power is taken by squaring in
+// double-double arithmetic (error ~ 2 log2(k) * 2^-104), which rounds to the correctly rounded double that glibc's pow returns
+__device__ __forceinline__ void dd_mul(double& hi, double& lo, double bh, double bl) {
+  const double p = hi * bh;
+  double e = fma(hi, bh, -p);
+  e = fma(hi, bl, fma(lo, bh, e));
+  hi = p + e;
+  lo = e - (hi - p);
+}
+__device__ __forceinline__ double bias_correction(double beta, int k) {
+  double rh = 1.0, rl = 0.0, xh = beta, xl = 0.0;
+  for (unsigned e = (unsigned)k; e; e >>= 1) {
+    if (e & 1) dd_mul(rh, rl, xh, xl);
+    if (e > 1) dd_mul(xh, xl, xh, xl);
+  }
+  return 1.0 - (rh + rl);
+}
+__device__ __forceinline__ AdamScalars adam_scalars(int k, double lr, double beta1, double beta2) {
+  return AdamScalars{(float)((lr / bias_correction(beta1, k)) * -1.0), (float)sqrt(bias_correction(beta2, k))};
+}
+
+__device__ __forceinline__ void adam_element(float& p, float& g, float& m, float& v, float is, float wd, float w1, float b2, float w2,
+                                             float eps, AdamScalars sc) {
+  float gr = __fmul_rn(g, is);
+  if (wd != 0.f) gr = __fmaf_rn(wd, p, gr);
+  const float diff = __fsub_rn(gr, m);
+  m = fabsf(w1) < 0.5f ? __fmaf_rn(w1, diff, m) : __fmaf_rn(-diff, __fsub_rn(1.f, w1), gr);
+  v = __fmaf_rn(w2, __fmul_rn(gr, gr), __fmul_rn(v, b2));
+  const float d = __fadd_rn(__fdiv_rn(__fsqrt_rn(v), sc.bc2_sqrt), eps);
+  p = __fmaf_rn(sc.step_size, __fdiv_rn(m, d), p);
+}
+
+__global__ void adam_step_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ m, float* __restrict__ v,
+                                 const unsigned char* __restrict__ group, long n, AdamGroups gr, int n_groups, double beta1, double beta2,
+                                 float w1, float b2, float w2, float eps, const int* steps, const float* inv_scale, const int* found_inf,
+                                 int zero_grad) {
+  __shared__ AdamScalars sc[4];
+  __shared__ float swd[4];
+  const bool skip = found_inf && *found_inf;
+  const float is = inv_scale ? *inv_scale : 1.0f;
+  if (threadIdx.x < n_groups) {
+    double lr = gr.lr[0];
+    float wd = gr.wd[0];
+#pragma unroll
+    for (int j = 1; j < 4; ++j)                       // constant indices: the kernel parameters stay out of local memory
+      if (threadIdx.x == j) { lr = gr.lr[j]; wd = gr.wd[j]; }
+    swd[threadIdx.x] = wd;
+    if (!skip) sc[threadIdx.x] = adam_scalars(*steps + 1, lr, beta1, beta2);
+  }
+  __syncthreads();
+  const long n4 = n / 4;
+  const long stride = (long)gridDim.x * blockDim.x;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n4; i += stride) {
+    float4 gv = reinterpret_cast<float4*>(g)[i];
+    if (!skip) {
+      float4 pv = reinterpret_cast<float4*>(p)[i], mv = reinterpret_cast<float4*>(m)[i], vv = reinterpret_cast<float4*>(v)[i];
+      const uchar4 k = reinterpret_cast<const uchar4*>(group)[i];
+      adam_element(pv.x, gv.x, mv.x, vv.x, is, swd[k.x & 3], w1, b2, w2, eps, sc[k.x & 3]);
+      adam_element(pv.y, gv.y, mv.y, vv.y, is, swd[k.y & 3], w1, b2, w2, eps, sc[k.y & 3]);
+      adam_element(pv.z, gv.z, mv.z, vv.z, is, swd[k.z & 3], w1, b2, w2, eps, sc[k.z & 3]);
+      adam_element(pv.w, gv.w, mv.w, vv.w, is, swd[k.w & 3], w1, b2, w2, eps, sc[k.w & 3]);
+      reinterpret_cast<float4*>(p)[i] = pv;
+      reinterpret_cast<float4*>(m)[i] = mv;
+      reinterpret_cast<float4*>(v)[i] = vv;
+    }
+    if (zero_grad) reinterpret_cast<float4*>(g)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  const long i = n4 * 4 + blockIdx.x * (long)blockDim.x + threadIdx.x;     // the tail of n % 4 elements
+  if (i < n) {
+    if (!skip) {
+      const int k = group[i] & 3;
+      adam_element(p[i], g[i], m[i], v[i], is, swd[k], w1, b2, w2, eps, sc[k]);
+    }
+    if (zero_grad) g[i] = 0.f;
+  }
+}
+
+int launch_adam_step(float* p, float* g, float* m, float* v, const unsigned char* group, long n, const double* lr, const float* wd,
+                     int n_groups, double beta1, double beta2, double eps, const int* steps, const float* inv_scale, const int* found_inf,
+                     int zero_grad, cudaStream_t s) {
+  MYOLO_REQUIRE(p && g && m && v && group && steps && n > 0 && n_groups >= 1 && n_groups <= 4, "adam_step: bad arguments");
+  MYOLO_REQUIRE(((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
+                  reinterpret_cast<uintptr_t>(v)) & 15) == 0 && (reinterpret_cast<uintptr_t>(group) & 3) == 0,
+                "adam_step: buffers must be 16-byte aligned (group: 4-byte)");
+  AdamGroups gr{};
+  for (int i = 0; i < n_groups; ++i) { gr.lr[i] = lr[i]; gr.wd[i] = wd[i]; }
+  // torch's scalars: 1 - beta1 (lerp weight), beta2, 1 - beta2 and eps, each Python double rounded to fp32
+  adam_step_kernel<<<grid_for_t(std::max<long>(1, n / 4), 256, 132 * 8), 256, 0, s>>>(
+      p, g, m, v, group, n, gr, n_groups, beta1, beta2, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps, steps,
+      inv_scale, found_inf, zero_grad);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+__global__ void adam_scalars_kernel(const int* steps, long n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt,
+                                    double* bc1, double* bc2) {
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const AdamScalars sc = adam_scalars(steps[i], lr, beta1, beta2);
+    step_size[i] = sc.step_size;
+    bc2_sqrt[i] = sc.bc2_sqrt;
+    bc1[i] = bias_correction(beta1, steps[i]);
+    bc2[i] = bias_correction(beta2, steps[i]);
+  }
+}
+int launch_adam_scalars(const int* steps, long n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt, double* bc1,
+                        double* bc2, cudaStream_t s) {
+  MYOLO_REQUIRE(steps && step_size && bc2_sqrt && bc1 && bc2 && n > 0, "adam_scalars: bad arguments");
+  adam_scalars_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(steps, n, lr, beta1, beta2, step_size, bc2_sqrt, bc1, bc2);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace myolo

@@ -81,6 +81,11 @@ int launch_bias_grad(const TensorView& dy, float* dbias, int co, cudaStream_t s)
 int launch_grads_check_finite(const float* g, long n, int* found_inf, cudaStream_t s);
 int launch_sgd_step(float* p, float* g, float* buf, const unsigned char* group, long n, const float* lr, const float* wd, int n_groups,
                     float momentum, int nesterov, const float* inv_scale, const int* found_inf, int zero_grad, cudaStream_t s);
+int launch_adam_step(float* p, float* g, float* m, float* v, const unsigned char* group, long n, const double* lr, const float* wd,
+                     int n_groups, double beta1, double beta2, double eps, const int* steps, const float* inv_scale, const int* found_inf,
+                     int zero_grad, cudaStream_t s);
+int launch_adam_scalars(const int* steps, long n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt, double* bc1,
+                        double* bc2, cudaStream_t s);
 // wgmma weight gradient (wgrad_tc.cu): dw_packed is a zeroed fp32 [co][k*k][ci] accumulation buffer owned by the caller
 bool conv_wgrad_tc_eligible(const TensorView& x, const TensorView& dy, int k, int stride, int dil, int co, int ci);
 size_t conv_wgrad_packed_bytes(const float* dW, int co, int ci, int k);   // 0: accumulates straight into dW

@@ -17,6 +17,16 @@ def shared_train_plans(model, B, shapes):
     return pbs, max([int(pb.workspace_bytes) for pb in pbs.values()], default=0)
 
 
+def flat_offsets(params):
+    """(offsets, total) of the parameters in the flat parameter / gradient / optimiser buffers: back to back in the given order, every
+    tensor starting on a 16-byte boundary (vector loads / vector reductions in the kernels); the gaps stay zero"""
+    offsets, off = [], 0
+    for p in params:
+        offsets.append(off)
+        off += (p.numel() + 3) // 4 * 4
+    return offsets, off
+
+
 class TrainArena:
     """One activation workspace and one gradient workspace shared by the train plans of one lane (Engine.reserve_train_shapes).
 
@@ -221,12 +231,7 @@ class Engine:
             return self._flat_grad
         for p in params:
             assert p.dtype == torch.float32 and p.is_cuda, "training keeps fp32 master parameters on the GPU"
-        # every tensor starts on a 16-byte boundary (vector loads / vector reductions in the kernels); the gaps stay zero
-        self._flat_offsets, off = [], 0
-        for p in params:
-            self._flat_offsets.append(off)
-            off += (p.numel() + 3) // 4 * 4
-        n = off
+        self._flat_offsets, n = flat_offsets(params)
         old = [p.grad for p in params]
         self._flat_grad = torch.zeros(n, dtype=torch.float32, device=params[0].device)
         self._grad_views = []

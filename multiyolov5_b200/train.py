@@ -10,8 +10,13 @@ parameters, gradients and momentum buffers live in three FLAT fp32 buffers, so t
 contiguous 31 MB region and the optimiser is a single HBM-bound launch (`myolo_sgd_step`) that also unscales, skips on overflow and
 clears the gradients.  `torch.distributed` is plumbing only (process group + all_reduce on the flat buffer).
 
+`Trainer(..., optimizer="adam")` is the reference's `--adam` (train.py:128-137): torch.optim.Adam with the same three groups, one
+more flat buffer for the second moment and one launch (`myolo_adam_step`).  `Trainer.state_dict()` / `load_state_dict()` convert the flat
+optimiser buffers to and from torch's `optimizer.state_dict()` format, which is what the reference's checkpoints hold in
+`ckpt['optimizer']` (train.py:482-494, restored at :155-160).
+
 Out of scope (the reference's outer loop, not the hot path): data loading, LR schedule / warm-up (call `set_lr` / `set_momentum`),
-EMA, checkpointing, plotting, DDP buffer broadcast.
+EMA, writing checkpoint files, plotting, DDP buffer broadcast.
 """
 import math
 import random
@@ -21,6 +26,7 @@ import torch
 import torch.nn as nn
 
 from . import _lib
+from .engine import flat_offsets
 from .parallel import allreduce_flat_grads
 from .utils.loss import ComputeLoss, FusedComputeLoss, SegmentationLosses
 
@@ -37,25 +43,152 @@ def scale_hyp(hyp: dict, nl: int, nc: int, imgsz: int, total_batch_size: int, nb
     return h
 
 
-def parameter_groups(model: nn.Module):
-    """{id(param): group} with group 0 = BatchNorm weights (no decay), 1 = other weights (decay), 2 = biases (reference train.py:108-116)"""
-    grp = {}
+def reference_param_groups(model: nn.Module):
+    """[pg0, pg1, pg2] = BatchNorm weights (no decay), other weights (decay), biases, each in named_modules() order, as reference
+    train.py:119-126 builds them.  The reference's optimizer numbers its parameters in this order (pg0, then pg1, then pg2), which is
+    neither model.parameters() order nor the flat buffers' order."""
+    pg0, pg1, pg2 = [], [], []
     for _, m in model.named_modules():
         b = getattr(m, "bias", None)
         if isinstance(b, nn.Parameter):
-            grp[id(b)] = 2
+            pg2.append(b)
         w = getattr(m, "weight", None)
         if isinstance(m, nn.BatchNorm2d):
-            grp[id(m.weight)] = 0
+            pg0.append(m.weight)
         elif isinstance(w, nn.Parameter):
-            grp[id(w)] = 1
-    return grp
+            pg1.append(w)
+    return [pg0, pg1, pg2]
+
+
+def parameter_groups(model: nn.Module):
+    """{id(param): group} with group 0 = BatchNorm weights (no decay), 1 = other weights (decay), 2 = biases (reference train.py:108-116)"""
+    return {id(p): k for k, pg in enumerate(reference_param_groups(model)) for p in pg}
+
+
+# ---- optimiser state in torch's format ---------------------------------------------------------------------------------------------
+OPTIMIZER_STATE = {"sgd": ("momentum_buffer",), "adam": ("exp_avg", "exp_avg_sq")}     # per-parameter state tensors, in torch's order
+
+
+def default_param_groups(optimizer: str, hyp: dict):
+    """the three param_groups entries (without 'params') of the reference's optimizer when it writes its first checkpoint: the keys and
+    defaults of torch.optim.SGD(nesterov=True) / torch.optim.Adam under the installed torch, built as train.py:128-137 builds them
+    (pg1 with hyp['weight_decay']), plus the 'initial_lr' = hyp['lr0'] that its LambdaLR adds"""
+    ps = [torch.zeros(1) for _ in range(3)]
+    if optimizer == "sgd":
+        opt = torch.optim.SGD(ps[:1], lr=hyp["lr0"], momentum=hyp["momentum"], nesterov=True)
+    elif optimizer == "adam":
+        opt = torch.optim.Adam(ps[:1], lr=hyp["lr0"], betas=(hyp["momentum"], 0.999))
+    else:
+        raise ValueError(f"optimizer must be 'sgd' or 'adam', got {optimizer!r}")
+    opt.add_param_group({"params": ps[1:2], "weight_decay": hyp["weight_decay"]})
+    opt.add_param_group({"params": ps[2:]})
+    return [dict({k: v for k, v in g.items() if k != "params"}, initial_lr=hyp["lr0"]) for g in opt.param_groups]
+
+
+def _flat_slices(model):
+    """{id(param): (offset, numel)} of the parameters in the flat buffers (engine.flat_offsets over model.parameters()), and n.
+    The flat buffers hold trainable parameters only, while the reference's groups (and so its state dict's indices) also number frozen
+    ones (its `freeze` list, train.py:106-112): a model with frozen parameters is refused."""
+    params = list(model.parameters())
+    frozen = [n for n, p in model.named_parameters() if not p.requires_grad]
+    if frozen:
+        raise ValueError(f"optimizer state of a model with frozen parameters is not supported: {frozen[:3]}{' ...' if len(frozen) > 3 else ''}")
+    offsets, n = flat_offsets(params)
+    return {id(p): (o, p.numel()) for p, o in zip(params, offsets)}, n
+
+
+def optimizer_state_dict(model, optimizer: str, groups, steps: int, buffers):
+    """torch's `optimizer.state_dict()` of the reference's optimizer over `model`, from flat buffers.
+    groups: the three groups' settings (dicts without 'params'); steps: optimiser steps taken that were not skipped (0: torch has no
+    state yet); buffers: {state name: flat fp32 tensor (CPU or CUDA)} laid out as the Trainer's flat buffers.  State tensors are copies on
+    the buffers' device; Adam's 'step' is a CPU float32 scalar, as torch keeps it (capturable=False)."""
+    slices, _ = _flat_slices(model)
+    state, param_groups, i = {}, [], 0
+    for g, ps in zip(groups, reference_param_groups(model)):
+        ids = list(range(i, i + len(ps)))
+        i += len(ps)
+        if steps:
+            for j, p in zip(ids, ps):
+                o, k = slices[id(p)]
+                st = {"step": torch.tensor(float(steps), dtype=torch.float32)} if optimizer == "adam" else {}
+                for name in OPTIMIZER_STATE[optimizer]:
+                    st[name] = buffers[name][o:o + k].view_as(p).clone()
+                state[j] = st
+        param_groups.append(dict(g, params=ids))
+    return {"state": state, "param_groups": param_groups}
+
+
+def optimizer_kind(sd) -> str:
+    """'sgd' or 'adam' from the keys of a state dict's param_groups"""
+    groups = sd.get("param_groups") if isinstance(sd, dict) else None
+    if not groups:
+        raise ValueError("not an optimizer state dict: no param_groups")
+    if all("betas" in g for g in groups):
+        return "adam"
+    if all("momentum" in g and "nesterov" in g for g in groups):
+        return "sgd"
+    raise ValueError("optimizer state dict is neither torch.optim.SGD's nor torch.optim.Adam's")
+
+
+def _check_same(groups, key):
+    vals = [g[key] for g in groups]
+    if any(v != vals[0] for v in vals[1:]):
+        raise ValueError(f"the flat optimiser step takes one {key!r} for all groups, the state dict has {vals}")
+
+
+def optimizer_state_from_dict(model, optimizer: str, sd, device=None):
+    """inverse of optimizer_state_dict: (groups, steps, buffers) from torch's state dict of the reference's optimizer over `model` (e.g. a
+    reference checkpoint's ckpt['optimizer'], tensors on any device).  groups keep every key of the dict's groups; buffers are new flat fp32
+    tensors on `device`, zero where the dict has no state; steps is Adam's step count, for SGD 1 when the dict has state, else 0.
+    Raises ValueError when the optimizer kind is not `optimizer`, the group sizes differ from the model's, a state tensor has the wrong
+    shape, state is missing for some parameters, the Adam step counts differ, or a setting is one the flat step does not implement."""
+    kind = optimizer_kind(sd)
+    if kind != optimizer:
+        raise ValueError(f"the state dict is {kind}'s, this optimizer is {optimizer}")
+    groups = sd["param_groups"]
+    pgs = reference_param_groups(model)
+    if [len(g["params"]) for g in groups] != [len(pg) for pg in pgs]:
+        raise ValueError(f"parameter group sizes {[len(g['params']) for g in groups]} != the model's {[len(pg) for pg in pgs]}")
+    if optimizer == "sgd":
+        if not all(g["nesterov"] and g.get("dampening", 0) == 0 and not g.get("maximize", False) for g in groups):
+            raise ValueError("only SGD(nesterov=True, dampening=0, maximize=False) is implemented")
+        _check_same(groups, "momentum")
+    else:
+        if any(g.get("amsgrad", False) or g.get("maximize", False) or g.get("decoupled_weight_decay", False) for g in groups):
+            raise ValueError("only Adam(amsgrad=False, maximize=False, decoupled_weight_decay=False) is implemented")
+        _check_same(groups, "betas")
+        _check_same(groups, "eps")
+    slices, n = _flat_slices(model)
+    buffers = {name: torch.zeros(n, dtype=torch.float32, device=device) for name in OPTIMIZER_STATE[optimizer]}
+    state, seen, steps = sd.get("state", {}), 0, set()
+    for g, ps in zip(groups, pgs):
+        for j, p in zip(g["params"], ps):
+            st = state.get(j)
+            if st is None:
+                continue
+            seen += 1
+            o, k = slices[id(p)]
+            for name in OPTIMIZER_STATE[optimizer]:
+                t = st.get(name)
+                if not isinstance(t, torch.Tensor) or tuple(t.shape) != tuple(p.shape):
+                    raise ValueError(f"state {j} {name!r}: expected a tensor of shape {tuple(p.shape)}, got "
+                                     f"{tuple(t.shape) if isinstance(t, torch.Tensor) else type(t).__name__}")
+                buffers[name][o:o + k].copy_(t.reshape(-1))
+            if optimizer == "adam":
+                steps.add(float(st["step"]))
+    if seen not in (0, sum(len(pg) for pg in pgs)):
+        raise ValueError(f"the state dict has state for {seen} of {sum(len(pg) for pg in pgs)} parameters")
+    if len(steps) > 1:
+        raise ValueError(f"Adam step counts differ between parameters: {sorted(steps)}")
+    nsteps = (int(steps.pop()) if optimizer == "adam" else 1) if seen else 0
+    return [{k: v for k, v in g.items() if k != "params"} for g in groups], nsteps, buffers
 
 
 class FlatState:
-    """Parameters, gradients and momentum of a model as three flat fp32 CUDA buffers; `p.data` / `p.grad` become views."""
+    """Parameters, gradients and momentum of a model as three flat fp32 CUDA buffers; `p.data` / `p.grad` become views.  With adam,
+    `momentum` is Adam's first moment (exp_avg) and a fourth buffer, `exp_avg_sq`, holds the second."""
 
-    def __init__(self, model: nn.Module):
+    def __init__(self, model: nn.Module, adam: bool = False):
         self.params = [p for p in model.parameters() if p.requires_grad]
         assert self.params and all(p.is_cuda and p.dtype == torch.float32 for p in self.params), "fp32 master parameters on the GPU"
         dev = self.params[0].device
@@ -65,6 +198,7 @@ class FlatState:
         self.n = n
         self.param = torch.zeros(n, dtype=torch.float32, device=dev)
         self.momentum = torch.zeros(n, dtype=torch.float32, device=dev)
+        self.exp_avg_sq = torch.zeros(n, dtype=torch.float32, device=dev) if adam else None
         self.group = torch.ones(n, dtype=torch.uint8, device=dev)
         groups = parameter_groups(model)
         for p, off in zip(self.params, self.offsets):
@@ -152,13 +286,18 @@ class Trainer:
 
     def __init__(self, model, hyp, batch_size, world_size=1, rank=-1, accumulate=1, detgain=0.6, seggain=0.35, init_scale=2.0 ** 16,
                  growth_interval=2000, process_group=None, graph_loss=True, fused_seg_loss=True, overlap_passes=True, fused_det_loss=True,
-                 concurrent_forwards=None, multi_scale=None, det_shapes=None):
+                 concurrent_forwards=None, multi_scale=None, det_shapes=None, optimizer="sgd"):
         """multi_scale: a MultiScale.  The det lane's train plans for every size it can draw from an imgsz x imgsz batch are reserved on
         one shared workspace (Engine.reserve_train_shapes); rescale each det batch with `multi_scale(imgs)` before `step`, as the reference
         does before its forward (train.py:354-359).  A det batch of fewer images (the loader's partial last batch) reserves its sizes on
         the same workspace the first time it comes; a batch of more images than batch_size does not fit it and raises MyoloError.
         det_shapes: the (H, W) shapes of the det batches (--rect: DetRectLoader.batch_shapes).  Their train plans are reserved on that one
-        shared workspace instead of a private pair per shape; with multi_scale, every size it can draw from each of them."""
+        shared workspace instead of a private pair per shape; with multi_scale, every size it can draw from each of them.
+        optimizer: "sgd" (torch.optim.SGD(momentum=hyp['momentum'], nesterov=True)) or "adam" (the reference's --adam:
+        torch.optim.Adam(betas=(hyp['momentum'], 0.999), eps=1e-8)), both over the reference's three groups.  Adam keeps its second
+        moment in one more flat fp32 buffer: 4 bytes per parameter element (31 MB for s/PSP, 94 MB for m/Lab)."""
+        if optimizer not in OPTIMIZER_STATE:
+            raise ValueError(f"optimizer must be 'sgd' or 'adam', got {optimizer!r}")
         assert next(model.parameters()).is_cuda, "model.cuda() first"
         self.model, self.hyp, self.batch_size = model, hyp, batch_size
         self.world_size, self.rank, self.accumulate, self.pg = world_size, rank, accumulate, process_group
@@ -173,11 +312,16 @@ class Trainer:
         self.n_seg_outputs = 3 if type(model.model[-2]).__name__ == "SegMaskBiSe" else 1
         # BiSe returns [out, aux16, aux32]: loss1 + 1.5*aux_weight*loss2 + 0.5*aux_weight*loss3 (reference train.py:387-388, utils/loss.py:239-244)
         self.compute_seg_loss = SegmentationLosses(ignore_index=-1, aux=self.n_seg_outputs == 3, aux_num=2)
-        self.flat = FlatState(model)
+        self.optimizer = optimizer
+        self.flat = FlatState(model, adam=optimizer == "adam")
         dev = self.flat.param.device
         self.lr = [hyp["lr0"]] * 3
-        self.wd = [0.0, hyp["weight_decay"], 0.0]
         self.momentum = hyp["momentum"]
+        self.betas, self.eps = (hyp["momentum"], 0.999), 1e-8                # train.py:129; used by "adam" only
+        self.param_groups = default_param_groups(optimizer, hyp)            # every other key of the groups, for state_dict()
+        self.wd = [g["weight_decay"] for g in self.param_groups]             # 0, hyp['weight_decay'], 0
+        # optimiser steps taken that were not skipped, counted on the device (Adam's bias corrections; whether torch would have state)
+        self.steps = torch.zeros((), dtype=torch.int32, device=dev)
         self.scale = torch.full((), float(init_scale), device=dev)
         self.growth_tracker = torch.zeros((), dtype=torch.int32, device=dev)
         self.growth_interval = growth_interval
@@ -215,7 +359,37 @@ class Trainer:
         self.lr = [float(lr_bn), float(lr_weight), float(lr_bias)]
 
     def set_momentum(self, m):
+        if self.optimizer == "adam":
+            raise ValueError("Adam's groups have no 'momentum': the reference's warm-up (train.py:351-352) leaves beta1 at hyp['momentum']")
         self.momentum = float(m)
+
+    # ---- optimiser state in torch's format (reference checkpoints' ckpt['optimizer']) ----------------------------------------------
+    def _state_buffers(self):
+        f = self.flat
+        return {"momentum_buffer": f.momentum} if self.optimizer == "sgd" else {"exp_avg": f.momentum, "exp_avg_sq": f.exp_avg_sq}
+
+    def state_dict(self):
+        """`optimizer.state_dict()` of the reference's optimizer (SGD or --adam) over this model, as its checkpoints hold it; state tensors
+        are CUDA copies.  Synchronises with the device (reads the step counter)."""
+        key = {"momentum": self.momentum} if self.optimizer == "sgd" else {"betas": self.betas, "eps": self.eps}
+        groups = [dict(g, lr=lr, weight_decay=wd, **key) for g, lr, wd in zip(self.param_groups, self.lr, self.wd)]
+        return optimizer_state_dict(self.model, self.optimizer, groups, int(self.steps), self._state_buffers())
+
+    def load_state_dict(self, sd):
+        """restores a state_dict() of this class or a reference checkpoint's ckpt['optimizer'] (tensors on any device): the moments, the step
+        count and each group's lr, weight decay and momentum / betas.  The loss scale is not touched (the reference does not save its
+        GradScaler).  ValueError when the dict does not fit this optimizer and model (see optimizer_state_from_dict)."""
+        groups, steps, bufs = optimizer_state_from_dict(self.model, self.optimizer, sd, device=self.flat.param.device)
+        for name, dst in self._state_buffers().items():
+            dst.copy_(bufs[name])
+        self.steps.fill_(steps)
+        self.param_groups = groups
+        self.lr = [g["lr"] for g in groups]
+        self.wd = [g["weight_decay"] for g in groups]
+        if self.optimizer == "sgd":
+            self.momentum = groups[0]["momentum"]
+        else:
+            self.betas, self.eps = groups[0]["betas"], groups[0]["eps"]
 
     # ---- the two passes --------------------------------------------------------------------------------------------
     def _det_loss_scaled(self, p, targets):
@@ -315,12 +489,19 @@ class Trainer:
         L, sp = _lib.lib(), _lib.stream_ptr()
         torch.reciprocal(self.scale * float(self.world_size), out=self.inv_scale)  # DDP averages: sum / world_size
         _lib.check(L.myolo_grads_check_finite(_lib.ptr(f.grad), f.n, _lib.ptr(self.found_inf), sp))
-        lr = (C.c_float * 3)(*self.lr)
         wd = (C.c_float * 3)(*self.wd)
-        _lib.check(L.myolo_sgd_step(_lib.ptr(f.param), _lib.ptr(f.grad), _lib.ptr(f.momentum), _lib.ptr(f.group), f.n, lr, wd, 3,
-                                    float(self.momentum), 1, _lib.ptr(self.inv_scale), _lib.ptr(self.found_inf), 1, sp))
+        if self.optimizer == "adam":
+            lr = (C.c_double * 3)(*self.lr)
+            _lib.check(L.myolo_adam_step(_lib.ptr(f.param), _lib.ptr(f.grad), _lib.ptr(f.momentum), _lib.ptr(f.exp_avg_sq), _lib.ptr(f.group),
+                                         f.n, lr, wd, 3, float(self.betas[0]), float(self.betas[1]), float(self.eps), _lib.ptr(self.steps),
+                                         _lib.ptr(self.inv_scale), _lib.ptr(self.found_inf), 1, sp))
+        else:
+            lr = (C.c_float * 3)(*self.lr)
+            _lib.check(L.myolo_sgd_step(_lib.ptr(f.param), _lib.ptr(f.grad), _lib.ptr(f.momentum), _lib.ptr(f.group), f.n, lr, wd, 3,
+                                        float(self.momentum), 1, _lib.ptr(self.inv_scale), _lib.ptr(self.found_inf), 1, sp))
         # amp.GradScaler.update: halve on overflow, double after growth_interval clean steps (device-side, no host sync)
         bad = self.found_inf[0] != 0
+        self.steps.add_((~bad).to(torch.int32))                               # after the launch: every block read the old count
         tracker = torch.where(bad, torch.zeros_like(self.growth_tracker), self.growth_tracker + 1)
         grow = tracker >= self.growth_interval
         self.scale.copy_(torch.where(bad, self.scale * 0.5, torch.where(grow, self.scale * 2.0, self.scale)))   # in place: graphs read it
