@@ -132,6 +132,10 @@ int myolo_plan_set_conv_weights(myolo_plan* plan, int weight_slot, const float* 
  * parameters changed in place - optimizer.step() reference train.py:396-398 - and every fp16 copy, forward and data-gradient, follows).
  * The pointers must still be valid; call myolo_plan_set_conv_weights again for a slot whose tensors moved. */
 int myolo_plan_repack_weights(myolo_plan* plan, void* stream);
+/* Overwrites n words of the plan's extra table (the `extra` of myolo_plan_create) from offset on, with n int32 / fp32 words read from
+ * DEVICE memory `src`, stream-ordered and at the table's device address (captured graphs stay valid).  Inference plans refresh each
+ * DETECT_DECODE op's anchors with it when the model's anchor_grid moved (an EMA averages it).  MYOLO_E_INVALID out of range. */
+int myolo_plan_set_extra(myolo_plan* plan, int offset, const void* src, int n, void* stream);
 /* One forward pass.  x: (B,3,H,W) NCHW of x_dtype (F32/F16 in [0,1], or U8 scaled by 1/255 like detect.py:137).
  * z: (B, sum_i 3*ny_i*nx_i, 5+nc) fp32;  raw[i]: (B,3,ny_i,nx_i,5+nc) fp32 (nullable);
  * seg: (B,n_segcls,H,W) of seg_dtype (nullable); seg_argmax: (B,H,W) int64 class ids (nullable, fused path). */
@@ -208,6 +212,23 @@ int myolo_adam_step(float* param, float* grad, float* exp_avg, float* exp_avg_sq
  * (float)sqrt(bc2[i]). */
 int myolo_adam_scalars(const int32_t* steps, int64_t n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt,
                        double* bc1, double* bc2, void* stream);
+/* ModelEMA.update (reference utils/torch_utils.py:290-300) over every floating-point state_dict entry in one launch, bit-identical with
+ * its three torch statements `v *= d; v += (1. - d) * msd[k]`, each rounding to its own dtype.  With df = (float)decay and
+ * d1f = (float)(1.0 - decay) (torch rounds a Python scalar to the op's fp32 math type):
+ *   fp32 EMA:  v = rn(rn(v * df) + rn(d1f * m))
+ *   fp16 EMA:  v = half_rn(rn(float(half_rn(float(v) * df)) + rn(d1f * m)))      (after the reference's ema.half() of test.py:45,124)
+ * chunks: DEVICE array of n_chunks pieces, each n (1 .. any) elements of one entry; the EMA side is MYOLO_F32 or MYOLO_F16, the source
+ * (the training model's entry) is always fp32.  The caller cuts entries at multiples of MYOLO_EMA_CHUNK elements (one CTA per chunk).  A
+ * chunk whose two pointers are 16-byte (fp16 EMA: 8-byte) aligned runs 4-wide; any other runs element by element.  MYOLO_E_INVALID for
+ * a null table, n_chunks < 1 or decay outside [0, 1]; the table's contents are the caller's to validate (Python: ValueError). */
+#define MYOLO_EMA_CHUNK 8192
+typedef struct {
+  void* ema;           /* fp32 or fp16 EMA elements, updated in place */
+  const float* src;    /* fp32 training-model elements */
+  int32_t n;           /* elements in this chunk */
+  int32_t dtype;       /* MYOLO_F32 or MYOLO_F16: the EMA side's dtype */
+} myolo_ema_chunk;
+int myolo_ema_update(const myolo_ema_chunk* chunks /* device */, int n_chunks, double decay, void* stream);
 
 /* Detection loss forward + backward in four launches (reference utils/loss.py:115-217 `ComputeLoss.__call__` / `build_targets` + autograd):
  * p[l] / dp[l]: the nl raw head outputs (B, na, ny[l], nx[l], no) fp32 and their gradients (overwritten); targets (nt, 6) [image, class,

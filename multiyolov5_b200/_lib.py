@@ -37,7 +37,7 @@ EXPORTS = [
     "myolo_grads_check_finite", "myolo_sgd_step", "myolo_conv_wgrad", "myolo_letterbox", "myolo_seg_lut_blend", "myolo_seg_metrics", "myolo_plan_backward_seg_ce", "myolo_plan_read_grad_view", "myolo_plan_set_seed", "myolo_plan_train_forward_multi", "myolo_plan_backward_multi", "myolo_plan_conv_info", "myolo_allreduce_grads", "myolo_det_loss", "myolo_det_loss_workspace_bytes", "myolo_plan_set_defer_running", "myolo_plan_apply_running",
     "myolo_resize_u8", "myolo_augment_det", "myolo_augment_seg", "myolo_det_match", "myolo_det_ap", "myolo_det_ap_workspace_bytes",
     "myolo_resize_area_u8", "myolo_resize_bilinear", "myolo_plan_create_shared", "myolo_augment_det_hw", "myolo_adam_step",
-    "myolo_adam_scalars",
+    "myolo_adam_scalars", "myolo_ema_update", "myolo_plan_set_extra",
 ]
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
 
@@ -71,6 +71,14 @@ class SegItem(C.Structure):
                 ("ky", C.c_int32), ("col", C.c_int32), ("row", C.c_int32), ("mcol", C.c_int32), ("mrow", C.c_int32),
                 ("order", C.c_int32 * 4), ("factor", C.c_float * 3), ("hue_shift", C.c_int32), ("reserved", C.c_int32),
                 ("lsum", C.c_uint64), ("lut", C.c_int32 * 256)]
+
+
+class EmaChunk(C.Structure):
+    """include/myolo.h myolo_ema_chunk: elements [ema, ema + n) of one EMA entry (dtype F32 / F16) and [src, src + n) of its fp32 source"""
+    _fields_ = [("ema", C.c_void_p), ("src", C.c_void_p), ("n", C.c_int32), ("dtype", C.c_int32)]
+
+
+EMA_CHUNK = 8192        # include/myolo.h MYOLO_EMA_CHUNK: entries are cut at multiples of it, one CTA per chunk
 
 
 class MyoloError(RuntimeError):
@@ -136,6 +144,8 @@ def lib():
     L.myolo_adam_step.argtypes = [vp, vp, vp, vp, vp, i64, C.POINTER(C.c_double), C.POINTER(f32), i32, C.c_double, C.c_double, C.c_double,
                                   vp, vp, vp, i32, vp]
     L.myolo_adam_scalars.argtypes = [vp, i64, C.c_double, C.c_double, C.c_double, vp, vp, vp, vp, vp]
+    L.myolo_ema_update.argtypes = [vp, i32, C.c_double, vp]
+    L.myolo_plan_set_extra.argtypes = [vp, i32, vp, i32, vp]
     L.myolo_allreduce_grads.argtypes = [vp, i64, vp, vp]
     L.myolo_det_loss_workspace_bytes.argtypes = [i32, i32, i32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
     L.myolo_det_loss_workspace_bytes.restype = i64

@@ -372,6 +372,14 @@ extern "C" int myolo_plan_repack_weights(myolo_plan* pl, void* stream) {
   return 0;
 }
 
+// the extra table is read by the ops (and baked into captured graphs) at its device address: refreshed in place, in stream order
+extern "C" int myolo_plan_set_extra(myolo_plan* pl, int offset, const void* src, int n, void* stream) {
+  MYOLO_REQUIRE(pl && src && offset >= 0 && n > 0 && (size_t)offset + (size_t)n <= pl->extra.size(),
+                "plan_set_extra: words [%d, %d) outside the extra table of %d words", offset, offset + n, pl ? (int)pl->extra.size() : 0);
+  MYOLO_CHECK_CUDA(cudaMemcpyAsync(pl->d_extra + offset, src, (size_t)n * 4, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return 0;
+}
+
 static int prepare_conv(myolo_plan* pl, int i) {
   const myolo_op& op = pl->ops[i];
   MYOLO_REQUIRE(op.weight_slot >= 0 && op.weight_slot < (int)pl->slots.size(), "op %d: bad weight slot", i);
@@ -1310,6 +1318,13 @@ extern "C" int myolo_adam_scalars(const int32_t* steps, int64_t n, double lr, do
   int rc = check_device(nullptr);
   if (rc) return rc;
   return launch_adam_scalars(steps, (long)n, lr, beta1, beta2, step_size, bc2_sqrt, bc1, bc2, (cudaStream_t)stream);
+}
+
+extern "C" int myolo_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay, void* stream) {
+  NvtxRange nvtx_("myolo_ema_update");
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_ema_update(chunks, n_chunks, decay, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1370,4 +1370,69 @@ int launch_adam_scalars(const int* steps, long n, double lr, double beta1, doubl
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// ModelEMA.update (reference utils/torch_utils.py:290-300) over every floating-point state_dict entry: one CTA per chunk of the device
+// table, 12 B of HBM traffic per fp32 element (8 B for an fp16 EMA).  The reference runs three torch ops per entry, each rounding to its
+// own dtype; the _rn intrinsics keep nvcc from contracting them into an FMA:
+//   v *= d                   rn(v * df)                   fp16 EMA: half_rn(float(v) * df)      (opmath float, stored as half)
+//   t  = (1. - d) * msd[k]   rn(d1f * m)                  fp32 (the source is the fp32 training model)
+//   v += t                   rn(v + t)                    fp16 EMA: half_rn(float(v) + t)       (promoted to fp32, stored as half)
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ float ema_f32(float v, float m, float df, float d1f) {
+  return __fadd_rn(__fmul_rn(v, df), __fmul_rn(d1f, m));
+}
+__device__ __forceinline__ __half ema_f16(__half v, float m, float df, float d1f) {
+  const float a = __half2float(__float2half_rn(__fmul_rn(__half2float(v), df)));
+  return __float2half_rn(__fadd_rn(a, __fmul_rn(d1f, m)));
+}
+
+__global__ void __launch_bounds__(256) ema_update_kernel(const myolo_ema_chunk* __restrict__ chunks, float df, float d1f) {
+  const myolo_ema_chunk c = chunks[blockIdx.x];
+  const float* __restrict__ src = c.src;
+  const int n = c.n;
+  int i0 = 0;                                              // first element of the scalar part
+  if (c.dtype == MYOLO_F32) {
+    float* __restrict__ v = static_cast<float*>(c.ema);
+    if (((reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(src)) & 15) == 0) {
+      const int n4 = n >> 2;
+      for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+        float4 a = reinterpret_cast<float4*>(v)[i];
+        const float4 m = __ldg(reinterpret_cast<const float4*>(src) + i);
+        a.x = ema_f32(a.x, m.x, df, d1f);
+        a.y = ema_f32(a.y, m.y, df, d1f);
+        a.z = ema_f32(a.z, m.z, df, d1f);
+        a.w = ema_f32(a.w, m.w, df, d1f);
+        reinterpret_cast<float4*>(v)[i] = a;
+      }
+      i0 = n4 * 4;
+    }
+    for (int i = i0 + threadIdx.x; i < n; i += blockDim.x) v[i] = ema_f32(v[i], __ldg(src + i), df, d1f);
+  } else {
+    __half* __restrict__ v = static_cast<__half*>(c.ema);
+    if ((reinterpret_cast<uintptr_t>(v) & 7) == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0) {
+      const int n4 = n >> 2;
+      for (int i = threadIdx.x; i < n4; i += blockDim.x) {
+        uint2 raw = reinterpret_cast<uint2*>(v)[i];
+        __half2* h = reinterpret_cast<__half2*>(&raw);
+        const float4 m = __ldg(reinterpret_cast<const float4*>(src) + i);
+        h[0] = __halves2half2(ema_f16(__low2half(h[0]), m.x, df, d1f), ema_f16(__high2half(h[0]), m.y, df, d1f));
+        h[1] = __halves2half2(ema_f16(__low2half(h[1]), m.z, df, d1f), ema_f16(__high2half(h[1]), m.w, df, d1f));
+        reinterpret_cast<uint2*>(v)[i] = raw;
+      }
+      i0 = n4 * 4;
+    }
+    for (int i = i0 + threadIdx.x; i < n; i += blockDim.x) v[i] = ema_f16(v[i], __ldg(src + i), df, d1f);
+  }
+}
+
+int launch_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay, cudaStream_t s) {
+  MYOLO_REQUIRE(chunks && n_chunks > 0, "ema_update: empty chunk table");
+  MYOLO_REQUIRE(decay >= 0.0 && decay <= 1.0, "ema_update: decay %g outside [0, 1]", decay);
+  MYOLO_REQUIRE((reinterpret_cast<uintptr_t>(chunks) & 7) == 0, "ema_update: chunk table must be 8-byte aligned");
+  // torch hands `d` and `1. - d` (Python doubles) to fp32-math kernels: each is rounded to fp32 once
+  ema_update_kernel<<<n_chunks, 256, 0, s>>>(chunks, (float)decay, (float)(1.0 - decay));
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace myolo

@@ -86,6 +86,7 @@ int launch_adam_step(float* p, float* g, float* m, float* v, const unsigned char
                      int zero_grad, cudaStream_t s);
 int launch_adam_scalars(const int* steps, long n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt, double* bc1,
                         double* bc2, cudaStream_t s);
+int launch_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay, cudaStream_t s);
 // wgmma weight gradient (wgrad_tc.cu): dw_packed is a zeroed fp32 [co][k*k][ci] accumulation buffer owned by the caller
 bool conv_wgrad_tc_eligible(const TensorView& x, const TensorView& dy, int k, int stride, int dil, int co, int ci);
 size_t conv_wgrad_packed_bytes(const float* dW, int co, int ci, int k);   // 0: accumulates straight into dW

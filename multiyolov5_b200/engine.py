@@ -123,6 +123,19 @@ class CompiledPlan:
         self.weights_uploaded = True
         self.weights_registered = sig
 
+    def refresh_anchors(self, det):
+        """rewrites each DETECT_DECODE op's anchors (pixels, in the plan's extra table since the plan was built) from det.anchor_grid as it
+        is now, in place: an EMA averages anchor_grid with every other floating-point entry (reference utils/torch_utils.py:297-300), so
+        its values move between validations.  fp16 after model.half(): the same values the plan would take from a fresh build."""
+        L, sp = _lib.lib(), _lib.stream_ptr()
+        ag = det.anchor_grid.detach().to(dtype=torch.float32).contiguous()     # (nl, 1, na, 1, 1, 2)
+        for o in self.pb.ops:
+            if o.kind == _lib.OP_DETECT_DECODE:
+                level, na, off = o.aux[0], o.aux[1], o.aux[5]
+                src = ag[level].reshape(-1)
+                assert src.numel() == 2 * na
+                _lib.check(L.myolo_plan_set_extra(self.handle, off, _lib.ptr(src), 2 * na, sp))
+
 
 class Engine:
     def __init__(self, model):
@@ -147,6 +160,7 @@ class Engine:
             self.weights_dirty = False
         if not p.weights_uploaded:
             p.upload_weights()
+            p.refresh_anchors(self.model.model[-1])
         self.last_plan = p
         return p
 

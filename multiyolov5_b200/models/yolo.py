@@ -199,15 +199,22 @@ class Model(nn.Module):
         if getattr(self, "_engine", None) is not None:
             self._engine.weights_dirty = True
 
+    def tensors_moved(self):
+        """parameters / buffers may have new storage or dtype (_apply, load_state_dict, the Trainer's flat buffers): bumps the counter
+        that tables of raw pointers into them (ModelEMA's device table) compare against"""
+        self._tensor_epoch = getattr(self, "_tensor_epoch", 0) + 1
+
     def load_state_dict(self, *a, **k):
         r = super().load_state_dict(*a, **k)
         self.invalidate_weights()
+        self.tensors_moved()
         return r
 
     def _apply(self, fn, *a, **k):
         r = super()._apply(fn, *a, **k)
         if getattr(self, "_engine", None) is not None:
             self._engine.weights_dirty = True
+        self.tensors_moved()
         return r
 
     # ---- pickling / deepcopy (reference train.py:485 `deepcopy(model).half()`, utils/torch_utils.py:282 ModelEMA, torch.save of the

@@ -15,8 +15,12 @@ more flat buffer for the second moment and one launch (`myolo_adam_step`).  `Tra
 optimiser buffers to and from torch's `optimizer.state_dict()` format, which is what the reference's checkpoints hold in
 `ckpt['optimizer']` (train.py:482-494, restored at :155-160).
 
+`Trainer(..., ema=ModelEMA(model))` is the reference's `ema.update(model)` after every optimizer step (train.py:401), including a step
+skipped for overflow: one launch (`myolo_ema_update`) over every floating-point entry of the model, bit-identical with the reference's
+per-entry statements.  Pass it on rank -1 / 0 and None elsewhere, as train.py:151 builds it.
+
 Out of scope (the reference's outer loop, not the hot path): data loading, LR schedule / warm-up (call `set_lr` / `set_momentum`),
-EMA, writing checkpoint files, plotting, DDP buffer broadcast.
+writing checkpoint files, plotting, DDP buffer broadcast.
 """
 import math
 import random
@@ -206,6 +210,8 @@ class FlatState:
             self.param[off:off + k].copy_(p.data.reshape(-1))
             p.data = self.param[off:off + k].view_as(p)
             self.group[off:off + k] = groups.get(id(p), 1)
+        if hasattr(model, "tensors_moved"):
+            model.tensors_moved()                                 # a ModelEMA built before the Trainer re-reads the new addresses
 
     def check_views(self, model):
         """cheap guard: someone re-assigned parameters (.half(), load_state_dict with assign, .to()) -> views are stale"""
@@ -286,7 +292,7 @@ class Trainer:
 
     def __init__(self, model, hyp, batch_size, world_size=1, rank=-1, accumulate=1, detgain=0.6, seggain=0.35, init_scale=2.0 ** 16,
                  growth_interval=2000, process_group=None, graph_loss=True, fused_seg_loss=True, overlap_passes=True, fused_det_loss=True,
-                 concurrent_forwards=None, multi_scale=None, det_shapes=None, optimizer="sgd"):
+                 concurrent_forwards=None, multi_scale=None, det_shapes=None, optimizer="sgd", ema=None):
         """multi_scale: a MultiScale.  The det lane's train plans for every size it can draw from an imgsz x imgsz batch are reserved on
         one shared workspace (Engine.reserve_train_shapes); rescale each det batch with `multi_scale(imgs)` before `step`, as the reference
         does before its forward (train.py:354-359).  A det batch of fewer images (the loader's partial last batch) reserves its sizes on
@@ -295,7 +301,9 @@ class Trainer:
         shared workspace instead of a private pair per shape; with multi_scale, every size it can draw from each of them.
         optimizer: "sgd" (torch.optim.SGD(momentum=hyp['momentum'], nesterov=True)) or "adam" (the reference's --adam:
         torch.optim.Adam(betas=(hyp['momentum'], 0.999), eps=1e-8)), both over the reference's three groups.  Adam keeps its second
-        moment in one more flat fp32 buffer: 4 bytes per parameter element (31 MB for s/PSP, 94 MB for m/Lab)."""
+        moment in one more flat fp32 buffer: 4 bytes per parameter element (31 MB for s/PSP, 94 MB for m/Lab).
+        ema: a utils.torch_utils.ModelEMA of this model (built before or after the Trainer), updated on the main stream right after every
+        optimizer step, when both passes have joined and the seg pass's deferred BatchNorm statistics are applied."""
         if optimizer not in OPTIMIZER_STATE:
             raise ValueError(f"optimizer must be 'sgd' or 'adam', got {optimizer!r}")
         assert next(model.parameters()).is_cuda, "model.cuda() first"
@@ -313,6 +321,7 @@ class Trainer:
         # BiSe returns [out, aux16, aux32]: loss1 + 1.5*aux_weight*loss2 + 0.5*aux_weight*loss3 (reference train.py:387-388, utils/loss.py:239-244)
         self.compute_seg_loss = SegmentationLosses(ignore_index=-1, aux=self.n_seg_outputs == 3, aux_num=2)
         self.optimizer = optimizer
+        self.ema = ema
         self.flat = FlatState(model, adam=optimizer == "adam")
         dev = self.flat.param.device
         self.lr = [hyp["lr0"]] * 3
@@ -507,6 +516,8 @@ class Trainer:
         self.scale.copy_(torch.where(bad, self.scale * 0.5, torch.where(grow, self.scale * 2.0, self.scale)))   # in place: graphs read it
         self.growth_tracker.copy_(torch.where(grow, torch.zeros_like(tracker), tracker))
         self.model.engine().weights_dirty = True
+        if self.ema is not None:
+            self.ema.update(self.model)            # train.py:401: every step, a skipped one too (reads parameters and BN buffers)
 
     def step(self, imgs, targets, segimgs, segtargets):
         """one iteration (train.py:363-401).  Returns (det loss items [lbox,lobj,lcls,loss], seg loss) as device tensors."""
