@@ -69,8 +69,14 @@ class CompiledPlan:
             _lib.check(L.myolo_plan_create_shared(*args, _lib.ptr(arena.ws), _lib.ptr(arena.gws), arena.capacity, C.byref(h)))
         self.handle = h
         self.B, self.H, self.W = B, H, W
-        self.weights_uploaded = False
+        self.weights_key = None              # Engine.weights_key() when the fp16 packs were last uploaded: stale when it differs
         self.weights_registered = None       # pointer signature of the tensors the library holds (myolo_plan_repack_weights)
+        # train plans only (Engine.prepare_train_plan / train_forward)
+        self._seed_set = False
+        self._ptr_sig = None                 # parameter / gradient pointers registered with the library
+        self._nbt = []                       # num_batches_tracked of the BatchNorm slots
+        self._defer_running = False          # Engine.set_defer_running
+        self.fwd_generation = 0              # train forwards of this plan (or of its arena): a backward is valid for the latest only
 
     def __del__(self):
         try:
@@ -94,7 +100,6 @@ class CompiledPlan:
         sig = self._pointer_signature()
         if self.weights_registered == sig and -1 not in sig and os.environ.get("MYOLO_REPACK", "1") != "0":
             _lib.check(L.myolo_plan_repack_weights(self.handle, sp))
-            self.weights_uploaded = True
             return
         keep = []
 
@@ -120,7 +125,6 @@ class CompiledPlan:
             co, ci, k = w.shape[0], w.shape[1], w.shape[2]
             _lib.check(L.myolo_plan_set_conv_weights(self.handle, i, _lib.ptr(w), co, ci, k, _lib.ptr(g), _lib.ptr(b), _lib.ptr(m),
                                                      _lib.ptr(v), eps, _lib.ptr(bias), sp))
-        self.weights_uploaded = True
         self.weights_registered = sig
 
     def refresh_anchors(self, det):
@@ -140,27 +144,43 @@ class CompiledPlan:
 class Engine:
     def __init__(self, model):
         self.model = model
-        self.plans: Dict[Tuple[int, int, int], CompiledPlan] = {}
-        self.weights_dirty = True
+        self.plans: Dict[Tuple[int, ...], CompiledPlan] = {}
+        self.param_epoch = 0   # writes to parameters / buffers that torch's version counters do not see (Model.invalidate_weights)
+        self.stats_epoch = 0   # train forwards: they move the BatchNorm running statistics through raw pointers
         self.last_plan = None
+        self.last_profile = None
         self.noalias = False   # debug: give every buffer private memory so intermediate views stay readable after forward
+        self._reserved = {}    # train plan key -> (TrainArena, host plan) (reserve_train_shapes)
+        self._arenas = {}      # lane -> TrainArena
+        self._train_params = []
+        self._flat_grad = None
+        self._flat_offsets = []
+        self._grad_views = []
+        self._anchor = None    # autograd input of _TrainFunction
+
+    def weights_key(self, train):
+        """what a plan's fp16 weight packs were made from; a plan re-packs before its next launch when the key differs from the one of its
+        last upload.  Inference packs fold BatchNorm, so every parameter and buffer counts, the running statistics included; train packs
+        do not fold it, so only the trainable parameters count (running statistics moving between optimiser steps repack nothing)."""
+        if train:
+            return sum(q._version for q in self._train_params), self.param_epoch
+        ver = sum(q._version for q in self.model.parameters()) + sum(q._version for q in self.model.buffers())
+        return ver, self.param_epoch, self.stats_epoch
+
+    def _upload_if_stale(self, p):
+        key = self.weights_key(p.train)
+        if p.weights_key != key:
+            p.upload_weights()                   # train plans: fp16, K-major, no BN folding
+            if not p.train:
+                p.refresh_anchors(self.model.model[-1])
+            p.weights_key = key
 
     def plan_for(self, B, H, W) -> CompiledPlan:
         key = (B, H, W)
         if key not in self.plans:
             self.plans[key] = CompiledPlan(self.model, B, H, W, self.noalias)
         p = self.plans[key]
-        ver = sum(q._version for q in self.model.parameters()) + sum(q._version for q in self.model.buffers())
-        if getattr(self, "_infer_version", None) != ver:      # in-place edits of parameters / buffers bump torch's version counters
-            self._infer_version = ver
-            self.weights_dirty = True
-        if self.weights_dirty:
-            for q in self.plans.values():
-                q.weights_uploaded = False
-            self.weights_dirty = False
-        if not p.weights_uploaded:
-            p.upload_weights()
-            p.refresh_anchors(self.model.model[-1])
+        self._upload_if_stale(p)
         self.last_plan = p
         return p
 
@@ -202,10 +222,10 @@ class Engine:
     # ---- training (SURVEY.md section 8 row a13) -----------------------------------------------------------------------
     def train_plan_for(self, B, H, W, lane=0) -> CompiledPlan:
         """lane: independent train plans of the same shape (own activation / gradient workspaces) so that the two passes of a training step
-        can be in flight at the same time (train.Trainer overlap_passes)"""
+        can be in flight at the same time (train.Trainer: the seg pass runs on lane 1)"""
         key = ("train", B, H, W) if lane == 0 else ("train", B, H, W, lane)
         if key not in self.plans:
-            arena, pb = getattr(self, "_reserved", {}).get(key, (None, None))
+            arena, pb = self._reserved.get(key, (None, None))
             self.plans[key] = CompiledPlan(self.model, B, H, W, train=True, arena=arena, pb=pb)
         return self.plans[key]
 
@@ -218,8 +238,6 @@ class Engine:
         shapes = sorted({(int(h), int(w)) for h, w in shapes})
         if not shapes:
             raise ValueError("reserve_train_shapes: no shapes")
-        self._reserved = getattr(self, "_reserved", {})
-        self._arenas = getattr(self, "_arenas", {})
         keys = {hw: (("train", B) + hw if lane == 0 else ("train", B) + hw + (lane,)) for hw in shapes}
         arena = self._arenas.get(lane)
         pbs, need = shared_train_plans(self.model, B, [hw for hw in shapes
@@ -240,7 +258,7 @@ class Engine:
         train.py:243-245 DDP semantics) that the backward kernels accumulate into."""
         params = [p for p in self.model.parameters() if p.requires_grad]
         self._train_params = params
-        if getattr(self, "_flat_grad", None) is not None and all(p.grad is not None and p.grad.data_ptr() == g.data_ptr()
+        if self._flat_grad is not None and all(p.grad is not None and p.grad.data_ptr() == g.data_ptr()
                                                                   for p, g in zip(params, self._grad_views)):
             return self._flat_grad
         for p in params:
@@ -258,30 +276,15 @@ class Engine:
         return self._flat_grad
 
     def prepare_train_plan(self, p):
-        """seed, fp16 weight packs and parameter / gradient pointers of a train plan for the current parameter values (idempotent; the
-        Trainer calls it ahead of time on the side stream for the seg pass)"""
+        """seed, fp16 weight packs and parameter / gradient pointers of a train plan for the current parameter values (idempotent)"""
         L = _lib.lib()
-        sp = _lib.stream_ptr()
         params = self._train_params
-        if not getattr(p, "_seed_set", False):       # dropout masks follow torch's global seed (one hash stream per plan)
+        if not p._seed_set:                      # dropout masks follow torch's global seed (one hash stream per plan)
             _lib.check(L.myolo_plan_set_seed(p.handle, C.c_uint64(torch.initial_seed() & 0xFFFFFFFFFFFFFFFF)))
             p._seed_set = True
-        # re-pack the fp16 weights only when the parameters changed (in-place torch updates bump _version; Trainer's fused optimiser
-        # writes through raw pointers and sets weights_dirty)
-        ver = sum(q._version for q in params)
-        if self.weights_dirty:
-            self._dirty_epoch = getattr(self, "_dirty_epoch", 0) + 1      # the fused optimiser wrote through raw pointers
-            self.weights_dirty = False
-            for q in self.plans.values():        # every plan (inference ones too) holds packed copies of the old values
-                q.weights_uploaded = False
-        sig_w = (ver, getattr(self, "_dirty_epoch", 0))
-        if getattr(p, "_w_version", None) != sig_w:
-            p.weights_uploaded = False
-        if not p.weights_uploaded:
-            p.upload_weights()                   # fp16, K-major, no BN folding
-            p._w_version = sig_w
+        self._upload_if_stale(p)
         sig = (self._flat_grad.data_ptr(), params[0].data_ptr(), params[-1].data_ptr(), len(params))
-        if getattr(p, "_ptr_sig", None) != sig:  # (re)register parameter / gradient pointers only when they moved
+        if p._ptr_sig != sig:                    # (re)register parameter / gradient pointers only when they moved
             for i, s in enumerate(p.pb.slots):
                 _lib.check(L.myolo_plan_set_conv_grad(p.handle, i, _lib.ptr(s.conv.weight.grad), _lib.ptr(s.conv.bias.grad if s.conv.bias is not None else None)))
             for i, bn in enumerate(p.pb.bn_slots):
@@ -301,7 +304,7 @@ class Engine:
         self.prepare_train_plan(p)
         L = _lib.lib()
         sp = _lib.stream_ptr()
-        if not getattr(p, "_defer_running", False):      # a deferring plan counts its batch in apply_running
+        if not p._defer_running:                         # a deferring plan counts its batch in apply_running
             torch._foreach_add_(p._nbt, 1)
         det, seg_head = self.model.model[-1], self.model.model[-2]
         dec = [o.in_ for o in p.pb.ops if o.kind == _lib.OP_DETECT_DECODE]
@@ -320,32 +323,29 @@ class Engine:
         # activations / batch statistics / dropout step of THIS forward live in the plan's single workspace: a backward is only valid
         # for the most recent train forward of the plan (the reference's order forward, backward, forward, backward - train.py:364-392);
         # plans on a shared workspace: for the most recent train forward of ANY plan bound to it
-        p.fwd_generation = gen if gen is not None else getattr(p, "fwd_generation", 0) + 1
-        # running_mean / running_var moved (raw pointers): every inference plan's BN-folded weights are stale now
-        for q in self.plans.values():
-            if not q.train:
-                q.weights_uploaded = False
+        p.fwd_generation = gen if gen is not None else p.fwd_generation + 1
+        self.stats_epoch += 1                            # running_mean / running_var moved: inference packs are stale
         self.last_plan = p
         return raws, (segs[0] if n_seg == 1 else segs), p
 
-    def set_defer_running(self, plan, on=True):
-        """a deferring train plan leaves running_mean / running_var / num_batches_tracked alone in its forward (apply_running moves them):
-        lets the seg pass's forward run next to the det pass's while the statistics still move in the reference's order"""
-        if getattr(plan, "_defer_running", False) != bool(on):
-            _lib.check(_lib.lib().myolo_plan_set_defer_running(plan.handle, int(bool(on))))
-            plan._defer_running = bool(on)
+    def set_defer_running(self, plan):
+        """from now on `plan`'s forwards leave running_mean / running_var / num_batches_tracked alone (apply_running moves them): lets the
+        seg pass's forward run next to the det pass's while the statistics still move in the reference's order"""
+        if not plan._defer_running:
+            _lib.check(_lib.lib().myolo_plan_set_defer_running(plan.handle, 1))
+            plan._defer_running = True
 
     def apply_running(self, plan):
         _lib.check(_lib.lib().myolo_plan_apply_running(plan.handle, _lib.stream_ptr()))
         torch._foreach_add_(plan._nbt, 1)
 
     def _check_generation(self, plan, generation):
-        a = getattr(plan, "arena", None)
+        a = plan.arena
         if a is not None and (a.owner is not plan or (generation is not None and generation != a.generation)):
             raise _lib.MyoloError(f"backward of a stale train-mode forward: another train forward ran on the shared workspace of "
                                   f"({plan.B},{plan.H},{plan.W}) after it and overwrote the saved activations (one outstanding forward per "
                                   "lane; run forward, backward, forward, backward like reference train.py:364-392)")
-        if generation is not None and generation != getattr(plan, "fwd_generation", 0):
+        if generation is not None and generation != plan.fwd_generation:
             raise _lib.MyoloError("backward of a stale train-mode forward: another forward of the same (B,H,W) ran in between and overwrote the "
                                   "saved activations (one outstanding forward per shape; run forward, backward, forward, backward like "
                                   "reference train.py:364-392)")
@@ -407,7 +407,7 @@ class _TrainFunction(torch.autograd.Function):
 
 def train_forward(model, x):
     eng = model.engine()
-    if not hasattr(eng, "_anchor"):
+    if eng._anchor is None:
         eng._anchor = torch.zeros((), device=x.device, requires_grad=True)
     out = _TrainFunction.apply(eng._anchor, eng, x)
     return [list(out[:3]), out[3] if len(out) == 4 else list(out[3:])]     # BiSe: seg = [out, aux16, aux32] (models/yolo.py:86)

@@ -196,8 +196,10 @@ class Model(nn.Module):
 
     # ---- plan / engine ---------------------------------------------------------------------------------------------
     def invalidate_weights(self):
+        """parameters or buffers were written where torch's version counters do not see it (raw pointers: the Trainer's fused optimiser,
+        ModelEMA.update; new storage: _apply, load_state_dict): every compiled plan re-packs its weights before its next launch"""
         if getattr(self, "_engine", None) is not None:
-            self._engine.weights_dirty = True
+            self._engine.param_epoch += 1
 
     def tensors_moved(self):
         """parameters / buffers may have new storage or dtype (_apply, load_state_dict, the Trainer's flat buffers): bumps the counter
@@ -212,8 +214,7 @@ class Model(nn.Module):
 
     def _apply(self, fn, *a, **k):
         r = super()._apply(fn, *a, **k)
-        if getattr(self, "_engine", None) is not None:
-            self._engine.weights_dirty = True
+        self.invalidate_weights()
         self.tensors_moved()
         return r
 

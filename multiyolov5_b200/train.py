@@ -32,7 +32,7 @@ import torch.nn as nn
 from . import _lib
 from .engine import flat_offsets
 from .parallel import allreduce_flat_grads
-from .utils.loss import ComputeLoss, FusedComputeLoss, SegmentationLosses
+from .utils.loss import FusedComputeLoss, SegmentationLosses
 
 
 def scale_hyp(hyp: dict, nl: int, nc: int, imgsz: int, total_batch_size: int, nbs: int = 64, label_smoothing: float = 0.0) -> dict:
@@ -291,8 +291,7 @@ class Trainer:
     """`Trainer(model, hyp, batch_size).step(imgs, targets, segimgs, segtargets)`; hyp already scaled (see scale_hyp)."""
 
     def __init__(self, model, hyp, batch_size, world_size=1, rank=-1, accumulate=1, detgain=0.6, seggain=0.35, init_scale=2.0 ** 16,
-                 growth_interval=2000, process_group=None, graph_loss=True, fused_seg_loss=True, overlap_passes=True, fused_det_loss=True,
-                 concurrent_forwards=None, multi_scale=None, det_shapes=None, optimizer="sgd", ema=None):
+                 growth_interval=2000, process_group=None, multi_scale=None, det_shapes=None, optimizer="sgd", ema=None):
         """multi_scale: a MultiScale.  The det lane's train plans for every size it can draw from an imgsz x imgsz batch are reserved on
         one shared workspace (Engine.reserve_train_shapes); rescale each det batch with `multi_scale(imgs)` before `step`, as the reference
         does before its forward (train.py:354-359).  A det batch of fewer images (the loader's partial last batch) reserves its sizes on
@@ -312,14 +311,16 @@ class Trainer:
         self.detgain, self.seggain = detgain, seggain          # train.py:290
         model.hyp, model.gr = hyp, getattr(model, "gr", 1.0)
         model.train()
-        self.compute_loss = ComputeLoss(model)
-        # detection loss forward + backward as four launches of the library (csrc/detloss.cu) instead of ~760 torch kernels; the torch
-        # formulation stays for focal loss / positive weights / autobalance and is what the tests compare it with
-        self._fused_det = FusedComputeLoss(model) if fused_det_loss else None
-        self.fused_det_loss = bool(fused_det_loss) and self._fused_det.supported
+        # detection loss forward + backward as four launches of the library (csrc/detloss.cu) instead of ~760 torch kernels.  Focal loss /
+        # positive weights / autobalance take the torch formulation (compute_loss), replayed as one captured CUDA graph (_det_graph)
+        self._fused_det = FusedComputeLoss(model)
+        self.compute_loss = self._fused_det.ref
         self.n_seg_outputs = 3 if type(model.model[-2]).__name__ == "SegMaskBiSe" else 1
         # BiSe returns [out, aux16, aux32]: loss1 + 1.5*aux_weight*loss2 + 0.5*aux_weight*loss3 (reference train.py:387-388, utils/loss.py:239-244)
         self.compute_seg_loss = SegmentationLosses(ignore_index=-1, aux=self.n_seg_outputs == 3, aux_num=2)
+        # seg CE + x8 upsample forward / backward in one kernel, no full-resolution logits: plain heads with 19 (Cityscapes) or 32 classes,
+        # the instantiations in csrc/train.cu; other heads take autograd
+        self.fused_seg = self.n_seg_outputs == 1 and model.model[-2].c_out in (19, 32)
         self.optimizer = optimizer
         self.ema = ema
         self.flat = FlatState(model, adam=optimizer == "adam")
@@ -337,16 +338,8 @@ class Trainer:
         self.found_inf = torch.zeros(1, dtype=torch.int32, device=dev)
         self.inv_scale = torch.ones((), device=dev)
         self.ni = 0
-        self.graph_loss = graph_loss        # replay the detection loss (forward + autograd backward, ~700 tiny kernels) as ONE CUDA graph
         self._det_graphs = {}
-        self.fused_seg_loss = fused_seg_loss  # CE + x8 upsample forward/backward in one kernel, no full-resolution logits (plain heads only)
-        # overlap_passes: the seg pass runs on its own train plan and stream.  Its forward starts when the det FORWARD has finished (BatchNorm
-        # running statistics are then updated in the reference's order, det batch first: train.py:364,381), so the seg forward/backward
-        # overlaps the det loss + backward; parameter gradients of both passes add up atomically in the one flat buffer.  At 4 images per
-        # pass the kernels are launch/latency bound and each pass alone leaves most of the 132 SMs idle.
-        self.overlap_passes = bool(overlap_passes) and (graph_loss or fused_det_loss)
-        self._s_seg = torch.cuda.Stream() if self.overlap_passes else None
-        self.concurrent_forwards = (concurrent_forwards is None or bool(concurrent_forwards)) and self.overlap_passes
+        self._s_seg = torch.cuda.Stream() if self.fused_seg else None          # the seg pass of _passes_concurrent
         self._ev_detfwd, self._ev_start, self._ev_seg = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
         self.multi_scale = multi_scale
         self.det_shapes = None if det_shapes is None else sorted({(int(h), int(w)) for h, w in det_shapes})
@@ -443,20 +436,15 @@ class Trainer:
         return st
 
     def backward_det(self, imgs, targets):
-        if self.fused_det_loss:
-            eng = self.model.engine()
+        eng = self.model.engine()
+        if self._fused_det.supported:
             raws, _, plan = eng.train_forward(imgs, want_seg=False)
             self._ev_detfwd.record(torch.cuda.current_stream())
             mult = (self.world_size if self.rank != -1 else 1) * self.detgain              # train.py:367-368 and :290
             grads, items = self._fused_det(raws, targets, mult=mult, scale=self.scale)
             eng.train_backward(plan, grads, None)
             return items
-        if not self.graph_loss:
-            pred = self.model(imgs)                                               # train mode: [[x0,x1,x2], seg]
-            loss, items = self._det_loss_scaled(pred[0], targets)
-            loss.backward()
-            return items
-        eng = self.model.engine()
+        # the torch formulation: forward + autograd backward (~700 tiny kernels) replayed as ONE CUDA graph
         B, _, H, W = imgs.shape
         det = self.model.model[-1]
         shapes = [(B, det.na, H // int(s), W // int(s), det.no) for s in det.stride.tolist()]
@@ -472,13 +460,14 @@ class Trainer:
         eng.train_backward(plan, [q.grad for q in st.p], None)
         return st.items.clone()                                                   # the static tensor is overwritten by the next replay
 
-    def backward_seg(self, segimgs, segtargets, lane=0):
-        # the fused kernels are instantiated for 19 (Cityscapes) and 32 classes; any other n_segcls takes the autograd path below
-        if self.fused_seg_loss and self.n_seg_outputs == 1 and self.model.model[-2].c_out in (19, 32):
-            eng = self.model.engine()
-            _, _, plan = eng.train_forward(segimgs, want_seg=False, lane=lane)
-            loss = eng.train_backward_seg_ce(plan, segtargets, factor=self.batch_size * self.seggain, scale=self.scale)
-            return loss * (self.batch_size * self.seggain)
+    def _seg_ce_backward(self, plan, segtargets):
+        f = self.batch_size * self.seggain                                                   # train.py:385-391
+        return self.model.engine().train_backward_seg_ce(plan, segtargets, factor=f, scale=self.scale) * f
+
+    def backward_seg(self, segimgs, segtargets):
+        if self.fused_seg:
+            _, _, plan = self.model.engine().train_forward(segimgs, want_seg=False)
+            return self._seg_ce_backward(plan, segtargets)
         pred = self.model(segimgs)
         outs = pred[1] if isinstance(pred[1], list) else [pred[1]]
         segloss = self.compute_seg_loss(*outs, segtargets) * self.batch_size * self.seggain   # train.py:385-391
@@ -515,46 +504,43 @@ class Trainer:
         grow = tracker >= self.growth_interval
         self.scale.copy_(torch.where(bad, self.scale * 0.5, torch.where(grow, self.scale * 2.0, self.scale)))   # in place: graphs read it
         self.growth_tracker.copy_(torch.where(grow, torch.zeros_like(tracker), tracker))
-        self.model.engine().weights_dirty = True
+        self.model.invalidate_weights()            # the step wrote the parameters through raw pointers
         if self.ema is not None:
             self.ema.update(self.model)            # train.py:401: every step, a skipped one too (reads parameters and BN buffers)
+
+    def _passes_sequential(self, imgs, targets, segimgs, segtargets):
+        return self.backward_det(imgs, targets), self.backward_seg(segimgs, segtargets)
+
+    def _passes_concurrent(self, imgs, targets, segimgs, segtargets):
+        """the seg pass on its own train plan (lane 1) and stream.  At 4 images per pass every kernel is small and each pass alone is a
+        latency-bound chain that leaves most of the 132 SMs idle, so both forwards start together.  The seg plan defers its BatchNorm
+        running statistics and applies them after the det forward, i.e. in the reference's order (train.py:364 det batch, :385 seg batch);
+        the two backwards overlap too, their parameter gradients add up atomically in the one flat buffer."""
+        eng = self.model.engine()
+        main = torch.cuda.current_stream()
+        self._ev_start.record(main)
+        with torch.cuda.stream(self._s_seg):
+            self._s_seg.wait_event(self._ev_start)
+            B, _, H, W = segimgs.shape
+            plan = eng.train_plan_for(B, H, W, lane=1)
+            eng.set_defer_running(plan)
+            eng.train_forward(segimgs, want_seg=False, lane=1)
+        items = self.backward_det(imgs, targets)                 # records _ev_detfwd right after the det forward
+        with torch.cuda.stream(self._s_seg):
+            self._s_seg.wait_event(self._ev_detfwd)
+            eng.apply_running(plan)
+            segloss = self._seg_ce_backward(plan, segtargets)
+            self._ev_seg.record(self._s_seg)
+        main.wait_event(self._ev_seg)
+        segimgs.record_stream(self._s_seg); segtargets.record_stream(self._s_seg)
+        return items, segloss
 
     def step(self, imgs, targets, segimgs, segtargets):
         """one iteration (train.py:363-401).  Returns (det loss items [lbox,lobj,lcls,loss], seg loss) as device tensors."""
         if self._ms_batches and imgs.shape[0] not in self._ms_batches:
             self._reserve_det(int(imgs.shape[0]))               # host plans only: the shared workspace is already there
-        fused_seg = self.fused_seg_loss and self.n_seg_outputs == 1 and self.model.model[-2].c_out in (19, 32)
-        if self.overlap_passes and fused_seg:
-            main = torch.cuda.current_stream()
-            self._ev_start.record(main)
-            # the seg pass runs on its own train plan and stream.  Its forward starts with the det forward (both are chains of small
-            # launches at 4 images: two chains fill the machine better than one); its BatchNorm running statistics are deferred and
-            # applied after the det forward, i.e. in the reference's order (train.py:364 det batch, :385 seg batch)
-            with torch.cuda.stream(self._s_seg):
-                self._s_seg.wait_event(self._ev_start)
-                eng = self.model.engine()
-                B, _, H, W = segimgs.shape
-                eng.ensure_flat_grads()
-                plan = eng.train_plan_for(B, H, W, lane=1)
-                eng.set_defer_running(plan, self.concurrent_forwards)
-                eng.prepare_train_plan(plan)
-                if self.concurrent_forwards:
-                    eng.train_forward(segimgs, want_seg=False, lane=1)
-            items = self.backward_det(imgs, targets)                 # records _ev_detfwd right after the det forward
-            with torch.cuda.stream(self._s_seg):
-                self._s_seg.wait_event(self._ev_detfwd)
-                if self.concurrent_forwards:
-                    eng.apply_running(plan)
-                    segloss = eng.train_backward_seg_ce(plan, segtargets, factor=self.batch_size * self.seggain, scale=self.scale)
-                    segloss = segloss * (self.batch_size * self.seggain)
-                else:                                                # forward after the det forward, overlapping the det backward
-                    segloss = self.backward_seg(segimgs, segtargets, lane=1)
-                self._ev_seg.record(self._s_seg)
-            main.wait_event(self._ev_seg)
-            segimgs.record_stream(self._s_seg); segtargets.record_stream(self._s_seg)
-        else:
-            items = self.backward_det(imgs, targets)
-            segloss = self.backward_seg(segimgs, segtargets)
+        passes = self._passes_concurrent if self.fused_seg else self._passes_sequential     # autograd's seg pass runs Model.forward: lane 0
+        items, segloss = passes(imgs, targets, segimgs, segtargets)
         self.ni += 1
         if self.ni % self.accumulate == 0:
             self.optimizer_step()

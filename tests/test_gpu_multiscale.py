@@ -1,7 +1,7 @@
 """GPU: --multi-scale training (reference train.py:354-359).  The rescale kernel against torch's F.interpolate on the same card, bit for
 bit; train steps through the det lane's shared workspace against the same steps through private plans (bar: the private plans' own
 run-to-run spread over several runs, the idea of
-test_gpu_train.py::test_concurrent_forwards_keep_the_reference_order_of_running_statistics); the stale-backward and capacity checks; and a 40-step multi-scale run at imgsz 1024 fed by the device batch builders."""
+test_gpu_train.py::test_concurrent_passes_keep_the_reference_order_of_running_statistics); the stale-backward and capacity checks; and a 40-step multi-scale run at imgsz 1024 fed by the device batch builders."""
 import ctypes as C
 import random
 

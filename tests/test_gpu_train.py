@@ -264,15 +264,16 @@ def test_conv_wgrad_kernels_match_torch(shape, path):
     assert err < 2e-3, err
 
 
-def test_graphed_det_loss_equals_eager_path():
-    """Trainer(graph_loss=True) replays ComputeLoss forward+backward as one CUDA graph on static buffers, targets zero-padded to a
-    multiple of 64 rows.  On identical head outputs the replayed graph must give the eager loss items and d loss / d head outputs
-    (same torch kernels: 1e-6), for several target counts incl. none; and the det pass must leave the seg head untouched."""
+def test_graphed_det_loss_equals_eager_path_and_runs_for_unfused_hyps():
+    """Where the fused detection loss does not cover the hyp, the Trainer replays ComputeLoss forward+backward as one CUDA graph on static
+    buffers, targets zero-padded to a multiple of 64 rows.  On identical head outputs the replayed graph must give the eager loss items and
+    d loss / d head outputs (same torch kernels: 1e-6), for several target counts incl. none; and the det pass must leave the seg head
+    untouched."""
     from multiyolov5_b200.train import Trainer, scale_hyp
     model, cfg, sd, _ = setup(B=2, H=128, W=256)
-    hyp = dict(lr0=0.01, momentum=0.937, weight_decay=5e-4, box=0.05, cls=0.5, cls_pw=1.0, obj=1.0, obj_pw=1.0, anchor_t=4.0, fl_gamma=0.0)
-    hyp = scale_hyp(hyp, nl=3, nc=cfg["nc"], imgsz=256, total_batch_size=4)
-    tr = Trainer(model, hyp, batch_size=2, init_scale=64.0, graph_loss=True)
+    hyp0 = dict(lr0=0.01, momentum=0.937, weight_decay=5e-4, box=0.05, cls=0.5, cls_pw=1.0, obj=1.0, obj_pw=1.0, anchor_t=4.0, fl_gamma=0.0)
+    hyp = scale_hyp(hyp0, nl=3, nc=cfg["nc"], imgsz=256, total_batch_size=4)
+    tr = Trainer(model, hyp, batch_size=2, init_scale=64.0)
     shapes = [(2, 3, 16, 32, 15), (2, 3, 8, 16, 15), (2, 3, 4, 8, 15)]
     st = tr._det_graph(shapes, 64, torch.device("cuda"))
     rs = np.random.RandomState(0)
@@ -298,7 +299,12 @@ def test_graphed_det_loss_equals_eager_path():
         assert torch.allclose(st.items, items, rtol=1e-6, atol=1e-7), (nt, st.items, items)
         for q, e in zip(st.p, pe):
             assert rel_f(q.grad.cpu(), e.grad.cpu()) < 1e-6, nt
-    # end to end through the network: second call replays the captured graphs (network and loss)
+    # end to end through the network with the positive weights of the reference's data/hyp.finetune.yaml, which the fused loss does not
+    # cover: backward_det replays the captured loss graph; the second call replays the captured graphs (network and loss)
+    model, _, _, _ = setup(B=2, H=128, W=256)
+    hyp = scale_hyp(dict(hyp0, cls_pw=0.631, obj_pw=0.911), nl=3, nc=cfg["nc"], imgsz=256, total_batch_size=4)
+    tr = Trainer(model, hyp, batch_size=2, init_scale=64.0)
+    assert not tr._fused_det.supported
     imgs = synth.synth_image(2, 128, 256, seed=1).cuda()
     for _ in range(2):
         model.zero_grad(set_to_none=False)
@@ -400,6 +406,52 @@ def test_eval_after_train_forward_uses_updated_running_statistics():
     assert torch.equal(z1, z2)                                      # ... and the cached inference plan saw them
 
 
+def test_weight_packs_upload_when_their_parameters_change(monkeypatch):
+    """a plan re-packs its fp16 weights exactly when what they were made from changed: the train plans of both passes at their first use
+    and after each optimizer step (accumulate=2: not in between, the running statistics moving does not touch a train pack); an inference
+    plan once after the train steps and not again for a second forward; the EMA's plan after ModelEMA.update."""
+    from multiyolov5_b200.engine import CompiledPlan
+    from multiyolov5_b200.train import Trainer, scale_hyp
+    from multiyolov5_b200.utils.torch_utils import ModelEMA
+    counts = {}
+    upload = CompiledPlan.upload_weights
+
+    def counted(plan):
+        counts[plan] = counts.get(plan, 0) + 1
+        return upload(plan)
+    monkeypatch.setattr(CompiledPlan, "upload_weights", counted)
+    B = 2
+    model, cfg, sd, x = setup(B=B, H=128, W=256)
+    hyp = dict(lr0=0.01, momentum=0.937, weight_decay=5e-4, box=0.05, cls=0.5, cls_pw=1.0, obj=1.0, obj_pw=1.0, anchor_t=4.0, fl_gamma=0.0)
+    tr = Trainer(model, scale_hyp(hyp, nl=3, nc=cfg["nc"], imgsz=256, total_batch_size=4), batch_size=B, accumulate=2, init_scale=2.0 ** 10)
+    rs = np.random.RandomState(0)
+    imgs, segimgs = synth.synth_image(B, 128, 256, seed=1).cuda(), synth.synth_image(B, 128, 256, seed=2).cuda()
+    t = np.zeros((6, 6), np.float32)
+    t[:, 0] = rs.randint(0, B, 6); t[:, 1] = rs.randint(0, cfg["nc"], 6)
+    t[:, 2:4] = rs.uniform(0.1, 0.9, (6, 2)); t[:, 4:6] = rs.uniform(0.05, 0.4, (6, 2))
+    targets = torch.from_numpy(t).cuda()
+    mask = torch.from_numpy(rs.randint(-1, 19, (B, 128, 256)).astype(np.int64)).cuda()
+    eng = model.engine()
+    history = []
+    for _ in range(4):                                   # optimizer steps after the second and the fourth
+        tr.step(imgs, targets, segimgs, mask)
+        history.append((counts.get(eng.plans[("train", B, 128, 256)]), counts.get(eng.plans[("train", B, 128, 256, 1)])))
+    assert history == [(1, 1), (1, 1), (2, 2), (2, 2)], history
+    model.eval()
+    model(x.cuda())
+    model(x.cuda())
+    assert counts[eng.plans[(B, 128, 256)]] == 1 and len(counts) == 3
+    ema = ModelEMA(model)
+    ema.ema(x.cuda())
+    ema.ema(x.cuda())
+    ema.update(model)
+    ema.ema(x.cuda())
+    torch.cuda.synchronize()
+    print(f"\nuploads: train plans (det, seg) after each step {history}, per plan {sorted(counts.values())}")
+    assert counts[ema.ema.engine().plans[(B, 128, 256)]] == 2
+    assert sum(counts.values()) == 2 + 2 + 1 + 2, counts
+
+
 @pytest.mark.parametrize("name", ["a", "empty", "edge"])
 def test_fused_det_loss_matches_reference_fixture(name):
     """`myolo_det_loss` (csrc/detloss.cu: target assignment, CIoU / BCE losses and THEIR GRADIENTS in four launches) against the fixtures written
@@ -491,10 +543,10 @@ def test_grouped_weight_repack_equals_per_slot_packs(monkeypatch):
     assert diff_g <= max(3 * noise_g, 5e-3), (diff_g, noise_g)
 
 
-def test_concurrent_forwards_keep_the_reference_order_of_running_statistics():
-    """Trainer(concurrent_forwards=True) runs the seg forward next to the det forward; the seg plan defers its BatchNorm running-statistics
-    update and applies it after the det forward.  running_mean / running_var / num_batches_tracked and the stepped parameters must equal
-    the strictly sequential schedule's (reference train.py:364-398: det forward+backward, seg forward+backward, optimizer.step)."""
+def test_concurrent_passes_keep_the_reference_order_of_running_statistics():
+    """Trainer.step runs the seg forward next to the det forward; the seg plan defers its BatchNorm running-statistics update and applies
+    it after the det forward.  running_mean / running_var / num_batches_tracked and the stepped parameters must equal the strictly
+    sequential schedule's (reference train.py:364-398: det forward+backward, seg forward+backward, optimizer.step)."""
     from multiyolov5_b200.train import Trainer, scale_hyp
     B = 2
     rs = np.random.RandomState(0)
@@ -506,17 +558,25 @@ def test_concurrent_forwards_keep_the_reference_order_of_running_statistics():
     targets = torch.from_numpy(t).cuda()
     mask = torch.from_numpy(rs.randint(-1, 19, (B, 128, 256)).astype(np.int64)).cuda()
 
-    def run(**kw):
+    def run(concurrent):
         model, cfg, sd, _ = setup(B=B, H=128, W=256)
         hyp = dict(lr0=0.01, momentum=0.937, weight_decay=5e-4, box=0.05, cls=0.5, cls_pw=1.0, obj=1.0, obj_pw=1.0, anchor_t=4.0, fl_gamma=0.0)
         hyp = scale_hyp(hyp, nl=3, nc=cfg["nc"], imgsz=256, total_batch_size=4)
-        tr = Trainer(model, hyp, batch_size=B, init_scale=2.0 ** 10, **kw)
-        items, segloss = tr.step(imgs, targets, segimgs, mask)
+        tr = Trainer(model, hyp, batch_size=B, init_scale=2.0 ** 10)
+        assert tr.fused_seg
+
+        def step():
+            if concurrent:
+                return tr.step(imgs, targets, segimgs, mask)
+            out = tr._passes_sequential(imgs, targets, segimgs, mask)
+            tr.optimizer_step()
+            return out
+        items, segloss = step()
         torch.cuda.synchronize()
         first = ({k: v.detach().float().cpu().clone() for k, v in model.state_dict().items() if "running_" in k or "num_batches" in k},
                  [float(v) for v in items])
         for _ in range(2):                                   # the schedule keeps working step after step
-            items, segloss = tr.step(imgs, targets, segimgs, mask)
+            items, segloss = step()
         torch.cuda.synchronize()
         nbt = [int(v) for k, v in model.state_dict().items() if k.endswith("num_batches_tracked")]
         assert all(np.isfinite(float(v)) for v in items) and np.isfinite(float(segloss))
@@ -524,9 +584,9 @@ def test_concurrent_forwards_keep_the_reference_order_of_running_statistics():
 
     # compared after ONE step: from the second step on the two schedules legitimately differ (the seg pass draws its dropout masks from its
     # own plan's counter in the concurrent schedule), the first step's forward statistics do not depend on any mask
-    (sa, la), na = run(concurrent_forwards=True)
-    (sb, lb), nb = run(overlap_passes=False)
-    (sc, lc), _ = run(overlap_passes=False)                  # run-to-run spread of the sequential schedule (fp32 atomics in the batch sums)
+    (sa, la), na = run(concurrent=True)
+    (sb, lb), nb = run(concurrent=False)
+    (sc, lc), _ = run(concurrent=False)                      # run-to-run spread of the sequential schedule (fp32 atomics in the batch sums)
     assert set(na) == set(nb) == {6}, (set(na), set(nb))     # 3 steps x (det batch + seg batch)
 
     def spread(x, y):

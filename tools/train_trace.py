@@ -1,14 +1,12 @@
 """CUPTI timeline of ONE training step (tools/bench_train.make_workload): wall, busy time per stream, union coverage, kernels ranked by total
-device time.  Usage: python tools/train_trace.py [--no-overlap] [--out DIR]   (full per-kernel listing: DIR/train_trace_full.txt,
-default a temporary directory)"""
+device time.  Usage: python tools/train_trace.py [--out DIR]   (full per-kernel listing: DIR/train_trace_full.txt, default a temporary
+directory)"""
 import collections, json, os, sys, tempfile
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from tools.bench_train import make_workload
 wl = make_workload(1, 0, 4)
 tr, NROT = wl["tr"], wl["NROT"]
-if "--no-overlap" in sys.argv:
-    tr.overlap_passes = False
 def step(i):
     k = i % NROT
     return tr.step(wl["imgs"][k], wl["tg"][k], wl["segimgs"][k], wl["masks"][k])
