@@ -301,6 +301,16 @@ int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int 
  * to the batch shape, random_perspective at (W, H), flips over H and W), out (B,3,H,W).  myolo_augment_det is its H = W = S case. */
 int myolo_augment_det_hw(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, void* stream);
 
+/* myolo_collate_quad: the pixels of `--quad`'s LoadImagesAndLabels.collate_fn4 (reference utils/datasets.py:602-625) over one drawn batch,
+ * one launch on `stream`, no synchronisation.  imgs: DEVICE uint8 (B,3,H,W) RGB, B >= 4; tile: HOST array of B/4 flags,
+ * one per quad in order (the caller's `random.random() >= 0.5`), at most MYOLO_QUAD_MAX; they travel as kernel parameters.  Quad q of
+ * out (B/4,3,2H,2W) is the 2x2 tile of items 4q (top left), 4q+1 (bottom left), 4q+2 (top right), 4q+3 (bottom right)
+ * when tile[q], else F.interpolate(item 4q, scale_factor=2., mode='bilinear', align_corners=False) truncated to uint8, in integer
+ * arithmetic that equals torch's bit for bit.  Items past 4 * (B/4) are not read.  out_dtype MYOLO_U8 / MYOLO_F16 / MYOLO_F32 (float =
+ * value / 255, as imgs.float() / 255 on the GPU).  W % 8 == 0 with imgs 8-byte and out 16-byte aligned takes 8 pixels per thread. */
+#define MYOLO_QUAD_MAX 1024
+int myolo_collate_quad(const uint8_t* imgs, int B, int H, int W, const uint8_t* tile, void* out, int out_dtype, void* stream);
+
 /* ---- segmentation training batches (reference SegmentationDataset.py:118-151 `_sync_transform` + ColorJitter + ToTensor, and the
  * testval items of :81-94) ----
  * myolo_augment_seg: B items in two launches on `stream`.  Per item: Pillow's bilinear Image.resize of the source (mirrored when `flip`)

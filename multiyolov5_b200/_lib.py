@@ -37,7 +37,7 @@ EXPORTS = [
     "myolo_grads_check_finite", "myolo_sgd_step", "myolo_conv_wgrad", "myolo_letterbox", "myolo_seg_lut_blend", "myolo_seg_metrics", "myolo_plan_backward_seg_ce", "myolo_plan_read_grad_view", "myolo_plan_set_seed", "myolo_plan_train_forward_multi", "myolo_plan_backward_multi", "myolo_plan_conv_info", "myolo_allreduce_grads", "myolo_det_loss", "myolo_det_loss_workspace_bytes", "myolo_plan_set_defer_running", "myolo_plan_apply_running",
     "myolo_resize_u8", "myolo_augment_det", "myolo_augment_seg", "myolo_det_match", "myolo_det_ap", "myolo_det_ap_workspace_bytes",
     "myolo_resize_area_u8", "myolo_resize_bilinear", "myolo_plan_create_shared", "myolo_augment_det_hw", "myolo_adam_step",
-    "myolo_adam_scalars", "myolo_ema_update", "myolo_plan_set_extra",
+    "myolo_adam_scalars", "myolo_ema_update", "myolo_plan_set_extra", "myolo_collate_quad",
 ]
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
 
@@ -124,6 +124,7 @@ def lib():
     L.myolo_resize_bilinear.argtypes = [vp, i32, i32, i32, i32, i32, vp, i32, i32, i32, vp]
     L.myolo_augment_det.argtypes = [vp, i32, i32, vp, i32, vp]
     L.myolo_augment_det_hw.argtypes = [vp, i32, i32, i32, vp, i32, vp]
+    L.myolo_collate_quad.argtypes = [vp, i32, i32, i32, vp, vp, i32, vp]
     L.myolo_augment_seg.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp]
     L.myolo_seg_lut_blend.argtypes = [vp, i32, i64, vp, i32, i32, i32, vp, vp, f32, f32, vp, vp]
     L.myolo_seg_metrics.argtypes = [vp, i32, vp, i64, i32, vp, vp]

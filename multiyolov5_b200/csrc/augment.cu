@@ -244,4 +244,143 @@ int launch_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, 
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------------
+// --quad (reference utils/datasets.py:602-625 LoadImagesAndLabels.collate_fn4): quad q of the output is either the 2x2 tile of items
+// 4q (top left), 4q+1 (bottom left), 4q+2 (top right), 4q+3 (bottom right), or
+//   F.interpolate(img[4q].float()[None], scale_factor=2., mode='bilinear', align_corners=False)[0].type(uint8)
+// computed in integers.  With scale 1/2 the source coordinate of output row Y is Y/2 - 1/4 clamped at 0, so an even row 2r takes rows
+// (r-1, r) with weights (1/4, 3/4) and an odd row 2r+1 rows (r, r+1) with (3/4, 1/4); row 0 and a last odd row take one row with weight 1,
+// which is the same sum with the missing row clamped to its neighbour.  Columns likewise.  Every partial result torch forms is a multiple
+// of 1/16 in [0, 256) and so exact in fp32, whatever its order of evaluation (tests/test_quad_host.py proves it), and the truncating
+// uint8 cast is floor(sum / 16) of the integer sum with weights {1, 3} x {1, 3}.
+// ------------------------------------------------------------------------------------------------
+struct QuadFlags {                   // a __grid_constant__ parameter: indexed in place, not copied to local memory
+  unsigned w[MYOLO_QUAD_MAX / 32];   // bit q: quad q is the 2x2 tile, else the x2 upsample of its first item
+};
+
+__device__ __forceinline__ bool quad_is_tile(const QuadFlags& f, int q) { return (f.w[q >> 5] >> (q & 31)) & 1u; }
+
+// the float outputs are imgs.float() / 255 on the device (reference train.py:342), as augment_det_kernel writes them
+__device__ __forceinline__ float quad_unit(int v) { return __fmul_rn((float)v, 1.0f / 255.0f); }
+
+// 8 consecutive output pixels [X0, X0 + 8) of row Y in one (quad, channel) plane; W % 8 == 0, so X0 is 8-aligned, a tile never straddles
+// an 8-pixel group, and every load and store below is naturally aligned
+template <int OUT>
+__global__ void __launch_bounds__(256) collate_quad_vec_kernel(const unsigned char* __restrict__ imgs, int H, int W,
+                                                               const __grid_constant__ QuadFlags flags, void* __restrict__ out) {
+  const int Wo = 2 * W, Ho = 2 * H, groups = Wo >> 3;
+  const long gid = blockIdx.x * (long)blockDim.x + threadIdx.x;
+  if (gid >= (long)Ho * groups) return;
+  const int plane = blockIdx.y, q = plane / 3, c = plane - 3 * q;
+  const int Y = (int)(gid / groups), X0 = (int)(gid - (long)Y * groups) << 3;
+  const size_t HW = (size_t)H * W;
+  int v[8];
+  if (quad_is_tile(flags, q)) {
+    const int item = 4 * q + (Y >= H ? 1 : 0) + (X0 >= W ? 2 : 0);     // cat over H (i, i+1) then over W ((i, i+1), (i+2, i+3))
+    const int y = Y >= H ? Y - H : Y, x = X0 >= W ? X0 - W : X0;
+    const uint2 p = __ldg(reinterpret_cast<const uint2*>(imgs + ((size_t)item * 3 + c) * HW + (size_t)y * W + x));
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      v[j] = (p.x >> (8 * j)) & 255u;
+      v[4 + j] = (p.y >> (8 * j)) & 255u;
+    }
+  } else {
+    const unsigned char* src = imgs + ((size_t)(4 * q) * 3 + c) * HW;
+    const int r = Y >> 1;
+    const int ya = (Y & 1) ? r : max(r - 1, 0), yb = (Y & 1) ? min(r + 1, H - 1) : r;   // weights (3, 1) for odd rows, (1, 3) for even
+    const int wa = (Y & 1) ? 3 : 1, wb = 4 - wa;
+    const int k = X0 >> 1;                                                               // source columns k-1 .. k+4, clamped
+    int h[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) h[j] = 0;
+#pragma unroll
+    for (int t = 0; t < 2; ++t) {
+      const unsigned char* row = src + (size_t)(t ? yb : ya) * W;
+      const int wy = t ? wb : wa;
+      const unsigned mid = __ldg(reinterpret_cast<const unsigned*>(row + k));
+      int a[6];
+      a[0] = __ldg(row + max(k - 1, 0));
+#pragma unroll
+      for (int j = 0; j < 4; ++j) a[1 + j] = (mid >> (8 * j)) & 255u;
+      a[5] = __ldg(row + min(k + 4, W - 1));
+#pragma unroll
+      for (int m = 0; m < 4; ++m) {                       // output columns 2(k+m) and 2(k+m)+1
+        h[2 * m] += wy * (a[m] + 3 * a[m + 1]);
+        h[2 * m + 1] += wy * (3 * a[m + 1] + a[m + 2]);
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = h[j] >> 4;
+  }
+  const size_t o = ((size_t)plane * Ho + Y) * Wo + X0;
+  if (OUT == MYOLO_U8) {
+    uint2 p;
+    p.x = v[0] | (v[1] << 8) | (v[2] << 16) | ((unsigned)v[3] << 24);
+    p.y = v[4] | (v[5] << 8) | (v[6] << 16) | ((unsigned)v[7] << 24);
+    *reinterpret_cast<uint2*>(reinterpret_cast<unsigned char*>(out) + o) = p;
+  } else if (OUT == MYOLO_F16) {
+    __align__(16) __half hv[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) hv[j] = __float2half_rn(quad_unit(v[j]));
+    *reinterpret_cast<uint4*>(reinterpret_cast<__half*>(out) + o) = *reinterpret_cast<const uint4*>(hv);
+  } else {
+    float4* d = reinterpret_cast<float4*>(reinterpret_cast<float*>(out) + o);
+    d[0] = make_float4(quad_unit(v[0]), quad_unit(v[1]), quad_unit(v[2]), quad_unit(v[3]));
+    d[1] = make_float4(quad_unit(v[4]), quad_unit(v[5]), quad_unit(v[6]), quad_unit(v[7]));
+  }
+}
+
+// any W or alignment: one output pixel per thread, the same arithmetic with byte loads
+__global__ void __launch_bounds__(256) collate_quad_kernel(const unsigned char* __restrict__ imgs, int H, int W,
+                                                           const __grid_constant__ QuadFlags flags, void* __restrict__ out, int out_dtype) {
+  const int Wo = 2 * W, Ho = 2 * H;
+  const long gid = blockIdx.x * (long)blockDim.x + threadIdx.x;
+  if (gid >= (long)Ho * Wo) return;
+  const int plane = blockIdx.y, q = plane / 3, c = plane - 3 * q;
+  const int Y = (int)(gid / Wo), X = (int)(gid - (long)Y * Wo);
+  const size_t HW = (size_t)H * W;
+  int v;
+  if (quad_is_tile(flags, q)) {
+    const int item = 4 * q + (Y >= H ? 1 : 0) + (X >= W ? 2 : 0);
+    v = __ldg(imgs + ((size_t)item * 3 + c) * HW + (size_t)(Y >= H ? Y - H : Y) * W + (X >= W ? X - W : X));
+  } else {
+    const unsigned char* src = imgs + ((size_t)(4 * q) * 3 + c) * HW;
+    const int r = Y >> 1, k = X >> 1;
+    const int ya = (Y & 1) ? r : max(r - 1, 0), yb = (Y & 1) ? min(r + 1, H - 1) : r, wya = (Y & 1) ? 3 : 1;
+    const int xa = (X & 1) ? k : max(k - 1, 0), xb = (X & 1) ? min(k + 1, W - 1) : k, wxa = (X & 1) ? 3 : 1;
+    const unsigned char* ra = src + (size_t)ya * W;
+    const unsigned char* rb = src + (size_t)yb * W;
+    const int top = wxa * __ldg(ra + xa) + (4 - wxa) * __ldg(ra + xb);
+    const int bot = wxa * __ldg(rb + xa) + (4 - wxa) * __ldg(rb + xb);
+    v = (wya * top + (4 - wya) * bot) >> 4;
+  }
+  const size_t o = ((size_t)plane * Ho + Y) * Wo + X;
+  if (out_dtype == MYOLO_U8) reinterpret_cast<unsigned char*>(out)[o] = (unsigned char)v;
+  else if (out_dtype == MYOLO_F16) reinterpret_cast<__half*>(out)[o] = __float2half_rn(quad_unit(v));
+  else reinterpret_cast<float*>(out)[o] = quad_unit(v);
+}
+
+int launch_collate_quad(const unsigned char* imgs, int B, int H, int W, const unsigned char* tile, void* out, int out_dtype, cudaStream_t s) {
+  MYOLO_REQUIRE(imgs && out && tile && B >= 4 && H > 0 && W > 0, "collate_quad: bad arguments (B %d H %d W %d)", B, H, W);
+  MYOLO_REQUIRE(B / 4 <= MYOLO_QUAD_MAX, "collate_quad: %d quads, at most %d", B / 4, MYOLO_QUAD_MAX);
+  MYOLO_REQUIRE((long)H * W <= (1L << 28), "collate_quad: %dx%d images are too large", H, W);
+  MYOLO_REQUIRE(out_dtype == MYOLO_U8 || out_dtype == MYOLO_F16 || out_dtype == MYOLO_F32, "collate_quad: output dtype %d", out_dtype);
+  const int n = B / 4;
+  QuadFlags f = {};
+  for (int q = 0; q < n; ++q)
+    if (tile[q]) f.w[q >> 5] |= 1u << (q & 31);
+  const long Ho = 2L * H, Wo = 2L * W;
+  if (W % 8 == 0 && ((uintptr_t)imgs & 7) == 0 && ((uintptr_t)out & 15) == 0) {
+    const dim3 grid((unsigned)((Ho * (Wo / 8) + 255) / 256), 3 * n);
+    if (out_dtype == MYOLO_U8) collate_quad_vec_kernel<MYOLO_U8><<<grid, 256, 0, s>>>(imgs, H, W, f, out);
+    else if (out_dtype == MYOLO_F16) collate_quad_vec_kernel<MYOLO_F16><<<grid, 256, 0, s>>>(imgs, H, W, f, out);
+    else collate_quad_vec_kernel<MYOLO_F32><<<grid, 256, 0, s>>>(imgs, H, W, f, out);
+  } else {
+    const dim3 grid((unsigned)((Ho * Wo + 255) / 256), 3 * n);
+    collate_quad_kernel<<<grid, 256, 0, s>>>(imgs, H, W, f, out, out_dtype);
+  }
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace myolo

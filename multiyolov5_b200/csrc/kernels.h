@@ -37,6 +37,7 @@ int launch_resize_u8(const unsigned char* src, int H0, int W0, unsigned char* ds
 int launch_resize_area_u8(const unsigned char* src, int H0, int W0, unsigned char* dst, int H, int W, cudaStream_t s);
 int launch_augment_det(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, cudaStream_t s);
 int launch_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo, cudaStream_t s);
+int launch_collate_quad(const unsigned char* imgs, int B, int H, int W, const unsigned char* tile, void* out, int out_dtype, cudaStream_t s);
 
 // segmentation training batches (augment_seg.cu): crop-window resample + pad + mask LUT, then the ColorJitter / ToTensor kernel
 int launch_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int mw, const int* tables, unsigned char* scratch, void* out,

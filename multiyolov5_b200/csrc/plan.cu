@@ -1215,6 +1215,12 @@ extern "C" int myolo_resize_bilinear(const void* src, int src_dtype, int B, int 
   return launch_resize_bilinear(src, src_dtype, B, C, H, W, dst, dst_dtype, Ho, Wo, (cudaStream_t)stream);
 }
 
+extern "C" int myolo_collate_quad(const uint8_t* imgs, int B, int H, int W, const uint8_t* tile, void* out, int out_dtype, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_collate_quad(imgs, B, H, W, tile, out, out_dtype, (cudaStream_t)stream);
+}
+
 extern "C" int myolo_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int mw, const int32_t* tables, uint8_t* scratch,
                                  void* out_img, int out_dtype, int64_t* out_mask, void* stream) {
   int rc = check_device(nullptr);

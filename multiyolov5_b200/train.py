@@ -19,6 +19,9 @@ optimiser buffers to and from torch's `optimizer.state_dict()` format, which is 
 skipped for overflow: one launch (`myolo_ema_update`) over every floating-point entry of the model, bit-identical with the reference's
 per-entry statements.  Pass it on rank -1 / 0 and None elsewhere, as train.py:151 builds it.
 
+`Trainer(..., quad=True)` is the reference's `--quad`: det batches from `utils.datasets.collate_quad` (collate_fn4) and the det loss x 4
+(train.py:368-369).
+
 Out of scope (the reference's outer loop, not the hot path): data loading, LR schedule / warm-up (call `set_lr` / `set_momentum`),
 writing checkpoint files, plotting, DDP buffer broadcast.
 """
@@ -291,7 +294,7 @@ class Trainer:
     """`Trainer(model, hyp, batch_size).step(imgs, targets, segimgs, segtargets)`; hyp already scaled (see scale_hyp)."""
 
     def __init__(self, model, hyp, batch_size, world_size=1, rank=-1, accumulate=1, detgain=0.6, seggain=0.35, init_scale=2.0 ** 16,
-                 growth_interval=2000, process_group=None, multi_scale=None, det_shapes=None, optimizer="sgd", ema=None):
+                 growth_interval=2000, process_group=None, multi_scale=None, det_shapes=None, optimizer="sgd", ema=None, quad=False):
         """multi_scale: a MultiScale.  The det lane's train plans for every size it can draw from an imgsz x imgsz batch are reserved on
         one shared workspace (Engine.reserve_train_shapes); rescale each det batch with `multi_scale(imgs)` before `step`, as the reference
         does before its forward (train.py:354-359).  A det batch of fewer images (the loader's partial last batch) reserves its sizes on
@@ -302,13 +305,21 @@ class Trainer:
         torch.optim.Adam(betas=(hyp['momentum'], 0.999), eps=1e-8)), both over the reference's three groups.  Adam keeps its second
         moment in one more flat fp32 buffer: 4 bytes per parameter element (31 MB for s/PSP, 94 MB for m/Lab).
         ema: a utils.torch_utils.ModelEMA of this model (built before or after the Trainer), updated on the main stream right after every
-        optimizer step, when both passes have joined and the seg pass's deferred BatchNorm statistics are applied."""
+        optimizer step, when both passes have joined and the seg pass's deferred BatchNorm statistics are applied.
+        quad: the reference's --quad.  Det batches come from utils.datasets.collate_quad: batch_size // 4 images of twice the loader's
+        height and width, and the det loss is multiplied by 4 (train.py:368-369).  The reserved det plans (multi_scale / det_shapes) are
+        for batch_size // 4 images at the doubled shapes, with multi_scale every size it can draw from them.  The seg pass and its
+        batch_size factor are unchanged (train.py:385).  The reference's loop skips a det batch of one image (train.py:338), so with quad
+        a per-GPU batch_size below 8 never trains; the Trainer steps whatever it is given."""
         if optimizer not in OPTIMIZER_STATE:
             raise ValueError(f"optimizer must be 'sgd' or 'adam', got {optimizer!r}")
+        if quad and batch_size < 4:
+            raise ValueError(f"quad: a batch of {batch_size} images has no quad (collate_fn4 needs at least 4)")
         assert next(model.parameters()).is_cuda, "model.cuda() first"
         self.model, self.hyp, self.batch_size = model, hyp, batch_size
         self.world_size, self.rank, self.accumulate, self.pg = world_size, rank, accumulate, process_group
         self.detgain, self.seggain = detgain, seggain          # train.py:290
+        self.quad = bool(quad)
         model.hyp, model.gr = hyp, getattr(model, "gr", 1.0)
         model.train()
         # detection loss forward + backward as four launches of the library (csrc/detloss.cu) instead of ~760 torch kernels.  Focal loss /
@@ -345,12 +356,14 @@ class Trainer:
         self.det_shapes = None if det_shapes is None else sorted({(int(h), int(w)) for h, w in det_shapes})
         self._ms_batches = set()
         if multi_scale is not None or det_shapes is not None:
-            self._reserve_det(batch_size)
+            self._reserve_det(batch_size // 4 if self.quad else batch_size)
 
     def det_train_shapes(self):
         """every (H, W) the det lane's shared workspace holds plans for"""
         ms = self.multi_scale
         base = self.det_shapes if self.det_shapes is not None else [(ms.imgsz, ms.imgsz)]
+        if self.quad:
+            base = [(2 * h, 2 * w) for h, w in base]
         return base if ms is None else sorted({hw for shape in base for hw in ms.shapes(shape)})
 
     def _reserve_det(self, B):
@@ -398,14 +411,20 @@ class Trainer:
         loss, items = self.compute_loss(p, targets)
         if self.rank != -1:
             loss = loss * self.world_size                                         # train.py:367-368
+        if self.quad:
+            loss = loss * 4.                                                      # train.py:368-369
         return loss * self.detgain * self.scale, items
+
+    def det_mult(self):
+        """the fused det loss's multiplier: world_size under DDP, 4 with quad, detgain (train.py:367-370 and :290)"""
+        return (self.world_size if self.rank != -1 else 1) * (4. if self.quad else 1) * self.detgain
 
     def _det_graph(self, shapes, nt_pad, dev):
         """static inputs (head outputs, padded targets) -> static outputs (d loss / d head outputs, loss items), captured once per
         (grid shapes, padded target count).  Padding rows are all-zero targets: zero width/height never matches an anchor."""
         # every scalar the captured kernels bake in is part of the key: changing hyp / gains / gr / autobalance state re-captures
         cl = self.compute_loss
-        key = (tuple(shapes), nt_pad, self.detgain, self.world_size, self.rank, float(getattr(self.model, "gr", 1.0)),
+        key = (tuple(shapes), nt_pad, self.detgain, self.world_size, self.rank, self.quad, float(getattr(self.model, "gr", 1.0)),
                tuple(sorted((k, float(v)) for k, v in self.hyp.items() if isinstance(v, (int, float)))),
                tuple(float(b) for b in getattr(cl, "balance", ())), bool(getattr(cl, "autobalance", False)))
         st = self._det_graphs.get(key)
@@ -440,8 +459,7 @@ class Trainer:
         if self._fused_det.supported:
             raws, _, plan = eng.train_forward(imgs, want_seg=False)
             self._ev_detfwd.record(torch.cuda.current_stream())
-            mult = (self.world_size if self.rank != -1 else 1) * self.detgain              # train.py:367-368 and :290
-            grads, items = self._fused_det(raws, targets, mult=mult, scale=self.scale)
+            grads, items = self._fused_det(raws, targets, mult=self.det_mult(), scale=self.scale)
             eng.train_backward(plan, grads, None)
             return items
         # the torch formulation: forward + autograd backward (~700 tiny kernels) replayed as ONE CUDA graph

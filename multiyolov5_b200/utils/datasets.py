@@ -5,6 +5,7 @@
     DeviceImageCache(images, img_size, labels) / DetAugmenter(cache, hyp)(indices) -> (imgs, targets)   :518-599 (augment=True)
     DeviceImageCache(images, img_size, labels) / DetRectLoader(cache, hyp, batch_size)(positions) -> (imgs, targets), iterable
                                                                              :347-439 + :518-599 (augment=True, rect=True: --rect)
+    collate_quad(imgs, targets) -> (imgs4, targets4)                               :602-625 collate_fn4 (--quad) over either batch
     DeviceImageCache(images, img_size, labels, augment=False) / DetValLoader(cache, batch_size) -> iterable of (imgs, targets, paths,
         shapes) for test(data, model=m, dataloader=DetValLoader(cache, 32))                          :347-452 + :518-599 (rect=True)
     DeviceSegCache(images, masks, mask_map) / SegAugmenter(cache, base_size, crop_size, preset)(indices) -> (segimgs, segtargets)
@@ -161,7 +162,8 @@ class DetAugmenter:
     the reference (mosaic choice, mosaic centre and partners, random_perspective, mixup, HSV gains, flips), so a seeded run gives the
     reference's batch bit for bit.  Labels are transformed on the host with the reference's numpy formulas; the pixels (mosaic, affine
     warp, mixup, HSV, flips, BGR->RGB / CHW) are one kernel launch per batch on the current stream, without a device synchronisation.
-    Not built (raises): perspective != 0 (warpPerspective), label segments, the 9-image mosaic and the quad collate."""
+    `--quad` is a collate step over the drawn batch, as in the reference: pass this batch (uint8) to `collate_quad`.
+    Not built (raises): perspective != 0 (warpPerspective), label segments, the 9-image mosaic, and `quad=True` here."""
 
     def __init__(self, cache, hyp, stride=32, mosaic9=False, quad=False):
         if float(hyp.get("perspective", 0.0)) != 0.0:
@@ -169,7 +171,8 @@ class DetAugmenter:
         if mosaic9:
             raise NotImplementedError("DetAugmenter: load_mosaic9 (9-image mosaic) is not built")
         if quad:
-            raise NotImplementedError("DetAugmenter: the quad collate (collate_fn4) is not built")
+            raise NotImplementedError("DetAugmenter: quad is a collate step, not a dataset option: pass the uint8 batch to "
+                                      "utils.datasets.collate_quad (collate_fn4)")
         self.cache, self.hyp, self.stride = cache, dict(hyp), stride
         self.img_size, self.n = cache.img_size, cache.n
         self.indices = range(self.n)
@@ -538,6 +541,59 @@ class DetRectLoader:
 
     def __iter__(self):
         return self.batches()
+
+
+# ------------------------------------------------------------------------------------------------
+# quad training batches (reference train.py:197-199 create_dataloader(..., quad=opt.quad): LoadImagesAndLabels.collate_fn4, :602-625)
+# ------------------------------------------------------------------------------------------------
+_QUAD_HO = (0., 0, 0, 1, 0, 0)      # collate_fn4's ho, wo and s
+_QUAD_WO = (0., 0, 1, 0, 0, 0)
+_QUAD_S = (1, 1, .5, .5, .5, .5)
+
+
+def collate_quad(imgs, targets, rng=random, out_dtype=torch.uint8):
+    """`--quad`'s collate_fn4 over one drawn batch on the device: `imgs` uint8 (B, 3, h, w) and `targets` (n, 6) float32 [image, class,
+    x, y, w, h] as DetAugmenter(...)(indices), DetRectLoader(...)(positions) or its iterator give them, both on the GPU.  Returns (imgs4
+    (B // 4, 3, 2h, 2w) of out_dtype, targets4 (m, 6) float32) on the device; float outputs are uint8 / 255 as the training loop's
+    imgs.float() / 255.
+
+    One `rng.random()` per quad, in quad order, as the reference draws them after the whole batch: below 0.5 the quad is item 4q
+    bilinearly up-scaled x2 (F.interpolate(..., scale_factor=2.) truncated to uint8) with its labels unchanged, and items 4q+1 .. 4q+3 are
+    dropped; otherwise the 2x2 tile of the four items (4q top left, 4q+1 bottom left, 4q+2 top right, 4q+3 bottom right) with their labels
+    shifted and halved by the reference's float32 operations in its order.  Items past 4 * (B // 4) are dropped.  The pixels are one
+    myolo_collate_quad launch on the current stream; selecting the kept label rows synchronises with the device once, because their
+    number is known only there.  ValueError for fewer than 4 images, as collate_fn4's torch.stack([]) fails on them."""
+    if not (isinstance(imgs, torch.Tensor) and imgs.is_cuda and imgs.dtype == torch.uint8 and imgs.dim() == 4 and imgs.shape[1] == 3):
+        raise ValueError("collate_quad: imgs must be a CUDA uint8 (B, 3, h, w) tensor")
+    if not (isinstance(targets, torch.Tensor) and targets.is_cuda and targets.dtype == torch.float32 and targets.dim() == 2
+            and targets.shape[1] == 6):
+        raise ValueError("collate_quad: targets must be a CUDA float32 (n, 6) tensor")
+    if out_dtype not in (torch.uint8, torch.float16, torch.float32):
+        raise ValueError(f"collate_quad: out_dtype must be uint8, float16 or float32, got {out_dtype}")
+    B, _, h, w = imgs.shape
+    n = B // 4
+    if n == 0:
+        raise ValueError(f"collate_quad: a batch of {B} images has no quad (collate_fn4 needs at least 4)")
+    tile = [rng.random() >= 0.5 for _ in range(n)]
+    imgs = imgs.contiguous()
+    out = torch.empty((n, 3, 2 * h, 2 * w), dtype=out_dtype, device=imgs.device)
+    flags = (C.c_uint8 * n)(*tile)
+    _lib.check(_lib.lib().myolo_collate_quad(_lib.ptr(imgs), B, h, w, flags, _lib.ptr(out), _lib.torch_dtype_code(out_dtype),
+                                             _lib.stream_ptr()))
+    host = torch.tensor(_QUAD_HO + _QUAD_WO + _QUAD_S + tuple(float(v) for v in tile) + (0.0,), dtype=torch.float32).pin_memory()
+    dev = host.to(targets.device, non_blocking=True)             # one upload, no synchronisation
+    ho, wo, s, tile_q = dev[0:6], dev[6:12], dev[12:18], dev[18:] != 0
+    item = targets[:, 0].long()
+    q, k = item // 4, item % 4
+    t_row = tile_q[q.clamp(max=n)]                               # rows of items past the last quad index the False sentinel
+    keep = (q < n) & (t_row | (k == 0))
+    t, q, k, t_row = targets[keep], q[keep], k[keep], t_row[keep]
+    # label[i], label[i+1] + ho, label[i+2] + wo, label[i+3] + ho + wo, each then * s; the first item takes no addition
+    shifted = t + ho * ((k == 1) | (k == 3))[:, None] + wo * ((k == 2) | (k == 3))[:, None]
+    tiled = torch.where((k == 0)[:, None], t, shifted) * s
+    t = torch.where(t_row[:, None], tiled, t)
+    t[:, 0] = q.float()
+    return out, t
 
 
 # ------------------------------------------------------------------------------------------------
