@@ -167,6 +167,17 @@ int myolo_plan_set_seed(myolo_plan* plan, uint64_t seed);
  * reference's order (det batch first, then seg batch). */
 int myolo_plan_set_defer_running(myolo_plan* plan, int defer);
 int myolo_plan_apply_running(myolo_plan* plan, void* stream);
+/* Synchronised BatchNorm (torch.nn.SyncBatchNorm, the reference's --sync-bn, train.py:190-193): every train-mode BN layer normalises with
+ * the mean and biased variance over the batches of all ranks, updates its running statistics with them and the global count, and its
+ * backward uses {sum dz, sum dz*xhat} summed over ranks (d_gamma / d_beta stay local).
+ *   nccl_comm (ncclComm_t): ncclAllGather of each layer's {count, mean, var} record in the forward and ncclAllReduce of the two sums in
+ *     the backward, on this communicator and the plan's stream; world size and rank from ncclCommCount / ncclCommUserRank.  Every rank must
+ *     run the same plans in the same order (NCCL matches collectives by sequence).
+ *   rank_images[n_groups] (nccl_comm null): one-GPU rank emulation.  The batch is n_groups consecutive groups of images, each treated
+ *     as one rank's batch (unequal counts allowed; the counts sum to the plan's batch).
+ * Both null: off.  Both set: MYOLO_E_INVALID.  Not with myolo_plan_set_defer_running.  A synchronised plan runs its forward and backward
+ * in order on the caller's stream, without CUDA-graph replay.  Every BN layer must have C % 8 == 0 and C <= 2048. */
+int myolo_plan_set_bn_sync(myolo_plan* plan, void* nccl_comm, const int32_t* rank_images, int n_groups);
 /* train-mode forward: raw[i] (B,na,ny,nx,no) fp32 and seg (B,n_segcls,H,W) fp32, like Model.forward in training (models/yolo.py:225,316) */
 int myolo_plan_train_forward(myolo_plan* plan, const void* x, int x_dtype, float* const* raw, float* seg, void* stream);
 /* backward of the last train forward: grad_raw[i] / grad_seg are dL/d(raw[i]) / dL/d(seg) (fp32, nullable); parameter gradients are

@@ -37,7 +37,7 @@ EXPORTS = [
     "myolo_grads_check_finite", "myolo_sgd_step", "myolo_conv_wgrad", "myolo_letterbox", "myolo_seg_lut_blend", "myolo_seg_metrics", "myolo_plan_backward_seg_ce", "myolo_plan_read_grad_view", "myolo_plan_set_seed", "myolo_plan_train_forward_multi", "myolo_plan_backward_multi", "myolo_plan_conv_info", "myolo_allreduce_grads", "myolo_det_loss", "myolo_det_loss_workspace_bytes", "myolo_plan_set_defer_running", "myolo_plan_apply_running",
     "myolo_resize_u8", "myolo_augment_det", "myolo_augment_seg", "myolo_det_match", "myolo_det_ap", "myolo_det_ap_workspace_bytes",
     "myolo_resize_area_u8", "myolo_resize_bilinear", "myolo_plan_create_shared", "myolo_augment_det_hw", "myolo_adam_step",
-    "myolo_adam_scalars", "myolo_ema_update", "myolo_plan_set_extra", "myolo_collate_quad",
+    "myolo_adam_scalars", "myolo_ema_update", "myolo_plan_set_extra", "myolo_collate_quad", "myolo_plan_set_bn_sync",
 ]
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
 
@@ -137,6 +137,7 @@ def lib():
     L.myolo_plan_set_seed.argtypes = [vp, C.c_uint64]
     L.myolo_plan_set_defer_running.argtypes = [vp, i32]
     L.myolo_plan_apply_running.argtypes = [vp, vp]
+    L.myolo_plan_set_bn_sync.argtypes = [vp, vp, C.POINTER(C.c_int32), i32]
     L.myolo_plan_train_forward_multi.argtypes = [vp, vp, i32, C.POINTER(vp), C.POINTER(vp), vp]
     L.myolo_plan_backward_multi.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), vp]
     L.myolo_conv_wgrad.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp]

@@ -7,6 +7,7 @@ struct NvtxRange {
   explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
   ~NvtxRange() { nvtxRangePop(); }
 };
+#include <dlfcn.h>
 #include <stdarg.h>
 
 #include <algorithm>
@@ -55,6 +56,31 @@ static int check_device(int* sms) {
   }
   if (dev >= 0 && dev < 64) cached_sms[dev] = prop.multiProcessorCount;
   if (sms) *sms = prop.multiProcessorCount;
+  return 0;
+}
+
+// NCCL entry points, bound at run time from the libnccl already in the process (torch.distributed with the nccl backend loads it): the
+// library does not link NCCL, so a process that never exchanges never needs it
+static void* nccl_symbol(const char* name) {
+  void* sym = dlsym(RTLD_DEFAULT, name);
+  if (!sym) {
+    void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD | RTLD_GLOBAL);
+    if (h) sym = dlsym(h, name);
+  }
+  if (!sym) set_error("%s: no NCCL library is loaded in this process (torch.distributed with the nccl backend loads it)", name);
+  return sym;
+}
+typedef int (*PFN_ncclAllReduce)(const void*, void*, size_t, int /*ncclDataType_t*/, int /*ncclRedOp_t*/, void* /*ncclComm_t*/, cudaStream_t);
+typedef int (*PFN_ncclAllGather)(const void*, void*, size_t, int /*ncclDataType_t*/, void* /*ncclComm_t*/, cudaStream_t);
+typedef int (*PFN_ncclCommQuery)(void* /*ncclComm_t*/, int*);
+constexpr int kNcclFloat32 = 7, kNcclSum = 0;
+
+static int nccl_allreduce_sum(float* buf, size_t n, void* comm, cudaStream_t s) {
+  static PFN_ncclAllReduce fn = nullptr;
+  if (!fn && !(fn = reinterpret_cast<PFN_ncclAllReduce>(nccl_symbol("ncclAllReduce")))) return MYOLO_E_INVALID;
+  const int rc = fn(buf, buf, n, kNcclFloat32, kNcclSum, comm, s);
+  MYOLO_REQUIRE(rc == 0, "ncclAllReduce failed with ncclResult_t %d", rc);
+  g_launch_count++;
   return 0;
 }
 
@@ -131,6 +157,11 @@ struct myolo_plan {
   bool defer_running = false;
   RunningJob* d_run_jobs = nullptr;
   int n_run_jobs = 0;
+  // synchronised BatchNorm (myolo_plan_set_bn_sync): an NCCL communicator, or one-GPU rank emulation over groups of images
+  void* nccl_comm = nullptr;
+  int sync_ranks = 0, sync_rank = 0;  // records per BN layer (world size / number of groups; 0: off) and this process's rank
+  std::vector<int> sync_groups;       // rank emulation: images of each group, in rank order
+  std::vector<float*> bn_sync;        // per BN op: [records (sync_ranks x (kBnRecHead + 2C)) | backward sums (sync_ranks x 2C) | 1 / N]
   unsigned long long seed = 0;       // dropout
   unsigned long long* d_step = nullptr;
   void* ce_scratch = nullptr;      // 16 bytes for the fused seg loss (valid-pixel count, loss sum)
@@ -273,6 +304,7 @@ extern "C" void myolo_plan_destroy(myolo_plan* pl) {
     if (sl.zero_bias) cudaFree(sl.zero_bias);
   }
   for (auto p : pl->bn_stats) if (p) cudaFree(p);
+  for (auto p : pl->bn_sync) if (p) cudaFree(p);
   if (pl->gws && pl->owns_ws) cudaFree(pl->gws);
   for (auto& sl : pl->slots) if (sl.dw_packed) cudaFree(sl.dw_packed);
   if (pl->tmp16) cudaFree(pl->tmp16);
@@ -417,6 +449,67 @@ static int prepare_conv(myolo_plan* pl, int i) {
   return 0;
 }
 
+// ---- synchronised BatchNorm: the exchanges of one BN op (myolo_plan_set_bn_sync) ----
+static TensorView image_slice(TensorView v, int b0, int nb) {     // images [b0, b0 + nb) of a view
+  v.base = static_cast<unsigned char*>(v.base) + (size_t)b0 * v.H * v.W * v.ctot * (v.dtype == MYOLO_F16 ? 2 : 4);
+  v.B = nb;
+  return v;
+}
+static size_t bn_rec_stride(int C) { return kBnRecHead + 2 * (size_t)C; }
+
+// statistics of BN op i over all ranks: this rank's record (or each emulated group's), the all-gather, the combine into bn_stats[i]
+static int bn_sync_forward(myolo_plan* pl, int i, const TensorView& in, const BnParams& bn, cudaStream_t s) {
+  const int R = pl->sync_ranks, C = bn.C;
+  const size_t stride = bn_rec_stride(C);
+  if ((int)pl->bn_sync.size() <= i) pl->bn_sync.resize(pl->ops.size(), nullptr);
+  if (!pl->bn_sync[i]) {
+    const size_t n = (size_t)R * (stride + 2 * (size_t)C) + 4;
+    MYOLO_CHECK_CUDA(cudaMalloc(&pl->bn_sync[i], n * sizeof(float)));
+    MYOLO_CHECK_CUDA(cudaMemsetAsync(pl->bn_sync[i], 0, n * sizeof(float), s));
+  }
+  float* recs = pl->bn_sync[i];
+  float* inv_n = recs + (size_t)R * (stride + 2 * (size_t)C);
+  float* scratch = pl->bn_stats[i] + 2 * C;
+  int rc;
+  if (pl->nccl_comm) {
+    static PFN_ncclAllGather gather = nullptr;
+    if (!gather && !(gather = reinterpret_cast<PFN_ncclAllGather>(nccl_symbol("ncclAllGather")))) return MYOLO_E_INVALID;
+    float* mine = recs + (size_t)pl->sync_rank * stride;
+    if ((rc = launch_bn_stats_record(in, bn, mine, scratch, s))) return rc;
+    // in place: NCCL's all-gather takes sendbuff == recvbuff + rank * count.  A byte copy: the int32 count travels exactly.
+    const int nrc = gather(mine, recs, stride, kNcclFloat32, pl->nccl_comm, s);
+    MYOLO_REQUIRE(nrc == 0, "bn sync: ncclAllGather failed with ncclResult_t %d", nrc);
+    g_launch_count++;
+  } else {
+    for (int g = 0, b0 = 0; g < R; b0 += pl->sync_groups[g++])
+      if ((rc = launch_bn_stats_record(image_slice(in, b0, pl->sync_groups[g]), bn, recs + g * stride, scratch, s))) return rc;
+  }
+  return launch_bn_sync_combine(recs, R, bn, pl->bn_stats[i], inv_n, s);
+}
+
+// backward of BN op i over all ranks: local {sum dz, sum dz*xhat} (this rank's, or each group's), their sum over ranks, then dx with the
+// global sums and 1 / N.  d_gamma / d_beta take the LOCAL sums: the flat-gradient all-reduce averages them, as DDP does.
+static int bn_sync_backward(myolo_plan* pl, int i, const TensorView& u, const TensorView& dy, const TensorView& du, const TensorView* d_res,
+                            const BnParams& bn, int act, cudaStream_t s) {
+  MYOLO_REQUIRE(i < (int)pl->bn_sync.size() && pl->bn_sync[i], "backward: BN op %d has no synchronised forward", i);
+  const int R = pl->sync_ranks, C = bn.C;
+  float* sums = pl->bn_sync[i] + (size_t)R * bn_rec_stride(C);
+  const float* inv_n = sums + (size_t)R * 2 * C;
+  float* scratch = pl->bn_stats[i] + 2 * C;
+  int rc;
+  if (pl->nccl_comm) {
+    if ((rc = launch_bn_bwd_sums(u, dy, bn, pl->bn_stats[i], act, scratch, sums, s))) return rc;
+    if ((rc = nccl_allreduce_sum(sums, 2 * (size_t)C, pl->nccl_comm, s))) return rc;
+  } else {
+    for (int g = 0, b0 = 0; g < R; b0 += pl->sync_groups[g++])
+      if ((rc = launch_bn_bwd_sums(image_slice(u, b0, pl->sync_groups[g]), image_slice(dy, b0, pl->sync_groups[g]), bn, pl->bn_stats[i], act,
+                                   scratch, sums + (size_t)g * 2 * C, s)))
+        return rc;
+    if ((rc = launch_bn_sync_sum(sums, R, 2 * C, s))) return rc;
+  }
+  return launch_bn_act_bwd(u, dy, du, d_res, bn, pl->bn_stats[i], act, scratch, s, sums, inv_n);
+}
+
 static int run_op(myolo_plan* pl, int i, const void* x, int x_dtype, float* z, float* const* raw, void* seg, int seg_dtype,
                   int64_t* seg_argmax, cudaStream_t s) {
   const myolo_op& op = pl->ops[i];
@@ -504,7 +597,9 @@ static int run_op(myolo_plan* pl, int i, const void* x, int x_dtype, float* z, f
         MYOLO_CHECK_CUDA(cudaMalloc(&pl->bn_stats[i], (6 * (size_t)bn.C + 4) * sizeof(float)));
         MYOLO_CHECK_CUDA(cudaMemsetAsync(pl->bn_stats[i], 0, (6 * (size_t)bn.C + 4) * sizeof(float), s));
       }
-      if ((rc = launch_bn_stats(in, bn, pl->bn_stats[i], pl->bn_stats[i] + 2 * bn.C, s, pl->defer_running))) return rc;
+      if (pl->sync_ranks) rc = bn_sync_forward(pl, i, in, bn, s);
+      else rc = launch_bn_stats(in, bn, pl->bn_stats[i], pl->bn_stats[i] + 2 * bn.C, s, pl->defer_running);
+      if (rc) return rc;
       return launch_bn_act_fwd(in, has_res ? &in2 : nullptr, out, bn, pl->bn_stats[i], op.act, s);
     }
     case MYOLO_OP_ACT:
@@ -588,8 +683,9 @@ extern "C" int myolo_plan_forward(myolo_plan* pl, const void* x, int x_dtype, fl
   MYOLO_REQUIRE(pl && x, "plan_forward: null plan / input");
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t l0 = g_launch_count;
-  if (!pl->warmed) {
-    // first call (lazy tensor-map / attribute setup happens here): plain in-order replay
+  if (!pl->warmed || pl->sync_ranks) {
+    // first call (lazy tensor-map / attribute setup happens here): plain in-order replay.  A plan with synchronised BatchNorm always runs
+    // so: its NCCL exchanges are never captured into a graph (torch's communicator is used eagerly for the flat gradients as well)
     for (size_t i = 0; i < pl->ops.size(); ++i) {
       int rc = run_op(pl, (int)i, x, x_dtype, z, raw, seg, seg_dtype, seg_argmax, s);
       if (rc) return rc;
@@ -746,6 +842,7 @@ extern "C" int myolo_plan_set_bn(myolo_plan* pl, int bn_slot, int channels, floa
 // plan's scratch) and applies them with one launch once the first plan's forward has finished.
 extern "C" int myolo_plan_set_defer_running(myolo_plan* pl, int defer) {
   MYOLO_REQUIRE(pl, "set_defer_running: null plan");
+  MYOLO_REQUIRE(!defer || !pl->sync_ranks, "set_defer_running: the plan synchronises its BatchNorm statistics across ranks");
   if (pl->defer_running != (defer != 0)) pl->graph_dirty = true;     // baked into the captured BN launches
   pl->defer_running = defer != 0;
   return 0;
@@ -773,6 +870,41 @@ extern "C" int myolo_plan_apply_running(myolo_plan* pl, void* stream) {
     pl->n_run_jobs = (int)jobs.size();
   }
   return launch_bn_apply_running(pl->d_run_jobs, pl->n_run_jobs, s);
+}
+
+extern "C" int myolo_plan_set_bn_sync(myolo_plan* pl, void* nccl_comm, const int32_t* rank_images, int n_groups) {
+  MYOLO_REQUIRE(pl, "set_bn_sync: null plan");
+  MYOLO_REQUIRE(!(nccl_comm && rank_images), "set_bn_sync: an NCCL communicator or rank emulation, not both");
+  int ranks = 0, rank = 0;
+  std::vector<int> groups;
+  if (nccl_comm) {
+    auto count = reinterpret_cast<PFN_ncclCommQuery>(nccl_symbol("ncclCommCount"));
+    auto user_rank = reinterpret_cast<PFN_ncclCommQuery>(nccl_symbol("ncclCommUserRank"));
+    if (!count || !user_rank) return MYOLO_E_INVALID;
+    MYOLO_REQUIRE(count(nccl_comm, &ranks) == 0 && user_rank(nccl_comm, &rank) == 0 && ranks >= 1 && rank >= 0 && rank < ranks,
+                  "set_bn_sync: cannot query the NCCL communicator");
+  } else if (rank_images) {
+    MYOLO_REQUIRE(n_groups >= 1, "set_bn_sync: %d image groups", n_groups);
+    int total = 0;
+    for (int g = 0; g < n_groups; ++g) {
+      MYOLO_REQUIRE(rank_images[g] >= 1, "set_bn_sync: group %d has %d images", g, rank_images[g]);
+      total += rank_images[g];
+      groups.push_back(rank_images[g]);
+    }
+    MYOLO_REQUIRE(total == pl->B, "set_bn_sync: the groups hold %d images, the plan's batch is %d", total, pl->B);
+    ranks = n_groups;
+  }
+  MYOLO_REQUIRE(!ranks || !pl->defer_running, "set_bn_sync: the plan defers its running statistics (myolo_plan_set_defer_running)");
+  if (ranks != pl->sync_ranks) {        // the buffers hold one record per rank
+    for (auto& p : pl->bn_sync) if (p) { cudaFree(p); p = nullptr; }
+  }
+  pl->nccl_comm = nccl_comm;
+  pl->sync_ranks = ranks;
+  pl->sync_rank = rank;
+  pl->sync_groups = groups;
+  pl->graph_dirty = true;               // the BN launches of captured graphs are the unsynchronised ones
+  pl->bwd_dirty = true;
+  return 0;
 }
 
 extern "C" int myolo_plan_set_seed(myolo_plan* pl, uint64_t seed) {
@@ -995,8 +1127,9 @@ static int backward_run(myolo_plan* pl, int mask, std::vector<char>& live, cudaS
     pl->bwd_dirty = false;
   }
   int n_ops = 0;
-  if (!pl->bwd_warm[mask]) {
-    // first backward with this seed set: in order on the caller's stream (allocations, tensor maps, weight packs happen here)
+  if (!pl->bwd_warm[mask] || pl->sync_ranks) {
+    // first backward with this seed set: in order on the caller's stream (allocations, tensor maps, weight packs happen here); always
+    // with synchronised BatchNorm, whose exchanges are not captured (myolo_plan_forward)
     rc = backward_walk(pl, live, s, &n_ops);
     if (!rc && !pl->bwd_dirty) pl->bwd_warm[mask] = true;
     return rc;
@@ -1113,7 +1246,10 @@ static int backward_walk(myolo_plan* pl, std::vector<char>& live, cudaStream_t s
         if ((rc = resolve_view(pl, op.in, &a)) || (rc = grad_view(pl, op.out, &b)) || (rc = grad_view(pl, op.in, &c))) break;
         if (has_res && (rc = grad_view(pl, op.in2, &d))) break;
         const BnParams& bn = pl->bns[op.aux[0]];
-        rc = launch_bn_act_bwd(a, b, c, has_res ? &d : nullptr, bn, pl->bn_stats[i], op.act, pl->bn_stats[i] + 2 * bn.C, s);
+        // synchronised BN: one all-reduce per live BN op.  NCCL needs the same sequence of collectives on every rank; every rank runs
+        // the same op list (built from the same model), and which ops are live depends only on the seed mask, not on the data
+        if (pl->sync_ranks) rc = bn_sync_backward(pl, i, a, b, c, has_res ? &d : nullptr, bn, op.act, s);
+        else rc = launch_bn_act_bwd(a, b, c, has_res ? &d : nullptr, bn, pl->bn_stats[i], op.act, pl->bn_stats[i] + 2 * bn.C, s);
         break;
       }
       case MYOLO_OP_ACT:
@@ -1334,27 +1470,12 @@ extern "C" int myolo_ema_update(const myolo_ema_chunk* chunks, int n_chunks, dou
 }
 
 // ------------------------------------------------------------------------------------------------
-// gradient exchange: NCCL all-reduce of the flat gradient buffer, bound at run time from the libnccl already in the process
+// gradient exchange: NCCL all-reduce of the flat gradient buffer (nccl_symbol: the libnccl already in the process)
 // ------------------------------------------------------------------------------------------------
-#include <dlfcn.h>
-typedef int (*PFN_ncclAllReduce)(const void*, void*, size_t, int /*ncclDataType_t*/, int /*ncclRedOp_t*/, void* /*ncclComm_t*/, cudaStream_t);
 extern "C" int myolo_allreduce_grads(float* flat_grad, int64_t n, void* nccl_comm, void* stream) {
   NvtxRange nvtx_("myolo_allreduce_grads");
   MYOLO_REQUIRE(flat_grad && n > 0 && nccl_comm, "allreduce_grads: bad arguments");
-  static PFN_ncclAllReduce fn = nullptr;
-  if (!fn) {
-    void* sym = dlsym(RTLD_DEFAULT, "ncclAllReduce");
-    if (!sym) {
-      void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_NOLOAD | RTLD_GLOBAL);
-      if (h) sym = dlsym(h, "ncclAllReduce");
-    }
-    MYOLO_REQUIRE(sym, "allreduce_grads: no NCCL library is loaded in this process (torch.distributed with the nccl backend loads it)");
-    fn = reinterpret_cast<PFN_ncclAllReduce>(sym);
-  }
-  const int rc = fn(flat_grad, flat_grad, (size_t)n, 7 /* ncclFloat32 */, 0 /* ncclSum */, nccl_comm, (cudaStream_t)stream);
-  MYOLO_REQUIRE(rc == 0, "allreduce_grads: ncclAllReduce failed with ncclResult_t %d", rc);
-  g_launch_count++;
-  return 0;
+  return nccl_allreduce_sum(flat_grad, (size_t)n, nccl_comm, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------

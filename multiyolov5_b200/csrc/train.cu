@@ -99,11 +99,23 @@ __global__ void chan_reduce_kernel(TensorView a, TensorView bview, const float* 
 // on the distance of the mean from that value.  Summing u itself loses the variance of a channel whose mean is large against its spread
 // (flat image content: letterbox padding, sky, road): at mean/std = 200 the fp32 E[u^2] - mean^2 is off by ~1e-2 of the normalised output.
 // final_out (MODE 0, deferred running statistics): batch mean and biased variance; (MODE 1): the two sums.
+// rec (MODE 0, synchronised BN): the epilogue writes this rank's record {count, mean[C], biased var[C]} (bn_sync_combine_kernel) and
+// finalises nothing.
+// mean / inverse std and the running-statistics update of one channel from the batch mean and biased variance of n values: shared by the
+// local epilogue and the synchronised combine, so that a combine over one record repeats the local path bit for bit
+__device__ __forceinline__ void bn_finalize_channel(float mean, float var, float n, const BnParams& bn, int c, int C, float* stats_out) {
+  stats_out[c] = mean;
+  stats_out[C + c] = rsqrtf(var + bn.eps);
+  if (bn.running_mean) {                                       // running stats: unbiased variance, momentum 0.03
+    bn.running_mean[c] = (1.f - bn.momentum) * bn.running_mean[c] + bn.momentum * mean;
+    bn.running_var[c] = (1.f - bn.momentum) * bn.running_var[c] + bn.momentum * var * (n / fmaxf(n - 1.f, 1.f));
+  }
+}
 template <int MODE>
 __global__ void __launch_bounds__(256) chan_reduce_v_kernel(TensorView a, TensorView bview, const float* __restrict__ stats,
                                                             const float* __restrict__ gamma, const float* __restrict__ beta, int act,
                                                             float* out, long npix, int C, BnParams bn, float* stats_out,
-                                                            unsigned* ticket, float* final_out) {
+                                                            unsigned* ticket, float* final_out, float* rec) {
   __shared__ float sh[2][2048];
   __shared__ int is_last;
   pdl_enter();
@@ -164,6 +176,7 @@ __global__ void __launch_bounds__(256) chan_reduce_v_kernel(TensorView a, Tensor
   // the last block consumes the sums and leaves accumulators + ticket ZERO for the next launch on this scratch (allocated zeroed): no
   // memset node between the producing conv and this kernel, so the programmatic-launch edge survives
   if (t == 0) *ticket = 0u;
+  if (MODE == 0 && rec && t == 0) reinterpret_cast<int*>(rec)[0] = (int)npix;
   for (int c = t; c < C; c += 256) {
     const float x0 = __ldcg(out + c), x1 = __ldcg(out + C + c);
     out[c] = 0.f;
@@ -173,13 +186,9 @@ __global__ void __launch_bounds__(256) chan_reduce_v_kernel(TensorView a, Tensor
       const float d = x0 / n;
       const float mean = __half2float(bn_shift_ptr(a)[c]) + d;
       const float var = fmaxf(x1 / n - d * d, 0.f);                // biased variance normalises (F.batch_norm, training=True)
+      if (rec) { rec[kBnRecHead + c] = mean; rec[kBnRecHead + C + c] = var; continue; }
       if (final_out) { final_out[c] = mean; final_out[C + c] = var; }
-      stats_out[c] = mean;
-      stats_out[C + c] = rsqrtf(var + bn.eps);
-      if (bn.running_mean) {                                       // running stats: unbiased variance, momentum 0.03
-        bn.running_mean[c] = (1.f - bn.momentum) * bn.running_mean[c] + bn.momentum * mean;
-        bn.running_var[c] = (1.f - bn.momentum) * bn.running_var[c] + bn.momentum * var * (n / fmaxf(n - 1.f, 1.f));
-      }
+      bn_finalize_channel(mean, var, n, bn, c, C, stats_out);
     } else {
       if (final_out) { final_out[c] = x0; final_out[C + c] = x1; }
       // parameter gradients are accumulated atomically everywhere: the det and the seg backward of one training step may run concurrently
@@ -240,7 +249,8 @@ int launch_bn_stats(const TensorView& u, const BnParams& bn_in, float* stats, fl
   if (u.C % 8 == 0 && u.C <= 2048 && u.ctot % 8 == 0) {
     MYOLO_CHECK_CUDA(launch_pdl(chan_reduce_v_kernel<0>, dim3(reduce_v_grid(npix, u.C)), dim3(256), 0, s, u, u, (const float*)nullptr,
                                 (const float*)nullptr, (const float*)nullptr, 0, scratch, npix, u.C, bn, stats,
-                                reinterpret_cast<unsigned*>(scratch + 4 * u.C), defer_running ? scratch + 2 * u.C : (float*)nullptr));
+                                reinterpret_cast<unsigned*>(scratch + 4 * u.C), defer_running ? scratch + 2 * u.C : (float*)nullptr,
+                                (float*)nullptr));
     g_launch_count++;
     return 0;
   }
@@ -251,6 +261,73 @@ int launch_bn_stats(const TensorView& u, const BnParams& bn_in, float* stats, fl
   bn_finalize_kernel<<<ceil_div(u.C, 128), 128, 0, s>>>(u, scratch, stats, bn, npix);
   MYOLO_LAUNCH_CHECK();
   MYOLO_CHECK_CUDA(cudaMemsetAsync(scratch, 0, (2 * (size_t)u.C) * sizeof(float), s));    // contract of the scratch: zero between launches
+  return 0;
+}
+
+// ---- synchronised BatchNorm (torch.nn.SyncBatchNorm, torch/nn/modules/_functions.py) ----
+static bool bn_sync_shape_ok(const TensorView& u) { return u.dtype == MYOLO_F16 && u.C % 8 == 0 && u.C <= 2048 && u.ctot % 8 == 0; }
+
+int launch_bn_stats_record(const TensorView& u, const BnParams& bn, float* rec, float* scratch, cudaStream_t s) {
+  MYOLO_REQUIRE(bn.set && bn.C == u.C && bn_sync_shape_ok(u), "bn_stats_record: synchronised BatchNorm needs an fp16 view with C %% 8 == 0 "
+                "and C <= 2048 (C = %d)", u.C);
+  const long npix = (long)u.B * u.H * u.W;
+  MYOLO_REQUIRE(npix > 0 && npix < (1L << 31), "bn_stats_record: %ld values per channel do not fit the record's int32 count", npix);
+  MYOLO_CHECK_CUDA(launch_pdl(chan_reduce_v_kernel<0>, dim3(reduce_v_grid(npix, u.C)), dim3(256), 0, s, u, u, (const float*)nullptr,
+                              (const float*)nullptr, (const float*)nullptr, 0, scratch, npix, u.C, bn, (float*)nullptr,
+                              reinterpret_cast<unsigned*>(scratch + 4 * u.C), (float*)nullptr, rec));
+  g_launch_count++;
+  return 0;
+}
+
+// Global statistics from the gathered records, combined in rank order with the pairwise (Chan et al.) update in fp64:
+//   n = na + nb,  mean = ma + (mb - ma) nb / n,  M2 = M2a + M2b + (mb - ma)^2 na nb / n,  var = M2 / n   (biased)
+// One record is passed through unchanged, so the result is the local epilogue's to the bit.  Every rank combines the same records in the
+// same order and writes the same bits: running statistics stay identical across ranks.  inv_n = 1 / N for the backward.
+__global__ void bn_sync_combine_kernel(const float* __restrict__ recs, int n_rec, int C, BnParams bn, float* stats, float* inv_n) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  const long stride = kBnRecHead + 2L * C;
+  long n = reinterpret_cast<const int*>(recs)[0];
+  float mean = recs[kBnRecHead + c], var = recs[kBnRecHead + C + c];
+  if (n_rec > 1) {
+    double na = (double)n, ma = mean, m2 = (double)var * na;
+    for (int r = 1; r < n_rec; ++r) {
+      const float* rr = recs + r * stride;
+      const double nb = (double)reinterpret_cast<const int*>(rr)[0];
+      const double mb = rr[kBnRecHead + c], m2b = (double)rr[kBnRecHead + C + c] * nb;
+      const double nab = na + nb, delta = mb - ma;
+      ma += delta * nb / nab;
+      m2 += m2b + delta * delta * na * nb / nab;
+      na = nab;
+    }
+    n = (long)na;
+    mean = (float)ma;
+    var = (float)(m2 / na);
+  }
+  if (c == 0) *inv_n = 1.0f / (float)n;
+  bn_finalize_channel(mean, var, (float)n, bn, c, C, stats);
+}
+int launch_bn_sync_combine(const float* recs, int n_rec, const BnParams& bn, float* stats, float* inv_n, cudaStream_t s) {
+  MYOLO_REQUIRE(recs && n_rec >= 1 && stats && inv_n, "bn_sync_combine: bad arguments");
+  bn_sync_combine_kernel<<<ceil_div(bn.C, 128), 128, 0, s>>>(recs, n_rec, bn.C, bn, stats, inv_n);
+  MYOLO_LAUNCH_CHECK();
+  g_launch_count++;
+  return 0;
+}
+
+// sums[j] += sums[g * n + j] for g = 1 .. n_groups-1, in group order (the all-reduce of the backward sums between emulated ranks)
+__global__ void bn_sync_sum_kernel(float* sums, int n_groups, int n) {
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= n) return;
+  float acc = sums[j];
+  for (int g = 1; g < n_groups; ++g) acc += sums[(long)g * n + j];
+  sums[j] = acc;
+}
+int launch_bn_sync_sum(float* sums, int n_groups, int n, cudaStream_t s) {
+  if (n_groups <= 1) return 0;
+  bn_sync_sum_kernel<<<ceil_div(n, 256), 256, 0, s>>>(sums, n_groups, n);
+  MYOLO_LAUNCH_CHECK();
+  g_launch_count++;
   return 0;
 }
 
@@ -292,8 +369,9 @@ int launch_bn_act_fwd(const TensorView& u, const TensorView* res, const TensorVi
 
 __global__ void bn_act_bwd_kernel(TensorView u, TensorView dy, TensorView du, TensorView dres, bool has_res, const float* __restrict__ gamma,
                                   const float* __restrict__ beta, const float* __restrict__ stats, const float* __restrict__ sums, int act,
-                                  float inv_n) {
+                                  float inv_n_host, const float* __restrict__ inv_n_dev) {
   pdl_enter();
+  const float inv_n = inv_n_dev ? *inv_n_dev : inv_n_host;       // synchronised BN: 1 / N over all ranks, from bn_sync_combine_kernel
   const long total = (long)u.B * u.H * u.W * (u.C / 8);
   const int nv = u.C / 8, C = u.C;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -352,16 +430,30 @@ __global__ void add_acc_kernel(TensorView dst, TensorView src) {   // dst += src
     *dp = a;
   }
 }
+int launch_bn_bwd_sums(const TensorView& u, const TensorView& dy, const BnParams& bn, const float* stats, int act, float* scratch,
+                       float* sums_out, cudaStream_t s) {
+  MYOLO_REQUIRE(bn_sync_shape_ok(u) && dy.C == u.C && dy.ctot % 8 == 0, "bn_bwd_sums: synchronised BatchNorm needs C %% 8 == 0 and C <= 2048");
+  const long npix = (long)u.B * u.H * u.W;
+  MYOLO_CHECK_CUDA(launch_pdl(chan_reduce_v_kernel<1>, dim3(reduce_v_grid(npix, u.C)), dim3(256), 0, s, u, dy, stats, (const float*)bn.gamma,
+                              (const float*)bn.beta, act, scratch, npix, u.C, bn, (float*)nullptr,
+                              reinterpret_cast<unsigned*>(scratch + 4 * u.C), sums_out, (float*)nullptr));
+  g_launch_count++;
+  return 0;
+}
+
 int launch_bn_act_bwd(const TensorView& u, const TensorView& dy, const TensorView& du, const TensorView* d_res, const BnParams& bn,
-                      const float* stats, int act, float* scratch, cudaStream_t s) {
+                      const float* stats, int act, float* scratch, cudaStream_t s, const float* synced_sums, const float* inv_n) {
   MYOLO_REQUIRE(u.C % 8 == 0 && dy.C == u.C && du.C == u.C && dy.ctot % 8 == 0 && du.ctot % 8 == 0 && u.ctot % 8 == 0, "bn_act_bwd: bad views");
   MYOLO_REQUIRE(!d_res || (d_res->C == u.C && d_res->ctot % 8 == 0), "bn_act_bwd: bad residual gradient view");
+  MYOLO_REQUIRE(!synced_sums == !inv_n, "bn_act_bwd: synchronised sums and 1 / N go together");
   const long npix = (long)u.B * u.H * u.W;
   const float* sums = scratch;
-  if (u.C <= 2048) {
+  if (synced_sums) {
+    sums = synced_sums;                  // launch_bn_bwd_sums + the exchange already ran
+  } else if (u.C <= 2048) {
     MYOLO_CHECK_CUDA(launch_pdl(chan_reduce_v_kernel<1>, dim3(reduce_v_grid(npix, u.C)), dim3(256), 0, s, u, dy, stats, (const float*)bn.gamma,
                                 (const float*)bn.beta, act, scratch, npix, u.C, bn, (float*)nullptr,
-                                reinterpret_cast<unsigned*>(scratch + 4 * u.C), scratch + 2 * u.C));
+                                reinterpret_cast<unsigned*>(scratch + 4 * u.C), scratch + 2 * u.C, (float*)nullptr));
     g_launch_count++;
     sums = scratch + 2 * u.C;            // the reduce kernel leaves its accumulators zero and hands the totals over here
   } else {
@@ -373,7 +465,7 @@ int launch_bn_act_bwd(const TensorView& u, const TensorView& dy, const TensorVie
     MYOLO_LAUNCH_CHECK();
   }
   MYOLO_CHECK_CUDA(launch_pdl(bn_act_bwd_kernel, dim3(grid_for_t(npix * (u.C / 8), 256)), dim3(256), 0, s, u, dy, du, d_res ? *d_res : du,
-                              d_res != nullptr, (const float*)bn.gamma, (const float*)bn.beta, stats, sums, act, 1.0f / (float)npix));
+                              d_res != nullptr, (const float*)bn.gamma, (const float*)bn.beta, stats, sums, act, 1.0f / (float)npix, inv_n));
   g_launch_count++;
   if (sums == scratch) MYOLO_CHECK_CUDA(cudaMemsetAsync(scratch, 0, (2 * (size_t)u.C) * sizeof(float), s));   // (> 2048 channels: generic path)
   return 0;

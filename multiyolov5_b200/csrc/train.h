@@ -31,6 +31,15 @@ struct RunningJob {         // one BN layer of a deferred running-statistics upd
   float momentum;
 };
 int launch_bn_apply_running(const RunningJob* d_jobs, int n_jobs, cudaStream_t s);
+// synchronised BatchNorm (torch.nn.SyncBatchNorm).  A rank's record is kBnRecHead + 2*C floats: {count as int32 bits, 0, 0, 0, mean[C],
+// biased var[C]}; records of all ranks lie back to back (what ncclAllGather of one record per rank produces).
+constexpr int kBnRecHead = 4;
+// the record of u (C % 8 == 0, C <= 2048) into rec; scratch as launch_bn_stats'.  Finalises nothing.
+int launch_bn_stats_record(const TensorView& u, const BnParams& bn, float* rec, float* scratch, cudaStream_t s);
+// global mean / invstd -> stats, running statistics with the global count, *inv_n = 1 / N (device) from n_rec gathered records
+int launch_bn_sync_combine(const float* recs, int n_rec, const BnParams& bn, float* stats, float* inv_n, cudaStream_t s);
+// sums[0..n) += sums[g*n .. g*n+n) for g = 1 .. n_groups-1, in order
+int launch_bn_sync_sum(float* sums, int n_groups, int n, cudaStream_t s);
 // y = act(gamma*(u-mean)*invstd + beta) (+ residual)
 int launch_bn_act_fwd(const TensorView& u, const TensorView* res, const TensorView& y, const BnParams& bn, const float* stats, int act,
                       cudaStream_t s);
@@ -45,9 +54,14 @@ int launch_bump_step(unsigned long long* step, cudaStream_t s);
 
 // ---- backward ----
 // dz = dy*act'(z), z = gamma*xhat+beta; du = gamma*invstd*(dz - mean(dz) - xhat*mean(dz*xhat)); dgamma += sum(dz*xhat); dbeta += sum(dz)
-// d_res (nullable) += dy.  `scratch` holds 2*C floats.
+// d_res (nullable) += dy.  `scratch` holds 2*C floats.  Synchronised BN: synced_sums = {sum dz, sum dz*xhat} over all ranks (2*C
+// floats) and inv_n = 1 / N (device) replace the local reduce and 1 / npix.
 int launch_bn_act_bwd(const TensorView& u, const TensorView& dy, const TensorView& du, const TensorView* d_res, const BnParams& bn,
-                      const float* stats, int act, float* scratch, cudaStream_t s);
+                      const float* stats, int act, float* scratch, cudaStream_t s, const float* synced_sums = nullptr,
+                      const float* inv_n = nullptr);
+// the local {sum dz, sum dz*xhat} of a synchronised BN layer into sums_out (2*C floats); adds them to d_beta / d_gamma as well
+int launch_bn_bwd_sums(const TensorView& u, const TensorView& dy, const BnParams& bn, const float* stats, int act, float* scratch,
+                       float* sums_out, cudaStream_t s);
 int launch_act_bwd(const TensorView& x, const TensorView& dy, const TensorView& dx, int act, cudaStream_t s);
 // df += dout*(1+a);  da[b,c] += sum_p dout*f
 int launch_channel_scale_bwd(const TensorView& f, const TensorView& a, const TensorView& dout, const TensorView& df, const TensorView& da,

@@ -76,6 +76,8 @@ class CompiledPlan:
         self._ptr_sig = None                 # parameter / gradient pointers registered with the library
         self._nbt = []                       # num_batches_tracked of the BatchNorm slots
         self._defer_running = False          # Engine.set_defer_running
+        self._bn_owners = None               # (parent's _modules, name, module) of every BatchNorm slot, bound by the first prepare
+        self.bn_sync = None                  # Engine.set_bn_sync: None (local statistics), ("nccl", comm) or ("ranks", images per rank)
         self.fwd_generation = 0              # train forwards of this plan (or of its arena): a backward is valid for the latest only
 
     def __del__(self):
@@ -282,6 +284,10 @@ class Engine:
         if not p._seed_set:                      # dropout masks follow torch's global seed (one hash stream per plan)
             _lib.check(L.myolo_plan_set_seed(p.handle, C.c_uint64(torch.initial_seed() & 0xFFFFFFFFFFFFFFFF)))
             p._seed_set = True
+        if p._bn_owners is None:
+            self._bind_bn_sync(p)
+        elif any(d.get(name) is not bn for d, name, bn in p._bn_owners):
+            raise _lib.MyoloError(self._BN_CHANGED)
         self._upload_if_stale(p)
         sig = (self._flat_grad.data_ptr(), params[0].data_ptr(), params[-1].data_ptr(), len(params))
         if p._ptr_sig != sig:                    # (re)register parameter / gradient pointers only when they moved
@@ -292,6 +298,40 @@ class Engine:
                                                _lib.ptr(bn.running_var), _lib.ptr(bn.weight.grad), _lib.ptr(bn.bias.grad), float(bn.momentum), float(bn.eps)))
             p._ptr_sig = sig
             p._nbt = [bn.num_batches_tracked for bn in p.pb.bn_slots]
+
+    _BN_CHANGED = ("the model's BatchNorm layers were replaced after its train plans were built (torch.nn.SyncBatchNorm."
+                   "convert_sync_batchnorm?): those plans would normalise with the old layers' semantics.  Convert the model before its "
+                   "first train forward and before building a Trainer, as reference train.py:190-193 does")
+
+    def _bind_bn_sync(self, p):
+        """first prepare of train plan p: remembers where each of its BatchNorm layers sits in the model (a layer replaced later raises
+        instead of training with the old semantics) and, for SyncBatchNorm layers that synchronise (parallel.bn_sync_group), hands the
+        group's NCCL communicator to the plan"""
+        from .parallel import bn_sync_group, nccl_comm_ptr
+        owners = {id(c): (m._modules, name) for m in self.model.modules() for name, c in m._modules.items()}
+        if any(id(bn) not in owners for bn in p.pb.bn_slots):
+            raise _lib.MyoloError(self._BN_CHANGED)
+        group = bn_sync_group(p.pb.bn_slots)
+        if group is not None:
+            import torch.distributed as dist
+            dev = torch.device("cuda", torch.cuda.current_device())
+            comm = nccl_comm_ptr(group, dev)
+            if comm is None:                     # torch creates the group's communicator at its first collective
+                dist.all_reduce(torch.zeros(1, device=dev), group=group)
+                comm = nccl_comm_ptr(group, dev)
+            if comm is None:
+                raise _lib.MyoloError("SyncBatchNorm: the process group has no NCCL communicator the library can use")
+            self.set_bn_sync(p, comm=comm)
+        p._bn_owners = [owners[id(bn)] + (bn,) for bn in p.pb.bn_slots]
+
+    def set_bn_sync(self, plan, comm=None, rank_images=None):
+        """synchronised BatchNorm for train plan `plan` (myolo_plan_set_bn_sync): comm = a raw ncclComm_t (parallel.nccl_comm_ptr), or
+        rank_images = the images of each emulated rank (one-GPU rank emulation: the plan's batch split into consecutive groups); neither:
+        local statistics.  The plan then runs without CUDA-graph replay."""
+        imgs = None if rank_images is None else (C.c_int32 * len(rank_images))(*[int(n) for n in rank_images])
+        _lib.check(_lib.lib().myolo_plan_set_bn_sync(plan.handle, C.c_void_p(comm) if comm else None, imgs,
+                                                     0 if rank_images is None else len(rank_images)))
+        plan.bn_sync = ("nccl", comm) if comm else (("ranks", tuple(int(n) for n in rank_images)) if rank_images is not None else None)
 
     def train_forward(self, x: torch.Tensor, out_raws=None, want_seg=True, lane=0):
         """out_raws: optional list of three preallocated (B,na,ny,nx,no) fp32 tensors to write the head outputs into (static buffers of a

@@ -23,6 +23,31 @@ def aggregate_throughput(images_local: int, ms_local: float, device=None) -> flo
     return float(n.item() / (t.item() * 1e-3))
 
 
+def bn_sync_group(bns):
+    """The process group whose ranks train-mode BatchNorm layers `bns` exchange statistics over, or None when they normalise with local
+    statistics.  torch.nn.SyncBatchNorm synchronises only when torch.distributed is initialised and its group has more than one rank
+    (torch's `need_sync`); otherwise it is F.batch_norm, which is what the train plans compute without an exchange.
+    ValueError: SyncBatchNorm mixed with plain BatchNorm, SyncBatchNorm layers on different process groups (convert_sync_batchnorm gives
+    every layer the same one), or a synchronising group whose backend is not NCCL (the library exchanges over NCCL only)."""
+    sync = [m for m in bns if isinstance(m, torch.nn.SyncBatchNorm)]
+    if not sync:
+        return None
+    if len(sync) != len(bns):
+        raise ValueError(f"{len(sync)} of {len(bns)} BatchNorm layers are SyncBatchNorm: convert all of them "
+                         "(torch.nn.SyncBatchNorm.convert_sync_batchnorm) or none")
+    if len({id(m.process_group) for m in sync}) > 1:
+        raise ValueError("the SyncBatchNorm layers synchronise over different process groups; the train plans exchange over one")
+    if not (dist.is_available() and dist.is_initialized()):
+        return None
+    group = sync[0].process_group or dist.group.WORLD
+    if dist.get_world_size(group) <= 1:
+        return None
+    if dist.get_backend(group) != "nccl":
+        raise ValueError(f"SyncBatchNorm over a {dist.get_backend(group)} process group of {dist.get_world_size(group)} ranks: the train "
+                         "plans exchange BatchNorm statistics over NCCL only")
+    return group
+
+
 LAST_ALLREDUCE_PATH = "none"      # which route the last allreduce_flat_grads took (reported by bench.py's train record)
 
 

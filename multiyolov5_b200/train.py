@@ -22,6 +22,10 @@ per-entry statements.  Pass it on rank -1 / 0 and None elsewhere, as train.py:15
 `Trainer(..., quad=True)` is the reference's `--quad`: det batches from `utils.datasets.collate_quad` (collate_fn4) and the det loss x 4
 (train.py:368-369).
 
+A model converted with torch.nn.SyncBatchNorm.convert_sync_batchnorm (the reference's --sync-bn, train.py:190-193) trains with
+BatchNorm statistics exchanged across the ranks of its NCCL process group inside the train plans (Engine.set_bn_sync); the two passes of a
+step then run one after the other.  At world size 1, or without torch.distributed, it trains exactly like the plain model, as torch does.
+
 Out of scope (the reference's outer loop, not the hot path): data loading, LR schedule / warm-up (call `set_lr` / `set_momentum`),
 writing checkpoint files, plotting, DDP buffer broadcast.
 """
@@ -34,7 +38,7 @@ import torch.nn as nn
 
 from . import _lib
 from .engine import flat_offsets
-from .parallel import allreduce_flat_grads
+from .parallel import allreduce_flat_grads, bn_sync_group
 from .utils.loss import FusedComputeLoss, SegmentationLosses
 
 
@@ -60,7 +64,7 @@ def reference_param_groups(model: nn.Module):
         if isinstance(b, nn.Parameter):
             pg2.append(b)
         w = getattr(m, "weight", None)
-        if isinstance(m, nn.BatchNorm2d):
+        if isinstance(m, nn.modules.batchnorm._BatchNorm):     # nn.BatchNorm2d, and nn.SyncBatchNorm after convert_sync_batchnorm
             pg0.append(m.weight)
         elif isinstance(w, nn.Parameter):
             pg1.append(w)
@@ -350,6 +354,10 @@ class Trainer:
         self.inv_scale = torch.ones((), device=dev)
         self.ni = 0
         self._det_graphs = {}
+        # SyncBatchNorm layers that synchronise (torch.distributed initialised, more than one rank): the train plans exchange their
+        # statistics over NCCL, and the two passes run one after the other, so that every rank issues the exchanges in one order on one
+        # communicator (_passes_concurrent would interleave two streams of them differently on each rank)
+        self.sync_bn = bn_sync_group([m for m in model.modules() if isinstance(m, nn.modules.batchnorm._BatchNorm)]) is not None
         self._s_seg = torch.cuda.Stream() if self.fused_seg else None          # the seg pass of _passes_concurrent
         self._ev_detfwd, self._ev_start, self._ev_seg = torch.cuda.Event(), torch.cuda.Event(), torch.cuda.Event()
         self.multi_scale = multi_scale
@@ -557,7 +565,8 @@ class Trainer:
         """one iteration (train.py:363-401).  Returns (det loss items [lbox,lobj,lcls,loss], seg loss) as device tensors."""
         if self._ms_batches and imgs.shape[0] not in self._ms_batches:
             self._reserve_det(int(imgs.shape[0]))               # host plans only: the shared workspace is already there
-        passes = self._passes_concurrent if self.fused_seg else self._passes_sequential     # autograd's seg pass runs Model.forward: lane 0
+        # autograd's seg pass runs Model.forward: lane 0.  Synchronised BatchNorm: one stream of collectives, det pass then seg pass
+        passes = self._passes_concurrent if self.fused_seg and not self.sync_bn else self._passes_sequential
         items, segloss = passes(imgs, targets, segimgs, segtargets)
         self.ni += 1
         if self.ni % self.accumulate == 0:
