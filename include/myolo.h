@@ -193,6 +193,14 @@ int myolo_plan_backward_multi(myolo_plan* plan, const float* const* grad_raw, co
  * factor * (*scale_dev) * d(loss)/d(logits).  loss_out (device float, nullable) receives the mean CE.  scale_dev: device float, nullable. */
 int myolo_plan_backward_seg_ce(myolo_plan* plan, const int64_t* labels, int ignore_index, float factor, const float* scale_dev,
                                float* loss_out, void* stream);
+/* The same fused pass with the reference's OhemCELoss (utils/loss.py:303-328) in place of the mean CE: with n_min = (valid pixels) // 16,
+ * the pixels whose CE exceeds thresh_t (= -log(thresh), fp32) when there are at least n_min of them, else the n_min largest CEs (ignored
+ * pixels take part with CE 0; among pixels tied at the n_min-th value the lowest flat indices b*H*W + y*W + x), averaged over the pixels
+ * taken.  No hard pixel with n_min = 0 gives NaN and no gradient, as the reference does; a non-finite CE gives a NaN loss and NaN
+ * gradients.  The selection runs on the device with a fixed launch sequence (no host synchronisation; capturable, either branch on replay).
+ * Scratch of 4 bytes per full-resolution pixel plus ~5 KB is allocated on the first call and kept by the plan. */
+int myolo_plan_backward_seg_ohem(myolo_plan* plan, const int64_t* labels, int ignore_index, float thresh_t, float factor,
+                                 const float* scale_dev, float* loss_out, void* stream);
 /* debug: like myolo_plan_read_view, from the gradient workspace of the last backward */
 int myolo_plan_read_grad_view(myolo_plan* plan, myolo_view view, float* dst_nchw_f32, void* stream);
 /* Optimiser step over FLAT fp32 buffers (all parameters of the model laid out back to back; `group[i]` in 0..n_groups-1 selects the
@@ -251,6 +259,17 @@ int myolo_det_loss(const float* const* p, float* const* dp, const float* targets
                    const int32_t* nx, const float* anchors_grid, const float* balance, float hyp_box, float hyp_obj, float hyp_cls,
                    float anchor_t, float gr, float cp, float cn, float mult, const float* scale_dev, float* items_out, void* workspace,
                    int64_t workspace_bytes, void* stream);
+
+/* OhemCELoss.forward_once (reference utils/loss.py:321-328) over full-resolution logits (B, C, H, W) fp32 NCHW, any C, and labels (B, H, W)
+ * int64, with the selection of myolo_plan_backward_seg_ohem.  myolo_seg_ohem_loss writes the loss to loss_out (device float) and leaves
+ * its selection in the workspace; myolo_seg_ohem_loss_backward then writes grad_logits = (*grad_out) * d loss / d logits (grad_out: device
+ * float) from the same logits, labels and workspace.  Labels outside [0, C) other than ignore_index count as ignored.  No host
+ * synchronisation in either call.  Python: utils.loss.OhemCELoss. */
+int64_t myolo_seg_ohem_loss_workspace_bytes(int B, int H, int W);
+int myolo_seg_ohem_loss(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index, float thresh_t,
+                        float* loss_out, void* workspace, int64_t workspace_bytes, void* stream);
+int myolo_seg_ohem_loss_backward(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index,
+                                 const float* grad_out, float* grad_logits, const void* workspace, int64_t workspace_bytes, void* stream);
 
 /* The path's ONE exchange step (SURVEY.md section 8b/8e; reference train.py:243-245 wraps the model in DistributedDataParallel): in-place
  * SUM all-reduce of the flat fp32 gradient buffer over the ranks of `nccl_comm` (an ncclComm_t; averaging is folded into myolo_sgd_step's

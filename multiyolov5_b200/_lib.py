@@ -38,6 +38,7 @@ EXPORTS = [
     "myolo_resize_u8", "myolo_augment_det", "myolo_augment_seg", "myolo_det_match", "myolo_det_ap", "myolo_det_ap_workspace_bytes",
     "myolo_resize_area_u8", "myolo_resize_bilinear", "myolo_plan_create_shared", "myolo_augment_det_hw", "myolo_adam_step",
     "myolo_adam_scalars", "myolo_ema_update", "myolo_plan_set_extra", "myolo_collate_quad", "myolo_plan_set_bn_sync",
+    "myolo_plan_backward_seg_ohem", "myolo_seg_ohem_loss", "myolo_seg_ohem_loss_backward", "myolo_seg_ohem_loss_workspace_bytes",
 ]
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
 
@@ -133,6 +134,11 @@ def lib():
     L.myolo_det_ap_workspace_bytes.restype = i64
     L.myolo_det_ap.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp]
     L.myolo_plan_backward_seg_ce.argtypes = [vp, vp, i32, f32, vp, vp, vp]
+    L.myolo_plan_backward_seg_ohem.argtypes = [vp, vp, i32, f32, f32, vp, vp, vp]
+    L.myolo_seg_ohem_loss_workspace_bytes.argtypes = [i32, i32, i32]
+    L.myolo_seg_ohem_loss_workspace_bytes.restype = i64
+    L.myolo_seg_ohem_loss.argtypes = [vp, vp, i32, i32, i32, i32, i32, f32, vp, vp, i64, vp]
+    L.myolo_seg_ohem_loss_backward.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp, vp, i64, vp]
     L.myolo_plan_read_grad_view.argtypes = [vp, View, vp, vp]
     L.myolo_plan_set_seed.argtypes = [vp, C.c_uint64]
     L.myolo_plan_set_defer_running.argtypes = [vp, i32]

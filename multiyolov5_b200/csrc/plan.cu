@@ -167,6 +167,7 @@ struct myolo_plan {
   void* ce_scratch = nullptr;      // 16 bytes for the fused seg loss (valid-pixel count, loss sum)
   float* ce_gbuf = nullptr;        // per-pixel (softmax - onehot), NHWC fp32, of the fused seg loss
   size_t ce_gbuf_bytes = 0;
+  void* ohem_ws = nullptr;         // the OHEM seg loss's selection state and per-pixel losses (ohem_scratch_bytes of B*H*W pixels)
 };
 
 static int resolve_view(const myolo_plan* pl, const myolo_view& v, TensorView* out) {
@@ -311,6 +312,7 @@ extern "C" void myolo_plan_destroy(myolo_plan* pl) {
   if (pl->ce_scratch) cudaFree(pl->ce_scratch);
   if (pl->d_step) cudaFree(pl->d_step);
   if (pl->ce_gbuf) cudaFree(pl->ce_gbuf);
+  if (pl->ohem_ws) cudaFree(pl->ohem_ws);
   if (pl->spp_scratch) cudaFree(pl->spp_scratch);
   delete pl;
 }
@@ -1186,14 +1188,14 @@ extern "C" int myolo_plan_backward(myolo_plan* pl, const float* const* grad_raw,
 
 // fused seg loss (SURVEY.md section 8f rank 3): CE(ignore_index) of the x8-upsampled logits of the last train forward is evaluated and
 // differentiated straight from the low-resolution logits; the backward then runs as the seg pass (seed mask 8)
-extern "C" int myolo_plan_backward_seg_ce(myolo_plan* pl, const int64_t* labels, int ignore_index, float factor, const float* scale_dev,
-                                          float* loss_out, void* stream) {
-  NvtxRange nvtx_("myolo_plan_backward_seg_ce");
+// ohem: OhemCELoss(thresh) with thresh_t = -log(thresh) instead of the mean CE
+static int backward_seg_fused(myolo_plan* pl, const int64_t* labels, int ignore_index, float factor, const float* scale_dev, float* loss_out,
+                              cudaStream_t s, bool ohem, float thresh_t) {
   MYOLO_REQUIRE(pl && pl->train_fwd_done && labels, "backward_seg_ce: call myolo_plan_train_forward first / null labels");
-  cudaStream_t s = (cudaStream_t)stream;
   if (!pl->gws) MYOLO_CHECK_CUDA(cudaMalloc(&pl->gws, pl->ws_bytes));
   MYOLO_CHECK_CUDA(cudaMemsetAsync(pl->gws, 0, pl->ws_bytes, s));
   if (!pl->ce_scratch) MYOLO_CHECK_CUDA(cudaMalloc(&pl->ce_scratch, 16));
+  if (ohem && !pl->ohem_ws) MYOLO_CHECK_CUDA(cudaMalloc(&pl->ohem_ws, ohem_scratch_bytes((long)pl->B * pl->H * pl->W)));   // the plan's shape is fixed
   std::vector<char> live(pl->bufs.size(), 0);
   int rc = MYOLO_E_INVALID;
   for (const auto& op : pl->ops)
@@ -1210,11 +1212,23 @@ extern "C" int myolo_plan_backward_seg_ce(myolo_plan* pl, const int64_t* labels,
         pl->ce_gbuf_bytes = gb;
       }
       rc = launch_seg_ce_fused(lo, op.aux[0], reinterpret_cast<const long long*>(labels), pl->H, pl->W, ignore_index, dlo, factor, scale_dev,
-                               pl->ce_scratch, pl->ce_gbuf, loss_out, s);
+                               pl->ce_scratch, pl->ce_gbuf, loss_out, s, ohem ? pl->ohem_ws : nullptr, thresh_t);
       break;
     }
   if (rc) { if (rc == MYOLO_E_INVALID) set_error("backward_seg_ce: the plan has no segmentation output"); return rc; }
   return backward_run(pl, 8, live, s);
+}
+
+extern "C" int myolo_plan_backward_seg_ce(myolo_plan* pl, const int64_t* labels, int ignore_index, float factor, const float* scale_dev,
+                                          float* loss_out, void* stream) {
+  NvtxRange nvtx_("myolo_plan_backward_seg_ce");
+  return backward_seg_fused(pl, labels, ignore_index, factor, scale_dev, loss_out, (cudaStream_t)stream, false, 0.f);
+}
+
+extern "C" int myolo_plan_backward_seg_ohem(myolo_plan* pl, const int64_t* labels, int ignore_index, float thresh_t, float factor,
+                                            const float* scale_dev, float* loss_out, void* stream) {
+  NvtxRange nvtx_("myolo_plan_backward_seg_ohem");
+  return backward_seg_fused(pl, labels, ignore_index, factor, scale_dev, loss_out, (cudaStream_t)stream, true, thresh_t);
 }
 
 static int backward_walk(myolo_plan* pl, std::vector<char>& live, cudaStream_t s, int* n_ops) {
@@ -1460,6 +1474,32 @@ extern "C" int myolo_adam_scalars(const int32_t* steps, int64_t n, double lr, do
   int rc = check_device(nullptr);
   if (rc) return rc;
   return launch_adam_scalars(steps, (long)n, lr, beta1, beta2, step_size, bc2_sqrt, bc1, bc2, (cudaStream_t)stream);
+}
+
+extern "C" int64_t myolo_seg_ohem_loss_workspace_bytes(int B, int H, int W) { return (int64_t)ohem_scratch_bytes((long)B * H * W); }
+
+extern "C" int myolo_seg_ohem_loss(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index, float thresh_t,
+                                   float* loss_out, void* workspace, int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_seg_ohem_loss");
+  MYOLO_REQUIRE(logits && labels && loss_out && workspace && B > 0 && C > 0 && H > 0 && W > 0, "seg_ohem_loss: bad arguments");
+  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_ohem_loss_workspace_bytes(B, H, W), "seg_ohem_loss: workspace too small");
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_seg_ohem_loss(logits, reinterpret_cast<const long long*>(labels), B, C, H, W, ignore_index, thresh_t, workspace, loss_out,
+                              (cudaStream_t)stream);
+}
+
+extern "C" int myolo_seg_ohem_loss_backward(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index,
+                                            const float* grad_out, float* grad_logits, const void* workspace, int64_t workspace_bytes,
+                                            void* stream) {
+  NvtxRange nvtx_("myolo_seg_ohem_loss_backward");
+  MYOLO_REQUIRE(logits && labels && grad_out && grad_logits && workspace && B > 0 && C > 0 && H > 0 && W > 0,
+                "seg_ohem_loss_backward: bad arguments");
+  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_ohem_loss_workspace_bytes(B, H, W), "seg_ohem_loss_backward: workspace too small");
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_seg_ohem_loss_bwd(logits, reinterpret_cast<const long long*>(labels), B, C, H, W, ignore_index, workspace, grad_out,
+                                  grad_logits, (cudaStream_t)stream);
 }
 
 extern "C" int myolo_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay, void* stream) {

@@ -3,6 +3,7 @@
 // atomics; everything else is plain coalesced CUDA.  Reference semantics: torch.autograd through models/common.py / models/yolo.py
 // in train mode (BatchNorm with batch statistics, eps 1e-3, momentum 0.03: reference utils/torch_utils.py:150-152).
 #include <algorithm>
+#include <climits>
 
 #include "train.h"
 
@@ -875,11 +876,234 @@ __global__ void count_valid_kernel(const long long* __restrict__ labels, long n,
   if ((threadIdx.x & 31) == 0 && c) atomicAdd(out, (unsigned long long)c);
 }
 
+// ------------------------------------------------------------------------------------------------
+// OHEM selection (reference utils/loss.py:321-328 OhemCELoss.forward_once) over a per-pixel CE buffer of n values, on the device and
+// without a host synchronisation.  With n_min = n_valid // 16 and hard = #{loss > thresh_t}:
+//   hard >= n_min: the hard pixels, mean over `hard` (hard == 0 gives 0/0 = NaN and no gradient, as torch.mean of an empty tensor);
+//   otherwise:     the n_min largest losses (ignored pixels take part with loss 0), mean over n_min.  Among the pixels equal to the
+//                  n_min-th largest value the lowest flat indices are taken (torch.topk leaves that order unspecified).
+// The k-th largest value is a radix select over order-preserving 32-bit keys: four 8-bit histogram passes, each followed by a one-block
+// digit pick.  Every kernel is always launched; kernels the batch's branch does not need return after reading `branch`, so one captured
+// graph serves both branches.  A non-finite per-pixel loss makes the loss and every taken gradient NaN (GradScaler then skips the step).
+// ------------------------------------------------------------------------------------------------
+enum { kOhemThresh = 1, kOhemTopk = 2, kOhemNonFinite = 3 };
+constexpr int kOhemChunk = 4096;           // pixels per block of the tie count; the cut kernel walks one chunk with 256 x 16 pixels
+
+struct OhemSel {                           // zeroed before every selection
+  unsigned int hist[4][256];
+  unsigned long long n_valid;              // standalone loss: count_valid_kernel's output
+  unsigned int hard, nonfinite;
+  float hard_sum, gt_sum, thresh_t;
+  int branch;
+  unsigned int prefix;                     // after the four passes: the key of the n_min-th largest loss
+  unsigned int k_rem;                      // pixels still to take among those matching `prefix`
+  unsigned int tie_total;                  // pixels whose key equals the final prefix
+  long long cut;                           // the highest flat index taken among the tied pixels
+  float denom, loss_sum;
+};
+
+__device__ __forceinline__ unsigned ohem_key(float v) {
+  unsigned u = __float_as_uint(v);
+  if (u == 0x80000000u) u = 0u;                                   // -0.0 == +0.0: one key
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float ohem_key_value(unsigned k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7FFFFFFFu) : ~k);
+}
+__device__ __forceinline__ bool ohem_taken(int branch, float thresh_t, unsigned kth, long long cut, long i, float v) {
+  if (branch == kOhemThresh) return v > thresh_t;
+  if (branch == kOhemTopk) {
+    const unsigned k = ohem_key(v);
+    return k > kth || (k == kth && i <= cut);
+  }
+  return branch == kOhemNonFinite;
+}
+__device__ __forceinline__ float ohem_coef(const OhemSel* st, float num) { return st->denom == 0.f ? 0.f : num / st->denom; }
+
+// inclusive prefix sum over a 256-thread block; sh: 8 words of shared memory
+__device__ unsigned block_scan256(unsigned v, unsigned* sh) {
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (int o = 1; o < 32; o <<= 1) {
+    const unsigned u = __shfl_up_sync(0xFFFFFFFFu, v, o);
+    if (lane >= o) v += u;
+  }
+  if (lane == 31) sh[w] = v;
+  __syncthreads();
+  for (int i = 0; i < w; ++i) v += sh[i];
+  __syncthreads();
+  return v;
+}
+
+// pass p: histogram of key digit (31-8p .. 24-8p) over the pixels whose higher digits match the prefix; pass 0 also counts the hard pixels
+__global__ void __launch_bounds__(256) ohem_hist_kernel(const float* __restrict__ loss, long n, OhemSel* st, int pass, float thresh_t) {
+  if (pass > 0 && st->branch != kOhemTopk) return;
+  __shared__ unsigned cnt[256];
+  cnt[threadIdx.x] = 0;
+  __syncthreads();
+  const int shift = 24 - 8 * pass;
+  const unsigned mask = pass ? 0xFFFFFFFFu << (32 - 8 * pass) : 0u, prefix = pass ? st->prefix : 0u;
+  unsigned hard = 0, bad = 0;
+  float hsum = 0.f;
+  for (long base = (long)blockIdx.x * blockDim.x; base < n; base += (long)gridDim.x * blockDim.x) {    // warp-uniform trip count
+    const long i = base + threadIdx.x;
+    const float v = i < n ? loss[i] : 0.f;
+    const unsigned k = ohem_key(v);
+    const int d = (i < n && (k & mask) == prefix) ? (int)((k >> shift) & 255u) : 256;
+    const unsigned peers = __match_any_sync(0xFFFFFFFFu, d);
+    if (d < 256 && (int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&cnt[d], (unsigned)__popc(peers));
+    if (pass == 0 && i < n) {
+      if (v > thresh_t) { ++hard; hsum += v; }
+      bad |= !isfinite(v);
+    }
+  }
+  if (pass == 0) {
+    hard = __reduce_add_sync(0xFFFFFFFFu, hard);
+    bad = __reduce_or_sync(0xFFFFFFFFu, bad);
+    hsum = warp_sum(hsum);
+    if ((threadIdx.x & 31) == 0) {
+      if (hard) { atomicAdd(&st->hard, hard); atomicAdd(&st->hard_sum, hsum); }
+      if (bad) atomicOr(&st->nonfinite, 1u);
+    }
+  }
+  __syncthreads();
+  if (cnt[threadIdx.x]) atomicAdd(&st->hist[pass][threadIdx.x], cnt[threadIdx.x]);
+}
+
+// one block: pass 0 decides the branch; every pass of the top-k branch then picks the digit of the k-th largest key
+__global__ void __launch_bounds__(256) ohem_pick_kernel(OhemSel* st, const unsigned long long* __restrict__ n_valid, int pass, float thresh_t) {
+  __shared__ unsigned sh[8];
+  unsigned k, prefix;
+  if (pass == 0) {
+    const unsigned long long n_min = *n_valid / 16;
+    const unsigned hard = st->hard;
+    int branch = kOhemTopk;
+    if (st->nonfinite) branch = kOhemNonFinite;
+    else if (hard >= n_min) branch = kOhemThresh;
+    if (threadIdx.x == 0) {
+      st->branch = branch;
+      st->thresh_t = thresh_t;
+      st->denom = branch == kOhemNonFinite ? NAN : branch == kOhemThresh ? (float)hard : (float)n_min;
+      st->loss_sum = branch == kOhemNonFinite ? NAN : st->hard_sum;     // the top-k sum is written by ohem_cut_kernel
+    }
+    if (branch != kOhemTopk) return;
+    k = (unsigned)n_min;
+    prefix = 0u;
+  } else {
+    if (st->branch != kOhemTopk) return;
+    k = st->k_rem;
+    prefix = st->prefix;
+  }
+  const int d = 255 - (int)threadIdx.x;                                 // digits in descending order
+  const unsigned c = st->hist[pass][d];
+  const unsigned incl = block_scan256(c, sh);
+  if (incl >= k && incl - c < k) {                                       // exactly one thread: k >= 1 and the digits hold >= k keys
+    st->prefix = prefix | (unsigned)d << (24 - 8 * pass);
+    st->k_rem = k - (incl - c);
+    if (pass == 3) st->tie_total = c;
+  }
+}
+
+// top-k branch: per chunk, the pixels tied at the k-th key; and the sum of the losses above it
+__global__ void __launch_bounds__(256) ohem_tie_kernel(const float* __restrict__ loss, long n, OhemSel* st, unsigned* __restrict__ chunk_ties) {
+  if (st->branch != kOhemTopk) return;
+  __shared__ unsigned sh[8];
+  const unsigned kth = st->prefix;
+  const long lo = (long)blockIdx.x * kOhemChunk, hi = min(n, lo + kOhemChunk);
+  unsigned ties = 0;
+  float s = 0.f;
+  for (long i = lo + threadIdx.x; i < hi; i += blockDim.x) {
+    const float v = loss[i];
+    const unsigned k = ohem_key(v);
+    ties += k == kth;
+    if (k > kth) s += v;
+  }
+  s = warp_sum(s);
+  if ((threadIdx.x & 31) == 0 && s != 0.f) atomicAdd(&st->gt_sum, s);
+  ties = block_scan256(ties, sh);
+  if (threadIdx.x == 255) chunk_ties[blockIdx.x] = ties;
+}
+
+// top-k branch, one block: the loss sum, and the index cutoff among the tied pixels when fewer than all of them are taken
+__global__ void __launch_bounds__(256) ohem_cut_kernel(const float* __restrict__ loss, long n, OhemSel* st, const unsigned* __restrict__ chunk_ties,
+                                                       int n_chunks) {
+  if (st->branch != kOhemTopk) return;
+  __shared__ unsigned sh[8];
+  __shared__ int s_chunk;
+  __shared__ unsigned s_r, s_total;
+  const unsigned kth = st->prefix, need = st->k_rem;
+  if (threadIdx.x == 0) {
+    st->loss_sum = st->gt_sum + (float)need * ohem_key_value(kth);
+    st->cut = LLONG_MAX;
+    s_chunk = -1;
+  }
+  if (st->tie_total == need) return;
+  __syncthreads();
+  // the chunk holding the need-th tied pixel, then that pixel within it
+  unsigned before = 0;
+  for (int c0 = 0; c0 < n_chunks; c0 += 256) {
+    const unsigned c = c0 + (int)threadIdx.x < n_chunks ? chunk_ties[c0 + threadIdx.x] : 0u;
+    const unsigned incl = before + block_scan256(c, sh);
+    if (c && incl >= need && incl - c < need) { s_chunk = c0 + threadIdx.x; s_r = need - (incl - c); }
+    if (threadIdx.x == 255) s_total = incl;
+    __syncthreads();
+    if (s_chunk >= 0) break;
+    before = s_total;
+    __syncthreads();
+  }
+  if (s_chunk < 0) return;                 // unreachable: the chunk counts add up to tie_total > need
+  const long lo = (long)s_chunk * kOhemChunk + threadIdx.x * (kOhemChunk / 256), hi = min(n, lo + kOhemChunk / 256);
+  unsigned c = 0;
+  for (long i = lo; i < hi; ++i) c += ohem_key(loss[i]) == kth;
+  const unsigned incl = block_scan256(c, sh), r = s_r;
+  if (c && incl >= r && incl - c < r) {
+    unsigned left = r - (incl - c);
+    for (long i = lo; i < hi; ++i)
+      if (ohem_key(loss[i]) == kth && --left == 0) { st->cut = i; break; }
+  }
+}
+
+static int ohem_select(const float* loss, long n, const unsigned long long* n_valid, float thresh_t, OhemSel* st, unsigned* chunk_ties,
+                       cudaStream_t s) {
+  const int n_chunks = (int)((n + kOhemChunk - 1) / kOhemChunk);
+  for (int pass = 0; pass < 4; ++pass) {
+    ohem_hist_kernel<<<grid_for_t(n, 256, 132 * 4), 256, 0, s>>>(loss, n, st, pass, thresh_t);
+    MYOLO_LAUNCH_CHECK();
+    ohem_pick_kernel<<<1, 256, 0, s>>>(st, n_valid, pass, thresh_t);
+    MYOLO_LAUNCH_CHECK();
+  }
+  ohem_tie_kernel<<<n_chunks, 256, 0, s>>>(loss, n, st, chunk_ties);
+  MYOLO_LAUNCH_CHECK();
+  ohem_cut_kernel<<<1, 256, 0, s>>>(loss, n, st, chunk_ties, n_chunks);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+static size_t align256(size_t b) { return (b + 255) / 256 * 256; }
+// workspace: [OhemSel][per-chunk tie counts][per-pixel loss, n floats]
+size_t ohem_scratch_bytes(long n) {
+  return align256(sizeof(OhemSel)) + align256((size_t)((n + kOhemChunk - 1) / kOhemChunk) * sizeof(unsigned)) + (size_t)n * sizeof(float);
+}
+struct OhemScratch {
+  OhemSel* st;
+  unsigned* ties;
+  float* loss;
+  size_t head;                             // bytes before the loss buffer (zeroed per call)
+};
+static OhemScratch ohem_scratch(void* ws, long n) {
+  unsigned char* p = reinterpret_cast<unsigned char*>(ws);
+  const size_t a = align256(sizeof(OhemSel)), b = align256((size_t)((n + kOhemChunk - 1) / kOhemChunk) * sizeof(unsigned));
+  return {reinterpret_cast<OhemSel*>(p), reinterpret_cast<unsigned*>(p + a), reinterpret_cast<float*>(p + a + b), a + b};
+}
+
+__global__ void ohem_finalize_kernel(const OhemSel* st, float* loss_out) {
+  if (loss_out) *loss_out = st->loss_sum / st->denom;
+}
+
 // pass 1: one thread per FULL-resolution pixel: interpolated logits from the 4 low-res neighbours -> softmax -> (p - onehot) written as
-// NC_PAD fp32 per pixel (zeros for ignored pixels); the pixel's loss is reduced per warp.
+// NC_PAD fp32 per pixel (zeros for ignored pixels); the pixel's loss is reduced per warp, and written to pix_loss (OHEM, nullable).
 template <int NC, int NC_PAD>
 __global__ void seg_ce_pixel_kernel(TensorView lo, const long long* __restrict__ labels, int H, int W, int ignore_index, float* __restrict__ g,
-                                    float* loss_sum) {
+                                    float* loss_sum, float* __restrict__ pix_loss) {
   const long total = (long)lo.B * H * W;
   float loss_local = 0.f;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -887,7 +1111,7 @@ __global__ void seg_ce_pixel_kernel(TensorView lo, const long long* __restrict__
     const int Y = (int)((i / W) % H);
     const int b = (int)(i / ((long)W * H));
     const long long t = labels[i];
-    float v[NC_PAD];
+    float v[NC_PAD], l = 0.f;
 #pragma unroll
     for (int c = 0; c < NC_PAD; ++c) v[c] = 0.f;
     if (t != ignore_index && t >= 0 && t < NC) {
@@ -906,8 +1130,10 @@ __global__ void seg_ce_pixel_kernel(TensorView lo, const long long* __restrict__
       const float inv = 1.0f / ssum;
 #pragma unroll
       for (int c = 0; c < NC; ++c) v[c] = v[c] * inv - (c == (int)t ? 1.0f : 0.f);
-      loss_local += __logf(ssum) + m - zt;
+      l = __logf(ssum) + m - zt;
+      loss_local += l;
     }
+    if (pix_loss) pix_loss[i] = l;
     float4* dst = reinterpret_cast<float4*>(g + (size_t)i * NC_PAD);
 #pragma unroll
     for (int c = 0; c < NC_PAD; c += 4) dst[c / 4] = make_float4(v[c], v[c + 1], v[c + 2], v[c + 3]);
@@ -916,13 +1142,26 @@ __global__ void seg_ce_pixel_kernel(TensorView lo, const long long* __restrict__
   if ((threadIdx.x & 31) == 0 && loss_local != 0.f) atomicAdd(loss_sum, loss_local);
 }
 
-// pass 2: adjoint of the bilinear upsample, gathered per low-res pixel (x a chunk of its footprint rows) from the per-pixel gradients
+// pass 2: adjoint of the bilinear upsample, gathered per low-res pixel (x a chunk of its footprint rows) from the per-pixel gradients.
+// OHEM (sel non-null): only the pixels the selection took contribute, and the denominator is the selection's.
 template <int NC, int NC_PAD>
 __global__ void seg_ce_gather_kernel(const float* __restrict__ g, int H, int W, TensorView dlo, float factor, const float* __restrict__ scale_dev,
-                                     const unsigned long long* __restrict__ n_valid, int rsplit) {
+                                     const unsigned long long* __restrict__ n_valid, int rsplit, const OhemSel* __restrict__ sel,
+                                     const float* __restrict__ pix_loss) {
   const long total = (long)dlo.B * dlo.H * dlo.W * rsplit;
-  const unsigned long long nv = *n_valid;
-  const float coef = nv ? factor * (scale_dev ? *scale_dev : 1.0f) / (float)nv : 0.f;
+  const float num = factor * (scale_dev ? *scale_dev : 1.0f);
+  float coef;
+  int branch = 0;
+  float thresh_t = 0.f;
+  unsigned kth = 0;
+  long long cut = 0;
+  if (sel) {
+    coef = ohem_coef(sel, num);
+    branch = sel->branch; thresh_t = sel->thresh_t; kth = sel->prefix; cut = sel->cut;
+  } else {
+    const unsigned long long nv = *n_valid;
+    coef = nv ? num / (float)nv : 0.f;
+  }
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int part = (int)(i % rsplit);
     long p = i / rsplit;
@@ -948,6 +1187,10 @@ __global__ void seg_ce_gather_kernel(const float* __restrict__ g, int H, int W, 
         lerp_src(X, dlo.W, W, &b0, &b1, &v0, &v1);
         const float wgt = wy * ((b0 == x ? v0 : 0.f) + (b1 == x ? v1 : 0.f));
         if (wgt == 0.f) continue;
+        if (sel) {
+          const long pix = ((long)b * H + Y) * W + X;
+          if (!ohem_taken(branch, thresh_t, kth, cut, pix, pix_loss[pix])) continue;
+        }
         const float4* q = reinterpret_cast<const float4*>(row + (size_t)X * NC_PAD);
 #pragma unroll
         for (int c = 0; c < NC_PAD; c += 4) {
@@ -970,32 +1213,107 @@ __global__ void seg_ce_finalize_kernel(const float* loss_sum, const unsigned lon
 size_t seg_ce_scratch_bytes(int B, int H, int W, int n_cls) { return (size_t)B * H * W * (n_cls <= 20 ? 20 : 32) * sizeof(float); }
 
 // scratch16: 16 bytes (n_valid u64, loss_sum f32); gbuf: seg_ce_scratch_bytes.  loss_out (device, nullable) receives the mean CE.
+// ohem_ws (nullable): ohem_scratch_bytes(B*H*W) bytes; the loss becomes OhemCELoss(thresh) with thresh_t = -log(thresh).
 int launch_seg_ce_fused(const TensorView& lo, int n_cls, const long long* labels, int H, int W, int ignore_index, const TensorView& dlo,
-                        float factor, const float* scale_dev, void* scratch16, float* gbuf, float* loss_out, cudaStream_t s) {
+                        float factor, const float* scale_dev, void* scratch16, float* gbuf, float* loss_out, cudaStream_t s, void* ohem_ws,
+                        float thresh_t) {
   MYOLO_REQUIRE(lo.dtype == MYOLO_F32 && dlo.dtype == MYOLO_F32 && n_cls >= 1 && n_cls <= 32 && lo.C >= n_cls && labels && scratch16 && gbuf,
                 "seg_ce_fused: fp32 low-resolution logits with <= 32 classes expected");
+  MYOLO_REQUIRE(n_cls == 19 || n_cls == 32, "seg_ce_fused: instantiate the kernels for %d classes (19 and 32 are built)", n_cls);
   unsigned long long* n_valid = reinterpret_cast<unsigned long long*>(scratch16);
   float* loss_sum = reinterpret_cast<float*>(n_valid + 1);
   MYOLO_CHECK_CUDA(cudaMemsetAsync(scratch16, 0, 16, s));
   const long n = (long)lo.B * H * W;
+  OhemScratch oh{nullptr, nullptr, nullptr, 0};
+  if (ohem_ws) {
+    oh = ohem_scratch(ohem_ws, n);
+    MYOLO_CHECK_CUDA(cudaMemsetAsync(ohem_ws, 0, oh.head, s));
+  }
   count_valid_kernel<<<grid_for_t(n, 256, 132 * 8), 256, 0, s>>>(labels, n, ignore_index, n_cls, n_valid);
   MYOLO_LAUNCH_CHECK();
   const int rsplit = 4;
   const int g1 = grid_for_t(n, 128), g2 = grid_for_t((long)lo.B * lo.H * lo.W * rsplit, 128);
-  if (n_cls == 19) {
-    seg_ce_pixel_kernel<19, 20><<<g1, 128, 0, s>>>(lo, labels, H, W, ignore_index, gbuf, loss_sum);
-    MYOLO_LAUNCH_CHECK();
-    seg_ce_gather_kernel<19, 20><<<g2, 128, 0, s>>>(gbuf, H, W, dlo, factor, scale_dev, n_valid, rsplit);
-  } else if (n_cls <= 20) {
-    MYOLO_REQUIRE(false, "seg_ce_fused: instantiate the kernels for %d classes (19 and 21..32 are built)", n_cls);
-  } else {
-    MYOLO_REQUIRE(n_cls == 32, "seg_ce_fused: instantiate the kernels for %d classes (19 and 32 are built)", n_cls);
-    seg_ce_pixel_kernel<32, 32><<<g1, 128, 0, s>>>(lo, labels, H, W, ignore_index, gbuf, loss_sum);
-    MYOLO_LAUNCH_CHECK();
-    seg_ce_gather_kernel<32, 32><<<g2, 128, 0, s>>>(gbuf, H, W, dlo, factor, scale_dev, n_valid, rsplit);
-  }
+  if (n_cls == 19) seg_ce_pixel_kernel<19, 20><<<g1, 128, 0, s>>>(lo, labels, H, W, ignore_index, gbuf, loss_sum, oh.loss);
+  else seg_ce_pixel_kernel<32, 32><<<g1, 128, 0, s>>>(lo, labels, H, W, ignore_index, gbuf, loss_sum, oh.loss);
   MYOLO_LAUNCH_CHECK();
-  seg_ce_finalize_kernel<<<1, 1, 0, s>>>(loss_sum, n_valid, loss_out);
+  if (ohem_ws)
+    if (int rc = ohem_select(oh.loss, n, n_valid, thresh_t, oh.st, oh.ties, s)) return rc;
+  if (n_cls == 19) seg_ce_gather_kernel<19, 20><<<g2, 128, 0, s>>>(gbuf, H, W, dlo, factor, scale_dev, n_valid, rsplit, oh.st, oh.loss);
+  else seg_ce_gather_kernel<32, 32><<<g2, 128, 0, s>>>(gbuf, H, W, dlo, factor, scale_dev, n_valid, rsplit, oh.st, oh.loss);
+  MYOLO_LAUNCH_CHECK();
+  if (ohem_ws) ohem_finalize_kernel<<<1, 1, 0, s>>>(oh.st, loss_out);
+  else seg_ce_finalize_kernel<<<1, 1, 0, s>>>(loss_sum, n_valid, loss_out);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---- OhemCELoss over full-resolution NCHW fp32 logits of any class count (the standalone module: utils.loss.OhemCELoss) ----
+__global__ void ohem_ce_nchw_kernel(const float* __restrict__ x, const long long* __restrict__ labels, int B, int C, long HW, int ignore_index,
+                                    float* __restrict__ loss) {
+  const long n = (long)B * HW;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const long long t = labels[i];
+    float l = 0.f;
+    if (t != ignore_index && t >= 0 && t < C) {
+      const float* xp = x + (size_t)(i / HW) * C * HW + i % HW;
+      float m = -INFINITY;
+      for (int c = 0; c < C; ++c) m = fmaxf(m, xp[(size_t)c * HW]);
+      float s = 0.f;
+      for (int c = 0; c < C; ++c) s += expf(xp[(size_t)c * HW] - m);
+      l = logf(s) + m - xp[(size_t)t * HW];
+    }
+    loss[i] = l;
+  }
+}
+
+// dx = grad_out * taken * (softmax - onehot) / denominator; pixels the selection did not take get 0
+__global__ void ohem_ce_nchw_bwd_kernel(const float* __restrict__ x, const long long* __restrict__ labels, int B, int C, long HW, int ignore_index,
+                                        const float* __restrict__ pix_loss, const OhemSel* __restrict__ sel, const float* __restrict__ grad_out,
+                                        float* __restrict__ dx) {
+  const long n = (long)B * HW;
+  const float coef = ohem_coef(sel, *grad_out);
+  const int branch = sel->branch;
+  const float thresh_t = sel->thresh_t;
+  const unsigned kth = sel->prefix;
+  const long long cut = sel->cut;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const long long t = labels[i];
+    const size_t base = (size_t)(i / HW) * C * HW + i % HW;
+    const float* xp = x + base;
+    float* dp = dx + base;
+    if (t == ignore_index || t < 0 || t >= C || !ohem_taken(branch, thresh_t, kth, cut, i, pix_loss[i])) {
+      for (int c = 0; c < C; ++c) dp[(size_t)c * HW] = 0.f;
+      continue;
+    }
+    float m = -INFINITY;
+    for (int c = 0; c < C; ++c) m = fmaxf(m, xp[(size_t)c * HW]);
+    float s = 0.f;
+    for (int c = 0; c < C; ++c) s += expf(xp[(size_t)c * HW] - m);
+    const float inv = 1.0f / s;
+    for (int c = 0; c < C; ++c) dp[(size_t)c * HW] = coef * (expf(xp[(size_t)c * HW] - m) * inv - (c == (int)t ? 1.0f : 0.f));
+  }
+}
+
+int launch_seg_ohem_loss(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, float thresh_t, void* ws,
+                         float* loss_out, cudaStream_t s) {
+  const long n = (long)B * H * W;
+  OhemScratch oh = ohem_scratch(ws, n);
+  MYOLO_CHECK_CUDA(cudaMemsetAsync(ws, 0, oh.head, s));
+  count_valid_kernel<<<grid_for_t(n, 256, 132 * 8), 256, 0, s>>>(labels, n, ignore_index, C, &oh.st->n_valid);
+  MYOLO_LAUNCH_CHECK();
+  ohem_ce_nchw_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, labels, B, C, (long)H * W, ignore_index, oh.loss);
+  MYOLO_LAUNCH_CHECK();
+  if (int rc = ohem_select(oh.loss, n, &oh.st->n_valid, thresh_t, oh.st, oh.ties, s)) return rc;
+  ohem_finalize_kernel<<<1, 1, 0, s>>>(oh.st, loss_out);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+int launch_seg_ohem_loss_bwd(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const void* ws,
+                             const float* grad_out, float* dx, cudaStream_t s) {
+  const long n = (long)B * H * W;
+  OhemScratch oh = ohem_scratch(const_cast<void*>(ws), n);
+  ohem_ce_nchw_bwd_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, labels, B, C, (long)H * W, ignore_index, oh.loss, oh.st, grad_out, dx);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }

@@ -79,10 +79,19 @@ int launch_region_combine_bwd(const TensorView& dbins, const TensorView& datoms,
 // seg head: d(low-res logits fp32 NHWC) += adjoint of the final bilinear applied to dseg (B,C,H,W) fp32
 int launch_seg_upsample_bwd(const float* dseg, int n_cls, int H, int W, const TensorView& dlo, cudaStream_t s);
 // fused CE(ignore_index) of the bilinear-upsampled low-res logits: seeds d(low-res logits) += factor * (*scale_dev) * d(mean CE)/d(lo)
-// and writes the mean CE to loss_out (device, nullable); scratch16 = 16 bytes of device scratch
+// and writes the mean CE to loss_out (device, nullable); scratch16 = 16 bytes of device scratch.  With ohem_ws (ohem_scratch_bytes(B*H*W)
+// bytes) the loss is OhemCELoss's instead: the pixels a device-side selection takes (loss > thresh_t, or the n_valid // 16 largest)
 size_t seg_ce_scratch_bytes(int B, int H, int W, int n_cls);
+size_t ohem_scratch_bytes(long n_pixels);
 int launch_seg_ce_fused(const TensorView& lo, int n_cls, const long long* labels, int H, int W, int ignore_index, const TensorView& dlo,
-                        float factor, const float* scale_dev, void* scratch16, float* gbuf, float* loss_out, cudaStream_t s);
+                        float factor, const float* scale_dev, void* scratch16, float* gbuf, float* loss_out, cudaStream_t s,
+                        void* ohem_ws = nullptr, float thresh_t = 0.f);
+// OhemCELoss over full-resolution (B,C,H,W) fp32 logits: the forward leaves its selection in ws (ohem_scratch_bytes(B*H*W) bytes), the
+// backward reads it and writes dx = *grad_out * d(loss)/dx
+int launch_seg_ohem_loss(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, float thresh_t, void* ws,
+                         float* loss_out, cudaStream_t s);
+int launch_seg_ohem_loss_bwd(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const void* ws,
+                             const float* grad_out, float* dx, cudaStream_t s);
 // Detect: d(conv out fp32 NHWC)[b,y,x,a*no+o] = draw[b,a,y,x,o]
 int launch_detect_raw_bwd(const float* draw, int na, int no, const TensorView& dconv, cudaStream_t s);
 int launch_cast_f32_to_f16(const TensorView& src, const TensorView& dst, cudaStream_t s);

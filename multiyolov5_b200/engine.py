@@ -410,6 +410,17 @@ class Engine:
                                                          _lib.ptr(scale), _lib.ptr(loss), _lib.stream_ptr()))
         return loss
 
+    def train_backward_seg_ohem(self, plan, labels, thresh_t, factor=1.0, scale=None, ignore_index=-1):
+        """train_backward_seg_ce with the reference's OhemCELoss in place of the mean CE (myolo_plan_backward_seg_ohem): the pixels whose
+        CE exceeds thresh_t (= -log(thresh), utils.loss.OhemCELoss.thresh_t), or the (valid pixels // 16) largest when fewer are hard, chosen
+        on the device.  Returns the OHEM loss (device scalar)."""
+        assert labels.is_cuda and labels.dtype == torch.int64 and tuple(labels.shape) == (plan.B, plan.H, plan.W)
+        self._check_generation(plan, None)
+        loss = torch.empty((), dtype=torch.float32, device=labels.device)
+        _lib.check(_lib.lib().myolo_plan_backward_seg_ohem(plan.handle, _lib.ptr(labels.contiguous()), int(ignore_index), float(thresh_t),
+                                                           float(factor), _lib.ptr(scale), _lib.ptr(loss), _lib.stream_ptr()))
+        return loss
+
     def read_grad_view(self, v, plan=None):
         """debug: NHWC slice of the gradient workspace -> (B,C,H,W) fp32 torch tensor"""
         p = plan or self.last_plan

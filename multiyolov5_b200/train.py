@@ -19,6 +19,9 @@ optimiser buffers to and from torch's `optimizer.state_dict()` format, which is 
 skipped for overflow: one launch (`myolo_ema_update`) over every floating-point entry of the model, bit-identical with the reference's
 per-entry statements.  Pass it on rank -1 / 0 and None elsewhere, as train.py:151 builds it.
 
+`Trainer(..., seg_loss=OhemCELoss(0.7))` trains with the reference's OHEM segmentation loss (train.py:285-288) in place of
+SegmentationLosses.
+
 `Trainer(..., quad=True)` is the reference's `--quad`: det batches from `utils.datasets.collate_quad` (collate_fn4) and the det loss x 4
 (train.py:368-369).
 
@@ -39,7 +42,7 @@ import torch.nn as nn
 from . import _lib
 from .engine import flat_offsets
 from .parallel import allreduce_flat_grads, bn_sync_group
-from .utils.loss import FusedComputeLoss, SegmentationLosses
+from .utils.loss import FusedComputeLoss, OhemCELoss, SegmentationLosses
 
 
 def scale_hyp(hyp: dict, nl: int, nc: int, imgsz: int, total_batch_size: int, nbs: int = 64, label_smoothing: float = 0.0) -> dict:
@@ -298,7 +301,8 @@ class Trainer:
     """`Trainer(model, hyp, batch_size).step(imgs, targets, segimgs, segtargets)`; hyp already scaled (see scale_hyp)."""
 
     def __init__(self, model, hyp, batch_size, world_size=1, rank=-1, accumulate=1, detgain=0.6, seggain=0.35, init_scale=2.0 ** 16,
-                 growth_interval=2000, process_group=None, multi_scale=None, det_shapes=None, optimizer="sgd", ema=None, quad=False):
+                 growth_interval=2000, process_group=None, multi_scale=None, det_shapes=None, optimizer="sgd", ema=None, quad=False,
+                 seg_loss=None):
         """multi_scale: a MultiScale.  The det lane's train plans for every size it can draw from an imgsz x imgsz batch are reserved on
         one shared workspace (Engine.reserve_train_shapes); rescale each det batch with `multi_scale(imgs)` before `step`, as the reference
         does before its forward (train.py:354-359).  A det batch of fewer images (the loader's partial last batch) reserves its sizes on
@@ -314,11 +318,21 @@ class Trainer:
         height and width, and the det loss is multiplied by 4 (train.py:368-369).  The reserved det plans (multi_scale / det_shapes) are
         for batch_size // 4 images at the doubled shapes, with multi_scale every size it can draw from them.  The seg pass and its
         batch_size factor are unchanged (train.py:385).  The reference's loop skips a det batch of one image (train.py:338), so with quad
-        a per-GPU batch_size below 8 never trains; the Trainer steps whatever it is given."""
+        a per-GPU batch_size below 8 never trains; the Trainer steps whatever it is given.
+        seg_loss: None (SegmentationLosses, as the reference's default) or a utils.loss.OhemCELoss, multiplied by batch_size * seggain
+        like the default (train.py:385-391).  On a plain head with 19 or 32 classes it runs in the fused upsample + CE kernels; on any other
+        head through autograd on the model's full-resolution outputs.  Its aux must match the head: aux=True for BiSe's three outputs
+        only (ValueError otherwise)."""
         if optimizer not in OPTIMIZER_STATE:
             raise ValueError(f"optimizer must be 'sgd' or 'adam', got {optimizer!r}")
         if quad and batch_size < 4:
             raise ValueError(f"quad: a batch of {batch_size} images has no quad (collate_fn4 needs at least 4)")
+        if seg_loss is not None and not isinstance(seg_loss, OhemCELoss):
+            raise ValueError(f"seg_loss must be None or a utils.loss.OhemCELoss, got {type(seg_loss).__name__}")
+        n_seg_outputs = 3 if type(model.model[-2]).__name__ == "SegMaskBiSe" else 1
+        if seg_loss is not None and seg_loss.aux != (n_seg_outputs == 3):
+            raise ValueError(f"OhemCELoss(aux={seg_loss.aux}) does not fit a seg head with {n_seg_outputs} output(s): aux=True is for "
+                             "the BiSe head's [out, aux16, aux32]")
         assert next(model.parameters()).is_cuda, "model.cuda() first"
         self.model, self.hyp, self.batch_size = model, hyp, batch_size
         self.world_size, self.rank, self.accumulate, self.pg = world_size, rank, accumulate, process_group
@@ -330,9 +344,10 @@ class Trainer:
         # positive weights / autobalance take the torch formulation (compute_loss), replayed as one captured CUDA graph (_det_graph)
         self._fused_det = FusedComputeLoss(model)
         self.compute_loss = self._fused_det.ref
-        self.n_seg_outputs = 3 if type(model.model[-2]).__name__ == "SegMaskBiSe" else 1
+        self.n_seg_outputs = n_seg_outputs
         # BiSe returns [out, aux16, aux32]: loss1 + 1.5*aux_weight*loss2 + 0.5*aux_weight*loss3 (reference train.py:387-388, utils/loss.py:239-244)
         self.compute_seg_loss = SegmentationLosses(ignore_index=-1, aux=self.n_seg_outputs == 3, aux_num=2)
+        self.ohem = seg_loss                   # an OhemCELoss in place of compute_seg_loss, or None
         # seg CE + x8 upsample forward / backward in one kernel, no full-resolution logits: plain heads with 19 (Cityscapes) or 32 classes,
         # the instantiations in csrc/train.cu; other heads take autograd
         self.fused_seg = self.n_seg_outputs == 1 and model.model[-2].c_out in (19, 32)
@@ -488,15 +503,23 @@ class Trainer:
 
     def _seg_ce_backward(self, plan, segtargets):
         f = self.batch_size * self.seggain                                                   # train.py:385-391
-        return self.model.engine().train_backward_seg_ce(plan, segtargets, factor=f, scale=self.scale) * f
+        eng = self.model.engine()
+        if self.ohem is not None:
+            return eng.train_backward_seg_ohem(plan, segtargets, self.ohem.thresh_t, factor=f, scale=self.scale,
+                                               ignore_index=self.ohem.ignore_index) * f
+        return eng.train_backward_seg_ce(plan, segtargets, factor=f, scale=self.scale) * f
 
     def backward_seg(self, segimgs, segtargets):
         if self.fused_seg:
             _, _, plan = self.model.engine().train_forward(segimgs, want_seg=False)
             return self._seg_ce_backward(plan, segtargets)
         pred = self.model(segimgs)
-        outs = pred[1] if isinstance(pred[1], list) else [pred[1]]
-        segloss = self.compute_seg_loss(*outs, segtargets) * self.batch_size * self.seggain   # train.py:385-391
+        if self.ohem is not None:
+            loss = self.ohem(pred[1], segtargets)                   # the reference's call: the output, or the list of BiSe's three
+        else:
+            outs = pred[1] if isinstance(pred[1], list) else [pred[1]]
+            loss = self.compute_seg_loss(*outs, segtargets)
+        segloss = loss * self.batch_size * self.seggain                                     # train.py:385-391
         (segloss * self.scale).backward()
         return segloss.detach()
 

@@ -1,5 +1,5 @@
-"""Training losses behind the reference's surface: `ComputeLoss(model)(p, targets)` (reference utils/loss.py:89-217) and
-`SegmentationLosses` (:221-262).  They consume the train-mode outputs of `Model.forward` ([x_i (B,na,ny,nx,5+nc)] and seg logits)
+"""Training losses behind the reference's surface: `ComputeLoss(model)(p, targets)` (reference utils/loss.py:89-217),
+`SegmentationLosses` (:221-262) and `OhemCELoss` (:303-328).  They consume the train-mode outputs of `Model.forward` ([x_i (B,na,ny,nx,5+nc)] and seg logits)
 and, through torch.autograd, seed the hand-written backward of the network (engine._TrainFunction).
 
 Design notes (not a transcription of the reference):
@@ -234,3 +234,77 @@ class SegmentationLosses(nn.CrossEntropyLoss):
         assert self.aux_num == 1
         p1, p2 = preds
         return ce(p1, target) + self.aux_weight * ce(p2, target)
+
+
+def ohem_thresh_t(thresh):
+    """-log(thresh) as the reference's OhemCELoss computes it: in fp32 by torch (utils/loss.py:306).  ValueError outside (0, 1]: above 1
+    the threshold is negative and the reference would average the ignored pixels (CE 0) into the loss."""
+    thresh = float(thresh)
+    if not 0.0 < thresh <= 1.0:
+        raise ValueError(f"OhemCELoss: thresh must lie in (0, 1], got {thresh}")
+    return float(-torch.log(torch.tensor(thresh, dtype=torch.float32)))
+
+
+class _OhemCE(torch.autograd.Function):
+    """OhemCELoss.forward_once on the library (myolo_seg_ohem_loss / _backward): the selection stays on the device between the passes"""
+
+    @staticmethod
+    def forward(ctx, pred, labels, thresh_t, ignore_index):
+        from .. import _lib
+        B, Cc, H, W = pred.shape
+        L = _lib.lib()
+        need = int(L.myolo_seg_ohem_loss_workspace_bytes(B, H, W))
+        ws = torch.empty(need, dtype=torch.uint8, device=pred.device)
+        loss = torch.empty((), dtype=torch.float32, device=pred.device)
+        _lib.check(L.myolo_seg_ohem_loss(_lib.ptr(pred), _lib.ptr(labels), B, Cc, H, W, int(ignore_index), float(thresh_t), _lib.ptr(loss),
+                                         _lib.ptr(ws), need, _lib.stream_ptr()))
+        ctx.save_for_backward(pred, labels)
+        ctx.ws, ctx.ignore_index = ws, int(ignore_index)
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from .. import _lib
+        pred, labels = ctx.saved_tensors
+        B, Cc, H, W = pred.shape
+        g = grad_out.float().contiguous()
+        dx = torch.empty_like(pred)
+        _lib.check(_lib.lib().myolo_seg_ohem_loss_backward(_lib.ptr(pred), _lib.ptr(labels), B, Cc, H, W, ctx.ignore_index, _lib.ptr(g),
+                                                           _lib.ptr(dx), _lib.ptr(ctx.ws), ctx.ws.numel(), _lib.stream_ptr()))
+        return dx, None, None, None
+
+
+class OhemCELoss(nn.Module):
+    """The reference's OhemCELoss (utils/loss.py:303-328): per pixel CE(ignore_index); the pixels with CE > -log(thresh), or the
+    (valid pixels // 16) largest CEs when fewer are that hard, averaged.  With aux=True, preds is [out, aux16, aux32] (the BiSe head) and the
+    loss is f(out) + aux_weight[0] * f(aux16) + aux_weight[1] * f(aux32).  The reference's train.py:285-288 suggests thresh=0.7, aux=False
+    for the PSP, Lab and Base heads and thresh=0.7, aux=True, aux_weight=[0.15, 0.1] for BiSe.
+
+    Forward and backward are library kernels over (B, C, H, W) fp32 CUDA logits and (B, H, W) int64 CUDA labels, with no host
+    synchronisation: the selection (hard count, branch, the k-th largest CE by radix select) stays on the device.  Among pixels tied at the
+    k-th largest CE the lowest flat indices are taken (torch.topk leaves that order unspecified).  n_min = 0 with no hard pixel gives NaN and
+    zero gradients, as the reference does.  Labels outside [0, C) other than ignore_index count as ignored (torch would raise)."""
+
+    def __init__(self, thresh=0.5, ignore_index=-1, aux=False, aux_weight=(0.15, 0.05)):
+        super().__init__()
+        self.thresh_t = ohem_thresh_t(thresh)
+        self.ignore_index, self.aux, self.aux_weight = int(ignore_index), bool(aux), [float(w) for w in aux_weight]
+        if self.aux and len(self.aux_weight) != 2:
+            raise ValueError(f"OhemCELoss: aux=True takes two aux weights, got {aux_weight}")
+
+    def forward_once(self, pred, labels):
+        if not (isinstance(pred, torch.Tensor) and pred.is_cuda and pred.dtype == torch.float32 and pred.dim() == 4):
+            raise ValueError("OhemCELoss: expected (B, C, H, W) float32 CUDA logits")
+        if not (isinstance(labels, torch.Tensor) and labels.is_cuda and labels.dtype == torch.int64 and labels.device == pred.device
+                and tuple(labels.shape) == (pred.shape[0], pred.shape[2], pred.shape[3])):
+            raise ValueError(f"OhemCELoss: expected (B, H, W) = {(pred.shape[0], pred.shape[2], pred.shape[3])} int64 CUDA labels on the "
+                             "logits' device")
+        return _OhemCE.apply(pred.contiguous(), labels.contiguous(), self.thresh_t, self.ignore_index)
+
+    def forward(self, preds, labels):
+        if not self.aux:
+            return self.forward_once(preds, labels)
+        if not isinstance(preds, (list, tuple)) or len(preds) != 3:
+            raise ValueError("OhemCELoss(aux=True): preds must be the list [out, aux16, aux32]")
+        return (self.forward_once(preds[0], labels) + self.aux_weight[0] * self.forward_once(preds[1], labels)
+                + self.aux_weight[1] * self.forward_once(preds[2], labels))
