@@ -42,6 +42,7 @@ extern "C" {
 #define MYOLO_F32 1
 #define MYOLO_U8 2
 #define MYOLO_I64 3
+#define MYOLO_F64 4   /* myolo_anchor_metric only */
 
 /* activation of a conv op */
 #define MYOLO_ACT_NONE 0
@@ -259,6 +260,32 @@ int myolo_det_loss(const float* const* p, float* const* dp, const float* targets
                    const int32_t* nx, const float* anchors_grid, const float* balance, float hyp_box, float hyp_obj, float hyp_cls,
                    float anchor_t, float gr, float cp, float cn, float mult, const float* scale_dev, float* items_out, void* workspace,
                    int64_t workspace_bytes, void* stream);
+
+/* ---- autoanchor (reference utils/autoanchor.py:23-160; Python: utils.autoanchor) ---- */
+#define MYOLO_ANCHOR_MAX 32   /* anchors (na * nl) per call */
+typedef struct {
+  int64_t n_best;        /* labels whose best ratio x over the anchors is > thr */
+  int64_t n_x;           /* (label, anchor) pairs with x > thr */
+  double sum_x, sum_best, sum_x_above;   /* fp64 sums of x, of best, and of x over pairs with x > thr (fixed order: the same every run) */
+} myolo_anchor_stats;
+/* The reference's ratio metric of n labels' wh (n, 2) against na anchors (na, 2): r = wh / k, x = min(r, 1 / r) over both sides (correct
+ * rounding: torch's `1. / r` is r.reciprocal()), best = max over the anchors.  The arithmetic and the comparisons with thr (1 / anchor_t,
+ * cast to the compute dtype) run in fp64 when either input is MYOLO_F64 (torch promotes an fp32 tensor divided by a float64 numpy array),
+ * else in fp32.  wh_dtype, k_dtype: MYOLO_F32 or MYOLO_F64; device pointers; out: device myolo_anchor_stats.  workspace: device, at least
+ * myolo_anchor_metric_workspace_bytes().  No host synchronisation. */
+int64_t myolo_anchor_metric_workspace_bytes(void);
+int myolo_anchor_metric(const void* wh, int wh_dtype, int64_t n, const void* k, int k_dtype, int na, double thr, myolo_anchor_stats* out,
+                        void* workspace, int64_t workspace_bytes, void* stream);
+/* kmean_anchors' genetic evolution (utils/autoanchor.py:146-158) in one persistent cooperative kernel.  wh: (n, 2) fp32 device labels;
+ * k0: (na, 2) fp64 device start anchors (the sorted k-means result); v: (gen, na, 2) fp64 device mutation factors drawn on the host;
+ * thr: 1 / anchor_t.  Per generation kg = max(k * v, 2.0) in fp64, its fp32 cast scores fg = fp32(sum of best over labels with best > thr,
+ * summed exactly in fp64) / n in fp32, and kg replaces k when fg > f.  Outputs (device): k_out (na, 2) fp64, f_out[2] fp32 (the fitness
+ * of k0, the final fitness), fg_out (gen) fp32, accepted_out int32 (generations taken).  Needs 1 <= n < 2^26, 1 <= na <= MYOLO_ANCHOR_MAX and fp32(thr) >= 1/16 (anchor_t <= 16):
+ * the bounds of the exact sum; else MYOLO_E_INVALID.  workspace: device, at least myolo_anchor_evolve_workspace_bytes(n) (it depends on
+ * the current device).  A cooperative launch sized from the kernel's occupancy: a grid that cannot be co-resident is refused, never run. */
+int64_t myolo_anchor_evolve_workspace_bytes(int64_t n);
+int myolo_anchor_evolve(const float* wh, int64_t n, const double* k0, int na, const double* v, int gen, double thr, double* k_out,
+                        float* f_out, float* fg_out, int32_t* accepted_out, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* OhemCELoss.forward_once (reference utils/loss.py:321-328) over full-resolution logits (B, C, H, W) fp32 NCHW, any C, and labels (B, H, W)
  * int64, with the selection of myolo_plan_backward_seg_ohem.  myolo_seg_ohem_loss writes the loss to loss_out (device float) and leaves

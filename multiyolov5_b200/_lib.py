@@ -9,7 +9,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("MYOLO_LIB") or os.path.join(_HERE, "libmyolo_sm90a.so")   # MYOLO_LIB: developer builds (e.g. the clock64 timeline variant)
 
-F16, F32, U8, I64 = 0, 1, 2, 3
+F16, F32, U8, I64, F64 = 0, 1, 2, 3, 4     # F64: myolo_anchor_metric only
 ACT_NONE, ACT_SILU, ACT_SIGMOID = 0, 1, 2
 OP_INPUT_FOCUS = 1
 OP_CONV = 2
@@ -39,6 +39,7 @@ EXPORTS = [
     "myolo_resize_area_u8", "myolo_resize_bilinear", "myolo_plan_create_shared", "myolo_augment_det_hw", "myolo_adam_step",
     "myolo_adam_scalars", "myolo_ema_update", "myolo_plan_set_extra", "myolo_collate_quad", "myolo_plan_set_bn_sync",
     "myolo_plan_backward_seg_ohem", "myolo_seg_ohem_loss", "myolo_seg_ohem_loss_backward", "myolo_seg_ohem_loss_workspace_bytes",
+    "myolo_anchor_metric", "myolo_anchor_metric_workspace_bytes", "myolo_anchor_evolve", "myolo_anchor_evolve_workspace_bytes",
 ]
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
 
@@ -139,6 +140,12 @@ def lib():
     L.myolo_seg_ohem_loss_workspace_bytes.restype = i64
     L.myolo_seg_ohem_loss.argtypes = [vp, vp, i32, i32, i32, i32, i32, f32, vp, vp, i64, vp]
     L.myolo_seg_ohem_loss_backward.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp, vp, i64, vp]
+    L.myolo_anchor_metric_workspace_bytes.argtypes = []
+    L.myolo_anchor_metric_workspace_bytes.restype = i64
+    L.myolo_anchor_metric.argtypes = [vp, i32, i64, vp, i32, i32, C.c_double, vp, vp, i64, vp]
+    L.myolo_anchor_evolve_workspace_bytes.argtypes = [i64]
+    L.myolo_anchor_evolve_workspace_bytes.restype = i64
+    L.myolo_anchor_evolve.argtypes = [vp, i64, vp, i32, vp, i32, C.c_double, vp, vp, vp, vp, vp, i64, vp]
     L.myolo_plan_read_grad_view.argtypes = [vp, View, vp, vp]
     L.myolo_plan_set_seed.argtypes = [vp, C.c_uint64]
     L.myolo_plan_set_defer_running.argtypes = [vp, i32]

@@ -57,4 +57,12 @@ int launch_lut_blend(const void* idx, int idx_dtype, long n, const unsigned char
                      const unsigned char* im, float alpha, float beta, unsigned char* blend, cudaStream_t s);
 int launch_seg_hist(const void* pred, int pred_dtype, const long long* target, long n, int n_cls, unsigned long long* counters, cudaStream_t s);
 
+// autoanchor (autoanchor.cu): the ratio metric and the cooperative genetic evolution
+int64_t anchor_metric_workspace_bytes();
+int launch_anchor_metric(const void* wh, int wh_dtype, long n, const void* k, int k_dtype, int na, double thr, myolo_anchor_stats* out,
+                         void* workspace, cudaStream_t s);
+int anchor_evolve_workspace_bytes(long n, int64_t* bytes);
+int launch_anchor_evolve(const float* wh, long n, const double* k0, int na, const double* v, int gen, float thr, double* k_out,
+                         float* f_out, float* fg_out, int* accepted_out, void* workspace, int64_t workspace_bytes, cudaStream_t s);
+
 }  // namespace myolo

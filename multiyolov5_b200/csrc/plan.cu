@@ -1502,6 +1502,42 @@ extern "C" int myolo_seg_ohem_loss_backward(const float* logits, const int64_t* 
                                   grad_logits, (cudaStream_t)stream);
 }
 
+extern "C" int64_t myolo_anchor_metric_workspace_bytes(void) { return anchor_metric_workspace_bytes(); }
+
+extern "C" int myolo_anchor_metric(const void* wh, int wh_dtype, int64_t n, const void* k, int k_dtype, int na, double thr,
+                                   myolo_anchor_stats* out, void* workspace, int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_anchor_metric");
+  MYOLO_REQUIRE(wh && k && out && workspace && n > 0 && na >= 1 && na <= MYOLO_ANCHOR_MAX, "anchor_metric: bad arguments");
+  MYOLO_REQUIRE((wh_dtype == MYOLO_F32 || wh_dtype == MYOLO_F64) && (k_dtype == MYOLO_F32 || k_dtype == MYOLO_F64),
+                "anchor_metric: wh and k must be MYOLO_F32 or MYOLO_F64");
+  MYOLO_REQUIRE(workspace_bytes >= anchor_metric_workspace_bytes(), "anchor_metric: workspace too small");
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_anchor_metric(wh, wh_dtype, (long)n, k, k_dtype, na, thr, out, workspace, (cudaStream_t)stream);
+}
+
+extern "C" int64_t myolo_anchor_evolve_workspace_bytes(int64_t n) {
+  int64_t bytes = -1;
+  if (check_device(nullptr) || n <= 0 || anchor_evolve_workspace_bytes((long)n, &bytes)) return -1;
+  return bytes;
+}
+
+extern "C" int myolo_anchor_evolve(const float* wh, int64_t n, const double* k0, int na, const double* v, int gen, double thr,
+                                   double* k_out, float* f_out, float* fg_out, int32_t* accepted_out, void* workspace,
+                                   int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_anchor_evolve");
+  MYOLO_REQUIRE(wh && k0 && k_out && f_out && accepted_out && workspace && na >= 1 && na <= MYOLO_ANCHOR_MAX && gen >= 0 &&
+                (gen == 0 || (v && fg_out)), "anchor_evolve: bad arguments");
+  // the exact fp64 sum: every term a multiple of 2^-27 in [0, 1] (fp32(thr) >= 1/16) and fewer than 2^26 of them
+  MYOLO_REQUIRE(n >= 1 && n < (int64_t(1) << 26), "anchor_evolve: n = %lld labels, needs 1 <= n < 2^26", (long long)n);
+  const float thr32 = (float)thr;
+  MYOLO_REQUIRE(thr32 >= 0.0625f, "anchor_evolve: 1 / anchor_t = %g, needs anchor_t <= 16", thr);
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_anchor_evolve(wh, (long)n, k0, na, v, gen, thr32, k_out, f_out, fg_out, accepted_out, workspace, workspace_bytes,
+                              (cudaStream_t)stream);
+}
+
 extern "C" int myolo_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay, void* stream) {
   NvtxRange nvtx_("myolo_ema_update");
   int rc = check_device(nullptr);

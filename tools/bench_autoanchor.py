@@ -1,0 +1,104 @@
+#!/usr/bin/env python
+"""Benchmark of the reference's autoanchor on the device (utils.autoanchor: kmean_anchors with gen=1000, myolo_anchor_evolve).
+
+    python tools/bench_autoanchor.py [--repeats R]
+
+Prints ONE JSON line with the card's name, power limit and clocks read next to the measurement, for synthetic label sets of ~60 k
+(Cityscapes scale) and ~790 k (COCO scale) labels at img_size 1024 (oracle.restate_autoanchor.synth_dataset):
+  host_draws_ms   the 1000 generations' mutation factors drawn on the host (numpy, the reference's loop)
+  kmeans_ms       scipy's kmeans(wh / s, 9, iter=30), the reference's own call
+  evolve_ms       myolo_anchor_evolve over the filtered labels, CUDA events around the one cooperative launch (median and min of R)
+  end_to_end_ms   kmean_anchors(dataset, n=9, img_size=1024, gen=1000, verbose=False) on a host clock ending in a synchronise
+The reference's times on a CPU (8 torch threads) are quoted from its measurement, not re-run here: 10.5 s (3.8 s of it k-means) at 59 793
+labels and 121 s (42 s k-means) at 791 794 labels.
+"""
+import argparse
+import contextlib
+import io
+import json
+import os
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
+
+from tools.bench_augment import gpu_state  # noqa: E402
+
+CITY = [(12, 30), (25, 60), (40, 25), (90, 55), (200, 120), (8, 8), (30, 80), (150, 300)]
+SIZES = {"60k": (600, 100), "790k": (7900, 100)}
+QUOTED_CPU_S = {"60k": {"labels": 59793, "total_s": 10.5, "kmeans_s": 3.8}, "790k": {"labels": 791794, "total_s": 121.0, "kmeans_s": 42.0}}
+IMG, N, GEN = 1024, 9, 1000
+
+
+class _Dataset:
+    def __init__(self, shapes, labels):
+        self.shapes, self.labels = shapes, labels
+
+
+def one_size(tag, repeats):
+    from scipy.cluster.vq import kmeans
+
+    from multiyolov5_b200.utils import autoanchor as aa
+    from oracle import restate_autoanchor as ra
+    n_img, per = SIZES[tag]
+    shapes0, labels = ra.synth_dataset(17, n_img, per, CITY, spread=0.45, shapes=((1024, 2048), (720, 1280), (480, 640)))
+    ds = _Dataset(ra.shapes_wh(shapes0), labels)
+    wh0 = ra.label_wh(ds.shapes, labels, IMG)
+    wh = wh0[(wh0 >= 2.0).any(1)]
+    print(f"{tag}: {len(wh0)} labels", file=sys.stderr, flush=True)
+    np.random.seed(0)
+    t0 = time.perf_counter()
+    V = aa.draw_mutations(GEN, (N, 2))
+    draws_ms = (time.perf_counter() - t0) * 1e3
+    s = wh.std(0)
+    t0 = time.perf_counter()
+    k, _ = kmeans(wh / s, N, iter=30)
+    kmeans_ms = (time.perf_counter() - t0) * 1e3
+    print(f"{tag}: kmeans {kmeans_ms:.0f} ms", file=sys.stderr, flush=True)
+    k = ra.sort_by_area(k * s)
+    wh_d = torch.tensor(wh, dtype=torch.float32).cuda()
+    aa.evolve(wh_d, k, V[:10], 0.25)                               # warm-up: module load, allocator
+    ev = []
+    for _ in range(repeats):
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        out = aa.evolve(wh_d, k, V, 0.25)
+        e1.record()
+        torch.cuda.synchronize()
+        ev.append(e0.elapsed_time(e1))
+    e2e = []
+    for r in range(1 if tag == "790k" else 3):                     # scipy's kmeans alone takes ~40 s at 790 k labels on the CPU
+        np.random.seed(r)
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        with contextlib.redirect_stdout(io.StringIO()):
+            aa.kmean_anchors(ds, n=N, img_size=IMG, thr=4.0, gen=GEN, verbose=False)
+        torch.cuda.synchronize()
+        e2e.append((time.perf_counter() - t0) * 1e3)
+    # the evolve event window includes the host->device copies of k0 / v and the device->host reads of the results
+    return {"labels": int(len(wh0)), "labels_filtered": int(len(wh)), "host_draws_ms": round(draws_ms, 2), "kmeans_ms": round(kmeans_ms, 1),
+            "evolve_ms": {"median": round(float(np.median(ev)), 3), "min": round(float(np.min(ev)), 3), "n": len(ev)},
+            "evolve_us_per_generation": round(float(np.median(ev)) * 1e3 / GEN, 2), "accepted": out[4],
+            "end_to_end_ms": {"median": round(float(np.median(e2e)), 1), "min": round(float(np.min(e2e)), 1), "n": len(e2e)},
+            "reference_cpu_quoted": QUOTED_CPU_S[tag]}
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--repeats", type=int, default=10)
+    args = ap.parse_args()
+    assert torch.cuda.is_available(), "bench_autoanchor needs a GPU"
+    rec = {"bench": "autoanchor", "gpu": gpu_state(), "n": N, "img_size": IMG, "gen": GEN}
+    for tag in SIZES:
+        rec[tag] = one_size(tag, args.repeats)
+        print(f"{tag}: {json.dumps(rec[tag])}", file=sys.stderr, flush=True)
+    rec["gpu_after"] = gpu_state()
+    print(json.dumps(rec))
+
+
+if __name__ == "__main__":
+    main()
