@@ -202,6 +202,14 @@ int myolo_plan_backward_seg_ce(myolo_plan* plan, const int64_t* labels, int igno
  * Scratch of 4 bytes per full-resolution pixel plus ~5 KB is allocated on the first call and kept by the plan. */
 int myolo_plan_backward_seg_ohem(myolo_plan* plan, const int64_t* labels, int ignore_index, float thresh_t, float factor,
                                  const float* scale_dev, float* loss_out, void* stream);
+/* The same fused pass with the class-weighted CE and the focal loss in place of the mean CE: SegFocalLoss(gamma, alpha=class_weights,
+ * reduction='mean') (reference utils/loss.py:279-297) as myolo_seg_focal_loss defines it, which with gamma = 0 is
+ * CrossEntropyLoss(weight=class_weights) (SegmentationLosses(weight=...), train.py:269-278).  class_weights: n_segcls device floats owned
+ * by the caller, nullable (unit weights); gamma finite and >= 0.  With gamma > 0 the ignored pixels' softmax enters the loss, against
+ * class 0, as in the reference.  No host synchronisation.  Scratch of 8 bytes per full-resolution pixel plus 256 bytes is allocated on
+ * the first call and kept by the plan. */
+int myolo_plan_backward_seg_loss(myolo_plan* plan, const int64_t* labels, int ignore_index, const float* class_weights, float gamma,
+                                 float factor, const float* scale_dev, float* loss_out, void* stream);
 /* debug: like myolo_plan_read_view, from the gradient workspace of the last backward */
 int myolo_plan_read_grad_view(myolo_plan* plan, myolo_view view, float* dst_nchw_f32, void* stream);
 /* Optimiser step over FLAT fp32 buffers (all parameters of the model laid out back to back; `group[i]` in 0..n_groups-1 selects the
@@ -297,6 +305,23 @@ int myolo_seg_ohem_loss(const float* logits, const int64_t* labels, int B, int C
                         float* loss_out, void* workspace, int64_t workspace_bytes, void* stream);
 int myolo_seg_ohem_loss_backward(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index,
                                  const float* grad_out, float* grad_logits, const void* workspace, int64_t workspace_bytes, void* stream);
+
+/* SegFocalLoss(gamma, alpha=class_weights, ignore_index, reduction) (reference utils/loss.py:279-297) over full-resolution logits
+ * (B, C, H, W) fp32 NCHW, any C, and labels (B, H, W) int64.  With t' = t on valid pixels and 0 on ignored ones, p = softmax over C and
+ * N = B*H*W: loss = A * F, A = sum_valid w[t] CE / sum_valid w[t] and F = sum_all (1 - p_t')^gamma / N for MYOLO_REDUCTION_MEAN, the
+ * two sums themselves for MYOLO_REDUCTION_SUM (the reference's CE takes the outer reduction).  gamma = 0 with the mean is the class-weighted
+ * CrossEntropyLoss(weight=class_weights).  class_weights: C device floats, nullable (unit weights); gamma finite and >= 0.
+ * myolo_seg_focal_loss writes the loss to loss_out (device float) and leaves its coefficients in the workspace; myolo_seg_focal_loss_backward
+ * then writes grad_logits = (*grad_out) * d loss / d logits from the same logits, labels, weights, gamma and workspace.  Labels outside
+ * [0, C) other than ignore_index count as ignored.  No host synchronisation in either call.  Python: utils.loss.SegFocalLoss. */
+#define MYOLO_REDUCTION_MEAN 0
+#define MYOLO_REDUCTION_SUM 1
+int64_t myolo_seg_focal_loss_workspace_bytes(void);
+int myolo_seg_focal_loss(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index, const float* class_weights,
+                         float gamma, int reduction, float* loss_out, void* workspace, int64_t workspace_bytes, void* stream);
+int myolo_seg_focal_loss_backward(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index,
+                                  const float* class_weights, float gamma, const float* grad_out, float* grad_logits, const void* workspace,
+                                  int64_t workspace_bytes, void* stream);
 
 /* The path's ONE exchange step (SURVEY.md section 8b/8e; reference train.py:243-245 wraps the model in DistributedDataParallel): in-place
  * SUM all-reduce of the flat fp32 gradient buffer over the ranks of `nccl_comm` (an ncclComm_t; averaging is folded into myolo_sgd_step's

@@ -40,7 +40,9 @@ EXPORTS = [
     "myolo_adam_scalars", "myolo_ema_update", "myolo_plan_set_extra", "myolo_collate_quad", "myolo_plan_set_bn_sync",
     "myolo_plan_backward_seg_ohem", "myolo_seg_ohem_loss", "myolo_seg_ohem_loss_backward", "myolo_seg_ohem_loss_workspace_bytes",
     "myolo_anchor_metric", "myolo_anchor_metric_workspace_bytes", "myolo_anchor_evolve", "myolo_anchor_evolve_workspace_bytes",
+    "myolo_plan_backward_seg_loss", "myolo_seg_focal_loss", "myolo_seg_focal_loss_backward", "myolo_seg_focal_loss_workspace_bytes",
 ]
+REDUCTION_MEAN, REDUCTION_SUM = 0, 1        # include/myolo.h: MYOLO_REDUCTION_* of myolo_seg_focal_loss
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
 
 
@@ -140,6 +142,11 @@ def lib():
     L.myolo_seg_ohem_loss_workspace_bytes.restype = i64
     L.myolo_seg_ohem_loss.argtypes = [vp, vp, i32, i32, i32, i32, i32, f32, vp, vp, i64, vp]
     L.myolo_seg_ohem_loss_backward.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, vp, vp, i64, vp]
+    L.myolo_plan_backward_seg_loss.argtypes = [vp, vp, i32, vp, f32, f32, vp, vp, vp]
+    L.myolo_seg_focal_loss_workspace_bytes.argtypes = []
+    L.myolo_seg_focal_loss_workspace_bytes.restype = i64
+    L.myolo_seg_focal_loss.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, f32, i32, vp, vp, i64, vp]
+    L.myolo_seg_focal_loss_backward.argtypes = [vp, vp, i32, i32, i32, i32, i32, vp, f32, vp, vp, vp, i64, vp]
     L.myolo_anchor_metric_workspace_bytes.argtypes = []
     L.myolo_anchor_metric_workspace_bytes.restype = i64
     L.myolo_anchor_metric.argtypes = [vp, i32, i64, vp, i32, i32, C.c_double, vp, vp, i64, vp]

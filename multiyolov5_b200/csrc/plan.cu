@@ -168,6 +168,7 @@ struct myolo_plan {
   float* ce_gbuf = nullptr;        // per-pixel (softmax - onehot), NHWC fp32, of the fused seg loss
   size_t ce_gbuf_bytes = 0;
   void* ohem_ws = nullptr;         // the OHEM seg loss's selection state and per-pixel losses (ohem_scratch_bytes of B*H*W pixels)
+  void* wf_ws = nullptr;           // the weighted / focal seg loss's sums and per-pixel factors (seg_wf_scratch_bytes of B*H*W pixels)
 };
 
 static int resolve_view(const myolo_plan* pl, const myolo_view& v, TensorView* out) {
@@ -313,6 +314,7 @@ extern "C" void myolo_plan_destroy(myolo_plan* pl) {
   if (pl->d_step) cudaFree(pl->d_step);
   if (pl->ce_gbuf) cudaFree(pl->ce_gbuf);
   if (pl->ohem_ws) cudaFree(pl->ohem_ws);
+  if (pl->wf_ws) cudaFree(pl->wf_ws);
   if (pl->spp_scratch) cudaFree(pl->spp_scratch);
   delete pl;
 }
@@ -1188,14 +1190,15 @@ extern "C" int myolo_plan_backward(myolo_plan* pl, const float* const* grad_raw,
 
 // fused seg loss (SURVEY.md section 8f rank 3): CE(ignore_index) of the x8-upsampled logits of the last train forward is evaluated and
 // differentiated straight from the low-resolution logits; the backward then runs as the seg pass (seed mask 8)
-// ohem: OhemCELoss(thresh) with thresh_t = -log(thresh) instead of the mean CE
+// ohem: OhemCELoss(thresh) with thresh_t = -log(thresh) instead of the mean CE; wf: the class-weighted CE / focal loss (weights, gamma)
 static int backward_seg_fused(myolo_plan* pl, const int64_t* labels, int ignore_index, float factor, const float* scale_dev, float* loss_out,
-                              cudaStream_t s, bool ohem, float thresh_t) {
+                              cudaStream_t s, bool ohem, float thresh_t, bool wf = false, const float* weights = nullptr, float gamma = 0.f) {
   MYOLO_REQUIRE(pl && pl->train_fwd_done && labels, "backward_seg_ce: call myolo_plan_train_forward first / null labels");
   if (!pl->gws) MYOLO_CHECK_CUDA(cudaMalloc(&pl->gws, pl->ws_bytes));
   MYOLO_CHECK_CUDA(cudaMemsetAsync(pl->gws, 0, pl->ws_bytes, s));
   if (!pl->ce_scratch) MYOLO_CHECK_CUDA(cudaMalloc(&pl->ce_scratch, 16));
   if (ohem && !pl->ohem_ws) MYOLO_CHECK_CUDA(cudaMalloc(&pl->ohem_ws, ohem_scratch_bytes((long)pl->B * pl->H * pl->W)));   // the plan's shape is fixed
+  if (wf && !pl->wf_ws) MYOLO_CHECK_CUDA(cudaMalloc(&pl->wf_ws, seg_wf_scratch_bytes((long)pl->B * pl->H * pl->W)));
   std::vector<char> live(pl->bufs.size(), 0);
   int rc = MYOLO_E_INVALID;
   for (const auto& op : pl->ops)
@@ -1211,8 +1214,12 @@ static int backward_seg_fused(myolo_plan* pl, const int64_t* labels, int ignore_
         MYOLO_CHECK_CUDA(cudaMalloc(&pl->ce_gbuf, gb));
         pl->ce_gbuf_bytes = gb;
       }
-      rc = launch_seg_ce_fused(lo, op.aux[0], reinterpret_cast<const long long*>(labels), pl->H, pl->W, ignore_index, dlo, factor, scale_dev,
-                               pl->ce_scratch, pl->ce_gbuf, loss_out, s, ohem ? pl->ohem_ws : nullptr, thresh_t);
+      if (wf)
+        rc = launch_seg_wf_fused(lo, op.aux[0], reinterpret_cast<const long long*>(labels), pl->H, pl->W, ignore_index, dlo, factor,
+                                 scale_dev, pl->ce_gbuf, pl->wf_ws, weights, gamma, loss_out, s);
+      else
+        rc = launch_seg_ce_fused(lo, op.aux[0], reinterpret_cast<const long long*>(labels), pl->H, pl->W, ignore_index, dlo, factor,
+                                 scale_dev, pl->ce_scratch, pl->ce_gbuf, loss_out, s, ohem ? pl->ohem_ws : nullptr, thresh_t);
       break;
     }
   if (rc) { if (rc == MYOLO_E_INVALID) set_error("backward_seg_ce: the plan has no segmentation output"); return rc; }
@@ -1229,6 +1236,13 @@ extern "C" int myolo_plan_backward_seg_ohem(myolo_plan* pl, const int64_t* label
                                             const float* scale_dev, float* loss_out, void* stream) {
   NvtxRange nvtx_("myolo_plan_backward_seg_ohem");
   return backward_seg_fused(pl, labels, ignore_index, factor, scale_dev, loss_out, (cudaStream_t)stream, true, thresh_t);
+}
+
+extern "C" int myolo_plan_backward_seg_loss(myolo_plan* pl, const int64_t* labels, int ignore_index, const float* class_weights, float gamma,
+                                            float factor, const float* scale_dev, float* loss_out, void* stream) {
+  NvtxRange nvtx_("myolo_plan_backward_seg_loss");
+  return backward_seg_fused(pl, labels, ignore_index, factor, scale_dev, loss_out, (cudaStream_t)stream, false, 0.f, true, class_weights,
+                            gamma);
 }
 
 static int backward_walk(myolo_plan* pl, std::vector<char>& live, cudaStream_t s, int* n_ops) {
@@ -1500,6 +1514,34 @@ extern "C" int myolo_seg_ohem_loss_backward(const float* logits, const int64_t* 
   if (rc) return rc;
   return launch_seg_ohem_loss_bwd(logits, reinterpret_cast<const long long*>(labels), B, C, H, W, ignore_index, workspace, grad_out,
                                   grad_logits, (cudaStream_t)stream);
+}
+
+extern "C" int64_t myolo_seg_focal_loss_workspace_bytes(void) { return (int64_t)seg_focal_workspace_bytes(); }
+
+extern "C" int myolo_seg_focal_loss(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index,
+                                    const float* class_weights, float gamma, int reduction, float* loss_out, void* workspace,
+                                    int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_seg_focal_loss");
+  MYOLO_REQUIRE(logits && labels && loss_out && workspace && B > 0 && C > 0 && H > 0 && W > 0, "seg_focal_loss: bad arguments");
+  MYOLO_REQUIRE(reduction == MYOLO_REDUCTION_MEAN || reduction == MYOLO_REDUCTION_SUM, "seg_focal_loss: reduction must be mean or sum");
+  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_focal_loss_workspace_bytes(), "seg_focal_loss: workspace too small");
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_seg_focal_loss(logits, reinterpret_cast<const long long*>(labels), B, C, H, W, ignore_index, class_weights, gamma,
+                               reduction == MYOLO_REDUCTION_SUM, workspace, loss_out, (cudaStream_t)stream);
+}
+
+extern "C" int myolo_seg_focal_loss_backward(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index,
+                                             const float* class_weights, float gamma, const float* grad_out, float* grad_logits,
+                                             const void* workspace, int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_seg_focal_loss_backward");
+  MYOLO_REQUIRE(logits && labels && grad_out && grad_logits && workspace && B > 0 && C > 0 && H > 0 && W > 0,
+                "seg_focal_loss_backward: bad arguments");
+  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_focal_loss_workspace_bytes(), "seg_focal_loss_backward: workspace too small");
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_seg_focal_loss_bwd(logits, reinterpret_cast<const long long*>(labels), B, C, H, W, ignore_index, class_weights, gamma,
+                                   workspace, grad_out, grad_logits, (cudaStream_t)stream);
 }
 
 extern "C" int64_t myolo_anchor_metric_workspace_bytes(void) { return anchor_metric_workspace_bytes(); }

@@ -1099,6 +1099,53 @@ __global__ void ohem_finalize_kernel(const OhemSel* st, float* loss_out) {
   if (loss_out) *loss_out = st->loss_sum / st->denom;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Class-weighted CE and focal loss (reference SegmentationLosses(weight=w), utils/loss.py:221-237, and SegFocalLoss, :279-297).  With
+// t' = t for valid pixels and 0 for ignored ones (the reference's `target * (target != ignore_index)`), p = softmax(z), N pixels:
+//   A = sum_valid w[t] CE / sum_valid w[t]  (mean)  or  sum_valid w[t] CE  (sum)         the CE inside SegFocalLoss takes its reduction
+//   F = sum_all (1 - p_t')^gamma / N        (mean)  or  sum_all (1 - p_t')^gamma (sum)   ignored pixels take part, with class 0
+//   loss = A * F;   d loss / d z_i = (c1 * w[t_i] [valid_i] + c2 * gamma (1 - p_t')^(gamma-1) p_t') * (p_i - e_t')
+// with c1 = F / sum w (mean) or F (sum), c2 = A / N (mean) or A (sum).  gamma = 0 is the weighted CE: F = 1 (or N) exactly and c2 = 0,
+// as torch's pow backward returns zeros for a zero exponent.  Three sums over the pixels, then one finalize thread writes the loss and
+// the coefficients; nothing returns to the host.  Null weights are unit weights.  No valid pixel gives A = 0 / 0 = NaN, and the gradient
+// is NaN with gamma > 0 (A enters every pixel's gradient) and zero with gamma = 0, as in the reference.
+// ------------------------------------------------------------------------------------------------
+struct SegWfSt {
+  float s_wl, s_w, s_f;                    // zeroed per call: sum_valid w[t] CE, sum_valid w[t], sum_all (1 - p_t')^gamma
+  float c1, c2, loss;
+};
+constexpr size_t kSegWfHead = 256;         // the SegWfSt, padded; the fused pass's per-pixel factors follow it
+
+__device__ __forceinline__ float focal_grad_factor(float pt, float gamma) {
+  return gamma == 0.f ? 0.f : gamma * powf(1.f - pt, gamma - 1.f) * pt;   // p_t' = 1 with gamma < 1: inf, as torch's pow backward
+}
+
+__device__ __forceinline__ void seg_wf_accumulate(SegWfSt* st, float swl, float sw, float sf) {
+  swl = warp_sum(swl); sw = warp_sum(sw); sf = warp_sum(sf);
+  if ((threadIdx.x & 31) == 0) {
+    if (sw != 0.f || swl != 0.f) { atomicAdd(&st->s_wl, swl); atomicAdd(&st->s_w, sw); }
+    if (sf != 0.f) atomicAdd(&st->s_f, sf);
+  }
+}
+
+__global__ void seg_wf_finalize_kernel(SegWfSt* st, float gamma, float n, int sum, float* loss_out) {
+  const float A = sum ? st->s_wl : st->s_wl / st->s_w;
+  const float F = gamma == 0.f ? (sum ? n : 1.f) : (sum ? st->s_f : st->s_f / n);
+  st->c1 = sum ? F : (st->s_w == 0.f ? 0.f : F / st->s_w);
+  st->c2 = gamma == 0.f ? 0.f : (sum ? A : A / n);
+  st->loss = A * F;
+  if (loss_out) *loss_out = st->loss;
+}
+
+// the weighted / focal mode of the fused pass: per-class weights (nullable), gamma, and per pixel the two factors
+// (w[t] [valid], gamma (1 - p_t')^(gamma-1) p_t') the gather combines with the finalized c1, c2
+struct SegWf {
+  const float* w;
+  float gamma;
+  SegWfSt* st;
+  float2* pf;
+};
+
 // pass 1: one thread per FULL-resolution pixel: interpolated logits from the 4 low-res neighbours -> softmax -> (p - onehot) written as
 // NC_PAD fp32 per pixel (zeros for ignored pixels); the pixel's loss is reduced per warp, and written to pix_loss (OHEM, nullable).
 template <int NC, int NC_PAD>
@@ -1142,12 +1189,67 @@ __global__ void seg_ce_pixel_kernel(TensorView lo, const long long* __restrict__
   if ((threadIdx.x & 31) == 0 && loss_local != 0.f) atomicAdd(loss_sum, loss_local);
 }
 
+// pass 1 of the weighted / focal loss: seg_ce_pixel_kernel's per-pixel (p - onehot(t')), and the pixel's two factors (w[t] [valid],
+// gamma (1 - p_t')^(gamma-1) p_t') for the gather; the three sums are reduced per warp.  With gamma != 0 the ignored pixels' softmax is
+// taken too, against class 0.
+template <int NC, int NC_PAD>
+__global__ void seg_wf_pixel_kernel(TensorView lo, const long long* __restrict__ labels, int H, int W, int ignore_index, float* __restrict__ g,
+                                    SegWf wf) {
+  const long total = (long)lo.B * H * W;
+  float swl = 0.f, sw = 0.f, sf = 0.f;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int X = (int)(i % W);
+    const int Y = (int)((i / W) % H);
+    const int b = (int)(i / ((long)W * H));
+    const long long t = labels[i];
+    const bool valid = t != ignore_index && t >= 0 && t < NC;
+    const int tt = valid ? (int)t : 0;
+    float v[NC_PAD];
+    float2 f = make_float2(0.f, 0.f);
+#pragma unroll
+    for (int c = 0; c < NC_PAD; ++c) v[c] = 0.f;
+    if (valid || wf.gamma != 0.f) {
+      int a0, a1, b0, b1; float w0, w1, v0, v1;
+      lerp_src(Y, lo.H, H, &a0, &a1, &w0, &w1);
+      lerp_src(X, lo.W, W, &b0, &b1, &v0, &v1);
+      const float* q00 = tvf(lo, b, a0, b0); const float* q01 = tvf(lo, b, a0, b1);
+      const float* q10 = tvf(lo, b, a1, b0); const float* q11 = tvf(lo, b, a1, b1);
+      const float c00 = w0 * v0, c01 = w0 * v1, c10 = w1 * v0, c11 = w1 * v1;
+      float m = -INFINITY, zt = 0.f, et = 0.f;
+#pragma unroll
+      for (int c = 0; c < NC; ++c) { v[c] = c00 * q00[c] + c01 * q01[c] + c10 * q10[c] + c11 * q11[c]; m = fmaxf(m, v[c]); }
+      float ssum = 0.f;
+#pragma unroll
+      for (int c = 0; c < NC; ++c) { if (c == tt) zt = v[c]; v[c] = __expf(v[c] - m); if (c == tt) et = v[c]; ssum += v[c]; }
+      const float inv = 1.0f / ssum;
+#pragma unroll
+      for (int c = 0; c < NC; ++c) v[c] = v[c] * inv - (c == tt ? 1.0f : 0.f);
+      const float pt = et * inv;
+      if (valid) {
+        f.x = wf.w ? wf.w[tt] : 1.f;
+        swl += f.x * (__logf(ssum) + m - zt);
+        sw += f.x;
+      }
+      if (wf.gamma != 0.f) {
+        f.y = focal_grad_factor(pt, wf.gamma);
+        sf += powf(1.f - pt, wf.gamma);
+      }
+    }
+    wf.pf[i] = f;
+    float4* dst = reinterpret_cast<float4*>(g + (size_t)i * NC_PAD);
+#pragma unroll
+    for (int c = 0; c < NC_PAD; c += 4) dst[c / 4] = make_float4(v[c], v[c + 1], v[c + 2], v[c + 3]);
+  }
+  seg_wf_accumulate(wf.st, swl, sw, sf);
+}
+
 // pass 2: adjoint of the bilinear upsample, gathered per low-res pixel (x a chunk of its footprint rows) from the per-pixel gradients.
 // OHEM (sel non-null): only the pixels the selection took contribute, and the denominator is the selection's.
-template <int NC, int NC_PAD>
+// WF: each pixel's gradient is scaled by c1 * pf.x + c2 * pf.y (seg_wf_finalize_kernel).
+template <int NC, int NC_PAD, bool WF>
 __global__ void seg_ce_gather_kernel(const float* __restrict__ g, int H, int W, TensorView dlo, float factor, const float* __restrict__ scale_dev,
                                      const unsigned long long* __restrict__ n_valid, int rsplit, const OhemSel* __restrict__ sel,
-                                     const float* __restrict__ pix_loss) {
+                                     const float* __restrict__ pix_loss, const SegWfSt* __restrict__ wst, const float2* __restrict__ pf) {
   const long total = (long)dlo.B * dlo.H * dlo.W * rsplit;
   const float num = factor * (scale_dev ? *scale_dev : 1.0f);
   float coef;
@@ -1155,7 +1257,11 @@ __global__ void seg_ce_gather_kernel(const float* __restrict__ g, int H, int W, 
   float thresh_t = 0.f;
   unsigned kth = 0;
   long long cut = 0;
-  if (sel) {
+  float c1 = 0.f, c2 = 0.f;
+  if constexpr (WF) {
+    coef = num;
+    c1 = wst->c1; c2 = wst->c2;
+  } else if (sel) {
     coef = ohem_coef(sel, num);
     branch = sel->branch; thresh_t = sel->thresh_t; kth = sel->prefix; cut = sel->cut;
   } else {
@@ -1185,9 +1291,14 @@ __global__ void seg_ce_gather_kernel(const float* __restrict__ g, int H, int W, 
       for (int X = xlo; X <= xhi; ++X) {
         int b0, b1; float v0, v1;
         lerp_src(X, dlo.W, W, &b0, &b1, &v0, &v1);
-        const float wgt = wy * ((b0 == x ? v0 : 0.f) + (b1 == x ? v1 : 0.f));
+        float wgt = wy * ((b0 == x ? v0 : 0.f) + (b1 == x ? v1 : 0.f));
         if (wgt == 0.f) continue;
-        if (sel) {
+        if constexpr (WF) {
+          const float2 f = pf[((long)b * H + Y) * W + X];
+          const float k = c1 * f.x + c2 * f.y;
+          if (k == 0.f) continue;
+          wgt *= k;
+        } else if (sel) {
           const long pix = ((long)b * H + Y) * W + X;
           if (!ohem_taken(branch, thresh_t, kth, cut, pix, pix_loss[pix])) continue;
         }
@@ -1238,11 +1349,121 @@ int launch_seg_ce_fused(const TensorView& lo, int n_cls, const long long* labels
   MYOLO_LAUNCH_CHECK();
   if (ohem_ws)
     if (int rc = ohem_select(oh.loss, n, n_valid, thresh_t, oh.st, oh.ties, s)) return rc;
-  if (n_cls == 19) seg_ce_gather_kernel<19, 20><<<g2, 128, 0, s>>>(gbuf, H, W, dlo, factor, scale_dev, n_valid, rsplit, oh.st, oh.loss);
-  else seg_ce_gather_kernel<32, 32><<<g2, 128, 0, s>>>(gbuf, H, W, dlo, factor, scale_dev, n_valid, rsplit, oh.st, oh.loss);
+  if (n_cls == 19)
+    seg_ce_gather_kernel<19, 20, false><<<g2, 128, 0, s>>>(gbuf, H, W, dlo, factor, scale_dev, n_valid, rsplit, oh.st, oh.loss, nullptr, nullptr);
+  else
+    seg_ce_gather_kernel<32, 32, false><<<g2, 128, 0, s>>>(gbuf, H, W, dlo, factor, scale_dev, n_valid, rsplit, oh.st, oh.loss, nullptr, nullptr);
   MYOLO_LAUNCH_CHECK();
   if (ohem_ws) ohem_finalize_kernel<<<1, 1, 0, s>>>(oh.st, loss_out);
   else seg_ce_finalize_kernel<<<1, 1, 0, s>>>(loss_sum, n_valid, loss_out);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+size_t seg_wf_scratch_bytes(long n) { return kSegWfHead + (size_t)n * sizeof(float2); }
+
+// the weighted / focal loss in place of the mean CE: wf_ws = seg_wf_scratch_bytes(B*H*W) bytes; weights: n_cls device floats (nullable)
+int launch_seg_wf_fused(const TensorView& lo, int n_cls, const long long* labels, int H, int W, int ignore_index, const TensorView& dlo,
+                        float factor, const float* scale_dev, float* gbuf, void* wf_ws, const float* weights, float gamma, float* loss_out,
+                        cudaStream_t s) {
+  MYOLO_REQUIRE(lo.dtype == MYOLO_F32 && dlo.dtype == MYOLO_F32 && lo.C >= n_cls && labels && gbuf && wf_ws,
+                "seg_loss_fused: fp32 low-resolution logits expected");
+  MYOLO_REQUIRE(n_cls == 19 || n_cls == 32, "seg_loss_fused: instantiate the kernels for %d classes (19 and 32 are built)", n_cls);
+  MYOLO_REQUIRE(gamma >= 0.f && isfinite(gamma), "seg_loss_fused: gamma must be finite and >= 0, got %g", (double)gamma);
+  const long n = (long)lo.B * H * W;
+  SegWf wf{weights, gamma, reinterpret_cast<SegWfSt*>(wf_ws), reinterpret_cast<float2*>(reinterpret_cast<unsigned char*>(wf_ws) + kSegWfHead)};
+  MYOLO_CHECK_CUDA(cudaMemsetAsync(wf_ws, 0, sizeof(SegWfSt), s));
+  const int rsplit = 4;
+  const int g1 = grid_for_t(n, 128), g2 = grid_for_t((long)lo.B * lo.H * lo.W * rsplit, 128);
+  if (n_cls == 19) seg_wf_pixel_kernel<19, 20><<<g1, 128, 0, s>>>(lo, labels, H, W, ignore_index, gbuf, wf);
+  else seg_wf_pixel_kernel<32, 32><<<g1, 128, 0, s>>>(lo, labels, H, W, ignore_index, gbuf, wf);
+  MYOLO_LAUNCH_CHECK();
+  seg_wf_finalize_kernel<<<1, 1, 0, s>>>(wf.st, gamma, (float)n, 0, loss_out);
+  MYOLO_LAUNCH_CHECK();
+  if (n_cls == 19)
+    seg_ce_gather_kernel<19, 20, true><<<g2, 128, 0, s>>>(gbuf, H, W, dlo, factor, scale_dev, nullptr, rsplit, nullptr, nullptr, wf.st, wf.pf);
+  else
+    seg_ce_gather_kernel<32, 32, true><<<g2, 128, 0, s>>>(gbuf, H, W, dlo, factor, scale_dev, nullptr, rsplit, nullptr, nullptr, wf.st, wf.pf);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---- SegFocalLoss over full-resolution NCHW fp32 logits of any class count (the standalone module: utils.loss.SegFocalLoss) ----
+__global__ void seg_focal_nchw_kernel(const float* __restrict__ x, const long long* __restrict__ labels, int B, int C, long HW,
+                                      int ignore_index, const float* __restrict__ w, float gamma, SegWfSt* st) {
+  const long n = (long)B * HW;
+  float swl = 0.f, sw = 0.f, sf = 0.f;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const long long t = labels[i];
+    const bool valid = t != ignore_index && t >= 0 && t < C;
+    if (!valid && gamma == 0.f) continue;
+    const int tt = valid ? (int)t : 0;
+    const float* xp = x + (size_t)(i / HW) * C * HW + i % HW;
+    float m = -INFINITY;
+    for (int c = 0; c < C; ++c) m = fmaxf(m, xp[(size_t)c * HW]);
+    float s = 0.f;
+    for (int c = 0; c < C; ++c) s += expf(xp[(size_t)c * HW] - m);
+    const float zt = xp[(size_t)tt * HW];
+    if (valid) {
+      const float a = w ? w[tt] : 1.f;
+      swl += a * (logf(s) + m - zt);
+      sw += a;
+    }
+    if (gamma != 0.f) sf += powf(1.f - expf(zt - m) / s, gamma);
+  }
+  seg_wf_accumulate(st, swl, sw, sf);
+}
+
+// dx = grad_out * (c1 * w[t] [valid] + c2 * gamma (1 - p_t')^(gamma-1) p_t') * (softmax - onehot(t'))
+__global__ void seg_focal_nchw_bwd_kernel(const float* __restrict__ x, const long long* __restrict__ labels, int B, int C, long HW,
+                                          int ignore_index, const float* __restrict__ w, float gamma, const SegWfSt* __restrict__ st,
+                                          const float* __restrict__ grad_out, float* __restrict__ dx) {
+  const long n = (long)B * HW;
+  const float go = *grad_out, c1 = st->c1, c2 = st->c2;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const long long t = labels[i];
+    const bool valid = t != ignore_index && t >= 0 && t < C;
+    const int tt = valid ? (int)t : 0;
+    const size_t base = (size_t)(i / HW) * C * HW + i % HW;
+    const float* xp = x + base;
+    float* dp = dx + base;
+    float m = -INFINITY, s = 0.f, k = 0.f;
+    if (valid || gamma != 0.f) {
+      for (int c = 0; c < C; ++c) m = fmaxf(m, xp[(size_t)c * HW]);
+      for (int c = 0; c < C; ++c) s += expf(xp[(size_t)c * HW] - m);
+      const float a = valid ? (w ? w[tt] : 1.f) : 0.f;
+      k = go * (c1 * a + c2 * focal_grad_factor(expf(xp[(size_t)tt * HW] - m) / s, gamma));
+    }
+    if (k == 0.f) {
+      for (int c = 0; c < C; ++c) dp[(size_t)c * HW] = 0.f;
+      continue;
+    }
+    const float inv = 1.0f / s;
+    for (int c = 0; c < C; ++c) dp[(size_t)c * HW] = k * (expf(xp[(size_t)c * HW] - m) * inv - (c == tt ? 1.0f : 0.f));
+  }
+}
+
+size_t seg_focal_workspace_bytes() { return kSegWfHead; }
+
+int launch_seg_focal_loss(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const float* weights,
+                          float gamma, int sum, void* ws, float* loss_out, cudaStream_t s) {
+  MYOLO_REQUIRE(gamma >= 0.f && isfinite(gamma), "seg_focal_loss: gamma must be finite and >= 0, got %g", (double)gamma);
+  const long n = (long)B * H * W;
+  SegWfSt* st = reinterpret_cast<SegWfSt*>(ws);
+  MYOLO_CHECK_CUDA(cudaMemsetAsync(ws, 0, sizeof(SegWfSt), s));
+  seg_focal_nchw_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, labels, B, C, (long)H * W, ignore_index, weights, gamma, st);
+  MYOLO_LAUNCH_CHECK();
+  seg_wf_finalize_kernel<<<1, 1, 0, s>>>(st, gamma, (float)n, sum, loss_out);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+int launch_seg_focal_loss_bwd(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const float* weights,
+                              float gamma, const void* ws, const float* grad_out, float* dx, cudaStream_t s) {
+  MYOLO_REQUIRE(gamma >= 0.f && isfinite(gamma), "seg_focal_loss_backward: gamma must be finite and >= 0, got %g", (double)gamma);
+  const long n = (long)B * H * W;
+  seg_focal_nchw_bwd_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, labels, B, C, (long)H * W, ignore_index, weights, gamma,
+                                                                 reinterpret_cast<const SegWfSt*>(ws), grad_out, dx);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }

@@ -92,6 +92,19 @@ int launch_seg_ohem_loss(const float* x, const long long* labels, int B, int C, 
                          float* loss_out, cudaStream_t s);
 int launch_seg_ohem_loss_bwd(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const void* ws,
                              const float* grad_out, float* dx, cudaStream_t s);
+// the same fused pass with the class-weighted CE / focal loss (weights: n_cls device floats, nullable; gamma = 0 is the weighted CE) in
+// place of the mean CE, reduction 'mean'; wf_ws: seg_wf_scratch_bytes(B*H*W) bytes (the loss's sums and coefficients, 8 bytes per pixel)
+size_t seg_wf_scratch_bytes(long n_pixels);
+int launch_seg_wf_fused(const TensorView& lo, int n_cls, const long long* labels, int H, int W, int ignore_index, const TensorView& dlo,
+                        float factor, const float* scale_dev, float* gbuf, void* wf_ws, const float* weights, float gamma, float* loss_out,
+                        cudaStream_t s);
+// SegFocalLoss over full-resolution (B,C,H,W) fp32 logits (sum = 0: 'mean', 1: 'sum'): the forward leaves its coefficients in ws
+// (seg_focal_workspace_bytes()), the backward reads them and writes dx = *grad_out * d(loss)/dx
+size_t seg_focal_workspace_bytes();
+int launch_seg_focal_loss(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const float* weights,
+                          float gamma, int sum, void* ws, float* loss_out, cudaStream_t s);
+int launch_seg_focal_loss_bwd(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const float* weights,
+                              float gamma, const void* ws, const float* grad_out, float* dx, cudaStream_t s);
 // Detect: d(conv out fp32 NHWC)[b,y,x,a*no+o] = draw[b,a,y,x,o]
 int launch_detect_raw_bwd(const float* draw, int na, int no, const TensorView& dconv, cudaStream_t s);
 int launch_cast_f32_to_f16(const TensorView& src, const TensorView& dst, cudaStream_t s);

@@ -421,6 +421,19 @@ class Engine:
                                                            float(factor), _lib.ptr(scale), _lib.ptr(loss), _lib.stream_ptr()))
         return loss
 
+    def train_backward_seg_loss(self, plan, labels, weights=None, gamma=0.0, factor=1.0, scale=None, ignore_index=-1):
+        """train_backward_seg_ce with the class-weighted CE / focal loss in place of the mean CE (myolo_plan_backward_seg_loss):
+        SegFocalLoss(gamma, alpha=weights, reduction='mean'), which with gamma = 0 is CrossEntropyLoss(weight=weights).  weights: None or
+        an (n_segcls,) fp32 CUDA tensor, read by the kernels at their launch.  Returns the loss (device scalar)."""
+        assert labels.is_cuda and labels.dtype == torch.int64 and tuple(labels.shape) == (plan.B, plan.H, plan.W)
+        assert weights is None or (weights.is_cuda and weights.dtype == torch.float32 and weights.is_contiguous())
+        self._check_generation(plan, None)
+        loss = torch.empty((), dtype=torch.float32, device=labels.device)
+        _lib.check(_lib.lib().myolo_plan_backward_seg_loss(plan.handle, _lib.ptr(labels.contiguous()), int(ignore_index), _lib.ptr(weights),
+                                                           float(gamma), float(factor), _lib.ptr(scale), _lib.ptr(loss),
+                                                           _lib.stream_ptr()))
+        return loss
+
     def read_grad_view(self, v, plan=None):
         """debug: NHWC slice of the gradient workspace -> (B,C,H,W) fp32 torch tensor"""
         p = plan or self.last_plan

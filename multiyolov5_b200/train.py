@@ -20,7 +20,8 @@ skipped for overflow: one launch (`myolo_ema_update`) over every floating-point 
 per-entry statements.  Pass it on rank -1 / 0 and None elsewhere, as train.py:151 builds it.
 
 `Trainer(..., seg_loss=OhemCELoss(0.7))` trains with the reference's OHEM segmentation loss (train.py:285-288) in place of
-SegmentationLosses.
+SegmentationLosses; `seg_loss=SegmentationLosses(weight=w)` with its class-weighted CE (train.py:269-282), and
+`seg_loss=SegFocalLoss(gamma=2, ignore_index=-1)` with its focal loss (train_custom.py:284).
 
 `Trainer(..., quad=True)` is the reference's `--quad`: det batches from `utils.datasets.collate_quad` (collate_fn4) and the det loss x 4
 (train.py:368-369).
@@ -42,7 +43,7 @@ import torch.nn as nn
 from . import _lib
 from .engine import flat_offsets
 from .parallel import allreduce_flat_grads, bn_sync_group
-from .utils.loss import FusedComputeLoss, OhemCELoss, SegmentationLosses
+from .utils.loss import FusedComputeLoss, OhemCELoss, SegFocalLoss, SegmentationLosses, seg_focal_loss
 
 
 def scale_hyp(hyp: dict, nl: int, nc: int, imgsz: int, total_batch_size: int, nbs: int = 64, label_smoothing: float = 0.0) -> dict:
@@ -297,6 +298,34 @@ def resize_bilinear(x, size, out_dtype=torch.float32):
     return out
 
 
+def _check_weighted_seg_loss(seg_loss, n_seg_outputs, n_segcls):
+    """ValueError unless a SegmentationLosses / SegFocalLoss seg_loss fits the head and the loop (ignore_index -1, the segtargets'
+    marker); returns its class weights (None: unit weights).  Other losses pass through with None."""
+    if isinstance(seg_loss, SegmentationLosses):
+        name = "SegmentationLosses"
+        if seg_loss.weight is None:
+            raise ValueError("seg_loss=SegmentationLosses() without weight is the default loss: pass seg_loss=None for it")
+        bise = n_seg_outputs == 3
+        if seg_loss.aux != bise or (bise and seg_loss.aux_num != 2):
+            raise ValueError(f"SegmentationLosses(aux={seg_loss.aux}, aux_num={seg_loss.aux_num}) does not fit a seg head with "
+                             f"{n_seg_outputs} output(s): aux=True, aux_num=2 is for the BiSe head's [out, aux16, aux32] only")
+        weight = seg_loss.weight
+    elif isinstance(seg_loss, SegFocalLoss):
+        name = "SegFocalLoss"
+        if n_seg_outputs != 1:
+            raise ValueError("SegFocalLoss has no auxiliary outputs: it does not fit the BiSe head's [out, aux16, aux32]")
+        if seg_loss.reduction != "mean":
+            raise ValueError(f"SegFocalLoss(reduction={seg_loss.reduction!r}): the training loop takes reduction='mean'")
+        weight = seg_loss.weight
+    else:
+        return None
+    if seg_loss.ignore_index != -1:
+        raise ValueError(f"{name}(ignore_index={seg_loss.ignore_index}): the seg targets mark ignored pixels with -1; pass ignore_index=-1")
+    if weight is not None and weight.numel() != n_segcls:
+        raise ValueError(f"{name}: {weight.numel()} class weights for a seg head of {n_segcls} classes")
+    return weight
+
+
 class Trainer:
     """`Trainer(model, hyp, batch_size).step(imgs, targets, segimgs, segtargets)`; hyp already scaled (see scale_hyp)."""
 
@@ -319,20 +348,26 @@ class Trainer:
         for batch_size // 4 images at the doubled shapes, with multi_scale every size it can draw from them.  The seg pass and its
         batch_size factor are unchanged (train.py:385).  The reference's loop skips a det batch of one image (train.py:338), so with quad
         a per-GPU batch_size below 8 never trains; the Trainer steps whatever it is given.
-        seg_loss: None (SegmentationLosses, as the reference's default) or a utils.loss.OhemCELoss, multiplied by batch_size * seggain
-        like the default (train.py:385-391).  On a plain head with 19 or 32 classes it runs in the fused upsample + CE kernels; on any other
-        head through autograd on the model's full-resolution outputs.  Its aux must match the head: aux=True for BiSe's three outputs
-        only (ValueError otherwise)."""
+        seg_loss: None (SegmentationLosses, as the reference's default), a utils.loss.OhemCELoss, a SegmentationLosses with `weight` set
+        (n_segcls class weights: the class-weighted CE of train.py:269-282) or a utils.loss.SegFocalLoss (train_custom.py:284), multiplied
+        by batch_size * seggain like the default (train.py:385-391).  On a plain head with 19 or 32 classes it runs in the fused upsample +
+        CE kernels; on any other head through autograd on the model's full-resolution outputs, in the library's loss kernels.  The class
+        weights are uploaded once, here.  ValueError for a loss that does not fit: an aux that does not match the head (aux=True, and
+        aux_num=2 for SegmentationLosses, for BiSe's three outputs only), SegFocalLoss on BiSe (it has no aux), a SegFocalLoss reduction
+        other than 'mean', a weight vector whose length is not n_segcls, an ignore_index other than -1, and SegmentationLosses without
+        weight (the default: pass seg_loss=None)."""
         if optimizer not in OPTIMIZER_STATE:
             raise ValueError(f"optimizer must be 'sgd' or 'adam', got {optimizer!r}")
         if quad and batch_size < 4:
             raise ValueError(f"quad: a batch of {batch_size} images has no quad (collate_fn4 needs at least 4)")
-        if seg_loss is not None and not isinstance(seg_loss, OhemCELoss):
-            raise ValueError(f"seg_loss must be None or a utils.loss.OhemCELoss, got {type(seg_loss).__name__}")
+        if seg_loss is not None and not isinstance(seg_loss, (OhemCELoss, SegmentationLosses, SegFocalLoss)):
+            raise ValueError("seg_loss must be None or a utils.loss.OhemCELoss, SegmentationLosses(weight=...) or SegFocalLoss, got "
+                             f"{type(seg_loss).__name__}")
         n_seg_outputs = 3 if type(model.model[-2]).__name__ == "SegMaskBiSe" else 1
-        if seg_loss is not None and seg_loss.aux != (n_seg_outputs == 3):
+        if isinstance(seg_loss, OhemCELoss) and seg_loss.aux != (n_seg_outputs == 3):
             raise ValueError(f"OhemCELoss(aux={seg_loss.aux}) does not fit a seg head with {n_seg_outputs} output(s): aux=True is for "
                              "the BiSe head's [out, aux16, aux32]")
+        seg_weight = _check_weighted_seg_loss(seg_loss, n_seg_outputs, model.model[-2].c_out)
         assert next(model.parameters()).is_cuda, "model.cuda() first"
         self.model, self.hyp, self.batch_size = model, hyp, batch_size
         self.world_size, self.rank, self.accumulate, self.pg = world_size, rank, accumulate, process_group
@@ -347,7 +382,15 @@ class Trainer:
         self.n_seg_outputs = n_seg_outputs
         # BiSe returns [out, aux16, aux32]: loss1 + 1.5*aux_weight*loss2 + 0.5*aux_weight*loss3 (reference train.py:387-388, utils/loss.py:239-244)
         self.compute_seg_loss = SegmentationLosses(ignore_index=-1, aux=self.n_seg_outputs == 3, aux_num=2)
-        self.ohem = seg_loss                   # an OhemCELoss in place of compute_seg_loss, or None
+        self.ohem = seg_loss if isinstance(seg_loss, OhemCELoss) else None     # an OhemCELoss in place of compute_seg_loss, or None
+        # the class-weighted CE / focal loss in place of compute_seg_loss (SegFocalLoss with gamma = 0 is the weighted CE): its weights,
+        # uploaded once, and gamma; None for the other losses
+        self.seg_wf = None
+        if isinstance(seg_loss, (SegmentationLosses, SegFocalLoss)):
+            gamma = seg_loss.gamma if isinstance(seg_loss, SegFocalLoss) else 0.0
+            w = None if seg_weight is None else seg_weight.detach().to(device=next(model.parameters()).device, dtype=torch.float32).contiguous()
+            aux_weight = float(seg_loss.aux_weight) if isinstance(seg_loss, SegmentationLosses) and seg_loss.aux else None
+            self.seg_wf = (w, float(gamma), aux_weight)
         # seg CE + x8 upsample forward / backward in one kernel, no full-resolution logits: plain heads with 19 (Cityscapes) or 32 classes,
         # the instantiations in csrc/train.cu; other heads take autograd
         self.fused_seg = self.n_seg_outputs == 1 and model.model[-2].c_out in (19, 32)
@@ -507,6 +550,9 @@ class Trainer:
         if self.ohem is not None:
             return eng.train_backward_seg_ohem(plan, segtargets, self.ohem.thresh_t, factor=f, scale=self.scale,
                                                ignore_index=self.ohem.ignore_index) * f
+        if self.seg_wf is not None:
+            w, gamma, _ = self.seg_wf
+            return eng.train_backward_seg_loss(plan, segtargets, w, gamma, factor=f, scale=self.scale) * f
         return eng.train_backward_seg_ce(plan, segtargets, factor=f, scale=self.scale) * f
 
     def backward_seg(self, segimgs, segtargets):
@@ -516,6 +562,12 @@ class Trainer:
         pred = self.model(segimgs)
         if self.ohem is not None:
             loss = self.ohem(pred[1], segtargets)                   # the reference's call: the output, or the list of BiSe's three
+        elif self.seg_wf is not None:
+            w, gamma, aux_weight = self.seg_wf
+            outs = pred[1] if isinstance(pred[1], list) else [pred[1]]
+            parts = [seg_focal_loss(o, segtargets, w, gamma) for o in outs]
+            # BiSe: loss1 + 1.5 * aux_weight * loss2 + 0.5 * aux_weight * loss3 (reference utils/loss.py:239-244)
+            loss = parts[0] if len(parts) == 1 else parts[0] + aux_weight * 1.5 * parts[1] + aux_weight / 2.0 * parts[2]
         else:
             outs = pred[1] if isinstance(pred[1], list) else [pred[1]]
             loss = self.compute_seg_loss(*outs, segtargets)

@@ -1,5 +1,5 @@
 """Training losses behind the reference's surface: `ComputeLoss(model)(p, targets)` (reference utils/loss.py:89-217),
-`SegmentationLosses` (:221-262) and `OhemCELoss` (:303-328).  They consume the train-mode outputs of `Model.forward` ([x_i (B,na,ny,nx,5+nc)] and seg logits)
+`SegmentationLosses` (:221-262), `SegFocalLoss` (:279-297) and `OhemCELoss` (:303-328).  They consume the train-mode outputs of `Model.forward` ([x_i (B,na,ny,nx,5+nc)] and seg logits)
 and, through torch.autograd, seed the hand-written backward of the network (engine._TrainFunction).
 
 Design notes (not a transcription of the reference):
@@ -308,3 +308,81 @@ class OhemCELoss(nn.Module):
             raise ValueError("OhemCELoss(aux=True): preds must be the list [out, aux16, aux32]")
         return (self.forward_once(preds[0], labels) + self.aux_weight[0] * self.forward_once(preds[1], labels)
                 + self.aux_weight[1] * self.forward_once(preds[2], labels))
+
+
+class _SegFocal(torch.autograd.Function):
+    """SegFocalLoss.forward on the library (myolo_seg_focal_loss / _backward): the loss's coefficients stay on the device between the
+    passes"""
+
+    @staticmethod
+    def forward(ctx, pred, labels, weight, gamma, ignore_index, reduction):
+        from .. import _lib
+        B, Cc, H, W = pred.shape
+        L = _lib.lib()
+        need = int(L.myolo_seg_focal_loss_workspace_bytes())
+        ws = torch.empty(need, dtype=torch.uint8, device=pred.device)
+        loss = torch.empty((), dtype=torch.float32, device=pred.device)
+        red = _lib.REDUCTION_SUM if reduction == "sum" else _lib.REDUCTION_MEAN
+        _lib.check(L.myolo_seg_focal_loss(_lib.ptr(pred), _lib.ptr(labels), B, Cc, H, W, int(ignore_index), _lib.ptr(weight), float(gamma),
+                                          red, _lib.ptr(loss), _lib.ptr(ws), need, _lib.stream_ptr()))
+        ctx.save_for_backward(pred, labels)
+        ctx.ws, ctx.weight, ctx.gamma, ctx.ignore_index = ws, weight, float(gamma), int(ignore_index)
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        from .. import _lib
+        pred, labels = ctx.saved_tensors
+        B, Cc, H, W = pred.shape
+        g = grad_out.float().contiguous()
+        dx = torch.empty_like(pred)
+        _lib.check(_lib.lib().myolo_seg_focal_loss_backward(_lib.ptr(pred), _lib.ptr(labels), B, Cc, H, W, ctx.ignore_index,
+                                                            _lib.ptr(ctx.weight), ctx.gamma, _lib.ptr(g), _lib.ptr(dx), _lib.ptr(ctx.ws),
+                                                            ctx.ws.numel(), _lib.stream_ptr()))
+        return dx, None, None, None, None, None
+
+
+def seg_focal_loss(pred, labels, weight=None, gamma=0.0, ignore_index=-1, reduction="mean", who="SegFocalLoss"):
+    """SegFocalLoss's value on the library, differentiable in pred: (B, C, H, W) fp32 CUDA logits, (B, H, W) int64 CUDA labels, weight
+    None or C values.  gamma = 0 with reduction 'mean' is CrossEntropyLoss(weight=weight, ignore_index=ignore_index)."""
+    if not (isinstance(pred, torch.Tensor) and pred.is_cuda and pred.dtype == torch.float32 and pred.dim() == 4):
+        raise ValueError(f"{who}: expected (B, C, H, W) float32 CUDA logits")
+    if not (isinstance(labels, torch.Tensor) and labels.is_cuda and labels.dtype == torch.int64 and labels.device == pred.device
+            and tuple(labels.shape) == (pred.shape[0], pred.shape[2], pred.shape[3])):
+        raise ValueError(f"{who}: expected (B, H, W) = {(pred.shape[0], pred.shape[2], pred.shape[3])} int64 CUDA labels on the "
+                         "logits' device")
+    if weight is not None:
+        if weight.numel() != pred.shape[1]:
+            raise ValueError(f"{who}: {weight.numel()} class weights for {pred.shape[1]} classes")
+        weight = weight.to(device=pred.device, dtype=torch.float32).contiguous()
+    return _SegFocal.apply(pred.contiguous(), labels.contiguous(), weight, float(gamma), int(ignore_index), reduction)
+
+
+class SegFocalLoss(nn.Module):
+    """The reference's SegFocalLoss (utils/loss.py:279-297): with t' = the label on valid pixels and 0 on ignored ones (the reference's
+    `target * (target != ignore_index)`) and p = softmax(input, 1),
+        loss = reduce((1 - p_t')^gamma) * CrossEntropyLoss(weight=alpha, ignore_index, reduction)(input, target)
+    where both reductions are `reduction` (the reference overwrites the CE's): 'mean' gives the alpha-weighted mean CE times the mean of
+    (1 - p_t')^gamma over every pixel, ignored ones included; 'sum' the weighted CE sum times the sum.  'none' would broadcast the
+    (B, 1, H, W) focal factor against the (B, H, W) CE into (B, B, H, W) and is not provided (NotImplementedError).
+
+    Forward and backward are library kernels over (B, C, H, W) fp32 CUDA logits of any class count and (B, H, W) int64 CUDA labels, with no
+    host synchronisation.  Labels outside [0, C) other than ignore_index count as ignored (torch would raise).  With gamma < 1 a pixel whose
+    p_t' rounds to 1 has an infinite (1 - p_t')^(gamma - 1): its gradient is NaN, as the reference's autograd gives.  A batch with no valid
+    pixel gives a NaN loss, as the reference does."""
+
+    def __init__(self, gamma=2, alpha=None, ignore_index=-100, reduction="mean"):
+        super().__init__()
+        if reduction == "none":
+            raise NotImplementedError("SegFocalLoss(reduction='none'): the reference broadcasts the (B, 1, H, W) focal factor against the "
+                                      "(B, H, W) cross entropy into a (B, B, H, W) loss; use 'mean' or 'sum'")
+        if reduction not in ("mean", "sum"):
+            raise ValueError(f"SegFocalLoss: {reduction!r} is not a valid value for reduction")
+        gamma = float(gamma)
+        if not (math.isfinite(gamma) and gamma >= 0.0):
+            raise ValueError(f"SegFocalLoss: gamma must be finite and >= 0, got {gamma}")
+        self.gamma, self.ignore_index, self.reduction = gamma, int(ignore_index), reduction
+        self.register_buffer("weight", None if alpha is None else torch.as_tensor(alpha, dtype=torch.float32).reshape(-1).clone())
+
+    def forward(self, input_, target):
+        return seg_focal_loss(input_, target, self.weight, self.gamma, self.ignore_index, self.reduction)
