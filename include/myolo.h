@@ -475,6 +475,11 @@ int myolo_bilinear_nchw(const float* src, int B, int C, int h, int w, int H, int
 int myolo_conv_bn_silu(const void* x_nhwc_f16, int B, int H, int W, int ci, const float* w, int co, int k, int stride,
                        int dil, const float* gamma, const float* beta, const float* mean, const float* var, float eps,
                        const float* bias, int act, const void* residual_nhwc_f16, void* y_nhwc_f16, int path, void* stream);
+/* the same into a channel slice: y points at the slice's first channel of pixel 0 of a buffer with y_ctot channels per pixel */
+int myolo_conv_bn_silu_slice(const void* x_nhwc_f16, int B, int H, int W, int ci, const float* w, int co, int k, int stride,
+                             int dil, const float* gamma, const float* beta, const float* mean, const float* var, float eps,
+                             const float* bias, int act, const void* residual_nhwc_f16, void* y_nhwc_f16, int y_ctot, int path,
+                             void* stream);
 
 #ifdef __cplusplus
 }

@@ -63,9 +63,11 @@ struct ConvOp {
   CUtensorMap tmA[4], tmB;
   ConvTcParams p;
   int grid = 0, smem = 0;
+  int ctas_per_sm = 1;        // resident CTAs per SM the launch is sized for (conv_tc_prepare)
 };
 
-// decides whether the tensor-core (wgmma) path can run this op; fills tile geometry (no device pointers needed)
+// decides whether the tensor-core (wgmma) path can run this op (the output and residual views must already be resolved: their
+// base pointers are checked for 16-byte alignment)
 bool conv_tc_eligible(const ConvOp& op);
 // builds tensor maps / params; requires op.in/out/res/w/bias device pointers to be final
 int conv_tc_prepare(ConvOp& op, int num_sms);

@@ -14,8 +14,10 @@
 // * warp roles (384 threads = 3 warpgroups): warp 0 = TMA producer (one elected lane issues), warps 1-3 idle, warpgroups 1 and 2 =
 //   consumers.  Consumer warpgroup w issues m64nBNk16 wgmma for pixel rows [64w, 64w+64) of the tile into its register accumulators,
 //   releases each operand stage as soon as the MMAs that read it have retired, and runs the epilogue (bias, activation, residual,
-//   fp16 / fp32 stores) straight from the accumulator fragment while the producer already fetches the next tile.
-// * persistent grid (one CTA per SM, deep operand ring), programmatic dependent launch (prologue overlaps the previous kernel's tail).
+//   fp16 / fp32 stores) from the accumulator registers while the producer already fetches the next tile; fp16 tiles are written as
+//   16-byte vectors of 8 channels after a transpose within each quad of lanes (epilogue()).
+// * persistent grid (one CTA per SM with a deep operand ring; two for 1x1 layers with BN <= 64, see conv_tc_prepare), programmatic
+//   dependent launch (prologue overlaps the previous kernel's tail).
 //
 // Reference semantics: Conv.fuseforward (reference models/common.py:45-46) with BN folded as in
 // utils/torch_utils.py:182-202; Bottleneck shortcut add (models/common.py:105).
@@ -32,6 +34,8 @@ static constexpr int kMinResidentStages = 6;   // A stages a layer keeps next to
                                                // 3x3 s2 64->128 layer left 4 stages and ran 5 us slower than streamed with 6)
 static constexpr int kMaxStripBlocks = 4;      // channel blocks of a strip-mode layer (mma_strip_row instantiations)
 static constexpr int kSmemBudget = 227 * 1024;
+static constexpr int kSmemBudgetTwoCtas = 228 * 1024 / 2 - 1024;   // per CTA when two share an SM (228 KB, 1 KB reserved per CTA)
+static constexpr int kMinTwoCtaStages = 4;
 static constexpr int kBiasBytes = 8192;   // bias vector of the layer in shared memory (<= 1920 output channels: the data gradient
                                           // of SPP.cv2 has 1024)
 static constexpr int kSiluSfuEvery = 2;   // every n-th output channel of a 16-channel group takes the two-MUFU SiLU (balances the FMA
@@ -69,11 +73,37 @@ __device__ __forceinline__ float act_out(float v, int act, int ch) {
   return v;
 }
 
-// the residual values of the thread's epilogue fragment, all loads in flight at once.  Issued before the tile's last MMAs retire: loaded
-// one by one inside the store loop, each load waits behind the previous store (the output may alias the residual, as it does in the
-// data-gradient convs), and a tile's epilogue pays the global-load latency 2 * BN / 8 times.
+// The m64nBN accumulator fragment holds, for j < BN/8 and h < 2, output channels 8j + 2(lane%4) + {0,1} of tile row
+// 16*(warp%4) + lane/4 + 8h, in acc[4j + 2h + {0,1}]: the four lanes of a quad share a row, and lane q holds 32-bit word q (two fp16
+// channels) of every 8-channel group j.  The fp16 epilogue transposes each 4x4 block of words (groups 4g .. 4g+3) within the quad, so
+// that lane q owns all 8 channels of group 4g + q and writes them with one 16-byte store: a warp instruction then covers 64 contiguous
+// bytes in each of 8 rows instead of 16.  A last block of two groups (BN % 32 == 16) is padded with zero words that no lane stores.
 template <int BN>
-__device__ __forceinline__ void load_residual(const ConvTcParams& p, const TileCoord& tc, int row0, __half2 (&res)[2][BN / 8]) {
+struct EpiGroups { static constexpr int n = (BN + 31) / 32; };
+
+// before: lane q of the quad holds w[i] = word q of group i; after: w[i] = word i of group q.  Two butterfly steps (lane masks 1 and 2);
+// in each, a lane keeps the words whose index agrees with its own lane bit and trades the other two with its partner.  Every lane of
+// the warp takes part (full mask): callers run it before any per-row early exit.
+__device__ __forceinline__ void quad_transpose(uint32_t (&w)[4]) {
+  const int q = threadIdx.x & 3;
+#pragma unroll
+  for (int m = 1; m <= 2; m <<= 1) {
+    const bool hi = (q & m) != 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      if (i & m) continue;
+      const uint32_t recv = __shfl_xor_sync(0xffffffffu, hi ? w[i] : w[i | m], m);
+      if (hi) w[i] = recv;
+      else w[i | m] = recv;
+    }
+  }
+}
+
+// the residual values of the thread's epilogue, all loads in flight at once, each one 16-byte vector: the 8 channels of group 4g + lane%4
+// that this lane will store (so an output aliasing the residual, as in the data-gradient convs, is read and written by the same lane,
+// and all of the warp's loads are issued before its first store).  Issued before the tile's last MMAs retire.
+template <int BN>
+__device__ __forceinline__ void load_residual(const ConvTcParams& p, const TileCoord& tc, int row0, uint4 (&res)[2][EpiGroups<BN>::n]) {
   const int lane = threadIdx.x & 31;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -82,42 +112,73 @@ __device__ __forceinline__ void load_residual(const ConvTcParams& p, const TileC
     const bool in_map = py < p.Ho && px < p.Wo;
     const size_t pix = ((size_t)tc.b * p.Ho + py) * p.Wo + px;
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int n = tc.n0 + 8 * j + 2 * (lane & 3);
-      res[h][j] = in_map && n < p.out_c && n < p.Co ? *reinterpret_cast<const __half2*>(p.residual + pix * p.res_ctot + n)
-                                                     : __floats2half2_rn(0.f, 0.f);
+    for (int g = 0; g < EpiGroups<BN>::n; ++g) {
+      const int j = 4 * g + (lane & 3);
+      const int n = tc.n0 + 8 * j;
+      res[h][g] = in_map && j < BN / 8 && n < p.out_c && n < p.Co ? *reinterpret_cast<const uint4*>(p.residual + pix * p.res_ctot + n)
+                                                                  : make_uint4(0u, 0u, 0u, 0u);
     }
   }
 }
 
-// epilogue of one consumer warpgroup: the m64nBN accumulator fragment holds, for j < BN/8 and h < 2, output channels 8j + 2(lane%4) + {0,1}
-// of tile row 16*(warp%4) + lane/4 + 8h, in acc[4j + 2h + {0,1}]
+__device__ __forceinline__ uint32_t half2_bits(__half2 v) { return *reinterpret_cast<uint32_t*>(&v); }
+__device__ __forceinline__ __half2 bits_half2(uint32_t v) { return *reinterpret_cast<__half2*>(&v); }
+
+// epilogue of one consumer warpgroup: bias, activation, residual (fp32, before the single fp16 rounding), stores into the output slice
 template <int BN, bool RES>
-__device__ __forceinline__ void epilogue(const ConvTcParams& p, const float (&acc)[BN / 2], const __half2 (&res)[2][BN / 8],
+__device__ __forceinline__ void epilogue(const ConvTcParams& p, const float (&acc)[BN / 2], uint4 (&res)[2][EpiGroups<BN>::n],
                                          const float* bias_s, const TileCoord& tc, int row0) {
   const int lane = threadIdx.x & 31;
+  const int q = lane & 3;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int row = row0 + (lane >> 2) + 8 * h;
     const int py = tc.y0 + (row >> p.log2_tw), px = tc.x0 + (row & (p.tw - 1));
-    if (py >= p.Ho || px >= p.Wo) continue;
+    const bool in_map = py < p.Ho && px < p.Wo;   // uniform over the quad: the transposes below run for every row regardless
     const size_t pix = ((size_t)tc.b * p.Ho + py) * p.Wo + px;
+    if (p.out_mode == 0) {
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int c = 8 * j + 2 * (lane & 3);
-      const int n = tc.n0 + c;
-      float v0 = act_out(acc[4 * j + 2 * h] + bias_s[n], p.act, c);
-      float v1 = act_out(acc[4 * j + 2 * h + 1] + bias_s[n + 1], p.act, c + 1);
-      if (p.out_mode == 0) {
-        if (n >= p.out_c) continue;
-        if (RES && n < p.Co) {
-          const float2 r = __half22float2(res[h][j]);
-          v0 += r.x;
-          v1 += r.y;
+      for (int g = 0; g < EpiGroups<BN>::n; ++g) {
+        uint32_t r[4] = {0u, 0u, 0u, 0u};
+        if constexpr (RES) {                   // back to the fragment layout: r[i] = this lane's two channels of group 4g + i
+          r[0] = res[h][g].x;
+          r[1] = res[h][g].y;
+          r[2] = res[h][g].z;
+          r[3] = res[h][g].w;
+          quad_transpose(r);
         }
-        *reinterpret_cast<__half2*>(p.out_f16 + pix * p.out_ctot + n) = __floats2half2_rn(v0, v1);
-      } else if (n < p.out_ctot) {
-        *reinterpret_cast<float2*>(p.out_f32 + pix * p.out_ctot + n) = make_float2(v0, v1);
+        uint32_t w[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const int j = 4 * g + i;
+          w[i] = 0u;
+          if (j < BN / 8) {
+            const int c = 8 * j + 2 * q;
+            const int n = tc.n0 + c;
+            float v0 = act_out(acc[4 * j + 2 * h] + bias_s[n], p.act, c);
+            float v1 = act_out(acc[4 * j + 2 * h + 1] + bias_s[n + 1], p.act, c + 1);
+            if (RES && n < p.Co) {
+              const float2 rf = __half22float2(bits_half2(r[i]));
+              v0 += rf.x;
+              v1 += rf.y;
+            }
+            w[i] = half2_bits(__floats2half2_rn(v0, v1));
+          }
+        }
+        quad_transpose(w);                     // w = the 8 channels of group 4g + q
+        const int j = 4 * g + q;
+        const int n = tc.n0 + 8 * j;
+        if (in_map && j < BN / 8 && n < p.out_c)
+          *reinterpret_cast<uint4*>(p.out_f16 + pix * p.out_ctot + n) = make_uint4(w[0], w[1], w[2], w[3]);
+      }
+    } else if (in_map) {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int c = 8 * j + 2 * q;
+        const int n = tc.n0 + c;
+        const float v0 = act_out(acc[4 * j + 2 * h] + bias_s[n], p.act, c);
+        const float v1 = act_out(acc[4 * j + 2 * h + 1] + bias_s[n + 1], p.act, c + 1);
+        if (n < p.out_ctot) *reinterpret_cast<float2*>(p.out_f32 + pix * p.out_ctot + n) = make_float2(v0, v1);
       }
     }
   }
@@ -160,8 +221,8 @@ __device__ __forceinline__ void mma_strip_row(float (&acc)[BN / 2], uint32_t sa,
   wgmma_commit();
 }
 
-template <int KC, int BN, bool RES>
-__global__ void __launch_bounds__(kNumThreads, 1)
+template <int KC, int BN, bool RES, int CTAS_PER_SM>
+__global__ void __launch_bounds__(kNumThreads, CTAS_PER_SM)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__ CUtensorMap tmA1,
                const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmA3,
                const __grid_constant__ CUtensorMap tmB, const __grid_constant__ ConvTcParams p) {
@@ -296,7 +357,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
         if (++stage == S) { stage = 0; phase ^= 1; }
       }
       const int row0 = cw * 64 + (warp & 3) * 16;
-      __half2 res[2][BN / 8];
+      uint4 res[2][EpiGroups<BN>::n];
       if constexpr (RES) load_residual<BN>(p, t, row0, res);
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
@@ -383,8 +444,10 @@ bool conv_tc_eligible(const ConvOp& op) {
   if (op.stride == 2 && ((op.in.H | op.in.W) & 1)) return false;
   if (op.in.ctot % 8 != 0) return false;
   if (op.out.dtype == MYOLO_F16) {
-    if (op.out.C % 8 != 0 || op.out.ctot % 8 != 0) return false;
-    if (op.has_res && (op.res.dtype != MYOLO_F16 || op.res.ctot % 8 != 0 || op.Co % 16 != 0)) return false;
+    // the epilogue stores (and loads the residual in) 16-byte vectors of 8 channels: the slices must start on a 16-byte boundary
+    auto aligned16 = [](const void* ptr) { return reinterpret_cast<uintptr_t>(ptr) % 16 == 0; };
+    if (op.out.C % 8 != 0 || op.out.ctot % 8 != 0 || !aligned16(op.out.base)) return false;
+    if (op.has_res && (op.res.dtype != MYOLO_F16 || op.res.ctot % 8 != 0 || op.Co % 16 != 0 || !aligned16(op.res.base))) return false;
   } else {
     if (op.has_res || op.out.ctot % 4 != 0) return false;
   }
@@ -466,12 +529,20 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
     p.strip_sub_bytes = (int)align_up(p.strip_box_bytes, 1024);
     p.strip = (kSmemBudget - misc - b_resident_bytes) / (p.cblocks * p.strip_sub_bytes) >= 2;
   }
+  // two CTAs per SM: a 1x1 layer with resident weights and BN <= 64 (few MMAs per tile, so a tile is mostly barrier waits and the
+  // epilogue) keeps a second CTA on each SM, whose waits and MMAs overlap the first one's epilogue.  Each CTA gets half the shared memory,
+  // with at least kMinTwoCtaStages A stages.  Not with a residual: those kernels do not fit the 80 registers of two 384-thread CTAs.
+  op.ctas_per_sm = 1;
+  if (p.resident && p.taps == 1 && p.BN <= 64 && !op.has_res && p.total_tiles > num_sms &&
+      b_resident_bytes + kMinTwoCtaStages * p.a_stage_bytes + misc <= kSmemBudgetTwoCtas)
+    op.ctas_per_sm = 2;
+  const int smem_budget = op.ctas_per_sm == 2 ? kSmemBudgetTwoCtas : kSmemBudget;
   int S;
   if (p.resident) {
-    grid = grid_resident;
+    grid = op.ctas_per_sm == 2 ? (p.total_tiles < 2 * num_sms ? p.total_tiles : 2 * num_sms) / p.n_tiles_n * p.n_tiles_n : grid_resident;
     p.b_stage_bytes = 0;
     if (p.strip) p.a_stage_bytes = p.cblocks * p.strip_sub_bytes;
-    S = (kSmemBudget - misc - b_resident_bytes) / p.a_stage_bytes;
+    S = (smem_budget - misc - b_resident_bytes) / p.a_stage_bytes;
     p.b_bytes = b_resident_bytes;
   } else {
     S = (kSmemBudget - misc) / (p.a_stage_bytes + p.b_stage_bytes);
@@ -518,15 +589,26 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
   return 0;
 }
 
-template <int KC, int BN, bool RES>
-static cudaError_t launch_bn(const ConvOp& op, const cudaLaunchConfig_t& cfg) {
+template <int KC, int BN, bool RES, int CTAS_PER_SM>
+static cudaError_t launch_kernel(const ConvOp& op, const cudaLaunchConfig_t& cfg) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<KC, BN, RES>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
+    cudaError_t e = cudaFuncSetAttribute(conv_tc_kernel<KC, BN, RES, CTAS_PER_SM>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBudget);
+    if (e == cudaSuccess && CTAS_PER_SM == 2)   // two CTAs need the whole 228 KB carve-out, not whatever the driver would pick
+      e = cudaFuncSetAttribute(conv_tc_kernel<KC, BN, RES, CTAS_PER_SM>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                               cudaSharedmemCarveoutMaxShared);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  return cudaLaunchKernelEx(&cfg, conv_tc_kernel<KC, BN, RES>, op.tmA[0], op.tmA[1], op.tmA[2], op.tmA[3], op.tmB, op.p);
+  return cudaLaunchKernelEx(&cfg, conv_tc_kernel<KC, BN, RES, CTAS_PER_SM>, op.tmA[0], op.tmA[1], op.tmA[2], op.tmA[3], op.tmB, op.p);
+}
+
+template <int KC, int BN, bool RES>
+static cudaError_t launch_bn(const ConvOp& op, const cudaLaunchConfig_t& cfg) {
+  if constexpr (BN <= 64 && !RES)
+    if (op.ctas_per_sm == 2) return launch_kernel<KC, BN, RES, 2>(op, cfg);
+  if (op.ctas_per_sm != 1) return cudaErrorInvalidValue;
+  return launch_kernel<KC, BN, RES, 1>(op, cfg);
 }
 
 template <int KC, bool RES>

@@ -786,7 +786,7 @@ extern "C" int64_t myolo_plan_last_launch_count(const myolo_plan* pl) { return p
 // which kernel a conv op of the plan takes and how it is tiled (valid after the first forward): info[0..11] =
 // {1 wgmma / 0 CUDA-core, grid, dynamic smem bytes, BN, pipeline stages, mode (0: one TMA box per tap, 1: one strip per filter row),
 //  weights-stationary (1: the CTA keeps its weight slice in shared memory),
-//  tiles per accumulator round (always 1), total tiles, n tiles in N, kc, CTAs per SM (always 1)}
+//  tiles per accumulator round (always 1), total tiles, n tiles in N, kc, CTAs per SM (1 or 2)}
 extern "C" int myolo_plan_conv_info(myolo_plan* pl, int op_index, int32_t* info) {
   MYOLO_REQUIRE(pl && info && op_index >= 0 && op_index < (int)pl->ops.size(), "conv_info: bad arguments");
   MYOLO_REQUIRE(pl->ops[op_index].kind == MYOLO_OP_CONV, "conv_info: op %d is not a conv", op_index);
@@ -798,7 +798,7 @@ extern "C" int myolo_plan_conv_info(myolo_plan* pl, int op_index, int32_t* info)
   if (c.use_tc) {
     info[1] = c.grid; info[2] = c.smem; info[3] = c.p.BN; info[4] = c.p.num_stages; info[5] = c.p.strip;
     info[6] = c.p.resident; info[7] = 1; info[8] = c.p.total_tiles; info[9] = c.p.n_tiles_n; info[10] = c.p.kc;
-    info[11] = 1;
+    info[11] = c.ctas_per_sm;
   }
   return 0;
 }
@@ -1599,10 +1599,10 @@ extern "C" int myolo_allreduce_grads(float* flat_grad, int64_t n, void* nccl_com
 // ------------------------------------------------------------------------------------------------
 // standalone fused conv (per-op parity tests, ncu captures)
 // ------------------------------------------------------------------------------------------------
-extern "C" int myolo_conv_bn_silu(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,
-                                  const float* gamma, const float* beta, const float* mean, const float* var, float eps,
-                                  const float* bias, int act, const void* residual, void* y, int path, void* stream) {
-  MYOLO_REQUIRE(x && w && y && B > 0 && H > 0 && W > 0 && ci > 0 && co > 0, "conv_bn_silu: bad arguments");
+extern "C" int myolo_conv_bn_silu_slice(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,
+                                        const float* gamma, const float* beta, const float* mean, const float* var, float eps,
+                                        const float* bias, int act, const void* residual, void* y, int y_ctot, int path, void* stream) {
+  MYOLO_REQUIRE(x && w && y && B > 0 && H > 0 && W > 0 && ci > 0 && co > 0 && y_ctot >= co, "conv_bn_silu: bad arguments");
   MYOLO_REQUIRE(ci % 16 == 0 && co % 8 == 0, "conv_bn_silu: standalone entry needs ci %% 16 == 0 and co %% 8 == 0");
   int sms = 0;
   int rc = check_device(&sms);
@@ -1618,7 +1618,7 @@ extern "C" int myolo_conv_bn_silu(const void* x, int B, int H, int W, int ci, co
   const int pad = dil * (k / 2);
   const int ho = (H + 2 * pad - dil * (k - 1) - 1) / stride + 1, wo = (W + 2 * pad - dil * (k - 1) - 1) / stride + 1;
   c.in = TensorView{const_cast<void*>(x), B, H, W, ci, ci, MYOLO_F16};
-  c.out = TensorView{y, B, ho, wo, co, co, MYOLO_F16};
+  c.out = TensorView{y, B, ho, wo, co, y_ctot, MYOLO_F16};
   c.has_res = residual != nullptr;
   if (c.has_res) c.res = TensorView{const_cast<void*>(residual), B, ho, wo, co, co, MYOLO_F16};
   c.k = k;
@@ -1651,4 +1651,11 @@ extern "C" int myolo_conv_bn_silu(const void* x, int B, int H, int W, int ci, co
     rc = MYOLO_E_CUDA;
   }
   return rc;
+}
+
+extern "C" int myolo_conv_bn_silu(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,
+                                  const float* gamma, const float* beta, const float* mean, const float* var, float eps,
+                                  const float* bias, int act, const void* residual, void* y, int path, void* stream) {
+  return myolo_conv_bn_silu_slice(x, B, H, W, ci, w, co, k, stride, dil, gamma, beta, mean, var, eps, bias, act, residual, y, co, path,
+                                  stream);
 }
