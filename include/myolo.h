@@ -294,6 +294,25 @@ int myolo_anchor_metric(const void* wh, int wh_dtype, int64_t n, const void* k, 
 int64_t myolo_anchor_evolve_workspace_bytes(int64_t n);
 int myolo_anchor_evolve(const float* wh, int64_t n, const double* k0, int na, const double* v, int gen, double thr, double* k_out,
                         float* f_out, float* fg_out, int32_t* accepted_out, void* workspace, int64_t workspace_bytes, void* stream);
+/* scipy.cluster.vq.kmeans(obs, k, iter=restarts, thresh) with an int k (kmean_anchors' `kmeans(wh / s, n, iter=30)`,
+ * utils/autoanchor.py:125), bit for bit with scipy >= 1.17: one CTA per restart, all restarts in one ordinary launch.  obs: (n, d) fp64
+ * device; init_idx: (restarts, k) int64 device, each restart's start rows (numpy.random's `choice(n, k, replace=False)`, drawn by the
+ * caller as scipy's `_kpoints` draws them).  Per restart: Lloyd iterations (vq without fused multiply-adds, the first nearest code;
+ * numpy's pairwise mean of the distances; per-cluster sequential fp64 member sums in observation order, empty clusters dropped) while
+ * |prev - cur| > thresh from prev = inf, then one more vq with the final book for its distortion.  Outputs (device): books
+ * (restarts, k, d) fp64 (the first book_k[r] rows valid, the rest zero), book_k (restarts) int32, dists (restarts) fp64, iters (restarts)
+ * int32 (Lloyd iterations), best int32 (the first restart with the smallest distortion: scipy's winner), status int32 (zeroed by the call;
+ * bits MYOLO_KMEANS_MAX_ITER: a restart was still moving after max_iter iterations, MYOLO_KMEANS_BAD_INDEX: an init_idx row outside
+ * [0, n)).  Needs d == 2, 1 <= k <= MYOLO_KMEANS_KMAX, k <= n < 2^30, max_iter >= 1 and restarts at most the co-resident CTA count of
+ * the current device; else MYOLO_E_INVALID.  workspace: device, at least myolo_kmeans_workspace_bytes(n, k, restarts).  No host
+ * synchronisation. */
+#define MYOLO_KMEANS_KMAX 32
+#define MYOLO_KMEANS_MAX_ITER 1
+#define MYOLO_KMEANS_BAD_INDEX 2
+int64_t myolo_kmeans_workspace_bytes(int64_t n, int k, int restarts);
+int myolo_kmeans(const double* obs, int64_t n, int d, const int64_t* init_idx, int k, int restarts, double thresh, int max_iter,
+                 double* books, int32_t* book_k, double* dists, int32_t* iters, int32_t* best, int32_t* status, void* workspace,
+                 int64_t workspace_bytes, void* stream);
 
 /* OhemCELoss.forward_once (reference utils/loss.py:321-328) over full-resolution logits (B, C, H, W) fp32 NCHW, any C, and labels (B, H, W)
  * int64, with the selection of myolo_plan_backward_seg_ohem.  myolo_seg_ohem_loss writes the loss to loss_out (device float) and leaves

@@ -65,4 +65,10 @@ int anchor_evolve_workspace_bytes(long n, int64_t* bytes);
 int launch_anchor_evolve(const float* wh, long n, const double* k0, int na, const double* v, int gen, float thr, double* k_out,
                          float* f_out, float* fg_out, int* accepted_out, void* workspace, int64_t workspace_bytes, cudaStream_t s);
 
+// scipy's k-means (kmeans.cu): one CTA per restart
+int64_t kmeans_workspace_bytes(long n, int restarts);
+int launch_kmeans(const double* obs, long n, const int64_t* init_idx, int k, int restarts, double thresh, int max_iter, double* books,
+                  int32_t* book_k, double* dists, int32_t* iters, int32_t* best, int32_t* status, void* ws, int64_t ws_bytes,
+                  cudaStream_t s);
+
 }  // namespace myolo

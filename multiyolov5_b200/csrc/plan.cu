@@ -1580,6 +1580,26 @@ extern "C" int myolo_anchor_evolve(const float* wh, int64_t n, const double* k0,
                               (cudaStream_t)stream);
 }
 
+extern "C" int64_t myolo_kmeans_workspace_bytes(int64_t n, int k, int restarts) {
+  if (n < 1 || n >= (int64_t(1) << 30) || k < 1 || restarts < 1) return -1;
+  return kmeans_workspace_bytes((long)n, restarts);
+}
+
+extern "C" int myolo_kmeans(const double* obs, int64_t n, int d, const int64_t* init_idx, int k, int restarts, double thresh, int max_iter,
+                            double* books, int32_t* book_k, double* dists, int32_t* iters, int32_t* best, int32_t* status, void* workspace,
+                            int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_kmeans");
+  MYOLO_REQUIRE(obs && init_idx && books && book_k && dists && iters && best && status && workspace && restarts >= 1 && max_iter >= 1,
+                "kmeans: bad arguments");
+  MYOLO_REQUIRE(d == 2, "kmeans: d = %d features, only d = 2 is built", d);
+  MYOLO_REQUIRE(k >= 1 && k <= MYOLO_KMEANS_KMAX, "kmeans: k = %d, needs 1 <= k <= %d", k, MYOLO_KMEANS_KMAX);
+  MYOLO_REQUIRE(n >= k && n < (int64_t(1) << 30), "kmeans: n = %lld observations, needs k <= n < 2^30", (long long)n);
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_kmeans(obs, (long)n, init_idx, k, restarts, thresh, max_iter, books, book_k, dists, iters, best, status, workspace,
+                       workspace_bytes, (cudaStream_t)stream);
+}
+
 extern "C" int myolo_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay, void* stream) {
   NvtxRange nvtx_("myolo_ema_update");
   int rc = check_device(nullptr);

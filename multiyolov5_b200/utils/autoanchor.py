@@ -10,11 +10,12 @@ Same names, signatures, printed lines and random draws as the reference:
 `dataset` is a `utils.datasets.DeviceImageCache` (its original (h0, w0) `shapes0` and float32 `labels`) or any object with the reference
 dataset's `shapes` ((n, 2) [w, h]) and `labels`.  A path (`str`) raises NotImplementedError: loading data files is not built.
 
-What runs where.  The ratio metric and the 1000-generation evolution run on the GPU (csrc/autoanchor.cu): the evolution is one persistent
-kernel, with every generation's mutation factors drawn up front on the host from `numpy.random` in the reference's order and count (its loop
-never reads the anchors or the fitness).  So a seeded run leaves `numpy.random` and `random` where the reference leaves them, and the
-augmenters that draw next see the same streams.  Scipy's `kmeans(wh / s, n, iter=30)` is the reference's own call (it also draws from
-numpy's global state), as are the numpy filtering and whitening, `print_results`' sort and the torch writes into the Detect buffers.
+What runs where.  The ratio metric, scipy's k-means and the 1000-generation evolution run on the GPU.  The evolution is one persistent
+kernel (csrc/autoanchor.cu), with every generation's mutation factors drawn up front on the host from `numpy.random` in the reference's
+order and count (its loop never reads the anchors or the fitness).  `kmeans(wh / s, n, iter=30)` returns what scipy.cluster.vq.kmeans
+returns, bit for bit, with all restarts in one launch (csrc/kmeans.cu) from starts drawn up front as scipy draws them; scipy is not needed
+at run time.  So a seeded run leaves `numpy.random` and `random` where the reference leaves them, and the augmenters that draw next see the
+same streams.  The numpy filtering and whitening, `print_results`' sort and the torch writes into the Detect buffers stay on the host.
 
 Exactness.  Each generation's fitness is the fp32 mean of per-label terms, summed exactly in fp64 (DESIGN.md section 3b), and every
 comparison runs in the dtype torch uses (fp64 where the reference divides an fp32 tensor by a float64 numpy array).  Torch's own fp32
@@ -142,6 +143,63 @@ def evolve(wh, k0, v, thr):
     return (k_out.cpu().numpy().reshape(na, 2), np.float32(f[0]), np.float32(f[1]), fg.cpu().numpy()[:gen].copy(), int(acc.item()))
 
 
+KMEANS_ITER_CAP = 1000      # scipy has no cap; restarts on label sets take 9 to about 130 Lloyd iterations
+
+
+def kmeans_restarts(obs, idx, thresh=1e-5, max_iter=KMEANS_ITER_CAP):
+    """every restart of scipy's k-means from the start rows idx (restarts, k) int, in one launch (myolo_kmeans) and one read-back:
+    ([book (k'_r, d) float64 per restart], distortions (restarts,) float64, Lloyd iterations (restarts,) int32, index of scipy's winner).
+    obs: (n, d) float64 numpy.  A restart still moving after max_iter iterations raises MyoloError."""
+    n, d = obs.shape
+    R, k = idx.shape
+    dev = _device()
+    L = _lib.lib()
+    need = int(L.myolo_kmeans_workspace_bytes(n, k, R))
+    if need < 0:
+        raise _lib.MyoloError(f"kmeans: n = {n}, k = {k}, {R} restarts: no workspace size")
+    obs_d = torch.from_numpy(np.ascontiguousarray(obs, dtype=np.float64)).to(dev)
+    idx_d = torch.from_numpy(np.ascontiguousarray(idx, dtype=np.int64)).to(dev)
+    ws = torch.empty(need, dtype=torch.uint8, device=dev)
+    # one output buffer: books (R, k, d) f64 | dists (R) f64 | book_k (R) i32 | iters (R) i32 | best i32 | status i32
+    nb = R * k * d * 8
+    o_dist, o_bk, o_it, o_best = nb, nb + 8 * R, nb + 12 * R, nb + 16 * R
+    out = torch.zeros(o_best + 8, dtype=torch.uint8, device=dev)
+    p = out.data_ptr()
+    _lib.check(L.myolo_kmeans(_lib.ptr(obs_d), n, d, _lib.ptr(idx_d), k, R, float(thresh), int(max_iter), p, p + o_bk, p + o_dist, p + o_it,
+                              p + o_best, p + o_best + 4, _lib.ptr(ws), need, _lib.stream_ptr()))
+    buf = out.cpu().numpy()
+    books = buf[:nb].view(np.float64).reshape(R, k, d)
+    book_k = buf[o_bk:o_it].view(np.int32)
+    best, status = (int(v) for v in buf[o_best:].view(np.int32))
+    if status & _lib.KMEANS_MAX_ITER:
+        raise _lib.MyoloError(f"kmeans: a restart was still moving after {max_iter} Lloyd iterations")
+    if status:
+        raise _lib.MyoloError(f"kmeans: start indices outside [0, {n})")
+    dists, iters = buf[o_dist:o_bk].view(np.float64).copy(), buf[o_it:o_best].view(np.int32).copy()
+    return [books[r, :book_k[r]].copy() for r in range(R)], dists, iters, best
+
+
+def kmeans(obs, k, iter=20, thresh=1e-5):
+    """scipy.cluster.vq.kmeans(obs, k, iter, thresh) for an int k on the device, bit for bit: (code book (k', 2) float64, mean distance
+    float64).  obs: (n, 2) float64 numpy, e.g. kmean_anchors' whitened `wh / s`.  Every restart's start is drawn up front from numpy's
+    global state exactly as scipy draws them (`choice(n, k, replace=False)` per restart), so `numpy.random` ends where scipy leaves it and
+    n < k raises numpy's ValueError from that call, as in scipy.  The checks before the draws raise scipy's ValueErrors."""
+    obs = np.asarray(obs)
+    if not np.isfinite(obs).all():
+        raise ValueError("array must not contain infs or NaNs")
+    if iter < 1:
+        raise ValueError(f"iter must be at least 1, got {iter}")
+    if k < 1:
+        raise ValueError(f"Asked for {k} clusters.")
+    if obs.dtype != np.float64 or obs.ndim != 2:
+        raise TypeError("kmeans: obs must be a (n, d) float64 array")
+    idx = np.stack([np.random.choice(obs.shape[0], k, replace=False) for _ in range(iter)])
+    books, dists, _, best = kmeans_restarts(obs, idx, thresh)
+    if best < 0:
+        raise ValueError("kmeans: no restart has a finite distortion")
+    return books[best], np.float64(dists[best])
+
+
 def _mean32(count, n):
     """torch's fp32 mean of `n` values that sum to the integer `count` (exact in fp32 below 2^24): the sum divided by n in fp32"""
     return np.float32(np.float32(count) / np.float32(n))
@@ -190,7 +248,6 @@ def check_anchors(dataset, model, thr=4.0, imgsz=640):
 def kmean_anchors(dataset, n=9, img_size=640, thr=4.0, gen=1000, verbose=True):
     """k-means anchors of the dataset's labels, evolved by the reference's genetic algorithm on the device.  thr: hyp['anchor_t'].
     Returns the (n, 2) float64 anchors, sorted small to large."""
-    from scipy.cluster.vq import kmeans
     thr = 1. / thr
     prefix = colorstr("autoanchor: ")
     shapes, labels = dataset_shapes_labels(dataset)
