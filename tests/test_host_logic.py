@@ -77,6 +77,65 @@ def test_planner_op_and_buffer_invariants(tag, B, H, W):
     assert sum(pb.det_rows) == 3 * ((H // 8) * (W // 8) + (H // 16) * (W // 16) + (H // 32) * (W // 32))
 
 
+def execution_intervals(pb):
+    """[first, last] execution position of every base buffer of an inference plan, in the order the executor runs the ops: INPUT_FOCUS
+    first, a group member in its head's launch, DETECT_DECODE and SEG_UPSAMPLE after the captured graph (csrc/plan.cu myolo_plan_forward)"""
+    from multiyolov5_b200 import _lib
+    n = len(pb.ops)
+    pos, head = [], -1
+    for i, o in enumerate(pb.ops):
+        if o.flags & _lib.OP_GROUP_HEAD:
+            head = i
+        if o.kind == _lib.OP_INPUT_FOCUS:
+            pos.append(-1)
+        elif o.kind in (_lib.OP_DETECT_DECODE, _lib.OP_SEG_UPSAMPLE):
+            pos.append(n)
+        else:
+            pos.append(head if o.flags & _lib.OP_GROUP_MEMBER else i)
+    live = {}
+    for o, p in zip(pb.ops, pos):
+        for v in (o.in_, o.in2, o.out):
+            if v is not None:
+                b = v.buf.alias_of or v.buf
+                f, l = live.get(b.id, (p, p))
+                live[b.id] = (min(f, p), max(l, p))
+    return pos, live
+
+
+@pytest.mark.parametrize("tag", list(NETS))
+def test_workspace_packing_respects_execution_order(tag):
+    """buffers that share workspace bytes are never live at the same time in EXECUTION order (which differs from plan order: group
+    members run in their head's launch, the caller-output ops after the graph), and no member of a grouped launch writes what another
+    member of the same launch reads"""
+    from multiyolov5_b200 import _lib
+    from multiyolov5_b200.models.yolo import Model
+    from multiyolov5_b200.plan import build_plan
+    model = Model(NETS[tag])
+    for B in (1, 2, 16):
+        for H, W in ((128, 256), (256, 512), (416, 736), (512, 1024), (640, 640)):
+            pb = build_plan(model, B, H, W)
+            pos, live = execution_intervals(pb)
+            bufs = {b.id: b for b in pb.bufs if b.alias_of is None and b.id in live}
+            spans = sorted((b.offset, b.offset + b.nbytes(B), b.id) for b in bufs.values())
+            for i, (o0, e0, a) in enumerate(spans):
+                for o1, e1, b in spans[i + 1:]:
+                    if o1 >= e0:
+                        break
+                    (fa, la), (fb, lb) = live[a], live[b]
+                    assert la < fb or lb < fa, (B, H, W, f"buffers {a} and {b} share bytes and are live together: {live[a]} {live[b]}")
+            for h in (i for i, o in enumerate(pb.ops) if o.flags & _lib.OP_GROUP_HEAD):
+                members = pb.ops[h:h + pb.ops[h].aux[7]]
+                for j, m in enumerate(members):
+                    for k, r in enumerate(members):
+                        for v in (r.in_, r.in2):
+                            if j == k or v is None:
+                                continue
+                            wb, vb = m.out.buf.alias_of or m.out.buf, v.buf.alias_of or v.buf
+                            same = wb is vb and m.out.c_off < v.c_off + v.c and v.c_off < m.out.c_off + m.out.c
+                            apart = wb is not vb and (wb.offset + wb.nbytes(B) <= vb.offset or vb.offset + vb.nbytes(B) <= wb.offset)
+                            assert not same and (wb is vb or apart), (B, H, W, h, j, k)
+
+
 def test_adaptive_bins_match_torch():
     from multiyolov5_b200.plan import adaptive_bins
     import torch.nn.functional as F
