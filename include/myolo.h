@@ -314,6 +314,29 @@ int myolo_kmeans(const double* obs, int64_t n, int d, const int64_t* init_idx, i
                  double* books, int32_t* book_k, double* dists, int32_t* iters, int32_t* best, int32_t* status, void* workspace,
                  int64_t workspace_bytes, void* stream);
 
+/* --image-weights (reference train.py:255,305-316, utils/general.py:216-240), bit for bit with numpy 2 and Python 3.12's random.  A label's
+ * class is its float32 class value truncated toward zero, as astype(int) does; a class outside [0, nc) is skipped and sets
+ * MYOLO_IW_BAD_CLASS.  Every sum over the nc classes is numpy's np.add.reduce order (pairwise blocks of 8 accumulators, added to the
+ * initial 0.0), in fp64 without fused multiply-adds.  status: int32 device word, only OR-ed (the caller zeroes it).  Needs
+ * 1 <= nc <= MYOLO_IW_NC_MAX; else MYOLO_E_INVALID.  All pointers are device pointers; no host synchronisation.
+ *   myolo_class_weights   labels_to_class_weights(labels, nc): cls is the (n_labels) float32 class column of every label; counts (nc) int64
+ *                         the exact per-class counts; weights (nc) fp64 = (1 / max(count, 1)) / their sum.
+ *   myolo_image_weights   labels_to_image_weights(labels, nc, cw): image i's labels are cls[offsets[i] .. offsets[i + 1]) (offsets:
+ *                         n + 1 int64); iw (n) fp64 = the sum over c of cw[c] * count_i(c).
+ *   myolo_weighted_draw   random.choices(range(n), weights=w, k=n) given its n random() values u (fp64): cum (n) fp64 the sequential
+ *                         cumulative sums (itertools.accumulate), total (1) fp64 = cum[n - 1] + 0.0; total <= 0 sets MYOLO_IW_TOTAL_NONPOS,
+ *                         a non-finite total MYOLO_IW_TOTAL_NONFINITE, and then idx is left unwritten; else idx (n) int32 =
+ *                         bisect_right(cum, u[i] * total, 0, n - 1).  Needs 1 <= n < 2^31. */
+#define MYOLO_IW_NC_MAX 1024
+#define MYOLO_IW_BAD_CLASS 1
+#define MYOLO_IW_TOTAL_NONPOS 2
+#define MYOLO_IW_TOTAL_NONFINITE 4
+int myolo_class_weights(const float* cls, int64_t n_labels, int nc, int64_t* counts, double* weights, int32_t* status, void* stream);
+int myolo_image_weights(const float* cls, const int64_t* offsets, int64_t n, const double* cw, int nc, double* iw, int32_t* status,
+                        void* stream);
+int myolo_weighted_draw(const double* w, const double* u, int64_t n, double* cum, double* total, int32_t* idx, int32_t* status,
+                        void* stream);
+
 /* OhemCELoss.forward_once (reference utils/loss.py:321-328) over full-resolution logits (B, C, H, W) fp32 NCHW, any C, and labels (B, H, W)
  * int64, with the selection of myolo_plan_backward_seg_ohem.  myolo_seg_ohem_loss writes the loss to loss_out (device float) and leaves
  * its selection in the workspace; myolo_seg_ohem_loss_backward then writes grad_logits = (*grad_out) * d loss / d logits (grad_out: device

@@ -40,12 +40,14 @@ EXPORTS = [
     "myolo_adam_scalars", "myolo_ema_update", "myolo_plan_set_extra", "myolo_collate_quad", "myolo_plan_set_bn_sync",
     "myolo_plan_backward_seg_ohem", "myolo_seg_ohem_loss", "myolo_seg_ohem_loss_backward", "myolo_seg_ohem_loss_workspace_bytes",
     "myolo_anchor_metric", "myolo_anchor_metric_workspace_bytes", "myolo_anchor_evolve", "myolo_anchor_evolve_workspace_bytes",
-    "myolo_kmeans", "myolo_kmeans_workspace_bytes",
+    "myolo_kmeans", "myolo_kmeans_workspace_bytes", "myolo_class_weights", "myolo_image_weights", "myolo_weighted_draw",
     "myolo_plan_backward_seg_loss", "myolo_seg_focal_loss", "myolo_seg_focal_loss_backward", "myolo_seg_focal_loss_workspace_bytes",
 ]
 REDUCTION_MEAN, REDUCTION_SUM = 0, 1        # include/myolo.h: MYOLO_REDUCTION_* of myolo_seg_focal_loss
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
 KMEANS_MAX_ITER, KMEANS_BAD_INDEX = 1, 2                                 # include/myolo.h: bits of myolo_kmeans' status word
+IW_BAD_CLASS, IW_TOTAL_NONPOS, IW_TOTAL_NONFINITE = 1, 2, 4              # include/myolo.h: bits of the image-weights status word
+IW_NC_MAX = 1024                                                         # include/myolo.h MYOLO_IW_NC_MAX
 
 
 class BufDesc(C.Structure):
@@ -158,6 +160,9 @@ def lib():
     L.myolo_kmeans_workspace_bytes.argtypes = [i64, i32, i32]
     L.myolo_kmeans_workspace_bytes.restype = i64
     L.myolo_kmeans.argtypes = [vp, i64, i32, vp, i32, i32, C.c_double, i32, vp, vp, vp, vp, vp, vp, vp, i64, vp]
+    L.myolo_class_weights.argtypes = [vp, i64, i32, vp, vp, vp, vp]
+    L.myolo_image_weights.argtypes = [vp, vp, i64, vp, i32, vp, vp, vp]
+    L.myolo_weighted_draw.argtypes = [vp, vp, i64, vp, vp, vp, vp, vp]
     L.myolo_plan_read_grad_view.argtypes = [vp, View, vp, vp]
     L.myolo_plan_set_seed.argtypes = [vp, C.c_uint64]
     L.myolo_plan_set_defer_running.argtypes = [vp, i32]

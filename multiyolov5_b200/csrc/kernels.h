@@ -71,4 +71,12 @@ int launch_kmeans(const double* obs, long n, const int64_t* init_idx, int k, int
                   int32_t* book_k, double* dists, int32_t* iters, int32_t* best, int32_t* status, void* ws, int64_t ws_bytes,
                   cudaStream_t s);
 
+// --image-weights (image_weights.cu): class weights, image weights, the weighted draw
+int launch_class_weights(const float* cls, long long n_labels, int nc, unsigned long long* counts, double* weights, int32_t* status,
+                         cudaStream_t s);
+int launch_image_weights(const float* cls, const int64_t* offsets, long long n, const double* cw, int nc, double* iw, int32_t* status,
+                         cudaStream_t s);
+int launch_weighted_draw(const double* w, const double* u, long long n, double* cum, double* total, int32_t* idx, int32_t* status,
+                         cudaStream_t s);
+
 }  // namespace myolo

@@ -1600,6 +1600,37 @@ extern "C" int myolo_kmeans(const double* obs, int64_t n, int d, const int64_t* 
                        workspace_bytes, (cudaStream_t)stream);
 }
 
+extern "C" int myolo_class_weights(const float* cls, int64_t n_labels, int nc, int64_t* counts, double* weights, int32_t* status,
+                                   void* stream) {
+  NvtxRange nvtx_("myolo_class_weights");
+  MYOLO_REQUIRE((cls || n_labels == 0) && n_labels >= 0 && counts && weights && status, "class_weights: bad arguments");
+  MYOLO_REQUIRE(nc >= 1 && nc <= MYOLO_IW_NC_MAX, "class_weights: nc = %d, needs 1 <= nc <= %d", nc, MYOLO_IW_NC_MAX);
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_class_weights(cls, (long long)n_labels, nc, reinterpret_cast<unsigned long long*>(counts), weights, status,
+                              (cudaStream_t)stream);
+}
+
+extern "C" int myolo_image_weights(const float* cls, const int64_t* offsets, int64_t n, const double* cw, int nc, double* iw,
+                                   int32_t* status, void* stream) {
+  NvtxRange nvtx_("myolo_image_weights");
+  MYOLO_REQUIRE(cls && offsets && cw && iw && status && n >= 1, "image_weights: bad arguments");
+  MYOLO_REQUIRE(nc >= 1 && nc <= MYOLO_IW_NC_MAX, "image_weights: nc = %d, needs 1 <= nc <= %d", nc, MYOLO_IW_NC_MAX);
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_image_weights(cls, offsets, (long long)n, cw, nc, iw, status, (cudaStream_t)stream);
+}
+
+extern "C" int myolo_weighted_draw(const double* w, const double* u, int64_t n, double* cum, double* total, int32_t* idx, int32_t* status,
+                                   void* stream) {
+  NvtxRange nvtx_("myolo_weighted_draw");
+  MYOLO_REQUIRE(w && u && cum && total && idx && status, "weighted_draw: bad arguments");
+  MYOLO_REQUIRE(n >= 1 && n < (int64_t(1) << 31), "weighted_draw: n = %lld, needs 1 <= n < 2^31", (long long)n);
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_weighted_draw(w, u, (long long)n, cum, total, idx, status, (cudaStream_t)stream);
+}
+
 extern "C" int myolo_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay, void* stream) {
   NvtxRange nvtx_("myolo_ema_update");
   int rc = check_device(nullptr);

@@ -6,6 +6,8 @@
     DeviceImageCache(images, img_size, labels) / DetRectLoader(cache, hyp, batch_size)(positions) -> (imgs, targets), iterable
                                                                              :347-439 + :518-599 (augment=True, rect=True: --rect)
     collate_quad(imgs, targets) -> (imgs4, targets4)                               :602-625 collate_fn4 (--quad) over either batch
+    ImageWeights(DetAugmenter(...)).draw(class_weights, maps) -> indices, then (...)(positions) -> (imgs, targets)
+                                                                    train.py:305-316 --image-weights + :519 index = self.indices[index]
     DeviceImageCache(images, img_size, labels, augment=False) / DetValLoader(cache, batch_size) -> iterable of (imgs, targets, paths,
         shapes) for test(data, model=m, dataloader=DetValLoader(cache, 32))                          :347-452 + :518-599 (rect=True)
     DeviceSegCache(images, masks, mask_map) / SegAugmenter(cache, base_size, crop_size, preset)(indices) -> (segimgs, segtargets)
@@ -466,6 +468,21 @@ class DetValLoader:
             yield imgs, targets, batch.indices, batch.shapes
 
 
+def distributed_positions(n, epoch, rank, world_size, seed=0):
+    """rank's positions of one epoch over a dataset of n under DistributedSampler(dataset, shuffle=True, seed=seed) after
+    set_epoch(epoch): randperm from a generator seeded with seed + epoch, padded with its own head to a multiple of world_size, then every
+    world_size-th from rank"""
+    if not 0 <= rank < world_size:
+        raise ValueError(f"rank {rank} outside world size {world_size}")
+    g = torch.Generator()
+    g.manual_seed(seed + epoch)
+    idx = torch.randperm(n, generator=g).tolist()
+    total = math.ceil(n / world_size) * world_size
+    pad = total - len(idx)
+    idx += (idx * math.ceil(pad / len(idx)))[:pad] if pad else []
+    return idx[rank:total:world_size]
+
+
 # ------------------------------------------------------------------------------------------------
 # rect training batches (reference train.py:196-198 create_dataloader(..., augment=True, rect=opt.rect): LoadImagesAndLabels with
 # augment=True, rect=True (:347-439, __getitem__ :518-592 without mosaic) + collate_fn)
@@ -521,17 +538,8 @@ class DetRectLoader:
         return self.aug.launch([self.item(p) for p in positions], H, W, out_dtype)
 
     def epoch_positions(self, epoch, rank, world_size, seed=0):
-        """rank's positions of one epoch under DistributedSampler(dataset, shuffle=True, seed=seed) after set_epoch(epoch): randperm from
-        a generator seeded with seed + epoch, padded with its own head to a multiple of world_size, then every world_size-th from rank"""
-        if not 0 <= rank < world_size:
-            raise ValueError(f"DetRectLoader: rank {rank} outside world size {world_size}")
-        g = torch.Generator()
-        g.manual_seed(seed + epoch)
-        idx = torch.randperm(self.n, generator=g).tolist()
-        total = math.ceil(self.n / world_size) * world_size
-        pad = total - len(idx)
-        idx += (idx * math.ceil(pad / len(idx)))[:pad] if pad else []
-        return idx[rank:total:world_size]
+        """rank's positions of one epoch under DistributedSampler(dataset, shuffle=True, seed=seed) after set_epoch(epoch)"""
+        return distributed_positions(self.n, epoch, rank, world_size, seed)
 
     def batches(self, positions=None, out_dtype=torch.uint8):
         """the batches of runs of batch_size `positions` (default: every position in order), the last one partial"""
@@ -541,6 +549,87 @@ class DetRectLoader:
 
     def __iter__(self):
         return self.batches()
+
+
+# ------------------------------------------------------------------------------------------------
+# image-weighted training batches (reference train.py:255,305-316 --image-weights; utils/datasets.py:354,519,677)
+# ------------------------------------------------------------------------------------------------
+class ImageWeights:
+    """`--image-weights` over a DetAugmenter: once per epoch, `draw(model_class_weights, maps, rank, group)` is the reference's
+    train.py:305-316 block and sets the indices its dataset then reads.  Batches are `aug([iwts.indices[p] for p in positions])`, or
+    `iwts(positions)`, with `positions` from `epoch_positions`: sequential at rank -1 (a plain DataLoader), DistributedSampler(shuffle=True,
+    seed=0) after set_epoch(epoch) under DDP.  `collate_quad` and `train.MultiScale` apply to these batches unchanged.  The reference turns
+    `--rect` off under `--image-weights` (its dataset's rect = False), so the square DetAugmenter batches are the ones it trains on.
+
+    `model_class_weights` is train.py:255's `labels_to_class_weights(dataset.labels, nc).to(device) * nc` (utils.general), `maps` the
+    float64 per-class mAP of the last test() (np.zeros(nc) before the first).  On rank -1 / 0, `draw`:
+      - computes `cw = model_class_weights * (1 - maps) ** 2 / nc` with numpy on the host, as the reference does (nc values);
+      - computes labels_to_image_weights for it on the device (myolo_image_weights), over labels uploaded at the first draw;
+      - draws n `random.random()` values in the reference's order and runs random.choices(range(n), weights=iw, k=n) on the device
+        (myolo_weighted_draw), bit for bit; when the total weight is not positive and finite it raises random.choices' ValueError and
+        leaves `random` where it was, as random.choices does.
+    Under DDP (rank >= 0, `group` an initialised process group) rank 0 broadcasts the int32 indices and a status word (NCCL: from the
+    device), and the other ranks draw nothing and raise rank 0's ValueError if it had one.  Every rank then reads the indices back once
+    and sets `aug.indices` to them, so DetAugmenter's mosaic partners (`random.choices(self.indices, k=3)`) come from the drawn list, as
+    in the reference; mixup's `random.randint(0, n - 1)` does not.  The cache's labels are the dataset's: for `--single-cls` build it
+    from labels whose class column is zeroed, as LoadImagesAndLabels(single_cls=True) does, with nc = 1."""
+
+    def __init__(self, aug):
+        self.aug, self.n = aug, aug.n
+        self.indices = list(range(self.n))
+        self._labels = None
+
+    def _draw(self, cw):
+        """the device work of rank -1 / 0: (int32 (n + 1) device tensor of the indices and the status word, `random`'s state before
+        the draws)"""
+        from .general import device_image_weights, label_classes
+        if self._labels is None:
+            self._labels = label_classes(self.aug.cache.labels)
+        cls, offsets = self._labels
+        n, dev = self.n, cls.device
+        buf = torch.zeros(n + 1, dtype=torch.int32, device=dev)
+        status = buf[n:]
+        iw = device_image_weights(cls, offsets, cw, status)
+        state = random.getstate()
+        u = torch.tensor([random.random() for _ in range(n)], dtype=torch.float64).to(dev)
+        cum = torch.empty(n, dtype=torch.float64, device=dev)
+        total = torch.empty(1, dtype=torch.float64, device=dev)
+        _lib.check(_lib.lib().myolo_weighted_draw(_lib.ptr(iw), _lib.ptr(u), n, _lib.ptr(cum), _lib.ptr(total), _lib.ptr(buf),
+                                                  _lib.ptr(status), _lib.stream_ptr()))
+        return buf, state
+
+    def draw(self, class_weights, maps, rank=-1, group=None):
+        """one epoch's drawn indices (a list of n ints), also set as `self.indices` and `aug.indices`"""
+        state = None
+        if rank in (-1, 0):
+            cwm = class_weights.detach().cpu().numpy() if isinstance(class_weights, torch.Tensor) else np.asarray(class_weights)
+            nc = len(cwm)
+            cw = cwm * (1 - maps) ** 2 / nc
+            buf, state = self._draw(cw)
+        if rank != -1:
+            import torch.distributed as dist
+            nccl = dist.get_backend(group) == "nccl"
+            dev = torch.device("cuda", torch.cuda.current_device()) if nccl else torch.device("cpu")
+            buf = buf.to(dev) if rank == 0 else torch.zeros(self.n + 1, dtype=torch.int32, device=dev)
+            dist.broadcast(buf, 0, group=group)
+        host = buf.cpu().numpy()
+        status = int(host[self.n])
+        if status:
+            from .general import iw_status_error
+            if state is not None:
+                random.setstate(state)
+            raise iw_status_error(status)
+        self.indices = host[:self.n].tolist()
+        self.aug.indices = self.indices
+        return self.indices
+
+    def epoch_positions(self, epoch=0, rank=-1, world_size=1, seed=0):
+        """rank's dataset positions of one epoch: 0 .. n-1 at rank -1, else DistributedSampler's (distributed_positions)"""
+        return list(range(self.n)) if rank == -1 else distributed_positions(self.n, epoch, rank, world_size, seed)
+
+    def __call__(self, positions, out_dtype=torch.uint8):
+        """the batch of dataset `positions`: aug([indices[p] for p in positions])"""
+        return self.aug([self.indices[int(p)] for p in positions], out_dtype)
 
 
 # ------------------------------------------------------------------------------------------------

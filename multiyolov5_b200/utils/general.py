@@ -1,6 +1,7 @@
 """Post-process of the hot path behind the reference's names (reference utils/general.py, detect.py:191-193)."""
 import ctypes as C
 
+import numpy as np
 import torch
 
 from .. import _lib
@@ -56,6 +57,77 @@ def box_iou(box1, box2):
     area2 = (box2[:, 2] - box2[:, 0]) * (box2[:, 3] - box2[:, 1])
     inter = (torch.min(box1[:, None, 2:], box2[:, 2:]) - torch.max(box1[:, None, :2], box2[:, :2])).clamp(0).prod(2)
     return inter / (area1[:, None] + area2 - inter)
+
+
+# ---- --image-weights (reference utils/general.py:216-240, train.py:255,305-316; csrc/image_weights.cu) ----
+_IW_ERRORS = ((_lib.IW_BAD_CLASS, "labels_to_image_weights: a label's class is outside [0, nc)"),
+              (_lib.IW_TOTAL_NONPOS, "Total of weights must be greater than zero"),      # random.choices' own messages
+              (_lib.IW_TOTAL_NONFINITE, "Total of weights must be finite"))
+
+
+def iw_status_error(status):
+    """the ValueError for a nonzero image-weights status word (a bad class first, as bincount raises before random.choices)"""
+    return next(ValueError(msg) for bit, msg in _IW_ERRORS if status & bit)
+
+
+def label_classes(labels, device=None):
+    """the float32 class column of every image's (k, 5) labels, concatenated, and each image's [start, end) in it ((n + 1) int64), both
+    uploaded to the device once"""
+    cols = [np.asarray(x, np.float32).reshape(-1, 5)[:, 0] for x in labels]
+    offsets = np.zeros(len(cols) + 1, np.int64)
+    np.cumsum([len(c) for c in cols], out=offsets[1:])
+    dev = device or torch.device("cuda", torch.cuda.current_device())
+    cls = torch.from_numpy(np.concatenate(cols) if cols else np.zeros(0, np.float32)).to(dev)
+    return cls, torch.from_numpy(offsets).to(dev)
+
+
+def _nc(nc):
+    if not 1 <= int(nc) <= _lib.IW_NC_MAX:
+        raise ValueError(f"nc = {nc}: image weights are built for 1 <= nc <= {_lib.IW_NC_MAX}")
+    return int(nc)
+
+
+def labels_to_class_weights(labels, nc=80):
+    """the reference's labels_to_class_weights on the device, bit for bit: inverse class frequencies (empty classes count 1), normalised
+    by numpy's sum over nc.  Returns a float64 CUDA tensor of nc (the reference returns a CPU one; train.py moves it with `.to(device)`
+    and multiplies it by nc).  A class outside [0, nc) raises ValueError.  Reads one status word back."""
+    if labels[0] is None:
+        return torch.Tensor()
+    nc = _nc(nc)
+    cls, _ = label_classes(labels)
+    counts = torch.empty(nc, dtype=torch.int64, device=cls.device)
+    w = torch.empty(nc, dtype=torch.float64, device=cls.device)
+    status = torch.zeros(1, dtype=torch.int32, device=cls.device)
+    _lib.check(_lib.lib().myolo_class_weights(_lib.ptr(cls), cls.numel(), nc, _lib.ptr(counts), _lib.ptr(w), _lib.ptr(status),
+                                              _lib.stream_ptr()))
+    if int(status.item()):
+        raise iw_status_error(int(status.item()))
+    return w
+
+
+def device_image_weights(cls, offsets, cw, status):
+    """myolo_image_weights over uploaded labels (label_classes) for the nc class weights `cw` (float64 numpy): a float64 CUDA tensor of
+    the n image weights; a bad class ORs the status word"""
+    cw = np.ascontiguousarray(cw, np.float64)
+    nc = _nc(cw.size)
+    n = offsets.numel() - 1
+    cw_d = torch.from_numpy(cw).to(cls.device)
+    iw = torch.empty(n, dtype=torch.float64, device=cls.device)
+    _lib.check(_lib.lib().myolo_image_weights(_lib.ptr(cls), _lib.ptr(offsets), n, _lib.ptr(cw_d), nc, _lib.ptr(iw), _lib.ptr(status),
+                                              _lib.stream_ptr()))
+    return iw
+
+
+def labels_to_image_weights(labels, nc=80, class_weights=np.ones(80)):
+    """the reference's labels_to_image_weights on the device, bit for bit: per image, the sum over nc of class_weights * its label count
+    per class, in numpy's order.  Returns a float64 numpy array of len(labels).  A class outside [0, nc) raises ValueError."""
+    cw = np.asarray(class_weights, np.float64).reshape(nc)
+    cls, offsets = label_classes(labels)
+    status = torch.zeros(1, dtype=torch.int32, device=cls.device)
+    iw = device_image_weights(cls, offsets, cw, status)
+    if int(status.item()):
+        raise iw_status_error(int(status.item()))
+    return iw.cpu().numpy()
 
 
 def strip_optimizer(f="best.pt", s=""):
