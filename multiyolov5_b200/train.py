@@ -30,19 +30,25 @@ A model converted with torch.nn.SyncBatchNorm.convert_sync_batchnorm (the refere
 BatchNorm statistics exchanged across the ranks of its NCCL process group inside the train plans (Engine.set_bn_sync); the two passes of a
 step then run one after the other.  At world size 1, or without torch.distributed, it trains exactly like the plain model, as torch does.
 
-Out of scope (the reference's outer loop, not the hot path): data loading, LR schedule / warm-up (call `set_lr` / `set_momentum`),
-writing checkpoint files, plotting, DDP buffer broadcast.
+`fit(model, hyp, opt, det_batches, seg_batches, ...)` is the reference's epoch loop (train.py:44-543) around the step: `LRSchedule` (warm-up,
+LambdaLR, momentum, accumulation), the validation cadence, fitness2 and best.pt, results.txt, last.pt / best.pt and resume.
+`DetEpochBatches` / `SegEpochBatches` give each epoch's batches from the device loaders in the reference's order.
+
+Out of scope: loading and decoding data files, plotting, W&B / TensorBoard, --evolve's generations, --bucket, DDP buffer broadcast.
 """
+import collections
 import math
 import random
 import ctypes as C
 
+import numpy as np
 import torch
 import torch.nn as nn
 
 from . import _lib
 from .engine import flat_offsets
 from .parallel import allreduce_flat_grads, bn_sync_group
+from .utils.general import init_seeds, one_cycle
 from .utils.loss import FusedComputeLoss, OhemCELoss, SegFocalLoss, SegmentationLosses, seg_focal_loss
 
 
@@ -636,14 +642,354 @@ class Trainer:
         segimgs.record_stream(self._s_seg); segtargets.record_stream(self._s_seg)
         return items, segloss
 
-    def step(self, imgs, targets, segimgs, segtargets):
-        """one iteration (train.py:363-401).  Returns (det loss items [lbox,lobj,lcls,loss], seg loss) as device tensors."""
+    def step(self, imgs, targets, segimgs, segtargets, ni=None):
+        """one iteration (train.py:363-401).  Returns (det loss items [lbox,lobj,lcls,loss], seg loss) as device tensors.
+        ni: the reference's iteration number (train.py:341, which also counts skipped batches); when given, the optimizer steps when
+        ni % self.accumulate == 0 (train.py:396), else every `accumulate` calls of this method."""
         if self._ms_batches and imgs.shape[0] not in self._ms_batches:
             self._reserve_det(int(imgs.shape[0]))               # host plans only: the shared workspace is already there
         # autograd's seg pass runs Model.forward: lane 0.  Synchronised BatchNorm: one stream of collectives, det pass then seg pass
         passes = self._passes_concurrent if self.fused_seg and not self.sync_bn else self._passes_sequential
         items, segloss = passes(imgs, targets, segimgs, segtargets)
         self.ni += 1
-        if self.ni % self.accumulate == 0:
+        if (self.ni if ni is None else ni) % self.accumulate == 0:
             self.optimizer_step()
         return items, segloss
+
+
+# ---- the epoch loop (reference train.py:44-543) ---------------------------------------------------------------------------------------
+NBS = 64                # nominal batch size (train.py:115)
+WARMUP_MIN = 800        # least number of warm-up iterations (train.py:260: this fork's 800; upstream YOLOv5 uses 1000)
+EMA_ATTRS = ("yaml", "nc", "hyp", "gr", "names", "stride", "class_weights")         # ema.update_attr's include list (train.py:433)
+
+Iteration = collections.namedtuple("Iteration", "ni lr momentum accumulate step")
+
+
+class LRSchedule:
+    """The learning rates, momentum and gradient accumulation of reference train.py, per iteration and per epoch:
+
+        nw = max(round(hyp['warmup_epochs'] * nb), 800)                                  (train.py:260; nb counts det batches)
+        while ni <= nw (ni = i + nb * epoch):                                            (train.py:344-352)
+            accumulate = max(1, interp(ni, [0, nw], [1, floor(64 / total_batch_size)]).round())
+            lr[j]      = interp(ni, [0, nw], [hyp['warmup_bias_lr'] if j == 2 else 0.0, initial_lr[j] * lf(epoch)])
+            momentum   = interp(ni, [0, nw], [hyp['warmup_momentum'], hyp['momentum']])  (SGD only: Adam's groups have no 'momentum')
+        after each epoch: lr[j] = lr0 * lf(epoch + 1)                                    (LambdaLR.step, train.py:428)
+
+    with lf = one_cycle(1, lrf, epochs), or the linear ramp of --linear-lr (train.py:143-147).  Outside the warm-up every value stays where
+    the last warm-up iteration (or the last epoch end) left it; `accumulate` starts at max(round(64 / total_batch_size), 1) (train.py:116),
+    which is also what weight decay is scaled for, and the warm-up ends it at floor(64 / total_batch_size).  The floats are numpy's
+    float64 interp and torch LambdaLR's `base_lr * lf(epoch)`, computed by the same operations in the same order.
+
+    Resume (start_epoch > 0): pass the checkpoint optimizer's `param_groups`; lr, momentum and initial_lr come from them, as
+    optimizer.load_state_dict sets them (train.py:157-158), and the epoch count is extended when fine-tuning past the end (train.py:174-177).
+    The cosine lf keeps the epoch count it was built with, the linear one reads the extended count when called, as the reference's
+    closure over `epochs` does.
+
+    `iteration(epoch, i)` is called for each batch that trains (not for the batches of one image the loop skips) and returns
+    Iteration(ni, (lr_bn, lr_weight, lr_bias), momentum (None for Adam), accumulate, step: whether the optimizer steps).  `step()` is the
+    epoch end.  `state_dict()` is the schedule's state: the epoch count, last_epoch, lr, momentum, initial_lr, accumulate."""
+
+    def __init__(self, hyp, epochs, nb, total_batch_size, linear_lr=False, optimizer="sgd", start_epoch=0, param_groups=None, nbs=NBS):
+        if optimizer not in OPTIMIZER_STATE:
+            raise ValueError(f"optimizer must be 'sgd' or 'adam', got {optimizer!r}")
+        if nb < 1:
+            raise ValueError(f"an epoch of {nb} det batches has no iteration")
+        h = self.hyp = dict(hyp)
+        self.nb, self.nbs, self.total_batch_size, self.sgd = int(nb), nbs, total_batch_size, optimizer == "sgd"
+        self.epochs = epochs + start_epoch - 1 if start_epoch > 0 and epochs < start_epoch else epochs
+        if linear_lr:
+            n = self.epochs
+            self.lf = lambda x: (1 - x / (n - 1)) * (1.0 - h["lrf"]) + h["lrf"]
+        else:
+            self.lf = one_cycle(1, h["lrf"], epochs)
+        self.nw = max(round(h["warmup_epochs"] * self.nb), WARMUP_MIN)
+        self.base_lrs = [h["lr0"]] * 3                       # LambdaLR's, from the groups' lr when it was built: this run's lr0
+        self.last_epoch = start_epoch - 1
+        self.accumulate = max(round(nbs / total_batch_size), 1)
+        if param_groups is None:
+            self.initial_lr = list(self.base_lrs)
+            self.lr = [b * self.lf(0) for b in self.base_lrs]           # LambdaLR's first step, in its constructor
+            self.momentum = h["momentum"] if self.sgd else None
+        else:
+            if len(param_groups) != 3:
+                raise ValueError(f"expected the reference's three parameter groups, got {len(param_groups)}")
+            self.initial_lr = [g.get("initial_lr", h["lr0"]) for g in param_groups]
+            self.lr = [g["lr"] for g in param_groups]
+            self.momentum = param_groups[0]["momentum"] if self.sgd else None
+
+    def iteration(self, epoch, i):
+        ni = i + self.nb * epoch
+        if ni <= self.nw:
+            xi = [0, self.nw]
+            self.accumulate = int(max(1, np.interp(ni, xi, [1, math.floor(self.nbs / self.total_batch_size)]).round()))
+            self.lr = [float(np.interp(ni, xi, [self.hyp["warmup_bias_lr"] if j == 2 else 0.0, self.initial_lr[j] * self.lf(epoch)]))
+                       for j in range(3)]
+            if self.sgd:
+                self.momentum = float(np.interp(ni, xi, [self.hyp["warmup_momentum"], self.hyp["momentum"]]))
+        return Iteration(ni, tuple(self.lr), self.momentum, self.accumulate, ni % self.accumulate == 0)
+
+    def step(self):
+        self.last_epoch += 1
+        self.lr = [b * self.lf(self.last_epoch) for b in self.base_lrs]
+
+    def state_dict(self):
+        return {"epochs": self.epochs, "last_epoch": self.last_epoch, "lr": list(self.lr), "momentum": self.momentum,
+                "initial_lr": list(self.initial_lr), "accumulate": self.accumulate}
+
+
+class DetEpochBatches:
+    """`det_batches` for fit: `batches(epoch)` iterates one epoch's det batches as the reference's train loader yields them.
+
+    source: a utils.datasets.DetAugmenter (the square mosaic loader), DetRectLoader (--rect) or ImageWeights (--image-weights); each
+    builds the batch of a list of dataset positions.  Positions run 0 .. n-1 in order at rank -1 (the loader has no sampler), and are
+    DistributedSampler's (utils.datasets.distributed_positions, seed 0, set_epoch(epoch)) under DDP; a batch is a run of `batch_size`
+    of them, the last one partial.  With ImageWeights, `ImageWeights.draw(class_weights, maps, rank, group)` runs when the epoch's
+    iterable is made (train.py:305-316), with `maps` the per-class mAP fit stores in `self.maps` after each test() (zeros before).
+    quad: each uint8 batch goes through utils.datasets.collate_quad (collate_fn4).  Batches are built when they are asked for, so the
+    random draws come in the reference's order when fit zips them with the seg batches."""
+
+    def __init__(self, source, batch_size, rank=-1, world_size=1, quad=False, class_weights=None, group=None, out_dtype=torch.float32):
+        from .utils.datasets import ImageWeights
+        self.image_weights = isinstance(source, ImageWeights)
+        if self.image_weights and class_weights is None:
+            raise ValueError("DetEpochBatches: ImageWeights needs the model's class weights (labels_to_class_weights(labels, nc) * nc)")
+        self.source, self.batch_size, self.rank, self.world_size = source, int(batch_size), rank, world_size
+        self.quad, self.class_weights, self.group, self.out_dtype = bool(quad), class_weights, group, out_dtype
+        self.n = source.n
+        self.maps = None
+
+    def positions(self, epoch):
+        from .utils.datasets import distributed_positions
+        return list(range(self.n)) if self.rank == -1 else distributed_positions(self.n, epoch, self.rank, self.world_size)
+
+    def __len__(self):
+        n = self.n if self.rank == -1 else math.ceil(self.n / self.world_size)
+        return math.ceil(n / self.batch_size)
+
+    def __call__(self, epoch):
+        if self.image_weights:
+            cw = self.class_weights
+            self.source.draw(cw, np.zeros(len(cw)) if self.maps is None else self.maps, self.rank, self.group)
+        return self._batches(self.positions(epoch))
+
+    def _batches(self, positions):
+        from .utils.datasets import collate_quad
+        for k in range(0, len(positions), self.batch_size):
+            chunk = positions[k:k + self.batch_size]
+            if self.quad:
+                yield collate_quad(*self.source(chunk, torch.uint8), out_dtype=self.out_dtype)
+            else:
+                yield self.source(chunk, self.out_dtype)
+
+
+class SegEpochBatches:
+    """`seg_batches` for fit: one epoch's seg batches from a utils.datasets.SegAugmenter in the order of the reference's
+    DataLoader(shuffle=True, drop_last=...) (SegmentationDataset.get_*_loader: drop_last=False for get_citys_loader, True for the
+    citysbdd and custom loaders).  The order is torch's own: a DataLoader over range(n) with those settings, iterated by index batches,
+    so its RandomSampler draws from torch's default generator exactly when the reference's does (the loader's base seed when the epoch's
+    iterator is made, the permutation's seed at its first batch), before the items' ColorJitter draws."""
+
+    def __init__(self, aug, batch_size, drop_last=False, out_dtype=torch.float32):
+        self.aug, self.batch_size, self.drop_last, self.out_dtype = aug, int(batch_size), bool(drop_last), out_dtype
+        self.n = aug.cache.n
+
+    def __len__(self):
+        return self.n // self.batch_size if self.drop_last else math.ceil(self.n / self.batch_size)
+
+    def order(self):
+        """the epoch's index batches (an iterator of int64 tensors), made now"""
+        return iter(torch.utils.data.DataLoader(range(self.n), batch_size=self.batch_size, shuffle=True, drop_last=self.drop_last))
+
+    def __call__(self, epoch):
+        return (self.aug(idx.tolist(), self.out_dtype) for idx in self.order())
+
+
+def _unsupported_flags(opt):
+    """NotImplementedError naming the first flag of `opt` the loop cannot honour"""
+    for name, on in (("bucket", getattr(opt, "bucket", "")), ("entity", getattr(opt, "entity", None)),
+                     ("upload_dataset", getattr(opt, "upload_dataset", False)), ("data", isinstance(getattr(opt, "data", None), str))):
+        if on:
+            raise NotImplementedError(f"fit: --{name} is not built (W&B, gsutil uploads and loading a data yaml are not part of the loop)")
+
+
+def _load_start(path, model, hyp, opt, device):
+    """the checkpoint of train.py:86-95 and :152-177 (this loop's or the reference's): loads its model weights into `model` and returns it"""
+    from .models.experimental import load_checkpoint
+    ckpt = load_checkpoint(path, map_location=device)
+    exclude = ["anchor"] if (getattr(opt, "cfg", "") or hyp.get("anchors")) and not opt.resume else []
+    msd = model.state_dict()
+    sd = {k: v for k, v in ckpt["model"].float().state_dict().items()
+          if k in msd and not any(x in k for x in exclude) and v.shape == msd[k].shape}          # intersect_dicts
+    model.load_state_dict(sd, strict=False)
+    return ckpt
+
+
+def fit(model, hyp, opt, det_batches, seg_batches, *, test_loader=None, segval_loader=None, save_dir, ema=None, log_interval=50,
+        **trainer_kwargs):
+    """The training run of reference train.py:train() (train.py:44-543) over device batches; returns `results` as it does:
+    (P, R, mAP@.5, mAP@.5:.95, val box, obj, cls loss) of the last test().
+
+    model: a CUDA models.yolo.Model (fp32) with `names` set, built as train.py:86-98 builds it; hyp: the unscaled hyper-parameters (this
+    scales weight decay and the loss gains as train.py:116-117 and :248-251 do).  opt: an argparse.Namespace with the reference's flag
+    names: epochs, batch_size (total), img_size ([train, test]), linear_lr, adam, notest, nosave, evolve, multi_scale, quad, single_cls,
+    resume, global_rank, world_size, label_smoothing, and `weights` (a .pt to start from, or '') and `cfg` as train.py reads them.
+    det_batches(epoch) / seg_batches(epoch): that epoch's iterables of (imgs, targets, ...) and (segimgs, segtargets) device batches,
+    with len(det_batches) = nb; DetEpochBatches / SegEpochBatches build them from the device loaders in the reference's order.  Det images
+    are float (B, 3, H, W) = uint8 / 255, or uint8 under multi_scale.  test_loader: DetValLoader batches for test.test (None: no test,
+    results stay zeros); segval_loader: mode='testval' seg batches for test.seg_validation (None: mIoU 0).  save_dir: results.txt and
+    weights/last.pt, best.pt go there.  ema: a ModelEMA of `model` (built here on rank -1 / 0 when None).  trainer_kwargs go to Trainer
+    (seg_loss, process_group, det_shapes, ...).
+
+    Per run: init_seeds(2 + rank); the EMA; the start checkpoint (opt.weights ending in .pt): model weights, optimizer state and
+    best_fitness, EMA and its update count, results.txt, start_epoch, and the fine-tune extension of the epoch count; then, when not
+    resuming, model.half().float() (train.py:225); the Trainer and the LRSchedule.  Per iteration (train.py:335-410): batches of one
+    image are skipped but still counted in `i`; the schedule goes to Trainer.set_lr / set_momentum / accumulate; MultiScale rescales the
+    det batch under multi_scale; Trainer.step(..., ni=ni).  The running mean losses stay on the device and are read and printed every
+    `log_interval` iterations and at the epoch end only, where the reference formats them every iteration (a host synchronisation per
+    step).  Per epoch (train.py:426-500): the schedule's step, ema.update_attr, seg_validation on ema.ema when epoch % 10 == 0 or
+    epochs - epoch < 40 (mIoU 0 otherwise), test.test(model=ema.ema) unless notest and always on the final epoch, fitness2 and
+    best_fitness, the results.txt line in the reference's format, and last.pt / best.pt with the reference's keys unless nosave (the
+    final epoch saves unless evolve).
+
+    Deviations: test() runs with plots=False on the final epoch too (plots are not built); autoanchor (train.py:223-224) is the caller's,
+    before fit; no W&B, TensorBoard or --bucket (NotImplementedError), no data yaml (opt.data must not be a path), no strip_optimizer or
+    COCO re-test after the last epoch.  Reproducibility: a seeded run's batches equal the reference's only under --workers 0, since
+    DataLoader worker processes draw from `random` / `numpy.random` streams of their own; and torch's default generator, which the seg
+    order and ColorJitter draw from, has also served the reference's model initialisation before its first epoch."""
+    from copy import deepcopy
+    from pathlib import Path
+    from . import test as _test
+    from .utils.metrics import fitness2
+    from .utils.torch_utils import ModelEMA
+
+    _unsupported_flags(opt)
+    save_dir = Path(save_dir)
+    wdir = save_dir / "weights"
+    wdir.mkdir(parents=True, exist_ok=True)
+    last, best, results_file = wdir / "last.pt", wdir / "best.pt", save_dir / "results.txt"
+    rank, world_size = getattr(opt, "global_rank", -1), getattr(opt, "world_size", 1)
+    total_batch_size = opt.batch_size
+    batch_size = total_batch_size // world_size if rank != -1 else total_batch_size
+    epochs = opt.epochs
+    device = next(model.parameters()).device
+    init_seeds(2 + rank)
+
+    det = model.model[-1]
+    nc = 1 if opt.single_cls else int(det.nc)
+    nl = det.nl
+    gs = max(int(model.stride.max()), 32)
+    imgsz, imgsz_test = (list(opt.img_size) * 2)[:2]
+    if imgsz % gs or imgsz_test % gs:
+        raise ValueError(f"image sizes {imgsz}, {imgsz_test} must be multiples of the grid size {gs}")
+
+    weights = getattr(opt, "weights", "") or ""
+    if isinstance(opt.resume, str):
+        weights = opt.resume
+    ckpt = _load_start(weights, model, hyp, opt, device) if weights.endswith(".pt") else None
+    if ema is None and rank in (-1, 0):
+        ema = ModelEMA(model)                                                      # train.py:151
+    start_epoch, best_fitness = 0, 0.0
+    if ckpt is not None:
+        if ckpt.get("optimizer") is not None:
+            best_fitness = ckpt["best_fitness"]
+        if ema is not None and ckpt.get("ema") is not None:
+            ema.ema.load_state_dict(ckpt["ema"].float().state_dict())
+            ema.updates = ckpt["updates"]
+        if ckpt.get("training_results") is not None:
+            results_file.write_text(ckpt["training_results"])
+        start_epoch = ckpt["epoch"] + 1
+        if opt.resume and start_epoch <= 0:
+            raise ValueError(f"{weights} training to {epochs} epochs is finished, nothing to resume")
+    if rank in (-1, 0) and not opt.resume:
+        model.half().float()                                                       # train.py:225: pre-reduce anchor precision
+
+    h = scale_hyp(hyp, nl=nl, nc=nc, imgsz=imgsz, total_batch_size=total_batch_size, nbs=NBS, label_smoothing=opt.label_smoothing)
+    nb = len(det_batches)
+    optimizer = "adam" if opt.adam else "sgd"
+    groups = ckpt["optimizer"]["param_groups"] if ckpt is not None and ckpt.get("optimizer") is not None else None
+    sched = LRSchedule(hyp, epochs, nb, total_batch_size, linear_lr=opt.linear_lr, optimizer=optimizer, start_epoch=start_epoch,
+                       param_groups=groups)
+    epochs = sched.epochs
+    multi_scale = MultiScale(imgsz, gs) if opt.multi_scale else None
+    tr = Trainer(model, h, batch_size, world_size=world_size, rank=rank, accumulate=sched.accumulate, optimizer=optimizer, ema=ema,
+                 quad=opt.quad, multi_scale=multi_scale, **trainer_kwargs)
+    if groups is not None:
+        tr.load_state_dict(ckpt["optimizer"])
+    del ckpt
+    model.nc = nc
+    cl = tr.compute_loss
+
+    results = (0, 0, 0, 0, 0, 0, 0)
+    maps = np.zeros(nc)
+    for epoch in range(start_epoch, epochs):
+        mIoU = 0
+        model.train()
+        mloss = torch.zeros(4, device=device)
+        msegloss = torch.zeros(1, device=device)
+        s = None
+        for (i, det_batch), (_, seg_batch) in zip(enumerate(det_batches(epoch)), enumerate(seg_batches(epoch))):
+            imgs, targets = det_batch[0], det_batch[1]
+            segimgs, segtargets = seg_batch[0], seg_batch[1]
+            if len(imgs) == 1 or len(segimgs) == 1:                               # train.py:338-339
+                continue
+            it = sched.iteration(epoch, i)
+            tr.set_lr(*it.lr)
+            if it.momentum is not None:
+                tr.set_momentum(it.momentum)
+            tr.accumulate = it.accumulate
+            if multi_scale is not None:
+                imgs = multi_scale(imgs)
+            elif not imgs.is_floating_point():
+                raise ValueError("fit: det images must be float (uint8 / 255) unless multi_scale converts them")
+            loss_items, segloss = tr.step(imgs, targets, segimgs, segtargets, ni=it.ni)
+            if rank in (-1, 0):
+                mloss = (mloss * i + loss_items) / (i + 1)
+                msegloss = (msegloss * i + segloss.detach() / total_batch_size) / (i + 1)
+                s = (epoch, targets.shape[0], imgs.shape[-1])
+                if (i + 1) % log_interval == 0:
+                    print(_progress(epoch, epochs, mloss, msegloss, *s[1:]), flush=True)
+        sched.step()                                                               # train.py:428
+        tr.set_lr(*sched.lr)
+
+        if rank in (-1, 0):
+            if s is None:
+                raise ValueError(f"epoch {epoch} trained no batch")
+            line = _progress(epoch, epochs, mloss, msegloss, *s[1:])
+            print(line, flush=True)
+            ema.update_attr(model, include=EMA_ATTRS)
+            if epoch % 10 == 0 or (epochs - epoch) < 40:
+                if segval_loader is not None:
+                    mIoU = _test.seg_validation(model=ema.ema, valloader=segval_loader, device=device, n_segcls=model.model[-2].c_out,
+                                                half_precision=True)
+            final_epoch = epoch + 1 == epochs
+            if (not opt.notest or final_epoch) and test_loader is not None:
+                results, maps, _ = _test.test({"nc": nc}, batch_size=batch_size * 2, imgsz=imgsz_test, model=ema.ema,
+                                              single_cls=opt.single_cls, dataloader=test_loader, save_dir=save_dir,
+                                              verbose=nc < 50 and final_epoch, plots=False, compute_loss=cl)
+                if hasattr(det_batches, "maps"):
+                    det_batches.maps = maps
+            with open(results_file, "a") as f:
+                f.write(line + "%10.4g" * 7 % results + "\n")                     # train.py:456-457
+            fi = fitness2(np.array(results).reshape(1, -1), mIoU)
+            if fi > best_fitness:
+                best_fitness = fi
+            if (not opt.nosave) or (final_epoch and not opt.evolve):
+                ckpt = {"epoch": epoch,
+                        "best_fitness": best_fitness,
+                        "training_results": results_file.read_text(),
+                        "model": deepcopy(model).half(),
+                        "ema": deepcopy(ema.ema).half(),
+                        "updates": ema.updates,
+                        "optimizer": tr.state_dict(),
+                        "wandb_id": None}
+                torch.save(ckpt, last)
+                if best_fitness == fi:
+                    torch.save(ckpt, best)
+                del ckpt
+    return results
+
+
+def _progress(epoch, epochs, mloss, msegloss, n_targets, imgshape):
+    """the progress line of train.py:407-409 (reads the device means: a host synchronisation)"""
+    mem = "%.3gG" % (torch.cuda.memory_reserved() / 1E9 if torch.cuda.is_available() else 0)
+    return ("%10s" * 2 + "%10.4g" * 7) % ("%g/%g" % (epoch, epochs - 1), mem, *mloss.tolist(), *msegloss.tolist(), n_targets, imgshape)

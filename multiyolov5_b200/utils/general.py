@@ -1,5 +1,6 @@
 """Post-process of the hot path behind the reference's names (reference utils/general.py, detect.py:191-193)."""
 import ctypes as C
+import math
 
 import numpy as np
 import torch
@@ -146,6 +147,24 @@ def strip_optimizer(f="best.pt", s=""):
     torch.save(x, s or f)
     mb = os.path.getsize(s or f) / 1e6
     print(f"Optimizer stripped from {f},{(' saved as %s,' % s) if s else ''} {mb:.1f}MB")
+
+
+def init_seeds(seed=0):
+    """reference utils/general.py:39-43 with torch_utils.init_torch_seeds: seeds `random`, `numpy.random` and torch's default generator;
+    seed 0 asks cuDNN for determinism, any other seed for its benchmark mode"""
+    import random
+    random.seed(seed)
+    np.random.seed(seed)
+    torch.manual_seed(seed)
+    torch.backends.cudnn.benchmark, torch.backends.cudnn.deterministic = (False, True) if seed == 0 else (True, False)
+
+
+def one_cycle(y1=0.0, y2=1.0, steps=100):
+    """the cosine ramp from y1 at x = 0 to y2 at x = steps of reference utils/general.py:186-188, its operations in its order so that
+    every float is the reference's"""
+    def f(x):
+        return ((1 - math.cos(x * math.pi / steps)) / 2) * (y2 - y1) + y1
+    return f
 
 
 def non_max_suppression(prediction, conf_thres=0.25, iou_thres=0.45, classes=None, agnostic=False, multi_label=False, labels=(),
