@@ -522,6 +522,11 @@ int myolo_conv_bn_silu_slice(const void* x_nhwc_f16, int B, int H, int W, int ci
                              int dil, const float* gamma, const float* beta, const float* mean, const float* var, float eps,
                              const float* bias, int act, const void* residual_nhwc_f16, void* y_nhwc_f16, int y_ctot, int path,
                              void* stream);
+/* the same, and reports the launch's routing in info[0..11] (the slots of myolo_plan_conv_info) */
+int myolo_conv_bn_silu_info(const void* x_nhwc_f16, int B, int H, int W, int ci, const float* w, int co, int k, int stride,
+                            int dil, const float* gamma, const float* beta, const float* mean, const float* var, float eps,
+                            const float* bias, int act, const void* residual_nhwc_f16, void* y_nhwc_f16, int y_ctot, int path,
+                            int32_t* info, void* stream);
 
 #ifdef __cplusplus
 }

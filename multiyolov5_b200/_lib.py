@@ -33,7 +33,7 @@ EXPORTS = [
     "myolo_abi_version", "myolo_last_error", "myolo_device_info", "myolo_plan_create", "myolo_plan_destroy",
     "myolo_plan_set_conv_weights", "myolo_plan_repack_weights", "myolo_plan_forward", "myolo_plan_read_view", "myolo_plan_last_launch_count",
     "myolo_plan_profile", "myolo_nms_workspace_bytes", "myolo_nms", "myolo_seg_upsample_argmax", "myolo_bilinear_nchw",
-    "myolo_conv_bn_silu", "myolo_conv_bn_silu_slice", "myolo_plan_set_bn", "myolo_plan_set_conv_grad", "myolo_plan_train_forward", "myolo_plan_backward",
+    "myolo_conv_bn_silu", "myolo_conv_bn_silu_slice", "myolo_conv_bn_silu_info", "myolo_plan_set_bn", "myolo_plan_set_conv_grad", "myolo_plan_train_forward", "myolo_plan_backward",
     "myolo_grads_check_finite", "myolo_sgd_step", "myolo_conv_wgrad", "myolo_letterbox", "myolo_seg_lut_blend", "myolo_seg_metrics", "myolo_plan_backward_seg_ce", "myolo_plan_read_grad_view", "myolo_plan_set_seed", "myolo_plan_train_forward_multi", "myolo_plan_backward_multi", "myolo_plan_conv_info", "myolo_allreduce_grads", "myolo_det_loss", "myolo_det_loss_workspace_bytes", "myolo_plan_set_defer_running", "myolo_plan_apply_running",
     "myolo_resize_u8", "myolo_augment_det", "myolo_augment_seg", "myolo_det_match", "myolo_det_ap", "myolo_det_ap_workspace_bytes",
     "myolo_resize_area_u8", "myolo_resize_bilinear", "myolo_plan_create_shared", "myolo_augment_det_hw", "myolo_adam_step",
@@ -192,6 +192,8 @@ def lib():
     L.myolo_conv_bn_silu.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, vp]
     L.myolo_conv_bn_silu_slice.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, i32,
                                            vp]
+    L.myolo_conv_bn_silu_info.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, i32,
+                                          C.POINTER(C.c_int32), vp]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError here == header / library mismatch
     if L.myolo_abi_version() != 1:

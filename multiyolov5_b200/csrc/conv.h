@@ -36,6 +36,7 @@ struct ConvTcParams {
   int a_stage_bytes, b_stage_bytes;
   int resident;          // 1: the CTA's whole weight slice stays in shared memory (one slot per K chunk), loaded by its first tile
   int b_bytes;           // shared memory of the weight region: resident slots or num_stages ring stages
+  int bias_bytes;        // shared memory of the bias vector: n_tiles_n * BN floats, 128-byte aligned
   int strip;             // 1: 3x3 stride 1, one A box {kc, tw + 2 dil, th} per filter row and channel block feeds the row's three taps
   int strip_w;           // tw + 2 dil: pixels per strip row
   int strip_box_bytes, strip_sub_bytes;   // bytes of one strip box / its 1024-aligned slot in the stage

@@ -16,8 +16,9 @@
 //   releases each operand stage as soon as the MMAs that read it have retired, and runs the epilogue (bias, activation, residual,
 //   fp16 / fp32 stores) from the accumulator registers while the producer already fetches the next tile; fp16 tiles are written as
 //   16-byte vectors of 8 channels after a transpose within each quad of lanes (epilogue()).
-// * persistent grid (one CTA per SM with a deep operand ring; two for 1x1 layers with BN <= 64, see conv_tc_prepare), programmatic
-//   dependent launch (prologue overlaps the previous kernel's tail).
+// * persistent grid (one CTA per SM with a deep operand ring, or two with resident weights and BN <= 64 where half the shared memory
+//   still holds a useful ring, see conv_tc_prepare), programmatic dependent launch (prologue overlaps the previous kernel's tail).
+//   At two CTAs per SM the producer warpgroup hands its registers to the consumers (setmaxnreg).
 //
 // Reference semantics: Conv.fuseforward (reference models/common.py:45-46) with BN folded as in
 // utils/torch_utils.py:182-202; Bottleneck shortcut add (models/common.py:105).
@@ -35,9 +36,15 @@ static constexpr int kMinResidentStages = 6;   // A stages a layer keeps next to
 static constexpr int kMaxStripBlocks = 4;      // channel blocks of a strip-mode layer (mma_strip_row instantiations)
 static constexpr int kSmemBudget = 227 * 1024;
 static constexpr int kSmemBudgetTwoCtas = 228 * 1024 / 2 - 1024;   // per CTA when two share an SM (228 KB, 1 KB reserved per CTA)
-static constexpr int kMinTwoCtaStages = 4;
-static constexpr int kBiasBytes = 8192;   // bias vector of the layer in shared memory (<= 1920 output channels: the data gradient
-                                          // of SPP.cv2 has 1024)
+static constexpr int kMinTwoCtaStages = 4;       // A stages per CTA at two CTAs per SM on the per-tap path (strip mode: 2 strip stages)
+static constexpr int kTwoCtaMaxBN = 64;          // widest N tile whose consumers fit kConsumerRegs (BN / 2 accumulators + residual vectors)
+static constexpr int kProducerRegs = 24;         // setmaxnreg at two CTAs per SM: 128 x 24 + 256 x 104 <= 384 x 80, the pool of one CTA
+static constexpr int kConsumerRegs = 104;
+static constexpr int kMaxBiasBytes = 8192;       // bias vector of the layer in shared memory (<= 1920 output channels: the data gradient
+                                                 // of SPP.cv2 has 1024)
+// weight packs up to this size stay resident: 121 KB, room for kMinResidentStages A stages and 10 KB of barriers, the largest bias vector
+// and slack, whatever the layer's Co (the 128 KB packs measured the same resident or streamed, DESIGN §5)
+static constexpr int kResidentPackLimit = kSmemBudget - 10 * 1024 - kMinResidentStages * kTileM * kKStage * 2;
 static constexpr int kSiluSfuEvery = 2;   // every n-th output channel of a 16-channel group takes the two-MUFU SiLU (balances the FMA
                                           // pipe and the SFU)
 
@@ -66,6 +73,12 @@ __device__ __forceinline__ TileCoord decode_tile(const ConvTcParams& p, int tile
   t.n0 = n_tile * p.BN;
   return t;
 }
+
+// register reallocation between warpgroups (every warp of the warpgroup executes the same instruction)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 
 __device__ __forceinline__ float act_out(float v, int act, int ch) {
   if (act == MYOLO_ACT_SILU) return (ch & 15) % kSiluSfuEvery == kSiluSfuEvery - 1 ? silu_f_sfu(v) : silu_f(v);
@@ -233,7 +246,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem_a + S * p.a_stage_bytes;                         // resident: K chunk q in slot q; else one ring stage per A stage
   float* bias_s = reinterpret_cast<float*>(smem_b + p.b_bytes);           // [n_tiles_n * BN] fp32
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(bias_s) + kBiasBytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(bias_s) + p.bias_bytes);
   uint64_t* empty_bar = full_bar + S;
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);   // warp-uniform for the compiler: wgmma is issued under role branches
@@ -258,8 +271,10 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
   }
   __syncthreads();
 
-  if (warp == 0) {
-    // ===================== TMA producer (warp-converged; one elected lane issues) =====================
+  if (warp < 4) {
+    // ===================== TMA producer (warp 0, warp-converged; one elected lane issues) =====================
+    if constexpr (CTAS_PER_SM == 2) setmaxnreg_dec<kProducerRegs>();   // warps 1-3 take part, then leave
+    if (warp != 0) return;
     const bool leader = elect_one();
     // Activations come from predecessor kernels.  The weights are loaded after this wait as well: the training step repacks them
     // (myolo_plan_repack_weights) on the same stream before the forward, and only this wait orders that repack before the loads.
@@ -305,8 +320,9 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA0, const __grid_constant__
         if (++stage == S) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp >= 4) {
+  } else {
     // ===================== consumers: two warpgroups, 64 pixel rows each =====================
+    if constexpr (CTAS_PER_SM == 2) setmaxnreg_inc<kConsumerRegs>();
     const int cw = (warp >> 2) - 1;
     const bool signaller = (threadIdx.x & 127) == 0;
     if (RES) asm volatile("griddepcontrol.wait;" ::: "memory");   // the residual is a predecessor's output
@@ -453,8 +469,63 @@ bool conv_tc_eligible(const ConvOp& op) {
   }
   // tiny maps run on the generic kernel (TMA boxes larger than the tensor are avoided on purpose)
   if (op.out.W < 8 || op.out.H < 2 || op.out.W * op.out.H < 128) return false;
-  if (align_up(op.Co, 16) * 4 + 512 > kBiasBytes) return false;   // the bias vector lives in shared memory
+  if (align_up(op.Co, 16) * 4 + 512 > kMaxBiasBytes) return false;   // the bias vector lives in shared memory
   return true;
+}
+
+// N tile bn and what follows from it: tile count, residency, strip mode, CTAs per SM, stage count, grid and shared memory.  Returns the
+// CTAs per SM.
+//
+// One CTA per SM gets as deep an operand ring as shared memory allows.  The weight slice of one N tile stays resident when it is at most
+// kResidentPackLimit and every CTA of the persistent grid keeps one N tile (grid % n_tiles_n == 0): a CTA then reads its weights from L2
+// once instead of once per tile.  Strip mode (3x3 stride 1 with resident weights, tw >= 64 so that each consumer's 64 pixels lie in one
+// strip line): a stage holds one filter row's strips of all channel blocks; at least two such stages must fit.
+//
+// Two CTAs per SM: with resident weights, BN <= kTwoCtaMaxBN and more tiles than SMs, a second CTA on each SM overlaps its waits and MMAs
+// with the first one's epilogue, which both consumer warpgroups of a CTA run on the same tile while the tensor pipe idles.  Each CTA gets
+// half the shared memory, which must hold kMinTwoCtaStages A stages on the per-tap path or two strip stages.
+static int size_launch(ConvOp& op, int bn, int num_sms) {
+  ConvTcParams& p = op.p;
+  p.BN = bn;
+  p.n_tiles_n = ceil_div((int)align_up(op.Co, 16), bn);
+  p.total_tiles = p.B * p.tiles_x * p.tiles_y * p.n_tiles_n;
+  p.fd_ntn = make_fastdiv((unsigned)p.n_tiles_n);
+  p.a_stage_bytes = kTileM * kKStage * 2;
+  p.b_stage_bytes = (int)align_up(bn * kKStage * 2, 1024);
+  p.bias_bytes = (int)align_up(p.n_tiles_n * bn * 4, 128);
+  const int misc = 1024 /*barriers*/ + p.bias_bytes + 1024 /*alignment slack*/;
+  const int b_resident_bytes = (int)align_up(p.n_chunks * bn * p.kc * 2, 1024);
+  int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
+  const int grid_resident = grid / p.n_tiles_n * p.n_tiles_n;
+  p.resident = op.reuse && grid_resident > 0 && b_resident_bytes <= kResidentPackLimit;
+  p.strip = p.strip_w = p.strip_box_bytes = p.strip_sub_bytes = 0;
+  if (p.resident && op.k == 3 && op.stride == 1 && p.tw >= 64 && p.cblocks <= kMaxStripBlocks && p.tw + 2 * op.dil <= 256) {
+    p.strip_w = p.tw + 2 * op.dil;
+    p.strip_box_bytes = p.strip_w * p.th * p.kc * 2;
+    p.strip_sub_bytes = (int)align_up(p.strip_box_bytes, 1024);
+    p.strip = (kSmemBudget - misc - b_resident_bytes) / (p.cblocks * p.strip_sub_bytes) >= 2;
+  }
+  if (p.strip) p.a_stage_bytes = p.cblocks * p.strip_sub_bytes;
+  op.ctas_per_sm = p.resident && bn <= kTwoCtaMaxBN && p.total_tiles > num_sms &&
+                           (kSmemBudgetTwoCtas - misc - b_resident_bytes) / p.a_stage_bytes >= (p.strip ? 2 : kMinTwoCtaStages)
+                       ? 2
+                       : 1;
+  const int smem_budget = op.ctas_per_sm == 2 ? kSmemBudgetTwoCtas : kSmemBudget;
+  int S;
+  if (p.resident) {
+    grid = op.ctas_per_sm == 2 ? (p.total_tiles < 2 * num_sms ? p.total_tiles : 2 * num_sms) / p.n_tiles_n * p.n_tiles_n : grid_resident;
+    p.b_stage_bytes = 0;
+    S = (smem_budget - misc - b_resident_bytes) / p.a_stage_bytes;
+    p.b_bytes = b_resident_bytes;
+  } else {
+    S = (kSmemBudget - misc) / (p.a_stage_bytes + p.b_stage_bytes);
+  }
+  if (S > kMaxStages) S = kMaxStages;
+  p.num_stages = S;
+  if (!p.resident) p.b_bytes = S * p.b_stage_bytes;
+  op.smem = S * p.a_stage_bytes + p.b_bytes + misc;
+  op.grid = grid;
+  return op.ctas_per_sm;
 }
 
 int conv_tc_prepare(ConvOp& op, int num_sms) {
@@ -470,16 +541,6 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
   p.tiles_x = ceil_div(Wo, p.tw);
   p.tiles_y = ceil_div(Ho, p.th);
   p.Co = op.Co;
-  // N tile: whole Co if it fits in 128, else the largest multiple of 16 <= 128 dividing Co16 (Co_pad sized by the caller)
-  const int co16 = (int)align_up(op.Co, 16);
-  p.BN = co16 <= 128 ? co16 : 128;
-  if (co16 > 128 && co16 % 128 != 0) {
-    for (int bn = 128; bn >= 16; bn -= 16)
-      if (co16 % bn == 0) { p.BN = bn; break; }
-  }
-  p.n_tiles_n = ceil_div(co16, p.BN);
-  MYOLO_REQUIRE(op.Co_pad >= p.n_tiles_n * p.BN, "conv_tc: Co_pad %d < %d", op.Co_pad, p.n_tiles_n * p.BN);
-  p.total_tiles = p.B * p.tiles_x * p.tiles_y * p.n_tiles_n;
   p.kc = op.Ci_pad % 64 == 0 ? 64 : (op.Ci_pad % 32 == 0 ? 32 : 16);
   p.cblocks = op.Ci_pad / p.kc;
   p.taps = op.k * op.k;
@@ -507,53 +568,24 @@ int conv_tc_prepare(ConvOp& op, int num_sms) {
       p.tap_dx[t] = (kx == 0) ? -1 : 0;
     }
   }
-  p.fd_ntn = make_fastdiv((unsigned)p.n_tiles_n);
   p.fd_tpi = make_fastdiv((unsigned)(p.tiles_x * p.tiles_y));
   p.fd_tx = make_fastdiv((unsigned)p.tiles_x);
-  // stage geometry: one CTA per SM with as deep an operand ring as shared memory allows.  The weight slice of one N tile stays resident
-  // when it fits next to kMinResidentStages A stages and every CTA of the persistent grid keeps one N tile (grid % n_tiles_n == 0):
-  // a CTA then reads its weights from L2 once instead of once per tile.
-  p.a_stage_bytes = kTileM * kKStage * 2;
-  p.b_stage_bytes = (int)align_up(p.BN * kKStage * 2, 1024);
-  const int misc = 1024 /*barriers*/ + kBiasBytes + 1024 /*alignment slack*/;
-  const int b_resident_bytes = (int)align_up(p.n_chunks * p.BN * p.kc * 2, 1024);
-  int grid = p.total_tiles < num_sms ? p.total_tiles : num_sms;
-  const int grid_resident = grid / p.n_tiles_n * p.n_tiles_n;
-  p.resident = op.reuse && grid_resident > 0 && b_resident_bytes + kMinResidentStages * p.a_stage_bytes + misc <= kSmemBudget;
-  // strip mode (3x3 stride 1 with resident weights, tw >= 64 so that each consumer's 64 pixels lie in one strip line): a stage holds
-  // one filter row's strips of all channel blocks; at least two such stages must fit
   p.dil = op.dil;
-  if (p.resident && op.k == 3 && op.stride == 1 && p.tw >= 64 && p.cblocks <= kMaxStripBlocks && p.tw + 2 * op.dil <= 256) {
-    p.strip_w = p.tw + 2 * op.dil;
-    p.strip_box_bytes = p.strip_w * p.th * p.kc * 2;
-    p.strip_sub_bytes = (int)align_up(p.strip_box_bytes, 1024);
-    p.strip = (kSmemBudget - misc - b_resident_bytes) / (p.cblocks * p.strip_sub_bytes) >= 2;
+  // N tile: whole Co if it fits in 128, else the largest multiple of 16 <= 128 dividing Co16 (Co_pad sized by the caller).  A layer
+  // that this tile keeps at one CTA per SM takes BN = 64 instead when that admits the second CTA: each CTA then keeps half the pack and
+  // A is read once per N tile (the second read from L2).  Outputs do not depend on BN: every output's K order is the same, and the
+  // SiLU variant follows the channel mod 16, which n0 (a multiple of 16) leaves unchanged.
+  const int co16 = (int)align_up(op.Co, 16);
+  int bn = co16 <= 128 ? co16 : 128;
+  if (co16 > 128 && co16 % 128 != 0) {
+    for (int b = 128; b >= 16; b -= 16)
+      if (co16 % b == 0) { bn = b; break; }
   }
-  // two CTAs per SM: a 1x1 layer with resident weights and BN <= 64 (few MMAs per tile, so a tile is mostly barrier waits and the
-  // epilogue) keeps a second CTA on each SM, whose waits and MMAs overlap the first one's epilogue.  Each CTA gets half the shared memory,
-  // with at least kMinTwoCtaStages A stages.  Not with a residual: those kernels do not fit the 80 registers of two 384-thread CTAs.
-  op.ctas_per_sm = 1;
-  if (p.resident && p.taps == 1 && p.BN <= 64 && !op.has_res && p.total_tiles > num_sms &&
-      b_resident_bytes + kMinTwoCtaStages * p.a_stage_bytes + misc <= kSmemBudgetTwoCtas)
-    op.ctas_per_sm = 2;
-  const int smem_budget = op.ctas_per_sm == 2 ? kSmemBudgetTwoCtas : kSmemBudget;
-  int S;
-  if (p.resident) {
-    grid = op.ctas_per_sm == 2 ? (p.total_tiles < 2 * num_sms ? p.total_tiles : 2 * num_sms) / p.n_tiles_n * p.n_tiles_n : grid_resident;
-    p.b_stage_bytes = 0;
-    if (p.strip) p.a_stage_bytes = p.cblocks * p.strip_sub_bytes;
-    S = (smem_budget - misc - b_resident_bytes) / p.a_stage_bytes;
-    p.b_bytes = b_resident_bytes;
-  } else {
-    S = (kSmemBudget - misc) / (p.a_stage_bytes + p.b_stage_bytes);
-  }
-  if (S > kMaxStages) S = kMaxStages;
-  MYOLO_REQUIRE(S >= 2, "conv_tc: not enough shared memory for 2 stages");
-  MYOLO_REQUIRE(p.n_tiles_n * p.BN * 4 <= kBiasBytes, "conv_tc: %d output channels exceed the shared-memory bias buffer", p.n_tiles_n * p.BN);
-  p.num_stages = S;
-  if (!p.resident) p.b_bytes = S * p.b_stage_bytes;
-  op.smem = S * p.a_stage_bytes + p.b_bytes + misc;
-  op.grid = grid;
+  if (size_launch(op, bn, num_sms) == 1 && bn > kTwoCtaMaxBN && co16 % kTwoCtaMaxBN == 0 && size_launch(op, kTwoCtaMaxBN, num_sms) == 1)
+    size_launch(op, bn, num_sms);
+  MYOLO_REQUIRE(op.Co_pad >= p.n_tiles_n * p.BN, "conv_tc: Co_pad %d < %d", op.Co_pad, p.n_tiles_n * p.BN);
+  MYOLO_REQUIRE(p.num_stages >= 2, "conv_tc: not enough shared memory for 2 stages");
+  MYOLO_REQUIRE(p.n_tiles_n * p.BN * 4 <= kMaxBiasBytes, "conv_tc: %d output channels exceed the shared-memory bias buffer", p.n_tiles_n * p.BN);
 
   // ---- tensor maps ----
   const int esz = 2;
@@ -605,7 +637,7 @@ static cudaError_t launch_kernel(const ConvOp& op, const cudaLaunchConfig_t& cfg
 
 template <int KC, int BN, bool RES>
 static cudaError_t launch_bn(const ConvOp& op, const cudaLaunchConfig_t& cfg) {
-  if constexpr (BN <= 64 && !RES)
+  if constexpr (BN <= kTwoCtaMaxBN)
     if (op.ctas_per_sm == 2) return launch_kernel<KC, BN, RES, 2>(op, cfg);
   if (op.ctas_per_sm != 1) return cudaErrorInvalidValue;
   return launch_kernel<KC, BN, RES, 1>(op, cfg);

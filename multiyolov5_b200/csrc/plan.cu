@@ -783,6 +783,16 @@ extern "C" int myolo_plan_profile(myolo_plan* pl, const void* x, int x_dtype, fl
 
 extern "C" int64_t myolo_plan_last_launch_count(const myolo_plan* pl) { return pl ? pl->last_launches : 0; }
 
+static void conv_info_slots(const ConvOp& c, int32_t* info) {
+  for (int i = 0; i < 12; ++i) info[i] = 0;
+  info[0] = c.use_tc ? 1 : 0;
+  if (c.use_tc) {
+    info[1] = c.grid; info[2] = c.smem; info[3] = c.p.BN; info[4] = c.p.num_stages; info[5] = c.p.strip;
+    info[6] = c.p.resident; info[7] = 1; info[8] = c.p.total_tiles; info[9] = c.p.n_tiles_n; info[10] = c.p.kc;
+    info[11] = c.ctas_per_sm;
+  }
+}
+
 // which kernel a conv op of the plan takes and how it is tiled (valid after the first forward): info[0..11] =
 // {1 wgmma / 0 CUDA-core, grid, dynamic smem bytes, BN, pipeline stages, mode (0: one TMA box per tap, 1: one strip per filter row),
 //  weights-stationary (1: the CTA keeps its weight slice in shared memory),
@@ -792,14 +802,7 @@ extern "C" int myolo_plan_conv_info(myolo_plan* pl, int op_index, int32_t* info)
   MYOLO_REQUIRE(pl->ops[op_index].kind == MYOLO_OP_CONV, "conv_info: op %d is not a conv", op_index);
   int rc;
   if (!pl->conv_ready[op_index] && (rc = prepare_conv(pl, op_index))) return rc;
-  const ConvOp& c = pl->convs[op_index];
-  for (int i = 0; i < 12; ++i) info[i] = 0;
-  info[0] = c.use_tc ? 1 : 0;
-  if (c.use_tc) {
-    info[1] = c.grid; info[2] = c.smem; info[3] = c.p.BN; info[4] = c.p.num_stages; info[5] = c.p.strip;
-    info[6] = c.p.resident; info[7] = 1; info[8] = c.p.total_tiles; info[9] = c.p.n_tiles_n; info[10] = c.p.kc;
-    info[11] = c.ctas_per_sm;
-  }
+  conv_info_slots(pl->convs[op_index], info);
   return 0;
 }
 
@@ -1650,9 +1653,10 @@ extern "C" int myolo_allreduce_grads(float* flat_grad, int64_t n, void* nccl_com
 // ------------------------------------------------------------------------------------------------
 // standalone fused conv (per-op parity tests, ncu captures)
 // ------------------------------------------------------------------------------------------------
-extern "C" int myolo_conv_bn_silu_slice(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,
-                                        const float* gamma, const float* beta, const float* mean, const float* var, float eps,
-                                        const float* bias, int act, const void* residual, void* y, int y_ctot, int path, void* stream) {
+extern "C" int myolo_conv_bn_silu_info(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,
+                                       const float* gamma, const float* beta, const float* mean, const float* var, float eps,
+                                       const float* bias, int act, const void* residual, void* y, int y_ctot, int path, int32_t* info,
+                                       void* stream) {
   MYOLO_REQUIRE(x && w && y && B > 0 && H > 0 && W > 0 && ci > 0 && co > 0 && y_ctot >= co, "conv_bn_silu: bad arguments");
   MYOLO_REQUIRE(ci % 16 == 0 && co % 8 == 0, "conv_bn_silu: standalone entry needs ci %% 16 == 0 and co %% 8 == 0");
   int sms = 0;
@@ -1690,9 +1694,11 @@ extern "C" int myolo_conv_bn_silu_slice(const void* x, int B, int H, int W, int 
       rc = conv_simt_launch(c, s);
     } else {
       c.reuse = path != 3;     // path 3: streamed weights, the layout the reuse paths are checked against
+      c.use_tc = true;
       rc = conv_tc_prepare(c, sms);
       if (!rc) rc = conv_tc_launch(c, s);
     }
+    if (!rc && info) conv_info_slots(c, info);
   }
   cudaError_t e = cudaStreamSynchronize(s);
   cudaFree(wp);
@@ -1702,6 +1708,13 @@ extern "C" int myolo_conv_bn_silu_slice(const void* x, int B, int H, int W, int 
     rc = MYOLO_E_CUDA;
   }
   return rc;
+}
+
+extern "C" int myolo_conv_bn_silu_slice(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,
+                                        const float* gamma, const float* beta, const float* mean, const float* var, float eps,
+                                        const float* bias, int act, const void* residual, void* y, int y_ctot, int path, void* stream) {
+  return myolo_conv_bn_silu_info(x, B, H, W, ci, w, co, k, stride, dil, gamma, beta, mean, var, eps, bias, act, residual, y, y_ctot, path,
+                                 nullptr, stream);
 }
 
 extern "C" int myolo_conv_bn_silu(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,
