@@ -221,6 +221,23 @@ int myolo_plan_read_grad_view(myolo_plan* plan, myolo_view view, float* dst_nchw
  * dil*(k/2); dW fp32 [co][ci][k][k] is ACCUMULATED into.  path 0: mma.sync kernel, 1: wgmma kernel (needs ci % 64 == 0, Wo % 16 == 0) */
 int myolo_conv_wgrad(const void* x, const void* dy, int B, int H, int W, int ci, int co, int k, int stride, int dil, float* dW, int path,
                      void* stream);
+/* standalone backward of one conv through the train plan's own routing and launches (per-op tests).  Views are channel slices of NHWC
+ * buffers (base of the buffer, channels per pixel ctot, first channel c_off), as the plan passes them:
+ *   x     (B,H,W) fp16 / fp32, ci rounded up to 16 channels (the padding channels hold zeros);
+ *   dy    (B,Ho,Wo) fp16 with co channels, or an fp32 head gradient with co rounded up to 16 (zero padding);
+ *   gin   grad(in), nullable (no data gradient), x's dtype and channel count: ACCUMULATED into;
+ *   w     fp32 master weights [co][ci][k][k]; dW (same layout) and dbias [co] (nullable) are ACCUMULATED into.
+ * "same" padding dil*(k/2).  route: 0 as the plan, or MYOLO_CONV_BWD_* bits.  info (nullable) receives 16 slots:
+ *   0  data gradient: 0 none, 1 small (generic kernel, fp32 weights), 2 wgmma conv, 3 CUDA-core conv
+ *   1  weight gradient: 1 small, 2 mma.sync, 3 wgmma into dW, 4 wgmma through a packed buffer
+ *   2  bias gradient: 0 none, 1 summed from fp32 dY, 2 from fp16 dY
+ *   3-7  wgmma data gradient: kc, BN, CTAs per SM, weights resident, strip mode;  13-14: N tiles, padded output channels of the pack
+ *   8-12 wgmma weight gradient: pixels per step Kc, N, row slabs, rows per slab, rows in all */
+#define MYOLO_CONV_BWD_SIMT 1          /* data gradient on the CUDA-core conv (as MYOLO_FORCE_SIMT=1 does for a plan) */
+#define MYOLO_CONV_BWD_NO_WGRAD_TC 2   /* weight gradient on the mma.sync kernel where the wgmma one would run */
+int myolo_conv_backward(const void* x, int x_dtype, int B, int H, int W, int x_ctot, int x_coff, const void* dy, int dy_dtype, int dy_ctot,
+                        int dy_coff, void* gin, int gin_ctot, int gin_coff, const float* w, int co, int ci, int k, int stride, int dil,
+                        float* dW, float* dbias, int route, int32_t* info, void* stream);
 int myolo_grads_check_finite(const float* grad, int64_t n, int32_t* found_inf /* device */, void* stream);
 int myolo_sgd_step(float* param, float* grad, float* momentum_buf, const uint8_t* group, int64_t n, const float* lr,
                    const float* weight_decay, int n_groups, float momentum, int nesterov, const float* inv_scale /* device */,

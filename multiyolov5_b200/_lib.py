@@ -42,12 +42,14 @@ EXPORTS = [
     "myolo_anchor_metric", "myolo_anchor_metric_workspace_bytes", "myolo_anchor_evolve", "myolo_anchor_evolve_workspace_bytes",
     "myolo_kmeans", "myolo_kmeans_workspace_bytes", "myolo_class_weights", "myolo_image_weights", "myolo_weighted_draw",
     "myolo_plan_backward_seg_loss", "myolo_seg_focal_loss", "myolo_seg_focal_loss_backward", "myolo_seg_focal_loss_workspace_bytes",
+    "myolo_conv_backward",
 ]
 REDUCTION_MEAN, REDUCTION_SUM = 0, 1        # include/myolo.h: MYOLO_REDUCTION_* of myolo_seg_focal_loss
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
 KMEANS_MAX_ITER, KMEANS_BAD_INDEX = 1, 2                                 # include/myolo.h: bits of myolo_kmeans' status word
 IW_BAD_CLASS, IW_TOTAL_NONPOS, IW_TOTAL_NONFINITE = 1, 2, 4              # include/myolo.h: bits of the image-weights status word
 IW_NC_MAX = 1024                                                         # include/myolo.h MYOLO_IW_NC_MAX
+CONV_BWD_SIMT, CONV_BWD_NO_WGRAD_TC = 1, 2                               # include/myolo.h: route bits of myolo_conv_backward
 
 
 class BufDesc(C.Structure):
@@ -171,6 +173,8 @@ def lib():
     L.myolo_plan_train_forward_multi.argtypes = [vp, vp, i32, C.POINTER(vp), C.POINTER(vp), vp]
     L.myolo_plan_backward_multi.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), vp]
     L.myolo_conv_wgrad.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp]
+    L.myolo_conv_backward.argtypes = [vp, i32, i32, i32, i32, i32, i32, vp, i32, i32, i32, vp, i32, i32, vp, i32, i32, i32, i32, i32, vp, vp,
+                                      i32, C.POINTER(C.c_int32), vp]
     L.myolo_grads_check_finite.argtypes = [vp, i64, vp, vp]
     L.myolo_sgd_step.argtypes = [vp, vp, vp, vp, i64, C.POINTER(f32), C.POINTER(f32), i32, f32, i32, vp, vp, i32, vp]
     L.myolo_adam_step.argtypes = [vp, vp, vp, vp, vp, i64, C.POINTER(C.c_double), C.POINTER(f32), i32, C.c_double, C.c_double, C.c_double,

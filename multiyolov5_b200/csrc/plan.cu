@@ -985,9 +985,150 @@ static int ensure_tmp16(myolo_plan* pl, size_t bytes) {
   return 0;
 }
 
-// backward of one conv op: dY = grad(out); grad(in) += conv^T(dY, W); dW += ...; dbias += ...
-// `ws`: stream of the weight / bias gradient kernels.  Nothing downstream in the backward pass reads them, so the walk forks them onto a
-// side lane (ws != s) where they overlap the latency-bound chain of data-gradient / BN kernels; the caller joins the lane at the end.
+// which kernels the backward of one conv takes (myolo_conv_backward's info slots 0-2)
+enum { kDgradNone = 0, kDgradSmall = 1, kDgradWgmma = 2, kDgradSimt = 3 };
+enum { kWgradSmall = 1, kWgradMma = 2, kWgradWgmmaDirect = 3, kWgradWgmmaPacked = 4 };
+
+// tiny maps / fp32 inputs: generic kernels on the fp32 master weights
+static bool conv_bwd_small(const TensorView& xin, const TensorView& gout) {
+  return xin.dtype == MYOLO_F32 || (long)gout.B * gout.H * gout.W <= 1024 || gout.H * gout.W < 128;
+}
+
+// fp16 scratch of the backward of one conv: dY cast from fp32 (head gradients) at 0, the zero-stuffed stride-2 dY at *stuffed_off
+static size_t conv_bwd_tmp16_bytes(const TensorView& xin, const TensorView& gout, int co, int stride, size_t* stuffed_off) {
+  if (conv_bwd_small(xin, gout)) return 0;
+  const int cpad = (int)align_up(co, 16);
+  size_t need = 0;
+  if (gout.dtype == MYOLO_F32) need = (size_t)gout.B * gout.H * gout.W * cpad * 2;
+  if (stuffed_off) *stuffed_off = align_up((int64_t)need, 256);
+  if (stride == 2) need = align_up((int64_t)need, 256) + (size_t)gout.B * (2 * gout.H) * (2 * gout.W) * cpad * 2;
+  return need;
+}
+
+// the scratch the backward of one conv works in: the fp16 dY scratch (at least conv_bwd_tmp16_bytes) and the data-gradient conv, whose
+// tensor maps (built once, *dconv_ready) point into tmp16 and grad(in)
+struct ConvBwdScratch {
+  __half* tmp16;
+  ConvOp* dconv;
+  int* dconv_ready;
+};
+
+// backward of one conv on resolved views: dY = gout; grad(in) += conv^T(dY, W) when gin is given; dW += ...; dbias += ...
+// `ws`: stream of the weight / bias gradient kernels, forked from s at `fork` (null: they stay on s).  Nothing downstream in the backward
+// pass reads them, so the plan's walk forks them onto a side lane where they overlap the latency-bound chain of data-gradient / BN kernels;
+// the caller joins the lane at the end.  info (nullable, 16 slots): see myolo_conv_backward in include/myolo.h.
+static int conv_backward_views(const TensorView& xin, const TensorView& gout, const TensorView* gin, WeightSlot& sl, int k, int stride,
+                               int dil, const ConvBwdScratch& scr, int num_sms, bool force_simt, bool no_wgrad_tc, cudaStream_t s,
+                               cudaStream_t ws, cudaEvent_t fork, bool* used_side, int32_t* info) {
+  int rc;
+  if (info)
+    for (int j = 0; j < 16; ++j) info[j] = 0;
+  if (conv_bwd_small(xin, gout)) {
+    TensorView gy = gout;
+    gy.C = sl.co;
+    if (info) {
+      info[0] = gin ? kDgradSmall : kDgradNone;
+      info[1] = kWgradSmall;
+      info[2] = sl.d_bias ? (gout.dtype == MYOLO_F32 ? 1 : 2) : 0;
+    }
+    return launch_conv_small_bwd(xin, gy, gin, sl.w_master, sl.d_w, sl.d_bias, sl.co, sl.ci, k, stride, dil, s);
+  }
+  // dY in fp16 (cast fp32 head gradients; zero-stuff for stride 2)
+  const int cpad = (int)align_up(sl.co, 16);
+  TensorView dy16 = gout;
+  size_t stuffed_off = 0;
+  conv_bwd_tmp16_bytes(xin, gout, sl.co, stride, &stuffed_off);
+  const bool s2 = stride == 2;
+  if (gout.dtype == MYOLO_F32) {
+    dy16 = TensorView{scr.tmp16, gout.B, gout.H, gout.W, cpad, cpad, MYOLO_F16};
+    if ((rc = launch_cast_f32_to_f16(gout, dy16, s))) return rc;
+  } else {
+    MYOLO_REQUIRE(gout.C == sl.co && sl.co % 16 == 0, "conv backward: fp16 conv gradient needs Co %% 16 == 0 (Co=%d)", sl.co);
+  }
+  // weight / bias gradients
+  // dY in the shared fp16 scratch (fp32 head gradients) is overwritten by the next conv: those few layers stay on the main stream
+  cudaStream_t wst = (fork && ws != s && gout.dtype != MYOLO_F32) ? ws : s;
+  if (wst != s) {
+    MYOLO_CHECK_CUDA(cudaEventRecord(fork, s));          // dY (and everything before it on the main chain) is final here
+    MYOLO_CHECK_CUDA(cudaStreamWaitEvent(wst, fork, 0));
+    *used_side = true;
+  }
+  if (!no_wgrad_tc && conv_wgrad_tc_eligible(xin, dy16, k, stride, dil, sl.co, sl.ci)) {
+    const size_t nb = conv_wgrad_packed_bytes(sl.d_w, sl.co, sl.ci, k);
+    if (!sl.dw_packed && nb) {
+      MYOLO_CHECK_CUDA(cudaMalloc(&sl.dw_packed, nb));
+      MYOLO_CHECK_CUDA(cudaMemset(sl.dw_packed, 0, nb));
+    }
+    if (info) info[1] = nb ? kWgradWgmmaPacked : kWgradWgmmaDirect;
+    if ((rc = launch_conv_wgrad_tc(xin, dy16, k, stride, dil, sl.d_w, sl.dw_packed, sl.co, sl.ci, num_sms, wst, info ? info + 8 : nullptr)))
+      return rc;
+  } else {
+    if (info) info[1] = kWgradMma;
+    if ((rc = launch_conv_wgrad(xin, dy16, k, stride, dil, sl.d_w, sl.co, sl.ci, nullptr, wst))) return rc;
+  }
+  if (sl.d_bias) {   // the bias gradient of an fp32 head gradient is summed from the fp32 values, not from their fp16 cast
+    TensorView gy = gout.dtype == MYOLO_F32 ? gout : dy16;
+    gy.C = sl.co;
+    if (info) info[2] = gy.dtype == MYOLO_F32 ? 1 : 2;
+    if ((rc = launch_bias_grad(gy, sl.d_bias, sl.co, wst))) return rc;
+  }
+  if (!gin) return 0;
+  // data gradient = stride-1 conv of (zero-stuffed) dY with flipped / transposed weights, accumulated into grad(in).  Its N tile (sl.ci
+  // rounded up to 16 channels, or a multiple of 16 dividing that: conv_tc_prepare) never reaches past the padded pack.
+  const int n_pad = (int)align_up(sl.ci, 16);
+  if (!sl.w_dgrad) {
+    MYOLO_CHECK_CUDA(cudaMalloc(&sl.w_dgrad, (size_t)n_pad * k * k * cpad * 2));
+    MYOLO_CHECK_CUDA(cudaMalloc(&sl.zero_bias, (size_t)n_pad * 4));
+  }
+  if (!sl.dgrad_valid) {   // (first use; later refreshes happen in refresh_dgrad_packs, outside any captured graph)
+    if ((rc = pack_dgrad_weights(sl.w_master, sl.co, sl.ci, k, sl.w_dgrad, sl.zero_bias, n_pad, cpad, s))) return rc;
+    sl.dgrad_valid = true;
+    sl.dgrad_n_pad = n_pad;
+    sl.dgrad_cpad = cpad;
+  }
+  TensorView din = dy16;
+  if (s2) {
+    din = TensorView{reinterpret_cast<unsigned char*>(scr.tmp16) + stuffed_off, gout.B, 2 * gout.H, 2 * gout.W, cpad, cpad, MYOLO_F16};
+    TensorView src = dy16;
+    src.C = cpad;
+    if (gout.dtype != MYOLO_F32) { src = gout; }
+    MYOLO_REQUIRE(src.C == cpad, "conv backward: stride-2 gradient channel padding mismatch");
+    if ((rc = launch_zero_stuff2(src, din, s))) return rc;
+  }
+  ConvOp& c = *scr.dconv;
+  if (!*scr.dconv_ready) {
+    c = ConvOp();
+    c.in = din;
+    c.in.C = cpad;
+    c.out = *gin;
+    c.out.C = sl.ci;
+    c.has_res = true;
+    c.res = c.out;
+    c.k = k;
+    c.stride = 1;
+    c.dil = dil;
+    c.act = MYOLO_ACT_NONE;
+    c.w = sl.w_dgrad;
+    c.bias = sl.zero_bias;
+    c.Ci_pad = cpad;
+    c.Co_pad = n_pad;
+    c.Co = sl.ci;
+    MYOLO_REQUIRE(din.H == gin->H && din.W == gin->W, "conv backward: data-gradient geometry %dx%d vs %dx%d", din.H, din.W, gin->H, gin->W);
+    c.use_tc = !force_simt && conv_tc_eligible(c);
+    if (c.use_tc && (rc = conv_tc_prepare(c, num_sms))) return rc;
+    *scr.dconv_ready = 1;
+  }
+  if (info) {
+    info[0] = c.use_tc ? kDgradWgmma : kDgradSimt;
+    if (c.use_tc) {
+      info[3] = c.p.kc; info[4] = c.p.BN; info[5] = c.ctas_per_sm; info[6] = c.p.resident; info[7] = c.p.strip;
+      info[13] = c.p.n_tiles_n; info[14] = c.Co_pad;
+    }
+  }
+  return c.use_tc ? conv_tc_launch(c, s) : conv_simt_launch(c, s);
+}
+
+// backward of one conv op of the plan on its views in the activation / gradient workspaces
 static int conv_backward(myolo_plan* pl, int i, bool need_dgrad, cudaStream_t s, cudaStream_t ws, bool* used_side) {
   const myolo_op& op = pl->ops[i];
   WeightSlot& sl = pl->slots[op.weight_slot];
@@ -995,100 +1136,16 @@ static int conv_backward(myolo_plan* pl, int i, bool need_dgrad, cudaStream_t s,
   TensorView xin, gout, gin;
   int rc;
   if ((rc = resolve_view(pl, op.in, &xin)) || (rc = grad_view(pl, op.out, &gout)) || (rc = grad_view(pl, op.in, &gin))) return rc;
-  const long npix_out = (long)gout.B * gout.H * gout.W;
-  // tiny maps / fp32 inputs: generic kernels on the fp32 master weights
-  if (xin.dtype == MYOLO_F32 || npix_out <= 1024 || gout.H * gout.W < 128) {
-    TensorView gy = gout;
-    gy.C = sl.co;
-    return launch_conv_small_bwd(xin, gy, need_dgrad ? &gin : nullptr, sl.w_master, sl.d_w, sl.d_bias, sl.co, sl.ci, op.k, op.stride, op.dil, s);
-  }
-  // dY in fp16 (cast fp32 head gradients; zero-stuff for stride 2)
-  const int cpad = (int)align_up(sl.co, 16);
-  TensorView dy16 = gout;
-  size_t need = 0;
-  if (gout.dtype == MYOLO_F32) need = (size_t)npix_out * cpad * 2;
-  const bool s2 = op.stride == 2;
-  size_t stuffed_off = align_up((int64_t)need, 256);
-  if (s2) need = stuffed_off + (size_t)gout.B * (2 * gout.H) * (2 * gout.W) * cpad * 2;
+  const size_t need = conv_bwd_tmp16_bytes(xin, gout, sl.co, op.stride, nullptr);
   if (need && (rc = ensure_tmp16(pl, need))) return rc;
-  if (gout.dtype == MYOLO_F32) {
-    dy16 = TensorView{pl->tmp16, gout.B, gout.H, gout.W, cpad, cpad, MYOLO_F16};
-    if ((rc = launch_cast_f32_to_f16(gout, dy16, s))) return rc;
-  } else {
-    MYOLO_REQUIRE(gout.C == sl.co && sl.co % 16 == 0, "op %d: fp16 conv gradient needs Co %% 16 == 0 (Co=%d)", i, sl.co);
-  }
-  // weight / bias gradients
-  // dY in the shared fp16 scratch (fp32 head gradients) is overwritten by the next conv: those few layers stay on the main stream
-  cudaStream_t wst = (ws != s && gout.dtype != MYOLO_F32 && (int)pl->op_ev.size() > i) ? ws : s;
-  if (wst != s) {
-    MYOLO_CHECK_CUDA(cudaEventRecord(pl->op_ev[i], s));          // dY (and everything before it on the main chain) is final here
-    MYOLO_CHECK_CUDA(cudaStreamWaitEvent(wst, pl->op_ev[i], 0));
-    *used_side = true;
-  }
-  if (conv_wgrad_tc_eligible(xin, dy16, op.k, op.stride, op.dil, sl.co, sl.ci)) {
-    const size_t nb = conv_wgrad_packed_bytes(sl.d_w, sl.co, sl.ci, op.k);
-    if (!sl.dw_packed && nb) {
-      MYOLO_CHECK_CUDA(cudaMalloc(&sl.dw_packed, nb));
-      MYOLO_CHECK_CUDA(cudaMemset(sl.dw_packed, 0, nb));
-    }
-    if ((rc = launch_conv_wgrad_tc(xin, dy16, op.k, op.stride, op.dil, sl.d_w, sl.dw_packed, sl.co, sl.ci, pl->num_sms, wst))) return rc;
-  } else if ((rc = launch_conv_wgrad(xin, dy16, op.k, op.stride, op.dil, sl.d_w, sl.co, sl.ci, nullptr, wst))) {
-    return rc;
-  }
-  if (sl.d_bias) {   // the bias gradient of an fp32 head gradient is summed from the fp32 values, not from their fp16 cast
-    TensorView gy = gout.dtype == MYOLO_F32 ? gout : dy16;
-    gy.C = sl.co;
-    if ((rc = launch_bias_grad(gy, sl.d_bias, sl.co, wst))) return rc;
-  }
-  if (!need_dgrad) return 0;
-  // data gradient = stride-1 conv of (zero-stuffed) dY with flipped / transposed weights, accumulated into grad(in)
-  const int ci_out_pad = (int)align_up(sl.ci, 16);
-  const int n_pad = ((ci_out_pad <= 128) ? ci_out_pad : [&] { for (int bn = 128; bn >= 16; bn -= 16) if (ci_out_pad % bn == 0) return ci_out_pad; return ci_out_pad; }());
-  if (!sl.w_dgrad) {
-    MYOLO_CHECK_CUDA(cudaMalloc(&sl.w_dgrad, (size_t)n_pad * op.k * op.k * cpad * 2));
-    MYOLO_CHECK_CUDA(cudaMalloc(&sl.zero_bias, (size_t)n_pad * 4));
-    pl->pack_table_dirty = true;
-  }
-  if (!sl.dgrad_valid) {   // (first use; later refreshes happen in refresh_dgrad_packs, outside any captured graph)
-    if ((rc = pack_dgrad_weights(sl.w_master, sl.co, sl.ci, op.k, sl.w_dgrad, sl.zero_bias, n_pad, cpad, s))) return rc;
-    sl.dgrad_valid = true;
-    sl.dgrad_n_pad = n_pad;
-    sl.dgrad_cpad = cpad;
-  }
-  TensorView din = dy16;
-  if (s2) {
-    din = TensorView{reinterpret_cast<unsigned char*>(pl->tmp16) + stuffed_off, gout.B, 2 * gout.H, 2 * gout.W, cpad, cpad, MYOLO_F16};
-    TensorView src = dy16;
-    src.C = cpad;
-    if (gout.dtype != MYOLO_F32) { src = gout; }
-    MYOLO_REQUIRE(src.C == cpad, "op %d: stride-2 gradient channel padding mismatch", i);
-    if ((rc = launch_zero_stuff2(src, din, s))) return rc;
-  }
   if (pl->dconvs.size() != pl->ops.size()) { pl->dconvs.resize(pl->ops.size()); pl->dconv_ready.assign(pl->ops.size(), 0); }
-  ConvOp& c = pl->dconvs[i];
-  if (!pl->dconv_ready[i]) {
-    c = ConvOp();
-    c.in = din;
-    c.in.C = cpad;
-    c.out = gin;
-    c.out.C = sl.ci;
-    c.has_res = true;
-    c.res = c.out;
-    c.k = op.k;
-    c.stride = 1;
-    c.dil = op.dil;
-    c.act = MYOLO_ACT_NONE;
-    c.w = sl.w_dgrad;
-    c.bias = sl.zero_bias;
-    c.Ci_pad = cpad;
-    c.Co_pad = n_pad;
-    c.Co = sl.ci;
-    MYOLO_REQUIRE(din.H == gin.H && din.W == gin.W, "op %d: data-gradient geometry %dx%d vs %dx%d", i, din.H, din.W, gin.H, gin.W);
-    c.use_tc = !pl->force_simt && conv_tc_eligible(c);
-    if (c.use_tc && (rc = conv_tc_prepare(c, pl->num_sms))) return rc;
-    pl->dconv_ready[i] = 1;
-  }
-  return c.use_tc ? conv_tc_launch(c, s) : conv_simt_launch(c, s);
+  const bool had_pack = sl.w_dgrad != nullptr;
+  const ConvBwdScratch scr{pl->tmp16, &pl->dconvs[i], &pl->dconv_ready[i]};
+  cudaEvent_t fork = (ws != s && (int)pl->op_ev.size() > i) ? pl->op_ev[i] : nullptr;
+  rc = conv_backward_views(xin, gout, need_dgrad ? &gin : nullptr, sl, op.k, op.stride, op.dil, scr, pl->num_sms, pl->force_simt, false, s,
+                           ws, fork, used_side, nullptr);
+  if (!had_pack && sl.w_dgrad) pl->pack_table_dirty = true;   // the grouped repack refreshes the new data-gradient pack from now on
+  return rc;
 }
 
 // seeds: dL/d(raw x_i) and dL/d(seg) written into the gradient buffers of the head convs (caller-owned memory: never captured)
@@ -1456,6 +1513,58 @@ extern "C" int myolo_conv_wgrad(const void* x, const void* dy, int B, int H, int
   rc = launch_conv_wgrad_tc(xv, dv, k, stride, dil, dW, packed, co, ci, sms, s);
   cudaStreamSynchronize(s);
   if (packed) cudaFree(packed);
+  return rc;
+}
+
+extern "C" int myolo_conv_backward(const void* x, int x_dtype, int B, int H, int W, int x_ctot, int x_coff, const void* dy, int dy_dtype,
+                                   int dy_ctot, int dy_coff, void* gin, int gin_ctot, int gin_coff, const float* w, int co, int ci, int k,
+                                   int stride, int dil, float* dW, float* dbias, int route, int32_t* info, void* stream) {
+  NvtxRange nvtx_("myolo_conv_backward");
+  MYOLO_REQUIRE(x && dy && w && dW && B > 0 && H > 0 && W > 0 && co > 0 && ci > 0 && k >= 1 && k % 2 == 1 && (stride == 1 || stride == 2) &&
+                dil >= 1 && (route & ~(MYOLO_CONV_BWD_SIMT | MYOLO_CONV_BWD_NO_WGRAD_TC)) == 0, "conv_backward: bad arguments");
+  MYOLO_REQUIRE((x_dtype == MYOLO_F16 || x_dtype == MYOLO_F32) && (dy_dtype == MYOLO_F16 || dy_dtype == MYOLO_F32),
+                "conv_backward: x and dy must be MYOLO_F16 or MYOLO_F32");
+  // the plan's views: x and grad(in) carry ci rounded up to 16 channels; an fp32 head gradient carries co rounded up to 16 (zero padding)
+  const int xc = (int)align_up(ci, 16), dyc = dy_dtype == MYOLO_F32 ? (int)align_up(co, 16) : co;
+  MYOLO_REQUIRE(x_coff >= 0 && x_coff + xc <= x_ctot && dy_coff >= 0 && dy_coff + dyc <= dy_ctot &&
+                (!gin || (gin_coff >= 0 && gin_coff + xc <= gin_ctot)), "conv_backward: channel slice outside its buffer");
+  int sms = 0;
+  int rc = check_device(&sms);
+  if (rc) return rc;
+  const int pad = dil * (k / 2);
+  const int Ho = (H + 2 * pad - dil * (k - 1) - 1) / stride + 1, Wo = (W + 2 * pad - dil * (k - 1) - 1) / stride + 1;
+  MYOLO_REQUIRE(Ho > 0 && Wo > 0, "conv_backward: empty output map");
+  const size_t xes = x_dtype == MYOLO_F16 ? 2 : 4, dyes = dy_dtype == MYOLO_F16 ? 2 : 4;
+  const TensorView xv{const_cast<unsigned char*>(static_cast<const unsigned char*>(x)) + (size_t)x_coff * xes, B, H, W, xc, x_ctot, x_dtype};
+  const TensorView dv{const_cast<unsigned char*>(static_cast<const unsigned char*>(dy)) + (size_t)dy_coff * dyes, B, Ho, Wo, dyc, dy_ctot,
+                      dy_dtype};
+  const TensorView gv{gin ? static_cast<unsigned char*>(gin) + (size_t)gin_coff * xes : nullptr, B, H, W, xc, gin_ctot, x_dtype};
+  cudaStream_t s = (cudaStream_t)stream;
+  WeightSlot sl;
+  sl.co = co;
+  sl.ci = ci;
+  sl.k = k;
+  sl.set = true;
+  sl.w_master = w;
+  sl.d_w = dW;
+  sl.d_bias = dbias;
+  ConvOp dconv;
+  int dconv_ready = 0;
+  __half* tmp16 = nullptr;
+  const size_t need = conv_bwd_tmp16_bytes(xv, dv, co, stride, nullptr);
+  if (need) MYOLO_CHECK_CUDA(cudaMalloc(&tmp16, need));
+  bool used_side = false;
+  rc = conv_backward_views(xv, dv, gin ? &gv : nullptr, sl, k, stride, dil, ConvBwdScratch{tmp16, &dconv, &dconv_ready}, sms,
+                           (route & MYOLO_CONV_BWD_SIMT) != 0, (route & MYOLO_CONV_BWD_NO_WGRAD_TC) != 0, s, s, nullptr, &used_side, info);
+  const cudaError_t e = cudaStreamSynchronize(s);
+  if (tmp16) cudaFree(tmp16);
+  if (sl.w_dgrad) cudaFree(sl.w_dgrad);
+  if (sl.zero_bias) cudaFree(sl.zero_bias);
+  if (sl.dw_packed) cudaFree(sl.dw_packed);
+  if (!rc && e != cudaSuccess) {
+    set_error("conv_backward: kernel failed: %s", cudaGetErrorString(e));
+    rc = MYOLO_E_CUDA;
+  }
   return rc;
 }
 

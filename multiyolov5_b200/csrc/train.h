@@ -126,8 +126,9 @@ int launch_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay,
 // wgmma weight gradient (wgrad_tc.cu): dw_packed is a zeroed fp32 [co][k*k][ci] accumulation buffer owned by the caller
 bool conv_wgrad_tc_eligible(const TensorView& x, const TensorView& dy, int k, int stride, int dil, int co, int ci);
 size_t conv_wgrad_packed_bytes(const float* dW, int co, int ci, int k);   // 0: accumulates straight into dW
+// tiling (nullable): {pixels per step Kc, N, row slabs, rows per slab, rows in all}
 int launch_conv_wgrad_tc(const TensorView& x, const TensorView& dy, int k, int stride, int dil, float* dW, float* dw_packed, int co, int ci,
-                         int num_sms, cudaStream_t s);
+                         int num_sms, cudaStream_t s, int32_t* tiling = nullptr);
 // tiny maps / fp32 tensors: generic backward straight from the fp32 master weights (dx nullable: += ; dW += ; dbias += )
 int launch_conv_small_bwd(const TensorView& x, const TensorView& dy, const TensorView* dx, const float* w, float* dW, float* dbias, int co,
                           int ci, int k, int stride, int dil, cudaStream_t s);

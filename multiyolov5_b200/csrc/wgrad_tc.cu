@@ -237,7 +237,7 @@ size_t conv_wgrad_packed_bytes(const float* dW, int co, int ci, int k) {
 }
 
 int launch_conv_wgrad_tc(const TensorView& x, const TensorView& dy, int k, int stride, int dil, float* dW, float* dw_packed, int co, int ci,
-                         int num_sms, cudaStream_t s) {
+                         int num_sms, cudaStream_t s, int32_t* tiling) {
   MYOLO_REQUIRE(conv_wgrad_tc_eligible(x, dy, k, stride, dil, co, ci) && dW, "conv_wgrad_tc: unsupported geometry");
   const int cp = (ci + 15) / 16 * 16;
   const bool direct = conv_wgrad_packed_bytes(dW, co, ci, k) == 0;
@@ -273,6 +273,9 @@ int launch_conv_wgrad_tc(const TensorView& x, const TensorView& dy, int k, int s
   p.rows_per_cta = ceil_div(p.rows_total, slabs);
   slabs = ceil_div(p.rows_total, p.rows_per_cta);
   p.dw_packed = direct ? dW : dw_packed;
+  if (tiling) {
+    tiling[0] = p.Kc; tiling[1] = p.N; tiling[2] = slabs; tiling[3] = p.rows_per_cta; tiling[4] = p.rows_total;
+  }
 
   CUtensorMap tmDy, tmX[4];
   const int esz = 2;

@@ -39,3 +39,28 @@ def conv_bn_silu(x_nhwc: torch.Tensor, w: torch.Tensor, bn=None, bias=None, stri
     if info is not None:
         info[:] = list(slots)
     return y
+
+
+def conv_backward(x, w, dy, dW, gin=None, dbias=None, x_off=0, dy_off=0, gin_off=0, stride=1, dil=1, route=0):
+    """The train plan's backward of one conv (csrc/plan.cu conv_backward_views) on channel slices of NHWC CUDA buffers.
+    x: (B,H,W,ctot) fp16 / fp32 buffer whose channels [x_off, x_off + ci16) are the input (ci16: ci rounded up to 16, zero padding);
+    dy: (B,Ho,Wo,ctot) buffer holding dL/dy at [dy_off, dy_off + co) in fp16, or at [dy_off, dy_off + co16) in fp32 (zero padding);
+    gin: None or x's twin buffer, grad(in) += at [gin_off, gin_off + ci16); w: (co,ci,k,k) fp32 master weights; dW (same shape) and
+    dbias (co,) fp32 are accumulated into.  route: 0 as the plan, or _lib.CONV_BWD_* bits.  Returns the 16 info slots of
+    myolo_conv_backward (include/myolo.h): the routes taken and their tiling."""
+    B, H, W, _ = x.shape
+    co, ci, k, _ = w.shape
+    for t in (x, dy, gin):
+        assert t is None or (t.is_cuda and t.is_contiguous() and t.dtype in (torch.float16, torch.float32))
+    pad = dil * (k // 2)
+    Ho, Wo = (H + 2 * pad - dil * (k - 1) - 1) // stride + 1, (W + 2 * pad - dil * (k - 1) - 1) // stride + 1
+    assert dy.shape[:3] == (B, Ho, Wo), (dy.shape, (B, Ho, Wo))
+    assert gin is None or (gin.shape == x.shape and gin.dtype == x.dtype)
+    assert w.dtype == dW.dtype == torch.float32 and w.is_contiguous() and dW.is_contiguous() and dW.shape == w.shape
+    assert dbias is None or (dbias.dtype == torch.float32 and dbias.shape == (co,))
+    slots = (ctypes.c_int32 * 16)()
+    _lib.check(_lib.lib().myolo_conv_backward(_lib.ptr(x), _lib.torch_dtype_code(x.dtype), B, H, W, x.shape[3], x_off, _lib.ptr(dy),
+                                              _lib.torch_dtype_code(dy.dtype), dy.shape[3], dy_off, _lib.ptr(gin), x.shape[3], gin_off,
+                                              _lib.ptr(w), co, ci, k, stride, dil, _lib.ptr(dW), _lib.ptr(dbias), int(route), slots,
+                                              _lib.stream_ptr()))
+    return list(slots)

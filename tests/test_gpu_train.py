@@ -243,7 +243,9 @@ WGRAD_SHAPES = [  # B, H, W, ci, co, k, stride, dil
 @pytest.mark.parametrize("shape", WGRAD_SHAPES, ids=[f"w{i}" for i in range(len(WGRAD_SHAPES))])
 def test_conv_wgrad_kernels_match_torch(shape, path):
     """per-op: dW of one conv from fp16 NHWC x / dy, both kernels (0: mma.sync, 1: wgmma MN-major) against torch's conv weight
-    gradient in fp64 on the same fp16-rounded inputs; tolerance 2e-3 relative Frobenius (fp32 accumulation order only)."""
+    gradient in fp64 on the same fp16-rounded inputs; relative Frobenius error within the kernel's limit in test_gpu_conv_backward.py
+    (fp32 accumulation order only)."""
+    from tests.test_gpu_conv_backward import LIMIT_WGRAD
     from multiyolov5_b200 import _lib
     B, H, W, ci, co, k, stride, dil = shape
     g = torch.Generator().manual_seed(sum(shape))
@@ -261,7 +263,8 @@ def test_conv_wgrad_kernels_match_torch(shape, path):
     _lib.check(_lib.lib().myolo_conv_wgrad(_lib.ptr(xd), _lib.ptr(dyd), B, H, W, ci, co, k, stride, dil, _lib.ptr(dW), path, _lib.stream_ptr()))
     torch.cuda.synchronize()
     err = rel_f((dW - 1.0).cpu(), w.grad)
-    assert err < 2e-3, err
+    limit = LIMIT_WGRAD["mma.sync"][0] if path == 0 else max(LIMIT_WGRAD["wgmma direct"][0], LIMIT_WGRAD["wgmma packed"][0])
+    assert err < limit, err
 
 
 def test_graphed_det_loss_equals_eager_path_and_runs_for_unfused_hyps():
