@@ -530,7 +530,22 @@ int myolo_seg_upsample_argmax(const void* logits, int dtype, int B, int C, int h
 int myolo_bilinear_nchw(const float* src, int B, int C, int h, int w, int H, int W, float* dst, void* stream);
 
 /* ---- standalone kernels for per-op parity tests and ncu captures ---- */
-/* SiLU(conv(x)*bnscale+bnshift) on NHWC fp16: x (B,H,W,Ci) -> y (B,Ho,Wo,Co); w fp32 [Co][Ci][k][k]; path: 0 auto, 1 wgmma, 2 simt, 3 wgmma (same kernel as 1) */
+/* standalone forward of one conv through the plan's own routing and launches: y = act(conv(x, W) + b) (+ residual), W and b the fp16 pack
+ * and fp32 bias of fp32 master weights w [co][ci][k][k] with BatchNorm (gamma, beta, mean, var, eps; all four or none) folded in and the
+ * conv bias (nullable) added, as myolo_plan_set_conv_weights packs them.  Views are channel slices of NHWC buffers (base of the buffer,
+ * channels per pixel ctot, first channel c_off), as the plan passes them:
+ *   x    (B,H,W) fp16 / fp32, ci rounded up to 16 channels (the padding channels hold zeros);
+ *   y    (B,Ho,Wo) fp16 / fp32, co channels: exactly those are written;
+ *   res  nullable, (B,Ho,Wo) fp16, co channels, added after the activation; it may alias y.
+ * "same" padding dil*(k/2).  path: 0 as the plan, 1 wgmma (error when the op is not eligible), 2 CUDA-core, 3 wgmma with streamed weights
+ * and one A box per tap (the layout path 1's weight residency and strip are checked against).  info (nullable): the 12 slots of
+ * myolo_plan_conv_info. */
+int myolo_conv_forward(const void* x, int x_dtype, int B, int H, int W, int x_ctot, int x_coff, void* y, int y_dtype, int y_ctot, int y_coff,
+                       const void* res, int res_ctot, int res_coff, const float* w, int co, int ci, int k, int stride, int dil,
+                       const float* gamma, const float* beta, const float* mean, const float* var, float eps, const float* bias, int act,
+                       int path, int32_t* info, void* stream);
+/* SiLU(conv(x)*bnscale+bnshift) on NHWC fp16: x (B,H,W,Ci) -> y (B,Ho,Wo,Co); w fp32 [Co][Ci][k][k]; path: 0 auto, 1 wgmma, 2 simt, 3 wgmma (same kernel as 1).
+ * myolo_conv_forward on whole buffers (Ci % 16 == 0) */
 int myolo_conv_bn_silu(const void* x_nhwc_f16, int B, int H, int W, int ci, const float* w, int co, int k, int stride,
                        int dil, const float* gamma, const float* beta, const float* mean, const float* var, float eps,
                        const float* bias, int act, const void* residual_nhwc_f16, void* y_nhwc_f16, int path, void* stream);

@@ -42,7 +42,7 @@ EXPORTS = [
     "myolo_anchor_metric", "myolo_anchor_metric_workspace_bytes", "myolo_anchor_evolve", "myolo_anchor_evolve_workspace_bytes",
     "myolo_kmeans", "myolo_kmeans_workspace_bytes", "myolo_class_weights", "myolo_image_weights", "myolo_weighted_draw",
     "myolo_plan_backward_seg_loss", "myolo_seg_focal_loss", "myolo_seg_focal_loss_backward", "myolo_seg_focal_loss_workspace_bytes",
-    "myolo_conv_backward",
+    "myolo_conv_backward", "myolo_conv_forward",
 ]
 REDUCTION_MEAN, REDUCTION_SUM = 0, 1        # include/myolo.h: MYOLO_REDUCTION_* of myolo_seg_focal_loss
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
@@ -198,6 +198,8 @@ def lib():
                                            vp]
     L.myolo_conv_bn_silu_info.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, i32,
                                           C.POINTER(C.c_int32), vp]
+    L.myolo_conv_forward.argtypes = [vp, i32, i32, i32, i32, i32, i32, vp, i32, i32, i32, vp, i32, i32, vp, i32, i32, i32, i32, i32, vp, vp, vp,
+                                     vp, f32, vp, i32, i32, C.POINTER(C.c_int32), vp]
     for name in EXPORTS:
         getattr(L, name)  # AttributeError here == header / library mismatch
     if L.myolo_abi_version() != 1:

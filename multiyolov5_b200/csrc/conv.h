@@ -41,8 +41,8 @@ struct ConvTcParams {
   int strip_w;           // tw + 2 dil: pixels per strip row
   int strip_box_bytes, strip_sub_bytes;   // bytes of one strip box / its 1024-aligned slot in the stage
   int dil;
-  int out_mode;          // 0: fp16 NHWC slice, 1: fp32 NHWC
-  int out_c, out_ctot;   // channels of the output slice / channel pitch of its buffer
+  int out_mode;          // 0: fp16 NHWC slice, 1: fp32 NHWC slice
+  int out_c, out_ctot;   // channels of the output slice (fp32: min(out_c, Co) are stored) / channel pitch of its buffer
   const float* bias;
   const __half* residual;  // nullable; base of the residual slice (image 0, pixel 0, channel 0 of the slice)
   int res_ctot;

@@ -185,13 +185,16 @@ __device__ __forceinline__ void epilogue(const ConvTcParams& p, const float (&ac
           *reinterpret_cast<uint4*>(p.out_f16 + pix * p.out_ctot + n) = make_uint4(w[0], w[1], w[2], w[3]);
       }
     } else if (in_map) {
+      const int n_end = min(p.out_c, p.Co);   // the conv's channels inside the slice: never its neighbours or a buffer's padding
 #pragma unroll
       for (int j = 0; j < BN / 8; ++j) {
         const int c = 8 * j + 2 * q;
         const int n = tc.n0 + c;
         const float v0 = act_out(acc[4 * j + 2 * h] + bias_s[n], p.act, c);
         const float v1 = act_out(acc[4 * j + 2 * h + 1] + bias_s[n + 1], p.act, c + 1);
-        if (n < p.out_ctot) *reinterpret_cast<float2*>(p.out_f32 + pix * p.out_ctot + n) = make_float2(v0, v1);
+        float* dst = p.out_f32 + pix * p.out_ctot + n;
+        if (n + 1 < n_end) *reinterpret_cast<float2*>(dst) = make_float2(v0, v1);
+        else if (n < n_end) *dst = v0;
       }
     }
   }
@@ -465,7 +468,8 @@ bool conv_tc_eligible(const ConvOp& op) {
     if (op.out.C % 8 != 0 || op.out.ctot % 8 != 0 || !aligned16(op.out.base)) return false;
     if (op.has_res && (op.res.dtype != MYOLO_F16 || op.res.ctot % 8 != 0 || op.Co % 16 != 0 || !aligned16(op.res.base))) return false;
   } else {
-    if (op.has_res || op.out.ctot % 4 != 0) return false;
+    // the epilogue stores two channels as one 8-byte vector (an odd last channel alone): the slice must start on an 8-byte boundary
+    if (op.has_res || op.out.ctot % 4 != 0 || reinterpret_cast<uintptr_t>(op.out.base) % 8 != 0) return false;
   }
   // tiny maps run on the generic kernel (TMA boxes larger than the tensor are avoided on purpose)
   if (op.out.W < 8 || op.out.H < 2 || op.out.W * op.out.H < 128) return false;

@@ -416,6 +416,38 @@ extern "C" int myolo_plan_set_extra(myolo_plan* pl, int offset, const void* src,
   return 0;
 }
 
+// forward of one conv on resolved views (the plan's prepare_conv and myolo_conv_forward): the checks, the route (wgmma unless force_simt
+// or conv_tc_eligible refuses) and, on the wgmma path, the tiling and tensor maps.  res: nullable.  An fp16 output view has the weights'
+// co channels; an fp32 one at least co (the plan's fp32 head buffers carry co rounded up to 16), of which the conv writes the first co.
+static int conv_forward_views(ConvOp& c, const TensorView& in, const TensorView& out, const TensorView* res, const WeightSlot& s, int k,
+                              int stride, int dil, int act, bool force_simt, int num_sms) {
+  c = ConvOp();
+  c.in = in;
+  c.out = out;
+  c.has_res = res != nullptr;
+  if (res) c.res = *res;
+  c.k = k;
+  c.stride = stride;
+  c.dil = dil;
+  c.act = act;
+  c.w = s.w;
+  c.bias = s.bias;
+  c.Ci_pad = s.ci_pad;
+  c.Co_pad = s.co_pad;
+  c.Co = s.co;
+  MYOLO_REQUIRE(s.k == k, "conv: kernel size %d != packed weights %d", k, s.k);
+  MYOLO_REQUIRE(c.in.C == s.ci_pad, "conv: input view has %d channels, packed weights expect %d", c.in.C, s.ci_pad);
+  MYOLO_REQUIRE(c.out.dtype == MYOLO_F32 ? c.out.C >= s.co : c.out.C == s.co, "conv: output view has %d channels, weights produce %d",
+                c.out.C, s.co);
+  MYOLO_REQUIRE(!res || (res->dtype == MYOLO_F16 && res->C >= s.co), "conv: the residual must be fp16 with %d channels", s.co);
+  const int pad = dil * (k / 2);
+  const int ho = (c.in.H + 2 * pad - dil * (k - 1) - 1) / stride + 1;
+  const int wo = (c.in.W + 2 * pad - dil * (k - 1) - 1) / stride + 1;
+  MYOLO_REQUIRE(ho == c.out.H && wo == c.out.W, "conv: output %dx%d does not match the view's %dx%d", ho, wo, c.out.H, c.out.W);
+  c.use_tc = !force_simt && conv_tc_eligible(c);
+  return c.use_tc ? conv_tc_prepare(c, num_sms) : 0;
+}
+
 static int prepare_conv(myolo_plan* pl, int i) {
   const myolo_op& op = pl->ops[i];
   MYOLO_REQUIRE(op.weight_slot >= 0 && op.weight_slot < (int)pl->slots.size(), "op %d: bad weight slot", i);
@@ -424,31 +456,18 @@ static int prepare_conv(myolo_plan* pl, int i) {
     set_error("op %d: weights of slot %d were never set (call myolo_plan_set_conv_weights first)", i, op.weight_slot);
     return MYOLO_E_STATE;
   }
-  ConvOp& c = pl->convs[i];
-  c = ConvOp();
+  TensorView in, out, res;
   int rc;
-  if ((rc = resolve_view(pl, op.in, &c.in))) return rc;
-  if ((rc = resolve_view(pl, op.out, &c.out))) return rc;
-  c.has_res = op.in2.buf >= 0;
-  if (c.has_res && (rc = resolve_view(pl, op.in2, &c.res))) return rc;
-  c.k = op.k;
-  c.stride = op.stride;
-  c.dil = op.dil;
-  c.act = op.act;
-  c.w = s.w;
-  c.bias = s.bias;
-  c.Ci_pad = s.ci_pad;
-  c.Co_pad = s.co_pad;
-  c.Co = s.co;
-  MYOLO_REQUIRE(s.k == op.k, "op %d: kernel size %d != packed weights %d", i, op.k, s.k);
-  MYOLO_REQUIRE(c.in.C == s.ci_pad, "op %d: input view has %d channels, packed weights expect %d", i, c.in.C, s.ci_pad);
-  MYOLO_REQUIRE(c.out.dtype == MYOLO_F32 || c.out.C == s.co, "op %d: output view has %d channels, weights produce %d", i, c.out.C, s.co);
-  const int pad = op.dil * (op.k / 2);
-  const int ho = (c.in.H + 2 * pad - op.dil * (op.k - 1) - 1) / op.stride + 1;
-  const int wo = (c.in.W + 2 * pad - op.dil * (op.k - 1) - 1) / op.stride + 1;
-  MYOLO_REQUIRE(ho == c.out.H && wo == c.out.W, "op %d: conv output %dx%d does not match buffer %dx%d", i, ho, wo, c.out.H, c.out.W);
-  c.use_tc = !pl->force_simt && conv_tc_eligible(c);
-  if (c.use_tc && (rc = conv_tc_prepare(c, pl->num_sms))) return rc;
+  if ((rc = resolve_view(pl, op.in, &in))) return rc;
+  if ((rc = resolve_view(pl, op.out, &out))) return rc;
+  const bool has_res = op.in2.buf >= 0;
+  if (has_res && (rc = resolve_view(pl, op.in2, &res))) return rc;
+  if ((rc = conv_forward_views(pl->convs[i], in, out, has_res ? &res : nullptr, s, op.k, op.stride, op.dil, op.act, pl->force_simt,
+                               pl->num_sms))) {
+    const std::string msg = g_err;
+    set_error("op %d: %s", i, msg.c_str());
+    return rc;
+  }
   pl->conv_ready[i] = 1;
   return 0;
 }
@@ -1762,61 +1781,69 @@ extern "C" int myolo_allreduce_grads(float* flat_grad, int64_t n, void* nccl_com
 // ------------------------------------------------------------------------------------------------
 // standalone fused conv (per-op parity tests, ncu captures)
 // ------------------------------------------------------------------------------------------------
+extern "C" int myolo_conv_forward(const void* x, int x_dtype, int B, int H, int W, int x_ctot, int x_coff, void* y, int y_dtype, int y_ctot,
+                                  int y_coff, const void* res, int res_ctot, int res_coff, const float* w, int co, int ci, int k, int stride,
+                                  int dil, const float* gamma, const float* beta, const float* mean, const float* var, float eps,
+                                  const float* bias, int act, int path, int32_t* info, void* stream) {
+  NvtxRange nvtx_("myolo_conv_forward");
+  MYOLO_REQUIRE(x && y && w && B > 0 && H > 0 && W > 0 && co > 0 && ci > 0 && k >= 1 && k % 2 == 1 && (stride == 1 || stride == 2) &&
+                dil >= 1 && path >= 0 && path <= 3, "conv_forward: bad arguments");
+  MYOLO_REQUIRE((gamma && beta && mean && var) || (!gamma && !beta && !mean && !var), "conv_forward: partial BN parameters");
+  MYOLO_REQUIRE((x_dtype == MYOLO_F16 || x_dtype == MYOLO_F32) && (y_dtype == MYOLO_F16 || y_dtype == MYOLO_F32),
+                "conv_forward: x and y must be MYOLO_F16 or MYOLO_F32");
+  // the plan's views: x carries ci rounded up to 16 channels (the padding channels hold zeros), y and the residual co
+  const int xc = (int)align_up(ci, 16);
+  MYOLO_REQUIRE(x_coff >= 0 && x_coff + xc <= x_ctot && y_coff >= 0 && y_coff + co <= y_ctot &&
+                (!res || (res_coff >= 0 && res_coff + co <= res_ctot)), "conv_forward: channel slice outside its buffer");
+  int sms = 0;
+  int rc = check_device(&sms);
+  if (rc) return rc;
+  const int pad = dil * (k / 2);
+  const int Ho = (H + 2 * pad - dil * (k - 1) - 1) / stride + 1, Wo = (W + 2 * pad - dil * (k - 1) - 1) / stride + 1;
+  MYOLO_REQUIRE(Ho > 0 && Wo > 0, "conv_forward: empty output map");
+  const size_t xes = x_dtype == MYOLO_F16 ? 2 : 4, yes = y_dtype == MYOLO_F16 ? 2 : 4;
+  const TensorView xv{const_cast<unsigned char*>(static_cast<const unsigned char*>(x)) + (size_t)x_coff * xes, B, H, W, xc, x_ctot, x_dtype};
+  const TensorView yv{static_cast<unsigned char*>(y) + (size_t)y_coff * yes, B, Ho, Wo, co, y_ctot, y_dtype};
+  const TensorView rv{const_cast<unsigned char*>(static_cast<const unsigned char*>(res)) + (size_t)res_coff * 2, B, Ho, Wo, co, res_ctot,
+                      MYOLO_F16};
+  cudaStream_t s = (cudaStream_t)stream;
+  WeightSlot sl;
+  sl.co = co;
+  sl.ci = ci;
+  sl.k = k;
+  sl.co_pad = conv_n_pad(co);
+  sl.ci_pad = xc;
+  MYOLO_CHECK_CUDA(cudaMalloc(&sl.w, (size_t)sl.co_pad * k * k * sl.ci_pad * 2));
+  MYOLO_CHECK_CUDA(cudaMalloc(&sl.bias, (size_t)sl.co_pad * 4));
+  rc = pack_conv_weights(w, co, ci, k, gamma, beta, mean, var, eps, bias, sl.w, sl.bias, sl.co_pad, sl.ci_pad, s);
+  ConvOp c;
+  if (!rc) rc = conv_forward_views(c, xv, yv, res ? &rv : nullptr, sl, k, stride, dil, act, path == 2, sms);
+  if (!rc && (path == 1 || path == 3) && !c.use_tc) {
+    set_error("conv_forward: shape not eligible for the tensor-core path");
+    rc = MYOLO_E_INVALID;
+  }
+  if (!rc && path == 3) {      // streamed weights, one A box per tap: the layout the reuse paths are checked against
+    c.reuse = false;
+    rc = conv_tc_prepare(c, sms);
+  }
+  if (!rc) rc = c.use_tc ? conv_tc_launch(c, s) : conv_simt_launch(c, s);
+  if (!rc && info) conv_info_slots(c, info);
+  const cudaError_t e = cudaStreamSynchronize(s);
+  cudaFree(sl.w);
+  cudaFree(sl.bias);
+  if (!rc && e != cudaSuccess) {
+    set_error("conv_forward: kernel failed: %s", cudaGetErrorString(e));
+    rc = MYOLO_E_CUDA;
+  }
+  return rc;
+}
+
 extern "C" int myolo_conv_bn_silu_info(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,
                                        const float* gamma, const float* beta, const float* mean, const float* var, float eps,
                                        const float* bias, int act, const void* residual, void* y, int y_ctot, int path, int32_t* info,
                                        void* stream) {
-  MYOLO_REQUIRE(x && w && y && B > 0 && H > 0 && W > 0 && ci > 0 && co > 0 && y_ctot >= co, "conv_bn_silu: bad arguments");
-  MYOLO_REQUIRE(ci % 16 == 0 && co % 8 == 0, "conv_bn_silu: standalone entry needs ci %% 16 == 0 and co %% 8 == 0");
-  int sms = 0;
-  int rc = check_device(&sms);
-  if (rc) return rc;
-  cudaStream_t s = (cudaStream_t)stream;
-  const int co_pad = conv_n_pad(co), ci_pad = ci;
-  __half* wp = nullptr;
-  float* bp = nullptr;
-  MYOLO_CHECK_CUDA(cudaMalloc(&wp, (size_t)co_pad * k * k * ci_pad * 2));
-  MYOLO_CHECK_CUDA(cudaMalloc(&bp, (size_t)co_pad * 4));
-  rc = pack_conv_weights(w, co, ci, k, gamma, beta, mean, var, eps, bias, wp, bp, co_pad, ci_pad, s);
-  ConvOp c;
-  const int pad = dil * (k / 2);
-  const int ho = (H + 2 * pad - dil * (k - 1) - 1) / stride + 1, wo = (W + 2 * pad - dil * (k - 1) - 1) / stride + 1;
-  c.in = TensorView{const_cast<void*>(x), B, H, W, ci, ci, MYOLO_F16};
-  c.out = TensorView{y, B, ho, wo, co, y_ctot, MYOLO_F16};
-  c.has_res = residual != nullptr;
-  if (c.has_res) c.res = TensorView{const_cast<void*>(residual), B, ho, wo, co, co, MYOLO_F16};
-  c.k = k;
-  c.stride = stride;
-  c.dil = dil;
-  c.act = act;
-  c.w = wp;
-  c.bias = bp;
-  c.Ci_pad = ci_pad;
-  c.Co_pad = co_pad;
-  c.Co = co;
-  if (!rc) {
-    const bool elig = conv_tc_eligible(c);
-    if ((path == 1 || path == 3) && !elig) {
-      set_error("conv_bn_silu: shape not eligible for the tensor-core path");
-      rc = MYOLO_E_INVALID;
-    } else if (path == 2 || (path == 0 && !elig)) {
-      rc = conv_simt_launch(c, s);
-    } else {
-      c.reuse = path != 3;     // path 3: streamed weights, the layout the reuse paths are checked against
-      c.use_tc = true;
-      rc = conv_tc_prepare(c, sms);
-      if (!rc) rc = conv_tc_launch(c, s);
-    }
-    if (!rc && info) conv_info_slots(c, info);
-  }
-  cudaError_t e = cudaStreamSynchronize(s);
-  cudaFree(wp);
-  cudaFree(bp);
-  if (!rc && e != cudaSuccess) {
-    set_error("conv_bn_silu: kernel failed: %s", cudaGetErrorString(e));
-    rc = MYOLO_E_CUDA;
-  }
-  return rc;
+  return myolo_conv_forward(x, MYOLO_F16, B, H, W, ci, 0, y, MYOLO_F16, y_ctot, 0, residual, co, 0, w, co, ci, k, stride, dil, gamma, beta,
+                            mean, var, eps, bias, act, path, info, stream);
 }
 
 extern "C" int myolo_conv_bn_silu_slice(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,

@@ -32,13 +32,41 @@ def conv_bn_silu(x_nhwc: torch.Tensor, w: torch.Tensor, bn=None, bias=None, stri
     bias = bias.float().contiguous() if bias is not None else None
     if residual is not None:
         assert residual.shape == y.shape and residual.dtype == torch.float16 and residual.is_contiguous()
-    slots = (ctypes.c_int32 * 12)()
-    _lib.check(_lib.lib().myolo_conv_bn_silu_info(_lib.ptr(x_nhwc), B, H, W, Ci, _lib.ptr(w), Co, k, stride, dil, _lib.ptr(g),
-                                                  _lib.ptr(b), _lib.ptr(m), _lib.ptr(v), float(eps), _lib.ptr(bias), int(act),
-                                                  _lib.ptr(residual), _lib.ptr(y), y.stride(2), int(path), slots, _lib.stream_ptr()))
+    slots = _conv_forward(x_nhwc, Ci, 0, y, y.stride(2), 0, residual, Co, 0, w, g, b, m, v, eps, bias, stride, dil, act, path)
     if info is not None:
-        info[:] = list(slots)
+        info[:] = slots
     return y
+
+
+def _conv_forward(x, x_ctot, x_off, y, y_ctot, y_off, res, res_ctot, res_off, w, g, b, m, v, eps, bias, stride, dil, act, path):
+    Co, Ci, k, _ = w.shape
+    B, H, W = x.shape[:3]
+    slots = (ctypes.c_int32 * 12)()
+    _lib.check(_lib.lib().myolo_conv_forward(_lib.ptr(x), _lib.torch_dtype_code(x.dtype), B, H, W, x_ctot, x_off, _lib.ptr(y),
+                                             _lib.torch_dtype_code(y.dtype), y_ctot, y_off, _lib.ptr(res), res_ctot, res_off, _lib.ptr(w), Co,
+                                             Ci, k, stride, dil, _lib.ptr(g), _lib.ptr(b), _lib.ptr(m), _lib.ptr(v), float(eps), _lib.ptr(bias),
+                                             int(act), int(path), slots, _lib.stream_ptr()))
+    return list(slots)
+
+
+def conv_forward(x, w, y, bn=None, bias=None, residual=None, x_off=0, y_off=0, res_off=0, stride=1, dil=1, act=_lib.ACT_SILU, path=0,
+                 eps=1e-3):
+    """The plan's forward of one conv (csrc/plan.cu conv_forward_views) on channel slices of NHWC CUDA buffers.
+    x: (B,H,W,ctot) fp16 / fp32 buffer whose channels [x_off, x_off + ci16) are the input (ci16: ci rounded up to 16, zero padding);
+    y: (B,Ho,Wo,ctot) fp16 / fp32 buffer, y[..., y_off:y_off + co] = act(conv + bias) (+ residual[..., res_off:res_off + co]); residual:
+    None or an fp16 (B,Ho,Wo,ctot) buffer, y itself allowed.  w: (co,ci,k,k) fp32 masters; bn: (gamma,beta,mean,var) fp32 folded in with
+    eps, or None; bias: (co,) fp32 or None.  path: 0 as the plan, 1 wgmma, 2 CUDA-core, 3 wgmma with streamed weights.  Returns the 12 info
+    slots of myolo_plan_conv_info: the route taken and its tiling."""
+    for t in (x, y, residual):
+        assert t is None or (t.is_cuda and t.is_contiguous() and t.dim() == 4 and t.dtype in (torch.float16, torch.float32))
+    assert residual is None or (residual.dtype == torch.float16 and residual.shape[:3] == y.shape[:3])
+    w = w.float().contiguous()
+    g = b = m = v = None
+    if bn is not None:
+        g, b, m, v = [t.float().contiguous() for t in bn]
+    bias = bias.float().contiguous() if bias is not None else None
+    return _conv_forward(x, x.shape[3], x_off, y, y.shape[3], y_off, residual, residual.shape[3] if residual is not None else 0, res_off, w,
+                         g, b, m, v, eps, bias, stride, dil, act, path)
 
 
 def conv_backward(x, w, dy, dW, gin=None, dbias=None, x_off=0, dy_off=0, gin_off=0, stride=1, dil=1, route=0):

@@ -1,10 +1,11 @@
-"""GPU: the fused Conv+BN+SiLU(+residual) kernels (wgmma path and CUDA-core path) against a torch fp32 restatement of
-Conv.fuseforward (reference models/common.py:45-46, BN fold utils/torch_utils.py:182-202) on identical fp16-rounded inputs.
-Tolerance: |err| <= 2e-3 * max|ref| + fp16 output rounding (the kernels accumulate in fp32; only the sum order differs)."""
-import numpy as np
+"""GPU: the fused Conv+BN+SiLU(+residual) kernels (wgmma path and CUDA-core path) against Conv.fuseforward (reference
+models/common.py:45-46, BN fold utils/torch_utils.py:182-202) in fp64 on the values the kernels read: the fp16 input, the pack's fp16
+folded weights and fp32 bias (test_gpu_conv_forward.pack_ref), an exact SiLU and the residual before the one rounding of the output.
+Error and limit as in test_gpu_conv_forward.py: (|err| - fp16 rounding of the stored value) / max|ref|."""
 import pytest
 import torch
-import torch.nn.functional as F
+
+from tests.test_gpu_conv_forward import LIMIT, SILU, U16, conv64, pack_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -49,17 +50,12 @@ SHAPES = [
 ]
 
 
-def torch_ref(x_nhwc, w, bn, stride, dil, residual, eps=1e-3):
-    x = x_nhwc.float().permute(0, 3, 1, 2).cpu()
-    g, b, m, v = [t.cpu() for t in bn]
-    scale = g / torch.sqrt(v + eps)
-    wf = (w.cpu() * scale.view(-1, 1, 1, 1)).half().float()      # the pack kernel rounds folded weights to fp16
-    k = w.shape[2]
-    y = F.conv2d(x, wf, None, stride, dil * (k // 2), dil) + (b - m * scale).view(1, -1, 1, 1)
-    y = y * torch.sigmoid(y)
+def reference(x_nhwc, w, bn, stride, dil, residual, eps=1e-3):
+    wp, bp = pack_ref(w, bn, None, eps)
+    y = conv64(x_nhwc.permute(0, 3, 1, 2).double(), wp, bp, w.shape[2], stride, dil, SILU)
     if residual is not None:
-        y = y + residual.float().permute(0, 3, 1, 2).cpu()
-    return y.permute(0, 2, 3, 1).contiguous()
+        y = y + residual.permute(0, 3, 1, 2).double()
+    return y.permute(0, 2, 3, 1)
 
 
 # path 2: CUDA-core kernel, 1: wgmma kernel with the planner's tiling rules, 3: the same wgmma kernel through the standalone path-3 entry
@@ -83,7 +79,6 @@ def test_conv_bn_silu(shape, path):
     r = torch.randn(B, Ho, Wo, Co, generator=gsd).half().cuda() if res else None
     y = ops.conv_bn_silu(x, w, bn, stride=s, dil=d, residual=r, path=path)
     torch.cuda.synchronize()
-    ref = torch_ref(x, w, bn, s, d, r)
-    err = (y.float().cpu() - ref).abs().max().item()
-    tol = 2e-3 * ref.abs().max().item() + 1e-3
-    assert err <= tol, f"path={path} shape={shape}: max err {err:.4g} > {tol:.4g}"
+    ref = reference(x, w, bn, s, d, r)
+    err = float(((y.double() - ref).abs() - U16 * ref.abs()).clamp_min(0).max()) / float(ref.abs().max())
+    assert err <= LIMIT["fp16"], f"path={path} shape={shape}: error {err:.3g} over the limit {LIMIT['fp16']:.0e}"
