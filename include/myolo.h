@@ -279,7 +279,9 @@ int myolo_ema_update(const myolo_ema_chunk* chunks /* device */, int n_chunks, d
  * p[l] / dp[l]: the nl raw head outputs (B, na, ny[l], nx[l], no) fp32 and their gradients (overwritten); targets (nt, 6) [image, class,
  * x, y, w, h] normalised, all-zero rows never match; anchors_grid: nl*na*2 floats in grid units (host); balance: nl floats (host).
  * d loss / d p = mult * (*scale_dev) * d[bs-free ComputeLoss value]/dp with mult = batch * world * detgain chosen by the caller; items_out (device
- * float[4]) = lbox, lobj, lcls, their sum (detached, as the reference's loss_items).  fl_gamma = 0, cls_pw = obj_pw = 1 only. */
+ * float[4]) = lbox, lobj, lcls, their sum (detached, as the reference's loss_items).  fl_gamma = 0, cls_pw = obj_pw = 1 only; 1 <= nl <= 3,
+ * 1 <= na <= MYOLO_DET_LOSS_NA_MAX (the range of --evolve's `anchors` hyp). */
+#define MYOLO_DET_LOSS_NA_MAX 10
 int64_t myolo_det_loss_workspace_bytes(int B, int na, int nl, const int32_t* ny, const int32_t* nx);
 int myolo_det_loss(const float* const* p, float* const* dp, const float* targets, int nt, int B, int na, int no, int nl, const int32_t* ny,
                    const int32_t* nx, const float* anchors_grid, const float* balance, float hyp_box, float hyp_obj, float hyp_cls,

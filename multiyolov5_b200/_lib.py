@@ -49,6 +49,7 @@ DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include
 KMEANS_MAX_ITER, KMEANS_BAD_INDEX = 1, 2                                 # include/myolo.h: bits of myolo_kmeans' status word
 IW_BAD_CLASS, IW_TOTAL_NONPOS, IW_TOTAL_NONFINITE = 1, 2, 4              # include/myolo.h: bits of the image-weights status word
 IW_NC_MAX = 1024                                                         # include/myolo.h MYOLO_IW_NC_MAX
+DET_LOSS_NA_MAX = 10                                                     # include/myolo.h MYOLO_DET_LOSS_NA_MAX
 CONV_BWD_SIMT, CONV_BWD_NO_WGRAD_TC = 1, 2                               # include/myolo.h: route bits of myolo_conv_backward
 
 

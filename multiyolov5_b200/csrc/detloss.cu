@@ -25,7 +25,7 @@ struct DetLossParams {
   const float* p[3];
   float* dp[3];
   int ny[3], nx[3];
-  float anchors[3][6];      // [level][a*2 + {w,h}] in grid units
+  float anchors[3][2 * MYOLO_DET_LOSS_NA_MAX];   // [level][a*2 + {w,h}] in grid units (kernel parameter: 240 bytes at na = 10)
   float balance[3];
   int nl, B, na, no, nc, nt;
   const float* targets;     // (nt, 6): image, class, x, y, w, h (normalised)
@@ -225,7 +225,7 @@ extern "C" int myolo_det_loss(const float* const* p, float* const* dp, const flo
                               const int32_t* ny, const int32_t* nx, const float* anchors_grid, const float* balance, float hyp_box,
                               float hyp_obj, float hyp_cls, float anchor_t, float gr, float cp, float cn, float mult, const float* scale_dev,
                               float* items_out, void* workspace, int64_t workspace_bytes, void* stream) {
-  MYOLO_REQUIRE(p && dp && items_out && workspace && nl >= 1 && nl <= 3 && na >= 1 && na <= 3 && no >= 6 && B > 0 && nt >= 0,
+  MYOLO_REQUIRE(p && dp && items_out && workspace && nl >= 1 && nl <= 3 && na >= 1 && na <= MYOLO_DET_LOSS_NA_MAX && no >= 6 && B > 0 && nt >= 0,
                 "det_loss: bad arguments");
   MYOLO_REQUIRE(nt == 0 || targets, "det_loss: targets missing");
   MYOLO_REQUIRE(workspace_bytes >= myolo_det_loss_workspace_bytes(B, na, nl, ny, nx), "det_loss: workspace too small");

@@ -117,6 +117,8 @@ def parse_model(d, ch):
             c2 = sum(ch[x] for x in f)
         elif m is Detect:
             args.append([ch[x] for x in f])
+            if isinstance(args[1], int):  # an anchor count: placeholder anchors that autoanchor replaces (reference models/yolo.py:405-406)
+                args[1] = [list(range(args[1] * 2))] * len(f)
         elif m in _SEG_HEADS:
             args[1] = max(round(args[1] * gd), 1) if args[1] > 1 else args[1]
             args[2] = make_divisible(args[2] * gw, 8)

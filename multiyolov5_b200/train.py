@@ -34,11 +34,15 @@ step then run one after the other.  At world size 1, or without torch.distribute
 LambdaLR, momentum, accumulation), the validation cadence, fitness2 and best.pt, results.txt, last.pt / best.pt and resume.
 `DetEpochBatches` / `SegEpochBatches` give each epoch's batches from the device loaders in the reference's order.
 
-Out of scope: loading and decoding data files, plotting, W&B / TensorBoard, --evolve's generations, --bucket, DDP buffer broadcast.
+`evolve(hyp, opt, train_fn)` is the reference's --evolve (train.py:637-717): generations of `train_fn` (a training run such as `fit`),
+each with hyper-parameters mutated from the best earlier results in evolve.txt.
+
+Out of scope: loading and decoding data files, plotting, W&B / TensorBoard, --bucket, DDP buffer broadcast.
 """
 import collections
 import math
 import random
+import time
 import ctypes as C
 
 import numpy as np
@@ -993,3 +997,75 @@ def _progress(epoch, epochs, mloss, msegloss, n_targets, imgshape):
     """the progress line of train.py:407-409 (reads the device means: a host synchronisation)"""
     mem = "%.3gG" % (torch.cuda.memory_reserved() / 1E9 if torch.cuda.is_available() else 0)
     return ("%10s" * 2 + "%10.4g" * 7) % ("%g/%g" % (epoch, epochs - 1), mem, *mloss.tolist(), *msegloss.tolist(), n_targets, imgshape)
+
+
+# --evolve's mutation metadata (reference train.py:640-667): key -> (mutation gain 0-1, lower limit, upper limit), in the reference's order
+EVOLVE_META = {"lr0": (1, 1e-5, 1e-1), "lrf": (1, 0.01, 1.0), "momentum": (0.3, 0.6, 0.98), "weight_decay": (1, 0.0, 0.001),
+               "warmup_epochs": (1, 0.0, 5.0), "warmup_momentum": (1, 0.0, 0.95), "warmup_bias_lr": (1, 0.0, 0.2), "box": (1, 0.02, 0.2),
+               "cls": (1, 0.2, 4.0), "cls_pw": (1, 0.5, 2.0), "obj": (1, 0.2, 4.0), "obj_pw": (1, 0.5, 2.0), "iou_t": (0, 0.1, 0.7),
+               "anchor_t": (1, 2.0, 8.0), "anchors": (2, 2.0, 10.0), "fl_gamma": (0, 0.0, 2.0), "hsv_h": (1, 0.0, 0.1),
+               "hsv_s": (1, 0.0, 0.9), "hsv_v": (1, 0.0, 0.9), "degrees": (1, 0.0, 45.0), "translate": (1, 0.0, 0.9), "scale": (1, 0.0, 0.9),
+               "shear": (1, 0.0, 10.0), "perspective": (0, 0.0, 0.001), "flipud": (1, 0.0, 1.0), "fliplr": (0, 0.0, 1.0),
+               "mosaic": (1, 0.0, 1.0), "mixup": (1, 0.0, 1.0)}
+
+
+def choice_py38(n, weights, rng=random):
+    """`random.choices(range(n), weights=weights)[0]` as Python 3.8 computes it, the version the reference ran on: one rng.random()
+    scaled by the weights' total and a bisection of their running sums up to n - 1.  A total of zero (one earlier result, or tied
+    fitness) gives n - 1, where Python 3.9+ raises ValueError; with a positive total both versions give the same index."""
+    import bisect
+    import itertools
+    cum = list(itertools.accumulate(weights))
+    if len(cum) != n:
+        raise ValueError("The number of weights does not match the population")
+    total = cum[-1] + 0.0
+    return bisect.bisect(cum, rng.random() * total, 0, n - 1)
+
+
+def evolve(hyp, opt, train_fn, generations=300, evolve_txt="evolve.txt"):
+    """The reference's hyper-parameter evolution (train.py:637-717) around `results = train_fn(hyp.copy(), opt)`, a training run that
+    returns the 7 results of `fit` (P, R, mAP@.5, mAP@.5:.95, val box, obj, cls loss).  `hyp` holds exactly the keys of EVOLVE_META, in its
+    order (the mutation indexes evolve.txt's columns by hyp's key order), `anchors` included; it is updated in place.
+
+    Per generation: when `evolve_txt` exists (a previous generation, or an earlier run to resume), the parent is drawn from its top
+    min(5, n) rows by utils.metrics.fitness with weights fitness - min through the global `random` (choice_py38), and mutated with
+    numpy.random seeded from int(time.time()) until a factor differs from 1; then every value is clipped to EVOLVE_META's limits and
+    rounded to 5 decimals, train_fn runs, and utils.general.print_mutation appends the result to `evolve_txt` and writes
+    save_dir/hyp_evolved.yaml.  Sets opt.notest = opt.nosave = True; DDP (opt.global_rank or opt.local_rank other than -1) is refused.
+    Returns the path of hyp_evolved.yaml.  Nothing of a generation stays referenced here once train_fn returns."""
+    from pathlib import Path
+    from .utils.general import print_mutation
+    from .utils.metrics import fitness
+    if "anchors" not in hyp:
+        raise KeyError("anchors", "--evolve mutates hyp['anchors']: enable the commented line '# anchors: 3' of the hyp file")
+    if list(hyp) != list(EVOLVE_META):
+        raise ValueError(f"--evolve needs the hyp keys {list(EVOLVE_META)} in this order, got {list(hyp)}")
+    if getattr(opt, "global_rank", -1) != -1 or getattr(opt, "local_rank", -1) != -1:
+        raise ValueError("DDP mode not implemented for --evolve")
+    opt.notest, opt.nosave = True, True
+    yaml_file = Path(opt.save_dir) / "hyp_evolved.yaml"
+    evolve_txt = Path(evolve_txt)
+    g = np.array([m[0] for m in EVOLVE_META.values()])              # gains 0-1
+    ng = len(EVOLVE_META)
+    for _ in range(generations):
+        if evolve_txt.exists():
+            x = np.loadtxt(evolve_txt, ndmin=2)
+            n = min(5, len(x))                                        # number of previous results to consider
+            x = x[np.argsort(-fitness(x))][:n]
+            w = fitness(x) - fitness(x).min()
+            x = x[choice_py38(n, w)]
+            mp, s = 0.8, 0.2                                          # mutation probability, sigma
+            npr = np.random
+            npr.seed(int(time.time()))
+            v = np.ones(ng)
+            while all(v == 1):                                        # mutate until a change occurs
+                v = (g * (npr.random(ng) < mp) * npr.randn(ng) * npr.random() * s + 1).clip(0.3, 3.0)
+            for i, k in enumerate(hyp.keys()):
+                hyp[k] = float(x[i + 7] * v[i])
+        for k, (_, lo, hi) in EVOLVE_META.items():
+            hyp[k] = round(min(max(hyp[k], lo), hi), 5)
+        results = train_fn(hyp.copy(), opt)
+        print_mutation(hyp.copy(), results, yaml_file, evolve_txt)
+    print(f"Hyperparameter evolution complete. Best results saved as: {yaml_file}\n"
+          f"Command to train a new model with these hyperparameters: $ python train.py --hyp {yaml_file}")
+    return yaml_file

@@ -159,6 +159,29 @@ def init_seeds(seed=0):
     torch.backends.cudnn.benchmark, torch.backends.cudnn.deterministic = (False, True) if seed == 0 else (True, False)
 
 
+def print_mutation(hyp, results, yaml_file="hyp_evolved.yaml", evolve_txt="evolve.txt"):
+    """--evolve's record of one generation (reference utils/general.py:528-556, without the gsutil bucket): prints the hyp and the 7
+    results, appends them to evolve_txt, rewrites it as its unique rows sorted by fitness ('%10.3g'), and writes the best row's
+    hyper-parameters to yaml_file under a header with the generation count and its results"""
+    import yaml
+    from .metrics import fitness
+    a = "%10s" * len(hyp) % tuple(hyp.keys())
+    b = "%10.3g" * len(hyp) % tuple(hyp.values())
+    c = "%10.4g" * len(results) % tuple(results)
+    print("\n%s\n%s\nEvolved fitness: %s\n" % (a, b, c))
+    with open(evolve_txt, "a") as f:
+        f.write(c + b + "\n")
+    x = np.unique(np.loadtxt(evolve_txt, ndmin=2), axis=0)
+    x = x[np.argsort(-fitness(x))]
+    np.savetxt(evolve_txt, x, "%10.3g")
+    for i, k in enumerate(hyp.keys()):
+        hyp[k] = float(x[0, i + 7])
+    with open(yaml_file, "w") as f:
+        best = tuple(x[0, :7])
+        f.write("# Hyperparameter Evolution Results\n# Generations: %g\n# Metrics: " % len(x) + "%10.4g" * len(best) % best + "\n\n")
+        yaml.dump(hyp, f, sort_keys=False)
+
+
 def one_cycle(y1=0.0, y2=1.0, steps=100):
     """the cosine ramp from y1 at x = 0 to y2 at x = steps of reference utils/general.py:186-188, its operations in its order so that
     every float is the reference's"""

@@ -175,9 +175,11 @@ class FusedComputeLoss:
     `ComputeLoss(...)(p, targets)[0] * mult / batch * scale` with the batch factor already inside, i.e. of `loss * mult_after_bs * scale`."""
 
     def __init__(self, model):
+        from .. import _lib
         self.ref = ComputeLoss(model)
         r = self.ref
-        self.supported = (r.gamma == 0.0 and r.cls_pw == 1.0 and r.obj_pw == 1.0 and not r.autobalance and r.nl <= 3 and r.na <= 3)
+        self.supported = (r.gamma == 0.0 and r.cls_pw == 1.0 and r.obj_pw == 1.0 and not r.autobalance and r.nl <= 3
+                          and r.na <= _lib.DET_LOSS_NA_MAX)
         self._ws = None
 
     def __call__(self, p, targets, mult=1.0, scale=None):
