@@ -142,6 +142,14 @@ int myolo_plan_set_extra(myolo_plan* plan, int offset, const void* src, int n, v
  * seg: (B,n_segcls,H,W) of seg_dtype (nullable); seg_argmax: (B,H,W) int64 class ids (nullable, fused path). */
 int myolo_plan_forward(myolo_plan* plan, const void* x, int x_dtype, float* z, float* const* raw, void* seg, int seg_dtype,
                        int64_t* seg_argmax, void* stream);
+/* One pass of test-time augmentation (reference models/yolo.py:274-289): myolo_plan_forward without raw outputs, whose Detect decodes write
+ * the plan's rows into rows [z_row_offset, z_row_offset + plan rows) of z (B, z_rows_total, 5+nc) fp32, with the four box columns
+ * multiplied by z_inv_scale (`yi[..., :4] /= si` with z_inv_scale = 1.0f / (float)si) and, for z_flip_w > 0, column 0 replaced by
+ * (float)z_flip_w - x (`yi[..., 0] = img_size[1] - yi[..., 0]`), each rounded once.  (z_rows_total = plan rows, 0, 1.0f, 0) is
+ * myolo_plan_forward's z bit for bit.  The arguments reach only the decodes, which run after the captured graph: changing them between
+ * calls captures nothing again.  MYOLO_E_INVALID when the rows do not fit, z_inv_scale is not positive and finite or z_flip_w < 0. */
+int myolo_plan_forward_pass(myolo_plan* plan, const void* x, int x_dtype, float* z, int z_rows_total, int z_row_offset, float z_inv_scale,
+                            int z_flip_w, void* seg, int seg_dtype, int64_t* seg_argmax, void* stream);
 /* debugging / per-layer parity: copies the NHWC buffer slice of a view into dst as (B,C,H,W) fp32 */
 int myolo_plan_read_view(myolo_plan* plan, myolo_view view, float* dst_nchw, void* stream);
 /* number of kernels the last myolo_plan_forward launched (bench.py's gpu_launches) */
@@ -439,6 +447,12 @@ int myolo_resize_area_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H
  * MYOLO_U8 (each tap converted as imgs.float() / 255.0 converts it on the device: v * fp32(1/255)), MYOLO_F16 or MYOLO_F32; dst_dtype
  * MYOLO_F16 (the fp32 result rounded to nearest) or MYOLO_F32.  Equal sizes convert only. */
 int myolo_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo, void* stream);
+/* myolo_scale_img: scale_img of test-time augmentation (reference utils/torch_utils.py:248-258) in one launch: F.interpolate of NCHW src
+ * (B,C,H,W) to (Ho, Wo), bilinear, align_corners=False, as myolo_resize_bilinear computes it, then F.pad on the right and bottom to
+ * dst (B,C,Hp,Wp) with pad_value (the caller rounds it to the dtype, as torch's fill does); Hp < Ho or Wp < Wo crops.  flip_lr != 0
+ * resamples src.flip(3) instead.  src and dst share dtype, MYOLO_F16 or MYOLO_F32. */
+int myolo_scale_img(const void* src, int dtype, int B, int C, int H, int W, void* dst, int Ho, int Wo, int Hp, int Wp, int flip_lr,
+                    float pad_value, void* stream);
 int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, void* stream);
 /* myolo_augment_det_hw: the same per-pixel work on B augmented H x W images (`LoadImagesAndLabels(augment=True, rect=True)`: a letterbox
  * to the batch shape, random_perspective at (W, H), flips over H and W), out (B,3,H,W).  myolo_augment_det is its H = W = S case. */

@@ -42,7 +42,7 @@ EXPORTS = [
     "myolo_anchor_metric", "myolo_anchor_metric_workspace_bytes", "myolo_anchor_evolve", "myolo_anchor_evolve_workspace_bytes",
     "myolo_kmeans", "myolo_kmeans_workspace_bytes", "myolo_class_weights", "myolo_image_weights", "myolo_weighted_draw",
     "myolo_plan_backward_seg_loss", "myolo_seg_focal_loss", "myolo_seg_focal_loss_backward", "myolo_seg_focal_loss_workspace_bytes",
-    "myolo_conv_backward", "myolo_conv_forward",
+    "myolo_conv_backward", "myolo_conv_forward", "myolo_plan_forward_pass", "myolo_scale_img",
 ]
 REDUCTION_MEAN, REDUCTION_SUM = 0, 1        # include/myolo.h: MYOLO_REDUCTION_* of myolo_seg_focal_loss
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
@@ -121,6 +121,7 @@ def lib():
     L.myolo_plan_set_conv_weights.argtypes = [vp, i32, vp, i32, i32, i32, vp, vp, vp, vp, f32, vp, vp]
     L.myolo_plan_repack_weights.argtypes = [vp, vp]
     L.myolo_plan_forward.argtypes = [vp, vp, i32, vp, C.POINTER(vp), vp, i32, vp, vp]
+    L.myolo_plan_forward_pass.argtypes = [vp, vp, i32, vp, i32, i32, f32, i32, vp, i32, vp, vp]
     L.myolo_plan_read_view.argtypes = [vp, View, vp, vp]
     L.myolo_plan_last_launch_count.argtypes = [vp]
     L.myolo_plan_last_launch_count.restype = i64
@@ -133,6 +134,7 @@ def lib():
     L.myolo_resize_u8.argtypes = [vp, i32, i32, vp, i32, i32, vp]
     L.myolo_resize_area_u8.argtypes = [vp, i32, i32, vp, i32, i32, vp]
     L.myolo_resize_bilinear.argtypes = [vp, i32, i32, i32, i32, i32, vp, i32, i32, i32, vp]
+    L.myolo_scale_img.argtypes = [vp, i32, i32, i32, i32, i32, vp, i32, i32, i32, i32, i32, f32, vp]
     L.myolo_augment_det.argtypes = [vp, i32, i32, vp, i32, vp]
     L.myolo_augment_det_hw.argtypes = [vp, i32, i32, i32, vp, i32, vp]
     L.myolo_collate_quad.argtypes = [vp, i32, i32, i32, vp, vp, i32, vp]

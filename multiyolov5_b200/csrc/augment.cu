@@ -245,6 +245,61 @@ int launch_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, 
 }
 
 // ------------------------------------------------------------------------------------------------
+// scale_img (reference utils/torch_utils.py:248-258) of test-time augmentation, optionally of x.flip(3): F.interpolate to (Ho, Wo) as
+// resize_bilinear_kernel computes it, then F.pad on the right and bottom to (Hp, Wp) with `pad` (already rounded to the dtype by the
+// host; Hp < Ho or Wp < Wo crops, as F.pad's negative padding does).  flip reads source column W-1-w: the interpolation of the mirrored
+// image.  One thread per output pixel of one plane; grid (x tiles, rows, planes).
+// ------------------------------------------------------------------------------------------------
+template <typename T>
+__global__ void __launch_bounds__(128) scale_img_kernel(const T* __restrict__ src, int planes, int H, int W, T* __restrict__ dst, int Ho,
+                                                        int Wo, int Hp, int Wp, float rh, float rw, int flip, float pad) {
+  const int x = blockIdx.x * blockDim.x + threadIdx.x, y = blockIdx.y;
+  if (x >= Wp) return;
+  const bool inside = y < Ho && x < Wo;
+  const bool same = H == Ho && W == Wo;
+  int h0 = y, h1 = y, w0 = x, w1 = x;
+  float h0l = 1.f, h1l = 0.f, w0l = 1.f, w1l = 0.f;
+  if (inside && !same) {
+    bilinear_source(y, H, rh, &h0, &h1, &h0l, &h1l);
+    bilinear_source(x, W, rw, &w0, &w1, &w0l, &w1l);
+  }
+  if (flip) { w0 = W - 1 - w0; w1 = W - 1 - w1; }
+  for (int p = blockIdx.z; p < planes; p += gridDim.z) {
+    const T* s = src + (size_t)p * H * W;
+    float val = pad;
+    if (inside && same) {
+      val = bilinear_tap(s + (size_t)h0 * W + w0);
+    } else if (inside) {
+      const float a = bilinear_tap(s + (size_t)h0 * W + w0), b = bilinear_tap(s + (size_t)h0 * W + w1);
+      const float c = bilinear_tap(s + (size_t)h1 * W + w0), d = bilinear_tap(s + (size_t)h1 * W + w1);
+      const float top = __fmaf_rn(w0l, a, __fmul_rn(w1l, b));
+      const float bot = __fmaf_rn(w0l, c, __fmul_rn(w1l, d));
+      val = __fmaf_rn(h0l, top, __fmul_rn(h1l, bot));
+    }
+    const size_t o = ((size_t)p * Hp + y) * Wp + x;
+    if constexpr (sizeof(T) == 2) dst[o] = __float2half_rn(val);
+    else dst[o] = val;
+  }
+}
+
+int launch_scale_img(const void* src, int dtype, int B, int C, int H, int W, void* dst, int Ho, int Wo, int Hp, int Wp, int flip_lr, float pad,
+                     cudaStream_t s) {
+  MYOLO_REQUIRE(src && dst && B > 0 && C > 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0 && Hp > 0 && Wp > 0 && Hp <= 65535,
+                "scale_img: bad geometry (B %d C %d src %dx%d resized %dx%d padded %dx%d)", B, C, H, W, Ho, Wo, Hp, Wp);
+  MYOLO_REQUIRE(dtype == MYOLO_F16 || dtype == MYOLO_F32, "scale_img: dtype %d (fp16 or fp32 only)", dtype);
+  MYOLO_REQUIRE((long)B * C <= (1L << 31) - 1, "scale_img: too many planes");
+  const int planes = B * C;
+  const float rh = (float)H / (float)Ho, rw = (float)W / (float)Wo;     // area_pixel_compute_scale, as in launch_resize_bilinear
+  const dim3 grid((Wp + 127) / 128, Hp, std::min(planes, 65535));
+  if (dtype == MYOLO_F16)
+    scale_img_kernel<__half><<<grid, 128, 0, s>>>((const __half*)src, planes, H, W, (__half*)dst, Ho, Wo, Hp, Wp, rh, rw, flip_lr != 0, pad);
+  else
+    scale_img_kernel<float><<<grid, 128, 0, s>>>((const float*)src, planes, H, W, (float*)dst, Ho, Wo, Hp, Wp, rh, rw, flip_lr != 0, pad);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // --quad (reference utils/datasets.py:602-625 LoadImagesAndLabels.collate_fn4): quad q of the output is either the 2x2 tile of items
 // 4q (top left), 4q+1 (bottom left), 4q+2 (top right), 4q+3 (bottom right), or
 //   F.interpolate(img[4q].float()[None], scale_factor=2., mode='bilinear', align_corners=False)[0].type(uint8)

@@ -489,9 +489,12 @@ __device__ __forceinline__ float detect_decode_one(float v, int o, int x, int y,
 }
 // grid = (chunks of W*no/4, H, B*na).  For a fixed (image, anchor, row) both outputs are contiguous over (x, o): a thread takes FOUR consecutive
 // (x, o) positions - scalar reads of the head conv's fp32 NHWC rows (just written: L2), one 16-byte store each to raw and z.
+// Test-time augmentation's de-scale and de-flip of z (reference models/yolo.py:283-287) as torch computes them on fp32 CUDA tensors:
+// `yi[..., :4] /= si` multiplies by inv_scale = 1.0f / (float)si (ATen's reciprocal for a CPU-scalar divisor), `yi[..., 0] = W0 - yi[..., 0]`
+// is one fp32 subtraction.  Both are explicitly rounded so that nvcc cannot contract them into an FMA; inv_scale 1 leaves z unchanged.
 template <int NO>
 __global__ void detect_decode_kernel(TensorView in, int na, int no_rt, float stride, const float* __restrict__ anchors, float* raw,
-                                     float* z, int z_off, int z_rows, int vec) {
+                                     float* z, int z_off, int z_rows, int vec, float inv_scale, int flip_w) {
   const int no = NO > 0 ? NO : no_rt;
   const int j0 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
   const int row_elems = in.W * no;
@@ -507,6 +510,8 @@ __global__ void detect_decode_kernel(TensorView in, int na, int no_rt, float str
     const bool ok = j0 + k < row_elems;
     v[k] = ok ? src[(size_t)x * in.ctot + o] : 0.f;
     d[k] = (z && ok) ? detect_decode_one(v[k], o, x, y, a, stride, anchors) : 0.f;
+    if (o < 4) d[k] = __fmul_rn(d[k], inv_scale);
+    if (o == 0 && flip_w > 0) d[k] = __fsub_rn((float)flip_w, d[k]);
     if (++o == no) { o = 0; ++x; }
   }
   const bool full = vec && j0 + 3 < row_elems;       // rows that are not a multiple of 16 bytes (odd maps) take scalar stores
@@ -521,14 +526,16 @@ __global__ void detect_decode_kernel(TensorView in, int na, int no_rt, float str
   else for (int k = 0; k < 4 && j0 + k < row_elems; ++k) q[k] = d[k];
 }
 int launch_detect_decode(const TensorView& in, int na, int no, float stride, const float* d_anchors, float* raw, float* z,
-                         int z_row_offset, int z_rows_total, cudaStream_t s) {
+                         int z_row_offset, int z_rows_total, cudaStream_t s, float z_inv_scale, int z_flip_w) {
   MYOLO_REQUIRE(in.dtype == MYOLO_F32 && in.C >= na * no, "detect_decode: bad view");
   // 16-byte stores need (W * no) % 4 == 0 rows and 16-byte aligned bases (torch allocations are; z_row_offset * no * 4 must be too)
   const bool vec_ok = (in.W * no) % 4 == 0 && ((size_t)z_row_offset * no) % 4 == 0 && ((size_t)z_rows_total * no) % 4 == 0 &&
                       (!raw || (reinterpret_cast<uintptr_t>(raw) & 15) == 0) && (!z || (reinterpret_cast<uintptr_t>(z) & 15) == 0);
   const dim3 grid(ceil_div(ceil_div(in.W * no, 4), 128), in.H, in.B * na);
-  if (no == 15) detect_decode_kernel<15><<<grid, 128, 0, s>>>(in, na, no, stride, d_anchors, raw, z, z_row_offset, z_rows_total, (int)vec_ok);
-  else detect_decode_kernel<0><<<grid, 128, 0, s>>>(in, na, no, stride, d_anchors, raw, z, z_row_offset, z_rows_total, (int)vec_ok);
+  if (no == 15) detect_decode_kernel<15><<<grid, 128, 0, s>>>(in, na, no, stride, d_anchors, raw, z, z_row_offset, z_rows_total, (int)vec_ok,
+                                                                 z_inv_scale, z_flip_w);
+  else detect_decode_kernel<0><<<grid, 128, 0, s>>>(in, na, no, stride, d_anchors, raw, z, z_row_offset, z_rows_total, (int)vec_ok,
+                                                                 z_inv_scale, z_flip_w);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }

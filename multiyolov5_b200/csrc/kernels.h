@@ -20,9 +20,10 @@ int launch_region_combine(const TensorView& atoms, int atoms_nx, const int* d_bi
 int launch_channel_scale(const TensorView& feat, const TensorView& att, cudaStream_t s);
 int launch_add(const TensorView& a, const TensorView& b, const TensorView& out, cudaStream_t s);
 int launch_broadcast(const TensorView& in, const TensorView& out, cudaStream_t s);
-// Detect.forward (reference models/yolo.py:211-225): in = fp32 NHWC conv output (channel = a*no + o)
+// Detect.forward (reference models/yolo.py:211-225): in = fp32 NHWC conv output (channel = a*no + o).  Test-time augmentation
+// (models/yolo.py:274-289): z's four box columns are multiplied by z_inv_scale, and z_flip_w > 0 replaces x by z_flip_w - x
 int launch_detect_decode(const TensorView& in, int na, int no, float stride, const float* d_anchors /*na*2 px*/, float* raw,
-                         float* z, int z_row_offset, int z_rows_total, cudaStream_t s);
+                         float* z, int z_row_offset, int z_rows_total, cudaStream_t s, float z_inv_scale = 1.0f, int z_flip_w = 0);
 // final bilinear(align_corners) of the seg head: in = fp32 NHWC low-res logits; seg NCHW (fp32/fp16, nullable); argmax nullable
 int launch_seg_upsample(const TensorView& in, int n_cls, int H, int W, void* seg, int seg_dtype, int64_t* argmax,
                         cudaStream_t s);
@@ -37,6 +38,8 @@ int launch_resize_u8(const unsigned char* src, int H0, int W0, unsigned char* ds
 int launch_resize_area_u8(const unsigned char* src, int H0, int W0, unsigned char* dst, int H, int W, cudaStream_t s);
 int launch_augment_det(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, cudaStream_t s);
 int launch_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo, cudaStream_t s);
+int launch_scale_img(const void* src, int dtype, int B, int C, int H, int W, void* dst, int Ho, int Wo, int Hp, int Wp, int flip_lr, float pad,
+                     cudaStream_t s);
 int launch_collate_quad(const unsigned char* imgs, int B, int H, int W, const unsigned char* tile, void* out, int out_dtype, cudaStream_t s);
 
 // segmentation training batches (augment_seg.cu): crop-window resample + pad + mask LUT, then the ColorJitter / ToTensor kernel

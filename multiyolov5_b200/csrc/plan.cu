@@ -11,6 +11,7 @@ struct NvtxRange {
 #include <stdarg.h>
 
 #include <algorithm>
+#include <cmath>
 #include <string>
 #include <vector>
 
@@ -153,6 +154,10 @@ struct myolo_plan {
   int n_pack_jobs = 0, n_pack_chunks = 0, pack_jobs_cap = 0;
   bool pack_table_dirty = true;
   cudaStream_t decode_stream = nullptr;   // low-priority side stream of the Detect decodes (myolo_plan_forward)
+  // where the Detect decodes of the current call write z (myolo_plan_forward_pass): z_rows rows per image (0: the plan's own total), the
+  // plan's rows from z_off on, box columns times z_inv, x mirrored at z_flip_w (0: none).  Read by the decodes only, which are never captured.
+  int z_rows = 0, z_off = 0, z_flip_w = 0;
+  float z_inv = 1.0f;
   // deferred running statistics (myolo_plan_set_defer_running / myolo_plan_apply_running)
   bool defer_running = false;
   RunningJob* d_run_jobs = nullptr;
@@ -640,7 +645,8 @@ static int run_op(myolo_plan* pl, int i, const void* x, int x_dtype, float* z, f
       const int level = op.aux[0];
       MYOLO_REQUIRE(z != nullptr || raw != nullptr, "detect_decode: no output pointer");
       return launch_detect_decode(in, op.aux[1], op.aux[2], op.faux[0], reinterpret_cast<const float*>(pl->d_extra + op.aux[5]),
-                                  raw ? raw[level] : nullptr, z, op.aux[3], op.aux[4], s);
+                                  raw ? raw[level] : nullptr, z, pl->z_off + op.aux[3], pl->z_rows > 0 ? pl->z_rows : op.aux[4], s, pl->z_inv,
+                                  pl->z_flip_w);
     }
     case MYOLO_OP_SEG_UPSAMPLE: {
       if ((rc = resolve_view(pl, op.in, &in))) return rc;
@@ -766,6 +772,28 @@ extern "C" int myolo_plan_forward(myolo_plan* pl, const void* x, int x_dtype, fl
   }
   pl->last_launches = pl->n_graph_ops + n_ext;
   return 0;
+}
+
+extern "C" int myolo_plan_forward_pass(myolo_plan* pl, const void* x, int x_dtype, float* z, int z_rows_total, int z_row_offset,
+                                       float z_inv_scale, int z_flip_w, void* seg, int seg_dtype, int64_t* seg_argmax, void* stream) {
+  MYOLO_REQUIRE(pl && x && z, "plan_forward_pass: null plan / input / z");
+  int plan_rows = 0;
+  for (const auto& op : pl->ops)
+    if (op.kind == MYOLO_OP_DETECT_DECODE) plan_rows = op.aux[4];
+  MYOLO_REQUIRE(plan_rows > 0, "plan_forward_pass: the plan has no Detect decode");
+  MYOLO_REQUIRE(z_row_offset >= 0 && z_rows_total >= plan_rows && z_row_offset <= z_rows_total - plan_rows,
+                "plan_forward_pass: rows [%d, %d) of the plan's outputs do not fit in %d rows", z_row_offset, z_row_offset + plan_rows,
+                z_rows_total);
+  MYOLO_REQUIRE(z_inv_scale > 0.f && std::isfinite(z_inv_scale), "plan_forward_pass: inv_scale %g", z_inv_scale);
+  MYOLO_REQUIRE(z_flip_w >= 0, "plan_forward_pass: flip width %d", z_flip_w);
+  pl->z_rows = z_rows_total;
+  pl->z_off = z_row_offset;
+  pl->z_inv = z_inv_scale;
+  pl->z_flip_w = z_flip_w;
+  const int rc = myolo_plan_forward(pl, x, x_dtype, z, nullptr, seg, seg_dtype, seg_argmax, stream);
+  pl->z_rows = pl->z_off = pl->z_flip_w = 0;
+  pl->z_inv = 1.0f;
+  return rc;
 }
 
 // keeps the stream busy for `ns` nanoseconds: myolo_plan_profile enqueues every op and event behind it, so that the event-to-event times are
@@ -1456,6 +1484,13 @@ extern "C" int myolo_resize_bilinear(const void* src, int src_dtype, int B, int 
   int rc = check_device(nullptr);
   if (rc) return rc;
   return launch_resize_bilinear(src, src_dtype, B, C, H, W, dst, dst_dtype, Ho, Wo, (cudaStream_t)stream);
+}
+
+extern "C" int myolo_scale_img(const void* src, int dtype, int B, int C, int H, int W, void* dst, int Ho, int Wo, int Hp, int Wp, int flip_lr,
+                               float pad_value, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_scale_img(src, dtype, B, C, H, W, dst, Ho, Wo, Hp, Wp, flip_lr, pad_value, (cudaStream_t)stream);
 }
 
 extern "C" int myolo_collate_quad(const uint8_t* imgs, int B, int H, int W, const uint8_t* tile, void* out, int out_dtype, void* stream) {

@@ -4,6 +4,7 @@ import os
 import ctypes as C
 from typing import Dict, Tuple
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -53,10 +54,11 @@ class TrainArena:
 
 
 class CompiledPlan:
-    def __init__(self, model, B, H, W, noalias=False, train=False, arena=None, pb=None):
-        """arena: a TrainArena the (train) plan binds to instead of allocating private workspaces; pb: its already-built host plan"""
+    def __init__(self, model, B, H, W, noalias=False, train=False, arena=None, pb=None, seg=True):
+        """arena: a TrainArena the (train) plan binds to instead of allocating private workspaces; pb: its already-built host plan;
+        seg=False: an inference plan without the seg head (build_plan)"""
         self.train = train
-        self.pb = pb if pb is not None else build_plan(model, B, H, W, noalias=noalias, train=train)
+        self.pb = pb if pb is not None else build_plan(model, B, H, W, noalias=noalias, train=train, seg=seg)
         self.ops, self.bufs, self.extra = to_ctypes(self.pb)
         self.arena = arena                   # keeps the shared workspaces alive as long as the plan
         L = _lib.lib()
@@ -177,10 +179,11 @@ class Engine:
                 p.refresh_anchors(self.model.model[-1])
             p.weights_key = key
 
-    def plan_for(self, B, H, W) -> CompiledPlan:
-        key = (B, H, W)
+    def plan_for(self, B, H, W, seg=True) -> CompiledPlan:
+        """the inference plan of (B, H, W); seg=False: the one without the seg head (test-time augmentation's scaled passes)"""
+        key = (B, H, W) if seg else ("det", B, H, W)
         if key not in self.plans:
-            self.plans[key] = CompiledPlan(self.model, B, H, W, self.noalias)
+            self.plans[key] = CompiledPlan(self.model, B, H, W, self.noalias, seg=seg)
         p = self.plans[key]
         self._upload_if_stale(p)
         self.last_plan = p
@@ -217,6 +220,53 @@ class Engine:
         else:
             _lib.check(L.myolo_plan_forward(*args, _lib.stream_ptr()))
         out = [(z, raws), seg]
+        if seg_argmax:
+            out.append(amax)
+        return out
+
+    def forward_augment(self, x: torch.Tensor, seg_argmax=False, det_only_scaled=True):
+        """test-time augmentation, reference models/yolo.py:274-289 (Model.forward(augment=True)) with the fork's missing index restored
+        (`forward_once(xi)[0][0]`): `[(z, None), seg]`, plus the argmax map with seg_argmax=True.  z (B, rows of the three passes, no) fp32
+        holds, per image, pass 0's rows, then pass 1's (x.flip(3) scaled by 0.83), then pass 2's (scaled by 0.67), their boxes de-scaled
+        and pass 1's x mirrored back, each pass's Detect decodes writing straight into its slice.  seg / argmax are pass 0's, those of
+        augment=False; the scaled passes run plans without the seg head (det_only_scaled=False: the full plans, for comparison).  Every
+        launch goes to the current stream; nothing synchronises with the host."""
+        if not x.is_cuda:
+            raise _lib.MyoloError("Model.forward(augment=True) needs a CUDA tensor: multiyolov5_b200 has no CPU path")
+        if x.dtype not in (torch.float16, torch.float32):
+            raise TypeError(f"Model.forward(augment=True) takes fp16 or fp32 input scaled to [0, 1] (detect.py divides by 255 first), "
+                            f"not {x.dtype}")
+        assert x.dim() == 4 and x.shape[1] == 3, "expected (B,3,H,W)"
+        from .utils.torch_utils import scale_img, tta_passes
+        x = x.contiguous()
+        B, _, H, W = x.shape
+        det = self.model.model[-1]
+        gs = int(det.stride.max())
+        passes = tta_passes(H, W, gs)
+        offs = [0]
+        for _, _, _, (hp, wp) in passes:
+            offs.append(offs[-1] + sum(det.na * (hp // int(s)) * (wp // int(s)) for s in det.stride))
+        dev = x.device
+        z = torch.empty((B, offs[-1], det.no), dtype=torch.float32, device=dev)
+        half_model = next(self.model.parameters()).dtype == torch.float16
+        seg_dt = torch.float16 if (x.dtype == torch.float16 or half_model) else torch.float32
+        seg_head = self.model.model[-2]
+        seg = torch.empty((B, seg_head.c_out, H, W), dtype=seg_dt, device=dev) if not seg_argmax else None
+        amax = torch.empty((B, H, W), dtype=torch.int64, device=dev) if seg_argmax else None
+        L, sp = _lib.lib(), _lib.stream_ptr()
+        # each pass's plan is looked up (and on first use built) right before its launches, so that this host work overlaps the
+        # previous pass on the device
+        for k, (si, flip, _, (hp, wp)) in enumerate(passes):
+            p = self.plan_for(B, hp, wp, seg=(k == 0 or not det_only_scaled))
+            assert sum(p.pb.det_rows) == offs[k + 1] - offs[k]
+            if k == 0:
+                self.last_plan = p
+            xi = x if k == 0 else scale_img(x, si, gs=gs, flip_lr=flip)
+            inv = float(np.float32(1.0) / np.float32(si))          # `yi[..., :4] /= si`: ATen multiplies by the fp32 reciprocal
+            _lib.check(L.myolo_plan_forward_pass(p.handle, _lib.ptr(xi), _lib.torch_dtype_code(xi.dtype), _lib.ptr(z), offs[-1], offs[k],
+                                                 inv, W if flip else 0, _lib.ptr(seg if k == 0 else None), _lib.torch_dtype_code(seg_dt),
+                                                 _lib.ptr(amax if k == 0 else None), sp))
+        out = [(z, None), seg]
         if seg_argmax:
             out.append(amax)
         return out

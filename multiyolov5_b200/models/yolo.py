@@ -239,9 +239,16 @@ class Model(nn.Module):
 
     def forward(self, x, augment=False, profile=False, seg_argmax=False):
         """eval: `[(z, [x0,x1,x2]), seg]` like reference models/yolo.py:225,316.  `seg_argmax=True` additionally returns the
-        fused upsample+argmax class map (B,H,W) int64 as a third element and skips materialising logits."""
+        fused upsample+argmax class map (B,H,W) int64 as a third element and skips materialising logits.
+        augment=True (eval only): test-time augmentation, `[(z, None), seg]` (Engine.forward_augment): z of the three scaled and flipped
+        passes of reference models/yolo.py:274-289, seg the un-augmented one."""
         if augment:
-            raise NotImplementedError("TTA (augment=True) is broken in the reference fork itself (SURVEY.md section 2 #18)")
+            if self.training:
+                raise RuntimeError("Model.forward(augment=True) needs eval mode: the reference's augment loop decodes boxes, which a "
+                                   "train-mode forward does not (call model.eval())")
+            if profile:
+                raise ValueError("Model.forward: profile=True profiles one plain forward; it cannot be combined with augment=True")
+            return self.engine().forward_augment(x, seg_argmax=seg_argmax)
         if self.training:
             # train mode: `[[x0,x1,x2], seg]` with batch-statistics BatchNorm and a hand-written backward behind torch.autograd
             # (reference models/yolo.py:225,316; train.py:363-392).  All four heads; BiSe returns seg = [out, aux16, aux32] (models/yolo.py:86).

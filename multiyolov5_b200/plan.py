@@ -538,10 +538,14 @@ def infer_strides(model):
     return _layer_meta(model)[1]
 
 
-def build_plan(model, B: int, H: int, W: int, noalias: bool = False, train: bool = False) -> PlanBuilder:
-    """Lowers model.model (yaml layers) for a fixed input shape (train=True: batch-stat BN ops, everything kept for backward)."""
+def build_plan(model, B: int, H: int, W: int, noalias: bool = False, train: bool = False, seg: bool = True) -> PlanBuilder:
+    """Lowers model.model (yaml layers) for a fixed input shape (train=True: batch-stat BN ops, everything kept for backward).
+    seg=False (inference only): without the seg head's ops, for the scaled passes of test-time augmentation, whose seg output nobody
+    reads (reference models/yolo.py:274-289 keeps the Detect output only); every other op is lowered as in the full plan."""
     from .models import yolo as Y
     assert H % 32 == 0 and W % 32 == 0, "input H, W must be multiples of the max stride 32 (reference check_img_size)"
+    assert seg or not train, "a train plan keeps the seg head"
+    seg_types = (Y.SegMaskPSP, Y.SegMaskLab, Y.SegMaskBiSe, Y.SegMaskBase)
     pb = PlanBuilder(B, H, W, train=train)
     noalias = noalias or train
     ch, st = _layer_meta(model)
@@ -577,10 +581,11 @@ def build_plan(model, B: int, H: int, W: int, noalias: bool = False, train: bool
     order = list(range(n))
     if not train:
         for i in range(1, n):
-            seg_types = (Y.SegMaskPSP, Y.SegMaskLab, Y.SegMaskBiSe, Y.SegMaskBase)
             if isinstance(layers[i], Y.Detect) and isinstance(layers[i - 1], seg_types) and \
                     all(absf(i, j) < i - 1 for j in ([layers[i].f] if isinstance(layers[i].f, int) else layers[i].f)):
                 order[i - 1], order[i] = i, i - 1
+    if not seg:
+        order = [i for i in order if not isinstance(layers[i], seg_types)]
     for i in order:
         m = layers[i]
         pb.tag = f"L{i}:{type(m).__name__}"

@@ -7,6 +7,46 @@ import torch
 from .. import _lib
 
 
+def scale_img_shapes(h, w, ratio=1.0, same_shape=False, gs=32):
+    """((resized h, w), (output h, w)) of reference utils/torch_utils.py:248-258 scale_img, with its host arithmetic: int(h * ratio) for
+    the resize, math.ceil(h * ratio / gs) * gs for the padded output unless same_shape keeps (h, w).  ratio 1.0 returns the image as is."""
+    if ratio == 1.0:
+        return (h, w), (h, w)
+    s = (int(h * ratio), int(w * ratio))
+    if not same_shape:
+        h, w = [math.ceil(x * ratio / gs) * gs for x in (h, w)]
+    return s, (h, w)
+
+
+TTA_SCALES, TTA_FLIPS = (1, 0.83, 0.67), (False, True, False)      # reference models/yolo.py:276-277: flips None, 3 (left-right), None
+
+
+def tta_passes(h, w, gs=32):
+    """[(scale, left-right flip, (resized h, w), (input h, w))] of the three passes of test-time augmentation on an (h, w) input"""
+    return [(si, fi) + scale_img_shapes(h, w, si, gs=gs) for si, fi in zip(TTA_SCALES, TTA_FLIPS)]
+
+
+def scale_img(img, ratio=1.0, same_shape=False, gs=32, flip_lr=False):
+    """reference utils/torch_utils.py:248-258 on the device (myolo_scale_img, one launch): F.interpolate(img, bilinear,
+    align_corners=False) to int(h * ratio) x int(w * ratio), then F.pad on the right and bottom with 0.447 to a multiple of gs (or back
+    to (h, w) with same_shape).  flip_lr=True scales img.flip(3) instead.  img: (B, C, H, W) fp16 or fp32 CUDA; ratio 1.0 without
+    flip_lr returns img itself, as the reference does."""
+    if not img.is_cuda:
+        raise _lib.MyoloError("scale_img needs a CUDA tensor: multiyolov5_b200 has no CPU path")
+    if img.dtype not in (torch.float16, torch.float32):
+        raise TypeError(f"scale_img takes fp16 or fp32 images, not {img.dtype}")
+    if ratio == 1.0 and not flip_lr:
+        return img
+    h, w = img.shape[2:]
+    (ho, wo), (hp, wp) = scale_img_shapes(h, w, ratio, same_shape, gs)
+    img = img.contiguous()
+    out = torch.empty((img.shape[0], img.shape[1], hp, wp), dtype=img.dtype, device=img.device)
+    pad = float(torch.tensor(0.447, dtype=img.dtype))          # the value F.pad fills in: 0.447 rounded to the image's dtype
+    _lib.check(_lib.lib().myolo_scale_img(_lib.ptr(img), _lib.torch_dtype_code(img.dtype), img.shape[0], img.shape[1], h, w, _lib.ptr(out),
+                                          ho, wo, hp, wp, int(flip_lr), pad, _lib.stream_ptr()))
+    return out
+
+
 def is_parallel(model):
     return type(model) in (torch.nn.parallel.DataParallel, torch.nn.parallel.DistributedDataParallel)
 
