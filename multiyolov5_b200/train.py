@@ -32,7 +32,8 @@ step then run one after the other.  At world size 1, or without torch.distribute
 
 `fit(model, hyp, opt, det_batches, seg_batches, ...)` is the reference's epoch loop (train.py:44-543) around the step: `LRSchedule` (warm-up,
 LambdaLR, momentum, accumulation), the validation cadence, fitness2 and best.pt, results.txt, last.pt / best.pt and resume.
-`DetEpochBatches` / `SegEpochBatches` give each epoch's batches from the device loaders in the reference's order.
+`DetEpochBatches` / `SegEpochBatches` give each epoch's batches from the device loaders in the reference's order, and `SegValBatches` the
+seg validation batches (mode='val' or 'testval') for `fit(..., segval_loader=)`.
 
 `evolve(hyp, opt, train_fn)` is the reference's --evolve (train.py:637-717): generations of `train_fn` (a training run such as `fit`),
 each with hyper-parameters mutated from the best earlier results in evolve.txt.
@@ -808,6 +809,50 @@ class SegEpochBatches:
         return (self.aug(idx.tolist(), self.out_dtype) for idx in self.order())
 
 
+class SegValBatches:
+    """`segval_loader` for fit and `valloader` for test.seg_validation: the seg validation batches of a utils.datasets.SegAugmenter in the
+    order of the reference's DataLoader(shuffle=False, drop_last=False) (SegmentationDataset.get_*_loader with a mode other than
+    'train'): items 0 .. n-1 in runs of `batch_size`, the last one partial.  Iterable again for every validation pass; each batch is
+    built when it is asked for, so a pass holds one batch at a time.
+
+    mode='val': `aug.val(chunk, crop_size)`, train_citysbdd.py's validation (batch 4, int crop_size 512 over City+BDD sources of
+    different sizes).  mode='testval': `aug.testval(chunk)`, that of train.py (batch 4, base_size 1024) and of train_custom.py (batch 1,
+    base_size imgsz), at the augmenter's base_size; crop_size is unused, as in the reference.  The items of a testval batch must share
+    their source size, as default_collate requires: a batch that does not raises ValueError here, before any batch is built."""
+
+    def __init__(self, aug, batch_size, mode="val", crop_size=None, out_dtype=torch.float32):
+        from .utils.datasets import seg_val_crop
+        if mode not in ("val", "testval"):
+            raise ValueError(f"SegValBatches: mode must be 'val' or 'testval', got {mode!r}")
+        if int(batch_size) < 1:
+            raise ValueError(f"SegValBatches: batch_size must be positive, got {batch_size}")
+        if out_dtype not in (torch.uint8, torch.float16, torch.float32):
+            raise ValueError(f"SegValBatches: out_dtype must be uint8, float16 or float32, got {out_dtype}")
+        self.aug, self.batch_size, self.mode, self.out_dtype = aug, int(batch_size), mode, out_dtype
+        self.n = aug.cache.n
+        self.crop_size = seg_val_crop(crop_size) if mode == "val" else crop_size
+        if mode == "testval":
+            for chunk in self.chunks():
+                shapes = sorted({aug.cache.shapes[i] for i in chunk})
+                if len(shapes) != 1:
+                    raise ValueError(f"SegValBatches: testval batch of items {chunk[0]}..{chunk[-1]} mixes source sizes {shapes}, which "
+                                     "default_collate cannot stack (mode='val' crops them to one size)")
+
+    def __len__(self):
+        return math.ceil(self.n / self.batch_size)
+
+    def chunks(self):
+        """the index batches, in order"""
+        return [list(range(k, min(k + self.batch_size, self.n))) for k in range(0, self.n, self.batch_size)]
+
+    def __iter__(self):
+        for chunk in self.chunks():
+            if self.mode == "val":
+                yield self.aug.val(chunk, self.crop_size, self.out_dtype)
+            else:
+                yield self.aug.testval(chunk, self.out_dtype)
+
+
 def _unsupported_flags(opt):
     """NotImplementedError naming the first flag of `opt` the loop cannot honour"""
     for name, on in (("bucket", getattr(opt, "bucket", "")), ("entity", getattr(opt, "entity", None)),
@@ -840,7 +885,8 @@ def fit(model, hyp, opt, det_batches, seg_batches, *, test_loader=None, segval_l
     det_batches(epoch) / seg_batches(epoch): that epoch's iterables of (imgs, targets, ...) and (segimgs, segtargets) device batches,
     with len(det_batches) = nb; DetEpochBatches / SegEpochBatches build them from the device loaders in the reference's order.  Det images
     are float (B, 3, H, W) = uint8 / 255, or uint8 under multi_scale.  test_loader: DetValLoader batches for test.test (None: no test,
-    results stay zeros); segval_loader: mode='testval' seg batches for test.seg_validation (None: mIoU 0).  save_dir: results.txt and
+    results stay zeros); segval_loader: an iterable of seg validation batches for test.seg_validation, iterated again at every
+    validation (SegValBatches, mode='val' or 'testval'; None: mIoU 0).  save_dir: results.txt and
     weights/last.pt, best.pt go there.  ema: a ModelEMA of `model` (built here on rank -1 / 0 when None).  trainer_kwargs go to Trainer
     (seg_loss, process_group, det_shapes, ...).
 

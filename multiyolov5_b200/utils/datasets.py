@@ -12,6 +12,7 @@
         shapes) for test(data, model=m, dataloader=DetValLoader(cache, 32))                          :347-452 + :518-599 (rect=True)
     DeviceSegCache(images, masks, mask_map) / SegAugmenter(cache, base_size, crop_size, preset)(indices) -> (segimgs, segtargets)
                                                                              SegmentationDataset.py:118-151 + ColorJitter + ToTensor
+    SegAugmenter(...).val(indices, crop_size) / .testval(indices) -> (segimgs, segtargets)      :96-116 (mode='val') / :81-94 (testval)
 
 `img` is a uint8 HWC BGR frame (numpy array or torch tensor; a CPU input is uploaded as uint8 - 4x less than the fp32 the reference
 ships to the GPU); the resize (OpenCV's 8-bit INTER_LINEAR arithmetic, bit exact), the 114 border, the channel swap, the transpose and
@@ -852,8 +853,9 @@ class SegAugmenter:
     batch equals the reference's bit for bit.  The pixels are two kernel launches per batch on the current stream, after one pinned
     host-to-device copy of the parameters, without a device synchronisation.
 
-    `testval(indices)` gives the reference's mode='testval' items.  Not built: mode='val' (`_val_sync_transform`), which raises in every
-    reference loader because crop_size is a tuple there."""
+    `testval(indices)` gives the reference's mode='testval' items and `val(indices, crop_size)` its mode='val' items
+    (`_val_sync_transform`, with the int crop_size that train_citysbdd.py passes; the loaders' default tuple crop_size makes the
+    reference raise TypeError there)."""
 
     def __init__(self, cache, base_size=1024, crop_size=None, preset="citys", brightness=None, contrast=None, saturation=None, hue=None,
                  low=None, high=None, std=None):
@@ -980,3 +982,42 @@ class SegAugmenter:
         for b, i in enumerate(indices):
             items[b] = self._item(self.cache, i, False, ow, oh, 0, 0, ow, oh, W0, H0, [], [None] * 4, tables, mask_size=(W0, H0))
         return self._launch(items, tables, B, oh, ow, H0, W0, out_dtype)
+
+    def val(self, indices, crop_size, out_dtype=torch.float32):
+        """mode='val' items (`_val_sync_transform` + ToTensor, the item's mask map): (images (B, 3, c, c), labels (B, c, c) int64) with
+        c = crop_size.  Each item's short side is resized to c by Pillow's bilinear resize (the mask by NEAREST) and the c x c centre
+        crop taken (seg_val_geometry), so sources of different sizes share a batch.  Draws nothing from `random` or torch."""
+        c = seg_val_crop(crop_size)
+        if out_dtype not in (torch.uint8, torch.float16, torch.float32):
+            raise ValueError(f"SegAugmenter: out_dtype must be uint8, float16 or float32, got {out_dtype}")
+        B = len(indices)
+        items, tables = (_lib.SegItem * B)(), []
+        for b, i in enumerate(indices):
+            H0, W0 = self.cache.shapes[i]
+            ow, oh, x1, y1 = seg_val_geometry(W0, H0, c)
+            items[b] = self._item(self.cache, i, False, ow, oh, x1, y1, c, c, c, c, [], [None] * 4, tables)
+        return self._launch(items, tables, B, c, c, c, c, out_dtype)
+
+
+def seg_val_crop(crop_size):
+    """the int crop_size of mode='val'; a tuple (the default of get_citys_loader / get_citysbdd_loader, and what get_custom_loader always
+    passes) raises ValueError, where the reference's `_val_sync_transform` raises TypeError multiplying the tuple"""
+    if isinstance(crop_size, (tuple, list)):
+        raise ValueError(f"mode='val' needs an int crop_size, got {crop_size!r}: the reference's _val_sync_transform raises TypeError "
+                         "on a tuple crop_size (the default of get_citys_loader / get_citysbdd_loader and what get_custom_loader passes)")
+    if isinstance(crop_size, bool) or not isinstance(crop_size, (int, np.integer)) or crop_size <= 0:
+        raise ValueError(f"mode='val' needs a positive int crop_size, got {crop_size!r}")
+    return int(crop_size)
+
+
+def seg_val_geometry(w, h, crop):
+    """(ow, oh, x1, y1) of the reference's `_val_sync_transform` (SegmentationDataset.py:96-116) for a w x h source: the short side
+    resized to `crop` and the long side to int(1.0 * long * crop / short) (a square goes the portrait way), then the crop x crop centre
+    crop at int(round((ow - crop) / 2.)), Python's round half to even, and the same for y1"""
+    if w > h:
+        oh = crop
+        ow = int(1.0 * w * oh / h)
+    else:
+        ow = crop
+        oh = int(1.0 * h * ow / w)
+    return ow, oh, int(round((ow - crop) / 2.)), int(round((oh - crop) / 2.))
