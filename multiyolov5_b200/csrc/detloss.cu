@@ -72,6 +72,9 @@ __device__ __forceinline__ Cand decode_cand(const DetLossParams& P, int l, int c
   return c;
 }
 
+// share of d min(a, b) that goes to a: torch.min / torch.max (reference utils/general.py:358,368) split the gradient evenly at a tie
+__device__ __forceinline__ float min_share(float a, float b) { return a < b ? 1.0f : (a == b ? 0.5f : 0.0f); }
+
 __device__ __forceinline__ float warp_sum_f(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xFFFFFFFFu, v, o);
   return v;
@@ -140,15 +143,15 @@ __global__ void det_match_kernel(DetLossParams P) {
     const float g_iw = g_inter * ih, g_ih = g_inter * iw;
     const float g_iwr = iw_raw >= 0.f ? g_iw : 0.f, g_ihr = ih_raw >= 0.f ? g_ih : 0.f;
     float g_px1 = 0.f, g_px2 = 0.f, g_py1 = 0.f, g_py2 = 0.f;
-    if (px2 <= tx2) g_px2 += g_iwr;
-    if (px1 >= tx1) g_px1 -= g_iwr;
-    if (py2 <= ty2) g_py2 += g_ihr;
-    if (py1 >= ty1) g_py1 -= g_ihr;
+    g_px2 += g_iwr * min_share(px2, tx2);
+    g_px1 -= g_iwr * min_share(tx1, px1);
+    g_py2 += g_ihr * min_share(py2, ty2);
+    g_py1 -= g_ihr * min_share(ty1, py1);
     const float g_cw = g_c2 * 2.0f * cw, g_ch = g_c2 * 2.0f * ch;
-    if (px2 >= tx2) g_px2 += g_cw;
-    if (px1 <= tx1) g_px1 -= g_cw;
-    if (py2 >= ty2) g_py2 += g_ch;
-    if (py1 <= ty1) g_py1 -= g_ch;
+    g_px2 += g_cw * min_share(tx2, px2);
+    g_px1 -= g_cw * min_share(px1, tx1);
+    g_py2 += g_ch * min_share(ty2, py2);
+    g_py1 -= g_ch * min_share(py1, ty1);
     g_px1 += g_rho2 * (-0.5f * sx); g_px2 += g_rho2 * (-0.5f * sx);
     g_py1 += g_rho2 * (-0.5f * sy); g_py2 += g_rho2 * (-0.5f * sy);
     const float g_at1 = -(g_v * 2.0f * k4pi2 * dv);

@@ -206,7 +206,7 @@ class FusedComputeLoss:
             self._anchors_host = [float(v) for v in r.anchors.reshape(-1).tolist()]
             self._anchors_key = akey
         anchors = (C.c_float * (nl * na * 2))(*self._anchors_host)
-        balance = (C.c_float * nl)(*[float(b) for b in r.balance])
+        balance = (C.c_float * nl)(*[float(b) for b in r.balance[:nl]])     # below 3 levels ComputeLoss keeps a 5-entry list
         _lib.check(L.myolo_det_loss((vp * nl)(*[_lib.ptr(t) for t in p]), (vp * nl)(*[_lib.ptr(t) for t in dp]), _lib.ptr(targets),
                                     int(targets.shape[0]), B, na, no, nl, ny, nx, anchors, balance, float(r.hyp["box"]), float(r.hyp["obj"]),
                                     float(r.hyp["cls"]), float(r.hyp["anchor_t"]), float(r.gr), float(r.cp), float(r.cn), float(mult) * B,

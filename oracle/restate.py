@@ -555,85 +555,123 @@ def model_forward_train(cfg: dict, sd: Dict[str, torch.Tensor], x: torch.Tensor,
 # ------------------------------------------------------------------------------------------------
 # training losses (SURVEY.md section 8 row a13) - plain restatement, per-target Python loops; small cases only
 # ------------------------------------------------------------------------------------------------
-def ciou_xywh(pb: torch.Tensor, tb: torch.Tensor, eps: float = 1e-7) -> torch.Tensor:
-    """bbox_iou(box1.T, box2, x1y1x2y2=False, CIoU=True) of reference utils/general.py:343-380 for (n,4) xywh boxes."""
+DET_LOSS_MUTANTS = ("ties", "half_le", "gt_ge", "unclamped", "first_wins", "alpha_grad", "balance", "gr", "cp_cn")
+
+
+def ciou_xywh(pb: torch.Tensor, tb: torch.Tensor, eps: float = 1e-7, mutant: Optional[str] = None) -> torch.Tensor:
+    """bbox_iou(box1.T, box2, x1y1x2y2=False, CIoU=True) of reference utils/general.py:343-380 for (n,4) xywh boxes.  torch.min / torch.max
+    split the gradient evenly between equal arguments; mutant 'ties' gives all of it to the prediction's edge, 'alpha_grad' differentiates
+    through alpha."""
+    mn, mx = torch.min, torch.max
+    if mutant == "ties":
+        mn = lambda a, b: torch.where(a <= b, a, b)   # noqa: E731
+        mx = lambda a, b: torch.where(a >= b, a, b)   # noqa: E731
     px1, px2 = pb[:, 0] - pb[:, 2] / 2, pb[:, 0] + pb[:, 2] / 2
     py1, py2 = pb[:, 1] - pb[:, 3] / 2, pb[:, 1] + pb[:, 3] / 2
     tx1, tx2 = tb[:, 0] - tb[:, 2] / 2, tb[:, 0] + tb[:, 2] / 2
     ty1, ty2 = tb[:, 1] - tb[:, 3] / 2, tb[:, 1] + tb[:, 3] / 2
-    inter = (torch.min(px2, tx2) - torch.max(px1, tx1)).clamp(0) * (torch.min(py2, ty2) - torch.max(py1, ty1)).clamp(0)   # :358-359
+    inter = (mn(px2, tx2) - mx(px1, tx1)).clamp(0) * (mn(py2, ty2) - mx(py1, ty1)).clamp(0)                                # :358-359
     w1, h1 = px2 - px1, py2 - py1 + eps                                                                                    # :362
     w2, h2 = tx2 - tx1, ty2 - ty1 + eps                                                                                    # :363
     union = w1 * h1 + w2 * h2 - inter + eps
     iou = inter / union
-    cw = torch.max(px2, tx2) - torch.min(px1, tx1)
-    ch = torch.max(py2, ty2) - torch.min(py1, ty1)
+    cw = mx(px2, tx2) - mn(px1, tx1)
+    ch = mx(py2, ty2) - mn(py1, ty1)
     c2 = cw ** 2 + ch ** 2 + eps
     rho2 = ((tx1 + tx2 - px1 - px2) ** 2 + (ty1 + ty2 - py1 - py2) ** 2) / 4
     v = (4 / math.pi ** 2) * torch.pow(torch.atan(w2 / h2) - torch.atan(w1 / h1), 2)
-    with torch.no_grad():
+    with torch.set_grad_enabled(mutant == "alpha_grad" and torch.is_grad_enabled()):
         alpha = v / (v - iou + (1 + eps))                                                                                  # :378-379
     return iou - (rho2 / c2 + v * alpha)
 
 
-def build_targets_loop(shapes, targets: np.ndarray, anchors: np.ndarray, anchor_t: float):
+def _near(v, mutant: Optional[str] = None) -> bool:
+    """the neighbouring cell on this side is the nearer one: v % 1 < 0.5 and v > 1 (reference utils/loss.py:193-194); mutants 'half_le' and
+    'gt_ge' make either comparison inclusive"""
+    half = v % 1.0 <= 0.5 if mutant == "half_le" else v % 1.0 < 0.5
+    inside = v >= 1.0 if mutant == "gt_ge" else v > 1.0
+    return bool(half and inside)
+
+
+def build_targets_loop(shapes, targets: np.ndarray, anchors: np.ndarray, anchor_t: float, mutant: Optional[str] = None):
     """ComputeLoss.build_targets (reference utils/loss.py:164-217) as explicit loops.  shapes[i] = (ny, nx); anchors (nl, na, 2) in grid
-    units.  Returns per level a list of (img, anchor, gj, gi, tbox(4), cls) in the reference's candidate order: the 5 offsets
-    (centre, x-1, y-1, x+1, y+1) outermost, then anchors, then targets."""
+    units.  Returns per level a list of (img, anchor, gj, gi, tbox(4), cls, cand) in the reference's candidate order: the 5 offsets
+    (centre, x-1, y-1, x+1, y+1) outermost, then anchors, then targets; cand = (offset * na + anchor) * nt + target numbers them in that
+    order.  Mutant 'unclamped' takes the box offset relative to the unclamped cell; 'half_le' and 'gt_ge' are those of _near."""
     out = []
+    nt, na = len(targets), anchors.shape[1]
     offs = np.array([[0, 0], [1, 0], [0, 1], [-1, 0], [0, -1]], np.float32) * np.float32(0.5)
     for i, (ny, nx) in enumerate(shapes):
         gain = np.array([nx, ny], np.float32)
-        kept = []     # (anchor index, scaled target row)
-        for a in range(anchors.shape[1]):
-            for t in targets:
+        kept = []     # (anchor index, target index, scaled target row)
+        for a in range(na):
+            for ti, t in enumerate(targets):
                 gxy = t[2:4] * gain
                 gwh = t[4:6] * gain
                 r = gwh / anchors[i, a]
                 if max(np.maximum(r, np.float32(1.0) / r)) < anchor_t:                         # :185-186
-                    kept.append((a, int(t[0]), int(t[1]), gxy.astype(np.float32), gwh.astype(np.float32)))
+                    kept.append((a, ti, int(t[0]), int(t[1]), gxy.astype(np.float32), gwh.astype(np.float32)))
         rows = []
         for k in range(5):
-            for (a, img, cls, gxy, gwh) in kept:
+            for (a, ti, img, cls, gxy, gwh) in kept:
                 gxi = gain - gxy
                 if k == 0:
                     sel = True
                 elif k == 1:
-                    sel = (gxy[0] % 1.0 < 0.5) and (gxy[0] > 1.0)                              # j  :193
+                    sel = _near(gxy[0], mutant)                                                # j  :193
                 elif k == 2:
-                    sel = (gxy[1] % 1.0 < 0.5) and (gxy[1] > 1.0)                              # k
+                    sel = _near(gxy[1], mutant)                                                # k
                 elif k == 3:
-                    sel = (gxi[0] % 1.0 < 0.5) and (gxi[0] > 1.0)                              # l  :194
+                    sel = _near(gxi[0], mutant)                                                # l  :194
                 else:
-                    sel = (gxi[1] % 1.0 < 0.5) and (gxi[1] > 1.0)                              # m
+                    sel = _near(gxi[1], mutant)                                                # m
                 if not sel:
                     continue
                 gij = (gxy - offs[k]).astype(np.int64)                                         # .long() truncation :206
                 gi = int(min(max(gij[0], 0), nx - 1))
                 gj = int(min(max(gij[1], 0), ny - 1))
                 # gj/gi are VIEWS of gij and clamp_ is in place (:211), so the box offset (:212) is relative to the CLAMPED cell
-                tb = np.concatenate([gxy - np.array([gi, gj], np.float32), gwh]).astype(np.float32)
-                rows.append((img, a, gj, gi, tb, cls))
+                ci = gij if mutant == "unclamped" else np.array([gi, gj])
+                tb = np.concatenate([gxy - ci.astype(np.float32), gwh]).astype(np.float32)
+                rows.append((img, a, gj, gi, tb, cls, (k * na + a) * nt + ti))
         out.append(rows)
     return out
 
 
 def bce_logits(x: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
-    """nn.BCEWithLogitsLoss(pos_weight=1) elementwise"""
-    return x.clamp(min=0) - x * t + torch.log1p(torch.exp(-x.abs()))
+    """nn.BCEWithLogitsLoss(pos_weight=1) elementwise, ATen's formula.  Its autograd gradient is sigmoid(x) - t everywhere, as the
+    loss's own backward; that of max(x, 0) - x t + log1p(exp(-|x|)) is 1 - t at x = 0, where clamp and abs meet their kinks."""
+    return (1 - t) * x - F.logsigmoid(x)
 
 
-def compute_det_loss(p: List[torch.Tensor], targets: np.ndarray, anchors: np.ndarray, hyp: dict, nc: int, gr: float = 1.0):
-    """ComputeLoss.__call__ (reference utils/loss.py:115-162), fl_gamma = 0, label smoothing from hyp.  p[i]: (B, na, ny, nx, 5+nc).
-    Returns (loss * batch, items[lbox, lobj, lcls, loss])."""
+def compute_det_loss(p: List[torch.Tensor], targets: np.ndarray, anchors: np.ndarray, hyp: dict, nc: int, gr: float = 1.0,
+                     assignment: bool = False, mutant: Optional[str] = None):
+    """ComputeLoss.__call__ (reference utils/loss.py:115-162), fl_gamma = 0, label smoothing from hyp.  p[i]: (B, na, ny, nx, 5+nc),
+    any number of levels.  The decisions are the reference's float32 ones (build_targets_loop); the arithmetic is in the dtype of p, so
+    float64 p makes this the fp64 yardstick of the fused loss.  Returns (loss * batch, items[lbox, lobj, lcls, loss]) and, with
+    assignment=True, per level (number of valid candidates, (B, na, ny, nx) int64 array of the last valid candidate of every cell or -1,
+    the objectness targets).
+    `mutant` (one of DET_LOSS_MUTANTS) makes it deliberately wrong in one place, for tests that show their limits catch such errors:
+    'first_wins' lets the first candidate of a cell set its objectness target, 'balance' takes the other branch of the per-level
+    balance lookup, 'gr' ignores gr, 'cp_cn' swaps the smoothed class targets; the others are those of ciou_xywh and build_targets_loop."""
     eps_ls = hyp.get("label_smoothing", 0.0)
     cp, cn = 1.0 - 0.5 * eps_ls, 0.5 * eps_ls
-    balance = [4.0, 1.0, 0.4]
+    if mutant == "cp_cn":
+        cp, cn = cn, cp
+    if mutant == "gr":
+        gr = 1.0
+    nl = len(p)
+    balance = {3: [4.0, 1.0, 0.4]}.get(nl, [4.0, 1.0, 0.25, 0.06, 0.02])                                      # :104
+    if mutant == "balance":
+        balance = [4.0, 1.0, 0.25, 0.06, 0.02] if nl == 3 else [4.0, 1.0, 0.4]
     shapes = [(pi.shape[2], pi.shape[3]) for pi in p]
-    cand = build_targets_loop(shapes, targets, anchors, hyp["anchor_t"])
-    lbox = torch.zeros(1); lobj = torch.zeros(1); lcls = torch.zeros(1)
+    cand = build_targets_loop(shapes, targets, anchors, hyp["anchor_t"], mutant)
+    dt = p[0].dtype
+    lbox = torch.zeros(1, dtype=dt); lobj = torch.zeros(1, dtype=dt); lcls = torch.zeros(1, dtype=dt)
+    assigned = []
     for i, pi in enumerate(p):
-        tobj = torch.zeros(pi.shape[:4])
+        tobj = torch.zeros(pi.shape[:4], dtype=dt)
+        winner = np.full(pi.shape[:4], -1, np.int64)
         rows = cand[i]
         if rows:
             b = torch.tensor([r[0] for r in rows]); a = torch.tensor([r[1] for r in rows])
@@ -643,19 +681,23 @@ def compute_det_loss(p: List[torch.Tensor], targets: np.ndarray, anchors: np.nda
             ps = pi[b, a, gj, gi]
             pxy = ps[:, :2].sigmoid() * 2.0 - 0.5
             pwh = (ps[:, 2:4].sigmoid() * 2) ** 2 * torch.from_numpy(anchors[i])[a]
-            iou = ciou_xywh(torch.cat((pxy, pwh), 1), tb)
+            iou = ciou_xywh(torch.cat((pxy, pwh), 1), tb, mutant=mutant)
             lbox = lbox + (1.0 - iou).mean()
             vals = (1.0 - gr) + gr * iou.detach().clamp(0)
-            for r in range(len(rows)):                     # sequential writes: the last candidate of a cell wins (CPU index_put_)
+            order = range(len(rows)) if mutant != "first_wins" else reversed(range(len(rows)))
+            for r in order:                                # sequential writes: the last candidate of a cell wins (CPU index_put_)
                 tobj[b[r], a[r], gj[r], gi[r]] = vals[r]
+                winner[rows[r][0], rows[r][1], rows[r][2], rows[r][3]] = rows[r][6]
             if nc > 1:
                 t = torch.full_like(ps[:, 5:], cn)
                 t[torch.arange(len(rows)), tc] = cp
                 lcls = lcls + bce_logits(ps[:, 5:], t).mean()
         lobj = lobj + bce_logits(pi[..., 4], tobj).mean() * balance[i]
+        assigned.append((len(rows), winner, tobj))
     lbox = lbox * hyp["box"]; lobj = lobj * hyp["obj"]; lcls = lcls * hyp["cls"]
     loss = lbox + lobj + lcls
-    return loss * p[0].shape[0], torch.cat((lbox, lobj, lcls, loss)).detach()
+    out = loss * p[0].shape[0], torch.cat((lbox, lobj, lcls, loss)).detach()
+    return (*out, assigned) if assignment else out
 
 
 def seg_ce_loss(seg: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:

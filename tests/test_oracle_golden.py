@@ -116,6 +116,17 @@ def test_det_loss_product_matches_reference(name):
         assert np.abs(p[i].grad.numpy() - ref).max() <= 1e-5 * np.abs(ref).max()
 
 
+def test_bce_restatement_matches_the_loss_and_its_gradient_at_kinks():
+    """restate.bce_logits equals nn.BCEWithLogitsLoss bit for bit and its autograd gradient is sigmoid(x) - t, BCEWithLogitsLoss's own
+    backward, also at x = 0 and at the softplus threshold"""
+    x = torch.tensor([0.0, 0.0, 20.0, -20.0, 90.0, -90.0, 0.3], dtype=torch.float64, requires_grad=True)
+    t = torch.tensor([0.0, 0.95, 1.0, 0.05, 0.5, 0.0, 0.2], dtype=torch.float64)
+    loss = restate.bce_logits(x, t)
+    assert torch.equal(loss, torch.nn.functional.binary_cross_entropy_with_logits(x, t, reduction="none"))
+    loss.sum().backward()
+    assert torch.allclose(x.grad, torch.sigmoid(x.detach()) - t, rtol=0, atol=1e-15), x.grad - (torch.sigmoid(x.detach()) - t)
+
+
 def test_seg_loss_matches_reference():
     from multiyolov5_b200.utils.loss import SegmentationLosses
     g, _ = _loss_fixture()
