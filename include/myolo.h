@@ -500,12 +500,24 @@ int myolo_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int mw
  * myolo_seg_lut_blend: out[i][c] = lut[class_map[i]][c] (label2image / trainid2id, reference detect.py:69-77; reverse_channels gives the
  * BGR order of detect.py:193) and, if `blend` is given, blend[i][c] = cv2.addWeighted(out, alpha, image, beta, 0) (detect.py:194).
  * class_map: uint8 or int64 (dtype code); lut: device (n_entries x channels) uint8; out / blend: (n_pixels x channels) uint8, each nullable.
+ * lut2 / out2 (nullable): a second table (n_entries x channels2, read in its own channel order) written to out2 (n_pixels x channels2)
+ * from the same read of the class map: detect.py's mask, blend and trainid2id ids (detect.py:193-194,206) in one pass.
  * myolo_seg_metrics: the counters of utils/metrics.py:234-275 from a class map and int64 labels (-1 = ignore), ACCUMULATED into
  * counters[2 + 3*n_classes] (device uint64): [correct, labeled, intersection[n], prediction area[n], label area[n]]. */
 int myolo_seg_lut_blend(const void* class_map, int map_dtype, int64_t n_pixels, const uint8_t* lut, int n_entries, int channels,
-                        int reverse_channels, uint8_t* out, const uint8_t* image, float alpha, float beta, uint8_t* blend, void* stream);
+                        int reverse_channels, uint8_t* out, const uint8_t* image, float alpha, float beta, uint8_t* blend,
+                        const uint8_t* lut2, int channels2, uint8_t* out2, void* stream);
 int myolo_seg_metrics(const void* pred, int pred_dtype, const int64_t* target, int64_t n_pixels, int n_classes, uint64_t* counters,
                       void* stream);
+
+/* ---- detect.py's boxes in frame space (reference detect.py:166-177; multiyolov5_b200/detect.py) ----
+ * myolo_detect_boxes: for each of B frames, rows [0, counts[b]) of the padded NMS output rows (B, max_det, 6) fp32 are scaled IN PLACE to
+ * the frame: scale_coords(img_shape, rows[:, :4], im0_shape).round() (x -= pad, x /= gain, clamp to [0, w0] / [0, h0], round half to
+ * even), in fp32 IEEE arithmetic, equal to torch's CPU statements.  geom: device (B, 5) fp32 {pad_x, pad_y, gain, w0, h0}, the Python
+ * scalars of scale_coords rounded to fp32.  xywhn (nullable): (B, max_det, 4) fp32, xyxy2xywh(box) / (w0, h0, w0, h0) of --save-txt.
+ * class_counts (nullable): (B, nc) int32, each frame's rows per class id (ids that are not an integer in [0, nc) are not counted). */
+int myolo_detect_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, int nc, float* xywhn,
+                       int32_t* class_counts, void* stream);
 
 /* ---- detection validation statistics (reference test.py:175,183-265 and utils/metrics.py:24-112; multiyolov5_b200/utils/metrics.py
  * DetectionStats) ----

@@ -42,7 +42,7 @@ EXPORTS = [
     "myolo_anchor_metric", "myolo_anchor_metric_workspace_bytes", "myolo_anchor_evolve", "myolo_anchor_evolve_workspace_bytes",
     "myolo_kmeans", "myolo_kmeans_workspace_bytes", "myolo_class_weights", "myolo_image_weights", "myolo_weighted_draw",
     "myolo_plan_backward_seg_loss", "myolo_seg_focal_loss", "myolo_seg_focal_loss_backward", "myolo_seg_focal_loss_workspace_bytes",
-    "myolo_conv_backward", "myolo_conv_forward", "myolo_plan_forward_pass", "myolo_scale_img",
+    "myolo_conv_backward", "myolo_conv_forward", "myolo_plan_forward_pass", "myolo_scale_img", "myolo_detect_boxes",
 ]
 REDUCTION_MEAN, REDUCTION_SUM = 0, 1        # include/myolo.h: MYOLO_REDUCTION_* of myolo_seg_focal_loss
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
@@ -139,7 +139,8 @@ def lib():
     L.myolo_augment_det_hw.argtypes = [vp, i32, i32, i32, vp, i32, vp]
     L.myolo_collate_quad.argtypes = [vp, i32, i32, i32, vp, vp, i32, vp]
     L.myolo_augment_seg.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp]
-    L.myolo_seg_lut_blend.argtypes = [vp, i32, i64, vp, i32, i32, i32, vp, vp, f32, f32, vp, vp]
+    L.myolo_seg_lut_blend.argtypes = [vp, i32, i64, vp, i32, i32, i32, vp, vp, f32, f32, vp, vp, i32, vp, vp]
+    L.myolo_detect_boxes.argtypes = [vp, vp, i32, i32, vp, i32, vp, vp, vp]
     L.myolo_seg_metrics.argtypes = [vp, i32, vp, i64, i32, vp, vp]
     L.myolo_det_match.argtypes = [vp, vp, i32, i32, vp, i32, i32, i32, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp]
     L.myolo_det_ap_workspace_bytes.argtypes = [i32, i32, i32]

@@ -10,11 +10,16 @@ __device__ __forceinline__ int load_cls(const void* p, int dtype, long i) {
   return dtype == MYOLO_U8 ? (int)reinterpret_cast<const unsigned char*>(p)[i] : (int)reinterpret_cast<const long long*>(p)[i];
 }
 
-// out[i][c] = lut[idx[i]][reverse ? ch-1-c : c];  optional blend: dst[i][c] = sat(rint(out*alpha + im[i][c]*beta))  (fp32, round half even)
+// out[i][c] = lut[idx[i]][reverse ? ch-1-c : c];  optional blend: dst[i][c] = sat(rint(out*alpha + im[i][c]*beta))  (fp32, round half even);
+// optional second table: out2[i][c] = lut2[idx[i]][c] (same entries, ch2 channels, its own order), from the same class-map read
 __global__ void lut_blend_kernel(const void* idx, int idx_dtype, long n, const unsigned char* __restrict__ lut, int n_entries, int ch,
-                                 int reverse, unsigned char* out, const unsigned char* im, float alpha, float beta, unsigned char* blend) {
+                                 int reverse, unsigned char* out, const unsigned char* im, float alpha, float beta, unsigned char* blend,
+                                 const unsigned char* __restrict__ lut2, int ch2, unsigned char* out2) {
   extern __shared__ unsigned char s_lut[];
+  unsigned char* s_lut2 = s_lut + n_entries * ch;
   for (int k = threadIdx.x; k < n_entries * ch; k += blockDim.x) s_lut[k] = lut[k];
+  if (out2)
+    for (int k = threadIdx.x; k < n_entries * ch2; k += blockDim.x) s_lut2[k] = lut2[k];
   __syncthreads();
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
     int v = load_cls(idx, idx_dtype, i);
@@ -27,16 +32,71 @@ __global__ void lut_blend_kernel(const void* idx, int idx_dtype, long n, const u
         blend[i * ch + c] = (unsigned char)min(max(__float2int_rn(r), 0), 255);
       }
     }
+    if (out2)
+      for (int c = 0; c < ch2; ++c) out2[i * ch2 + c] = s_lut2[v * ch2 + c];
   }
 }
 
 int launch_lut_blend(const void* idx, int idx_dtype, long n, const unsigned char* lut, int n_entries, int ch, int reverse, unsigned char* out,
-                     const unsigned char* im, float alpha, float beta, unsigned char* blend, cudaStream_t s) {
-  MYOLO_REQUIRE(idx && lut && n > 0 && n_entries > 0 && ch > 0 && n_entries * ch <= 4096 && (out || blend) && (!blend || im),
+                     const unsigned char* im, float alpha, float beta, unsigned char* blend, const unsigned char* lut2, int ch2,
+                     unsigned char* out2, cudaStream_t s) {
+  MYOLO_REQUIRE(idx && lut && n > 0 && n_entries > 0 && ch > 0 && n_entries * ch <= 4096 && (out || blend || out2) && (!blend || im),
                 "lut_blend: bad arguments");
+  MYOLO_REQUIRE(!out2 || (lut2 && ch2 > 0 && n_entries * ch2 <= 4096), "lut_blend: the second table needs lut2 and 0 < channels2");
   MYOLO_REQUIRE(idx_dtype == MYOLO_U8 || idx_dtype == MYOLO_I64, "lut_blend: class map must be uint8 or int64");
-  lut_blend_kernel<<<(int)std::min<long>(132L * 8, (n + 255) / 256), 256, n_entries * ch, s>>>(idx, idx_dtype, n, lut, n_entries, ch, reverse, out,
-                                                                                              im, alpha, beta, blend);
+  const int smem = n_entries * (ch + (out2 ? ch2 : 0));
+  lut_blend_kernel<<<(int)std::min<long>(132L * 8, (n + 255) / 256), 256, smem, s>>>(idx, idx_dtype, n, lut, n_entries, ch, reverse, out, im,
+                                                                                     alpha, beta, blend, lut2, out2 ? ch2 : 0, out2);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+// detect.py:166-177 over a batch of padded NMS rows, one CTA per frame.  geom[b] = {pad_x, pad_y, gain, w0, h0}, each already rounded to
+// fp32 as torch's CPU kernels round a Python scalar.  In place on rows [0, counts[b]): x -= pad, x /= gain, clamp to the frame, round half to
+// even (scale_coords(...).round(), fp32 IEEE like the reference's CPU run).  xywhn (nullable): (xyxy2xywh(xyxy) / gn) of the rounded box.
+// class_counts (nullable): (B, nc) rows per integral class id in [0, nc).
+__global__ void detect_boxes_kernel(float* rows, const int32_t* counts, int max_det, const float* geom, int nc, float* xywhn,
+                                    int32_t* class_counts) {
+  extern __shared__ int s_cnt[];
+  const int b = blockIdx.x;
+  const float px = geom[b * 5 + 0], py = geom[b * 5 + 1], gain = geom[b * 5 + 2], w0 = geom[b * 5 + 3], h0 = geom[b * 5 + 4];
+  if (class_counts)
+    for (int k = threadIdx.x; k < nc; k += blockDim.x) s_cnt[k] = 0;
+  __syncthreads();
+  const int n = min(max(counts[b], 0), max_det);
+  for (int r = threadIdx.x; r < n; r += blockDim.x) {
+    float* row = rows + ((long)b * max_det + r) * 6;
+    float v[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float lim = (j & 1) ? h0 : w0;
+      const float x = __fdiv_rn(__fsub_rn(row[j], (j & 1) ? py : px), gain);
+      v[j] = rintf(fminf(fmaxf(x, 0.f), lim));
+      row[j] = v[j];
+    }
+    if (xywhn) {
+      float* o = xywhn + ((long)b * max_det + r) * 4;
+      o[0] = __fdiv_rn(__fmul_rn(__fadd_rn(v[0], v[2]), 0.5f), w0);
+      o[1] = __fdiv_rn(__fmul_rn(__fadd_rn(v[1], v[3]), 0.5f), h0);
+      o[2] = __fdiv_rn(__fsub_rn(v[2], v[0]), w0);
+      o[3] = __fdiv_rn(__fsub_rn(v[3], v[1]), h0);
+    }
+    if (class_counts) {
+      const float c = row[5];
+      if (c >= 0.f && c < (float)nc && c == truncf(c)) atomicAdd(&s_cnt[(int)c], 1);
+    }
+  }
+  if (class_counts) {
+    __syncthreads();
+    for (int k = threadIdx.x; k < nc; k += blockDim.x) class_counts[(long)b * nc + k] = s_cnt[k];
+  }
+}
+
+int launch_detect_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, int nc, float* xywhn, int32_t* class_counts,
+                        cudaStream_t s) {
+  MYOLO_REQUIRE(rows && counts && geom && B > 0 && max_det > 0, "detect_boxes: bad arguments");
+  MYOLO_REQUIRE(!class_counts || (nc > 0 && nc <= 4096), "detect_boxes: class counts need 0 < nc <= 4096");
+  detect_boxes_kernel<<<B, 128, class_counts ? nc * (int)sizeof(int) : 0, s>>>(rows, counts, max_det, geom, nc, xywhn, class_counts);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }

@@ -57,7 +57,10 @@ int launch_det_ap(const uint16_t* correct, const float* conf, const uint8_t* cls
 
 // seg output consumers (consumers.cu)
 int launch_lut_blend(const void* idx, int idx_dtype, long n, const unsigned char* lut, int n_entries, int ch, int reverse, unsigned char* out,
-                     const unsigned char* im, float alpha, float beta, unsigned char* blend, cudaStream_t s);
+                     const unsigned char* im, float alpha, float beta, unsigned char* blend, const unsigned char* lut2, int ch2,
+                     unsigned char* out2, cudaStream_t s);
+int launch_detect_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, int nc, float* xywhn, int32_t* class_counts,
+                        cudaStream_t s);
 int launch_seg_hist(const void* pred, int pred_dtype, const long long* target, long n, int n_cls, unsigned long long* counters, cudaStream_t s);
 
 // autoanchor (autoanchor.cu): the ratio metric and the cooperative genetic evolution

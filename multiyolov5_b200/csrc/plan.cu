@@ -1508,11 +1508,18 @@ extern "C" int myolo_augment_seg(myolo_seg_item* items, int B, int h, int w, int
 
 extern "C" int myolo_seg_lut_blend(const void* class_map, int map_dtype, int64_t n_pixels, const uint8_t* lut, int n_entries, int channels,
                                    int reverse_channels, uint8_t* out, const uint8_t* image, float alpha, float beta, uint8_t* blend,
-                                   void* stream) {
+                                   const uint8_t* lut2, int channels2, uint8_t* out2, void* stream) {
   int rc = check_device(nullptr);
   if (rc) return rc;
   return launch_lut_blend(class_map, map_dtype, (long)n_pixels, lut, n_entries, channels, reverse_channels, out, image, alpha, beta, blend,
-                          (cudaStream_t)stream);
+                          lut2, channels2, out2, (cudaStream_t)stream);
+}
+
+extern "C" int myolo_detect_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, int nc, float* xywhn,
+                                  int32_t* class_counts, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_detect_boxes(rows, counts, B, max_det, geom, nc, xywhn, class_counts, (cudaStream_t)stream);
 }
 
 extern "C" int myolo_seg_metrics(const void* pred, int pred_dtype, const int64_t* target, int64_t n_pixels, int n_classes, uint64_t* counters,

@@ -258,7 +258,7 @@ def _lut(table, device):
     return _lut_cache[key]
 
 
-def _lut_call(pred, table, reverse, image=None, alpha=0.0, beta=0.0, want_out=True):
+def _lut_call(pred, table, reverse, image=None, alpha=0.0, beta=0.0, want_out=True, table2=None):
     assert pred.is_cuda and pred.dtype in (torch.uint8, torch.int64), "class map: CUDA uint8 / int64 tensor"
     pred = pred.contiguous()
     lut = _lut(table, pred.device)
@@ -269,10 +269,15 @@ def _lut_call(pred, table, reverse, image=None, alpha=0.0, beta=0.0, want_out=Tr
         image = image.contiguous()
         assert image.dtype == torch.uint8 and tuple(image.shape) == tuple(pred.shape) + (ch,) and image.is_cuda
         blend = torch.empty_like(image)
+    lut2 = out2 = None
+    if table2 is not None:
+        lut2 = _lut(table2, pred.device)
+        assert lut2.shape[0] == n_entries, "the second table needs as many entries as the first"
+        out2 = torch.empty(tuple(pred.shape) + (lut2.shape[1],), dtype=torch.uint8, device=pred.device)
     _lib.check(_lib.lib().myolo_seg_lut_blend(_lib.ptr(pred), _lib.torch_dtype_code(pred.dtype), pred.numel(), _lib.ptr(lut), n_entries, ch,
                                               int(reverse), _lib.ptr(out), _lib.ptr(image), float(alpha), float(beta), _lib.ptr(blend),
-                                              _lib.stream_ptr()))
-    return out, blend
+                                              _lib.ptr(lut2), 0 if lut2 is None else lut2.shape[1], _lib.ptr(out2), _lib.stream_ptr()))
+    return (out, blend) if table2 is None else (out, blend, out2)
 
 
 def label2image(pred, COLORMAP=Cityscapes_COLORMAP):
@@ -285,7 +290,68 @@ def trainid2id(pred, IDMAP=Cityscapes_IDMAP):
     return _lut_call(pred, IDMAP, False)[0]
 
 
+def seg_products(pred, im0=None, mask=True, ids=False, COLORMAP=Cityscapes_COLORMAP, IDMAP=Cityscapes_IDMAP, alpha=0.4, beta=0.6):
+    """detect.py:193-194,206 in one pass over the class map: the BGR `mask`, the blend cv2.addWeighted(mask, alpha, im0, beta, 0) when
+    im0 is given and the trainid2id label `ids` (H,W,1), each only when asked for.  pred: (..., H, W) uint8 / int64 class map, im0:
+    (..., H, W, 3) uint8 BGR frames, both on the GPU.  Returns (mask, dst, ids), None for each product not asked for."""
+    if not (mask or im0 is not None or ids):
+        raise ValueError("seg_products: ask for at least one of mask, blend (im0) and ids")
+    out = _lut_call(pred, COLORMAP, True, image=im0, alpha=alpha, beta=beta, want_out=mask, table2=IDMAP if ids else None)
+    return out if ids else out + (None,)
+
+
 def seg_overlay(pred, im0, COLORMAP=Cityscapes_COLORMAP, alpha=0.4, beta=0.6):
     """detect.py:193-194 in one kernel: mask = label2image(pred)[:, :, ::-1] (BGR) and dst = cv2.addWeighted(mask, alpha, im0, beta, 0).
     pred: (H,W) class map, im0: (H,W,3) uint8 BGR frame, both on the GPU.  Returns (mask, dst)."""
     return _lut_call(pred, COLORMAP, True, image=im0, alpha=alpha, beta=beta)
+
+
+# ---- detect.py (reference utils/general.py:123-128,594-604; detect.py:166-177) ----
+def check_img_size(img_size, s=32):
+    """reference utils/general.py:123-128: img_size rounded up to a multiple of the stride s, with the reference's warning"""
+    from ..models.yolo import make_divisible
+    new_size = make_divisible(img_size, int(s))
+    if new_size != img_size:
+        print("WARNING: --img-size %g must be multiple of max stride %g, updating to %g" % (img_size, s, new_size))
+    return new_size
+
+
+def increment_path(path, exist_ok=True, sep=""):
+    """reference utils/general.py:594-604: runs/exp stays runs/exp when it is free (or exist_ok), else runs/exp{sep}N for one more than
+    the largest N already there (2 when there is none)"""
+    import glob
+    import re
+    from pathlib import Path
+    path = Path(path)
+    if (path.exists() and exist_ok) or (not path.exists()):
+        return str(path)
+    dirs = glob.glob(f"{path}{sep}*")
+    matches = [re.search(rf"%s{sep}(\d+)" % path.stem, d) for d in dirs]
+    i = [int(m.groups()[0]) for m in matches if m]
+    n = max(i) + 1 if i else 2
+    return f"{path}{sep}{n}"
+
+
+def scale_coords_geometry(img1_shape, img0_shape):
+    """the Python scalars of scale_coords(img1_shape, ., img0_shape) (float64, the reference's order) rounded to fp32 as torch's CPU
+    kernels round a scalar operand: float32 (B=1, 5) row {pad_x, pad_y, gain, w0, h0} of myolo_detect_boxes"""
+    gain = min(img1_shape[0] / img0_shape[0], img1_shape[1] / img0_shape[1])
+    pad = (img1_shape[1] - img0_shape[1] * gain) / 2, (img1_shape[0] - img0_shape[0] * gain) / 2
+    return np.array([pad[0], pad[1], gain, img0_shape[1], img0_shape[0]], np.float32)
+
+
+def detect_boxes(rows, counts, geom, nc=None, xywhn=False):
+    """detect.py:166-177 for a batch in one launch: rows (B, max_det, 6) fp32 CUDA padded NMS rows (non_max_suppression(...,
+    return_padded=True)) and counts (B,) int32 -> rows[b, :counts[b], :4] = scale_coords(...).round() IN PLACE, bit for bit torch's CPU
+    fp32.  geom: (B, 5) fp32 rows of scale_coords_geometry (host or device).  Returns (xywhn, class_counts): the (B, max_det, 4)
+    normalised xywh of --save-txt when xywhn, the (B, nc) int32 per-class row counts of the printed line when nc is given; None otherwise."""
+    if not (rows.is_cuda and rows.dtype == torch.float32 and rows.is_contiguous() and rows.dim() == 3 and rows.shape[2] == 6):
+        raise _lib.MyoloError("detect_boxes needs contiguous (B, max_det, 6) fp32 CUDA rows")
+    B, max_det, _ = rows.shape
+    counts = counts.to(device=rows.device, dtype=torch.int32).contiguous()
+    geom = torch.as_tensor(geom, dtype=torch.float32).reshape(B, 5).to(rows.device, non_blocking=True).contiguous()
+    wh = torch.empty((B, max_det, 4), dtype=torch.float32, device=rows.device) if xywhn else None
+    cc = torch.empty((B, int(nc)), dtype=torch.int32, device=rows.device) if nc is not None else None
+    _lib.check(_lib.lib().myolo_detect_boxes(_lib.ptr(rows), _lib.ptr(counts), B, max_det, _lib.ptr(geom), 0 if nc is None else int(nc),
+                                             _lib.ptr(wh), _lib.ptr(cc), _lib.stream_ptr()))
+    return wh, cc
