@@ -407,6 +407,24 @@ int myolo_allreduce_grads(float* flat_grad, int64_t n, void* nccl_comm, void* st
 int myolo_letterbox(const uint8_t* src, int B, int H0, int W0, int resized_w, int resized_h, int top, int left, int H, int W,
                     const int32_t* pad_bgr, void* out, int out_dtype, int chw, int swap_rb, void* stream);
 
+/* ---- autoShape's pre-process of a ragged batch (reference models/common.py:636-658) ----
+ * myolo_letterbox_items: B RGB uint8 HWC sources of different sizes, packed in one device buffer `src`, each letterboxed to the shared
+ * H x W (`letterbox(im, new_shape=shape1, auto=False)`, cv2.resize INTER_LINEAR bit exact with OpenCV's 8-bit path, border 114, no
+ * channel swap) into out (B,3,H,W): MYOLO_U8, or MYOLO_F16 / MYOLO_F32 holding value / 255 as torch's CPU division of
+ * `.type_as(p) / 255.` gives.  items: DEVICE array of B myolo_letterbox_item built on the host (multiyolov5_b200/utils/datasets.py
+ * letterbox_item_table); the kernel trusts its geometry (top + rh <= H, left + rw <= W, sources inside src). */
+typedef struct {
+  int64_t offset;            /* byte offset of the item's (H0, W0, 3) source in src */
+  double scale_x, scale_y;   /* cv2's 1 / (rw / W0) and 1 / (rh / H0), in double */
+  int32_t H0, W0;
+  int32_t mode;              /* 0: copy (rw == W0 and rh == H0), 1: bilinear, 2: exact 2x down-scale (cv2's 2x2 area mean) */
+  int32_t rw, rh;            /* resized (un-padded) size */
+  int32_t top, left;         /* border offsets inside H x W */
+  int32_t reserved;
+} myolo_letterbox_item;
+int myolo_letterbox_items(const uint8_t* src, const myolo_letterbox_item* items, int B, int H, int W, void* out, int out_dtype,
+                          void* stream);
+
 /* ---- detection training batches (reference utils/datasets.py:518-593 LoadImagesAndLabels.__getitem__, augment=True) ----
  * myolo_resize_u8: cv2.resize(src, (W, H), INTER_LINEAR) of one uint8 HWC image (H0,W0,3) into dst (H,W,3), bit exact with OpenCV's
  * 8-bit path (exact 2x down-scaling takes its area path): `load_image`'s resize to long side img_size (:629-643) for the device cache.
@@ -518,6 +536,13 @@ int myolo_seg_metrics(const void* pred, int pred_dtype, const int64_t* target, i
  * class_counts (nullable): (B, nc) int32, each frame's rows per class id (ids that are not an integer in [0, nc) are not counted). */
 int myolo_detect_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, int nc, float* xywhn,
                        int32_t* class_counts, void* stream);
+/* myolo_scale_boxes: autoShape's boxes in image space (reference models/common.py:668-669,680-688).  Rows [0, counts[b]) of the padded
+ * NMS rows (B, max_det, 6) fp32 become scale_coords(shape1, rows[:, :4], shape0[b]) IN PLACE (x -= pad, x /= gain, clamp to [0, w0] /
+ * [0, h0], no rounding), fp32 IEEE arithmetic equal to torch's CPU statements; geom as in myolo_detect_boxes.  Each nullable output is
+ * (B, max_det, 6) fp32 written for the same rows: xywh = xyxy2xywh(row), xyxyn = row / gn, xywhn = xywh / gn with
+ * gn = (w0, h0, w0, h0, 1, 1) (a division, as Detections.__init__ does).  Rows past the count are not touched. */
+int myolo_scale_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, float* xywh, float* xyxyn, float* xywhn,
+                      void* stream);
 
 /* ---- detection validation statistics (reference test.py:175,183-265 and utils/metrics.py:24-112; multiyolov5_b200/utils/metrics.py
  * DetectionStats) ----
@@ -554,6 +579,17 @@ int myolo_nms(const float* pred, int B, int A, int no, float conf_thres, float i
  * logits: (B,C,h,w) NCHW fp32/fp16.  out: (B,H,W) int64 (out_dtype I64) or uint8 (U8). */
 int myolo_seg_upsample_argmax(const void* logits, int dtype, int B, int C, int h, int w, int H, int W, void* out,
                               int out_dtype, void* stream);
+/* autoShape's per-image class maps: for item b, F.interpolate(logits[b:b+1, :, top:top+rh, left:left+rw], (h0, w0), 'bilinear',
+ * align_corners=True).argmax(1) (ties -> lowest class id; fp16 logits compare the fp16-rounded values, as torch's half interpolate returns
+ * them) written as uint8 (h0, w0) at out + offset.  logits: (B,C,H,W) NCHW fp32/fp16, C <= 256.  items: DEVICE array of B
+ * myolo_seg_crop_item, each window inside H x W; max_pixels: the largest h0 * w0, which sizes the grid.  One launch. */
+typedef struct {
+  int64_t offset;            /* byte offset of the item's (h0, w0) map in out */
+  int32_t top, left, rh, rw; /* the window of the letterboxed image in the logits */
+  int32_t h0, w0;            /* output size: the original image */
+} myolo_seg_crop_item;
+int myolo_seg_crop_upsample_argmax(const void* logits, int dtype, int B, int C, int H, int W, const myolo_seg_crop_item* items,
+                                   int64_t max_pixels, uint8_t* out, void* stream);
 /* F.interpolate(seg,(H,W),'bilinear',align_corners=True) on NCHW fp32 (materialised logits) */
 int myolo_bilinear_nchw(const float* src, int B, int C, int h, int w, int H, int W, float* dst, void* stream);
 

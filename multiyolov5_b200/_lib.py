@@ -43,6 +43,7 @@ EXPORTS = [
     "myolo_kmeans", "myolo_kmeans_workspace_bytes", "myolo_class_weights", "myolo_image_weights", "myolo_weighted_draw",
     "myolo_plan_backward_seg_loss", "myolo_seg_focal_loss", "myolo_seg_focal_loss_backward", "myolo_seg_focal_loss_workspace_bytes",
     "myolo_conv_backward", "myolo_conv_forward", "myolo_plan_forward_pass", "myolo_scale_img", "myolo_detect_boxes",
+    "myolo_letterbox_items", "myolo_scale_boxes", "myolo_seg_crop_upsample_argmax",
 ]
 REDUCTION_MEAN, REDUCTION_SUM = 0, 1        # include/myolo.h: MYOLO_REDUCTION_* of myolo_seg_focal_loss
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
@@ -141,6 +142,9 @@ def lib():
     L.myolo_augment_seg.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp]
     L.myolo_seg_lut_blend.argtypes = [vp, i32, i64, vp, i32, i32, i32, vp, vp, f32, f32, vp, vp, i32, vp, vp]
     L.myolo_detect_boxes.argtypes = [vp, vp, i32, i32, vp, i32, vp, vp, vp]
+    L.myolo_scale_boxes.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, vp]
+    L.myolo_letterbox_items.argtypes = [vp, vp, i32, i32, i32, vp, i32, vp]
+    L.myolo_seg_crop_upsample_argmax.argtypes = [vp, i32, i32, i32, i32, i32, vp, i64, vp, vp]
     L.myolo_seg_metrics.argtypes = [vp, i32, vp, i64, i32, vp, vp]
     L.myolo_det_match.argtypes = [vp, vp, i32, i32, vp, i32, i32, i32, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp]
     L.myolo_det_ap_workspace_bytes.argtypes = [i32, i32, i32]

@@ -101,6 +101,48 @@ int launch_detect_boxes(float* rows, const int32_t* counts, int B, int max_det, 
   return 0;
 }
 
+// autoShape's scale_coords(shape1, y[:, :4], shape0) (reference models/common.py:668-669), one CTA per image: as detect_boxes_kernel
+// without the round, then Detections.__init__'s xyxy2xywh and its divisions by gn = (w0, h0, w0, h0, 1, 1) (models/common.py:680-688)
+__global__ void scale_boxes_kernel(float* rows, const int32_t* counts, int max_det, const float* geom, float* xywh, float* xyxyn,
+                                   float* xywhn) {
+  const int b = blockIdx.x;
+  const float px = geom[b * 5 + 0], py = geom[b * 5 + 1], gain = geom[b * 5 + 2], w0 = geom[b * 5 + 3], h0 = geom[b * 5 + 4];
+  const float gn[6] = {w0, h0, w0, h0, 1.f, 1.f};
+  const int n = min(max(counts[b], 0), max_det);
+  for (int r = threadIdx.x; r < n; r += blockDim.x) {
+    const long o = ((long)b * max_det + r) * 6;
+    float a[6], w[6];
+#pragma unroll
+    for (int j = 0; j < 6; ++j) a[j] = rows[o + j];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float x = __fdiv_rn(__fsub_rn(a[j], (j & 1) ? py : px), gain);
+      a[j] = fminf(fmaxf(x, 0.f), (j & 1) ? h0 : w0);
+      rows[o + j] = a[j];
+    }
+    w[0] = __fdiv_rn(__fadd_rn(a[0], a[2]), 2.f);
+    w[1] = __fdiv_rn(__fadd_rn(a[1], a[3]), 2.f);
+    w[2] = __fsub_rn(a[2], a[0]);
+    w[3] = __fsub_rn(a[3], a[1]);
+    w[4] = a[4];
+    w[5] = a[5];
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+      if (xywh) xywh[o + j] = w[j];
+      if (xyxyn) xyxyn[o + j] = __fdiv_rn(a[j], gn[j]);
+      if (xywhn) xywhn[o + j] = __fdiv_rn(w[j], gn[j]);
+    }
+  }
+}
+
+int launch_scale_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, float* xywh, float* xyxyn, float* xywhn,
+                       cudaStream_t s) {
+  MYOLO_REQUIRE(rows && counts && geom && B > 0 && max_det > 0, "scale_boxes: bad arguments");
+  scale_boxes_kernel<<<B, 128, 0, s>>>(rows, counts, max_det, geom, xywh, xyxyn, xywhn);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
 // counters[0] = correct, [1] = labeled, [2..2+n) intersection, [2+n..2+2n) prediction area, [2+2n..2+3n) label area  (accumulated)
 __global__ void seg_hist_kernel(const void* pred, int pred_dtype, const long long* __restrict__ target, long n, int n_cls,
                                 unsigned long long* counters) {

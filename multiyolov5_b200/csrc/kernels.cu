@@ -801,6 +801,32 @@ __global__ void argmax_nchw_f16x8_kernel(const __half* __restrict__ src, int B, 
   }
 }
 
+// autoShape's class maps: item blockIdx.y's window [top, top+rh) x [left, left+rw) of its (C,H,W) logits resampled to (h0, w0) with
+// seg_argmax_nchw_kernel's arithmetic, uint8 out at the item's offset
+template <typename TIn>
+__global__ void seg_crop_argmax_kernel(const TIn* __restrict__ src, int C, int H, int W, const myolo_seg_crop_item* __restrict__ items,
+                                       uint8_t* out) {
+  const int b = blockIdx.y;
+  const myolo_seg_crop_item it = items[b];
+  const long total = (long)it.h0 * it.w0;
+  const TIn* base = src + (size_t)b * C * H * W + (size_t)it.top * W + it.left;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int x = (int)(i % it.w0);
+    const int y = (int)(i / it.w0);
+    const Lerp ly = lerp_axis(y, it.rh, it.h0), lx = lerp_axis(x, it.rw, it.w0);
+    float best = 0.f;
+    int bi = 0;
+    for (int c = 0; c < C; ++c) {
+      const TIn* pl = base + (size_t)c * H * W;
+      float val = bilerp((float)pl[ly.i0 * W + lx.i0], (float)pl[ly.i0 * W + lx.i1], (float)pl[ly.i1 * W + lx.i0],
+                         (float)pl[ly.i1 * W + lx.i1], ly, lx);
+      if (sizeof(TIn) == 2) val = __half2float(__float2half_rn(val));
+      if (c == 0 || val > best) { best = val; bi = c; }
+    }
+    out[it.offset + i] = (uint8_t)bi;
+  }
+}
+
 __global__ void bilinear_nchw_kernel(const float* __restrict__ src, int B, int C, int h, int w, int H, int W, float* dst) {
   const long total = (long)B * C * H * W;
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -869,6 +895,18 @@ extern "C" int myolo_seg_upsample_argmax(const void* logits, int dtype, int B, i
     if (out_dtype == MYOLO_I64) seg_argmax_nchw_kernel<__half, int64_t><<<g, 256, 0, s>>>((const __half*)logits, B, C, h, w, H, W, (int64_t*)out);
     else seg_argmax_nchw_kernel<__half, uint8_t><<<g, 256, 0, s>>>((const __half*)logits, B, C, h, w, H, W, (uint8_t*)out);
   }
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_seg_crop_upsample_argmax(const void* logits, int dtype, int B, int C, int H, int W, const myolo_seg_crop_item* items,
+                                              int64_t max_pixels, uint8_t* out, void* stream) {
+  MYOLO_REQUIRE(logits && items && out && B > 0 && B <= 65535 && C > 0 && C <= 256 && H > 0 && W > 0 && max_pixels > 0,
+                "seg_crop_upsample_argmax: bad arguments");
+  MYOLO_REQUIRE(dtype == MYOLO_F32 || dtype == MYOLO_F16, "seg_crop_upsample_argmax: unsupported dtype");
+  const dim3 grid((unsigned)grid_for(max_pixels, 256, std::max(1, 132 * 64 / B)), (unsigned)B);
+  if (dtype == MYOLO_F32) seg_crop_argmax_kernel<float><<<grid, 256, 0, (cudaStream_t)stream>>>((const float*)logits, C, H, W, items, out);
+  else seg_crop_argmax_kernel<__half><<<grid, 256, 0, (cudaStream_t)stream>>>((const __half*)logits, C, H, W, items, out);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }

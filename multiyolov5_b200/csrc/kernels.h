@@ -32,6 +32,8 @@ int launch_read_view(const TensorView& v, float* dst_nchw, cudaStream_t s);
 // pre-process (preprocess.cu): letterbox resize + border + channel swap / layout / dtype conversion of uint8 HWC frames
 int launch_letterbox(const unsigned char* src, int B, int H0, int W0, int rw, int rh, int top, int left, int H, int W, const int* pad3,
                      void* dst, int out_dtype, int chw, int swap_rb, cudaStream_t s);
+int launch_letterbox_items(const unsigned char* src, const myolo_letterbox_item* items, int B, int H, int W, void* dst, int out_dtype,
+                           cudaStream_t s);
 
 // detection training batches (augment.cu): image cache resize and the fused mosaic / warp / mixup / HSV / flip kernel
 int launch_resize_u8(const unsigned char* src, int H0, int W0, unsigned char* dst, int H, int W, cudaStream_t s);
@@ -61,6 +63,8 @@ int launch_lut_blend(const void* idx, int idx_dtype, long n, const unsigned char
                      unsigned char* out2, cudaStream_t s);
 int launch_detect_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, int nc, float* xywhn, int32_t* class_counts,
                         cudaStream_t s);
+int launch_scale_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, float* xywh, float* xyxyn, float* xywhn,
+                       cudaStream_t s);
 int launch_seg_hist(const void* pred, int pred_dtype, const long long* target, long n, int n_cls, unsigned long long* counters, cudaStream_t s);
 
 // autoanchor (autoanchor.cu): the ratio metric and the cooperative genetic evolution

@@ -1455,6 +1455,13 @@ extern "C" int myolo_letterbox(const uint8_t* src, int B, int H0, int W0, int re
   return launch_letterbox(src, B, H0, W0, resized_w, resized_h, top, left, H, W, pad_bgr, out, out_dtype, chw, swap_rb, (cudaStream_t)stream);
 }
 
+extern "C" int myolo_letterbox_items(const uint8_t* src, const myolo_letterbox_item* items, int B, int H, int W, void* out, int out_dtype,
+                                     void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_letterbox_items(src, items, B, H, W, out, out_dtype, (cudaStream_t)stream);
+}
+
 extern "C" int myolo_resize_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream) {
   int rc = check_device(nullptr);
   if (rc) return rc;
@@ -1520,6 +1527,13 @@ extern "C" int myolo_detect_boxes(float* rows, const int32_t* counts, int B, int
   int rc = check_device(nullptr);
   if (rc) return rc;
   return launch_detect_boxes(rows, counts, B, max_det, geom, nc, xywhn, class_counts, (cudaStream_t)stream);
+}
+
+extern "C" int myolo_scale_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, float* xywh, float* xyxyn,
+                                 float* xywhn, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_scale_boxes(rows, counts, B, max_det, geom, xywh, xyxyn, xywhn, (cudaStream_t)stream);
 }
 
 extern "C" int myolo_seg_metrics(const void* pred, int pred_dtype, const int64_t* target, int64_t n_pixels, int n_classes, uint64_t* counters,

@@ -63,4 +63,42 @@ int launch_letterbox(const unsigned char* src, int B, int H0, int W0, int rw, in
   return 0;
 }
 
+// autoShape's ragged batch (reference models/common.py:655-658): every item letterboxed to one H x W from its own packed RGB source, CHW
+// output, no channel swap.  Float outputs divide by 255 as torch's CPU `x / 255.` does (a true division, not the reciprocal product
+// of the CUDA `img /= 255.0` above); fp16 rounds that fp32 quotient, as CPU half division computes in fp32.
+__global__ void letterbox_items_kernel(const unsigned char* __restrict__ src, const myolo_letterbox_item* __restrict__ items, int B, int H,
+                                       int W, void* dst, int out_dtype) {
+  const long total = (long)B * H * W;
+  for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int x = (int)(i % W);
+    const int y = (int)((i / W) % H);
+    const int b = (int)(i / ((long)W * H));
+    const myolo_letterbox_item& it = items[b];
+    int v[3] = {114, 114, 114};
+    const int rx = x - it.left, ry = y - it.top;
+    if (rx >= 0 && ry >= 0 && rx < it.rw && ry < it.rh) {
+      ResizeGeom g;
+      g.H0 = it.H0; g.W0 = it.W0; g.scale_x = it.scale_x; g.scale_y = it.scale_y; g.mode = it.mode;
+      resize_pixel_u8(src + it.offset, g, rx, ry, v);
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const size_t o = (((size_t)b * 3 + c) * H + y) * W + x;
+      if (out_dtype == MYOLO_U8) reinterpret_cast<unsigned char*>(dst)[o] = (unsigned char)v[c];
+      else if (out_dtype == MYOLO_F16) reinterpret_cast<__half*>(dst)[o] = __float2half_rn(__fdiv_rn((float)v[c], 255.0f));
+      else reinterpret_cast<float*>(dst)[o] = __fdiv_rn((float)v[c], 255.0f);
+    }
+  }
+}
+
+int launch_letterbox_items(const unsigned char* src, const myolo_letterbox_item* items, int B, int H, int W, void* dst, int out_dtype,
+                           cudaStream_t s) {
+  MYOLO_REQUIRE(src && items && dst && B > 0 && H > 0 && W > 0, "letterbox_items: bad arguments (B %d, out %dx%d)", B, W, H);
+  MYOLO_REQUIRE(out_dtype == MYOLO_U8 || out_dtype == MYOLO_F16 || out_dtype == MYOLO_F32, "letterbox_items: output dtype");
+  const long total = (long)B * H * W;
+  letterbox_items_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(src, items, B, H, W, dst, out_dtype);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace myolo

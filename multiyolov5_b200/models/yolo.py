@@ -192,6 +192,16 @@ class Model(nn.Module):
         self.invalidate_weights()
         return self
 
+    def autoshape(self):  # reference models/yolo.py:363-367
+        """the model wrapped for in-memory inputs (models.common.autoShape), with its yaml, nc, hyp, names and stride (those it has)"""
+        from .common import autoShape
+        print("Adding autoShape... ")
+        m = autoShape(self)
+        for k in ("yaml", "nc", "hyp", "names", "stride"):     # copy_attr(m, self, include=...): instance attributes only
+            if k in self.__dict__:
+                setattr(m, k, self.__dict__[k])
+        return m
+
     def info(self, verbose=False, img_size=640):
         n_p = sum(x.numel() for x in self.parameters())
         print(f"Model Summary: {len(list(self.modules()))} layers, {n_p} parameters")

@@ -92,6 +92,43 @@ def preprocess(img0, img_size=640, stride=32, half=True, color=(114, 114, 114), 
     return (out if out.dim() == 4 else out[None]), geom[1], geom[2]
 
 
+# ---- autoShape's ragged batch (reference models/common.py:655-658; csrc/preprocess.cu letterbox_items_kernel) ----
+# include/myolo.h myolo_letterbox_item
+LETTERBOX_ITEM = np.dtype([("offset", "<i8"), ("scale_x", "<f8"), ("scale_y", "<f8"), ("H0", "<i4"), ("W0", "<i4"), ("mode", "<i4"),
+                           ("rw", "<i4"), ("rh", "<i4"), ("top", "<i4"), ("left", "<i4"), ("reserved", "<i4")])
+
+
+def resize_geometry(H0, W0, rh, rw):
+    """cv2.resize's INTER_LINEAR set-up for (H0, W0) -> (rh, rw), as csrc/resize.cuh resize_geom computes it: (scale_x, scale_y, mode),
+    scales 1 / (dst / src) in double, mode 0 copy, 1 bilinear, 2 exact 2x down-scale (cv2 takes its area path there)"""
+    sx, sy = 1.0 / (rw / W0), 1.0 / (rh / H0)
+    eps = 2.220446049250313e-16
+    mode = 0 if (rw == W0 and rh == H0) else 2 if (abs(sx - 2.0) < eps and abs(sy - 2.0) < eps) else 1
+    return sx, sy, mode
+
+
+def letterbox_item_table(shapes0, shape1, offsets):
+    """the myolo_letterbox_item table of letterbox(im, new_shape=shape1, auto=False) for images of shapes0 (h0, w0) whose HWC sources
+    start at byte `offsets` of the packed buffer"""
+    t = np.zeros(len(shapes0), LETTERBOX_ITEM)
+    for k, ((h0, w0), off) in enumerate(zip(shapes0, offsets)):
+        (rw, rh), _, _, (top, _, left, _) = letterbox_geometry((h0, w0), shape1, auto=False)
+        sx, sy, mode = resize_geometry(h0, w0, rh, rw)
+        t[k] = (off, sx, sy, h0, w0, mode, rw, rh, top, left, 0)
+    return t
+
+
+def letterbox_items(src, items, B, shape1, out_dtype=torch.float32):
+    """B packed RGB uint8 sources letterboxed to shape1 (H, W) in one launch: (B,3,H,W) uint8, or fp16 / fp32 value / 255.  src: the
+    CUDA uint8 buffer holding the sources; items: CUDA uint8 bytes of the letterbox_item_table"""
+    if not (src.is_cuda and items.is_cuda and src.dtype == torch.uint8 and items.numel() == B * LETTERBOX_ITEM.itemsize):
+        raise _lib.MyoloError("letterbox_items needs CUDA uint8 sources and a CUDA table of B items")
+    out = torch.empty((B, 3, int(shape1[0]), int(shape1[1])), dtype=out_dtype, device=src.device)
+    _lib.check(_lib.lib().myolo_letterbox_items(_lib.ptr(src), _lib.ptr(items), B, out.shape[2], out.shape[3], _lib.ptr(out),
+                                                _lib.torch_dtype_code(out_dtype), _lib.stream_ptr()))
+    return out
+
+
 # ------------------------------------------------------------------------------------------------
 # detection training batches (reference utils/datasets.py:518-599 LoadImagesAndLabels.__getitem__ + collate_fn, augment=True)
 # ------------------------------------------------------------------------------------------------

@@ -355,3 +355,50 @@ def detect_boxes(rows, counts, geom, nc=None, xywhn=False):
     _lib.check(_lib.lib().myolo_detect_boxes(_lib.ptr(rows), _lib.ptr(counts), B, max_det, _lib.ptr(geom), 0 if nc is None else int(nc),
                                              _lib.ptr(wh), _lib.ptr(cc), _lib.stream_ptr()))
     return wh, cc
+
+
+# ---- autoShape (reference models/common.py:661-672,680-688) ----
+# include/myolo.h myolo_seg_crop_item
+SEG_CROP_ITEM = np.dtype([("offset", "<i8"), ("top", "<i4"), ("left", "<i4"), ("rh", "<i4"), ("rw", "<i4"), ("h0", "<i4"), ("w0", "<i4")])
+
+
+def scale_boxes(rows, counts, geom):
+    """autoShape's `scale_coords(shape1, y[i][:, :4], shape0[i])` for a batch in one launch: rows (B, max_det, 6) fp32 CUDA padded NMS
+    rows (non_max_suppression(..., return_padded=True)), rows[b, :counts[b], :4] scaled IN PLACE without rounding, bit for bit torch's
+    CPU fp32.  geom: (B, 5) fp32 rows of scale_coords_geometry (host or device).  Returns Detections' (xywh, xyxyn, xywhn) as
+    (B, max_det, 6) fp32 tensors, valid for the same rows."""
+    if not (rows.is_cuda and rows.dtype == torch.float32 and rows.is_contiguous() and rows.dim() == 3 and rows.shape[2] == 6):
+        raise _lib.MyoloError("scale_boxes needs contiguous (B, max_det, 6) fp32 CUDA rows")
+    B, max_det, _ = rows.shape
+    counts = counts.to(device=rows.device, dtype=torch.int32).contiguous()
+    geom = torch.as_tensor(geom, dtype=torch.float32).reshape(B, 5).to(rows.device, non_blocking=True).contiguous()
+    xywh, xyxyn, xywhn = (torch.empty_like(rows) for _ in range(3))
+    _lib.check(_lib.lib().myolo_scale_boxes(_lib.ptr(rows), _lib.ptr(counts), B, max_det, _lib.ptr(geom), _lib.ptr(xywh), _lib.ptr(xyxyn),
+                                            _lib.ptr(xywhn), _lib.stream_ptr()))
+    return xywh, xyxyn, xywhn
+
+
+def seg_crop_item_table(windows, shapes0):
+    """the myolo_seg_crop_item table: windows (top, left, rh, rw) of the letterboxed images, shapes0 (h0, w0) the class map sizes, packed
+    one after the other"""
+    t = np.zeros(len(shapes0), SEG_CROP_ITEM)
+    off = 0
+    for k, ((top, left, rh, rw), (h0, w0)) in enumerate(zip(windows, shapes0)):
+        t[k] = (off, top, left, rh, rw, h0, w0)
+        off += h0 * w0
+    return t
+
+
+def seg_crop_argmax(seg, items, shapes0):
+    """autoShape's class maps in one launch: for image i, F.interpolate(seg[i:i+1, :, top:top+rh, left:left+rw], shapes0[i], 'bilinear',
+    align_corners=True).argmax(1) as a uint8 (h0, w0) CUDA tensor, all views of one packed buffer.  seg: (B,C,H,W) fp32 / fp16 CUDA
+    logits; items: CUDA uint8 bytes of the seg_crop_item_table (its windows must lie inside H x W)."""
+    if not (seg.is_cuda and items.is_cuda and seg.dim() == 4 and items.numel() == seg.shape[0] * SEG_CROP_ITEM.itemsize):
+        raise _lib.MyoloError("seg_crop_argmax needs (B,C,H,W) CUDA logits and a CUDA table of B items")
+    seg = seg.contiguous()
+    B, Cc, H, W = seg.shape
+    sizes = [int(h) * int(w) for h, w in shapes0]
+    out = torch.empty(sum(sizes), dtype=torch.uint8, device=seg.device)
+    _lib.check(_lib.lib().myolo_seg_crop_upsample_argmax(_lib.ptr(seg), _lib.torch_dtype_code(seg.dtype), B, Cc, H, W, _lib.ptr(items),
+                                                         max(sizes), _lib.ptr(out), _lib.stream_ptr()))
+    return [m.view(int(h), int(w)) for m, (h, w) in zip(out.split(sizes), shapes0)]
