@@ -562,6 +562,17 @@ int myolo_scale_boxes(float* rows, const int32_t* counts, int B, int max_det, co
 int myolo_det_match(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H, int W,
                     const float* geom, const float* iouv, int img_base, uint16_t* st_correct, float* st_conf, uint8_t* st_cls,
                     int32_t* st_rows, uint64_t* tcount, int32_t* err, void* stream);
+/* utils.metrics.ConfusionMatrix.process_batch (the fork's utils/metrics.py:115-162) for a batch of B images in one launch, into
+ * matrix: device int64 (nc+1, nc+1), row = true class (the fork's order), accumulated.  With geom != NULL the inputs are those of
+ * myolo_det_match (padded NMS rows in network space, normalised targets, H, W, geom) and are scaled to native space as test.py does;
+ * with geom == NULL, dets rows and targets [image, class, x1, y1, x2, y2] are native-space boxes already.  Detections with
+ * conf <= conf_thres are dropped; pairs with IoU > iou_thres match, each detection keeping its best label and then each label its
+ * best remaining detection (ties: lower label index, then lower detection index).  require_rows != 0 skips images without labels
+ * or without rows, as test() only calls process_batch for those.  Classes outside [0, nc) set MYOLO_DET_ERR_TARGET_CLASS /
+ * MYOLO_DET_ERR_PRED_CLASS in *err and are not counted; more than 1024 labels in one image sets MYOLO_DET_ERR_LABELS. */
+int myolo_confusion_update(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H,
+                           int W, const float* geom, int nc, float conf_thres, float iou_thres, int require_rows, int64_t* matrix,
+                           int32_t* err, void* stream);
 int64_t myolo_det_ap_workspace_bytes(int n_images, int max_det, int ncol);
 int myolo_det_ap(const uint16_t* correct, const float* conf, const uint8_t* cls, const int32_t* rows, int n_images, int max_det, int ncol,
                  const uint64_t* tcount, const double* px, const double* x101, double* out_ap, double* out_p, double* out_r,
@@ -575,6 +586,20 @@ int64_t myolo_nms_workspace_bytes(int B, int A, int no, int multi_label);
 int myolo_nms(const float* pred, int B, int A, int no, float conf_thres, float iou_thres, const int32_t* classes,
               int n_classes, int agnostic, int multi_label, int max_det, int max_nms, float max_wh, float* out,
               int32_t* out_count, void* workspace, int64_t workspace_bytes, void* stream);
+/* non_max_suppression(..., labels=lb) (utils/general.py:448-455, test.py --save-hybrid): as myolo_nms, with image b's apriori labels
+ * labels[label_offsets[b] .. label_offsets[b+1]) appended after its candidates.  labels: device (n,5) fp32 [cls, x, y, w, h] in network
+ * input pixels; label_offsets: device (B+1) int32.  max_labels bounds every image's label count (the number of rows n is always a
+ * valid bound; labels may be NULL when it is 0).  A label whose class id truncates to a value outside [0, nc) is dropped and sets
+ * MYOLO_NMS_ERR_LABEL_CLASS in *err; an image with more than max_labels labels sets MYOLO_NMS_ERR_LABEL_COUNT (its first max_labels
+ * labels are used).  *err is OR-ed into, never cleared, so one word can serve many calls.
+ * workspace: >= myolo_nms_labels_workspace_bytes(B,A,no,multi_label,max_labels). */
+#define MYOLO_NMS_ERR_LABEL_CLASS 1
+#define MYOLO_NMS_ERR_LABEL_COUNT 2
+int64_t myolo_nms_labels_workspace_bytes(int B, int A, int no, int multi_label, int max_labels);
+int myolo_nms_labels(const float* pred, int B, int A, int no, float conf_thres, float iou_thres, const int32_t* classes,
+                     int n_classes, int agnostic, int multi_label, int max_det, int max_nms, float max_wh, const float* labels,
+                     const int32_t* label_offsets, int max_labels, int32_t* err, float* out, int32_t* out_count, void* workspace,
+                     int64_t workspace_bytes, void* stream);
 /* detect.py:191-193: bilinear(align_corners=True) to (H,W) then argmax over C (first max wins).
  * logits: (B,C,h,w) NCHW fp32/fp16.  out: (B,H,W) int64 (out_dtype I64) or uint8 (U8). */
 int myolo_seg_upsample_argmax(const void* logits, int dtype, int B, int C, int h, int w, int H, int W, void* out,

@@ -43,10 +43,12 @@ EXPORTS = [
     "myolo_kmeans", "myolo_kmeans_workspace_bytes", "myolo_class_weights", "myolo_image_weights", "myolo_weighted_draw",
     "myolo_plan_backward_seg_loss", "myolo_seg_focal_loss", "myolo_seg_focal_loss_backward", "myolo_seg_focal_loss_workspace_bytes",
     "myolo_conv_backward", "myolo_conv_forward", "myolo_plan_forward_pass", "myolo_scale_img", "myolo_detect_boxes",
-    "myolo_letterbox_items", "myolo_scale_boxes", "myolo_seg_crop_upsample_argmax",
+    "myolo_letterbox_items", "myolo_scale_boxes", "myolo_seg_crop_upsample_argmax", "myolo_nms_labels", "myolo_nms_labels_workspace_bytes",
+    "myolo_confusion_update",
 ]
 REDUCTION_MEAN, REDUCTION_SUM = 0, 1        # include/myolo.h: MYOLO_REDUCTION_* of myolo_seg_focal_loss
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
+NMS_ERR_LABEL_CLASS, NMS_ERR_LABEL_COUNT = 1, 2                          # include/myolo.h: bits of myolo_nms_labels' error word
 KMEANS_MAX_ITER, KMEANS_BAD_INDEX = 1, 2                                 # include/myolo.h: bits of myolo_kmeans' status word
 IW_BAD_CLASS, IW_TOTAL_NONPOS, IW_TOTAL_NONFINITE = 1, 2, 4              # include/myolo.h: bits of the image-weights status word
 IW_NC_MAX = 1024                                                         # include/myolo.h MYOLO_IW_NC_MAX
@@ -147,6 +149,7 @@ def lib():
     L.myolo_seg_crop_upsample_argmax.argtypes = [vp, i32, i32, i32, i32, i32, vp, i64, vp, vp]
     L.myolo_seg_metrics.argtypes = [vp, i32, vp, i64, i32, vp, vp]
     L.myolo_det_match.argtypes = [vp, vp, i32, i32, vp, i32, i32, i32, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp]
+    L.myolo_confusion_update.argtypes = [vp, vp, i32, i32, vp, i32, i32, i32, vp, i32, f32, f32, i32, vp, vp, vp]
     L.myolo_det_ap_workspace_bytes.argtypes = [i32, i32, i32]
     L.myolo_det_ap_workspace_bytes.restype = i64
     L.myolo_det_ap.argtypes = [vp, vp, vp, vp, i32, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i64, vp]
@@ -199,6 +202,9 @@ def lib():
     L.myolo_nms_workspace_bytes.argtypes = [i32, i32, i32, i32]
     L.myolo_nms_workspace_bytes.restype = i64
     L.myolo_nms.argtypes = [vp, i32, i32, i32, f32, f32, vp, i32, i32, i32, i32, i32, f32, vp, vp, vp, i64, vp]
+    L.myolo_nms_labels_workspace_bytes.argtypes = [i32, i32, i32, i32, i32]
+    L.myolo_nms_labels_workspace_bytes.restype = i64
+    L.myolo_nms_labels.argtypes = [vp, i32, i32, i32, f32, f32, vp, i32, i32, i32, i32, i32, f32, vp, vp, i32, vp, vp, vp, vp, i64, vp]
     L.myolo_seg_upsample_argmax.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp]
     L.myolo_bilinear_nchw.argtypes = [vp, i32, i32, i32, i32, i32, i32, vp, vp]
     L.myolo_conv_bn_silu.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, vp]

@@ -49,6 +49,9 @@ int launch_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int m
                        int out_dtype, long long* out_mask, cudaStream_t s);
 
 // detection validation statistics (metrics.cu): per-batch matching into the stats store, ap_per_class over the whole store
+int launch_confusion(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H, int W,
+                     const float* geom, int nc, float conf_thres, float iou_thres, int require_rows, unsigned long long* matrix, int32_t* err,
+                     cudaStream_t s);
 int launch_det_match(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H, int W,
                      const float* geom, const float* iouv, int img_base, uint16_t* st_correct, float* st_conf, uint8_t* st_cls,
                      int32_t* st_rows, unsigned long long* tcount, int32_t* err, cudaStream_t s);

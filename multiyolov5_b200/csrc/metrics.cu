@@ -26,6 +26,28 @@ __device__ __forceinline__ float scale_x(float v, float pad, float gain, float h
   return fminf(fmaxf(__fdiv_rn(__fsub_rn(v, pad), gain), 0.f), hi);
 }
 
+// test.py:175,223-224: a target [x, y, w, h] (normalised) to pixels, xywh2xyxy, scale_coords(ratio_pad) and clip_coords
+__device__ __forceinline__ float4 target_box(const float* t, float H, float W, float padw, float padh, float gain, float w0, float h0) {
+  const float x = __fmul_rn(t[0], W), y = __fmul_rn(t[1], H), bw = __fmul_rn(t[2], W), bh = __fmul_rn(t[3], H);
+  const float hw = __fdiv_rn(bw, 2.f), hh = __fdiv_rn(bh, 2.f);
+  float4 bx;
+  bx.x = scale_x(__fsub_rn(x, hw), padw, gain, w0);
+  bx.y = scale_x(__fsub_rn(y, hh), padh, gain, h0);
+  bx.z = scale_x(__fadd_rn(x, hw), padw, gain, w0);
+  bx.w = scale_x(__fadd_rn(y, hh), padh, gain, h0);
+  return bx;
+}
+
+__device__ __forceinline__ float box_area(float4 b) { return __fmul_rn(__fsub_rn(b.z, b.x), __fsub_rn(b.w, b.y)); }
+
+// general.box_iou of one pair in either operand order (min / max and area1 + area2 commute)
+__device__ __forceinline__ float pair_iou(float4 a, float aa, float4 t, float ta) {
+  const float iw = fmaxf(__fsub_rn(fminf(a.z, t.z), fmaxf(a.x, t.x)), 0.f);
+  const float ih = fmaxf(__fsub_rn(fminf(a.w, t.w), fmaxf(a.y, t.y)), 0.f);
+  const float inter = __fmul_rn(iw, ih);
+  return __fdiv_rn(inter, __fsub_rn(__fadd_rn(aa, ta), inter));
+}
+
 // torch.max over a row: the first NaN if any, else the first maximum
 __device__ __forceinline__ void take_max(float v, int k, bool& have, float& best, int& bi) {
   if (!have) { have = true; best = v; bi = k; return; }
@@ -79,15 +101,9 @@ __global__ void __launch_bounds__(kMatchThreads) det_match_kernel(
           atomicAdd(&tcount[(int)c], 1ull);
         }
         // targets[:, 2:] *= [w, h, w, h]; xywh2xyxy; scale_coords(ratio_pad); clip_coords
-        const float x = __fmul_rn(t[2], W), y = __fmul_rn(t[3], H), bw = __fmul_rn(t[4], W), bh = __fmul_rn(t[5], H);
-        const float hw = __fdiv_rn(bw, 2.f), hh = __fdiv_rn(bh, 2.f);
-        float4 bx;
-        bx.x = scale_x(__fsub_rn(x, hw), padw, gain, w0);
-        bx.y = scale_x(__fsub_rn(y, hh), padh, gain, h0);
-        bx.z = scale_x(__fadd_rn(x, hw), padw, gain, w0);
-        bx.w = scale_x(__fadd_rn(y, hh), padh, gain, h0);
+        const float4 bx = target_box(t + 2, H, W, padw, padh, gain, w0, h0);
         s_tbox[k] = bx;
-        s_tarea[k] = __fmul_rn(__fsub_rn(bx.z, bx.x), __fsub_rn(bx.w, bx.y));
+        s_tarea[k] = box_area(bx);
         s_taken[k] = 0;
       }
     }
@@ -108,19 +124,15 @@ __global__ void __launch_bounds__(kMatchThreads) det_match_kernel(
     const float* r = dets + ((long)b * max_det + p) * 6;
     const float pc = r[5];
     if (!(pc >= 0.f && pc < 256.f && pc == floorf(pc))) atomicOr(err, MYOLO_DET_ERR_PRED_CLASS);
-    const float x1 = scale_x(r[0], padw, gain, w0), y1 = scale_x(r[1], padh, gain, h0);
-    const float x2 = scale_x(r[2], padw, gain, w0), y2 = scale_x(r[3], padh, gain, h0);
-    const float a1 = __fmul_rn(__fsub_rn(x2, x1), __fsub_rn(y2, y1));
+    const float4 pb = make_float4(scale_x(r[0], padw, gain, w0), scale_x(r[1], padh, gain, h0), scale_x(r[2], padw, gain, w0),
+                                  scale_x(r[3], padh, gain, h0));
+    const float a1 = box_area(pb);
     bool have = false;
     float best = 0.f;
     int bi = -1;
     for (int k = 0; k < nl; ++k) {
       if (s_tcls[k] != pc) continue;
-      const float4 t = s_tbox[k];
-      const float iw = fmaxf(__fsub_rn(fminf(x2, t.z), fmaxf(x1, t.x)), 0.f);
-      const float ih = fmaxf(__fsub_rn(fminf(y2, t.w), fmaxf(y1, t.y)), 0.f);
-      const float inter = __fmul_rn(iw, ih);
-      take_max(__fdiv_rn(inter, __fsub_rn(__fadd_rn(a1, s_tarea[k]), inter)), k, have, best, bi);
+      take_max(pair_iou(pb, a1, s_tbox[k], s_tarea[k]), k, have, best, bi);
     }
     uint16_t bits = 0;
     if (have)
@@ -161,6 +173,138 @@ int launch_det_match(const float* dets, const int32_t* counts, int B, int max_de
                 (n_targets == 0 || targets), "det_match: bad arguments (max_det <= %d)", kMaxDetRows);
   det_match_kernel<<<B, kMatchThreads, 0, s>>>(dets, counts, max_det, targets, n_targets, (float)H, (float)W, geom, iouv, img_base,
                                                st_correct, st_conf, st_cls, st_rows, tcount, err);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------------------
+// ConfusionMatrix.process_batch (the fork's utils/metrics.py:115-162), one CTA per image
+//
+// The fork keeps the pairs with IoU > iou_thres, sorts them by IoU (descending) and keeps each detection's first pair, sorts again and
+// keeps each label's first pair: every detection keeps its best label, then every label its best detection among those that kept it.
+// numpy's argsort there is not stable, so exact IoU ties are not pinned by the fork; here a detection's tie goes to the lower label
+// index and a label's tie to the lower detection row (the filtered detections keep their row order).
+// ---------------------------------------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool class_in(float c, int nc) { return c >= 0.f && c < (float)nc && c == floorf(c); }
+
+__global__ void __launch_bounds__(kMatchThreads) confusion_kernel(
+    const float* __restrict__ dets, const int32_t* __restrict__ counts, int max_det, const float* __restrict__ targets, int n_targets,
+    float H, float W, const float* __restrict__ geom, int nc, float conf_thres, float iou_thres, int require_rows,
+    unsigned long long* matrix, int32_t* err) {
+  __shared__ float4 s_tbox[kMaxLabels];
+  __shared__ float s_tarea[kMaxLabels];
+  __shared__ short s_tcls[kMaxLabels];      // -1: class outside [0, nc)
+  __shared__ short s_lmatch[kMaxLabels];    // the label's detection row, -1 none
+  __shared__ short s_dlab[kMaxDetRows];     // the detection's best label, -1 none (or dropped by conf)
+  __shared__ float s_diou[kMaxDetRows];
+  __shared__ short s_dcls[kMaxDetRows];
+  __shared__ unsigned char s_dmatched[kMaxDetRows];
+  __shared__ int s_wcount[kMatchThreads / 32];
+  __shared__ int s_nl, s_any;
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  float h0 = 0.f, w0 = 0.f, gain = 1.f, padw = 0.f, padh = 0.f;
+  if (geom) { h0 = geom[5 * b]; w0 = geom[5 * b + 1]; gain = geom[5 * b + 2]; padw = geom[5 * b + 3]; padh = geom[5 * b + 4]; }
+  if (tid == 0) { s_nl = 0; s_any = 0; }
+  __syncthreads();
+
+  // this image's labels in row order, as det_match_kernel gathers them
+  const float fb = (float)b;
+  for (int base = 0; base < n_targets; base += kMatchThreads) {
+    const int i = base + tid;
+    const bool mine = i < n_targets && targets[(long)i * 6] == fb;
+    const unsigned m = __ballot_sync(0xffffffffu, mine);
+    if (lane == 0) s_wcount[warp] = __popc(m);
+    __syncthreads();
+    int off = s_nl;
+    for (int w = 0; w < warp; ++w) off += s_wcount[w];
+    if (mine) {
+      const int k = off + __popc(m & ((1u << lane) - 1u));
+      const float* t = targets + (long)i * 6;
+      if (k >= kMaxLabels) {
+        atomicOr(err, MYOLO_DET_ERR_LABELS);
+      } else {
+        const bool ok = class_in(t[1], nc);
+        if (!ok) atomicOr(err, MYOLO_DET_ERR_TARGET_CLASS);
+        s_tcls[k] = ok ? (short)t[1] : (short)-1;
+        const float4 bx = geom ? target_box(t + 2, H, W, padw, padh, gain, w0, h0) : make_float4(t[2], t[3], t[4], t[5]);
+        s_tbox[k] = bx;
+        s_tarea[k] = box_area(bx);
+        s_lmatch[k] = -1;
+      }
+    }
+    __syncthreads();
+    if (tid == 0) {
+      int tot = 0;
+      for (int w = 0; w < kMatchThreads / 32; ++w) tot += s_wcount[w];
+      s_nl += tot;
+    }
+    __syncthreads();
+  }
+  const int nl = min(s_nl, kMaxLabels);
+  const int n = min(max(counts[b], 0), max_det);
+  if (require_rows && (nl == 0 || n == 0)) return;         // test.py:189-192: no process_batch for this image
+
+  // detections = detections[detections[:, 4] > conf]; each detection's best label with IoU > iou_thres
+  for (int p = tid; p < n; p += kMatchThreads) {
+    const float* r = dets + ((long)b * max_det + p) * 6;
+    const bool active = r[4] > conf_thres;
+    short dc = -1;
+    if (active) {
+      if (class_in(r[5], nc)) dc = (short)r[5];
+      else atomicOr(err, MYOLO_DET_ERR_PRED_CLASS);
+    }
+    int bk = -1;
+    float best = 0.f;
+    if (active) {
+      const float4 pb = geom ? make_float4(scale_x(r[0], padw, gain, w0), scale_x(r[1], padh, gain, h0), scale_x(r[2], padw, gain, w0),
+                                           scale_x(r[3], padh, gain, h0))
+                             : make_float4(r[0], r[1], r[2], r[3]);
+      const float pa = box_area(pb);
+      for (int k = 0; k < nl; ++k) {
+        const float iou = pair_iou(s_tbox[k], s_tarea[k], pb, pa);
+        if (iou > iou_thres && (bk < 0 || iou > best)) { best = iou; bk = k; }
+      }
+    }
+    s_dlab[p] = (short)bk;
+    s_diou[p] = best;
+    s_dcls[p] = dc;
+    s_dmatched[p] = 0;
+  }
+  __syncthreads();
+  // each label's best detection among those whose best label it is
+  for (int k = tid; k < nl; k += kMatchThreads) {
+    int bp = -1;
+    float best = 0.f;
+    for (int p = 0; p < n; ++p)
+      if (s_dlab[p] == k && (bp < 0 || s_diou[p] > best)) { best = s_diou[p]; bp = p; }
+    s_lmatch[k] = (short)bp;
+    if (bp >= 0) { s_dmatched[bp] = 1; s_any = 1; }
+  }
+  __syncthreads();
+  const unsigned long long ld = (unsigned long long)nc + 1;
+  for (int k = tid; k < nl; k += kMatchThreads) {
+    const int gc = s_tcls[k], bp = s_lmatch[k];
+    if (gc < 0) continue;
+    if (bp >= 0) {
+      if (s_dcls[bp] >= 0) atomicAdd(&matrix[gc * ld + s_dcls[bp]], 1ull);      // correct
+    } else {
+      atomicAdd(&matrix[nc * ld + gc], 1ull);                                     // background FP
+    }
+  }
+  if (s_any)                                                                      // `if n:` — only when the image has a match
+    for (int p = tid; p < n; p += kMatchThreads)
+      if (dets[((long)b * max_det + p) * 6 + 4] > conf_thres && !s_dmatched[p] && s_dcls[p] >= 0)
+        atomicAdd(&matrix[s_dcls[p] * ld + nc], 1ull);                            // background FN
+}
+
+int launch_confusion(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H, int W,
+                     const float* geom, int nc, float conf_thres, float iou_thres, int require_rows, unsigned long long* matrix, int32_t* err,
+                     cudaStream_t s) {
+  MYOLO_REQUIRE(dets && counts && matrix && err, "confusion: null argument");
+  MYOLO_REQUIRE(B > 0 && max_det > 0 && max_det <= kMaxDetRows && nc > 0 && nc <= 4096 && n_targets >= 0 && (n_targets == 0 || targets) &&
+                (geom == nullptr || (H > 0 && W > 0)), "confusion: bad arguments (max_det <= %d, nc <= 4096)", kMaxDetRows);
+  confusion_kernel<<<B, kMatchThreads, 0, s>>>(dets, counts, max_det, targets, n_targets, (float)H, (float)W, geom, nc, conf_thres, iou_thres,
+                                               require_rows, matrix, err);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }

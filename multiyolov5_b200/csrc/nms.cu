@@ -9,6 +9,11 @@
 //          loop stops as soon as 300 boxes are kept: exactly `i[:max_det]` of the reference) with a 256x256 bit matrix
 //          for the intra-chunk dependencies.  Every IoU operation is an explicit round-to-nearest fp32 op in the order
 //          of the torchvision CPU kernel, so kept indices are bit-exact with the reference.
+//
+// Apriori labels (myolo_nms_labels, :448-455, the autolabelling of test.py --save-hybrid): image b's k_b label rows [cls, x, y, w, h]
+// are virtual rows A .. A + k_b - 1 of that image with box = xywh, obj = 1 and a one-hot class.  Their candidate index i * nc + j
+// then sorts after every anchor of the image on equal scores, the position torch.cat((x, v), 0) gives them.  They skip the obj >
+// conf_thres pre-filter, as in the reference, and take every later step like any other candidate (so at conf_thres >= 1 they drop out).
 #include <nvtx3/nvToolsExt.h>
 #include "common.cuh"
 
@@ -24,6 +29,10 @@ struct NmsParams {
   float conf_thres, iou_thres, max_wh;
   const int32_t* classes;
   int n_classes, agnostic, multi_label, max_det, max_nms;
+  const float* labels;       // [n][5] cls, x, y, w, h (network-input pixels) or nullptr
+  const int32_t* label_off;  // [B + 1] image b's rows are labels[label_off[b] .. label_off[b + 1])
+  int max_labels;            // bound on any image's label count: the grid and key capacity are sized by it
+  int32_t* err;              // MYOLO_NMS_ERR_* bits, OR-ed in
   int32_t* counts;       // [B]
   unsigned long long* keys;  // [B][cap2]
   long cap, cap2;
@@ -43,10 +52,34 @@ __device__ __forceinline__ void push_key(const NmsParams& p, int b, float score,
   if (slot < p.cap) p.keys[(size_t)b * p.cap2 + slot] = ((unsigned long long)(~__float_as_uint(score)) << 32) | idx;
 }
 
+// class score of label row `lab` for class j: the one-hot column times obj = 1 (x[:, 5:] *= x[:, 4:5])
+__device__ __forceinline__ float label_score(int lc, int j) { return __fmul_rn(j == lc ? 1.0f : 0.0f, 1.0f); }
+
 __global__ void nms_filter_kernel(NmsParams p) {
   const int b = blockIdx.y;
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= p.A) return;
+  if (i == 0 && p.label_off != nullptr && p.label_off[b + 1] - p.label_off[b] > p.max_labels) atomicOr(p.err, MYOLO_NMS_ERR_LABEL_COUNT);
+  if (i >= p.A) {
+    const int k = i - p.A;
+    if (k >= p.max_labels) return;      // also the last block's spare threads, and every thread of myolo_nms (no label table)
+    const int k0 = p.label_off[b], nb = p.label_off[b + 1] - k0;
+    if (k >= nb) return;
+    const float c = p.labels[(size_t)(k0 + k) * 5];
+    // l[:, 0].long() must name a class column: ids >= nc are an index error in the reference, and negative ids write 1.0 into a box
+    // or obj column (or wrap into the class columns), which is no label at all; both set the error bit here
+    if (!(c > -1.0f && c < (float)p.nc)) { atomicOr(p.err, MYOLO_NMS_ERR_LABEL_CLASS); return; }
+    const int lc = (int)c;
+    if (p.multi_label) {
+      for (int j = 0; j < p.nc; ++j) {
+        const float s = label_score(lc, j);
+        if (s > p.conf_thres && class_ok(p, j)) push_key(p, b, s, (unsigned)((unsigned)i * p.nc + j));
+      }
+    } else {
+      const float s = label_score(lc, lc);        // the one 1.0 is the first maximum
+      if (s > p.conf_thres && class_ok(p, lc)) push_key(p, b, s, (unsigned)((unsigned)i * p.nc + lc));
+    }
+    return;
+  }
   const float* row = p.pred + ((size_t)b * p.A + i) * p.no;
   const float obj = row[4];
   if (!(obj > p.conf_thres)) return;                                   // :430,446
@@ -87,15 +120,24 @@ struct Cand { float x1, y1, x2, y2, conf, cls, ox1, oy1, ox2, oy2, area; };
 
 __device__ __forceinline__ Cand load_cand(const NmsParams& p, int b, unsigned long long key) {
   const unsigned idx = (unsigned)(key & 0xffffffffull);
-  const int i = idx / p.nc, j = idx % p.nc;
-  const float* row = p.pred + ((size_t)b * p.A + i) * p.no;
+  const unsigned i = idx / (unsigned)p.nc;
+  const int j = (int)(idx % (unsigned)p.nc);
+  const float* box;
   Cand c;
-  const float hw = __fdiv_rn(row[2], 2.0f), hh = __fdiv_rn(row[3], 2.0f);   // xywh2xyxy, utils/general.py:265-272
-  c.x1 = __fsub_rn(row[0], hw);
-  c.y1 = __fsub_rn(row[1], hh);
-  c.x2 = __fadd_rn(row[0], hw);
-  c.y2 = __fadd_rn(row[1], hh);
-  c.conf = __fmul_rn(row[5 + j], row[4]);
+  if (i >= (unsigned)p.A) {                                                  // a label row: box = xywh, one-hot class, obj 1
+    const float* lab = p.labels + (size_t)(p.label_off[b] + (int)(i - (unsigned)p.A)) * 5;
+    box = lab + 1;
+    c.conf = label_score((int)lab[0], j);
+  } else {
+    const float* row = p.pred + ((size_t)b * p.A + i) * p.no;
+    box = row;
+    c.conf = __fmul_rn(row[5 + j], row[4]);
+  }
+  const float hw = __fdiv_rn(box[2], 2.0f), hh = __fdiv_rn(box[3], 2.0f);   // xywh2xyxy, utils/general.py:265-272
+  c.x1 = __fsub_rn(box[0], hw);
+  c.y1 = __fsub_rn(box[1], hh);
+  c.x2 = __fadd_rn(box[0], hw);
+  c.y2 = __fadd_rn(box[1], hh);
   c.cls = (float)j;
   const float off = __fmul_rn(c.cls, p.agnostic ? 0.0f : p.max_wh);          // :491
   c.ox1 = __fadd_rn(c.x1, off);
@@ -264,31 +306,37 @@ static long next_pow2(long v) {
   return r;
 }
 
-extern "C" int64_t myolo_nms_workspace_bytes(int B, int A, int no, int multi_label) {
-  const long nc = no - 5;
-  const long cap = multi_label && nc > 1 ? (long)A * nc : (long)A;
-  return 256 + align_up((int64_t)B * 4, 256) + (int64_t)B * next_pow2(cap) * 8;
+static long nms_cap(int A, int nc, int multi_label, int max_labels) {
+  return multi_label && nc > 1 ? ((long)A + max_labels) * nc : (long)A + max_labels;
 }
 
-extern "C" int myolo_nms(const float* pred, int B, int A, int no, float conf_thres, float iou_thres, const int32_t* classes,
-                         int n_classes, int agnostic, int multi_label, int max_det, int max_nms, float max_wh, float* out,
-                         int32_t* out_count, void* workspace, int64_t workspace_bytes, void* stream) {
-  nvtxRangePushA("myolo_nms");
-  struct Pop { ~Pop() { nvtxRangePop(); } } nvtx_pop_;
+extern "C" int64_t myolo_nms_workspace_bytes(int B, int A, int no, int multi_label) {
+  return 256 + align_up((int64_t)B * 4, 256) + (int64_t)B * next_pow2(nms_cap(A, no - 5, multi_label, 0)) * 8;
+}
+
+extern "C" int64_t myolo_nms_labels_workspace_bytes(int B, int A, int no, int multi_label, int max_labels) {
+  return 256 + align_up((int64_t)B * 4, 256) + (int64_t)B * next_pow2(nms_cap(A, no - 5, multi_label, max_labels < 0 ? 0 : max_labels)) * 8;
+}
+
+static int nms_launch(const float* pred, int B, int A, int no, float conf_thres, float iou_thres, const int32_t* classes, int n_classes,
+                      int agnostic, int multi_label, int max_det, int max_nms, float max_wh, const float* labels, const int32_t* label_off,
+                      int max_labels, int32_t* err, float* out, int32_t* out_count, void* workspace, int64_t workspace_bytes, void* stream) {
   MYOLO_REQUIRE(pred && out && out_count && workspace, "nms: null pointer");
   MYOLO_REQUIRE(B > 0 && A > 0 && no > 5, "nms: bad shape B=%d A=%d no=%d", B, A, no);
   MYOLO_REQUIRE(max_det > 0 && max_det <= kMaxKept, "nms: max_det must be in [1,%d]", kMaxKept);
   const int nc = no - 5;
-  MYOLO_REQUIRE((long)A * nc < (1l << 32), "nms: A*nc does not fit the 32-bit candidate index");
+  MYOLO_REQUIRE(((long)A + max_labels) * nc < (1l << 32), "nms: (A + max_labels) * nc does not fit the 32-bit candidate index");
   multi_label = multi_label && nc > 1;   // :440
-  MYOLO_REQUIRE(workspace_bytes >= myolo_nms_workspace_bytes(B, A, no, multi_label), "nms: workspace too small");
+  const long cap = nms_cap(A, nc, multi_label, max_labels);
+  MYOLO_REQUIRE(workspace_bytes >= 256 + align_up((int64_t)B * 4, 256) + (int64_t)B * next_pow2(cap) * 8, "nms: workspace too small");
   cudaStream_t s = (cudaStream_t)stream;
   NmsParams p;
   p.pred = pred; p.B = B; p.A = A; p.no = no; p.nc = nc;
   p.conf_thres = conf_thres; p.iou_thres = iou_thres; p.max_wh = max_wh;
   p.classes = n_classes > 0 ? classes : nullptr; p.n_classes = n_classes;
   p.agnostic = agnostic; p.multi_label = multi_label; p.max_det = max_det; p.max_nms = max_nms;
-  p.cap = multi_label ? (long)A * nc : (long)A;
+  p.labels = labels; p.label_off = label_off; p.max_labels = max_labels; p.err = err;
+  p.cap = cap;
   p.cap2 = next_pow2(p.cap);
   unsigned char* ws = reinterpret_cast<unsigned char*>(workspace);
   ws = reinterpret_cast<unsigned char*>(align_up((int64_t)ws, 256));
@@ -296,7 +344,7 @@ extern "C" int myolo_nms(const float* pred, int B, int A, int no, float conf_thr
   p.keys = reinterpret_cast<unsigned long long*>(ws + align_up((int64_t)B * 4, 256));
   p.out = out; p.out_count = out_count;
   MYOLO_CHECK_CUDA(cudaMemsetAsync(p.counts, 0, (size_t)B * 4, s));
-  dim3 g1(ceil_div(A, 256), B);
+  dim3 g1(ceil_div(A + max_labels, 256), B);
   nms_filter_kernel<<<g1, 256, 0, s>>>(p);
   MYOLO_LAUNCH_CHECK();
   const size_t smem = (size_t)kSortSmemKeys * 8 + kMaxKept * 16 + kMaxKept * 4 + kChunk * 8 * 4 + kChunk * 16 + kChunk * 4;
@@ -308,4 +356,24 @@ extern "C" int myolo_nms(const float* pred, int B, int A, int no, float conf_thr
   nms_kernel<<<B, 1024, smem, s>>>(p);
   MYOLO_LAUNCH_CHECK();
   return 0;
+}
+
+extern "C" int myolo_nms(const float* pred, int B, int A, int no, float conf_thres, float iou_thres, const int32_t* classes,
+                         int n_classes, int agnostic, int multi_label, int max_det, int max_nms, float max_wh, float* out,
+                         int32_t* out_count, void* workspace, int64_t workspace_bytes, void* stream) {
+  nvtxRangePushA("myolo_nms");
+  struct Pop { ~Pop() { nvtxRangePop(); } } nvtx_pop_;
+  return nms_launch(pred, B, A, no, conf_thres, iou_thres, classes, n_classes, agnostic, multi_label, max_det, max_nms, max_wh, nullptr,
+                    nullptr, 0, nullptr, out, out_count, workspace, workspace_bytes, stream);
+}
+
+extern "C" int myolo_nms_labels(const float* pred, int B, int A, int no, float conf_thres, float iou_thres, const int32_t* classes,
+                                int n_classes, int agnostic, int multi_label, int max_det, int max_nms, float max_wh, const float* labels,
+                                const int32_t* label_offsets, int max_labels, int32_t* err, float* out, int32_t* out_count, void* workspace,
+                                int64_t workspace_bytes, void* stream) {
+  nvtxRangePushA("myolo_nms_labels");
+  struct Pop { ~Pop() { nvtxRangePop(); } } nvtx_pop_;
+  MYOLO_REQUIRE(label_offsets && err && max_labels >= 0 && (labels || max_labels == 0), "nms_labels: null pointer or bad max_labels");
+  return nms_launch(pred, B, A, no, conf_thres, iou_thres, classes, n_classes, agnostic, multi_label, max_det, max_nms, max_wh,
+                    labels, label_offsets, max_labels, err, out, out_count, workspace, workspace_bytes, stream);
 }

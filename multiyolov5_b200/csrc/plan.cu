@@ -1553,6 +1553,15 @@ extern "C" int myolo_det_match(const float* dets, const int32_t* counts, int B, 
                           reinterpret_cast<unsigned long long*>(tcount), err, (cudaStream_t)stream);
 }
 
+extern "C" int myolo_confusion_update(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets,
+                                      int H, int W, const float* geom, int nc, float conf_thres, float iou_thres, int require_rows,
+                                      int64_t* matrix, int32_t* err, void* stream) {
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  return launch_confusion(dets, counts, B, max_det, targets, n_targets, H, W, geom, nc, conf_thres, iou_thres, require_rows,
+                          reinterpret_cast<unsigned long long*>(matrix), err, (cudaStream_t)stream);
+}
+
 extern "C" int64_t myolo_det_ap_workspace_bytes(int n_images, int max_det, int ncol) {
   return det_ap_workspace_bytes(n_images, max_det, ncol);
 }

@@ -190,19 +190,89 @@ def one_cycle(y1=0.0, y2=1.0, steps=100):
     return f
 
 
+def coco80_to_coco91_class():
+    """COCO category ids (1..90 with the ten ids the 2017 detection set leaves unused) of the 80 contiguous class indices"""
+    return [i for i in range(1, 91) if i not in (12, 26, 29, 30, 45, 66, 68, 69, 71, 83)]
+
+
+class NmsLabels:
+    """Apriori labels for non_max_suppression(labels=...) packed for the device (utils/general.py:448-455, test.py --save-hybrid).
+
+        rows      (n, 5) fp32 [cls, x, y, w, h] in network-input pixels, image b's rows at rows[offsets[b]:offsets[b + 1]]
+        offsets   (B + 1) int32
+        max_labels  a bound on any image's label count (n is always one)
+        err       (1,) int32 device word the NMS ORs MYOLO_NMS_ERR_* bits into; check() reads it
+
+    `from_targets` builds it from collate_fn targets on the device without a host round trip, as test.py:175-176 does."""
+
+    def __init__(self, rows, offsets, max_labels, err=None):
+        self.rows = rows.float().contiguous()
+        self.offsets = offsets.to(torch.int32).contiguous()
+        self.max_labels = int(max_labels)
+        self.err = err if err is not None else torch.zeros(1, dtype=torch.int32, device=self.rows.device)
+
+    @classmethod
+    def from_targets(cls, targets, batch_size, img_hw, err=None):
+        """test.py:175-176: targets (n, 6) [image, class, x, y, w, h] normalised, scaled to pixels by (w, h) in fp32; each image's rows
+        keep their order (targets[targets[:, 0] == i, 1:])"""
+        t = targets.float().reshape(-1, 6)
+        height, width = img_hw
+        scale = torch.tensor([1.0, width, height, width, height], dtype=torch.float32, device=t.device)
+        img, order = torch.sort(t[:, 0], stable=True)
+        rows = t[order, 1:] * scale
+        offsets = torch.searchsorted(img.contiguous(), torch.arange(batch_size + 1, dtype=torch.float32, device=t.device))
+        return cls(rows, offsets, t.shape[0], err)
+
+    @classmethod
+    def from_list(cls, labels, nc, device):
+        """the reference's per-image list of (k, 5) [cls, x, y, w, h] tensors; class ids are checked on the host (an id outside [0, nc)
+        is an index error in the reference)"""
+        ls = [torch.as_tensor(l, dtype=torch.float32).reshape(-1, 5) for l in labels]
+        rows = torch.cat(ls).to(device) if ls else torch.zeros((0, 5), device=device)
+        c = rows[:, 0].cpu()
+        if len(c) and not bool(((c > -1) & (c < nc)).all()):
+            raise ValueError(f"label class ids must be in [0, {nc})")
+        sizes = [len(l) for l in ls]
+        offsets = torch.tensor(np.concatenate([[0], np.cumsum(sizes)]), dtype=torch.int32).to(device)
+        return cls(rows, offsets, max(sizes, default=0))
+
+    def check(self):
+        """reads the error word (one synchronisation) and raises on a bad label"""
+        check_nms_labels_error(int(self.err.item()))
+
+
+def check_nms_labels_error(e):
+    """raises for the MYOLO_NMS_ERR_* bits of a myolo_nms_labels error word"""
+    if e & _lib.NMS_ERR_LABEL_CLASS:
+        raise ValueError("a label class id is outside [0, nc)")
+    if e & _lib.NMS_ERR_LABEL_COUNT:
+        raise ValueError("an image has more labels than max_labels")
+
+
 def non_max_suppression(prediction, conf_thres=0.25, iou_thres=0.45, classes=None, agnostic=False, multi_label=False, labels=(),
                         max_det=300, return_padded=False):
     """reference utils/general.py:421-509.  prediction: (B,A,5+nc) fp32 CUDA.  Returns list[(n,6)] like the reference
-    ([x1,y1,x2,y2,conf,cls], descending conf, <=300 rows).  `labels` (auto-labelling apriori boxes) is not on the hot path."""
-    if labels:
-        raise NotImplementedError("non_max_suppression(labels=...) (autolabelling) is out of scope (SURVEY.md section 8)")
+    ([x1,y1,x2,y2,conf,cls], descending conf, <=300 rows).  `labels`: the reference's per-image list of (k, 5) [cls, x, y, w, h] apriori
+    labels (autolabelling), or an NmsLabels; with an NmsLabels and return_padded its error word is left to the caller's check()."""
     if not prediction.is_cuda:
         raise _lib.MyoloError("non_max_suppression needs a CUDA tensor: there is no CPU path in multiyolov5_b200")
     pred = prediction.float().contiguous()
     B, A, no = pred.shape
     L = _lib.lib()
     ml = bool(multi_label) and (no - 5) > 1
-    nbytes = int(L.myolo_nms_workspace_bytes(B, A, no, int(ml)))
+    lab = None
+    if isinstance(labels, NmsLabels):
+        lab = labels
+    elif labels is not None and len(labels):
+        if len(labels) != B:
+            raise ValueError("labels: one (k, 5) entry per image")
+        lab = NmsLabels.from_list(labels, no - 5, pred.device)
+    if lab is not None:
+        if lab.offsets.numel() != B + 1:
+            raise ValueError("labels: offsets must have B + 1 entries")
+        nbytes = int(L.myolo_nms_labels_workspace_bytes(B, A, no, int(ml), lab.max_labels))
+    else:
+        nbytes = int(L.myolo_nms_workspace_bytes(B, A, no, int(ml)))
     key = (pred.device, nbytes)
     ws = _ws_cache.get(key)
     if ws is None:
@@ -211,11 +281,19 @@ def non_max_suppression(prediction, conf_thres=0.25, iou_thres=0.45, classes=Non
     out = torch.zeros((B, max_det, 6), dtype=torch.float32, device=pred.device)
     cnt = torch.empty((B,), dtype=torch.int32, device=pred.device)
     cls_t = torch.tensor(list(classes), dtype=torch.int32, device=pred.device) if classes is not None else None
-    _lib.check(L.myolo_nms(_lib.ptr(pred), B, A, no, float(conf_thres), float(iou_thres), _lib.ptr(cls_t),
-                           0 if cls_t is None else cls_t.numel(), int(bool(agnostic)), int(ml), int(max_det), 30000, 4096.0,
-                           _lib.ptr(out), _lib.ptr(cnt), _lib.ptr(ws), nbytes, _lib.stream_ptr()))
+    if lab is None:
+        _lib.check(L.myolo_nms(_lib.ptr(pred), B, A, no, float(conf_thres), float(iou_thres), _lib.ptr(cls_t),
+                               0 if cls_t is None else cls_t.numel(), int(bool(agnostic)), int(ml), int(max_det), 30000, 4096.0,
+                               _lib.ptr(out), _lib.ptr(cnt), _lib.ptr(ws), nbytes, _lib.stream_ptr()))
+    else:
+        _lib.check(L.myolo_nms_labels(_lib.ptr(pred), B, A, no, float(conf_thres), float(iou_thres), _lib.ptr(cls_t),
+                                      0 if cls_t is None else cls_t.numel(), int(bool(agnostic)), int(ml), int(max_det), 30000, 4096.0,
+                                      _lib.ptr(lab.rows) if lab.rows.numel() else None, _lib.ptr(lab.offsets), lab.max_labels,
+                                      _lib.ptr(lab.err), _lib.ptr(out), _lib.ptr(cnt), _lib.ptr(ws), nbytes, _lib.stream_ptr()))
     if return_padded:
         return out, cnt
+    if lab is not None:
+        lab.check()
     counts = cnt.tolist()  # the one device->host sync, like the reference's shape checks (utils/general.py:458,484)
     return [out[b, :counts[b]] for b in range(B)]
 

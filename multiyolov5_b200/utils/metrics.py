@@ -220,6 +220,100 @@ class DetectionStats:
         return p, r, ap, f1, ap_class, tcount[:nc].astype(np.int64), self.seen
 
 
+class ConfusionMatrix:
+    """The fork's ConfusionMatrix (utils/metrics.py:115-187) with the counters on the device: one `myolo_confusion_update` launch per call,
+    int64 counts read once by `.matrix`.  Row = true class, column = predicted class (the fork's order, the transpose of upstream
+    YOLOv5); row nc holds unmatched labels (background FP), column nc unmatched detections (background FN).  Exactly equal IoUs are
+    broken towards the lower label index, then the lower detection row (the fork's unstable argsort leaves them open).
+
+        process_batch(detections, labels)                one image: (N, 6) [x1, y1, x2, y2, conf, cls], (M, 5) [cls, x1, y1, x2, y2]
+        update(dets, counts, targets, img_hw, shapes)    a batch of padded NMS rows with DetectionStats.update's arguments; only images
+                                                         with labels and rows count, as test.py:189-192 and :233-241 call process_batch
+        matrix                                           float64 (nc + 1, nc + 1) numpy array (synchronises); a fresh copy of the
+                                                         device counters on every read, not the fork's mutable attribute
+        print(), plot(save_dir, names)                   plot() draws confusion_matrix.png only when seaborn and matplotlib import
+
+    One image holds at most 1024 detections and 1024 labels (the fork takes any number); process_batch raises ValueError above
+    that, and update() reports more than 1024 labels in one image when `.matrix` is read."""
+
+    def __init__(self, nc, conf=0.25, iou_thres=0.45, device="cuda"):
+        self.nc, self.conf, self.iou_thres = int(nc), conf, iou_thres
+        self.device = torch.device(device)
+        self.counts = torch.zeros((self.nc + 1, self.nc + 1), dtype=torch.int64, device=self.device)
+        self.err = torch.zeros(1, dtype=torch.int32, device=self.device)
+
+    def _launch(self, dets, counts, B, max_det, targets, H, W, geom, require_rows):
+        tg = targets.reshape(-1, 6)
+        _lib.check(_lib.lib().myolo_confusion_update(_lib.ptr(dets), _lib.ptr(counts), B, max_det, _lib.ptr(tg) if tg.numel() else None,
+                                                     int(tg.shape[0]), int(H), int(W), _lib.ptr(geom), self.nc, float(self.conf),
+                                                     float(self.iou_thres), int(require_rows), _lib.ptr(self.counts), _lib.ptr(self.err),
+                                                     _lib.stream_ptr()))
+
+    def process_batch(self, detections, labels):
+        d = _to_device(detections, self.device, torch.float32).reshape(-1, 6)
+        lb = _to_device(labels, self.device, torch.float32).reshape(-1, 5)
+        n = d.shape[0]
+        if n > 1024 or lb.shape[0] > 1024:
+            raise ValueError("ConfusionMatrix.process_batch takes at most 1024 detections and 1024 labels per image")
+        dets = d if n else torch.zeros((1, 6), device=self.device)
+        cnt = torch.tensor([n], dtype=torch.int32).pin_memory().to(self.device, non_blocking=True)
+        tg = torch.cat([torch.zeros((lb.shape[0], 1), device=self.device), lb], 1).contiguous()
+        self._launch(dets.contiguous(), cnt, 1, max(n, 1), tg, 0, 0, None, 0)
+
+    def update(self, dets, counts, targets, img_hw, shapes):
+        B, max_det, six = dets.shape
+        if six != 6 or len(shapes) != B:
+            raise ValueError("dets must be (B, max_det, 6) padded NMS rows with one shapes entry per image")
+        if not dets.is_cuda:
+            raise _lib.MyoloError("ConfusionMatrix.update needs the device NMS output")
+        geom = _to_device(pack_geometry(img_hw, shapes), dets.device, torch.float32)
+        tg = _to_device(targets, dets.device, torch.float32).reshape(-1, 6)
+        self._launch(dets.float().contiguous(), counts.to(torch.int32).contiguous(), B, max_det, tg, img_hw[0], img_hw[1], geom, 1)
+
+    @property
+    def matrix(self):
+        head = torch.cat([self.err.long(), self.counts.reshape(-1)]).cpu().numpy()
+        err = int(head[0])
+        if err & _lib.DET_ERR_TARGET_CLASS:
+            raise ValueError(f"label class ids must be integers in [0, {self.nc})")
+        if err & _lib.DET_ERR_PRED_CLASS:
+            raise ValueError(f"detection class ids must be integers in [0, {self.nc})")
+        if err & _lib.DET_ERR_LABELS:
+            raise ValueError("an image has more than 1024 labels")
+        return head[1:].reshape(self.nc + 1, self.nc + 1).astype(np.float64)
+
+    def plot(self, save_dir="", names=()):
+        """the fork's plot: any failure of the drawing, a missing seaborn or matplotlib included, draws nothing.  A bad class id in the
+        counted batches still raises: the matrix is read before the drawing starts."""
+        matrix = self.matrix
+        try:
+            import matplotlib
+            matplotlib.use("Agg")
+            import matplotlib.pyplot as plt
+            import seaborn as sn
+            from pathlib import Path
+
+            array = matrix / (matrix.sum(0).reshape(1, self.nc + 1) + 1E-6)  # normalize
+            array[array < 0.005] = np.nan  # don't annotate (would appear as 0.00)
+            fig = plt.figure(figsize=(12, 9), tight_layout=True)
+            sn.set(font_scale=1.0 if self.nc < 50 else 0.8)
+            labels = (0 < len(names) < 99) and len(names) == self.nc
+            sn.heatmap(array, annot=self.nc < 30, annot_kws={"size": 8}, cmap="Blues", fmt=".2f", square=True,
+                       xticklabels=list(names) + ["background FP"] if labels else "auto",
+                       yticklabels=list(names) + ["background FN"] if labels else "auto").set_facecolor((1, 1, 1))
+            fig.axes[0].set_xlabel("True")
+            fig.axes[0].set_ylabel("Predicted")
+            fig.savefig(Path(save_dir) / "confusion_matrix.png", dpi=250)
+            plt.close(fig)
+        except Exception:
+            pass
+
+    def print(self):
+        m = self.matrix
+        for i in range(self.nc + 1):
+            print(" ".join(map(str, m[i])))
+
+
 def _class_ids(a, what):
     a = np.asarray(a.cpu().numpy() if isinstance(a, torch.Tensor) else a).reshape(-1)
     if len(a) and not (np.all(a >= 0) and np.all(a < 256) and np.all(a == np.floor(a))):
