@@ -103,8 +103,6 @@ typedef struct myolo_plan myolo_plan;
 /* ---- library ---- */
 int myolo_abi_version(void);
 const char* myolo_last_error(void);
-/* fills name (<=255 chars), SM count, compute capability major/minor of the current device */
-int myolo_device_info(char* name, int* sm_count, int* cc_major, int* cc_minor);
 
 /* ---- layer plan: what Model.__init__/fuse + forward_once become ---- */
 int myolo_plan_create(const myolo_op* ops, int n_ops, const myolo_buf_desc* bufs, int n_bufs,
@@ -116,7 +114,7 @@ int myolo_plan_create(const myolo_op* ops, int n_ops, const myolo_buf_desc* bufs
  * The addresses are baked into the plan's tensor maps and captured graphs: they must stay valid, at the same address, for the plan's life.
  * The caller zeroes `ws` before the plan's first forward and again whenever another plan has written it since (the plan reads some
  * never-written bytes, e.g. zero-padded channels, as zeros).  myolo_plan_destroy never frees them.
- * The library does not track which plan wrote the shared workspaces last: a backward (myolo_plan_backward*, myolo_plan_backward_seg_ce)
+ * The library does not track which plan wrote the shared workspaces last: a backward (myolo_plan_backward_multi, myolo_plan_backward_seg_*)
  * after ANOTHER plan's train forward on the same pair reads that plan's activations as its own and returns wrong gradients without an
  * error.  The caller keeps one outstanding train forward per pair: forward, backward, then the next plan's forward (the Python engine
  * refuses such a stale backward before it launches). */
@@ -154,8 +152,9 @@ int myolo_plan_forward_pass(myolo_plan* plan, const void* x, int x_dtype, float*
 int myolo_plan_read_view(myolo_plan* plan, myolo_view view, float* dst_nchw, void* stream);
 /* number of kernels the last myolo_plan_forward launched (bench.py's gpu_launches) */
 int64_t myolo_plan_last_launch_count(const myolo_plan* plan);
-/* which kernel conv op `op_index` takes and its tiling: info[12] = {1 wgmma / 0 CUDA-core, grid, smem bytes, BN, stages, mode (always 0:
- * one TMA box per tap), weights-stationary (0), tiles per round (1), tiles, N tiles, kc, CTAs per SM (1)}.  Feeds bench.py's roofline record. */
+/* which kernel conv op `op_index` takes and its tiling: info[12] = {1 wgmma / 0 CUDA-core, grid, smem bytes, BN, stages, strip (1: one
+ * input strip per filter row, 0: one TMA box per tap), resident (1: the CTA keeps its weight slice in shared memory), always 1, tiles,
+ * N tiles, kc, CTAs per SM (1 or 2)}.  Feeds bench.py's roofline record. */
 int myolo_plan_conv_info(myolo_plan* plan, int op_index, int32_t* info);
 /* per-op device time of the next forward (CUDA events around every op; host array of n_ops floats, ms) */
 int myolo_plan_profile(myolo_plan* plan, const void* x, int x_dtype, float* z, float* const* raw, void* seg, int seg_dtype,
@@ -187,14 +186,12 @@ int myolo_plan_apply_running(myolo_plan* plan, void* stream);
  * Both null: off.  Both set: MYOLO_E_INVALID.  Not with myolo_plan_set_defer_running.  A synchronised plan runs its forward and backward
  * in order on the caller's stream, without CUDA-graph replay.  Every BN layer must have C % 8 == 0 and C <= 2048. */
 int myolo_plan_set_bn_sync(myolo_plan* plan, void* nccl_comm, const int32_t* rank_images, int n_groups);
-/* train-mode forward: raw[i] (B,na,ny,nx,no) fp32 and seg (B,n_segcls,H,W) fp32, like Model.forward in training (models/yolo.py:225,316) */
-int myolo_plan_train_forward(myolo_plan* plan, const void* x, int x_dtype, float* const* raw, float* seg, void* stream);
-/* backward of the last train forward: grad_raw[i] / grad_seg are dL/d(raw[i]) / dL/d(seg) (fp32, nullable); parameter gradients are
- * ACCUMULATED into the registered pointers (the reference accumulates the det and the seg pass, train.py:371,392) */
-int myolo_plan_backward(myolo_plan* plan, const float* const* grad_raw, const float* grad_seg, void* stream);
-/* BiSe head in train mode returns three seg outputs [out, aux16, aux32] (reference models/yolo.py:70-79,86): seg[k] / grad_seg[k]
- * are arrays of three fp32 (B,n_segcls,H,W) pointers (nullable entries; k = 0 is the main output) */
+/* train-mode forward: raw[i] (B,na,ny,nx,no) fp32 and the seg outputs, like Model.forward in training (models/yolo.py:225,316).  seg is
+ * nullable or an array of three fp32 (B,n_segcls,H,W) pointers (nullable entries; k = 0 is the main output): the BiSe head in train mode
+ * returns three seg outputs [out, aux16, aux32] (reference models/yolo.py:70-79,86). */
 int myolo_plan_train_forward_multi(myolo_plan* plan, const void* x, int x_dtype, float* const* raw, float* const* seg, void* stream);
+/* backward of the last train forward: grad_raw[i] / grad_seg[k] are dL/d(raw[i]) / dL/d(seg[k]) (fp32, nullable; grad_seg as seg above);
+ * parameter gradients are ACCUMULATED into the registered pointers (the reference accumulates the det and the seg pass, train.py:371,392) */
 int myolo_plan_backward_multi(myolo_plan* plan, const float* const* grad_raw, const float* const* grad_seg, void* stream);
 /* Fused segmentation loss (SURVEY.md section 8f rank 3): mean CrossEntropyLoss(ignore_index) of the bilinear(align_corners) upsample of the
  * last train forward's low-resolution logits against `labels` (B,H,W) int64, WITHOUT materialising the full-resolution logits or their
@@ -220,33 +217,12 @@ int myolo_plan_backward_seg_loss(myolo_plan* plan, const int64_t* labels, int ig
                                  float factor, const float* scale_dev, float* loss_out, void* stream);
 /* debug: like myolo_plan_read_view, from the gradient workspace of the last backward */
 int myolo_plan_read_grad_view(myolo_plan* plan, myolo_view view, float* dst_nchw_f32, void* stream);
+int myolo_grads_check_finite(const float* grad, int64_t n, int32_t* found_inf /* device */, void* stream);
 /* Optimiser step over FLAT fp32 buffers (all parameters of the model laid out back to back; `group[i]` in 0..n_groups-1 selects the
  * lr / weight decay of element i): torch.optim.SGD(momentum, nesterov) as configured by reference train.py:108-126 (pg0 BN weights,
  * pg1 conv weights + decay, pg2 biases).  Gradients are multiplied by *inv_scale (device scalar: 1 / (loss scale x world size),
  * nullable = 1); when *found_inf != 0 the update is skipped (amp.GradScaler.step, train.py:396); zero_grad clears the gradients in the
  * same pass (optimizer.zero_grad, train.py:398).  lr / weight_decay are HOST arrays of n_groups (<= 4) floats. */
-/* standalone weight gradient of one conv (per-op parity tests / ncu): x (B,H,W,ci) and dy (B,Ho,Wo,co) NHWC fp16, "same" padding
- * dil*(k/2); dW fp32 [co][ci][k][k] is ACCUMULATED into.  path 0: mma.sync kernel, 1: wgmma kernel (needs ci % 64 == 0, Wo % 16 == 0) */
-int myolo_conv_wgrad(const void* x, const void* dy, int B, int H, int W, int ci, int co, int k, int stride, int dil, float* dW, int path,
-                     void* stream);
-/* standalone backward of one conv through the train plan's own routing and launches (per-op tests).  Views are channel slices of NHWC
- * buffers (base of the buffer, channels per pixel ctot, first channel c_off), as the plan passes them:
- *   x     (B,H,W) fp16 / fp32, ci rounded up to 16 channels (the padding channels hold zeros);
- *   dy    (B,Ho,Wo) fp16 with co channels, or an fp32 head gradient with co rounded up to 16 (zero padding);
- *   gin   grad(in), nullable (no data gradient), x's dtype and channel count: ACCUMULATED into;
- *   w     fp32 master weights [co][ci][k][k]; dW (same layout) and dbias [co] (nullable) are ACCUMULATED into.
- * "same" padding dil*(k/2).  route: 0 as the plan, or MYOLO_CONV_BWD_* bits.  info (nullable) receives 16 slots:
- *   0  data gradient: 0 none, 1 small (generic kernel, fp32 weights), 2 wgmma conv, 3 CUDA-core conv
- *   1  weight gradient: 1 small, 2 mma.sync, 3 wgmma into dW, 4 wgmma through a packed buffer
- *   2  bias gradient: 0 none, 1 summed from fp32 dY, 2 from fp16 dY
- *   3-7  wgmma data gradient: kc, BN, CTAs per SM, weights resident, strip mode;  13-14: N tiles, padded output channels of the pack
- *   8-12 wgmma weight gradient: pixels per step Kc, N, row slabs, rows per slab, rows in all */
-#define MYOLO_CONV_BWD_SIMT 1          /* data gradient on the CUDA-core conv (as MYOLO_FORCE_SIMT=1 does for a plan) */
-#define MYOLO_CONV_BWD_NO_WGRAD_TC 2   /* weight gradient on the mma.sync kernel where the wgmma one would run */
-int myolo_conv_backward(const void* x, int x_dtype, int B, int H, int W, int x_ctot, int x_coff, const void* dy, int dy_dtype, int dy_ctot,
-                        int dy_coff, void* gin, int gin_ctot, int gin_coff, const float* w, int co, int ci, int k, int stride, int dil,
-                        float* dW, float* dbias, int route, int32_t* info, void* stream);
-int myolo_grads_check_finite(const float* grad, int64_t n, int32_t* found_inf /* device */, void* stream);
 int myolo_sgd_step(float* param, float* grad, float* momentum_buf, const uint8_t* group, int64_t n, const float* lr,
                    const float* weight_decay, int n_groups, float momentum, int nesterov, const float* inv_scale /* device */,
                    const int32_t* found_inf /* device, nullable */, int zero_grad, void* stream);
@@ -428,11 +404,13 @@ int myolo_letterbox_items(const uint8_t* src, const myolo_letterbox_item* items,
 /* ---- detection training batches (reference utils/datasets.py:518-593 LoadImagesAndLabels.__getitem__, augment=True) ----
  * myolo_resize_u8: cv2.resize(src, (W, H), INTER_LINEAR) of one uint8 HWC image (H0,W0,3) into dst (H,W,3), bit exact with OpenCV's
  * 8-bit path (exact 2x down-scaling takes its area path): `load_image`'s resize to long side img_size (:629-643) for the device cache.
- * myolo_augment_det: one batch of B augmented S x S images.  items: DEVICE array of B myolo_aug_item, built on the host from the
- * reference's random draws (multiyolov5_b200/utils/datasets.py DetAugmenter).  Per output pixel: cv2.warpAffine (INTER_LINEAR, border 114)
- * of the virtual canvas of warp[0] (mosaic tiles or a letterboxed image, 114 elsewhere), optionally mixed with warp[1]
- * (trunc(a*mix_r + b*mix_q) in double), augment_hsv through the three LUTs, flipud / fliplr, BGR->RGB.
- * out: (B,3,S,S) of out_dtype MYOLO_U8 / MYOLO_F16 / MYOLO_F32 (float = value / 255, as imgs.float() / 255 on the GPU). */
+ * myolo_augment_det_hw: one batch of B augmented H x W images: the S x S batches of H = W = S, or the `--rect` batches at their batch
+ * shape (`LoadImagesAndLabels(augment=True, rect=True)`: a letterbox to the batch shape, random_perspective at (W, H), flips over H and W).
+ * items: DEVICE array of B myolo_aug_item, built on the host from the reference's random draws (multiyolov5_b200/utils/datasets.py
+ * DetAugmenter, DetRectLoader).  Per output pixel: cv2.warpAffine (INTER_LINEAR, border 114) of the virtual canvas of warp[0] (mosaic
+ * tiles or a letterboxed image, 114 elsewhere), optionally mixed with warp[1] (trunc(a*mix_r + b*mix_q) in double), augment_hsv through
+ * the three LUTs, flipud / fliplr, BGR->RGB.
+ * out: (B,3,H,W) of out_dtype MYOLO_U8 / MYOLO_F16 / MYOLO_F32 (float = value / 255, as imgs.float() / 255 on the GPU). */
 typedef struct {
   const uint8_t* src[4];  /* tile images: HWC BGR uint8, device */
   int32_t rect[4][4];     /* canvas rectangle [x1, x2) x [y1, y2) covered by tile t: x1, y1, x2, y2 */
@@ -471,9 +449,6 @@ int myolo_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, i
  * resamples src.flip(3) instead.  src and dst share dtype, MYOLO_F16 or MYOLO_F32. */
 int myolo_scale_img(const void* src, int dtype, int B, int C, int H, int W, void* dst, int Ho, int Wo, int Hp, int Wp, int flip_lr,
                     float pad_value, void* stream);
-int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, void* stream);
-/* myolo_augment_det_hw: the same per-pixel work on B augmented H x W images (`LoadImagesAndLabels(augment=True, rect=True)`: a letterbox
- * to the batch shape, random_perspective at (W, H), flips over H and W), out (B,3,H,W).  myolo_augment_det is its H = W = S case. */
 int myolo_augment_det_hw(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, void* stream);
 
 /* myolo_collate_quad: the pixels of `--quad`'s LoadImagesAndLabels.collate_fn4 (reference utils/datasets.py:602-625) over one drawn batch,
@@ -633,21 +608,23 @@ int myolo_conv_forward(const void* x, int x_dtype, int B, int H, int W, int x_ct
                        const void* res, int res_ctot, int res_coff, const float* w, int co, int ci, int k, int stride, int dil,
                        const float* gamma, const float* beta, const float* mean, const float* var, float eps, const float* bias, int act,
                        int path, int32_t* info, void* stream);
-/* SiLU(conv(x)*bnscale+bnshift) on NHWC fp16: x (B,H,W,Ci) -> y (B,Ho,Wo,Co); w fp32 [Co][Ci][k][k]; path: 0 auto, 1 wgmma, 2 simt, 3 wgmma (same kernel as 1).
- * myolo_conv_forward on whole buffers (Ci % 16 == 0) */
-int myolo_conv_bn_silu(const void* x_nhwc_f16, int B, int H, int W, int ci, const float* w, int co, int k, int stride,
-                       int dil, const float* gamma, const float* beta, const float* mean, const float* var, float eps,
-                       const float* bias, int act, const void* residual_nhwc_f16, void* y_nhwc_f16, int path, void* stream);
-/* the same into a channel slice: y points at the slice's first channel of pixel 0 of a buffer with y_ctot channels per pixel */
-int myolo_conv_bn_silu_slice(const void* x_nhwc_f16, int B, int H, int W, int ci, const float* w, int co, int k, int stride,
-                             int dil, const float* gamma, const float* beta, const float* mean, const float* var, float eps,
-                             const float* bias, int act, const void* residual_nhwc_f16, void* y_nhwc_f16, int y_ctot, int path,
-                             void* stream);
-/* the same, and reports the launch's routing in info[0..11] (the slots of myolo_plan_conv_info) */
-int myolo_conv_bn_silu_info(const void* x_nhwc_f16, int B, int H, int W, int ci, const float* w, int co, int k, int stride,
-                            int dil, const float* gamma, const float* beta, const float* mean, const float* var, float eps,
-                            const float* bias, int act, const void* residual_nhwc_f16, void* y_nhwc_f16, int y_ctot, int path,
-                            int32_t* info, void* stream);
+/* standalone backward of one conv through the train plan's own routing and launches (per-op tests).  Views are channel slices of NHWC
+ * buffers (base of the buffer, channels per pixel ctot, first channel c_off), as the plan passes them:
+ *   x     (B,H,W) fp16 / fp32, ci rounded up to 16 channels (the padding channels hold zeros);
+ *   dy    (B,Ho,Wo) fp16 with co channels, or an fp32 head gradient with co rounded up to 16 (zero padding);
+ *   gin   grad(in), nullable (no data gradient), x's dtype and channel count: ACCUMULATED into;
+ *   w     fp32 master weights [co][ci][k][k]; dW (same layout) and dbias [co] (nullable) are ACCUMULATED into.
+ * "same" padding dil*(k/2).  route: 0 as the plan, or MYOLO_CONV_BWD_* bits.  info (nullable) receives 16 slots:
+ *   0  data gradient: 0 none, 1 small (generic kernel, fp32 weights), 2 wgmma conv, 3 CUDA-core conv
+ *   1  weight gradient: 1 small, 2 mma.sync, 3 wgmma into dW, 4 wgmma through a packed buffer
+ *   2  bias gradient: 0 none, 1 summed from fp32 dY, 2 from fp16 dY
+ *   3-7  wgmma data gradient: kc, BN, CTAs per SM, weights resident, strip mode;  13-14: N tiles, padded output channels of the pack
+ *   8-12 wgmma weight gradient: pixels per step Kc, N, row slabs, rows per slab, rows in all */
+#define MYOLO_CONV_BWD_SIMT 1          /* data gradient on the CUDA-core conv (as MYOLO_FORCE_SIMT=1 does for a plan) */
+#define MYOLO_CONV_BWD_NO_WGRAD_TC 2   /* weight gradient on the mma.sync kernel where the wgmma one would run */
+int myolo_conv_backward(const void* x, int x_dtype, int B, int H, int W, int x_ctot, int x_coff, const void* dy, int dy_dtype, int dy_ctot,
+                        int dy_coff, void* gin, int gin_ctot, int gin_coff, const float* w, int co, int ci, int k, int stride, int dil,
+                        float* dW, float* dbias, int route, int32_t* info, void* stream);
 
 #ifdef __cplusplus
 }

@@ -30,12 +30,11 @@ OP_DROPOUT = 17
 OP_GROUP_HEAD, OP_GROUP_MEMBER = 2, 4      # include/myolo.h: consecutive ops of one kind executed as one launch
 
 EXPORTS = [
-    "myolo_abi_version", "myolo_last_error", "myolo_device_info", "myolo_plan_create", "myolo_plan_destroy",
+    "myolo_abi_version", "myolo_last_error", "myolo_plan_create", "myolo_plan_destroy",
     "myolo_plan_set_conv_weights", "myolo_plan_repack_weights", "myolo_plan_forward", "myolo_plan_read_view", "myolo_plan_last_launch_count",
     "myolo_plan_profile", "myolo_nms_workspace_bytes", "myolo_nms", "myolo_seg_upsample_argmax", "myolo_bilinear_nchw",
-    "myolo_conv_bn_silu", "myolo_conv_bn_silu_slice", "myolo_conv_bn_silu_info", "myolo_plan_set_bn", "myolo_plan_set_conv_grad", "myolo_plan_train_forward", "myolo_plan_backward",
-    "myolo_grads_check_finite", "myolo_sgd_step", "myolo_conv_wgrad", "myolo_letterbox", "myolo_seg_lut_blend", "myolo_seg_metrics", "myolo_plan_backward_seg_ce", "myolo_plan_read_grad_view", "myolo_plan_set_seed", "myolo_plan_train_forward_multi", "myolo_plan_backward_multi", "myolo_plan_conv_info", "myolo_allreduce_grads", "myolo_det_loss", "myolo_det_loss_workspace_bytes", "myolo_plan_set_defer_running", "myolo_plan_apply_running",
-    "myolo_resize_u8", "myolo_augment_det", "myolo_augment_seg", "myolo_det_match", "myolo_det_ap", "myolo_det_ap_workspace_bytes",
+    "myolo_plan_set_bn", "myolo_plan_set_conv_grad", "myolo_grads_check_finite", "myolo_sgd_step", "myolo_letterbox", "myolo_seg_lut_blend", "myolo_seg_metrics", "myolo_plan_backward_seg_ce", "myolo_plan_read_grad_view", "myolo_plan_set_seed", "myolo_plan_train_forward_multi", "myolo_plan_backward_multi", "myolo_plan_conv_info", "myolo_allreduce_grads", "myolo_det_loss", "myolo_det_loss_workspace_bytes", "myolo_plan_set_defer_running", "myolo_plan_apply_running",
+    "myolo_resize_u8", "myolo_augment_seg", "myolo_det_match", "myolo_det_ap", "myolo_det_ap_workspace_bytes",
     "myolo_resize_area_u8", "myolo_resize_bilinear", "myolo_plan_create_shared", "myolo_augment_det_hw", "myolo_adam_step",
     "myolo_adam_scalars", "myolo_ema_update", "myolo_plan_set_extra", "myolo_collate_quad", "myolo_plan_set_bn_sync",
     "myolo_plan_backward_seg_ohem", "myolo_seg_ohem_loss", "myolo_seg_ohem_loss_backward", "myolo_seg_ohem_loss_workspace_bytes",
@@ -114,7 +113,6 @@ def lib():
     vp, i32, i64, f32 = C.c_void_p, C.c_int, C.c_int64, C.c_float
     L.myolo_abi_version.restype = i32
     L.myolo_last_error.restype = C.c_char_p
-    L.myolo_device_info.argtypes = [C.c_char_p, C.POINTER(i32), C.POINTER(i32), C.POINTER(i32)]
     L.myolo_plan_create.argtypes = [C.POINTER(Op), i32, C.POINTER(BufDesc), i32, C.POINTER(C.c_int32), i32, i32, i32, i32, i64,
                                     i32, C.POINTER(vp)]
     L.myolo_plan_create_shared.argtypes = [C.POINTER(Op), i32, C.POINTER(BufDesc), i32, C.POINTER(C.c_int32), i32, i32, i32, i32, i64,
@@ -131,14 +129,11 @@ def lib():
     L.myolo_plan_profile.argtypes = [vp, vp, i32, vp, C.POINTER(vp), vp, i32, vp, C.POINTER(f32), vp]
     L.myolo_plan_set_bn.argtypes = [vp, i32, i32, vp, vp, vp, vp, vp, vp, f32, f32]
     L.myolo_plan_set_conv_grad.argtypes = [vp, i32, vp, vp]
-    L.myolo_plan_train_forward.argtypes = [vp, vp, i32, C.POINTER(vp), vp, vp]
-    L.myolo_plan_backward.argtypes = [vp, C.POINTER(vp), vp, vp]
     L.myolo_letterbox.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp, vp, i32, i32, i32, vp]
     L.myolo_resize_u8.argtypes = [vp, i32, i32, vp, i32, i32, vp]
     L.myolo_resize_area_u8.argtypes = [vp, i32, i32, vp, i32, i32, vp]
     L.myolo_resize_bilinear.argtypes = [vp, i32, i32, i32, i32, i32, vp, i32, i32, i32, vp]
     L.myolo_scale_img.argtypes = [vp, i32, i32, i32, i32, i32, vp, i32, i32, i32, i32, i32, f32, vp]
-    L.myolo_augment_det.argtypes = [vp, i32, i32, vp, i32, vp]
     L.myolo_augment_det_hw.argtypes = [vp, i32, i32, i32, vp, i32, vp]
     L.myolo_collate_quad.argtypes = [vp, i32, i32, i32, vp, vp, i32, vp]
     L.myolo_augment_seg.argtypes = [vp, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp, vp]
@@ -183,7 +178,6 @@ def lib():
     L.myolo_plan_set_bn_sync.argtypes = [vp, vp, C.POINTER(C.c_int32), i32]
     L.myolo_plan_train_forward_multi.argtypes = [vp, vp, i32, C.POINTER(vp), C.POINTER(vp), vp]
     L.myolo_plan_backward_multi.argtypes = [vp, C.POINTER(vp), C.POINTER(vp), vp]
-    L.myolo_conv_wgrad.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp]
     L.myolo_conv_backward.argtypes = [vp, i32, i32, i32, i32, i32, i32, vp, i32, i32, i32, vp, i32, i32, vp, i32, i32, i32, i32, i32, vp, vp,
                                       i32, C.POINTER(C.c_int32), vp]
     L.myolo_grads_check_finite.argtypes = [vp, i64, vp, vp]
@@ -207,11 +201,6 @@ def lib():
     L.myolo_nms_labels.argtypes = [vp, i32, i32, i32, f32, f32, vp, i32, i32, i32, i32, i32, f32, vp, vp, i32, vp, vp, vp, vp, i64, vp]
     L.myolo_seg_upsample_argmax.argtypes = [vp, i32, i32, i32, i32, i32, i32, i32, vp, i32, vp]
     L.myolo_bilinear_nchw.argtypes = [vp, i32, i32, i32, i32, i32, i32, vp, vp]
-    L.myolo_conv_bn_silu.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, vp]
-    L.myolo_conv_bn_silu_slice.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, i32,
-                                           vp]
-    L.myolo_conv_bn_silu_info.argtypes = [vp, i32, i32, i32, i32, vp, i32, i32, i32, i32, vp, vp, vp, vp, f32, vp, i32, vp, vp, i32, i32,
-                                          C.POINTER(C.c_int32), vp]
     L.myolo_conv_forward.argtypes = [vp, i32, i32, i32, i32, i32, i32, vp, i32, i32, i32, vp, i32, i32, vp, i32, i32, i32, i32, i32, vp, vp, vp,
                                      vp, f32, vp, i32, i32, C.POINTER(C.c_int32), vp]
     for name in EXPORTS:

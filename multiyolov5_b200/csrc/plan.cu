@@ -195,21 +195,6 @@ static int resolve_view(const myolo_plan* pl, const myolo_view& v, TensorView* o
 extern "C" int myolo_abi_version(void) { return MYOLO_ABI_VERSION; }
 extern "C" const char* myolo_last_error(void) { return g_err; }
 
-extern "C" int myolo_device_info(char* name, int* sm_count, int* cc_major, int* cc_minor) {
-  int dev = 0;
-  MYOLO_CHECK_CUDA(cudaGetDevice(&dev));
-  cudaDeviceProp prop;
-  MYOLO_CHECK_CUDA(cudaGetDeviceProperties(&prop, dev));
-  if (name) {
-    strncpy(name, prop.name, 255);
-    name[255] = 0;
-  }
-  if (sm_count) *sm_count = prop.multiProcessorCount;
-  if (cc_major) *cc_major = prop.major;
-  if (cc_minor) *cc_minor = prop.minor;
-  return 0;
-}
-
 // shared_ws / shared_gws: caller-owned activation / gradient workspaces of shared_capacity bytes each (myolo_plan_create_shared), or
 // null: the plan allocates (and frees) private ones
 static int plan_create(const myolo_op* ops, int n_ops, const myolo_buf_desc* bufs, int n_bufs, const int32_t* extra, int n_extra, int B,
@@ -976,17 +961,11 @@ extern "C" int myolo_plan_set_conv_grad(myolo_plan* pl, int slot, float* d_weigh
   return 0;
 }
 
-extern "C" int myolo_plan_train_forward(myolo_plan* pl, const void* x, int x_dtype, float* const* raw, float* seg, void* stream);
 extern "C" int myolo_plan_train_forward_multi(myolo_plan* pl, const void* x, int x_dtype, float* const* raw, float* const* seg, void* stream) {
-  NvtxRange nvtx_("myolo_plan_train_forward");
-  MYOLO_REQUIRE(pl, "train_forward: null plan");
+  NvtxRange nvtx_("myolo_plan_train_forward_multi");
+  MYOLO_REQUIRE(pl && x, "train_forward: null plan / input");
   pl->seg_outs[1] = seg ? seg[1] : nullptr;
   pl->seg_outs[2] = seg ? seg[2] : nullptr;
-  return myolo_plan_train_forward(pl, x, x_dtype, raw, seg ? seg[0] : nullptr, stream);
-}
-
-extern "C" int myolo_plan_train_forward(myolo_plan* pl, const void* x, int x_dtype, float* const* raw, float* seg, void* stream) {
-  MYOLO_REQUIRE(pl && x, "train_forward: null plan / input");
   if (!pl->d_step) {
     MYOLO_CHECK_CUDA(cudaMalloc(&pl->d_step, sizeof(unsigned long long)));
     MYOLO_CHECK_CUDA(cudaMemset(pl->d_step, 0, sizeof(unsigned long long)));
@@ -997,7 +976,7 @@ extern "C" int myolo_plan_train_forward(myolo_plan* pl, const void* x, int x_dty
   }
   // same executor as inference: first call in order (lazy allocations / tensor maps), then CUDA-graph replay of the internal
   // ops with the input conversion before and the caller-owned outputs (raw x_i, seg logits) after the graph
-  int rc = myolo_plan_forward(pl, x, x_dtype, nullptr, raw, seg, MYOLO_F32, nullptr, stream);
+  int rc = myolo_plan_forward(pl, x, x_dtype, nullptr, raw, seg ? seg[0] : nullptr, MYOLO_F32, nullptr, stream);
   if (rc) return rc;
   pl->train_fwd_done = true;
   return 0;
@@ -1268,19 +1247,8 @@ static int backward_run(myolo_plan* pl, int mask, std::vector<char>& live, cudaS
   return 0;
 }
 
-extern "C" int myolo_plan_backward(myolo_plan* pl, const float* const* grad_raw, const float* grad_seg, void* stream);
-extern "C" int myolo_plan_backward_multi(myolo_plan* pl, const float* const* grad_raw, const float* const* grad_seg, void* stream) {
-  NvtxRange nvtx_("myolo_plan_backward");
-  MYOLO_REQUIRE(pl, "backward: null plan");
-  pl->grad_segs[1] = grad_seg ? grad_seg[1] : nullptr;
-  pl->grad_segs[2] = grad_seg ? grad_seg[2] : nullptr;
-  int rc = myolo_plan_backward(pl, grad_raw, grad_seg ? grad_seg[0] : nullptr, stream);
-  pl->grad_segs[1] = pl->grad_segs[2] = nullptr;
-  return rc;
-}
-
-extern "C" int myolo_plan_backward(myolo_plan* pl, const float* const* grad_raw, const float* grad_seg, void* stream) {
-  MYOLO_REQUIRE(pl && pl->train_fwd_done, "backward: call myolo_plan_train_forward first");
+static int plan_backward(myolo_plan* pl, const float* const* grad_raw, const float* grad_seg, void* stream) {
+  MYOLO_REQUIRE(pl->train_fwd_done, "backward: call myolo_plan_train_forward_multi first");
   cudaStream_t s = (cudaStream_t)stream;
   if (!pl->gws) MYOLO_CHECK_CUDA(cudaMalloc(&pl->gws, pl->ws_bytes));
   MYOLO_CHECK_CUDA(cudaMemsetAsync(pl->gws, 0, pl->ws_bytes, s));
@@ -1295,12 +1263,22 @@ extern "C" int myolo_plan_backward(myolo_plan* pl, const float* const* grad_raw,
   return backward_run(pl, mask, live, s);
 }
 
+extern "C" int myolo_plan_backward_multi(myolo_plan* pl, const float* const* grad_raw, const float* const* grad_seg, void* stream) {
+  NvtxRange nvtx_("myolo_plan_backward_multi");
+  MYOLO_REQUIRE(pl, "backward: null plan");
+  pl->grad_segs[1] = grad_seg ? grad_seg[1] : nullptr;
+  pl->grad_segs[2] = grad_seg ? grad_seg[2] : nullptr;
+  int rc = plan_backward(pl, grad_raw, grad_seg ? grad_seg[0] : nullptr, stream);
+  pl->grad_segs[1] = pl->grad_segs[2] = nullptr;
+  return rc;
+}
+
 // fused seg loss (SURVEY.md section 8f rank 3): CE(ignore_index) of the x8-upsampled logits of the last train forward is evaluated and
 // differentiated straight from the low-resolution logits; the backward then runs as the seg pass (seed mask 8)
 // ohem: OhemCELoss(thresh) with thresh_t = -log(thresh) instead of the mean CE; wf: the class-weighted CE / focal loss (weights, gamma)
 static int backward_seg_fused(myolo_plan* pl, const int64_t* labels, int ignore_index, float factor, const float* scale_dev, float* loss_out,
                               cudaStream_t s, bool ohem, float thresh_t, bool wf = false, const float* weights = nullptr, float gamma = 0.f) {
-  MYOLO_REQUIRE(pl && pl->train_fwd_done && labels, "backward_seg_ce: call myolo_plan_train_forward first / null labels");
+  MYOLO_REQUIRE(pl && pl->train_fwd_done && labels, "backward_seg_ce: call myolo_plan_train_forward_multi first / null labels");
   if (!pl->gws) MYOLO_CHECK_CUDA(cudaMalloc(&pl->gws, pl->ws_bytes));
   MYOLO_CHECK_CUDA(cudaMemsetAsync(pl->gws, 0, pl->ws_bytes, s));
   if (!pl->ce_scratch) MYOLO_CHECK_CUDA(cudaMalloc(&pl->ce_scratch, 16));
@@ -1474,12 +1452,6 @@ extern "C" int myolo_resize_area_u8(const uint8_t* src, int H0, int W0, uint8_t*
   return launch_resize_area_u8(src, H0, W0, dst, H, W, (cudaStream_t)stream);
 }
 
-extern "C" int myolo_augment_det(const myolo_aug_item* items, int B, int S, void* out, int out_dtype, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_augment_det(items, B, S, S, out, out_dtype, (cudaStream_t)stream);
-}
-
 extern "C" int myolo_augment_det_hw(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, void* stream) {
   int rc = check_device(nullptr);
   if (rc) return rc;
@@ -1573,31 +1545,6 @@ extern "C" int myolo_det_ap(const uint16_t* correct, const float* conf, const ui
   if (rc) return rc;
   return launch_det_ap(correct, conf, cls, rows, n_images, max_det, ncol, reinterpret_cast<const unsigned long long*>(tcount), px, x101,
                        out_ap, out_p, out_r, out_info, workspace, workspace_bytes, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_conv_wgrad(const void* x, const void* dy, int B, int H, int W, int ci, int co, int k, int stride, int dil, float* dW,
-                                int path, void* stream) {
-  MYOLO_REQUIRE(x && dy && dW && B > 0 && (k == 1 || k == 3) && (stride == 1 || stride == 2), "conv_wgrad: bad arguments");
-  int sms = 0;
-  int rc = check_device(&sms);
-  if (rc) return rc;
-  const int pad = dil * (k / 2);
-  const int Ho = (H + 2 * pad - dil * (k - 1) - 1) / stride + 1, Wo = (W + 2 * pad - dil * (k - 1) - 1) / stride + 1;
-  TensorView xv{const_cast<void*>(x), B, H, W, ci, ci, MYOLO_F16};
-  TensorView dv{const_cast<void*>(dy), B, Ho, Wo, co, co, MYOLO_F16};
-  cudaStream_t s = (cudaStream_t)stream;
-  if (path == 0) return launch_conv_wgrad(xv, dv, k, stride, dil, dW, co, ci, nullptr, s);
-  MYOLO_REQUIRE(conv_wgrad_tc_eligible(xv, dv, k, stride, dil, co, ci), "conv_wgrad: geometry not supported by the wgmma kernel");
-  float* packed = nullptr;
-  const size_t nb = conv_wgrad_packed_bytes(dW, co, ci, k);
-  if (nb) {
-    MYOLO_CHECK_CUDA(cudaMalloc(&packed, nb));
-    MYOLO_CHECK_CUDA(cudaMemsetAsync(packed, 0, nb, s));
-  }
-  rc = launch_conv_wgrad_tc(xv, dv, k, stride, dil, dW, packed, co, ci, sms, s);
-  cudaStreamSynchronize(s);
-  if (packed) cudaFree(packed);
-  return rc;
 }
 
 extern "C" int myolo_conv_backward(const void* x, int x_dtype, int B, int H, int W, int x_ctot, int x_coff, const void* dy, int dy_dtype,
@@ -1901,26 +1848,4 @@ extern "C" int myolo_conv_forward(const void* x, int x_dtype, int B, int H, int 
     rc = MYOLO_E_CUDA;
   }
   return rc;
-}
-
-extern "C" int myolo_conv_bn_silu_info(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,
-                                       const float* gamma, const float* beta, const float* mean, const float* var, float eps,
-                                       const float* bias, int act, const void* residual, void* y, int y_ctot, int path, int32_t* info,
-                                       void* stream) {
-  return myolo_conv_forward(x, MYOLO_F16, B, H, W, ci, 0, y, MYOLO_F16, y_ctot, 0, residual, co, 0, w, co, ci, k, stride, dil, gamma, beta,
-                            mean, var, eps, bias, act, path, info, stream);
-}
-
-extern "C" int myolo_conv_bn_silu_slice(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,
-                                        const float* gamma, const float* beta, const float* mean, const float* var, float eps,
-                                        const float* bias, int act, const void* residual, void* y, int y_ctot, int path, void* stream) {
-  return myolo_conv_bn_silu_info(x, B, H, W, ci, w, co, k, stride, dil, gamma, beta, mean, var, eps, bias, act, residual, y, y_ctot, path,
-                                 nullptr, stream);
-}
-
-extern "C" int myolo_conv_bn_silu(const void* x, int B, int H, int W, int ci, const float* w, int co, int k, int stride, int dil,
-                                  const float* gamma, const float* beta, const float* mean, const float* var, float eps,
-                                  const float* bias, int act, const void* residual, void* y, int path, void* stream) {
-  return myolo_conv_bn_silu_slice(x, B, H, W, ci, w, co, k, stride, dil, gamma, beta, mean, var, eps, bias, act, residual, y, co, path,
-                                  stream);
 }

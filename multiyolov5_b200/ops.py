@@ -6,49 +6,6 @@ import torch
 from . import _lib
 
 
-def conv_bn_silu(x_nhwc: torch.Tensor, w: torch.Tensor, bn=None, bias=None, stride=1, dil=1, act=_lib.ACT_SILU, residual=None, path=0,
-                 eps=1e-3, out=None, info=None):
-    """x_nhwc: (B,H,W,Ci) fp16 CUDA; w: (Co,Ci,k,k) fp32 CUDA; bn: (gamma,beta,mean,var) fp32 or None.
-    path: 0 auto, 1 wgmma (tensor cores), 2 CUDA-core, 3 wgmma with streamed weights (the reference layout for path 1's weight
-    residency: same MMAs, same K order, bit-identical results).  out: optional (B,Ho,Wo,Co) fp16 channel slice of an NHWC buffer
-    (out = buf[..., c0:c0 + Co]) to write into; it may be the residual itself.  info: optional list that receives the launch's
-    routing, the 12 slots of myolo_plan_conv_info (slot 3 BN, slot 11 CTAs per SM).  Returns (B,Ho,Wo,Co) fp16."""
-    assert x_nhwc.is_cuda and x_nhwc.dtype == torch.float16 and x_nhwc.is_contiguous()
-    B, H, W, Ci = x_nhwc.shape
-    Co, _, k, _ = w.shape
-    pad = dil * (k // 2)
-    Ho = (H + 2 * pad - dil * (k - 1) - 1) // stride + 1
-    Wo = (W + 2 * pad - dil * (k - 1) - 1) // stride + 1
-    if out is None:
-        y = torch.empty((B, Ho, Wo, Co), dtype=torch.float16, device=x_nhwc.device)
-    else:
-        y = out
-        ctot = y.stride(2)
-        assert y.shape == (B, Ho, Wo, Co) and y.dtype == torch.float16 and y.stride() == (Ho * Wo * ctot, Wo * ctot, ctot, 1)
-    w = w.float().contiguous()
-    g = b = m = v = None
-    if bn is not None:
-        g, b, m, v = [t.float().contiguous() for t in bn]
-    bias = bias.float().contiguous() if bias is not None else None
-    if residual is not None:
-        assert residual.shape == y.shape and residual.dtype == torch.float16 and residual.is_contiguous()
-    slots = _conv_forward(x_nhwc, Ci, 0, y, y.stride(2), 0, residual, Co, 0, w, g, b, m, v, eps, bias, stride, dil, act, path)
-    if info is not None:
-        info[:] = slots
-    return y
-
-
-def _conv_forward(x, x_ctot, x_off, y, y_ctot, y_off, res, res_ctot, res_off, w, g, b, m, v, eps, bias, stride, dil, act, path):
-    Co, Ci, k, _ = w.shape
-    B, H, W = x.shape[:3]
-    slots = (ctypes.c_int32 * 12)()
-    _lib.check(_lib.lib().myolo_conv_forward(_lib.ptr(x), _lib.torch_dtype_code(x.dtype), B, H, W, x_ctot, x_off, _lib.ptr(y),
-                                             _lib.torch_dtype_code(y.dtype), y_ctot, y_off, _lib.ptr(res), res_ctot, res_off, _lib.ptr(w), Co,
-                                             Ci, k, stride, dil, _lib.ptr(g), _lib.ptr(b), _lib.ptr(m), _lib.ptr(v), float(eps), _lib.ptr(bias),
-                                             int(act), int(path), slots, _lib.stream_ptr()))
-    return list(slots)
-
-
 def conv_forward(x, w, y, bn=None, bias=None, residual=None, x_off=0, y_off=0, res_off=0, stride=1, dil=1, act=_lib.ACT_SILU, path=0,
                  eps=1e-3):
     """The plan's forward of one conv (csrc/plan.cu conv_forward_views) on channel slices of NHWC CUDA buffers.
@@ -60,13 +17,20 @@ def conv_forward(x, w, y, bn=None, bias=None, residual=None, x_off=0, y_off=0, r
     for t in (x, y, residual):
         assert t is None or (t.is_cuda and t.is_contiguous() and t.dim() == 4 and t.dtype in (torch.float16, torch.float32))
     assert residual is None or (residual.dtype == torch.float16 and residual.shape[:3] == y.shape[:3])
+    co, ci, k, _ = w.shape
+    B, H, W = x.shape[:3]
     w = w.float().contiguous()
     g = b = m = v = None
     if bn is not None:
         g, b, m, v = [t.float().contiguous() for t in bn]
     bias = bias.float().contiguous() if bias is not None else None
-    return _conv_forward(x, x.shape[3], x_off, y, y.shape[3], y_off, residual, residual.shape[3] if residual is not None else 0, res_off, w,
-                         g, b, m, v, eps, bias, stride, dil, act, path)
+    slots = (ctypes.c_int32 * 12)()
+    _lib.check(_lib.lib().myolo_conv_forward(_lib.ptr(x), _lib.torch_dtype_code(x.dtype), B, H, W, x.shape[3], x_off, _lib.ptr(y),
+                                             _lib.torch_dtype_code(y.dtype), y.shape[3], y_off, _lib.ptr(residual),
+                                             residual.shape[3] if residual is not None else 0, res_off, _lib.ptr(w), co, ci, k, stride, dil,
+                                             _lib.ptr(g), _lib.ptr(b), _lib.ptr(m), _lib.ptr(v), float(eps), _lib.ptr(bias), int(act), int(path),
+                                             slots, _lib.stream_ptr()))
+    return list(slots)
 
 
 def conv_backward(x, w, dy, dW, gin=None, dbias=None, x_off=0, dy_off=0, gin_off=0, stride=1, dil=1, route=0):

@@ -259,7 +259,33 @@ CASES = {
     "bias_head45": (dict(B=2, H=32, W=64, ci=128, co=45, dy_dt=F32, bias=True), {0: 2, 1: 3, 2: 1, 3: 16}),
     "bias_head57": (dict(B=2, H=16, W=64, ci=256, co=57, dy_dt=F32, bias=True), {0: 2, 1: 3, 2: 1}),
     "bias_f16_slice": (dict(B=2, H=32, W=64, ci=64, co=64, bias=True, dy_off=24, dy_ctot=128), {2: 2}),
+    # wgmma weight gradient of layer 0 at the --multi-scale widths 64 n + 32 (Wo = 272): steps of 16 output pixels, and with 16 input
+    # channels such a step is 512 bytes of X per tap, less than its 1024-byte aligned slot
+    "wg_ms_wo272_s1": (dict(B=2, H=16, W=272, ci=16, co=32, k=3, dgrad=False), {0: 0, 1: 4, 8: 16}),
+    "wg_ms_wo272_s2": (dict(B=2, H=32, W=544, ci=16, co=32, k=3, s=2, dgrad=False), {0: 0, 1: 4, 8: 16}),
 }
+
+# (B, H, W, ci, co, k, stride, dil): weight gradients on both tensor-core kernels, each shape at 2048 or more output pixels
+WGRAD_SHAPES = [
+    (2, 32, 64, 64, 64, 1, 1, 1), (2, 32, 64, 128, 256, 1, 1, 1), (1, 64, 128, 64, 128, 3, 1, 1), (2, 32, 32, 128, 64, 3, 1, 1),
+    (2, 64, 64, 64, 128, 3, 2, 1), (1, 32, 64, 64, 64, 3, 1, 2), (1, 32, 64, 192, 48, 1, 1, 1), (2, 16, 128, 256, 256, 3, 1, 1),
+    (1, 48, 80, 64, 96, 3, 1, 3), (2, 64, 128, 32, 64, 3, 2, 1), (1, 64, 128, 32, 32, 3, 1, 1), (1, 64, 64, 16, 32, 3, 1, 1),
+    (2, 32, 64, 32, 32, 1, 1, 1),
+]
+
+
+def wgrad_cases():
+    """WGRAD_SHAPES on the mma.sync kernel (route 2: MYOLO_CONV_BWD_NO_WGRAD_TC) and on the wgmma kernel, which accumulates straight into
+    dW for a 1x1 conv whose channels need no padding and through its packed buffer otherwise (conv_wgrad_packed_bytes)"""
+    out = {}
+    for i, (B, H, W, ci, co, k, s, d) in enumerate(WGRAD_SHAPES):
+        geo = dict(B=B, H=H, W=W, ci=ci, co=co, k=k, s=s, d=d, dgrad=False)
+        out[f"wgrad_mma_w{i}"] = (dict(geo, route=2), {0: 0, 1: 2})
+        out[f"wgrad_wgmma_w{i}"] = (geo, {0: 0, 1: 3 if k == 1 and ci % 16 == 0 else 4})
+    return out
+
+
+CASES.update(wgrad_cases())
 
 
 def case_args(name):

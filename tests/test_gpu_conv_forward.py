@@ -8,9 +8,12 @@ conv_forward_views, the function the plan's prepare_conv calls), against F.conv2
 Every view is a channel slice of a wider buffer, and every word outside the slices (other channels, the padding channels of an fp32 head
 buffer, pixel rows past the map) holds an fp16 / fp32 NaN that must survive; the input and a separate residual buffer must come back
 unchanged.  Each case asserts the route it was built for, so a silent fall-back fails; across the cases every instantiation of
-conv_tc_kernel<KC, BN, RES, CTAS_PER_SM> that conv_tc_launch can dispatch runs.  The census runs the entry at the exact geometry and slice
-layout of every conv op of two inference plans at two shapes and two train plans, and asserts that it routes and tiles each one as the
-plan does."""
+conv_tc_kernel<KC, BN, RES, CTAS_PER_SM> that conv_tc_launch can dispatch runs.  A case may launch a twin on the same inputs that must
+give the same output bit for bit: the streamed-weight layout with one A box per tap (path 3: the same MMAs in the same K order, so any
+difference is a layout or synchronisation bug of the resident weights, the strip or the second CTA), or the residual aliasing the
+output instead of a separate buffer.  The census runs the entry at the exact geometry and slice layout of every conv op of two inference
+plans at two shapes and two train plans, and asserts that it routes and tiles each one as the plan does; one more test pins which convs
+of the s/PSP forward keep their weights resident and take the strip."""
 from collections import defaultdict
 
 import pytest
@@ -22,7 +25,7 @@ pytestmark = pytest.mark.gpu
 U16 = 2.0 ** -11            # fp16 unit roundoff: one rounding of a stored value
 NAN16 = 0x7E01              # fp16 NaN bit pattern of the words no kernel may write
 NAN32 = 0x7FC01234          # fp32 NaN bit pattern
-PAD_PIX = 256               # pixels past the map in every buffer
+PAD_PIX = 256               # pixels past the map in every buffer, beyond 16 map rows (the tallest tile is 8 x 16)
 F16, F32 = torch.float16, torch.float32
 NONE, SILU, SIGMOID = 0, 1, 2
 
@@ -47,11 +50,12 @@ def out_hw(H, W, k, s, d):
 
 # ---- buffers -----------------------------------------------------------------------------------------------------------------------
 def sentinel_buffer(B, H, W, ctot, dtype):
-    """an NHWC buffer of B*H*W pixels + PAD_PIX more, every word a NaN; returns (whole flat buffer, (B,H,W,ctot) view of the map)"""
+    """an NHWC buffer of B*H*W pixels + 16*W + PAD_PIX more, every word a NaN; returns (whole flat buffer, (B,H,W,ctot) view of the map)"""
+    n = B * H * W + 16 * W + PAD_PIX
     if dtype == F16:
-        flat = torch.full((B * H * W + PAD_PIX, ctot), NAN16, dtype=torch.int16, device="cuda").view(F16)
+        flat = torch.full((n, ctot), NAN16, dtype=torch.int16, device="cuda").view(F16)
     else:
-        flat = torch.full((B * H * W + PAD_PIX, ctot), NAN32, dtype=torch.int32, device="cuda").view(F32)
+        flat = torch.full((n, ctot), NAN32, dtype=torch.int32, device="cuda").view(F32)
     return flat, flat[:B * H * W].view(B, H, W, ctot)
 
 
@@ -93,9 +97,11 @@ def conv64(x64, wp, bp, k, s, d, act):
 
 # ---- one run of the entry and its fp64 reference ---------------------------------------------------------------------------------
 def run(B, H, W, ci, co, k=1, s=1, d=1, x_dt=F16, y_dt=F16, act=SILU, res=None, bn=True, bias=True, x_off=0, y_off=0, r_off=0,
-        x_ctot=None, y_ctot=None, r_ctot=None, path=0, seed=0, images=None, res_cancel=False, mutant=None):
-    """runs ops.conv_forward once on random data; returns (info, {dtype: error, "change": mutant's relative change}, sentinels intact).
-    res: None, "sep" (own buffer) or "alias" (the output slice itself); images: the images compared (default all)"""
+        x_ctot=None, y_ctot=None, r_ctot=None, path=0, seed=0, images=None, res_cancel=False, mutant=None, twin=None):
+    """runs ops.conv_forward once on random data; returns (info, {dtype: error, "change": mutant's relative change}, sentinels intact,
+    twin).  res: None, "sep" (own buffer) or "alias" (the output slice itself); images: the images compared (default all).  twin: None,
+    "path3" (the same inputs again on path 3) or "alias" (again on the same path, with res "sep", the residual in the output slice); twin
+    is then (the twin's info, both output buffers bit-identical), else None"""
     from multiyolov5_b200 import ops
     g = torch.Generator(device="cuda").manual_seed(seed)
     Ho, Wo = out_hw(H, W, k, s, d)
@@ -137,9 +143,19 @@ def run(B, H, W, ci, co, k=1, s=1, d=1, x_dt=F16, y_dt=F16, act=SILU, res=None, 
 
     info = ops.conv_forward(xv, w, yv, bn=bnp, bias=bvec, residual=rbuf, x_off=x_off, y_off=y_off, res_off=r_off, stride=s, dil=d, act=act,
                             path=path, eps=eps)
+    if twin is not None:
+        assert twin == "path3" or res == "sep", (twin, res)
+        yflat2, yv2 = sentinel_buffer(B, Ho, Wo, y_ctot, y_dt)
+        rbuf2, r_off2 = rbuf, r_off
+        if res == "alias" or twin == "alias":
+            yv2[..., y_off:y_off + co] = rv_vals.half()
+            rbuf2, r_off2 = yv2, y_off
+        twin_info = ops.conv_forward(xv, w, yv2, bn=bnp, bias=bvec, residual=rbuf2, x_off=x_off, y_off=y_off, res_off=r_off2, stride=s,
+                                     dil=d, act=act, path=3 if twin == "path3" else path, eps=eps)
     torch.cuda.synchronize()
 
     ok = same_bits(xflat, x0) and (r0 is None or same_bits(rflat, r0)) and untouched(yflat, B * Ho * Wo, y_off, co)
+    twin = None if twin is None else (twin_info, same_bits(yflat, yflat2))
     with torch.no_grad():
         ref = conv64(x64, wp, bp, k, s, d, act)
         if res is not None:
@@ -155,7 +171,7 @@ def run(B, H, W, ci, co, k=1, s=1, d=1, x_dt=F16, y_dt=F16, act=SILU, res=None, 
             err["fp16"] = float(((ours - ref).abs() - U16 * ref.abs()).clamp_min(0).max()) / scale
         else:
             err["fp32"] = float((ours - ref).abs().max()) / scale
-    return info, err, ok
+    return info, err, ok, twin
 
 
 def wrong_reference(mutant, x64, w, bnp, bvec, eps, wp, bp, k, s, d, act, r64):
@@ -309,6 +325,130 @@ CASES = {
     "simt_tiny_map": (dict(B=4, H=4, W=8, ci=64, co=64, k=3, res="sep"), dict(tc=0)),
 }
 
+# (B, H, W, ci, co, k, stride, dil, residual): layer classes of the s and m models, and layers at bench scale
+LAYERS = [
+    (2, 32, 64, 64, 64, 1, 1, 1, False),      # plain 1x1, SW128
+    (1, 64, 128, 128, 128, 1, 1, 1, False),
+    (2, 16, 32, 512, 256, 1, 1, 1, False),    # 2 N tiles, 8 K stages
+    (1, 16, 32, 1024, 512, 1, 1, 1, False),   # SPP.cv2 class
+    (2, 64, 64, 16, 32, 3, 1, 1, False),      # Focus conv class: kc=16 (SW32), 9 taps
+    (2, 32, 64, 32, 32, 3, 1, 1, True),       # Bottleneck.cv2 + residual, kc=32 (SW64)
+    (1, 32, 64, 64, 64, 3, 1, 1, True),
+    (1, 16, 32, 128, 128, 3, 1, 1, False),
+    (2, 64, 128, 32, 64, 3, 2, 1, False),     # stride-2 parity maps
+    (1, 32, 64, 64, 128, 3, 2, 1, False),
+    (1, 32, 64, 64, 64, 3, 1, 2, False),      # dilated (RFB2 branch1/2)
+    (1, 32, 64, 64, 64, 3, 1, 3, False),
+    (1, 16, 32, 256, 128, 3, 1, 6, False),    # ASPP-like dilation
+    (1, 24, 40, 64, 64, 3, 1, 1, False),      # W, H not multiples of the tile -> OOB zero fill / clipped stores
+    (1, 16, 12, 64, 48, 1, 1, 1, False),      # box wider than the map, Co=48 (m model)
+    (1, 32, 32, 48, 96, 3, 1, 1, False),      # kc=16 with Ci=48, Co=96
+    (1, 16, 32, 192, 192, 1, 1, 1, False),    # Co=192 -> BN=96 x 2
+    (3, 8, 16, 64, 64, 1, 1, 1, False),       # exactly one tile per image
+    (2, 16, 128, 64, 64, 3, 1, 1, False),     # full-row tiles (tw=128)
+    (1, 12, 128, 64, 64, 3, 1, 2, True),      # full-row tiles + dilation 2 + residual
+    (1, 8, 128, 64, 64, 3, 1, 3, False),      # full-row tiles + dilation 3
+    (1, 8, 256, 256, 128, 3, 1, 1, False),    # 4 channel blocks, W=256 (2 tiles per row)
+    (2, 16, 256, 32, 32, 3, 1, 1, True),      # 64-byte rows (kc=32) + residual (L2 bottleneck class)
+    (2, 16, 512, 16, 32, 3, 1, 1, False),     # 32-byte rows (kc=16): Focus conv class
+    (1, 8, 128, 48, 96, 3, 1, 2, False),      # kc=16 x 3 channel blocks, dilation 2
+    (16, 64, 256, 32, 32, 3, 1, 1, True),     # many full-row tiles + residual
+    (16, 128, 256, 16, 32, 3, 1, 1, False),   # many full-row tiles, 32-byte rows (Focus conv at scale)
+    (8, 37, 512, 32, 32, 3, 1, 1, False),     # ragged image height (Ho = 37)
+    (16, 64, 256, 32, 32, 1, 1, 1, False),    # many tiles, BN=32
+    (8, 64, 128, 64, 64, 1, 1, 1, True),      # many tiles + residual
+    # layers at bench scale (more tiles than SMs: the persistent CTAs take several tiles each)
+    (16, 32, 64, 128, 128, 3, 1, 1, True),    # P4 bottleneck 3x3, residual
+    (16, 64, 128, 64, 64, 3, 1, 2, False),    # dilation 2, 1024 tiles
+    (16, 64, 128, 128, 256, 3, 2, 1, False),  # stride 2, two N tiles
+    (16, 32, 64, 128, 80, 3, 1, 1, False),    # N tile of 80 channels
+    (6, 64, 128, 256, 128, 3, 1, 1, False),   # FFM class: 4 channel blocks, 384 tiles
+]
+STREAMED = [s for s in LAYERS if s[0] >= 6 and s[5] == 3][-5:] + [(16, 32, 64, 256, 128, 1, 1, 1, False), (2, 32, 64, 64, 64, 1, 1, 1, False)]
+
+# (B, H, W, ci, co, k, stride, dil, residual): resident weights and strip loads on path 1, each against its streamed twin
+REUSE = [
+    (2, 64, 64, 16, 32, 3, 1, 1, False),      # kc = 16 (32-byte rows)
+    (1, 32, 32, 48, 96, 3, 1, 1, False),      # kc = 16, three channel blocks
+    (2, 32, 256, 32, 32, 3, 1, 1, True),      # kc = 32, tw = 128, residual
+    (1, 32, 64, 64, 64, 3, 1, 2, False),      # kc = 64, tw = 64 (th = 2), dilation 2
+    (1, 32, 64, 64, 64, 3, 1, 3, True),       # dilation 3 + residual
+    (1, 12, 128, 64, 64, 3, 1, 2, True),      # tw = 128, dilation 2 + residual
+    (1, 24, 40, 64, 64, 3, 1, 1, False),      # ragged right edge and height
+    (8, 37, 512, 32, 32, 3, 1, 1, False),     # ragged height, many tiles
+    (3, 8, 16, 64, 64, 1, 1, 1, False),       # fewer tiles than SMs
+    (2, 16, 32, 512, 256, 1, 1, 1, False),    # Co = 256: two N tiles
+    (4, 32, 64, 128, 256, 1, 1, 1, True),     # two N tiles + residual
+    (2, 16, 32, 192, 192, 1, 1, 1, False),    # BN = 96 x 2
+    (2, 32, 64, 480, 128, 1, 1, 1, False),    # pack 120 KB: just under the residency limit
+    (2, 32, 64, 496, 128, 1, 1, 1, False),    # pack 124 KB: just over (streamed on both paths)
+    (16, 64, 128, 32, 64, 3, 2, 1, False),    # stride 2, resident
+    (16, 64, 128, 64, 128, 3, 2, 1, False),   # stride 2, 144 KB pack (streamed)
+    # bench-scale layers of the s/PSP forward (batch 16 at 512x1024)
+    (16, 256, 256, 32, 64, 3, 1, 1, False),   # layer 0 on pixel pairs
+    (16, 128, 256, 32, 32, 3, 1, 1, True),    # C3 bottleneck 3x3 32->32 + residual
+    (16, 128, 256, 32, 32, 1, 1, 1, False),
+    (16, 64, 128, 64, 64, 3, 1, 1, True),     # C3 bottleneck 3x3 64->64 + residual
+    (16, 64, 128, 64, 64, 3, 1, 2, False),    # SegMaskPSP dilated 3x3
+    (16, 32, 64, 128, 128, 3, 1, 1, True),
+    (16, 16, 32, 256, 512, 1, 1, 1, False),   # four N tiles, resident
+    (6, 64, 128, 256, 128, 3, 1, 1, False),   # FFM 3x3 256->128 (576 KB pack: streamed)
+]
+
+# (B, H, W, ci, co, k, stride, residual, BN at two CTAs): two CTAs per SM beyond the narrow 1x1 layers, including Co = 128 / 256 layers
+# that take BN = 64 N tiles to admit the second CTA; every map is ragged in x (a tile width that does not divide the map's)
+TWO_CTA = [
+    (4, 37, 250, 32, 64, 3, 1, False, 64),    # 3x3 strip (layer 0 class)
+    (4, 21, 250, 32, 32, 3, 1, True, 32),     # 3x3 strip + residual (C3 bottleneck class)
+    (8, 64, 252, 32, 64, 3, 2, False, 64),    # 3x3 stride 2, per-tap boxes
+    (8, 40, 250, 64, 64, 1, 1, True, 64),     # 1x1 + residual
+    (8, 32, 120, 256, 128, 1, 1, False, 64),  # Co = 128: BN 128 -> 64
+    (8, 16, 100, 256, 256, 1, 1, False, 64),  # Co = 256: BN 128 -> 64, tw = 8 over width 100
+]
+
+# (B, H, W, ci, co, k, residual): the fp16 epilogue transposes each quad's accumulator words so that a lane stores the 8 channels of one
+# group as one 16-byte vector (a transposition error shows as gross mismatches); slices at channel 8, the smallest offset it allows
+EPILOGUE = [
+    (2, 37, 45, 32, 64, 3, False),     # ragged right edge and bottom (tiles reach past the map)
+    (1, 20, 70, 16, 48, 1, False),     # BN = 48: a last block of two 8-channel groups
+    (3, 11, 136, 64, 32, 1, False),    # tw = 128 over a ragged width
+    (16, 64, 128, 64, 64, 1, False),   # 1x1 at BN = 64 over many tiles (two CTAs per SM)
+    (2, 16, 32, 128, 256, 1, False),   # two N tiles
+    (2, 33, 40, 64, 64, 3, True),      # residual, ragged map
+    (4, 32, 64, 128, 256, 1, True),    # residual, two N tiles
+]
+
+
+def shape_list_cases():
+    """LAYERS on the CUDA-core kernel (path 2) and the wgmma kernel (path 1), STREAMED on path 3; REUSE on path 1 with a path-3 twin;
+    TWO_CTA on path 1 into a slice at channel 8 with a path-3 twin, and with a residual also against its aliasing twin; EPILOGUE on path 1
+    without BatchNorm into a slice at channel 8, and with a residual also against its aliasing twin"""
+    out = {}
+    for path, kind, shapes in ((2, "simt", LAYERS), (1, "tc", LAYERS), (3, "streamed", STREAMED)):
+        for i, (B, H, W, ci, co, k, s, d, res) in enumerate(shapes):
+            out[f"layer_{kind}_{i}"] = (dict(B=B, H=H, W=W, ci=ci, co=co, k=k, s=s, d=d, res="sep" if res else None, path=path),
+                                        dict(tc=int(path != 2)))
+    for B, H, W, ci, co, k, s, d, res in REUSE:
+        out[f"reuse_{ci}-{co}-k{k}s{s}d{d}-{B}x{H}x{W}{'-res' if res else ''}"] = (
+            dict(B=B, H=H, W=W, ci=ci, co=co, k=k, s=s, d=d, res="sep" if res else None, path=1, twin="path3"), dict(tc=1))
+    for B, H, W, ci, co, k, s, res, bn in TWO_CTA:
+        geo = dict(B=B, H=H, W=W, ci=ci, co=co, k=k, s=s, res="sep" if res else None, bn=False, y_off=8, path=1)
+        want = dict(tc=1, resident=1, ctas=2, BN=bn, strip=int(k == 3 and s == 1))
+        name = f"two_cta_{ci}-{co}-k{k}s{s}-{B}x{H}x{W}{'-res' if res else ''}"
+        out[name] = (dict(geo, twin="path3"), want)
+        if res:
+            out[name + "_alias"] = (dict(geo, twin="alias"), want)
+    for B, H, W, ci, co, k, res in EPILOGUE:
+        geo = dict(B=B, H=H, W=W, ci=ci, co=co, k=k, res="sep" if res else None, bn=False, y_off=8, path=1)
+        name = f"epilogue_{ci}-{co}-k{k}-{B}x{H}x{W}{'-res' if res else ''}"
+        out[name] = (geo, dict(tc=1))
+        if res:
+            out[name + "_alias"] = (dict(geo, twin="alias"), dict(tc=1))
+    return out
+
+
+CASES.update(shape_list_cases())
+
 
 def case_args(name):
     geo, _ = CASES[name]
@@ -325,15 +465,15 @@ def result(name):
     """the case's run, once per session (the coverage test reuses the cases' launches)"""
     if name not in _RESULTS:
         a = case_args(name)
-        info, err, ok = run(**a)
-        _RESULTS[name] = (a, info, err, ok)
+        _RESULTS[name] = (a, *run(**a))
     return _RESULTS[name]
 
 
 @pytest.mark.parametrize("name", list(CASES))
 def test_conv_forward_matches_fp64(name):
-    """one conv on the route the case was built for, through channel slices, against fp64"""
-    a, info, err, ok = result(name)
+    """one conv on the route the case was built for, through channel slices, against fp64 (a NaN or an infinity fails it); a twin
+    matches it bit for bit: a path-3 twin on streamed weights at one CTA per SM, an aliasing twin on the same route"""
+    a, info, err, ok, twin = result(name)
     print(f"\n[{name}] {describe(info)}\n[{name}] " + "  ".join(f"{k} {v:.2e}" for k, v in err.items()))
     want = CASES[name][1]
     got = {k: info[SLOT[k]] for k in want}
@@ -341,6 +481,15 @@ def test_conv_forward_matches_fp64(name):
     fails = check(name, info, err, ok)
     print_worst()
     assert not fails, "\n".join(fails)
+    if twin is not None:
+        twin_info, same = twin
+        print(f"[{name}] {a['twin']} twin: {describe(twin_info)}")
+        if a["twin"] == "path3":
+            got = {k: twin_info[SLOT[k]] for k in ("tc", "resident", "strip", "ctas")}
+            assert got == dict(tc=1, resident=0, strip=0, ctas=1), f"path-3 twin: {describe(twin_info)}"
+        else:
+            assert twin_info == info, f"aliasing twin routed {describe(twin_info)}"
+        assert same, f"the {a['twin']} twin's output buffer differs from the launch's"
 
 
 def test_conv_forward_reaches_every_instantiation():
@@ -350,7 +499,7 @@ def test_conv_forward_reaches_every_instantiation():
     assert len(want) == 72
     reached = defaultdict(list)
     for name in CASES:
-        a, info, _, _ = result(name)
+        a, info = result(name)[:2]
         if info[0]:
             reached[(info[10], info[3], int(a.get("res") is not None), info[11])].append(name)
     missing = sorted(want - set(reached))
@@ -417,7 +566,7 @@ def test_conv_forward_census_of_the_plans(monkeypatch):
     for tag, yml, B, H, W, train in CENSUS:
         count = defaultdict(int)
         for i, plan_info, a in census_ops(yml, B, H, W, train):
-            info, err, ok = run(**a)
+            info, err, ok, _ = run(**a)
             name = f"{tag} {'train ' if train else ''}{B}x{H}x{W} op {i}"
             if info != plan_info:
                 fails.append(f"{name}: entry routed {info}, the plan {plan_info}")
@@ -439,6 +588,48 @@ def test_conv_forward_census_of_the_plans(monkeypatch):
     assert total["wgmma 2 cta/SM"] >= 1 and total["wgmma strip"] >= 1 and total["wgmma fp32 out"] >= 1 and total["input slice"] >= 1, total
 
 
+SMEM_BUDGET = 227 * 1024
+RESIDENT_LIMIT = SMEM_BUDGET - (1024 + 8192 + 1024) - 6 * 128 * 64 * 2   # misc + six A stages (conv_tc.cu)
+
+
+def test_spsp_plan_reuse_paths():
+    import ctypes as C
+    from multiyolov5_b200 import _lib, synth
+    from multiyolov5_b200.models.yolo import Model
+    yml = "yolov5s_city_seg.yaml"
+    sd = synth.synth_state_dict(synth.load_manifest("s_psp"), synth.load_cfg(yml), seed=1)
+    model = Model(yml)
+    model.load_state_dict(sd)
+    model.cuda().eval().half()
+    model(torch.zeros(16, 3, 512, 1024, dtype=torch.float16, device="cuda"))
+    torch.cuda.synchronize()
+    plan = model.engine().last_plan
+    info = (C.c_int32 * 12)()
+    n_tc = n_res = n_strip = 0
+    for i, o in enumerate(plan.pb.ops):
+        if o.kind != _lib.OP_CONV:
+            continue
+        _lib.check(_lib.lib().myolo_plan_conv_info(plan.handle, i, info))
+        if not info[0]:
+            continue
+        n_tc += 1
+        s = plan.pb.slots[o.slot].conv
+        k, bn, kc, ntn, grid = s.kernel_size[0], info[3], info[10], info[9], info[1]
+        ci_pad = (s.in_channels + kc - 1) // kc * kc
+        pack = (k * k * ci_pad * bn * 2 + 1023) // 1024 * 1024
+        expect = pack <= RESIDENT_LIMIT
+        assert info[6] == int(expect), f"op {i} {o.tag} {s.in_channels}->{s.out_channels} k{k}: pack {pack} B, resident {info[6]}"
+        if info[6]:
+            assert grid % ntn == 0, f"op {i}: grid {grid} is not a multiple of {ntn} N tiles"
+        strip = bool(info[6]) and k == 3 and s.stride[0] == 1 and o.out.w >= 64 and ci_pad // kc <= 4
+        assert info[5] == int(strip), f"op {i} {o.tag} {s.in_channels}->{s.out_channels} k{k} @{o.out.h}x{o.out.w}: strip {info[5]}"
+        n_res += info[6]
+        n_strip += info[5]
+    # streamed: the 22 packs over 120 KB (3x3 with 64+ input channels and 1x1 with 512+ input channels, at BN = 128).
+    # strip: layer 0, the C3 bottleneck 3x3 layers at 128x256 and 64x128, and the three SegMaskPSP 3x3 64->64 layers
+    assert (n_tc, n_res, n_strip) == (65, 43, 9)
+
+
 # ---- sensitivity ---------------------------------------------------------------------------------------------------------------
 MUTANT_CASES = {  # wrong reference: the case it runs on
     "bf16": dict(B=2, H=24, W=40, ci=64, co=64, k=3, bn=True, act=SILU),
@@ -454,7 +645,7 @@ def test_conv_forward_limits_catch_wrong_references():
     misses its limit by at least 10x"""
     print()
     for mutant, a in MUTANT_CASES.items():
-        info, err, _ = run(**a, mutant=mutant)
+        info, err, _, _ = run(**a, mutant=mutant)
         m = "fp16" if a.get("y_dt", F16) == F16 else "fp32"
         over = err[m] / LIMIT[m]
         print(f"mutant {mutant:<24} ({describe(info)}): changes the output by {100 * err['change']:.3f} %, {m} error at {over:.0f}x its limit")

@@ -305,6 +305,12 @@ def test_evolve_three_generations_end_to_end(tmp_path, monkeypatch):
     x = np.loadtxt(tmp_path / "evolve.txt", ndmin=2)
     assert 1 <= len(rows) <= 3 and x.shape[1] == 7 + len(rev.HYP_SCRATCH)
     assert rows == [" ".join("%10.3g" % v for v in row) for row in x]            # np.savetxt(fmt='%10.3g'): 35 fields, one space apart
+    # print_mutation sorts the rows it reads back (the earlier generations' at '%10.3g', the last one's results at '%10.4g') by fitness
+    # and only then saves every row at '%10.3g', which can swap the order of near-tied fitness values: restore the last generation's
+    # results to what the sort saw, and the rows are in descending fitness exactly
+    seen = [float("%10.4g" % v) for v in results[-1]]
+    (last,) = [i for i, row in enumerate(x) if row[:7].tolist() == [float("%10.3g" % v) for v in seen]]
+    x[last, :7] = seen
     f = (x[:, :4] * [0.0, 0.0, 0.1, 0.9]).sum(1)
-    assert (np.diff(f) <= 0).all()
+    assert (np.diff(f) <= 0).all(), f
     assert (tmp_path / "run" / "hyp_evolved.yaml").read_text().startswith("# Hyperparameter Evolution Results\n# Generations: ")

@@ -90,33 +90,6 @@ def test_same_size_draw_returns_without_a_launch():
     assert out.shape == (4, 3, 1536, 1536) and torch.equal(out, _torch_ref(x8, (1536, 1536)))
 
 
-# ---- layer 0's weight gradient at the multi-scale widths 64 n + 32 ------------------------------------------------------------------
-@pytest.mark.parametrize("stride", [1, 2])
-def test_wgmma_weight_gradient_with_16_pixel_steps_and_16_channels(stride):
-    """the wgmma weight-gradient kernel steps over 16 output pixels when Wo % 32 == 16 (layer 0 at 544, 608, ... : 272, 304, ...); with
-    16 (padded) input channels such a step is 512 bytes of X per tap, less than its 1024-byte aligned slot.  Against torch's weight
-    gradient in fp64 on the same fp16 inputs, within the packed wgmma weight gradient's limit in test_gpu_conv_backward.py."""
-    from multiyolov5_b200 import _lib
-    from tests.test_gpu_conv_backward import LIMIT_WGRAD
-    B, ci, co, k = 2, 16, 32, 3
-    H, W = (16, 272) if stride == 1 else (32, 544)
-    g = torch.Generator().manual_seed(stride)
-    x = torch.randn((B, ci, H, W), generator=g).half()
-    Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
-    assert Wo % 32 == 16
-    dy = torch.randn((B, co, Ho, Wo), generator=g).half()
-    w = torch.zeros((co, ci, k, k), dtype=torch.float64, requires_grad=True)
-    (F.conv2d(x.double(), w, None, stride, 1) * dy.double()).sum().backward()
-    xd = x.permute(0, 2, 3, 1).contiguous().cuda()
-    dyd = dy.permute(0, 2, 3, 1).contiguous().cuda()
-    dW = torch.ones((co, ci, k, k), dtype=torch.float32, device="cuda")
-    _lib.check(_lib.lib().myolo_conv_wgrad(_lib.ptr(xd), _lib.ptr(dyd), B, H, W, ci, co, k, stride, 1, _lib.ptr(dW), 1, _lib.stream_ptr()))
-    torch.cuda.synchronize()
-    got = (dW - 1.0).cpu().double()
-    err = float((got - w.grad).norm() / w.grad.norm())
-    assert err < LIMIT_WGRAD["wgmma packed"][0], err
-
-
 # ---- train steps through the shared workspace ---------------------------------------------------------------------------------------
 HYP = dict(lr0=0.01, momentum=0.937, weight_decay=5e-4, box=0.05, cls=0.5, cls_pw=1.0, obj=1.0, obj_pw=1.0, anchor_t=4.0, fl_gamma=0.0)
 B = 4

@@ -1,7 +1,7 @@
 """GPU: `--rect` training batches built on the device (DeviceImageCache + DetRectLoader) against the reference's own batches
-(tests/golden/rect_cases.npz) and against the numpy restatement (oracle/restate_rect.py getitem_rect) at full size, bit exact; the
-square entry point against the H x W one; and Trainer steps over several rect shapes on one reserved workspace against the same steps on
-private plans (the bar of test_gpu_multiscale.py)."""
+(tests/golden/rect_cases.npz) and against the numpy restatement (oracle/restate_rect.py getitem_rect) at full size, bit exact; and
+Trainer steps over several rect shapes on one reserved workspace against the same steps on private plans (the bar of
+test_gpu_multiscale.py)."""
 import json
 import os
 import random
@@ -112,27 +112,6 @@ def test_device_batches_match_restatement_full_size(name):
                 ref = torch.from_numpy(wi).cuda()
                 assert torch.equal(imgs[k], ref), (name, h, b, k, int((imgs[k] != ref).sum()))
                 assert np.array_equal(t[t[:, 0] == k][:, 1:], wl), (name, h, b, k)
-
-
-def test_square_entry_point_is_the_hw_one_at_h_equal_w():
-    from multiyolov5_b200 import _lib
-    from multiyolov5_b200.utils.datasets import DetAugmenter, DeviceImageCache
-    rs = np.random.RandomState(2)
-    imgs0, labels0 = _frames(rs, [(300, 500), (400, 260), (640, 640)])
-    aug = DetAugmenter(DeviceImageCache(imgs0, 640, labels0), dict(_scratch(), degrees=10.0, shear=3.0, mixup=0.5, flipud=0.5))
-    random.seed(0)
-    np.random.seed(0)
-    its = [aug.item(i)[0] for i in (0, 1, 2, 0, 1, 2)]
-    items = (_lib.AugItem * len(its))(*its)
-    dev = torch.frombuffer(bytearray(items), dtype=torch.uint8).cuda()
-    L, sp = _lib.lib(), _lib.stream_ptr()
-    for dtype in (torch.uint8, torch.float16, torch.float32):
-        a = torch.empty((len(its), 3, 640, 640), dtype=dtype, device="cuda")
-        b = torch.full_like(a, 7)
-        _lib.check(L.myolo_augment_det(_lib.ptr(dev), len(its), 640, _lib.ptr(a), _lib.torch_dtype_code(dtype), sp))
-        _lib.check(L.myolo_augment_det_hw(_lib.ptr(dev), len(its), 640, 640, _lib.ptr(b), _lib.torch_dtype_code(dtype), sp))
-        assert torch.equal(a, b), dtype
-    torch.cuda.synchronize()
 
 
 # ---- train steps over rect shapes on one reserved workspace ------------------------------------------------------------------------

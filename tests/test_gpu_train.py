@@ -231,42 +231,6 @@ def test_trainer_overfits_a_fixed_batch():
     assert float(tr.scale) >= 1.0
 
 
-WGRAD_SHAPES = [  # B, H, W, ci, co, k, stride, dil
-    (2, 32, 64, 64, 64, 1, 1, 1), (2, 32, 64, 128, 256, 1, 1, 1), (1, 64, 128, 64, 128, 3, 1, 1), (2, 32, 32, 128, 64, 3, 1, 1),
-    (2, 64, 64, 64, 128, 3, 2, 1), (1, 32, 64, 64, 64, 3, 1, 2), (1, 32, 64, 192, 48, 1, 1, 1), (2, 16, 128, 256, 256, 3, 1, 1),
-    (1, 48, 80, 64, 96, 3, 1, 3), (2, 64, 128, 32, 64, 3, 2, 1), (1, 64, 128, 32, 32, 3, 1, 1), (1, 64, 64, 16, 32, 3, 1, 1),
-    (2, 32, 64, 32, 32, 1, 1, 1),
-]
-
-
-@pytest.mark.parametrize("path", [0, 1])
-@pytest.mark.parametrize("shape", WGRAD_SHAPES, ids=[f"w{i}" for i in range(len(WGRAD_SHAPES))])
-def test_conv_wgrad_kernels_match_torch(shape, path):
-    """per-op: dW of one conv from fp16 NHWC x / dy, both kernels (0: mma.sync, 1: wgmma MN-major) against torch's conv weight
-    gradient in fp64 on the same fp16-rounded inputs; relative Frobenius error within the kernel's limit in test_gpu_conv_backward.py
-    (fp32 accumulation order only)."""
-    from tests.test_gpu_conv_backward import LIMIT_WGRAD
-    from multiyolov5_b200 import _lib
-    B, H, W, ci, co, k, stride, dil = shape
-    g = torch.Generator().manual_seed(sum(shape))
-    x = torch.randn((B, ci, H, W), generator=g).half()
-    pad = dil * (k // 2)
-    Ho = (H + 2 * pad - dil * (k - 1) - 1) // stride + 1
-    Wo = (W + 2 * pad - dil * (k - 1) - 1) // stride + 1
-    dy = torch.randn((B, co, Ho, Wo), generator=g).half()
-    w = torch.zeros((co, ci, k, k), dtype=torch.float64, requires_grad=True)
-    y = torch.nn.functional.conv2d(x.double(), w, None, stride, pad, dil)
-    (y * dy.double()).sum().backward()
-    xd = x.permute(0, 2, 3, 1).contiguous().cuda()
-    dyd = dy.permute(0, 2, 3, 1).contiguous().cuda()
-    dW = torch.ones((co, ci, k, k), dtype=torch.float32, device="cuda")       # accumulate-into semantics: starts at 1
-    _lib.check(_lib.lib().myolo_conv_wgrad(_lib.ptr(xd), _lib.ptr(dyd), B, H, W, ci, co, k, stride, dil, _lib.ptr(dW), path, _lib.stream_ptr()))
-    torch.cuda.synchronize()
-    err = rel_f((dW - 1.0).cpu(), w.grad)
-    limit = LIMIT_WGRAD["mma.sync"][0] if path == 0 else max(LIMIT_WGRAD["wgmma direct"][0], LIMIT_WGRAD["wgmma packed"][0])
-    assert err < limit, err
-
-
 def test_graphed_det_loss_equals_eager_path_and_runs_for_unfused_hyps():
     """Where the fused detection loss does not cover the hyp, the Trainer replays ComputeLoss forward+backward as one CUDA graph on static
     buffers, targets zero-padded to a multiple of 64 rows.  On identical head outputs the replayed graph must give the eager loss items and

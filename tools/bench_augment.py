@@ -112,11 +112,11 @@ def augment_record(steps, warmup, B=16, s=1024):
     out = torch.empty((B, 3, s, s), dtype=torch.uint8, device="cuda")
     sp = _lib.stream_ptr()
     for _ in range(warmup):
-        _lib.check(L.myolo_augment_det(_lib.ptr(dev_items), B, s, _lib.ptr(out), _lib.U8, sp))
+        _lib.check(L.myolo_augment_det_hw(_lib.ptr(dev_items), B, s, s, _lib.ptr(out), _lib.U8, sp))
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(steps):
-        _lib.check(L.myolo_augment_det(_lib.ptr(dev_items), B, s, _lib.ptr(out), _lib.U8, sp))
+        _lib.check(L.myolo_augment_det_hw(_lib.ptr(dev_items), B, s, s, _lib.ptr(out), _lib.U8, sp))
     e1.record()
     torch.cuda.synchronize()
     kernel_ms = e0.elapsed_time(e1) / steps
