@@ -40,10 +40,12 @@ static constexpr int kMinTwoCtaStages = 4;       // A stages per CTA at two CTAs
 static constexpr int kTwoCtaMaxBN = 64;          // widest N tile whose consumers fit kConsumerRegs (BN / 2 accumulators + residual vectors)
 static constexpr int kProducerRegs = 24;         // setmaxnreg at two CTAs per SM: 128 x 24 + 256 x 104 <= 384 x 80, the pool of one CTA
 static constexpr int kConsumerRegs = 104;
-static constexpr int kMaxBiasBytes = 8192;       // bias vector of the layer in shared memory (<= 1920 output channels: the data gradient
-                                                 // of SPP.cv2 has 1024)
-// weight packs up to this size stay resident: 121 KB, room for kMinResidentStages A stages and 10 KB of barriers, the largest bias vector
-// and slack, whatever the layer's Co (the 128 KB packs measured the same resident or streamed, DESIGN §5)
+static constexpr int kMaxBiasBytes = 12288;      // bias vector of the layer in shared memory (<= 2944 output channels: the data gradient
+                                                 // of SPP.cv2 has 4 c_ = 1024 / 1536 / 2048 / 2560 in s / m / l / x).  The shared-memory
+                                                 // layout is sized per layer (size_launch), so a layer of at most 1920 channels is
+                                                 // launched exactly as it was under the former 8 KB bound
+// weight packs up to this size stay resident: 121 KB, room for kMinResidentStages A stages and 10 KB of barriers, a bias vector of up to
+// 1920 channels and slack (a wider layer keeps one A stage fewer; the 128 KB packs measured the same resident or streamed, DESIGN §5)
 static constexpr int kResidentPackLimit = kSmemBudget - 10 * 1024 - kMinResidentStages * kTileM * kKStage * 2;
 static constexpr int kSiluSfuEvery = 2;   // every n-th output channel of a 16-channel group takes the two-MUFU SiLU (balances the FMA
                                           // pipe and the SFU)

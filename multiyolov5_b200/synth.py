@@ -6,6 +6,7 @@ values are reproducible on the GPU box without shipping 31 MB of weights.
 BN statistics are randomised on purpose (reference defaults 0/1/1/0 would make BN folding trivial,
 SURVEY.md §8c "Weights").
 """
+import gzip
 import json
 import os
 from typing import Dict, List
@@ -24,14 +25,20 @@ def load_cfg(name: str) -> dict:
 
 
 def load_manifest(tag: str) -> List[list]:
-    with open(os.path.join(GOLDEN_DIR, f"manifest_{tag}.json")) as f:
+    path = os.path.join(GOLDEN_DIR, f"manifest_{tag}.json")
+    if not os.path.isfile(path):      # the l / x manifests are stored compressed
+        with gzip.open(path + ".gz", "rt") as f:
+            return json.load(f)
+    with open(path) as f:
         return json.load(f)
 
 
 def synth_state_dict(manifest: List[list], cfg: dict, seed: int = 1, gain: float = None) -> Dict[str, torch.Tensor]:
     """manifest: [[key, shape, dtype_str], ...] in the reference's state_dict order."""
-    if gain is None:  # near-critical gains keep activations O(1..10) through ~60 layers (calibrated, see DESIGN.md)
-        gain = 2.0 if cfg["width_multiple"] <= 0.5 else 1.9
+    if gain is None:  # near-critical gains keep activations O(1..10) through ~60 layers (calibrated, see DESIGN.md).  The deeper l / x
+        # C3 stacks amplify faster: at 1.9 their largest activation is 2e4 (l) and 1e6 (x); at 1.6 / 1.4 it is 11 / 10
+        w = cfg["width_multiple"]
+        gain = 2.0 if w <= 0.5 else (1.9 if w <= 0.75 else (1.6 if w <= 1.0 else 1.4))
     rs = np.random.RandomState(seed)
     sd = {}
     strides = [8.0, 16.0, 32.0]
