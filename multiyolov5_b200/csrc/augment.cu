@@ -28,14 +28,6 @@ __global__ void resize_u8_kernel(const unsigned char* src, ResizeGeom g, unsigne
   }
 }
 
-int launch_resize_u8(const unsigned char* src, int H0, int W0, unsigned char* dst, int H, int W, cudaStream_t s) {
-  MYOLO_REQUIRE(src && dst && H0 > 0 && W0 > 0 && H > 0 && W > 0, "resize_u8: bad geometry (src %dx%d dst %dx%d)", W0, H0, W, H);
-  const long total = (long)H * W;
-  resize_u8_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(src, resize_geom(H0, W0, H, W), dst, H, W);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
 // load_image's augment=False cache resize: cv2.INTER_AREA whenever the image shrinks
 __global__ void resize_area_u8_kernel(const unsigned char* __restrict__ src, AreaGeom g, unsigned char* __restrict__ dst, int H, int W) {
   const long total = (long)H * W;
@@ -46,15 +38,6 @@ __global__ void resize_area_u8_kernel(const unsigned char* __restrict__ src, Are
     dst[i * 3 + 1] = (unsigned char)v[1];
     dst[i * 3 + 2] = (unsigned char)v[2];
   }
-}
-
-int launch_resize_area_u8(const unsigned char* src, int H0, int W0, unsigned char* dst, int H, int W, cudaStream_t s) {
-  MYOLO_REQUIRE(src && dst && H0 > 0 && W0 > 0 && H > 0 && W > 0, "resize_area_u8: bad geometry (src %dx%d dst %dx%d)", W0, H0, W, H);
-  MYOLO_REQUIRE(H <= H0 && W <= W0, "resize_area_u8: down-scaling only (src %dx%d dst %dx%d)", W0, H0, W, H);
-  const long total = (long)H * W;
-  resize_area_u8_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(src, area_geom(H0, W0, H, W), dst, H, W);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
 }
 
 // one of the (up to) four tiles of a warp's virtual canvas
@@ -153,15 +136,6 @@ __global__ void __launch_bounds__(256) augment_det_kernel(const myolo_aug_item* 
   }
 }
 
-int launch_augment_det(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, cudaStream_t s) {
-  MYOLO_REQUIRE(items && out && B > 0 && H > 0 && W > 0, "augment_det: bad arguments (B %d H %d W %d)", B, H, W);
-  MYOLO_REQUIRE(out_dtype == MYOLO_U8 || out_dtype == MYOLO_F16 || out_dtype == MYOLO_F32, "augment_det: output dtype");
-  const long total = (long)B * H * W;
-  augment_det_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(items, B, H, W, out, out_dtype);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
 // ------------------------------------------------------------------------------------------------
 // --multi-scale (reference train.py:354-359): F.interpolate(imgs, size=ns, mode='bilinear', align_corners=False) of the det batch, bit
 // exact with ATen's CUDA kernel (UpSampleBilinear2d.cu upsample_bilinear2d_out_frame).  The host passes ATen's scales, float(in) / out.
@@ -228,22 +202,6 @@ static void launch_resize_bilinear_from(const Ts* src, int planes, int H, int W,
   else resize_bilinear_kernel<Ts, float><<<grid, 128, 0, s>>>(src, planes, H, W, (float*)dst, Ho, Wo, rh, rw);
 }
 
-int launch_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo, cudaStream_t s) {
-  MYOLO_REQUIRE(src && dst && B > 0 && C > 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0 && Ho <= 65535,
-                "resize_bilinear: bad geometry (B %d C %d src %dx%d dst %dx%d)", B, C, H, W, Ho, Wo);
-  MYOLO_REQUIRE(src_dtype == MYOLO_U8 || src_dtype == MYOLO_F16 || src_dtype == MYOLO_F32, "resize_bilinear: source dtype %d", src_dtype);
-  MYOLO_REQUIRE(dst_dtype == MYOLO_F16 || dst_dtype == MYOLO_F32, "resize_bilinear: output dtype %d", dst_dtype);
-  MYOLO_REQUIRE((long)B * C <= (1L << 31) - 1, "resize_bilinear: too many planes");
-  const int planes = B * C;
-  // area_pixel_compute_scale with no scale factor given: static_cast<float>(input_size) / output_size, in fp32 on the host
-  const float rh = (float)H / (float)Ho, rw = (float)W / (float)Wo;
-  if (src_dtype == MYOLO_U8) launch_resize_bilinear_from((const unsigned char*)src, planes, H, W, dst, dst_dtype, Ho, Wo, rh, rw, s);
-  else if (src_dtype == MYOLO_F16) launch_resize_bilinear_from((const __half*)src, planes, H, W, dst, dst_dtype, Ho, Wo, rh, rw, s);
-  else launch_resize_bilinear_from((const float*)src, planes, H, W, dst, dst_dtype, Ho, Wo, rh, rw, s);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
 // ------------------------------------------------------------------------------------------------
 // scale_img (reference utils/torch_utils.py:248-258) of test-time augmentation, optionally of x.flip(3): F.interpolate to (Ho, Wo) as
 // resize_bilinear_kernel computes it, then F.pad on the right and bottom to (Hp, Wp) with `pad` (already rounded to the dtype by the
@@ -280,23 +238,6 @@ __global__ void __launch_bounds__(128) scale_img_kernel(const T* __restrict__ sr
     if constexpr (sizeof(T) == 2) dst[o] = __float2half_rn(val);
     else dst[o] = val;
   }
-}
-
-int launch_scale_img(const void* src, int dtype, int B, int C, int H, int W, void* dst, int Ho, int Wo, int Hp, int Wp, int flip_lr, float pad,
-                     cudaStream_t s) {
-  MYOLO_REQUIRE(src && dst && B > 0 && C > 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0 && Hp > 0 && Wp > 0 && Hp <= 65535,
-                "scale_img: bad geometry (B %d C %d src %dx%d resized %dx%d padded %dx%d)", B, C, H, W, Ho, Wo, Hp, Wp);
-  MYOLO_REQUIRE(dtype == MYOLO_F16 || dtype == MYOLO_F32, "scale_img: dtype %d (fp16 or fp32 only)", dtype);
-  MYOLO_REQUIRE((long)B * C <= (1L << 31) - 1, "scale_img: too many planes");
-  const int planes = B * C;
-  const float rh = (float)H / (float)Ho, rw = (float)W / (float)Wo;     // area_pixel_compute_scale, as in launch_resize_bilinear
-  const dim3 grid((Wp + 127) / 128, Hp, std::min(planes, 65535));
-  if (dtype == MYOLO_F16)
-    scale_img_kernel<__half><<<grid, 128, 0, s>>>((const __half*)src, planes, H, W, (__half*)dst, Ho, Wo, Hp, Wp, rh, rw, flip_lr != 0, pad);
-  else
-    scale_img_kernel<float><<<grid, 128, 0, s>>>((const float*)src, planes, H, W, (float*)dst, Ho, Wo, Hp, Wp, rh, rw, flip_lr != 0, pad);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -415,7 +356,83 @@ __global__ void __launch_bounds__(256) collate_quad_kernel(const unsigned char* 
   else reinterpret_cast<float*>(out)[o] = quad_unit(v);
 }
 
-int launch_collate_quad(const unsigned char* imgs, int B, int H, int W, const unsigned char* tile, void* out, int out_dtype, cudaStream_t s) {
+}  // namespace myolo
+
+using namespace myolo;
+
+extern "C" int myolo_resize_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(src && dst && H0 > 0 && W0 > 0 && H > 0 && W > 0, "resize_u8: bad geometry (src %dx%d dst %dx%d)", W0, H0, W, H);
+  const long total = (long)H * W;
+  resize_u8_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(src, resize_geom(H0, W0, H, W), dst, H, W);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_resize_area_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(src && dst && H0 > 0 && W0 > 0 && H > 0 && W > 0, "resize_area_u8: bad geometry (src %dx%d dst %dx%d)", W0, H0, W, H);
+  MYOLO_REQUIRE(H <= H0 && W <= W0, "resize_area_u8: down-scaling only (src %dx%d dst %dx%d)", W0, H0, W, H);
+  const long total = (long)H * W;
+  resize_area_u8_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(src, area_geom(H0, W0, H, W), dst, H, W);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_augment_det_hw(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(items && out && B > 0 && H > 0 && W > 0, "augment_det: bad arguments (B %d H %d W %d)", B, H, W);
+  MYOLO_REQUIRE(out_dtype == MYOLO_U8 || out_dtype == MYOLO_F16 || out_dtype == MYOLO_F32, "augment_det: output dtype");
+  const long total = (long)B * H * W;
+  augment_det_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(items, B, H, W, out, out_dtype);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo,
+                                     void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(src && dst && B > 0 && C > 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0 && Ho <= 65535,
+                "resize_bilinear: bad geometry (B %d C %d src %dx%d dst %dx%d)", B, C, H, W, Ho, Wo);
+  MYOLO_REQUIRE(src_dtype == MYOLO_U8 || src_dtype == MYOLO_F16 || src_dtype == MYOLO_F32, "resize_bilinear: source dtype %d", src_dtype);
+  MYOLO_REQUIRE(dst_dtype == MYOLO_F16 || dst_dtype == MYOLO_F32, "resize_bilinear: output dtype %d", dst_dtype);
+  MYOLO_REQUIRE((long)B * C <= (1L << 31) - 1, "resize_bilinear: too many planes");
+  const int planes = B * C;
+  // area_pixel_compute_scale with no scale factor given: static_cast<float>(input_size) / output_size, in fp32 on the host
+  const float rh = (float)H / (float)Ho, rw = (float)W / (float)Wo;
+  if (src_dtype == MYOLO_U8) launch_resize_bilinear_from((const unsigned char*)src, planes, H, W, dst, dst_dtype, Ho, Wo, rh, rw, s);
+  else if (src_dtype == MYOLO_F16) launch_resize_bilinear_from((const __half*)src, planes, H, W, dst, dst_dtype, Ho, Wo, rh, rw, s);
+  else launch_resize_bilinear_from((const float*)src, planes, H, W, dst, dst_dtype, Ho, Wo, rh, rw, s);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_scale_img(const void* src, int dtype, int B, int C, int H, int W, void* dst, int Ho, int Wo, int Hp, int Wp, int flip_lr,
+                               float pad, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(src && dst && B > 0 && C > 0 && H > 0 && W > 0 && Ho > 0 && Wo > 0 && Hp > 0 && Wp > 0 && Hp <= 65535,
+                "scale_img: bad geometry (B %d C %d src %dx%d resized %dx%d padded %dx%d)", B, C, H, W, Ho, Wo, Hp, Wp);
+  MYOLO_REQUIRE(dtype == MYOLO_F16 || dtype == MYOLO_F32, "scale_img: dtype %d (fp16 or fp32 only)", dtype);
+  MYOLO_REQUIRE((long)B * C <= (1L << 31) - 1, "scale_img: too many planes");
+  const int planes = B * C;
+  const float rh = (float)H / (float)Ho, rw = (float)W / (float)Wo;     // area_pixel_compute_scale, as in myolo_resize_bilinear
+  const dim3 grid((Wp + 127) / 128, Hp, std::min(planes, 65535));
+  if (dtype == MYOLO_F16)
+    scale_img_kernel<__half><<<grid, 128, 0, s>>>((const __half*)src, planes, H, W, (__half*)dst, Ho, Wo, Hp, Wp, rh, rw, flip_lr != 0, pad);
+  else
+    scale_img_kernel<float><<<grid, 128, 0, s>>>((const float*)src, planes, H, W, (float*)dst, Ho, Wo, Hp, Wp, rh, rw, flip_lr != 0, pad);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_collate_quad(const uint8_t* imgs, int B, int H, int W, const uint8_t* tile, void* out, int out_dtype, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   MYOLO_REQUIRE(imgs && out && tile && B >= 4 && H > 0 && W > 0, "collate_quad: bad arguments (B %d H %d W %d)", B, H, W);
   MYOLO_REQUIRE(B / 4 <= MYOLO_QUAD_MAX, "collate_quad: %d quads, at most %d", B / 4, MYOLO_QUAD_MAX);
   MYOLO_REQUIRE((long)H * W <= (1L << 28), "collate_quad: %dx%d images are too large", H, W);
@@ -437,5 +454,3 @@ int launch_collate_quad(const unsigned char* imgs, int B, int H, int W, const un
   MYOLO_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace myolo

@@ -189,19 +189,23 @@ __global__ void __launch_bounds__(256) seg_jitter_kernel(const myolo_seg_item* _
   }
 }
 
-int launch_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int mw, const int* tables, unsigned char* scratch, void* out,
-                       int out_dtype, long long* out_mask, cudaStream_t s) {
+}  // namespace myolo
+
+using namespace myolo;
+
+extern "C" int myolo_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int mw, const int32_t* tables, uint8_t* scratch,
+                                 void* out, int out_dtype, int64_t* out_mask, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   MYOLO_REQUIRE(items && tables && scratch && out && out_mask && B > 0 && h > 0 && w > 0 && mh > 0 && mw > 0 && B <= 65535,
                 "augment_seg: bad arguments (B %d image %dx%d mask %dx%d)", B, w, h, mw, mh);
   MYOLO_REQUIRE(out_dtype == MYOLO_U8 || out_dtype == MYOLO_F16 || out_dtype == MYOLO_F32, "augment_seg: output dtype");
   const long n = std::max((long)h * w, (long)mh * mw);
   const int per_item = (int)std::max<long>(1, std::min<long>((n + 255) / 256, (132L * 16 + B - 1) / B));
-  seg_resample_kernel<<<dim3(per_item, B), 256, 0, s>>>(items, h, w, mh, mw, tables, scratch, out_mask);
+  seg_resample_kernel<<<dim3(per_item, B), 256, 0, s>>>(items, h, w, mh, mw, tables, scratch, reinterpret_cast<long long*>(out_mask));
   MYOLO_LAUNCH_CHECK();
   const int per_item2 = (int)std::max<long>(1, std::min<long>(((long)h * w + 255) / 256, (132L * 16 + B - 1) / B));
   seg_jitter_kernel<<<dim3(per_item2, B), 256, 0, s>>>(items, h, w, scratch, out, out_dtype);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace myolo

@@ -182,10 +182,21 @@ int evolve_grid(long n, int* grid) {
 
 }  // namespace
 
-int64_t anchor_metric_workspace_bytes() { return (int64_t)kMetricBlocks * sizeof(MetricPartial); }
+}  // namespace myolo
 
-int launch_anchor_metric(const void* wh, int wh_dtype, long n, const void* k, int k_dtype, int na, double thr, myolo_anchor_stats* out,
-                         void* workspace, cudaStream_t s) {
+using namespace myolo;
+
+extern "C" int64_t myolo_anchor_metric_workspace_bytes(void) { return (int64_t)kMetricBlocks * sizeof(MetricPartial); }
+
+extern "C" int myolo_anchor_metric(const void* wh, int wh_dtype, int64_t n, const void* k, int k_dtype, int na, double thr,
+                                   myolo_anchor_stats* out, void* workspace, int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_anchor_metric");
+  MYOLO_REQUIRE(wh && k && out && workspace && n > 0 && na >= 1 && na <= MYOLO_ANCHOR_MAX, "anchor_metric: bad arguments");
+  MYOLO_REQUIRE((wh_dtype == MYOLO_F32 || wh_dtype == MYOLO_F64) && (k_dtype == MYOLO_F32 || k_dtype == MYOLO_F64),
+                "anchor_metric: wh and k must be MYOLO_F32 or MYOLO_F64");
+  MYOLO_REQUIRE(workspace_bytes >= myolo_anchor_metric_workspace_bytes(), "anchor_metric: workspace too small");
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   const int grid = (int)std::max(1L, std::min<long>(kMetricBlocks, (n + kThreads - 1) / kThreads));
   auto* part = static_cast<MetricPartial*>(workspace);
   const bool w64 = wh_dtype == MYOLO_F64, k64 = k_dtype == MYOLO_F64;
@@ -199,27 +210,33 @@ int launch_anchor_metric(const void* wh, int wh_dtype, long n, const void* k, in
   return 0;
 }
 
-int anchor_evolve_workspace_bytes(long n, int64_t* bytes) {
+extern "C" int64_t myolo_anchor_evolve_workspace_bytes(int64_t n) {
   int grid = 0;
-  const int rc = evolve_grid(n, &grid);
-  if (rc) return rc;
-  *bytes = 2 * (int64_t)grid * (int64_t)sizeof(double);
-  return 0;
+  if (check_device(nullptr) || n <= 0 || evolve_grid(n, &grid)) return -1;
+  return 2 * (int64_t)grid * (int64_t)sizeof(double);
 }
 
-int launch_anchor_evolve(const float* wh, long n, const double* k0, int na, const double* v, int gen, float thr, double* k_out,
-                         float* f_out, float* fg_out, int* accepted_out, void* workspace, int64_t workspace_bytes, cudaStream_t s) {
+extern "C" int myolo_anchor_evolve(const float* wh, int64_t n, const double* k0, int na, const double* v, int gen, double thr,
+                                   double* k_out, float* f_out, float* fg_out, int32_t* accepted_out, void* workspace,
+                                   int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_anchor_evolve");
+  MYOLO_REQUIRE(wh && k0 && k_out && f_out && accepted_out && workspace && na >= 1 && na <= MYOLO_ANCHOR_MAX && gen >= 0 &&
+                (gen == 0 || (v && fg_out)), "anchor_evolve: bad arguments");
+  // the exact fp64 sum: every term a multiple of 2^-27 in [0, 1] (fp32(thr) >= 1/16) and fewer than 2^26 of them
+  MYOLO_REQUIRE(n >= 1 && n < (int64_t(1) << 26), "anchor_evolve: n = %lld labels, needs 1 <= n < 2^26", (long long)n);
+  const float thr32 = (float)thr;
+  MYOLO_REQUIRE(thr32 >= 0.0625f, "anchor_evolve: 1 / anchor_t = %g, needs anchor_t <= 16", thr);
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   int grid = 0;
   int rc = evolve_grid(n, &grid);
   if (rc) return rc;
   MYOLO_REQUIRE(workspace_bytes >= 2 * (int64_t)grid * (int64_t)sizeof(double), "anchor_evolve: workspace too small");
   double* partials = static_cast<double*>(workspace);
   const float2* wh2 = reinterpret_cast<const float2*>(wh);
-  void* args[] = {(void*)&wh2, (void*)&n, (void*)&k0, (void*)&na, (void*)&v, (void*)&gen, (void*)&thr, (void*)&partials, (void*)&k_out,
+  void* args[] = {(void*)&wh2, (void*)&n, (void*)&k0, (void*)&na, (void*)&v, (void*)&gen, (void*)&thr32, (void*)&partials, (void*)&k_out,
                   (void*)&f_out, (void*)&fg_out, (void*)&accepted_out};
   MYOLO_CHECK_CUDA(cudaLaunchCooperativeKernel((const void*)anchor_evolve_kernel, dim3(grid), dim3(kThreads), args, 0, s));
   MYOLO_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace myolo

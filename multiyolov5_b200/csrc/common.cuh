@@ -3,6 +3,7 @@
 #include <cuda.h>
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <nvtx3/nvToolsExt.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -17,6 +18,14 @@ namespace myolo {
 // ------------------------------------------------------------------------------------------------
 void set_error(const char* fmt, ...);
 extern thread_local int64_t g_launch_count;
+// 0 when the current device is an sm_90 part (its SM count into *sms, nullable), else MYOLO_E_NODEVICE with the reason set
+int check_device(int* sms);
+
+// NVTX ranges around every C-ABI entry point that launches work (SURVEY.md section 5): visible in nsys / ncu --nvtx, free when no tool is attached
+struct NvtxRange {
+  explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
+  ~NvtxRange() { nvtxRangePop(); }
+};
 
 #define MYOLO_CHECK_CUDA(expr)                                                                         \
   do {                                                                                                 \

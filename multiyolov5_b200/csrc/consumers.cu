@@ -37,20 +37,6 @@ __global__ void lut_blend_kernel(const void* idx, int idx_dtype, long n, const u
   }
 }
 
-int launch_lut_blend(const void* idx, int idx_dtype, long n, const unsigned char* lut, int n_entries, int ch, int reverse, unsigned char* out,
-                     const unsigned char* im, float alpha, float beta, unsigned char* blend, const unsigned char* lut2, int ch2,
-                     unsigned char* out2, cudaStream_t s) {
-  MYOLO_REQUIRE(idx && lut && n > 0 && n_entries > 0 && ch > 0 && n_entries * ch <= 4096 && (out || blend || out2) && (!blend || im),
-                "lut_blend: bad arguments");
-  MYOLO_REQUIRE(!out2 || (lut2 && ch2 > 0 && n_entries * ch2 <= 4096), "lut_blend: the second table needs lut2 and 0 < channels2");
-  MYOLO_REQUIRE(idx_dtype == MYOLO_U8 || idx_dtype == MYOLO_I64, "lut_blend: class map must be uint8 or int64");
-  const int smem = n_entries * (ch + (out2 ? ch2 : 0));
-  lut_blend_kernel<<<(int)std::min<long>(132L * 8, (n + 255) / 256), 256, smem, s>>>(idx, idx_dtype, n, lut, n_entries, ch, reverse, out, im,
-                                                                                     alpha, beta, blend, lut2, out2 ? ch2 : 0, out2);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
 // detect.py:166-177 over a batch of padded NMS rows, one CTA per frame.  geom[b] = {pad_x, pad_y, gain, w0, h0}, each already rounded to
 // fp32 as torch's CPU kernels round a Python scalar.  In place on rows [0, counts[b]): x -= pad, x /= gain, clamp to the frame, round half to
 // even (scale_coords(...).round(), fp32 IEEE like the reference's CPU run).  xywhn (nullable): (xyxy2xywh(xyxy) / gn) of the rounded box.
@@ -92,15 +78,6 @@ __global__ void detect_boxes_kernel(float* rows, const int32_t* counts, int max_
   }
 }
 
-int launch_detect_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, int nc, float* xywhn, int32_t* class_counts,
-                        cudaStream_t s) {
-  MYOLO_REQUIRE(rows && counts && geom && B > 0 && max_det > 0, "detect_boxes: bad arguments");
-  MYOLO_REQUIRE(!class_counts || (nc > 0 && nc <= 4096), "detect_boxes: class counts need 0 < nc <= 4096");
-  detect_boxes_kernel<<<B, 128, class_counts ? nc * (int)sizeof(int) : 0, s>>>(rows, counts, max_det, geom, nc, xywhn, class_counts);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
 // autoShape's scale_coords(shape1, y[:, :4], shape0) (reference models/common.py:668-669), one CTA per image: as detect_boxes_kernel
 // without the round, then Detections.__init__'s xyxy2xywh and its divisions by gn = (w0, h0, w0, h0, 1, 1) (models/common.py:680-688)
 __global__ void scale_boxes_kernel(float* rows, const int32_t* counts, int max_det, const float* geom, float* xywh, float* xyxyn,
@@ -135,14 +112,6 @@ __global__ void scale_boxes_kernel(float* rows, const int32_t* counts, int max_d
   }
 }
 
-int launch_scale_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, float* xywh, float* xyxyn, float* xywhn,
-                       cudaStream_t s) {
-  MYOLO_REQUIRE(rows && counts && geom && B > 0 && max_det > 0, "scale_boxes: bad arguments");
-  scale_boxes_kernel<<<B, 128, 0, s>>>(rows, counts, max_det, geom, xywh, xyxyn, xywhn);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
 // counters[0] = correct, [1] = labeled, [2..2+n) intersection, [2+n..2+2n) prediction area, [2+2n..2+3n) label area  (accumulated)
 __global__ void seg_hist_kernel(const void* pred, int pred_dtype, const long long* __restrict__ target, long n, int n_cls,
                                 unsigned long long* counters) {
@@ -167,15 +136,57 @@ __global__ void seg_hist_kernel(const void* pred, int pred_dtype, const long lon
     if (sh[k]) atomicAdd(&counters[k], (unsigned long long)sh[k]);
 }
 
-int launch_seg_hist(const void* pred, int pred_dtype, const long long* target, long n, int n_cls, unsigned long long* counters,
-                    cudaStream_t s) {
-  MYOLO_REQUIRE(pred && target && counters && n > 0 && n_cls > 0 && n_cls <= 1024, "seg_hist: bad arguments");
-  MYOLO_REQUIRE(pred_dtype == MYOLO_U8 || pred_dtype == MYOLO_I64, "seg_hist: prediction must be uint8 or int64");
-  // one block sees at most 2^32 - 1 pixels per counter: blocks of <= 2^24 pixels each
-  const int blocks = (int)std::max<long>(std::min<long>(132L * 8, (n + 255) / 256), (n + (1L << 24) - 1) >> 24);
-  seg_hist_kernel<<<blocks, 256, (2 + 3 * n_cls) * sizeof(unsigned int), s>>>(pred, pred_dtype, target, n, n_cls, counters);
+}  // namespace myolo
+
+using namespace myolo;
+
+extern "C" int myolo_seg_lut_blend(const void* idx, int idx_dtype, int64_t n, const uint8_t* lut, int n_entries, int ch, int reverse,
+                                   uint8_t* out, const uint8_t* im, float alpha, float beta, uint8_t* blend, const uint8_t* lut2, int ch2,
+                                   uint8_t* out2, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(idx && lut && n > 0 && n_entries > 0 && ch > 0 && n_entries * ch <= 4096 && (out || blend || out2) && (!blend || im),
+                "lut_blend: bad arguments");
+  MYOLO_REQUIRE(!out2 || (lut2 && ch2 > 0 && n_entries * ch2 <= 4096), "lut_blend: the second table needs lut2 and 0 < channels2");
+  MYOLO_REQUIRE(idx_dtype == MYOLO_U8 || idx_dtype == MYOLO_I64, "lut_blend: class map must be uint8 or int64");
+  const int smem = n_entries * (ch + (out2 ? ch2 : 0));
+  lut_blend_kernel<<<(int)std::min<long>(132L * 8, (n + 255) / 256), 256, smem, s>>>(idx, idx_dtype, n, lut, n_entries, ch, reverse, out, im,
+                                                                                     alpha, beta, blend, lut2, out2 ? ch2 : 0, out2);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }
 
-}  // namespace myolo
+extern "C" int myolo_detect_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, int nc, float* xywhn,
+                                  int32_t* class_counts, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(rows && counts && geom && B > 0 && max_det > 0, "detect_boxes: bad arguments");
+  MYOLO_REQUIRE(!class_counts || (nc > 0 && nc <= 4096), "detect_boxes: class counts need 0 < nc <= 4096");
+  detect_boxes_kernel<<<B, 128, class_counts ? nc * (int)sizeof(int) : 0, s>>>(rows, counts, max_det, geom, nc, xywhn, class_counts);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_scale_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, float* xywh, float* xyxyn,
+                                 float* xywhn, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(rows && counts && geom && B > 0 && max_det > 0, "scale_boxes: bad arguments");
+  scale_boxes_kernel<<<B, 128, 0, s>>>(rows, counts, max_det, geom, xywh, xyxyn, xywhn);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_seg_metrics(const void* pred, int pred_dtype, const int64_t* target, int64_t n, int n_cls, uint64_t* counters,
+                                 void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(pred && target && counters && n > 0 && n_cls > 0 && n_cls <= 1024, "seg_hist: bad arguments");
+  MYOLO_REQUIRE(pred_dtype == MYOLO_U8 || pred_dtype == MYOLO_I64, "seg_hist: prediction must be uint8 or int64");
+  // one block sees at most 2^32 - 1 pixels per counter: blocks of <= 2^24 pixels each
+  const int blocks = (int)std::max<long>(std::min<long>(132L * 8, (n + 255) / 256), (n + (1L << 24) - 1) >> 24);
+  seg_hist_kernel<<<blocks, 256, (2 + 3 * n_cls) * sizeof(unsigned int), s>>>(pred, pred_dtype, reinterpret_cast<const long long*>(target), n,
+                                                                              n_cls, reinterpret_cast<unsigned long long*>(counters));
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}

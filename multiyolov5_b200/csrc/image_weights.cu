@@ -176,20 +176,35 @@ int sm_count() {
 
 }  // namespace
 
-int launch_class_weights(const float* cls, long long n_labels, int nc, unsigned long long* counts, double* weights, int32_t* status,
-                         cudaStream_t s) {
+}  // namespace myolo
+
+using namespace myolo;
+
+extern "C" int myolo_class_weights(const float* cls, int64_t n_labels, int nc, int64_t* counts, double* weights, int32_t* status,
+                                   void* stream) {
+  NvtxRange nvtx_("myolo_class_weights");
+  MYOLO_REQUIRE((cls || n_labels == 0) && n_labels >= 0 && counts && weights && status, "class_weights: bad arguments");
+  MYOLO_REQUIRE(nc >= 1 && nc <= MYOLO_IW_NC_MAX, "class_weights: nc = %d, needs 1 <= nc <= %d", nc, MYOLO_IW_NC_MAX);
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   MYOLO_CHECK_CUDA(cudaMemsetAsync(counts, 0, sizeof(unsigned long long) * nc, s));
   const long long want = (n_labels + kHistThreads - 1) / kHistThreads;
   const int grid = (int)max(1LL, min(want, (long long)sm_count() * 8));
-  class_count_kernel<<<grid, kHistThreads, sizeof(unsigned int) * nc, s>>>(cls, n_labels, nc, counts, status);
+  class_count_kernel<<<grid, kHistThreads, sizeof(unsigned int) * nc, s>>>(cls, n_labels, nc, reinterpret_cast<unsigned long long*>(counts),
+                                                                           status);
   MYOLO_LAUNCH_CHECK();
-  class_weights_kernel<<<1, kHistThreads, 0, s>>>(counts, nc, weights);
+  class_weights_kernel<<<1, kHistThreads, 0, s>>>(reinterpret_cast<unsigned long long*>(counts), nc, weights);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }
 
-int launch_image_weights(const float* cls, const int64_t* offsets, long long n, const double* cw, int nc, double* iw, int32_t* status,
-                         cudaStream_t s) {
+extern "C" int myolo_image_weights(const float* cls, const int64_t* offsets, int64_t n, const double* cw, int nc, double* iw,
+                                   int32_t* status, void* stream) {
+  NvtxRange nvtx_("myolo_image_weights");
+  MYOLO_REQUIRE(cls && offsets && cw && iw && status && n >= 1, "image_weights: bad arguments");
+  MYOLO_REQUIRE(nc >= 1 && nc <= MYOLO_IW_NC_MAX, "image_weights: nc = %d, needs 1 <= nc <= %d", nc, MYOLO_IW_NC_MAX);
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   const size_t smem = sizeof(double) * nc + sizeof(unsigned int) * nc * kImageWarps;
   const long long want = (n + kImageWarps - 1) / kImageWarps;
   const int grid = (int)max(1LL, min(want, (long long)sm_count() * 16));
@@ -198,13 +213,16 @@ int launch_image_weights(const float* cls, const int64_t* offsets, long long n, 
   return 0;
 }
 
-int launch_weighted_draw(const double* w, const double* u, long long n, double* cum, double* total, int32_t* idx, int32_t* status,
-                         cudaStream_t s) {
+extern "C" int myolo_weighted_draw(const double* w, const double* u, int64_t n, double* cum, double* total, int32_t* idx, int32_t* status,
+                                   void* stream) {
+  NvtxRange nvtx_("myolo_weighted_draw");
+  MYOLO_REQUIRE(w && u && cum && total && idx && status, "weighted_draw: bad arguments");
+  MYOLO_REQUIRE(n >= 1 && n < (int64_t(1) << 31), "weighted_draw: n = %lld, needs 1 <= n < 2^31", (long long)n);
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   weighted_scan_kernel<<<1, kScanThreads, 0, s>>>(w, n, cum, total, status);
   MYOLO_LAUNCH_CHECK();
   weighted_draw_kernel<<<(unsigned)((n + kDrawThreads - 1) / kDrawThreads), kDrawThreads, 0, s>>>(cum, total, u, n, idx, status);
   MYOLO_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace myolo

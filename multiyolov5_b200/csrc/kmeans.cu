@@ -250,16 +250,31 @@ int kmeans_ctas(int* ctas) {
 
 }  // namespace
 
-int64_t kmeans_workspace_bytes(long n, int restarts) { return kHeader + (int64_t)restarts * layout(n).stride; }
+}  // namespace myolo
 
-int launch_kmeans(const double* obs, long n, const int64_t* init_idx, int k, int restarts, double thresh, int max_iter, double* books,
-                  int32_t* book_k, double* dists, int32_t* iters, int32_t* best, int32_t* status, void* ws, int64_t ws_bytes,
-                  cudaStream_t s) {
+using namespace myolo;
+
+extern "C" int64_t myolo_kmeans_workspace_bytes(int64_t n, int k, int restarts) {
+  if (n < 1 || n >= (int64_t(1) << 30) || k < 1 || restarts < 1) return -1;
+  return kHeader + (int64_t)restarts * layout(n).stride;
+}
+
+extern "C" int myolo_kmeans(const double* obs, int64_t n, int d, const int64_t* init_idx, int k, int restarts, double thresh, int max_iter,
+                            double* books, int32_t* book_k, double* dists, int32_t* iters, int32_t* best, int32_t* status, void* ws,
+                            int64_t ws_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_kmeans");
+  MYOLO_REQUIRE(obs && init_idx && books && book_k && dists && iters && best && status && ws && restarts >= 1 && max_iter >= 1,
+                "kmeans: bad arguments");
+  MYOLO_REQUIRE(d == 2, "kmeans: d = %d features, only d = 2 is built", d);
+  MYOLO_REQUIRE(k >= 1 && k <= MYOLO_KMEANS_KMAX, "kmeans: k = %d, needs 1 <= k <= %d", k, MYOLO_KMEANS_KMAX);
+  MYOLO_REQUIRE(n >= k && n < (int64_t(1) << 30), "kmeans: n = %lld observations, needs k <= n < 2^30", (long long)n);
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   int ctas = 0;
   int rc = kmeans_ctas(&ctas);
   if (rc) return rc;
   MYOLO_REQUIRE(restarts <= ctas, "kmeans: %d restarts, at most %d (one co-resident CTA each)", restarts, ctas);
-  MYOLO_REQUIRE(ws_bytes >= kmeans_workspace_bytes(n, restarts), "kmeans: workspace too small");
+  MYOLO_REQUIRE(ws_bytes >= myolo_kmeans_workspace_bytes(n, k, restarts), "kmeans: workspace too small");
   MYOLO_CHECK_CUDA(cudaMemsetAsync(ws, 0, sizeof(unsigned int), s));
   MYOLO_CHECK_CUDA(cudaMemsetAsync(status, 0, sizeof(int32_t), s));
   kmeans_kernel<<<restarts, kThreads, 0, s>>>(reinterpret_cast<const double2*>(obs), (int)n, reinterpret_cast<const long long*>(init_idx),
@@ -268,5 +283,3 @@ int launch_kmeans(const double* obs, long n, const int64_t* init_idx, int k, int
   MYOLO_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace myolo

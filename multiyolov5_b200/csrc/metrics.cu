@@ -165,18 +165,6 @@ __global__ void __launch_bounds__(kMatchThreads) det_match_kernel(
   }
 }
 
-int launch_det_match(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H, int W,
-                     const float* geom, const float* iouv, int img_base, uint16_t* st_correct, float* st_conf, uint8_t* st_cls,
-                     int32_t* st_rows, unsigned long long* tcount, int32_t* err, cudaStream_t s) {
-  MYOLO_REQUIRE(dets && counts && geom && iouv && st_correct && st_conf && st_cls && st_rows && tcount && err, "det_match: null argument");
-  MYOLO_REQUIRE(B > 0 && max_det > 0 && max_det <= kMaxDetRows && H > 0 && W > 0 && img_base >= 0 && n_targets >= 0 &&
-                (n_targets == 0 || targets), "det_match: bad arguments (max_det <= %d)", kMaxDetRows);
-  det_match_kernel<<<B, kMatchThreads, 0, s>>>(dets, counts, max_det, targets, n_targets, (float)H, (float)W, geom, iouv, img_base,
-                                               st_correct, st_conf, st_cls, st_rows, tcount, err);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
 // ---------------------------------------------------------------------------------------------------------------------------------
 // ConfusionMatrix.process_batch (the fork's utils/metrics.py:115-162), one CTA per image
 //
@@ -297,18 +285,6 @@ __global__ void __launch_bounds__(kMatchThreads) confusion_kernel(
         atomicAdd(&matrix[s_dcls[p] * ld + nc], 1ull);                            // background FN
 }
 
-int launch_confusion(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H, int W,
-                     const float* geom, int nc, float conf_thres, float iou_thres, int require_rows, unsigned long long* matrix, int32_t* err,
-                     cudaStream_t s) {
-  MYOLO_REQUIRE(dets && counts && matrix && err, "confusion: null argument");
-  MYOLO_REQUIRE(B > 0 && max_det > 0 && max_det <= kMaxDetRows && nc > 0 && nc <= 4096 && n_targets >= 0 && (n_targets == 0 || targets) &&
-                (geom == nullptr || (H > 0 && W > 0)), "confusion: bad arguments (max_det <= %d, nc <= 4096)", kMaxDetRows);
-  confusion_kernel<<<B, kMatchThreads, 0, s>>>(dets, counts, max_det, targets, n_targets, (float)H, (float)W, geom, nc, conf_thres, iou_thres,
-                                               require_rows, matrix, err);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
 // ---------------------------------------------------------------------------------------------------------------------------------
 // ap_per_class
 // ---------------------------------------------------------------------------------------------------------------------------------
@@ -350,11 +326,6 @@ static size_t ap_layout(int n_images, int max_det, int ncol, ApWorkspace* w, cha
   t.env = (double*)take(sizeof(double) * (size_t)ncol * nmax);
   if (w) *w = t;
   return off;
-}
-
-int64_t det_ap_workspace_bytes(int n_images, int max_det, int ncol) {
-  if (n_images <= 0 || max_det <= 0 || ncol <= 0) return 0;
-  return (int64_t)ap_layout(n_images, max_det, ncol, nullptr, nullptr);
 }
 
 // block-wide inclusive scan (sum or max) over kApThreads values in shared memory
@@ -619,15 +590,54 @@ __global__ void __launch_bounds__(kApThreads) ap_class_kernel(const uint16_t* __
   }
 }
 
-int launch_det_ap(const uint16_t* correct, const float* conf, const uint8_t* cls, const int32_t* rows, int n_images, int max_det, int ncol,
-                  const unsigned long long* tcount, const double* px, const double* x101, double* out_ap, double* out_p, double* out_r,
-                  int32_t* out_info, void* workspace, int64_t workspace_bytes, cudaStream_t s) {
+}  // namespace myolo
+
+using namespace myolo;
+
+extern "C" int myolo_det_match(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H, int W,
+                               const float* geom, const float* iouv, int img_base, uint16_t* st_correct, float* st_conf, uint8_t* st_cls,
+                               int32_t* st_rows, uint64_t* tcount, int32_t* err, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(dets && counts && geom && iouv && st_correct && st_conf && st_cls && st_rows && tcount && err, "det_match: null argument");
+  MYOLO_REQUIRE(B > 0 && max_det > 0 && max_det <= kMaxDetRows && H > 0 && W > 0 && img_base >= 0 && n_targets >= 0 &&
+                (n_targets == 0 || targets), "det_match: bad arguments (max_det <= %d)", kMaxDetRows);
+  det_match_kernel<<<B, kMatchThreads, 0, s>>>(dets, counts, max_det, targets, n_targets, (float)H, (float)W, geom, iouv, img_base,
+                                               st_correct, st_conf, st_cls, st_rows, reinterpret_cast<unsigned long long*>(tcount), err);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_confusion_update(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets,
+                                      int H, int W, const float* geom, int nc, float conf_thres, float iou_thres, int require_rows,
+                                      int64_t* matrix, int32_t* err, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(dets && counts && matrix && err, "confusion: null argument");
+  MYOLO_REQUIRE(B > 0 && max_det > 0 && max_det <= kMaxDetRows && nc > 0 && nc <= 4096 && n_targets >= 0 && (n_targets == 0 || targets) &&
+                (geom == nullptr || (H > 0 && W > 0)), "confusion: bad arguments (max_det <= %d, nc <= 4096)", kMaxDetRows);
+  confusion_kernel<<<B, kMatchThreads, 0, s>>>(dets, counts, max_det, targets, n_targets, (float)H, (float)W, geom, nc, conf_thres, iou_thres,
+                                               require_rows, reinterpret_cast<unsigned long long*>(matrix), err);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int64_t myolo_det_ap_workspace_bytes(int n_images, int max_det, int ncol) {
+  if (n_images <= 0 || max_det <= 0 || ncol <= 0) return 0;
+  return (int64_t)ap_layout(n_images, max_det, ncol, nullptr, nullptr);
+}
+
+extern "C" int myolo_det_ap(const uint16_t* correct, const float* conf, const uint8_t* cls, const int32_t* rows, int n_images, int max_det,
+                            int ncol, const uint64_t* tcount, const double* px, const double* x101, double* out_ap, double* out_p,
+                            double* out_r, int32_t* out_info, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   MYOLO_REQUIRE(correct && conf && cls && rows && tcount && px && x101 && out_ap && out_p && out_r && out_info && workspace,
                 "det_ap: null argument");
   MYOLO_REQUIRE(n_images > 0 && max_det > 0 && ncol >= 1 && ncol <= 16, "det_ap: bad arguments");
   const long nmax = (long)n_images * max_det;
   MYOLO_REQUIRE(nmax < (1L << 31), "det_ap: store too large");
-  MYOLO_REQUIRE(workspace_bytes >= det_ap_workspace_bytes(n_images, max_det, ncol), "det_ap: workspace too small");
+  MYOLO_REQUIRE(workspace_bytes >= myolo_det_ap_workspace_bytes(n_images, max_det, ncol), "det_ap: workspace too small");
   ApWorkspace w;
   ap_layout(n_images, max_det, ncol, &w, (char*)workspace);
   long L;
@@ -649,11 +659,9 @@ int launch_det_ap(const uint16_t* correct, const float* conf, const uint8_t* cls
     MYOLO_LAUNCH_CHECK();
     cur ^= 1;
   }
-  ap_class_kernel<<<dim3(256, ncol), kApThreads, 0, s>>>(correct, conf, tcount, w.hdr, w.vals[cur], nmax, ncol, px, x101, w.tpc, w.env,
-                                                         out_ap, out_p, out_r);
+  ap_class_kernel<<<dim3(256, ncol), kApThreads, 0, s>>>(correct, conf, reinterpret_cast<const unsigned long long*>(tcount), w.hdr, w.vals[cur],
+                                                         nmax, ncol, px, x101, w.tpc, w.env, out_ap, out_p, out_r);
   MYOLO_LAUNCH_CHECK();
   MYOLO_CHECK_CUDA(cudaMemcpyAsync(out_info, w.hdr, 2 * sizeof(int32_t), cudaMemcpyDeviceToDevice, s));
   return 0;
 }
-
-}  // namespace myolo

@@ -14,7 +14,6 @@
 // are virtual rows A .. A + k_b - 1 of that image with box = xywh, obj = 1 and a one-hot class.  Their candidate index i * nc + j
 // then sorts after every anchor of the image on equal scores, the position torch.cat((x, v), 0) gives them.  They skip the obj >
 // conf_thres pre-filter, as in the reference, and take every later step like any other candidate (so at conf_thres >= 1 they drop out).
-#include <nvtx3/nvToolsExt.h>
 #include "common.cuh"
 
 namespace myolo {
@@ -361,8 +360,7 @@ static int nms_launch(const float* pred, int B, int A, int no, float conf_thres,
 extern "C" int myolo_nms(const float* pred, int B, int A, int no, float conf_thres, float iou_thres, const int32_t* classes,
                          int n_classes, int agnostic, int multi_label, int max_det, int max_nms, float max_wh, float* out,
                          int32_t* out_count, void* workspace, int64_t workspace_bytes, void* stream) {
-  nvtxRangePushA("myolo_nms");
-  struct Pop { ~Pop() { nvtxRangePop(); } } nvtx_pop_;
+  NvtxRange nvtx_("myolo_nms");
   return nms_launch(pred, B, A, no, conf_thres, iou_thres, classes, n_classes, agnostic, multi_label, max_det, max_nms, max_wh, nullptr,
                     nullptr, 0, nullptr, out, out_count, workspace, workspace_bytes, stream);
 }
@@ -371,8 +369,7 @@ extern "C" int myolo_nms_labels(const float* pred, int B, int A, int no, float c
                                 int n_classes, int agnostic, int multi_label, int max_det, int max_nms, float max_wh, const float* labels,
                                 const int32_t* label_offsets, int max_labels, int32_t* err, float* out, int32_t* out_count, void* workspace,
                                 int64_t workspace_bytes, void* stream) {
-  nvtxRangePushA("myolo_nms_labels");
-  struct Pop { ~Pop() { nvtxRangePop(); } } nvtx_pop_;
+  NvtxRange nvtx_("myolo_nms_labels");
   MYOLO_REQUIRE(label_offsets && err && max_labels >= 0 && (labels || max_labels == 0), "nms_labels: null pointer or bad max_labels");
   return nms_launch(pred, B, A, no, conf_thres, iou_thres, classes, n_classes, agnostic, multi_label, max_det, max_nms, max_wh,
                     labels, label_offsets, max_labels, err, out, out_count, workspace, workspace_bytes, stream);

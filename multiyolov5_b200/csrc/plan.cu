@@ -1,12 +1,6 @@
 // C ABI + layer-plan executor: what Model.__init__/fuse() and Model.forward_once (reference models/yolo.py:293-316,339-347)
 // become on the device.  The host-side planner (multiyolov5_b200/plan.py) lowers the module tree to a flat op list over
 // liveness-packed NHWC buffers; this file resolves views, owns packed weights / tensor maps and replays the list on a stream.
-#include <nvtx3/nvToolsExt.h>
-// NVTX ranges around every C-ABI entry point that launches work (SURVEY.md section 5): visible in nsys / ncu --nvtx, free when no tool is attached
-struct NvtxRange {
-  explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
-  ~NvtxRange() { nvtxRangePop(); }
-};
 #include <dlfcn.h>
 #include <stdarg.h>
 
@@ -31,7 +25,7 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
-static int check_device(int* sms) {
+int check_device(int* sms) {
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) {
@@ -1426,127 +1420,6 @@ static int backward_walk(myolo_plan* pl, std::vector<char>& live, cudaStream_t s
   return rc;
 }
 
-extern "C" int myolo_letterbox(const uint8_t* src, int B, int H0, int W0, int resized_w, int resized_h, int top, int left, int H, int W,
-                               const int32_t* pad_bgr, void* out, int out_dtype, int chw, int swap_rb, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_letterbox(src, B, H0, W0, resized_w, resized_h, top, left, H, W, pad_bgr, out, out_dtype, chw, swap_rb, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_letterbox_items(const uint8_t* src, const myolo_letterbox_item* items, int B, int H, int W, void* out, int out_dtype,
-                                     void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_letterbox_items(src, items, B, H, W, out, out_dtype, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_resize_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_resize_u8(src, H0, W0, dst, H, W, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_resize_area_u8(const uint8_t* src, int H0, int W0, uint8_t* dst, int H, int W, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_resize_area_u8(src, H0, W0, dst, H, W, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_augment_det_hw(const myolo_aug_item* items, int B, int H, int W, void* out, int out_dtype, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_augment_det(items, B, H, W, out, out_dtype, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_resize_bilinear(const void* src, int src_dtype, int B, int C, int H, int W, void* dst, int dst_dtype, int Ho, int Wo,
-                                     void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_resize_bilinear(src, src_dtype, B, C, H, W, dst, dst_dtype, Ho, Wo, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_scale_img(const void* src, int dtype, int B, int C, int H, int W, void* dst, int Ho, int Wo, int Hp, int Wp, int flip_lr,
-                               float pad_value, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_scale_img(src, dtype, B, C, H, W, dst, Ho, Wo, Hp, Wp, flip_lr, pad_value, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_collate_quad(const uint8_t* imgs, int B, int H, int W, const uint8_t* tile, void* out, int out_dtype, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_collate_quad(imgs, B, H, W, tile, out, out_dtype, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_augment_seg(myolo_seg_item* items, int B, int h, int w, int mh, int mw, const int32_t* tables, uint8_t* scratch,
-                                 void* out_img, int out_dtype, int64_t* out_mask, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_augment_seg(items, B, h, w, mh, mw, tables, scratch, out_img, out_dtype, (long long*)out_mask, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_seg_lut_blend(const void* class_map, int map_dtype, int64_t n_pixels, const uint8_t* lut, int n_entries, int channels,
-                                   int reverse_channels, uint8_t* out, const uint8_t* image, float alpha, float beta, uint8_t* blend,
-                                   const uint8_t* lut2, int channels2, uint8_t* out2, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_lut_blend(class_map, map_dtype, (long)n_pixels, lut, n_entries, channels, reverse_channels, out, image, alpha, beta, blend,
-                          lut2, channels2, out2, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_detect_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, int nc, float* xywhn,
-                                  int32_t* class_counts, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_detect_boxes(rows, counts, B, max_det, geom, nc, xywhn, class_counts, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_scale_boxes(float* rows, const int32_t* counts, int B, int max_det, const float* geom, float* xywh, float* xyxyn,
-                                 float* xywhn, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_scale_boxes(rows, counts, B, max_det, geom, xywh, xyxyn, xywhn, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_seg_metrics(const void* pred, int pred_dtype, const int64_t* target, int64_t n_pixels, int n_classes, uint64_t* counters,
-                                 void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_seg_hist(pred, pred_dtype, reinterpret_cast<const long long*>(target), (long)n_pixels, n_classes,
-                         reinterpret_cast<unsigned long long*>(counters), (cudaStream_t)stream);
-}
-
-extern "C" int myolo_det_match(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets, int H, int W,
-                               const float* geom, const float* iouv, int img_base, uint16_t* st_correct, float* st_conf, uint8_t* st_cls,
-                               int32_t* st_rows, uint64_t* tcount, int32_t* err, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_det_match(dets, counts, B, max_det, targets, n_targets, H, W, geom, iouv, img_base, st_correct, st_conf, st_cls, st_rows,
-                          reinterpret_cast<unsigned long long*>(tcount), err, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_confusion_update(const float* dets, const int32_t* counts, int B, int max_det, const float* targets, int n_targets,
-                                      int H, int W, const float* geom, int nc, float conf_thres, float iou_thres, int require_rows,
-                                      int64_t* matrix, int32_t* err, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_confusion(dets, counts, B, max_det, targets, n_targets, H, W, geom, nc, conf_thres, iou_thres, require_rows,
-                          reinterpret_cast<unsigned long long*>(matrix), err, (cudaStream_t)stream);
-}
-
-extern "C" int64_t myolo_det_ap_workspace_bytes(int n_images, int max_det, int ncol) {
-  return det_ap_workspace_bytes(n_images, max_det, ncol);
-}
-
-extern "C" int myolo_det_ap(const uint16_t* correct, const float* conf, const uint8_t* cls, const int32_t* rows, int n_images, int max_det,
-                            int ncol, const uint64_t* tcount, const double* px, const double* x101, double* out_ap, double* out_p,
-                            double* out_r, int32_t* out_info, void* workspace, int64_t workspace_bytes, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_det_ap(correct, conf, cls, rows, n_images, max_det, ncol, reinterpret_cast<const unsigned long long*>(tcount), px, x101,
-                       out_ap, out_p, out_r, out_info, workspace, workspace_bytes, (cudaStream_t)stream);
-}
-
 extern "C" int myolo_conv_backward(const void* x, int x_dtype, int B, int H, int W, int x_ctot, int x_coff, const void* dy, int dy_dtype,
                                    int dy_ctot, int dy_coff, void* gin, int gin_ctot, int gin_coff, const float* w, int co, int ci, int k,
                                    int stride, int dil, float* dW, float* dbias, int route, int32_t* info, void* stream) {
@@ -1597,188 +1470,6 @@ extern "C" int myolo_conv_backward(const void* x, int x_dtype, int B, int H, int
     rc = MYOLO_E_CUDA;
   }
   return rc;
-}
-
-extern "C" int myolo_grads_check_finite(const float* grad, int64_t n, int32_t* found_inf, void* stream) {
-  MYOLO_REQUIRE(grad && found_inf && n > 0, "grads_check_finite: bad arguments");
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_grads_check_finite(grad, (long)n, found_inf, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_sgd_step(float* param, float* grad, float* momentum_buf, const uint8_t* group, int64_t n, const float* lr,
-                              const float* weight_decay, int n_groups, float momentum, int nesterov, const float* inv_scale,
-                              const int32_t* found_inf, int zero_grad, void* stream) {
-  NvtxRange nvtx_("myolo_sgd_step");
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_sgd_step(param, grad, momentum_buf, group, (long)n, lr, weight_decay, n_groups, momentum, nesterov, inv_scale, found_inf,
-                         zero_grad, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_adam_step(float* param, float* grad, float* exp_avg, float* exp_avg_sq, const uint8_t* group, int64_t n, const double* lr,
-                               const float* weight_decay, int n_groups, double beta1, double beta2, double eps, const int32_t* steps,
-                               const float* inv_scale, const int32_t* found_inf, int zero_grad, void* stream) {
-  NvtxRange nvtx_("myolo_adam_step");
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_adam_step(param, grad, exp_avg, exp_avg_sq, group, (long)n, lr, weight_decay, n_groups, beta1, beta2, eps, steps, inv_scale,
-                          found_inf, zero_grad, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_adam_scalars(const int32_t* steps, int64_t n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt,
-                                  double* bc1, double* bc2, void* stream) {
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_adam_scalars(steps, (long)n, lr, beta1, beta2, step_size, bc2_sqrt, bc1, bc2, (cudaStream_t)stream);
-}
-
-extern "C" int64_t myolo_seg_ohem_loss_workspace_bytes(int B, int H, int W) { return (int64_t)ohem_scratch_bytes((long)B * H * W); }
-
-extern "C" int myolo_seg_ohem_loss(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index, float thresh_t,
-                                   float* loss_out, void* workspace, int64_t workspace_bytes, void* stream) {
-  NvtxRange nvtx_("myolo_seg_ohem_loss");
-  MYOLO_REQUIRE(logits && labels && loss_out && workspace && B > 0 && C > 0 && H > 0 && W > 0, "seg_ohem_loss: bad arguments");
-  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_ohem_loss_workspace_bytes(B, H, W), "seg_ohem_loss: workspace too small");
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_seg_ohem_loss(logits, reinterpret_cast<const long long*>(labels), B, C, H, W, ignore_index, thresh_t, workspace, loss_out,
-                              (cudaStream_t)stream);
-}
-
-extern "C" int myolo_seg_ohem_loss_backward(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index,
-                                            const float* grad_out, float* grad_logits, const void* workspace, int64_t workspace_bytes,
-                                            void* stream) {
-  NvtxRange nvtx_("myolo_seg_ohem_loss_backward");
-  MYOLO_REQUIRE(logits && labels && grad_out && grad_logits && workspace && B > 0 && C > 0 && H > 0 && W > 0,
-                "seg_ohem_loss_backward: bad arguments");
-  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_ohem_loss_workspace_bytes(B, H, W), "seg_ohem_loss_backward: workspace too small");
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_seg_ohem_loss_bwd(logits, reinterpret_cast<const long long*>(labels), B, C, H, W, ignore_index, workspace, grad_out,
-                                  grad_logits, (cudaStream_t)stream);
-}
-
-extern "C" int64_t myolo_seg_focal_loss_workspace_bytes(void) { return (int64_t)seg_focal_workspace_bytes(); }
-
-extern "C" int myolo_seg_focal_loss(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index,
-                                    const float* class_weights, float gamma, int reduction, float* loss_out, void* workspace,
-                                    int64_t workspace_bytes, void* stream) {
-  NvtxRange nvtx_("myolo_seg_focal_loss");
-  MYOLO_REQUIRE(logits && labels && loss_out && workspace && B > 0 && C > 0 && H > 0 && W > 0, "seg_focal_loss: bad arguments");
-  MYOLO_REQUIRE(reduction == MYOLO_REDUCTION_MEAN || reduction == MYOLO_REDUCTION_SUM, "seg_focal_loss: reduction must be mean or sum");
-  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_focal_loss_workspace_bytes(), "seg_focal_loss: workspace too small");
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_seg_focal_loss(logits, reinterpret_cast<const long long*>(labels), B, C, H, W, ignore_index, class_weights, gamma,
-                               reduction == MYOLO_REDUCTION_SUM, workspace, loss_out, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_seg_focal_loss_backward(const float* logits, const int64_t* labels, int B, int C, int H, int W, int ignore_index,
-                                             const float* class_weights, float gamma, const float* grad_out, float* grad_logits,
-                                             const void* workspace, int64_t workspace_bytes, void* stream) {
-  NvtxRange nvtx_("myolo_seg_focal_loss_backward");
-  MYOLO_REQUIRE(logits && labels && grad_out && grad_logits && workspace && B > 0 && C > 0 && H > 0 && W > 0,
-                "seg_focal_loss_backward: bad arguments");
-  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_focal_loss_workspace_bytes(), "seg_focal_loss_backward: workspace too small");
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_seg_focal_loss_bwd(logits, reinterpret_cast<const long long*>(labels), B, C, H, W, ignore_index, class_weights, gamma,
-                                   workspace, grad_out, grad_logits, (cudaStream_t)stream);
-}
-
-extern "C" int64_t myolo_anchor_metric_workspace_bytes(void) { return anchor_metric_workspace_bytes(); }
-
-extern "C" int myolo_anchor_metric(const void* wh, int wh_dtype, int64_t n, const void* k, int k_dtype, int na, double thr,
-                                   myolo_anchor_stats* out, void* workspace, int64_t workspace_bytes, void* stream) {
-  NvtxRange nvtx_("myolo_anchor_metric");
-  MYOLO_REQUIRE(wh && k && out && workspace && n > 0 && na >= 1 && na <= MYOLO_ANCHOR_MAX, "anchor_metric: bad arguments");
-  MYOLO_REQUIRE((wh_dtype == MYOLO_F32 || wh_dtype == MYOLO_F64) && (k_dtype == MYOLO_F32 || k_dtype == MYOLO_F64),
-                "anchor_metric: wh and k must be MYOLO_F32 or MYOLO_F64");
-  MYOLO_REQUIRE(workspace_bytes >= anchor_metric_workspace_bytes(), "anchor_metric: workspace too small");
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_anchor_metric(wh, wh_dtype, (long)n, k, k_dtype, na, thr, out, workspace, (cudaStream_t)stream);
-}
-
-extern "C" int64_t myolo_anchor_evolve_workspace_bytes(int64_t n) {
-  int64_t bytes = -1;
-  if (check_device(nullptr) || n <= 0 || anchor_evolve_workspace_bytes((long)n, &bytes)) return -1;
-  return bytes;
-}
-
-extern "C" int myolo_anchor_evolve(const float* wh, int64_t n, const double* k0, int na, const double* v, int gen, double thr,
-                                   double* k_out, float* f_out, float* fg_out, int32_t* accepted_out, void* workspace,
-                                   int64_t workspace_bytes, void* stream) {
-  NvtxRange nvtx_("myolo_anchor_evolve");
-  MYOLO_REQUIRE(wh && k0 && k_out && f_out && accepted_out && workspace && na >= 1 && na <= MYOLO_ANCHOR_MAX && gen >= 0 &&
-                (gen == 0 || (v && fg_out)), "anchor_evolve: bad arguments");
-  // the exact fp64 sum: every term a multiple of 2^-27 in [0, 1] (fp32(thr) >= 1/16) and fewer than 2^26 of them
-  MYOLO_REQUIRE(n >= 1 && n < (int64_t(1) << 26), "anchor_evolve: n = %lld labels, needs 1 <= n < 2^26", (long long)n);
-  const float thr32 = (float)thr;
-  MYOLO_REQUIRE(thr32 >= 0.0625f, "anchor_evolve: 1 / anchor_t = %g, needs anchor_t <= 16", thr);
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_anchor_evolve(wh, (long)n, k0, na, v, gen, thr32, k_out, f_out, fg_out, accepted_out, workspace, workspace_bytes,
-                              (cudaStream_t)stream);
-}
-
-extern "C" int64_t myolo_kmeans_workspace_bytes(int64_t n, int k, int restarts) {
-  if (n < 1 || n >= (int64_t(1) << 30) || k < 1 || restarts < 1) return -1;
-  return kmeans_workspace_bytes((long)n, restarts);
-}
-
-extern "C" int myolo_kmeans(const double* obs, int64_t n, int d, const int64_t* init_idx, int k, int restarts, double thresh, int max_iter,
-                            double* books, int32_t* book_k, double* dists, int32_t* iters, int32_t* best, int32_t* status, void* workspace,
-                            int64_t workspace_bytes, void* stream) {
-  NvtxRange nvtx_("myolo_kmeans");
-  MYOLO_REQUIRE(obs && init_idx && books && book_k && dists && iters && best && status && workspace && restarts >= 1 && max_iter >= 1,
-                "kmeans: bad arguments");
-  MYOLO_REQUIRE(d == 2, "kmeans: d = %d features, only d = 2 is built", d);
-  MYOLO_REQUIRE(k >= 1 && k <= MYOLO_KMEANS_KMAX, "kmeans: k = %d, needs 1 <= k <= %d", k, MYOLO_KMEANS_KMAX);
-  MYOLO_REQUIRE(n >= k && n < (int64_t(1) << 30), "kmeans: n = %lld observations, needs k <= n < 2^30", (long long)n);
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_kmeans(obs, (long)n, init_idx, k, restarts, thresh, max_iter, books, book_k, dists, iters, best, status, workspace,
-                       workspace_bytes, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_class_weights(const float* cls, int64_t n_labels, int nc, int64_t* counts, double* weights, int32_t* status,
-                                   void* stream) {
-  NvtxRange nvtx_("myolo_class_weights");
-  MYOLO_REQUIRE((cls || n_labels == 0) && n_labels >= 0 && counts && weights && status, "class_weights: bad arguments");
-  MYOLO_REQUIRE(nc >= 1 && nc <= MYOLO_IW_NC_MAX, "class_weights: nc = %d, needs 1 <= nc <= %d", nc, MYOLO_IW_NC_MAX);
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_class_weights(cls, (long long)n_labels, nc, reinterpret_cast<unsigned long long*>(counts), weights, status,
-                              (cudaStream_t)stream);
-}
-
-extern "C" int myolo_image_weights(const float* cls, const int64_t* offsets, int64_t n, const double* cw, int nc, double* iw,
-                                   int32_t* status, void* stream) {
-  NvtxRange nvtx_("myolo_image_weights");
-  MYOLO_REQUIRE(cls && offsets && cw && iw && status && n >= 1, "image_weights: bad arguments");
-  MYOLO_REQUIRE(nc >= 1 && nc <= MYOLO_IW_NC_MAX, "image_weights: nc = %d, needs 1 <= nc <= %d", nc, MYOLO_IW_NC_MAX);
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_image_weights(cls, offsets, (long long)n, cw, nc, iw, status, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_weighted_draw(const double* w, const double* u, int64_t n, double* cum, double* total, int32_t* idx, int32_t* status,
-                                   void* stream) {
-  NvtxRange nvtx_("myolo_weighted_draw");
-  MYOLO_REQUIRE(w && u && cum && total && idx && status, "weighted_draw: bad arguments");
-  MYOLO_REQUIRE(n >= 1 && n < (int64_t(1) << 31), "weighted_draw: n = %lld, needs 1 <= n < 2^31", (long long)n);
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_weighted_draw(w, u, (long long)n, cum, total, idx, status, (cudaStream_t)stream);
-}
-
-extern "C" int myolo_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay, void* stream) {
-  NvtxRange nvtx_("myolo_ema_update");
-  int rc = check_device(nullptr);
-  if (rc) return rc;
-  return launch_ema_update(chunks, n_chunks, decay, (cudaStream_t)stream);
 }
 
 // ------------------------------------------------------------------------------------------------

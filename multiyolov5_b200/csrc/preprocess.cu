@@ -47,22 +47,6 @@ __global__ void letterbox_kernel(const LetterboxParams p) {
   }
 }
 
-int launch_letterbox(const unsigned char* src, int B, int H0, int W0, int rw, int rh, int top, int left, int H, int W, const int* pad3,
-                     void* dst, int out_dtype, int chw, int swap_rb, cudaStream_t s) {
-  MYOLO_REQUIRE(src && dst && B > 0 && H0 > 0 && W0 > 0 && rw > 0 && rh > 0 && H >= rh + top && W >= rw + left && top >= 0 && left >= 0,
-                "letterbox: bad geometry (src %dx%d resized %dx%d out %dx%d offset %d,%d)", W0, H0, rw, rh, W, H, left, top);
-  MYOLO_REQUIRE(out_dtype == MYOLO_U8 || out_dtype == MYOLO_F16 || out_dtype == MYOLO_F32, "letterbox: output dtype");
-  LetterboxParams p;
-  p.src = src; p.dst = dst; p.B = B; p.rw = rw; p.rh = rh; p.top = top; p.left = left; p.H = H; p.W = W;
-  p.g = resize_geom(H0, W0, rh, rw);
-  p.out_dtype = out_dtype; p.chw = chw; p.swap_rb = swap_rb;
-  for (int c = 0; c < 3; ++c) p.pad[c] = pad3 ? pad3[c] : 114;
-  const long total = (long)B * H * W;
-  letterbox_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(p);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
 // autoShape's ragged batch (reference models/common.py:655-658): every item letterboxed to one H x W from its own packed RGB source, CHW
 // output, no channel swap.  Float outputs divide by 255 as torch's CPU `x / 255.` does (a true division, not the reciprocal product
 // of the CUDA `img /= 255.0` above); fp16 rounds that fp32 quotient, as CPU half division computes in fp32.
@@ -91,8 +75,32 @@ __global__ void letterbox_items_kernel(const unsigned char* __restrict__ src, co
   }
 }
 
-int launch_letterbox_items(const unsigned char* src, const myolo_letterbox_item* items, int B, int H, int W, void* dst, int out_dtype,
-                           cudaStream_t s) {
+}  // namespace myolo
+
+using namespace myolo;
+
+extern "C" int myolo_letterbox(const uint8_t* src, int B, int H0, int W0, int rw, int rh, int top, int left, int H, int W, const int32_t* pad3,
+                               void* dst, int out_dtype, int chw, int swap_rb, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(src && dst && B > 0 && H0 > 0 && W0 > 0 && rw > 0 && rh > 0 && H >= rh + top && W >= rw + left && top >= 0 && left >= 0,
+                "letterbox: bad geometry (src %dx%d resized %dx%d out %dx%d offset %d,%d)", W0, H0, rw, rh, W, H, left, top);
+  MYOLO_REQUIRE(out_dtype == MYOLO_U8 || out_dtype == MYOLO_F16 || out_dtype == MYOLO_F32, "letterbox: output dtype");
+  LetterboxParams p;
+  p.src = src; p.dst = dst; p.B = B; p.rw = rw; p.rh = rh; p.top = top; p.left = left; p.H = H; p.W = W;
+  p.g = resize_geom(H0, W0, rh, rw);
+  p.out_dtype = out_dtype; p.chw = chw; p.swap_rb = swap_rb;
+  for (int c = 0; c < 3; ++c) p.pad[c] = pad3 ? pad3[c] : 114;
+  const long total = (long)B * H * W;
+  letterbox_kernel<<<(int)std::min<long>(132L * 16, (total + 255) / 256), 256, 0, s>>>(p);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_letterbox_items(const uint8_t* src, const myolo_letterbox_item* items, int B, int H, int W, void* dst, int out_dtype,
+                                     void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   MYOLO_REQUIRE(src && items && dst && B > 0 && H > 0 && W > 0, "letterbox_items: bad arguments (B %d, out %dx%d)", B, W, H);
   MYOLO_REQUIRE(out_dtype == MYOLO_U8 || out_dtype == MYOLO_F16 || out_dtype == MYOLO_F32, "letterbox_items: output dtype");
   const long total = (long)B * H * W;
@@ -100,5 +108,3 @@ int launch_letterbox_items(const unsigned char* src, const myolo_letterbox_item*
   MYOLO_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace myolo

@@ -1443,31 +1443,6 @@ __global__ void seg_focal_nchw_bwd_kernel(const float* __restrict__ x, const lon
   }
 }
 
-size_t seg_focal_workspace_bytes() { return kSegWfHead; }
-
-int launch_seg_focal_loss(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const float* weights,
-                          float gamma, int sum, void* ws, float* loss_out, cudaStream_t s) {
-  MYOLO_REQUIRE(gamma >= 0.f && isfinite(gamma), "seg_focal_loss: gamma must be finite and >= 0, got %g", (double)gamma);
-  const long n = (long)B * H * W;
-  SegWfSt* st = reinterpret_cast<SegWfSt*>(ws);
-  MYOLO_CHECK_CUDA(cudaMemsetAsync(ws, 0, sizeof(SegWfSt), s));
-  seg_focal_nchw_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, labels, B, C, (long)H * W, ignore_index, weights, gamma, st);
-  MYOLO_LAUNCH_CHECK();
-  seg_wf_finalize_kernel<<<1, 1, 0, s>>>(st, gamma, (float)n, sum, loss_out);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
-int launch_seg_focal_loss_bwd(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const float* weights,
-                              float gamma, const void* ws, const float* grad_out, float* dx, cudaStream_t s) {
-  MYOLO_REQUIRE(gamma >= 0.f && isfinite(gamma), "seg_focal_loss_backward: gamma must be finite and >= 0, got %g", (double)gamma);
-  const long n = (long)B * H * W;
-  seg_focal_nchw_bwd_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, labels, B, C, (long)H * W, ignore_index, weights, gamma,
-                                                                 reinterpret_cast<const SegWfSt*>(ws), grad_out, dx);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
 // ---- OhemCELoss over full-resolution NCHW fp32 logits of any class count (the standalone module: utils.loss.OhemCELoss) ----
 __global__ void ohem_ce_nchw_kernel(const float* __restrict__ x, const long long* __restrict__ labels, int B, int C, long HW, int ignore_index,
                                     float* __restrict__ loss) {
@@ -1513,30 +1488,6 @@ __global__ void ohem_ce_nchw_bwd_kernel(const float* __restrict__ x, const long 
     const float inv = 1.0f / s;
     for (int c = 0; c < C; ++c) dp[(size_t)c * HW] = coef * (expf(xp[(size_t)c * HW] - m) * inv - (c == (int)t ? 1.0f : 0.f));
   }
-}
-
-int launch_seg_ohem_loss(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, float thresh_t, void* ws,
-                         float* loss_out, cudaStream_t s) {
-  const long n = (long)B * H * W;
-  OhemScratch oh = ohem_scratch(ws, n);
-  MYOLO_CHECK_CUDA(cudaMemsetAsync(ws, 0, oh.head, s));
-  count_valid_kernel<<<grid_for_t(n, 256, 132 * 8), 256, 0, s>>>(labels, n, ignore_index, C, &oh.st->n_valid);
-  MYOLO_LAUNCH_CHECK();
-  ohem_ce_nchw_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, labels, B, C, (long)H * W, ignore_index, oh.loss);
-  MYOLO_LAUNCH_CHECK();
-  if (int rc = ohem_select(oh.loss, n, &oh.st->n_valid, thresh_t, oh.st, oh.ties, s)) return rc;
-  ohem_finalize_kernel<<<1, 1, 0, s>>>(oh.st, loss_out);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
-int launch_seg_ohem_loss_bwd(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const void* ws,
-                             const float* grad_out, float* dx, cudaStream_t s) {
-  const long n = (long)B * H * W;
-  OhemScratch oh = ohem_scratch(const_cast<void*>(ws), n);
-  ohem_ce_nchw_bwd_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, labels, B, C, (long)H * W, ignore_index, oh.loss, oh.st, grad_out, dx);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
 }
 
 __global__ void detect_raw_bwd_kernel(const float* __restrict__ draw, int na, int no, TensorView dconv) {
@@ -1833,13 +1784,6 @@ __global__ void grads_check_finite_kernel(const float* __restrict__ g, long n, i
   bad = __syncthreads_or(bad);
   if (threadIdx.x == 0 && bad) atomicOr(found_inf, 1);
 }
-int launch_grads_check_finite(const float* g, long n, int* found_inf, cudaStream_t s) {
-  MYOLO_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "grads_check_finite: gradient buffer must be 16-byte aligned");
-  MYOLO_CHECK_CUDA(cudaMemsetAsync(found_inf, 0, sizeof(int), s));
-  grads_check_finite_kernel<<<grid_for_t(std::max<long>(1, n / 4), 256, 132 * 8), 256, 0, s>>>(g, n, found_inf);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
 
 struct SgdGroups { float lr[4]; float wd[4]; };
 __global__ void sgd_step_kernel(float* __restrict__ p, float* __restrict__ g, float* __restrict__ buf, const unsigned char* __restrict__ group,
@@ -1858,15 +1802,6 @@ __global__ void sgd_step_kernel(float* __restrict__ p, float* __restrict__ g, fl
     }
     if (zero_grad) g[i] = 0.f;
   }
-}
-int launch_sgd_step(float* p, float* g, float* buf, const unsigned char* group, long n, const float* lr, const float* wd, int n_groups,
-                    float momentum, int nesterov, const float* inv_scale, const int* found_inf, int zero_grad, cudaStream_t s) {
-  MYOLO_REQUIRE(p && g && buf && group && n > 0 && n_groups >= 1 && n_groups <= 4, "sgd_step: bad arguments");
-  SgdGroups gr{};
-  for (int i = 0; i < n_groups; ++i) { gr.lr[i] = lr[i]; gr.wd[i] = wd[i]; }
-  sgd_step_kernel<<<grid_for_t(n, 256, 132 * 8), 256, 0, s>>>(p, g, buf, group, n, gr, momentum, nesterov, inv_scale, found_inf, zero_grad);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1966,23 +1901,6 @@ __global__ void adam_step_kernel(float* __restrict__ p, float* __restrict__ g, f
   }
 }
 
-int launch_adam_step(float* p, float* g, float* m, float* v, const unsigned char* group, long n, const double* lr, const float* wd,
-                     int n_groups, double beta1, double beta2, double eps, const int* steps, const float* inv_scale, const int* found_inf,
-                     int zero_grad, cudaStream_t s) {
-  MYOLO_REQUIRE(p && g && m && v && group && steps && n > 0 && n_groups >= 1 && n_groups <= 4, "adam_step: bad arguments");
-  MYOLO_REQUIRE(((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
-                  reinterpret_cast<uintptr_t>(v)) & 15) == 0 && (reinterpret_cast<uintptr_t>(group) & 3) == 0,
-                "adam_step: buffers must be 16-byte aligned (group: 4-byte)");
-  AdamGroups gr{};
-  for (int i = 0; i < n_groups; ++i) { gr.lr[i] = lr[i]; gr.wd[i] = wd[i]; }
-  // torch's scalars: 1 - beta1 (lerp weight), beta2, 1 - beta2 and eps, each Python double rounded to fp32
-  adam_step_kernel<<<grid_for_t(std::max<long>(1, n / 4), 256, 132 * 8), 256, 0, s>>>(
-      p, g, m, v, group, n, gr, n_groups, beta1, beta2, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps, steps,
-      inv_scale, found_inf, zero_grad);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
-}
-
 __global__ void adam_scalars_kernel(const int* steps, long n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt,
                                     double* bc1, double* bc2) {
   for (long i = blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
@@ -1992,13 +1910,6 @@ __global__ void adam_scalars_kernel(const int* steps, long n, double lr, double 
     bc1[i] = bias_correction(beta1, steps[i]);
     bc2[i] = bias_correction(beta2, steps[i]);
   }
-}
-int launch_adam_scalars(const int* steps, long n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt, double* bc1,
-                        double* bc2, cudaStream_t s) {
-  MYOLO_REQUIRE(steps && step_size && bc2_sqrt && bc1 && bc2 && n > 0, "adam_scalars: bad arguments");
-  adam_scalars_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(steps, n, lr, beta1, beta2, step_size, bc2_sqrt, bc1, bc2);
-  MYOLO_LAUNCH_CHECK();
-  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2056,7 +1967,145 @@ __global__ void __launch_bounds__(256) ema_update_kernel(const myolo_ema_chunk* 
   }
 }
 
-int launch_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay, cudaStream_t s) {
+}  // namespace myolo
+
+using namespace myolo;
+
+extern "C" int64_t myolo_seg_focal_loss_workspace_bytes(void) { return (int64_t)kSegWfHead; }
+
+extern "C" int myolo_seg_focal_loss(const float* x, const int64_t* labels, int B, int C, int H, int W, int ignore_index, const float* weights,
+                                    float gamma, int reduction, float* loss_out, void* ws, int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_seg_focal_loss");
+  MYOLO_REQUIRE(x && labels && loss_out && ws && B > 0 && C > 0 && H > 0 && W > 0, "seg_focal_loss: bad arguments");
+  MYOLO_REQUIRE(reduction == MYOLO_REDUCTION_MEAN || reduction == MYOLO_REDUCTION_SUM, "seg_focal_loss: reduction must be mean or sum");
+  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_focal_loss_workspace_bytes(), "seg_focal_loss: workspace too small");
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(gamma >= 0.f && isfinite(gamma), "seg_focal_loss: gamma must be finite and >= 0, got %g", (double)gamma);
+  const long n = (long)B * H * W;
+  SegWfSt* st = reinterpret_cast<SegWfSt*>(ws);
+  MYOLO_CHECK_CUDA(cudaMemsetAsync(ws, 0, sizeof(SegWfSt), s));
+  seg_focal_nchw_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, reinterpret_cast<const long long*>(labels), B, C, (long)H * W, ignore_index, weights,
+                                                             gamma, st);
+  MYOLO_LAUNCH_CHECK();
+  seg_wf_finalize_kernel<<<1, 1, 0, s>>>(st, gamma, (float)n, reduction == MYOLO_REDUCTION_SUM, loss_out);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_seg_focal_loss_backward(const float* x, const int64_t* labels, int B, int C, int H, int W, int ignore_index,
+                                             const float* weights, float gamma, const float* grad_out, float* dx, const void* ws,
+                                             int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_seg_focal_loss_backward");
+  MYOLO_REQUIRE(x && labels && grad_out && dx && ws && B > 0 && C > 0 && H > 0 && W > 0, "seg_focal_loss_backward: bad arguments");
+  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_focal_loss_workspace_bytes(), "seg_focal_loss_backward: workspace too small");
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(gamma >= 0.f && isfinite(gamma), "seg_focal_loss_backward: gamma must be finite and >= 0, got %g", (double)gamma);
+  const long n = (long)B * H * W;
+  seg_focal_nchw_bwd_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, reinterpret_cast<const long long*>(labels), B, C, (long)H * W, ignore_index,
+                                                                 weights, gamma, reinterpret_cast<const SegWfSt*>(ws), grad_out, dx);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int64_t myolo_seg_ohem_loss_workspace_bytes(int B, int H, int W) { return (int64_t)ohem_scratch_bytes((long)B * H * W); }
+
+extern "C" int myolo_seg_ohem_loss(const float* x, const int64_t* labels, int B, int C, int H, int W, int ignore_index, float thresh_t,
+                                   float* loss_out, void* ws, int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_seg_ohem_loss");
+  MYOLO_REQUIRE(x && labels && loss_out && ws && B > 0 && C > 0 && H > 0 && W > 0, "seg_ohem_loss: bad arguments");
+  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_ohem_loss_workspace_bytes(B, H, W), "seg_ohem_loss: workspace too small");
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  const long n = (long)B * H * W;
+  OhemScratch oh = ohem_scratch(ws, n);
+  MYOLO_CHECK_CUDA(cudaMemsetAsync(ws, 0, oh.head, s));
+  count_valid_kernel<<<grid_for_t(n, 256, 132 * 8), 256, 0, s>>>(reinterpret_cast<const long long*>(labels), n, ignore_index, C,
+                                                                  &oh.st->n_valid);
+  MYOLO_LAUNCH_CHECK();
+  ohem_ce_nchw_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, reinterpret_cast<const long long*>(labels), B, C, (long)H * W, ignore_index,
+                                                          oh.loss);
+  MYOLO_LAUNCH_CHECK();
+  if (int rc = ohem_select(oh.loss, n, &oh.st->n_valid, thresh_t, oh.st, oh.ties, s)) return rc;
+  ohem_finalize_kernel<<<1, 1, 0, s>>>(oh.st, loss_out);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_seg_ohem_loss_backward(const float* x, const int64_t* labels, int B, int C, int H, int W, int ignore_index,
+                                            const float* grad_out, float* dx, const void* ws, int64_t workspace_bytes, void* stream) {
+  NvtxRange nvtx_("myolo_seg_ohem_loss_backward");
+  MYOLO_REQUIRE(x && labels && grad_out && dx && ws && B > 0 && C > 0 && H > 0 && W > 0, "seg_ohem_loss_backward: bad arguments");
+  MYOLO_REQUIRE(workspace_bytes >= myolo_seg_ohem_loss_workspace_bytes(B, H, W), "seg_ohem_loss_backward: workspace too small");
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  const long n = (long)B * H * W;
+  OhemScratch oh = ohem_scratch(const_cast<void*>(ws), n);
+  ohem_ce_nchw_bwd_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(x, reinterpret_cast<const long long*>(labels), B, C, (long)H * W, ignore_index,
+                                                              oh.loss, oh.st, grad_out, dx);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_grads_check_finite(const float* g, int64_t n, int32_t* found_inf, void* stream) {
+  MYOLO_REQUIRE(g && found_inf && n > 0, "grads_check_finite: bad arguments");
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE((reinterpret_cast<uintptr_t>(g) & 15) == 0, "grads_check_finite: gradient buffer must be 16-byte aligned");
+  MYOLO_CHECK_CUDA(cudaMemsetAsync(found_inf, 0, sizeof(int), s));
+  grads_check_finite_kernel<<<grid_for_t(std::max<long>(1, n / 4), 256, 132 * 8), 256, 0, s>>>(g, n, found_inf);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_sgd_step(float* p, float* g, float* buf, const uint8_t* group, int64_t n, const float* lr, const float* wd, int n_groups,
+                              float momentum, int nesterov, const float* inv_scale, const int32_t* found_inf, int zero_grad, void* stream) {
+  NvtxRange nvtx_("myolo_sgd_step");
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(p && g && buf && group && n > 0 && n_groups >= 1 && n_groups <= 4, "sgd_step: bad arguments");
+  SgdGroups gr{};
+  for (int i = 0; i < n_groups; ++i) { gr.lr[i] = lr[i]; gr.wd[i] = wd[i]; }
+  sgd_step_kernel<<<grid_for_t(n, 256, 132 * 8), 256, 0, s>>>(p, g, buf, group, n, gr, momentum, nesterov, inv_scale, found_inf, zero_grad);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_adam_step(float* p, float* g, float* m, float* v, const uint8_t* group, int64_t n, const double* lr, const float* wd,
+                               int n_groups, double beta1, double beta2, double eps, const int32_t* steps, const float* inv_scale,
+                               const int32_t* found_inf, int zero_grad, void* stream) {
+  NvtxRange nvtx_("myolo_adam_step");
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(p && g && m && v && group && steps && n > 0 && n_groups >= 1 && n_groups <= 4, "adam_step: bad arguments");
+  MYOLO_REQUIRE(((reinterpret_cast<uintptr_t>(p) | reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(m) |
+                  reinterpret_cast<uintptr_t>(v)) & 15) == 0 && (reinterpret_cast<uintptr_t>(group) & 3) == 0,
+                "adam_step: buffers must be 16-byte aligned (group: 4-byte)");
+  AdamGroups gr{};
+  for (int i = 0; i < n_groups; ++i) { gr.lr[i] = lr[i]; gr.wd[i] = wd[i]; }
+  // torch's scalars: 1 - beta1 (lerp weight), beta2, 1 - beta2 and eps, each Python double rounded to fp32
+  adam_step_kernel<<<grid_for_t(std::max<long>(1, n / 4), 256, 132 * 8), 256, 0, s>>>(
+      p, g, m, v, group, n, gr, n_groups, beta1, beta2, (float)(1.0 - beta1), (float)beta2, (float)(1.0 - beta2), (float)eps, steps,
+      inv_scale, found_inf, zero_grad);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_adam_scalars(const int32_t* steps, int64_t n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt,
+                                  double* bc1, double* bc2, void* stream) {
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
+  MYOLO_REQUIRE(steps && step_size && bc2_sqrt && bc1 && bc2 && n > 0, "adam_scalars: bad arguments");
+  adam_scalars_kernel<<<grid_for_t(n, 256), 256, 0, s>>>(steps, n, lr, beta1, beta2, step_size, bc2_sqrt, bc1, bc2);
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int myolo_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay, void* stream) {
+  NvtxRange nvtx_("myolo_ema_update");
+  if (int rc = check_device(nullptr)) return rc;
+  const cudaStream_t s = (cudaStream_t)stream;
   MYOLO_REQUIRE(chunks && n_chunks > 0, "ema_update: empty chunk table");
   MYOLO_REQUIRE(decay >= 0.0 && decay <= 1.0, "ema_update: decay %g outside [0, 1]", decay);
   MYOLO_REQUIRE((reinterpret_cast<uintptr_t>(chunks) & 7) == 0, "ema_update: chunk table must be 8-byte aligned");
@@ -2065,5 +2114,3 @@ int launch_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay,
   MYOLO_LAUNCH_CHECK();
   return 0;
 }
-
-}  // namespace myolo

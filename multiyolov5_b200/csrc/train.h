@@ -86,25 +86,12 @@ size_t ohem_scratch_bytes(long n_pixels);
 int launch_seg_ce_fused(const TensorView& lo, int n_cls, const long long* labels, int H, int W, int ignore_index, const TensorView& dlo,
                         float factor, const float* scale_dev, void* scratch16, float* gbuf, float* loss_out, cudaStream_t s,
                         void* ohem_ws = nullptr, float thresh_t = 0.f);
-// OhemCELoss over full-resolution (B,C,H,W) fp32 logits: the forward leaves its selection in ws (ohem_scratch_bytes(B*H*W) bytes), the
-// backward reads it and writes dx = *grad_out * d(loss)/dx
-int launch_seg_ohem_loss(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, float thresh_t, void* ws,
-                         float* loss_out, cudaStream_t s);
-int launch_seg_ohem_loss_bwd(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const void* ws,
-                             const float* grad_out, float* dx, cudaStream_t s);
 // the same fused pass with the class-weighted CE / focal loss (weights: n_cls device floats, nullable; gamma = 0 is the weighted CE) in
 // place of the mean CE, reduction 'mean'; wf_ws: seg_wf_scratch_bytes(B*H*W) bytes (the loss's sums and coefficients, 8 bytes per pixel)
 size_t seg_wf_scratch_bytes(long n_pixels);
 int launch_seg_wf_fused(const TensorView& lo, int n_cls, const long long* labels, int H, int W, int ignore_index, const TensorView& dlo,
                         float factor, const float* scale_dev, float* gbuf, void* wf_ws, const float* weights, float gamma, float* loss_out,
                         cudaStream_t s);
-// SegFocalLoss over full-resolution (B,C,H,W) fp32 logits (sum = 0: 'mean', 1: 'sum'): the forward leaves its coefficients in ws
-// (seg_focal_workspace_bytes()), the backward reads them and writes dx = *grad_out * d(loss)/dx
-size_t seg_focal_workspace_bytes();
-int launch_seg_focal_loss(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const float* weights,
-                          float gamma, int sum, void* ws, float* loss_out, cudaStream_t s);
-int launch_seg_focal_loss_bwd(const float* x, const long long* labels, int B, int C, int H, int W, int ignore_index, const float* weights,
-                              float gamma, const void* ws, const float* grad_out, float* dx, cudaStream_t s);
 // Detect: d(conv out fp32 NHWC)[b,y,x,a*no+o] = draw[b,a,y,x,o]
 int launch_detect_raw_bwd(const float* draw, int na, int no, const TensorView& dconv, cudaStream_t s);
 int launch_cast_f32_to_f16(const TensorView& src, const TensorView& dst, cudaStream_t s);
@@ -113,16 +100,6 @@ int launch_cast_f16_to_f32_acc(const TensorView& src, const TensorView& dst, cud
 int launch_conv_wgrad(const TensorView& x, const TensorView& dy, int k, int stride, int dil, float* dW, int co, int ci, float* dbias,
                       cudaStream_t s);
 int launch_bias_grad(const TensorView& dy, float* dbias, int co, cudaStream_t s);                     // dbias[co] += sum_p dy (fp32 or fp16 view)
-// optimiser over the flat parameter / gradient buffers (see train.cu)
-int launch_grads_check_finite(const float* g, long n, int* found_inf, cudaStream_t s);
-int launch_sgd_step(float* p, float* g, float* buf, const unsigned char* group, long n, const float* lr, const float* wd, int n_groups,
-                    float momentum, int nesterov, const float* inv_scale, const int* found_inf, int zero_grad, cudaStream_t s);
-int launch_adam_step(float* p, float* g, float* m, float* v, const unsigned char* group, long n, const double* lr, const float* wd,
-                     int n_groups, double beta1, double beta2, double eps, const int* steps, const float* inv_scale, const int* found_inf,
-                     int zero_grad, cudaStream_t s);
-int launch_adam_scalars(const int* steps, long n, double lr, double beta1, double beta2, float* step_size, float* bc2_sqrt, double* bc1,
-                        double* bc2, cudaStream_t s);
-int launch_ema_update(const myolo_ema_chunk* chunks, int n_chunks, double decay, cudaStream_t s);
 // wgmma weight gradient (wgrad_tc.cu): dw_packed is a zeroed fp32 [co][k*k][ci] accumulation buffer owned by the caller
 bool conv_wgrad_tc_eligible(const TensorView& x, const TensorView& dy, int k, int stride, int dil, int co, int ci);
 size_t conv_wgrad_packed_bytes(const float* dW, int co, int ci, int k);   // 0: accumulates straight into dW
