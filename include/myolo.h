@@ -148,6 +148,16 @@ int myolo_plan_forward(myolo_plan* plan, const void* x, int x_dtype, float* z, f
  * calls captures nothing again.  MYOLO_E_INVALID when the rows do not fit, z_inv_scale is not positive and finite or z_flip_w < 0. */
 int myolo_plan_forward_pass(myolo_plan* plan, const void* x, int x_dtype, float* z, int z_rows_total, int z_row_offset, float z_inv_scale,
                             int z_flip_w, void* seg, int seg_dtype, int64_t* seg_argmax, void* stream);
+/* The seg output of a model ensemble (models.experimental.Ensemble) over plans[0..K) of K <= MYOLO_ENSEMBLE_MAX members, after each
+ * plan's latest forward on the same input (myolo_plan_forward_pass with seg = seg_argmax = NULL leaves its low-res logits in its
+ * workspace).  Per output pixel and class: each member's x8 upsampled logit as its own forward would store it in seg_dtype, the fp32
+ * mean of those K values as torch's CUDA `torch.stack(maps).mean(0)` computes it (its per-thread partial sums, and the member groups it
+ * reduces separately when the stacked maps exceed 32-bit byte offsets), then seg (B,n_segcls,H,W) of seg_dtype (nullable)
+ * and/or seg_argmax (B,H,W) int64, the argmax of the fp32 mean, first maximum wins (nullable, not both null).  The plans must share
+ * B, H, W, n_segcls and the low-res size.  MYOLO_E_INVALID when they do not, or when K members' staged source rows exceed the device's
+ * shared memory per block. */
+#define MYOLO_ENSEMBLE_MAX 8
+int myolo_seg_ensemble(myolo_plan* const* plans, int K, void* seg, int seg_dtype, int64_t* seg_argmax, void* stream);
 /* debugging / per-layer parity: copies the NHWC buffer slice of a view into dst as (B,C,H,W) fp32 */
 int myolo_plan_read_view(myolo_plan* plan, myolo_view view, float* dst_nchw, void* stream);
 /* number of kernels the last myolo_plan_forward launched (bench.py's gpu_launches) */

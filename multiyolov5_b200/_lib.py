@@ -43,13 +43,14 @@ EXPORTS = [
     "myolo_plan_backward_seg_loss", "myolo_seg_focal_loss", "myolo_seg_focal_loss_backward", "myolo_seg_focal_loss_workspace_bytes",
     "myolo_conv_backward", "myolo_conv_forward", "myolo_plan_forward_pass", "myolo_scale_img", "myolo_detect_boxes",
     "myolo_letterbox_items", "myolo_scale_boxes", "myolo_seg_crop_upsample_argmax", "myolo_nms_labels", "myolo_nms_labels_workspace_bytes",
-    "myolo_confusion_update",
+    "myolo_confusion_update", "myolo_seg_ensemble",
 ]
 REDUCTION_MEAN, REDUCTION_SUM = 0, 1        # include/myolo.h: MYOLO_REDUCTION_* of myolo_seg_focal_loss
 DET_ERR_TARGET_CLASS, DET_ERR_PRED_CLASS, DET_ERR_LABELS = 1, 2, 4     # include/myolo.h: bits of myolo_det_match's error word
 NMS_ERR_LABEL_CLASS, NMS_ERR_LABEL_COUNT = 1, 2                          # include/myolo.h: bits of myolo_nms_labels' error word
 KMEANS_MAX_ITER, KMEANS_BAD_INDEX = 1, 2                                 # include/myolo.h: bits of myolo_kmeans' status word
 IW_BAD_CLASS, IW_TOTAL_NONPOS, IW_TOTAL_NONFINITE = 1, 2, 4              # include/myolo.h: bits of the image-weights status word
+ENSEMBLE_MAX = 8                                                         # include/myolo.h MYOLO_ENSEMBLE_MAX
 IW_NC_MAX = 1024                                                         # include/myolo.h MYOLO_IW_NC_MAX
 DET_LOSS_NA_MAX = 10                                                     # include/myolo.h MYOLO_DET_LOSS_NA_MAX
 CONV_BWD_SIMT, CONV_BWD_NO_WGRAD_TC = 1, 2                               # include/myolo.h: route bits of myolo_conv_backward
@@ -123,6 +124,7 @@ def lib():
     L.myolo_plan_repack_weights.argtypes = [vp, vp]
     L.myolo_plan_forward.argtypes = [vp, vp, i32, vp, C.POINTER(vp), vp, i32, vp, vp]
     L.myolo_plan_forward_pass.argtypes = [vp, vp, i32, vp, i32, i32, f32, i32, vp, i32, vp, vp]
+    L.myolo_seg_ensemble.argtypes = [C.POINTER(vp), i32, vp, i32, vp, vp]
     L.myolo_plan_read_view.argtypes = [vp, View, vp, vp]
     L.myolo_plan_last_launch_count.argtypes = [vp]
     L.myolo_plan_last_launch_count.restype = i64

@@ -672,6 +672,184 @@ int launch_seg_upsample(const TensorView& in, int n_cls, int H, int W, void* seg
 }
 
 // ------------------------------------------------------------------------------------------------
+// ensemble seg (models.experimental.Ensemble): the mean over K members of their x8 upsampled logits, without any full-size
+// per-member map.  Same CTA layout as seg_upsample_kernel, with the K members' vertically blended rows staged side by side.  Every
+// member value is seg_upsample_kernel's value rounded to TOut (what that member's own forward would store); the sum is torch's CUDA
+// mean over dim 0 of the stacked fp32 maps (ATen Reduce.cuh).  One reduction launch adds its members with four partial sums from 0
+// (member k into partial k % 4) combined in order.  When the stacked maps exceed 32-bit byte offsets, torch splits the member axis into
+// halves (TensorIterator::with_32bit_indexing) until each part fits, reduces the parts in order and adds each part's sum to the output;
+// `group_end` holds those parts.  The total is multiplied by factor.
+// ------------------------------------------------------------------------------------------------
+struct EnsembleViews {
+  TensorView v[MYOLO_ENSEMBLE_MAX];
+  int group_end[MYOLO_ENSEMBLE_MAX];   // member k belongs to the first group g with k < group_end[g]
+  int n_groups;
+};
+
+// The member groups of torch's reduction over K stacked maps of n_out fp32 elements each: SplitUntil32Bit halves the member axis (the
+// operand dimension of the largest byte extent, the first half floor(K / 2) members) while a part's byte offsets do not fit in int32.
+static void torch_mean_groups(int lo, int hi, int64_t n_out, EnsembleViews* v) {
+  const int64_t k = hi - lo, imax = 2147483647LL;
+  const bool fits = n_out * k <= imax && 4 * n_out * k - 3 <= imax;      // TensorIteratorBase::can_use_32bit_indexing of the input
+  if (fits || k == 1) {
+    v->group_end[v->n_groups++] = hi;
+    return;
+  }
+  torch_mean_groups(lo, lo + (int)(k / 2), n_out, v);
+  torch_mean_groups(lo + (int)(k / 2), hi, n_out, v);
+}
+
+template <typename TOut, int PPT, bool AMAX>
+__global__ void __launch_bounds__(256) seg_ensemble_kernel(const __grid_constant__ EnsembleViews ins, int K, int ncls, int H, int W,
+                                                           float factor, TOut* seg, int64_t* amax) {
+  extern __shared__ float sup_smem[];
+  const TensorView& in0 = ins.v[0];
+  const int segs = (W + PPT * blockDim.x - 1) / (PPT * blockDim.x);
+  const int sx = blockIdx.x % segs;
+  const int y = (blockIdx.x / segs) % H;
+  const int b = blockIdx.x / (segs * H);
+  const int xbeg = sx * PPT * blockDim.x;
+  const int xend = min(W, xbeg + PPT * (int)blockDim.x);
+  const Lerp ly = lerp_axis(y, in0.H, H);
+  const int c0 = lerp_axis(xbeg, in0.W, W).i0;
+  const int c1 = lerp_axis(xend - 1, in0.W, W).i1;
+  const int ncol = c1 - c0 + 1;
+  const int pitch = ncol | 1;
+  const int c4n = (ncls + 3) / 4;
+  for (int k = 0; k < K; ++k) {                    // [K][ncls][pitch]
+    const TensorView& in = ins.v[k];
+    float* sv = sup_smem + (size_t)k * ncls * pitch;
+    for (int i = threadIdx.x; i < ncol * c4n; i += blockDim.x) {
+      const int col = i / c4n, c4 = i - col * c4n;
+      const float4 t = __ldg(reinterpret_cast<const float4*>(vptr_f(in, b, ly.i0, c0 + col)) + c4);
+      const float4 u = __ldg(reinterpret_cast<const float4*>(vptr_f(in, b, ly.i1, c0 + col)) + c4);
+      const float vv[4] = {fmaf(ly.l1, u.x, ly.l0 * t.x), fmaf(ly.l1, u.y, ly.l0 * t.y), fmaf(ly.l1, u.z, ly.l0 * t.z),
+                           fmaf(ly.l1, u.w, ly.l0 * t.w)};
+      float* d = sv + col;
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (c4 * 4 + j < ncls) d[(c4 * 4 + j) * pitch] = vv[j];
+    }
+  }
+  __syncthreads();
+  const int x0 = xbeg + PPT * threadIdx.x;
+  if (x0 >= W) return;
+  int i0[PPT], i1[PPT];
+  float l0[PPT], l1[PPT];
+#pragma unroll
+  for (int j = 0; j < PPT; ++j) {
+    const Lerp lx = lerp_axis(min(x0 + j, W - 1), in0.W, W);
+    i0[j] = lx.i0 - c0; i1[j] = lx.i1 - c0; l0[j] = lx.l0; l1[j] = lx.l1;
+  }
+  float best[PPT];
+  int bi[PPT];
+#pragma unroll
+  for (int j = 0; j < PPT; ++j) { best[j] = 0.f; bi[j] = 0; }
+  const bool full = (x0 + PPT - 1 < W) && (W % PPT == 0);
+  for (int c = 0; c < ncls; ++c) {
+    float v[PPT];
+    for (int g = 0, k = 0; g < ins.n_groups; ++g) {
+      float acc[PPT][4];
+#pragma unroll
+      for (int j = 0; j < PPT; ++j)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) acc[j][q] = 0.f;
+      for (int q = 0; k < ins.group_end[g]; ++k, q = (q + 1) & 3) {
+        const float* r = sup_smem + ((size_t)k * ncls + c) * pitch;
+#pragma unroll
+        for (int j = 0; j < PPT; ++j) {
+          const float t = fmaf(l1[j], r[i1[j]], l0[j] * r[i0[j]]);
+#pragma unroll
+          for (int qq = 0; qq < 4; ++qq)          // register-indexed: the partial sums stay in registers
+            if (qq == q) acc[j][qq] += (float)(TOut)t;
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < PPT; ++j) {
+        const float part = ((acc[j][0] + acc[j][1]) + acc[j][2]) + acc[j][3];
+        v[j] = g == 0 ? part : v[j] + part;     // a later group accumulates into the output of the earlier ones
+      }
+    }
+#pragma unroll
+    for (int j = 0; j < PPT; ++j) {
+      v[j] *= factor;
+      if (AMAX && (c == 0 || v[j] > best[j])) { best[j] = v[j]; bi[j] = c; }
+    }
+    if (seg) {
+      TOut* o = seg + (((size_t)b * ncls + c) * H + y) * W + x0;
+      if (full) {
+        if (PPT == 8) Pack8<TOut>::store(o, v);
+        else Pack4<TOut>::store(o, v[0], v[1], v[2], v[3]);
+      } else {
+        for (int j = 0; j < PPT && x0 + j < W; ++j) o[j] = (TOut)v[j];
+      }
+    }
+  }
+  if (AMAX) {
+    int64_t* o = amax + ((size_t)b * H + y) * W + x0;
+    for (int j = 0; j < PPT && x0 + j < W; ++j) o[j] = bi[j];
+  }
+}
+
+template <typename TOut, int PPT, bool AMAX>
+static int launch_seg_ensemble_k(const EnsembleViews& ins, int K, int n_cls, int H, int W, float factor, TOut* seg, int64_t* argmax,
+                                 size_t smem, int threads, cudaStream_t s) {
+  auto kern = seg_ensemble_kernel<TOut, PPT, AMAX>;
+  static thread_local int opted[64] = {};          // per device: the dynamic shared memory this instance was last allowed
+  int dev = 0;
+  MYOLO_CHECK_CUDA(cudaGetDevice(&dev));
+  if (smem > 48 * 1024 && (dev >= 64 || opted[dev] < (int)smem)) {
+    MYOLO_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (dev < 64) opted[dev] = (int)smem;
+  }
+  const long blocks = (long)ins.v[0].B * H * ceil_div(W, PPT * threads);
+  kern<<<(unsigned)blocks, threads, smem, s>>>(ins, K, n_cls, H, W, factor, seg, argmax);
+  return 0;
+}
+
+template <typename TOut>
+static int launch_seg_ensemble_t(const EnsembleViews& ins, int K, int n_cls, int H, int W, float factor, TOut* seg, int64_t* argmax,
+                                 size_t smem, cudaStream_t s) {
+  const bool wide = (W % 8 == 0) && W >= 256 && (reinterpret_cast<uintptr_t>(seg) & 15) == 0;
+  if (wide) {
+    const int threads = W >= 1024 ? 128 : (W >= 512 ? 64 : 32);
+    return argmax ? launch_seg_ensemble_k<TOut, 8, true>(ins, K, n_cls, H, W, factor, seg, argmax, smem, threads, s)
+                  : launch_seg_ensemble_k<TOut, 8, false>(ins, K, n_cls, H, W, factor, seg, argmax, smem, threads, s);
+  }
+  const int threads = W >= 1024 ? 256 : (W >= 512 ? 128 : 64);
+  return argmax ? launch_seg_ensemble_k<TOut, 4, true>(ins, K, n_cls, H, W, factor, seg, argmax, smem, threads, s)
+                : launch_seg_ensemble_k<TOut, 4, false>(ins, K, n_cls, H, W, factor, seg, argmax, smem, threads, s);
+}
+
+int launch_seg_ensemble(const TensorView* ins, int K, int n_cls, int H, int W, void* seg, int seg_dtype, int64_t* argmax, cudaStream_t s) {
+  MYOLO_REQUIRE(K >= 1 && K <= MYOLO_ENSEMBLE_MAX, "seg_ensemble: %d members (1..%d)", K, MYOLO_ENSEMBLE_MAX);
+  EnsembleViews v{};
+  for (int k = 0; k < K; ++k) {
+    const TensorView& in = ins[k];
+    MYOLO_REQUIRE(in.dtype == MYOLO_F32 && in.ctot % 4 == 0 && in.ctot >= ((n_cls + 3) / 4) * 4, "seg_ensemble: bad view of member %d", k);
+    MYOLO_REQUIRE(in.B == ins[0].B && in.H == ins[0].H && in.W == ins[0].W,
+                  "seg_ensemble: member %d's low-res logits are %dx%dx%d, member 0's %dx%dx%d", k, in.B, in.H, in.W, ins[0].B, ins[0].H,
+                  ins[0].W);
+    v.v[k] = in;
+  }
+  int dev = 0, optin = 0;
+  MYOLO_CHECK_CUDA(cudaGetDevice(&dev));
+  MYOLO_CHECK_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  const size_t smem = (size_t)K * n_cls * ((ins[0].W + 2) | 1) * 4;     // seg_upsample's per-member bound, K times
+  MYOLO_REQUIRE(smem <= (size_t)optin, "seg_ensemble: %d members x %d classes x %d source columns need %zu bytes of shared memory, the "
+                "device allows %d per block", K, n_cls, ins[0].W, smem, optin);
+  // torch's CUDA mean: sum * (float(outputs) / inputs), the sum over the member groups of its 32-bit split
+  const int64_t nout = (int64_t)ins[0].B * n_cls * H * W;
+  const float factor = static_cast<float>(nout) / (nout * K);
+  torch_mean_groups(0, K, nout, &v);
+  int rc = seg_dtype == MYOLO_F16 ? launch_seg_ensemble_t<__half>(v, K, n_cls, H, W, factor, (__half*)seg, argmax, smem, s)
+                                  : launch_seg_ensemble_t<float>(v, K, n_cls, H, W, factor, (float*)seg, argmax, smem, s);
+  if (rc) return rc;
+  MYOLO_LAUNCH_CHECK();
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // standalone post-process entry points on NCHW logits (detect.py:191-193)
 // ------------------------------------------------------------------------------------------------
 template <typename TIn, typename TOut>

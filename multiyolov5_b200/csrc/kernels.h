@@ -27,6 +27,8 @@ int launch_detect_decode(const TensorView& in, int na, int no, float stride, con
 // final bilinear(align_corners) of the seg head: in = fp32 NHWC low-res logits; seg NCHW (fp32/fp16, nullable); argmax nullable
 int launch_seg_upsample(const TensorView& in, int n_cls, int H, int W, void* seg, int seg_dtype, int64_t* argmax,
                         cudaStream_t s);
+// the ensemble's seg (myolo_seg_ensemble): ins[0..K) = the members' fp32 NHWC low-res logits (same extents)
+int launch_seg_ensemble(const TensorView* ins, int K, int n_cls, int H, int W, void* seg, int seg_dtype, int64_t* argmax, cudaStream_t s);
 int launch_read_view(const TensorView& v, float* dst_nchw, cudaStream_t s);
 
 }  // namespace myolo

@@ -775,6 +775,34 @@ extern "C" int myolo_plan_forward_pass(myolo_plan* pl, const void* x, int x_dtyp
   return rc;
 }
 
+// The low-res logits stay valid after a forward: the planner keeps whatever the external ops read live to the end of the plan, and an
+// inference plan owns its workspace, so another member's launches never write there.
+extern "C" int myolo_seg_ensemble(myolo_plan* const* plans, int K, void* seg, int seg_dtype, int64_t* seg_argmax, void* stream) {
+  NvtxRange nvtx_("myolo_seg_ensemble");
+  MYOLO_REQUIRE(plans && K >= 1 && K <= MYOLO_ENSEMBLE_MAX, "seg_ensemble: %d members (1..%d)", K, MYOLO_ENSEMBLE_MAX);
+  MYOLO_REQUIRE(seg || seg_argmax, "seg_ensemble: no output");
+  MYOLO_REQUIRE(!seg || seg_dtype == MYOLO_F16 || seg_dtype == MYOLO_F32, "seg_ensemble: seg dtype %d", seg_dtype);
+  int rc = check_device(nullptr);
+  if (rc) return rc;
+  TensorView ins[MYOLO_ENSEMBLE_MAX];
+  int n_cls = 0;
+  for (int k = 0; k < K; ++k) {
+    const myolo_plan* pl = plans[k];
+    MYOLO_REQUIRE(pl, "seg_ensemble: member %d has no plan", k);
+    const myolo_op* up = nullptr;
+    for (const auto& op : pl->ops)
+      if (op.kind == MYOLO_OP_SEG_UPSAMPLE && op.aux[1] == 0) up = &op;
+    MYOLO_REQUIRE(up, "seg_ensemble: member %d's plan has no seg output", k);
+    MYOLO_REQUIRE(pl->B == plans[0]->B && pl->H == plans[0]->H && pl->W == plans[0]->W,
+                  "seg_ensemble: member %d's plan is %dx%dx%d, member 0's %dx%dx%d", k, pl->B, pl->H, pl->W, plans[0]->B, plans[0]->H,
+                  plans[0]->W);
+    MYOLO_REQUIRE(k == 0 || up->aux[0] == n_cls, "seg_ensemble: member %d has %d seg classes, member 0 %d", k, up->aux[0], n_cls);
+    n_cls = up->aux[0];
+    if ((rc = resolve_view(pl, up->in, &ins[k]))) return rc;
+  }
+  return launch_seg_ensemble(ins, K, n_cls, plans[0]->H, plans[0]->W, seg, seg_dtype, seg_argmax, (cudaStream_t)stream);
+}
+
 // keeps the stream busy for `ns` nanoseconds: myolo_plan_profile enqueues every op and event behind it, so that the event-to-event times are
 // device times of back-to-back kernels and not the CPU's launch cadence (~10 us per op with six tensor maps in the argument list)
 __global__ void profile_blocker_kernel(long long ns) {

@@ -231,28 +231,59 @@ class Engine:
         and pass 1's x mirrored back, each pass's Detect decodes writing straight into its slice.  seg / argmax are pass 0's, those of
         augment=False; the scaled passes run plans without the seg head (det_only_scaled=False: the full plans, for comparison).  Every
         launch goes to the current stream; nothing synchronises with the host."""
+        x = self._augment_input(x)
+        B, _, H, W = x.shape
+        det = self.model.model[-1]
+        rows = self.augment_rows(H, W)
+        dev = x.device
+        z = torch.empty((B, rows, det.no), dtype=torch.float32, device=dev)
+        seg_dt = self.seg_dtype(x)
+        seg_head = self.model.model[-2]
+        seg = torch.empty((B, seg_head.c_out, H, W), dtype=seg_dt, device=dev) if not seg_argmax else None
+        amax = torch.empty((B, H, W), dtype=torch.int64, device=dev) if seg_argmax else None
+        self.augment_passes(x, z, 0, seg, seg_dt, amax, det_only_scaled)
+        out = [(z, None), seg]
+        if seg_argmax:
+            out.append(amax)
+        return out
+
+    @staticmethod
+    def _augment_input(x):
         if not x.is_cuda:
             raise _lib.MyoloError("Model.forward(augment=True) needs a CUDA tensor: multiyolov5_b200 has no CPU path")
         if x.dtype not in (torch.float16, torch.float32):
             raise TypeError(f"Model.forward(augment=True) takes fp16 or fp32 input scaled to [0, 1] (detect.py divides by 255 first), "
                             f"not {x.dtype}")
         assert x.dim() == 4 and x.shape[1] == 3, "expected (B,3,H,W)"
+        return x.contiguous()
+
+    def seg_dtype(self, x):
+        """like the reference: fp16 in (or model.half(), detect.py:96-103) -> fp16 seg logits; otherwise fp32"""
+        half_model = next(self.model.parameters()).dtype == torch.float16
+        return torch.float16 if (x.dtype == torch.float16 or half_model) else torch.float32
+
+    def plain_rows(self, H, W):
+        """z rows per image of a plain forward at (H, W)"""
+        det = self.model.model[-1]
+        return sum(det.na * (H // int(s)) * (W // int(s)) for s in det.stride)
+
+    def augment_rows(self, H, W):
+        """z rows per image of a test-time augmentation forward at (H, W): the three passes' rows"""
+        from .utils.torch_utils import tta_passes
+        gs = int(self.model.model[-1].stride.max())
+        return sum(self.plain_rows(hp, wp) for _, _, _, (hp, wp) in tta_passes(H, W, gs))
+
+    def augment_passes(self, x, z, z_off, seg, seg_dt, amax, det_only_scaled=True):
+        """forward_augment's three passes over contiguous x, writing this model's rows from row z_off of z (B, rows, no) on, and pass 0's
+        seg / argmax (both may be None: the pass-0 plan then keeps its low-res logits for myolo_seg_ensemble)"""
         from .utils.torch_utils import scale_img, tta_passes
-        x = x.contiguous()
         B, _, H, W = x.shape
         det = self.model.model[-1]
         gs = int(det.stride.max())
         passes = tta_passes(H, W, gs)
-        offs = [0]
+        offs = [z_off]
         for _, _, _, (hp, wp) in passes:
-            offs.append(offs[-1] + sum(det.na * (hp // int(s)) * (wp // int(s)) for s in det.stride))
-        dev = x.device
-        z = torch.empty((B, offs[-1], det.no), dtype=torch.float32, device=dev)
-        half_model = next(self.model.parameters()).dtype == torch.float16
-        seg_dt = torch.float16 if (x.dtype == torch.float16 or half_model) else torch.float32
-        seg_head = self.model.model[-2]
-        seg = torch.empty((B, seg_head.c_out, H, W), dtype=seg_dt, device=dev) if not seg_argmax else None
-        amax = torch.empty((B, H, W), dtype=torch.int64, device=dev) if seg_argmax else None
+            offs.append(offs[-1] + self.plain_rows(hp, wp))
         L, sp = _lib.lib(), _lib.stream_ptr()
         # each pass's plan is looked up (and on first use built) right before its launches, so that this host work overlaps the
         # previous pass on the device
@@ -263,13 +294,9 @@ class Engine:
                 self.last_plan = p
             xi = x if k == 0 else scale_img(x, si, gs=gs, flip_lr=flip)
             inv = float(np.float32(1.0) / np.float32(si))          # `yi[..., :4] /= si`: ATen multiplies by the fp32 reciprocal
-            _lib.check(L.myolo_plan_forward_pass(p.handle, _lib.ptr(xi), _lib.torch_dtype_code(xi.dtype), _lib.ptr(z), offs[-1], offs[k],
+            _lib.check(L.myolo_plan_forward_pass(p.handle, _lib.ptr(xi), _lib.torch_dtype_code(xi.dtype), _lib.ptr(z), z.shape[1], offs[k],
                                                  inv, W if flip else 0, _lib.ptr(seg if k == 0 else None), _lib.torch_dtype_code(seg_dt),
                                                  _lib.ptr(amax if k == 0 else None), sp))
-        out = [(z, None), seg]
-        if seg_argmax:
-            out.append(amax)
-        return out
 
     # ---- training (SURVEY.md section 8 row a13) -----------------------------------------------------------------------
     def train_plan_for(self, B, H, W, lane=0) -> CompiledPlan:
@@ -500,6 +527,49 @@ class Engine:
         out = torch.empty((p.B, v.c, v.h, v.w), dtype=torch.float32, device="cuda")
         _lib.check(_lib.lib().myolo_plan_read_view(p.handle, _lib.View(v.buf.id, v.c_off, v.c), _lib.ptr(out), _lib.stream_ptr()))
         return out
+
+
+def forward_ensemble(members, x: torch.Tensor, augment=False, seg_argmax=False):
+    """Ensemble.forward in eval mode (models.experimental.Ensemble): `[(z, None), seg]`, plus the argmax map with seg_argmax=True.
+    z (B, the members' rows, no) fp32 holds member 0's rows, then member 1's, ..., each member's Detect decodes writing straight into its
+    slice (augment=True: each member's block is its forward_augment rows).  seg is the mean of the members' plain seg logits in the dtype
+    one member returns, and the argmax map that of the fp32 mean: one myolo_seg_ensemble launch over the low-res logits the members'
+    passes leave in their plans, with no full-size map per member.  The members were checked to agree (Ensemble.check_members).  Every
+    launch goes to the current stream; nothing synchronises with the host."""
+    if augment:
+        x = Engine._augment_input(x)
+    else:
+        if not x.is_cuda:
+            raise _lib.MyoloError("Ensemble.forward needs a CUDA tensor: multiyolov5_b200 has no CPU path (use the oracle for CPU numbers)")
+        assert x.dim() == 4 and x.shape[1] == 3, "expected (B,3,H,W)"
+        x = x.contiguous()
+    B, _, H, W = x.shape
+    engines = [m.engine() for m in members]
+    rows = [e.augment_rows(H, W) if augment else e.plain_rows(H, W) for e in engines]
+    offs = np.cumsum([0] + rows).tolist()
+    dev = x.device
+    z = torch.empty((B, offs[-1], members[0].model[-1].no), dtype=torch.float32, device=dev)
+    seg_dt = engines[0].seg_dtype(x)
+    L, sp = _lib.lib(), _lib.stream_ptr()
+    plans = []
+    for e, off, n in zip(engines, offs, rows):
+        if augment:
+            e.augment_passes(x, z, off, None, seg_dt, None)
+            p = e.plans[(B, H, W)]                   # pass 0's plan: the plain one, with the seg head
+        else:
+            p = e.plan_for(B, H, W)                  # looked up right before its launches, as forward_augment does
+            assert sum(p.pb.det_rows) == n
+            _lib.check(L.myolo_plan_forward_pass(p.handle, _lib.ptr(x), _lib.torch_dtype_code(x.dtype), _lib.ptr(z), offs[-1], off, 1.0,
+                                                 0, None, _lib.torch_dtype_code(seg_dt), None, sp))
+        plans.append(p.handle)
+    seg = torch.empty((B, members[0].model[-2].c_out, H, W), dtype=seg_dt, device=dev) if not seg_argmax else None
+    amax = torch.empty((B, H, W), dtype=torch.int64, device=dev) if seg_argmax else None
+    _lib.check(L.myolo_seg_ensemble((C.c_void_p * len(plans))(*[h.value for h in plans]), len(plans), _lib.ptr(seg),
+                                    _lib.torch_dtype_code(seg_dt), _lib.ptr(amax), sp))
+    out = [(z, None), seg]
+    if seg_argmax:
+        out.append(amax)
+    return out
 
 
 class _TrainFunction(torch.autograd.Function):

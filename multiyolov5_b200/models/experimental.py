@@ -73,15 +73,51 @@ def _compat_fixup(model):
 
 
 class Ensemble(nn.ModuleList):
-    """reference models/experimental.py:95-110: NMS ensemble - the members' decoded predictions are concatenated along the anchor axis"""
+    """reference models/experimental.py:98-110: several models on one input.  In eval mode forward returns what Model.forward returns,
+    `[(z, None), seg]` (plus the argmax map with seg_argmax=True): z concatenates the members' decoded predictions along the anchor axis
+    (the reference's "nms ensemble" with the fork's missing index restored, `module(x, augment)[0][0]`), and seg is the mean of the
+    members' seg logits (the reference's commented "mean ensemble" applied to the seg output; the fork defines none).  On the device:
+    engine.forward_ensemble."""
 
-    def forward(self, x, augment=False):
-        y = [m(x, augment)[0][0] for m in self]
-        return torch.cat(y, 1), None
+    def check_members(self):
+        """raises ValueError unless the members can share one output: the same Detect.no, seg classes, Detect.stride, device and parameter
+        dtype, and at most MYOLO_ENSEMBLE_MAX of them.  Runs once per member list and dtype / device state."""
+        from .. import _lib
+        for k, m in enumerate(self):
+            if not isinstance(m, _yolo.Model):
+                raise ValueError(f"Ensemble member {k} is a {type(m).__name__}, not a Model")
+        params = [next(m.parameters()) for m in self]
+        key = tuple((id(m), p.dtype, p.device) for m, p in zip(self, params))
+        if getattr(self, "_checked", None) == key:
+            return
+        if not 1 <= len(self) <= _lib.ENSEMBLE_MAX:
+            raise ValueError(f"Ensemble: {len(self)} members; the device path takes 1 to {_lib.ENSEMBLE_MAX}")
+
+        def props(m, p):
+            det, seg = m.model[-1], m.model[-2]
+            return {"Detect.no (5 + nc)": int(det.no), "seg classes": int(seg.c_out), "Detect.stride": [float(s) for s in det.stride],
+                    "device": p.device, "parameter dtype": p.dtype}
+        first = props(self[0], params[0])
+        for k, (m, p) in enumerate(zip(self, params)):
+            for name, v in props(m, p).items():
+                if v != first[name]:
+                    raise ValueError(f"Ensemble member {k} has {name} {v}, member 0 has {first[name]}: members must agree to share one output")
+        self._checked = key
+
+    def forward(self, x, augment=False, profile=False, seg_argmax=False):
+        if self.training or any(m.training for m in self):
+            raise RuntimeError("Ensemble.forward needs eval mode: the members' decoded predictions are concatenated, which a train-mode "
+                               "forward does not produce (call ensemble.eval())")
+        if profile:
+            raise ValueError("Ensemble.forward: profile=True profiles one plain Model forward; it cannot be combined with an ensemble")
+        self.check_members()
+        from ..engine import forward_ensemble
+        return forward_ensemble(list(self), x, augment=augment, seg_argmax=seg_argmax)
 
 
 def attempt_load(weights, map_location=None):
-    """reference models/experimental.py:113-134.  Returns the model (or an Ensemble) in fp32, `.fuse().eval()`-ed."""
+    """reference models/experimental.py:113-134.  Returns the model (or an Ensemble) in fp32, `.fuse().eval()`-ed.  An Ensemble's members
+    are checked (Ensemble.check_members) here, so mismatched checkpoints fail before any input is read."""
     model = Ensemble()
     for w in weights if isinstance(weights, (list, tuple)) else [weights]:
         ckpt = load_checkpoint(w, map_location=map_location)
@@ -89,6 +125,8 @@ def attempt_load(weights, map_location=None):
         model.append(_compat_fixup(m).float().fuse().eval())
     if len(model) == 1:
         return model[-1]
+    print('Ensemble created with %s\n' % (weights,))
     for k in ("names", "stride"):
         setattr(model, k, getattr(model[-1], k))
+    model.check_members()
     return model

@@ -11,6 +11,8 @@ train.py:207-210 (`create_dataloader(..., rect=True, pad=0.5)`), bit exact with 
 
 test()'s options, as the reference's test.py has them:
   augment      the TTA forward (model(img, augment=True)[0] is (z, None), so compute_loss cannot go with it)
+  model        a Model or an Ensemble (models.experimental.attempt_load of several weights: its [0] is (z, None) too, so compute_loss
+               cannot go with it; model.half() reaches every member)
   save_hybrid  the labels join each image's NMS candidates (non_max_suppression with an NmsLabels, myolo_nms_labels), so the
                statistics include them, as in the reference
   plots        the confusion matrix (utils.metrics.ConfusionMatrix, one myolo_confusion_update launch per batch) and its plot();
@@ -26,6 +28,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .models.experimental import Ensemble
 from .utils.general import NmsLabels, check_nms_labels_error, coco80_to_coco91_class, non_max_suppression, scale_boxes
 from .utils.metrics import ConfusionMatrix, DetectionStats, _class_map, pack_geometry
 
@@ -66,6 +69,9 @@ def test(data, weights=None, batch_size=32, imgsz=640, conf_thres=0.001, iou_thr
         raise NotImplementedError("test(model=None): loading weights and data files is not built; pass model= and dataloader=")
     if wandb_logger:
         raise NotImplementedError("test(wandb_logger=...): W&B logging is not built")
+    if compute_loss and isinstance(model, Ensemble):
+        raise ValueError("test(model=Ensemble) returns no training outputs (model(img)[0] is (z, None)), so compute_loss cannot be "
+                         "evaluated with it")
     if next(model.parameters()).device.type != "cuda":
         raise NotImplementedError("test() on a CPU model: there is no CPU path; move the model to the GPU")
     if augment and compute_loss:
